@@ -1,17 +1,20 @@
 #!/usr/bin/env python
 """bench.py — tokens/s of the data-parallel pretraining step (forward + backward + sharded AdamW) on synthetic tokens.
 
-    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--workload NAME] [--impl reference] [--dump-outputs DIR]
 
 Workloads (BASELINE.json `configs`):
     gpt2-110m        C2  Wenzhong-GPT2-110M, seq 1024, 32 sequences per GPU, bf16            (default at any N; weak scaling)
-    ziya-llama-13b   C4  Ziya-LLaMA-13B, seq 2048, 32 sequences per GPU, ZeRO-2, bf16        (needs >= 4 GPUs of HBM)
+    ziya-llama-13b   C4  Ziya-LLaMA-13B, seq 1024, 32 sequences per GPU, ZeRO-2, bf16        (needs 8 GPUs of 80 GB)
     ziya-llama-13b-L{n}  same width, n layers (NOT a BASELINE config; kernel bring-up / profiling only)
 A "step" is one optimizer step over the per-GPU batch (micro-batches x gradient accumulation). `value` is whole-job
 tokens/s with the token tensors already resident in HBM; `e2e` repeats the measurement through the public step API
 (fsb200.trainer.PretrainStep.step) from pinned host memory, with the host->device copies and the loss read-back inside
 the timed region. Timing: CUDA events, barrier + synchronize on both sides, max over ranks.
 `--impl reference` times the reference's own CPU implementation of the same step on the host cores (see DESIGN.md).
+`--dump-outputs DIR` writes what the last timed step handed its caller (see dump_step_outputs) as float32 .npy files, so that
+two builds can be compared output for output: model initialisation and token batches are seeded, the inputs are identical
+from run to run.
 """
 import argparse
 import json
@@ -47,9 +50,12 @@ WORKLOADS = {
     "randeng-t5-784m": dict(family="t5", vocab_size=32600, d_model=1024, d_kv=64, d_ff=2816, num_layers=24, num_heads=16,
                             seq=512, seq_dec=512, per_gpu=32, micro=32, lr=1e-4, betas=(0.9, 0.999), wd=0.1, clip=1.0,
                             label="Randeng-T5-784M seq2seq pretrain, enc 512 / dec 512, batch 32/GPU, ZeRO-2 (BASELINE configs[4])"),
+    # On 8 x 80 GB the ZeRO-2 state is ~58 GB per GPU and nothing is recomputed: activations take ~0.34 GB per layer and 1024
+    # tokens (measured on one H100 with 4 layers), so seq 1024 at micro-batch 1 is what fits; BASELINE words seq 2048
     "ziya-llama-13b": dict(family="llama", vocab_size=39424, hidden_size=5120, num_hidden_layers=40,
-                           num_attention_heads=40, seq=2048, per_gpu=32, micro=4, lr=1e-4, betas=(0.9, 0.95), wd=0.1,
-                           clip=1.0, label="Ziya-LLaMA-13B pretrain, seq 2048, global batch 32/GPU, ZeRO-2 (BASELINE configs[3])"),
+                           num_attention_heads=40, seq=1024, per_gpu=32, micro=1, lr=1e-4, betas=(0.9, 0.95), wd=0.1,
+                           clip=1.0, label="Ziya-LLaMA-13B pretrain, seq 1024, global batch 32/GPU, ZeRO-2 (BASELINE configs[3] at the "
+                                       "sequence length 80 GB allows)"),
 }
 
 
@@ -85,48 +91,11 @@ def flops_per_token(w):
     return 6.0 * n_mm + 3.0 * attn
 
 
-# DRAM traffic of the dominant kernel's largest-share launch: parsed AT RUN TIME from the committed `ncu --set full`
-# summaries under profiles/ (dram__bytes_read.sum + dram__bytes_write.sum of ONE launch), next to its algorithmic bytes
-# (A + B read once, D written once). Newest round first; null when no committed capture names the shape.
-NCU_SHAPES = {
-    "gpt2": ("32768x3072x768", "fsb::gemm_bf16_kernel<NN,256,pair> 32768x3072x768 (c_fc forward)", (32768, 3072, 768)),
-    "bert": ("32768x3072x768", "fsb::gemm_bf16_kernel<NN,256,pair> 32768x3072x768 (same MLP shape family)", (32768, 3072, 768)),
-    "llama": ("8192x15360x5120", "fsb::gemm_bf16_kernel<NT,256,pair> 8192x15360x5120 (QKV forward)", (8192, 15360, 5120)),
-    "t5": ("16384x5632x1024", "fsb::gemm_bf16_kernel<NT,256,pair> 16384x5632x1024 (wi_0|wi_1 forward)", (16384, 5632, 1024)),
-}
-NCU_FILES = ("profiles/r02_ncu_gemm.summary.txt", "profiles/r01_ncu_gemm_final.summary.txt")
-_UNIT = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-
-
-def ncu_traffic(family):
-    marker, launch, (M, N, K) = NCU_SHAPES.get(family, (None, None, (0, 0, 0)))
-    if marker is None:
-        return None
-    for rel in NCU_FILES:
-        path = os.path.join(ROOT, rel)
-        if not os.path.exists(path):
-            continue
-        block, hit = [], False
-        for line in open(path):
-            if line.startswith("=="):
-                if hit:
-                    break
-                hit = marker in line
-                continue
-            if hit:
-                block.append(line.split())
-        if not hit and not block:
-            continue
-        vals = {t[0]: (float(t[1]), t[2] if len(t) > 2 else "") for t in block if len(t) >= 2}
-        try:
-            rd = vals["dram__bytes_read.sum"][0] * _UNIT[vals["dram__bytes_read.sum"][1]]
-            wr = vals["dram__bytes_write.sum"][0] * _UNIT[vals["dram__bytes_write.sum"][1]]
-        except KeyError:
-            continue
-        tp = vals.get("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active", (None,))[0]
-        return {"launch": launch, "traffic": rd + wr, "dram_read": rd, "dram_write": wr,
-                "algorithmic": (M * K + K * N + M * N) * 2.0, "tensor_pipe_active_pct": tp, "source": rel}
-    return None
+# NVIDIA's data sheet for the H100 SXM (700 W): dense BF16 tensor rate and HBM3 bandwidth. Never reached figures: the
+# `frac_of_spec` keys divide by them.
+H100_SPEC = {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}
+# Parameters written by --dump-outputs: all of them up to this count, else a fixed, seeded sample of this size (16 MB as fp32).
+DUMP_PARAMS = 4 << 20
 
 
 def peaks():
@@ -135,11 +104,12 @@ def peaks():
         d = json.load(open(p))
         return {"bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "bf16_burst": d.get("bf16_tflops"),
                 "hbm_gbs": d.get("hbm_gbs"), "src": "measured (MEASURED_PEAKS.json, sustained)"}
-    return {"bf16_tflops": 1400.0, "bf16_burst": None, "hbm_gbs": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": H100_SPEC["bf16_tflops"], "bf16_burst": None, "hbm_gbs": H100_SPEC["hbm_gbs"],
+            "src": "fallback: H100 SXM data sheet (700 W), not measured"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle sampling DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -353,10 +323,31 @@ def cpu_reference_run(w, steps, warmup, budget_s=None):
             "sample": sample, "cores": n_thr}
 
 
-def run_workload(name, args, world, rank, device, pg, steps, warmup, want_e2e=True, profile_steps=2, overrides=None):
+def dump_step_outputs(out_dir, stepper, timed_losses):
+    """What the timed path hands its caller after its last step, as float32 .npy files under `out_dir`: the step's loss
+    (loss.npy), the loss of every timed step (losses.npy) and the updated parameters (params.npy: the flat bf16 parameter
+    vector, or the entries at DUMP_PARAMS sorted indices drawn from a generator seeded with 0 when it is longer)."""
+    import numpy as np
+    stepper.engine.wait_params()
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), timed_losses[-1].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "losses.npy"), torch.stack(timed_losses).float().cpu().numpy())
+    params = stepper.model.flat.params
+    n = params.numel()
+    if n > DUMP_PARAMS:
+        idx = torch.randint(0, n, (DUMP_PARAMS,), generator=torch.Generator().manual_seed(0)).sort().values
+    else:
+        idx = torch.arange(n)
+    np.save(os.path.join(out_dir, "params.npy"), params[idx.to(params.device)].float().cpu().numpy())
+
+
+def run_workload(name, args, world, rank, device, pg, steps, warmup, want_e2e=True, profile_steps=2, overrides=None,
+                 dump_dir=None):
     """Build the model + engine for workload `name`, warm up, time `steps` optimizer steps with the batches resident in
     HBM (`value`), then through the public API from pinned host memory (`e2e`), then `profile_steps` EXTRA steps with CUDA
-    events around every GEMM launch (the roofline block) — the timed regions themselves carry no instrumentation."""
+    events around every GEMM launch (the roofline block) — the timed regions themselves carry no instrumentation.
+    With `dump_dir`, rank 0 writes the outputs of the last timed step there before anything else runs."""
     from fsb200 import lib as L, ops
     from fsb200.schedules import polynomial_lr
     from fsb200.trainer import PretrainStep
@@ -387,6 +378,8 @@ def run_workload(name, args, world, rank, device, pg, steps, warmup, want_e2e=Tr
     clocks = sampler.stop() if sampler else None
     launches = L.kernel_launches - k0
     ms_per_step = ms / steps
+    if dump_dir is not None and rank == 0:
+        dump_step_outputs(dump_dir, stepper, losses[warmup:])
     value = world * tokens_step_gpu / (ms_per_step / 1000.0)
 
     e2e = None
@@ -433,21 +426,19 @@ def run_workload(name, args, world, rank, device, pg, steps, warmup, want_e2e=Tr
     pk = peaks()
     gemm_tf = gsum["work"] / (gsum["ms"] / 1000.0) / 1e12 if gsum["ms"] > 0 else 0.0
     step_tf = value * ftok / world / 1e12
-    tr = ncu_traffic(w["family"])
     out = {
         "name": name, "workload": w["label"], "value": value, "ms_per_step": ms_per_step, "e2e": e2e, "launches": launches,
         "clocks": clocks, "final_loss": final_loss, "first_loss": first_loss, "ftok": ftok, "w": w, "ga": ga,
-        "roofline": {"bound": "tensor", "kernel": "fsb::gemm_bf16_kernel (tcgen05)", "achieved": gemm_tf,
+        "roofline": {"bound": "tensor", "kernel": "fsb::gemm_bf16_kernel (wgmma)", "achieved": gemm_tf,
                      "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": gemm_tf / pk["bf16_tflops"],
                      "frac_of_burst_peak": gemm_tf / pk["bf16_burst"] if pk.get("bf16_burst") else None,
-                     "frac_of_spec_2250": gemm_tf / 2250.0,
-                     "traffic": tr["traffic"] if tr else None, "traffic_detail": tr, "peak_source": pk["src"],
+                     "frac_of_spec": gemm_tf / H100_SPEC["bf16_tflops"], "peak_source": pk["src"],
                      "timing": f"CUDA events around each GEMM launch in {profile_steps} extra steps after the timed region",
                      "launches_per_step": gsum["launches"] / max(1, profile_steps),
                      "kernel_share_of_step": gsum["ms"] / prof_ms if prof_ms > 0 else None,
                      "step_achieved_tflops_per_gpu": step_tf, "step_frac": step_tf / pk["bf16_tflops"],
                      "step_frac_of_burst_peak": step_tf / pk["bf16_burst"] if pk.get("bf16_burst") else None,
-                     "step_frac_of_spec_2250": step_tf / 2250.0},
+                     "step_frac_of_spec": step_tf / H100_SPEC["bf16_tflops"]},
         "memory": dict(stepper.engine.memory_report(), peak_allocated=torch.cuda.max_memory_allocated(device)),
         "comm_bytes_per_step_per_gpu": stepper.engine.comm_bytes // max(1, stepper.engine.step_count),
     }
@@ -517,7 +508,9 @@ def parity_block(world, rank, device):
     return res
 
 
-HEADLINE = {8: ("ziya-llama-13b", 3, 1), 4: ("megatronbert-1.3b", 5, 2)}   # gpus -> (workload, timed steps, warm-up)
+# gpus -> (workload, timed steps, warm-up). C4 runs with ZeRO-2 only: a ZeRO-1 variant would keep the full 26.2 GB of bf16
+# gradients on every GPU on top of ~58 GB of ZeRO-2 state and the activations, which does not fit 80 GB.
+HEADLINE = {8: ("ziya-llama-13b", 3, 1), 4: ("megatronbert-1.3b", 5, 2)}
 
 
 def main():
@@ -540,8 +533,9 @@ def main():
     ap.add_argument("--headline-zero-stage", type=int, default=0,
                     help="override the ZeRO stage of the headline block (diagnostic: 1 = reduce once per optimizer step instead of "
                          "once per micro-batch; BASELINE's C4 is stage 2)")
-    ap.add_argument("--no-zero1-variant", action="store_true", help="skip the ZeRO-1 variant of the C4 headline block")
     ap.add_argument("--no-graph-block", action="store_true", help="skip the extra CUDA-graph measurement at --gpus 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32; see dump_step_outputs)")
     ap.add_argument("--breakdown", action="store_true",
                     help="after the timed runs, profile 2 more steps with CUDA events around every fsb_* call and print the "
                          "per-entry-point time table to stderr (diagnostic; not part of the JSON line)")
@@ -566,9 +560,12 @@ def main():
     cfg_common = {"workload": w["label"], "name": args.workload, "seq_len": w["seq"], "per_gpu_batch": w["per_gpu"],
                   "global_batch": w["per_gpu"] * max(1, args.gpus), "micro_batch": w["micro"],
                   "grad_accum": w["per_gpu"] // w["micro"], "zero_stage": w.get("stage", 2), "dropout": 0.0,
-                  "flops_per_token": ftok, "l2": "working set (weights + activations, GBs) exceeds the 126 MB L2; no flush"}
+                  "flops_per_token": ftok, "l2": "working set (weights + activations, GBs) exceeds the 50 MB L2; no flush"}
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs writes what the fsb200 step computed; the reference arm times a bounded CPU sample and "
+                             "has nothing comparable to write")
         if rank != 0:
             return
         r = cpu_reference_run(w, steps=args.steps, warmup=args.warmup)
@@ -594,7 +591,7 @@ def main():
 
     warm = max(3, args.warmup)
     main_run = run_workload(args.workload, args, world, rank, device, pg, args.steps, warm, want_e2e=not args.no_e2e,
-                            overrides=over)
+                            overrides=over, dump_dir=args.dump_outputs)
     graph_block = None
     if world == 1 and not args.cuda_graph and not args.no_graph_block:
         # the same workload with the whole optimizer step captured in ONE CUDA graph and replayed (bit-identical results,
@@ -622,26 +619,12 @@ def main():
                     "step_tflops_per_gpu": hr["roofline"]["step_achieved_tflops_per_gpu"],
                     "step_frac_of_sustained_peak": hr["roofline"]["step_frac"],
                     "step_frac_of_burst_peak": hr["roofline"]["step_frac_of_burst_peak"],
-                    "step_frac_of_spec_2250": hr["roofline"]["step_frac_of_spec_2250"],
-                    "gemm": {k: hr["roofline"][k] for k in ("achieved", "frac", "frac_of_burst_peak", "frac_of_spec_2250",
+                    "step_frac_of_spec": hr["roofline"]["step_frac_of_spec"],
+                    "gemm": {k: hr["roofline"][k] for k in ("achieved", "frac", "frac_of_burst_peak", "frac_of_spec",
                                                             "kernel_share_of_step", "launches_per_step")},
                     "clocks": hr["clocks"], "first_loss": hr["first_loss"], "final_loss": hr["final_loss"],
                     "memory_bytes": hr["memory"], "comm_bytes_per_step_per_gpu": hr["comm_bytes_per_step_per_gpu"],
                     "gpu_launches": hr["launches"]}
-        if hname == "ziya-llama-13b" and not args.headline_zero_stage and not args.no_zero1_variant:
-            # the same model and batch with ZeRO STAGE 1 semantics (full bf16 gradients accumulate locally, ONE reduce-scatter
-            # per bucket and optimizer step instead of one per micro-batch): 1/8 of the gradient traffic and no per-micro-batch
-            # fp32 shard accumulation. 131 GB peak per GPU — on 180 GB parts gradient sharding is not needed for this model.
-            try:   # memory is symmetric across ranks: an out-of-memory here hits every rank at model construction, before any collective
-                vr = run_workload(hname, args, world, rank, device, pg, 3, 1, want_e2e=False, profile_steps=0,
-                                  overrides={"stage": 1})
-                headline["zero1_variant"] = {"tokens_per_s": vr["value"], "ms_per_step": vr["ms_per_step"], "steps": 3, "warmup": 1,
-                                             "step_frac_of_sustained_peak": vr["roofline"]["step_frac"],
-                                             "final_loss": vr["final_loss"], "clocks": vr["clocks"], "memory_bytes": vr["memory"],
-                                             "comm_bytes_per_step_per_gpu": vr["comm_bytes_per_step_per_gpu"]}
-            except torch.cuda.OutOfMemoryError as e:
-                headline["zero1_variant"] = {"error": f"out of memory: {str(e)[:120]}"}
-                torch.cuda.empty_cache()
 
     if rank != 0:
         if world > 1:

@@ -1,7 +1,7 @@
 """Drop-in for the reference's pybind module `scaled_masked_softmax_cuda`
 (fengshen/models/megatron/fused_kernels/scaled_masked_softmax.cpp:70-83): same three functions, same tensor contract
 (input [b, np, sq, sk] half-precision, mask [b|1, 1, sq, sk] uint8/bool with 1 = masked, float scale; backward returns the
-gradient written IN PLACE over `output_grads`), executed by libfsb200.so. Only bf16 is implemented (the B200 path trains in
+gradient written IN PLACE over `output_grads`), executed by libfsb200.so. Only bf16 is implemented (the GPU path trains in
 bf16); an fp16 tensor raises instead of silently falling back."""
 import torch
 

@@ -1,16 +1,17 @@
-// fsb200 — fused attention backward on tcgen05 / TMEM (replaces 3P flash_attn_cuda.bwd called from
+// fsb200 — fused attention backward on wgmma (replaces 3P flash_attn_cuda.bwd called from
 // fengshen/models/megatron/layers/flash_attention.py:81-101 and the autograd of the baddbmm/softmax/bmm path,
 // transformer.py:307-408; softmax backward formula dx = y*(dy - sum(dy*y)) as in scaled_masked_softmax.h:240-335).
 //
 // Three launches, all deterministic (no atomics):
 //   1. delta[b,h,q] = sum_d dO*O                                   (HBM-bound preprocess)
 //   2. dQ kernel : CTA = (b, head, 128 queries), loops over 64-key steps:
-//        S = Q K^T, dP = dO V^T  (TMEM, double-buffered)  ->  threads (1 per query row): P = exp2(S*c - lse),
-//        dS = P*(dP - delta) -> bf16 smem (K-major, 128B swizzle)  ->  dQ += dS K  (TMEM accumulator, K as MN-major B)
-//   3. dKV kernel: CTA = (b, head, 128 keys), loops over 64-query steps with the TRANSPOSED products so that
-//        TMEM lane == key row:  S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T (bf16 smem) -> dV += P^T dO, dK += dS^T Q
+//        S = Q K^T, dP = dO V^T (wgmma, fp32 in registers) -> P = exp2(S*c - lse), dS = P*(dP - delta) in registers
+//        -> dQ += dS K (dS as the register A operand, K read MN-major from the same shared-memory tile)
+//   3. dKV kernel: CTA = (b, head, 128 keys), loops over 64-query steps with the TRANSPOSED products so that a
+//        register row is a key row:  S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q
 //        (dO / Q tiles reused as MN-major B operands; nothing is transposed in memory).
 // S and dP are recomputed in both kernels (7 GEMMs instead of 5) — the price of determinism without a dQ reduction.
+// Both kernels: warpgroup 0 = TMA producer, warpgroups 1-2 = 64 resident rows each, working on the same streamed stage.
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -19,41 +20,24 @@ namespace fsb {
 int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
                    int box_rows);
 
-// warps 0-15: math — 4 threads per row, 16 of the step's 64 columns each (warp w: TMEM lane quadrant w & 3, column part w >> 2).
-// The per-step chain (tcgen05.ld -> exp2 / multiply -> bf16 tile in smem -> arrive) is latency-bound, so four warps per
-// scheduler with a quarter of the work each beat two with half each. warp 16: TMA; warp 17: MMA + TMEM owner.
-constexpr int AB_PARTS = 4;
-constexpr int AB_PC = 64 / AB_PARTS;   // columns per thread and step
-constexpr int AB_MATH = 128 * AB_PARTS;
-constexpr int AB_THREADS = AB_MATH + 64;
-constexpr int AB_W_TMA = AB_MATH / 32, AB_W_MMA = AB_MATH / 32 + 1;
-
-constexpr int AB_BM = 128;       // rows owned by the CTA (queries for dQ, keys for dKV) == TMEM lanes
+constexpr int AB_THREADS = 384;
+constexpr int AB_BM = 128;       // rows owned by the CTA (queries for dQ, keys for dKV)
 constexpr int AB_BN = 64;        // streamed tile (keys for dQ, queries for dKV)
+constexpr int AB_NDIAG = AB_BM + AB_BN - 1;   // diagonals k - q of one 128 x 64 step (bias gradient)
+constexpr int AB_DSTRIDE = 192;               // floats per step in the bias-gradient workspace (>= AB_NDIAG)
 
 struct AttBwdParams {
   const float* lse;     // [B,H,Sq] log2 domain
   const float* delta;   // [B,H,Sq]
   const uint8_t* kv_mask;
   const float* rel_bias;     // [nheads, seq_q + seq_kv - 1] additive bias over k - q (natural-log units) or nullptr
-  float* dbias_part;         // per-warp partial diagonal sums of dS written by the dQ kernel (see attn_dbias_reduce_kernel)
-  int64_t dbias_tstride;     // floats per (b, head, q tile, warp): n_all * 64
-  const __nv_bfloat16 *q, *dout, *k, *v;   // raw views: at D = 64 each math thread parks its own Q / dO (dQ kernel) or K / V (dKV kernel) row in TMEM as MMA A operands
-  int64_t q_row_stride, do_row_stride, k_row_stride, v_row_stride;
+  float* dbias_part;         // per-step diagonal sums of dS written by the dQ kernel (see attn_dbias_reduce_kernel)
   __nv_bfloat16 *dq, *dk, *dv;
   int64_t dq_row_stride, dk_row_stride, dv_row_stride, dq_head_stride, dk_head_stride, dv_head_stride;
   int q_head_stride, k_head_stride, v_head_stride, do_head_stride;
   int seq_q, seq_kv, nheads, batch, causal;
   float scale, scale_log2;
 };
-
-// Optional cycle trace of one CTA (development aid; compiled in only with -DFSB_ATTN_TRACE)
-#ifdef FSB_ATTN_TRACE
-__device__ long long g_attn_trace[2][64][8];
-#define TRACE(role, step, k) do { if (trace_on && (step) < 64) g_attn_trace[role][step][k] = clock64(); } while (0)
-#else
-#define TRACE(role, step, k) do { } while (0)
-#endif
 
 // ------------------------------------------------------------------------------------------------ delta preprocess
 template <int D>
@@ -87,24 +71,37 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 }
 
 // ------------------------------------------------------------------------------------------------ shared layout
-template <int D, int kStages, int kTBufs>
+template <int D, bool kDS>
 struct AttBwdSmem {
   static constexpr int BIG_BYTES = AB_BM * D * 2;    // a resident 128-row tile
   static constexpr int SML_BYTES = AB_BN * D * 2;    // a streamed 64-row tile
-  static constexpr int T_BYTES = AB_BM * AB_BN * 2;  // bf16 [128 x 64] P / dS tile
-  static constexpr int STAGES = kStages;  // streamed-tile ring depth: must cover the TMA round trip (~2 us)
+  static constexpr int STAGES = 3;                   // streamed-tile ring depth
   static constexpr int OFF_BIG0 = 0;                       // dQ: Q     | dKV: K
   static constexpr int OFF_BIG1 = OFF_BIG0 + BIG_BYTES;    // dQ: dO    | dKV: V
   static constexpr int OFF_SML0 = OFF_BIG1 + BIG_BYTES;    // dQ: K_j   | dKV: Q_i   (STAGES)
   static constexpr int OFF_SML1 = OFF_SML0 + STAGES * SML_BYTES;  // dQ: V_j | dKV: dO_i
-  static constexpr int OFF_T0 = OFF_SML1 + STAGES * SML_BYTES;    // dQ: dS[2] | dKV: P^T[2]
-  static constexpr int OFF_T1 = OFF_T0 + 2 * T_BYTES;             //           | dKV: dS^T[2]
-  static constexpr int OFF_STATS = OFF_T0 + kTBufs * T_BYTES;     // float [2][2][64] (dKV only)
-  static constexpr int OFF_BAR = OFF_STATS + 2 * 2 * 64 * 4;
-  static constexpr int NBAR = 1 + 2 * STAGES + 2 + 2 + 1;  // big_full, sml_full[S], sml_empty[S], s_full[2], t_ready[2], done
-  static constexpr int TOTAL = OFF_BAR + NBAR * 8 + 16 + 1024;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into on sm_100");
+  static constexpr int OFF_DS = OFF_SML1 + STAGES * SML_BYTES;    // dQ with a bias gradient: fp32 dS tile [128][65]
+  static constexpr int OFF_BAR = OFF_DS + (kDS ? (AB_BM * (AB_BN + 1) * 4 + 15) / 16 * 16 : 0);
+  static constexpr int NBAR = 1 + 2 * STAGES;  // big_full, sml_full[S], sml_empty[S]
+  static constexpr int TOTAL = OFF_BAR + NBAR * 8 + 1024;
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
 };
+
+template <int D>
+__device__ __forceinline__ void wgmma_rs_acc(float (&o)[D / 2], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (D == 128) wgmma_rs_n128<1>(o, a, db, 1u);
+  else wgmma_rs_n64<1>(o, a, db, 1u);
+}
+// shared-memory byte offset of the 16-wide K slice kk of a K-major tile with `rows` rows (64-column swizzle chunks)
+__device__ __forceinline__ uint32_t kslice(int kk, int rows) { return (kk / 4) * (rows * 128) + (kk % 4) * 32; }
+// 16-key slice kk of a [64 x 64] fp32 accumulator as bf16 register A fragments
+__device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (&a)[4]) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int i = 2 * kk + (r >> 1), h = r & 1;
+    a[r] = pack_bf16x2(x[4 * i + 2 * h], x[4 * i + 2 * h + 1]);
+  }
+}
 
 // ================================================================================================ dQ kernel
 template <int D, bool kBias>
@@ -112,32 +109,14 @@ __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                    const AttBwdParams p) {
-  using S = AttBwdSmem<D, (D == 64 ? 6 : 4), 2>;
+  using S = AttBwdSmem<D, kBias>;
   constexpr int STAGES = S::STAGES;
-  constexpr int TMEM_COLS = 512;
-  // All three products take their A operand from TENSOR MEMORY (row == lane, bf16 pairs per 32-bit column), so the tensor
-  // core only streams the K / V tiles from shared memory (an SS-mode 128x64x16 MMA reads 6 KB per 32 cycles — 192 B/clk
-  // against the 128 B/clk an SM's shared memory delivers; with A in TMEM it is 2 KB):
-  //   Q, dO : parked once per CTA by the math threads (each thread loads its own row slice from global)
-  //   dS(j) : written by the math threads over the S(j) columns they have just consumed (part p -> columns 16p..16p+7)
-  constexpr int TM_S = 0;     // S[buf] at buf*128, dP[buf] at buf*128 + 64
-  constexpr int TM_DQ = 256;  // D columns
-  constexpr bool kQT = (D == 64);          // Q / dO as TMEM operands: measured -16 % per step at D = 64, +4 % at D = 128 (kept in smem there)
-  constexpr int TM_Q = 256 + D;            // D/2 columns
-  constexpr int TM_DO = 256 + D + D / 2;   // D/2 columns  (256 + 2 D <= 512)
-  constexpr uint32_t IDESC_S = make_idesc_bf16(AB_BM, AB_BN, 0, 0);
-  constexpr uint32_t IDESC_DQ = make_idesc_bf16(AB_BM, D, 0, 1);
-
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
   uint64_t* big_full = bars;
   uint64_t* sml_full = big_full + 1;
   uint64_t* sml_empty = sml_full + STAGES;
-  uint64_t* s_full = sml_empty + STAGES;
-  uint64_t* t_ready = s_full + 2;
-  uint64_t* done = t_ready + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(done + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = gridDim.x - 1 - blockIdx.x;
@@ -145,49 +124,25 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int q0 = tile * AB_BM;
   const int n_all = (p.seq_kv + AB_BN - 1) / AB_BN;
   const int n_steps = p.causal ? min(n_all, (min(q0 + AB_BM, p.seq_q) + AB_BN - 1) / AB_BN) : n_all;
-#ifdef FSB_ATTN_TRACE
-  const bool trace_on = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (threadIdx.x & 31) == 0 &&
-                        (warp == 0 || warp == AB_W_MMA);
-#endif
 
-  if (warp == AB_W_TMA && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-    mbar_init(big_full, kQT ? AB_MATH / 32 : 1);   // Q / dO parked in TMEM (one arrival per math warp) or loaded by TMA
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&t_ready[i], AB_MATH / 32); }
-    mbar_init(done, 1);
+    mbar_init(big_full, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == AB_W_MMA) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-  // relative-position bias: the window of this head's vector the CTA can touch, in shared memory (the dS tile buffers of the
-  // pre-TMEM design are unused), pre-multiplied by log2 e and zero-padded past the vector
-  [[maybe_unused]] const int b_lo = (p.seq_q - 1) - min(q0 + AB_BM - 1, p.seq_q - 1);
-  [[maybe_unused]] const int b_len = AB_BM + n_steps * AB_BN;
-  [[maybe_unused]] const bool bias_in_smem = kBias && b_len <= (2 * S::T_BYTES) / 4;
-  if constexpr (kBias) {
-    if (bias_in_smem) {
-      float* bs = reinterpret_cast<float*>(smem + S::OFF_T0);
-      const int n_rel_ = p.seq_q + p.seq_kv - 1;
-      const float* src = p.rel_bias + int64_t(head) * n_rel_ + b_lo;
-      for (int i = threadIdx.x; i < b_len; i += AB_THREADS) bs[i] = (b_lo + i < n_rel_) ? __ldg(src + i) * 1.4426950408889634f : 0.f;
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == AB_W_TMA) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dec<24>();
+    if (threadIdx.x == 0) {
+      const int qc = head * p.q_head_stride, dc = head * p.do_head_stride;
       const int kc = head * p.k_head_stride, vc = head * p.v_head_stride;
-      if constexpr (!kQT) {
-        const int qc = head * p.q_head_stride, dc = head * p.do_head_stride;
-        mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
+      mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
 #pragma unroll
-        for (int h = 0; h < D / 64; ++h) {
-          tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmQ, big_full, qc + h * 64, q0, b);
-          tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmdO, big_full, dc + h * 64, q0, b);
-        }
+      for (int h = 0; h < D / 64; ++h) {
+        tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmQ, big_full, qc + h * 64, q0, b);
+        tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmdO, big_full, dc + h * 64, q0, b);
       }
       int st = 0; uint32_t ph = 0;
       for (int j = 0; j < n_steps; ++j) {
@@ -195,243 +150,122 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         mbar_expect_tx(&sml_full[st], 2 * S::SML_BYTES);
 #pragma unroll
         for (int h = 0; h < D / 64; ++h) {
-          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmK, &sml_full[st], kc + h * 64,
-                      j * AB_BN, b);
-          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmV, &sml_full[st], vc + h * 64,
-                      j * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmK, &sml_full[st], kc + h * 64, j * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmV, &sml_full[st], vc + h * 64, j * AB_BN, b);
         }
         if (++st == STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp == AB_W_MMA) {
-    // Warp-uniform loop; one elected lane issues. Descriptors are base constants plus compile-time offsets (>> 4).
-    const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG0), 0, 1024);
-    const uint64_t dsc_do = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG1), 0, 1024);
-    const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), 0, 1024);          // K-major view (S)
-    const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), 0, 1024);
-    const uint64_t dsc_kmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);  // MN-major view (dQ)
-    auto issue_s_dp = [&](int buf, int st) {
-      if (elect_one()) {
-        const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t oa = ((kk / 4) * (AB_BM * 128) + (kk % 4) * 32) >> 4, ob = ((kk / 4) * (AB_BN * 128) + (kk % 4) * 32) >> 4;
-          if constexpr (kQT) umma_bf16_ts(tmem_base + TM_S + buf * 128, tmem_base + TM_Q + kk * 8, dsc_k + sto + ob, IDESC_S, kk != 0);
-          else umma_bf16(tmem_base + TM_S + buf * 128, dsc_q + oa, dsc_k + sto + ob, IDESC_S, kk != 0);
-        }
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t oa = ((kk / 4) * (AB_BM * 128) + (kk % 4) * 32) >> 4, ob = ((kk / 4) * (AB_BN * 128) + (kk % 4) * 32) >> 4;
-          if constexpr (kQT) umma_bf16_ts(tmem_base + TM_S + buf * 128 + 64, tmem_base + TM_DO + kk * 8, dsc_v + sto + ob, IDESC_S, kk != 0);
-          else umma_bf16(tmem_base + TM_S + buf * 128 + 64, dsc_do + oa, dsc_v + sto + ob, IDESC_S, kk != 0);
-        }
-        umma_commit(&s_full[buf]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(big_full, 0);   // Q and dO rows are in TMEM
-    tc_fence_after();
-    if (n_steps > 0) {
-      mbar_wait(&sml_full[0], 0);
-      tc_fence_after();
-      issue_s_dp(0, 0);
-    }
-    int st = 0; uint32_t ph = 0;
-    for (int j = 0; j < n_steps; ++j) {
-      int st1 = st + 1; uint32_t ph1 = ph;
-      if (st1 == STAGES) { st1 = 0; ph1 ^= 1; }
-      TRACE(1, j, 0);
-      if (j + 1 < n_steps) {
-        mbar_wait(&sml_full[st1], ph1);
-        TRACE(1, j, 1);
-        tc_fence_after();
-        issue_s_dp((j + 1) & 1, st1);
-      }
-      TRACE(1, j, 2);
-      mbar_wait(&t_ready[j & 1], (j >> 1) & 1);
-      TRACE(1, j, 3);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t db = dsc_kmn + uint64_t(st) * (S::SML_BYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < AB_BN / 16; ++kk)   // dS(j): key slice kk sits where column part kk read its S values
-          umma_bf16_ts(tmem_base + TM_DQ, tmem_base + TM_S + (j & 1) * 128 + 16 * kk, db + ((kk * 2048) >> 4), IDESC_DQ,
-                       (j | kk) != 0);
-        umma_commit(&sml_empty[st]);
-      }
-      __syncwarp();
-      TRACE(1, j, 4);
-      st = st1; ph = ph1;
-    }
-    if (elect_one()) umma_commit(done);
-    __syncwarp();
-  } else {
-    // ---- math warps: four threads per query row (warps w, w+4, w+8, w+12 share a TMEM lane quadrant, 16 key columns each)
-    const int quad = warp & 3, part = warp >> 2;
-    const int r_in = quad * 32 + lane;
-    const int q_row = q0 + r_in;
-    const uint32_t t_lane = tmem_base + (uint32_t(quad * 32) << 16);
-    const bool row_ok = q_row < p.seq_q;
-    const int64_t stat_idx = (int64_t(b) * p.nheads + head) * p.seq_q + q_row;
-    const float lse = row_ok ? p.lse[stat_idx] : INFINITY;
-    const float delta = row_ok ? p.delta[stat_idx] : 0.f;
-    const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
-    const int kmax = p.causal ? min(q_row, p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
-    // relative-position bias (mT5): this row reads entries (c0 + c - q_row + seq_q - 1) of its head's vector
-    const int n_rel = p.seq_q + p.seq_kv - 1;
-    const float* brow = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row, p.seq_q - 1)) : nullptr;
-    [[maybe_unused]] const int bias_k0 = (p.seq_q - 1 - min(q_row, p.seq_q - 1)) - b_lo;   // this row's offset into the smem window
-    float* dpart = kBias && p.dbias_part
-                       ? p.dbias_part + (((int64_t(b) * p.nheads + head) * gridDim.x + tile) * (AB_MATH / 32) + warp) * p.dbias_tstride
-                       : nullptr;
-    if constexpr (kQT) {  // park this thread's quarter of its Q and dO rows in TMEM (bf16 pairs, column = d / 2): the A operands of S and dP
-      constexpr int W = D / 2 / AB_PARTS;   // 32-bit words per thread: 8 (D = 64) or 16 (D = 128)
-      uint32_t wq[W], wd[W];
-      const uint4* gq = reinterpret_cast<const uint4*>(p.q + (int64_t(b) * p.seq_q + q_row) * p.q_row_stride +
-                                                       int64_t(head) * p.q_head_stride + part * (2 * W));
-      const uint4* gd = reinterpret_cast<const uint4*>(p.dout + (int64_t(b) * p.seq_q + q_row) * p.do_row_stride +
-                                                       int64_t(head) * p.do_head_stride + part * (2 * W));
-#pragma unroll
-      for (int i = 0; i < W / 4; ++i) {
-        const uint4 a = row_ok ? gq[i] : make_uint4(0, 0, 0, 0), c = row_ok ? gd[i] : make_uint4(0, 0, 0, 0);
-        wq[4 * i] = a.x; wq[4 * i + 1] = a.y; wq[4 * i + 2] = a.z; wq[4 * i + 3] = a.w;
-        wd[4 * i] = c.x; wd[4 * i + 1] = c.y; wd[4 * i + 2] = c.z; wd[4 * i + 3] = c.w;
-      }
-      if constexpr (W == 8) { tmem_st8(t_lane + TM_Q + part * W, wq); tmem_st8(t_lane + TM_DO + part * W, wd); }
-      else { tmem_st16(t_lane + TM_Q + part * W, wq); tmem_st16(t_lane + TM_DO + part * W, wd); }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(big_full);
-    }
-    for (int j = 0; j < n_steps; ++j) {
-      const int buf = j & 1;
-      TRACE(0, j, 0);
-      mbar_wait(&s_full[buf], (j >> 1) & 1);
-      TRACE(0, j, 1);
-      tc_fence_after();
-      uint32_t s[AB_PC], d[AB_PC];
-      tmem_ld16(t_lane + TM_S + buf * 128 + part * AB_PC, s);
-      tmem_ld16(t_lane + TM_S + buf * 128 + 64 + part * AB_PC, d);
-      tmem_ld_wait();
-      TRACE(0, j, 2);
-      const int c0 = j * AB_BN + part * AB_PC;
-      const bool need_mask = (p.causal && j * AB_BN + AB_BN - 1 > q0) || (j * AB_BN + AB_BN > p.seq_kv) || mrow;
-      uint32_t pk[AB_PC / 2];
-      [[maybe_unused]] float bl[AB_PC];   // bias of this thread's columns, log2 domain
-      [[maybe_unused]] float ds[AB_PC];   // dS in fp32 (for the bias gradient)
-      if constexpr (kBias) {
-        constexpr float kLog2e = 1.4426950408889634f;
-        if (bias_in_smem) {
-          const float* bs = reinterpret_cast<const float*>(smem + S::OFF_T0) + bias_k0 + c0;
-#pragma unroll
-          for (int c = 0; c < AB_PC; ++c) bl[c] = bs[c];
-        } else {
-#pragma unroll
-          for (int c = 0; c < AB_PC; ++c) bl[c] = __ldg(brow + min(c0 + c, p.seq_kv - 1)) * kLog2e;
-        }
-      }
-      if (!need_mask) {
-#pragma unroll
-        for (int c = 0; c < AB_PC; c += 2) {
-          float x0 = __uint_as_float(s[c]) * p.scale_log2 - lse, x1 = __uint_as_float(s[c + 1]) * p.scale_log2 - lse;
-          if constexpr (kBias) { x0 += bl[c]; x1 += bl[c + 1]; }
-          const float d0 = ex2_approx(x0) * (__uint_as_float(d[c]) - delta), d1 = ex2_approx(x1) * (__uint_as_float(d[c + 1]) - delta);
-          if constexpr (kBias) { ds[c] = d0; ds[c + 1] = d1; }
-          pk[c >> 1] = pack_bf16x2(d0, d1);
-        }
-      } else if (mrow == nullptr) {
-        // causal / ragged tail: a per-row column limit, applied as a select on the probability (no per-element branches —
-        // the branchy form made a diagonal step cost 2000 cycles against 1000 for an interior one)
-        const int lim = kmax - c0;                // keep columns c <= lim
-#pragma unroll
-        for (int c = 0; c < AB_PC; c += 2) {
-          float x0 = __uint_as_float(s[c]) * p.scale_log2 - lse, x1 = __uint_as_float(s[c + 1]) * p.scale_log2 - lse;
-          if constexpr (kBias) { x0 += bl[c]; x1 += bl[c + 1]; }
-          const float e0 = ex2_approx(x0), e1 = ex2_approx(x1);
-          const float p0 = (c <= lim) ? e0 : 0.f, p1 = (c + 1 <= lim) ? e1 : 0.f;
-          const float d0 = p0 * (__uint_as_float(d[c]) - delta), d1 = p1 * (__uint_as_float(d[c + 1]) - delta);
-          if constexpr (kBias) { ds[c] = d0; ds[c + 1] = d1; }
-          pk[c >> 1] = pack_bf16x2(d0, d1);
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < AB_PC; c += 2) {
-          float pv[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = c0 + c + e;
-            bool keep = col < p.seq_kv && !(p.causal && col > q_row);
-            if (keep) keep = mrow[col] != 0;
-            float x = __uint_as_float(s[c + e]) * p.scale_log2 - lse;
-            if constexpr (kBias) x += bl[c + e];
-            const float pe = ex2_approx(x);
-            pv[e] = keep ? pe : 0.f;
-          }
-          const float d0 = pv[0] * (__uint_as_float(d[c]) - delta), d1 = pv[1] * (__uint_as_float(d[c + 1]) - delta);
-          if constexpr (kBias) { ds[c] = d0; ds[c + 1] = d1; }
-          pk[c >> 1] = pack_bf16x2(d0, d1);
-        }
-      }
-      if constexpr (kBias) {
-        // Bias gradient: dBias[h, r] = sum over (b, q) of dS[q, q + r]. Sum this warp's 32 rows x 16 columns along the
-        // diagonals with a systolic shuffle (A_c[l] = dS[l][c] + A_{c-1}[l-1]): after column c the value leaving lane 31 is
-        // the finished diagonal c - 32, after the last column lane l holds diagonal 15 - l. The 47 sums go to this warp's
-        // private slice of the workspace (slot = diagonal + 31 of step j; steps do not overlap: 47 < 64), plain stores, no
-        // atomics — attn_dbias_reduce_kernel adds the slices up in a fixed order.
-        if (dpart != nullptr) {
-          float A = 0.f, E[AB_PC];
-#pragma unroll
-          for (int c = 0; c < AB_PC; ++c) {
-            const float t = __shfl_sync(0xffffffffu, A, (lane + 31) & 31);
-            E[c] = t;
-            A = ds[c] + (lane == 0 ? 0.f : t);
-          }
-          float* dst = dpart + int64_t(j) * 64;
-          dst[46 - lane] = A;
-          if (lane == 0) {
-#pragma unroll
-            for (int c = 1; c < AB_PC; ++c) dst[c - 1] = E[c];
-          }
-        }
-      }
-      tmem_st8(t_lane + TM_S + buf * 128 + part * AB_PC, pk);   // dS(j) over the S(j) columns this thread has consumed
-      TRACE(0, j, 3);
-      tmem_st_wait();
-      TRACE(0, j, 4);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_ready[buf]);
-      TRACE(0, j, 5);
-    }
-    // ---- epilogue: the four threads of a row take 16-column chunks of dQ (chunk index = cc * 4 + part)
-    mbar_wait(done, 0);
-    tc_fence_after();
-    if (n_steps > 0) {
-      __nv_bfloat16* dqp = p.dq + (int64_t(b) * p.seq_q + q_row) * p.dq_row_stride + int64_t(head) * p.dq_head_stride;
-#pragma unroll
-      for (int cc = 0; cc < D / 64; ++cc) {
-        const int ch = cc * AB_PARTS + part;
-        uint32_t t[AB_PC];
-        tmem_ld16(t_lane + TM_DQ + ch * AB_PC, t);
-        tmem_ld_wait();
-        if (row_ok) {
-#pragma unroll
-          for (int c = 0; c < AB_PC; c += 8) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(t[c + e]) * p.scale;
-            *reinterpret_cast<uint4*>(dqp + ch * AB_PC + c) = pack8(f);
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == AB_W_MMA) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
+
+  reg_inc<240>();
+  const int wg = (threadIdx.x >> 7) - 1;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows r_lo, r_lo + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG0) + wg * (64 * 128), 0, 1024);
+  const uint64_t dsc_do = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG1) + wg * (64 * 128), 0, 1024);
+  const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), 0, 1024);              // K-major view (S)
+  const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), 0, 1024);
+  const uint64_t dsc_kmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);  // MN-major view (dQ)
+  const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
+  const int n_rel = p.seq_q + p.seq_kv - 1;
+  int q_row[2], kmax[2];
+  float lse[2], delta[2];
+  const float* brow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    q_row[h] = q0 + r_lo + 8 * h;
+    const bool ok = q_row[h] < p.seq_q;
+    const int64_t si = (int64_t(b) * p.nheads + head) * p.seq_q + q_row[h];
+    lse[h] = ok ? p.lse[si] : INFINITY;
+    delta[h] = ok ? p.delta[si] : 0.f;
+    kmax[h] = p.causal ? min(q_row[h], p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
+    // relative-position bias (mT5): this row reads entries (k - q_row + seq_q - 1) of its head's vector
+    brow[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row[h], p.seq_q - 1)) : nullptr;
+  }
+  float* dpart = kBias && p.dbias_part ? p.dbias_part + ((int64_t(b) * p.nheads + head) * gridDim.x + tile) * n_all * AB_DSTRIDE
+                                       : nullptr;
+  float dq[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
+
+  mbar_wait(big_full, 0);
+  for (int j = 0; j < n_steps; ++j) {
+    const int st = j % STAGES;
+    const uint32_t ph = (j / STAGES) & 1;
+    const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
+    float s[32], dp[32];
+    mbar_wait(&sml_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss_n64<0, 0>(s, dsc_q + (kslice(kk, AB_BM) >> 4), dsc_k + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss_n64<0, 0>(dp, dsc_do + (kslice(kk, AB_BM) >> 4), dsc_v + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+    wgmma_fence_acc(dp);
+    const int c0 = j * AB_BN;
+    const bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int h = e >> 1, col = c0 + 8 * i + cq + (e & 1);
+        float x = s[4 * i + e] * p.scale_log2 - lse[h];
+        if constexpr (kBias) x = fmaf(__ldg(brow[h] + min(col, p.seq_kv - 1)), 1.4426950408889634f, x);
+        float pe = ex2_approx(x);
+        if (need_mask) {
+          bool keep = col <= kmax[h];
+          if (mrow != nullptr && keep) keep = mrow[col] != 0;
+          pe = keep ? pe : 0.f;
+        }
+        s[4 * i + e] = pe * (dp[4 * i + e] - delta[h]);   // dS
+      }
+    }
+    if constexpr (kBias) {
+      // Bias gradient: dBias[h, k - q] = sum of dS over each diagonal. The step's 128 x 64 dS tile goes to shared memory and
+      // thread t sums diagonal t - 127 of it in row order into its own slot of the workspace (plain stores, no atomics);
+      // attn_dbias_reduce_kernel adds the slots up in a fixed order.
+      if (dpart != nullptr) {
+        float* tds = reinterpret_cast<float*>(smem + S::OFF_DS);
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) tds[(r_lo + 8 * (e >> 1)) * (AB_BN + 1) + 8 * i + cq + (e & 1)] = s[4 * i + e];
+        bar_sync(1, 256);
+        const int t = threadIdx.x - 128;
+        if (t < AB_NDIAG) {
+          const int o = t - (AB_BM - 1);
+          float acc = 0.f;
+          for (int r = max(0, -o); r < min(AB_BM, AB_BN - o); ++r) acc += tds[r * (AB_BN + 2) + o];
+          dpart[int64_t(j) * AB_DSTRIDE + t] = acc;
+        }
+        bar_sync(1, 256);
+      }
+    }
+    uint32_t a[AB_BN / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < AB_BN / 16; ++kk) to_frag(s, kk, a[kk]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dq, a[kk], dsc_kmn + sto + ((kk * 2048) >> 4));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(dq);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sml_empty[st]);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (q_row[h] >= p.seq_q) continue;
+    __nv_bfloat16* dqp = p.dq + (int64_t(b) * p.seq_q + q_row[h]) * p.dq_row_stride + int64_t(head) * p.dq_head_stride + cq;
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i)
+      *reinterpret_cast<uint32_t*>(dqp + 8 * i) = pack_bf16x2(dq[4 * i + 2 * h] * p.scale, dq[4 * i + 2 * h + 1] * p.scale);
   }
 }
 
@@ -441,30 +275,14 @@ __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                     const AttBwdParams p) {
-  using S = AttBwdSmem<D, (D == 64 ? 6 : 3), 4>;
+  using S = AttBwdSmem<D, false>;
   constexpr int STAGES = S::STAGES;
-  constexpr int TMEM_COLS = 512;
-  constexpr int TM_S = 0;             // S^T[buf] at buf*128, dP^T[buf] at buf*128 + 64
-  constexpr int TM_DV = 256;          // D columns
-  constexpr int TM_DK = 256 + D;      // D columns (D <= 128)
-  // K / V rows as TMEM-resident A operands of S^T and dP^T (fits only at D = 64). Implemented and parity-tested, but measured
-  // +2.5 % on the whole backward (the A reads compete with the math warps' tcgen05.ld / st for TMEM bandwidth): left off.
-  constexpr bool kKT = false;
-  [[maybe_unused]] constexpr int TM_K = 256 + 2 * D;   // D/2 columns
-  [[maybe_unused]] constexpr int TM_V = 256 + 2 * D + D / 2;
-  constexpr uint32_t IDESC_S = make_idesc_bf16(AB_BM, AB_BN, 0, 0);
-  constexpr uint32_t IDESC_DKV = make_idesc_bf16(AB_BM, D, 0, 1);
-
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
   uint64_t* big_full = bars;
   uint64_t* sml_full = big_full + 1;
   uint64_t* sml_empty = sml_full + STAGES;
-  uint64_t* s_full = sml_empty + STAGES;
-  uint64_t* t_ready = s_full + 2;
-  uint64_t* done = t_ready + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(done + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x;  // early key tiles see the most queries under a causal mask: they come first already
@@ -474,31 +292,24 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int i_start = p.causal ? min(n_q, kv0 / AB_BN) : 0;
   const int n_steps = n_q - i_start;
 
-  if (warp == AB_W_TMA && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-    mbar_init(big_full, kKT ? AB_MATH / 32 : 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&t_ready[i], AB_MATH / 32); }
-    mbar_init(done, 1);
+    mbar_init(big_full, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == AB_W_MMA) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == AB_W_TMA) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dec<24>();
+    if (threadIdx.x == 0) {
       const int qc = head * p.q_head_stride, dc = head * p.do_head_stride;
       const int kc = head * p.k_head_stride, vc = head * p.v_head_stride;
-      if constexpr (!kKT) {
-        mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
+      mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
 #pragma unroll
-        for (int h = 0; h < D / 64; ++h) {
-          tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmK, big_full, kc + h * 64, kv0, b);
-          tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmV, big_full, vc + h * 64, kv0, b);
-        }
+      for (int h = 0; h < D / 64; ++h) {
+        tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmK, big_full, kc + h * 64, kv0, b);
+        tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmV, big_full, vc + h * 64, kv0, b);
       }
       int st = 0; uint32_t ph = 0;
       for (int i = 0; i < n_steps; ++i) {
@@ -514,202 +325,110 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         if (++st == STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp == AB_W_MMA) {
-    const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG0), 0, 1024);
-    const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG1), 0, 1024);
-    const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), 0, 1024);           // K-major view (S^T)
-    const uint64_t dsc_do = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), 0, 1024);
-    const uint64_t dsc_qmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);  // MN-major view (dK)
-    const uint64_t dsc_domn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), AB_BN * 128, 1024); // MN-major view (dV)
-    auto issue_st_dpt = [&](int buf, int st) {
-      if (elect_one()) {
-        const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t oa = ((kk / 4) * (AB_BM * 128) + (kk % 4) * 32) >> 4, ob = ((kk / 4) * (AB_BN * 128) + (kk % 4) * 32) >> 4;
-          if constexpr (kKT) umma_bf16_ts(tmem_base + TM_S + buf * 128, tmem_base + TM_K + kk * 8, dsc_q + sto + ob, IDESC_S, kk != 0);
-          else umma_bf16(tmem_base + TM_S + buf * 128, dsc_k + oa, dsc_q + sto + ob, IDESC_S, kk != 0);
-        }
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t oa = ((kk / 4) * (AB_BM * 128) + (kk % 4) * 32) >> 4, ob = ((kk / 4) * (AB_BN * 128) + (kk % 4) * 32) >> 4;
-          if constexpr (kKT) umma_bf16_ts(tmem_base + TM_S + buf * 128 + 64, tmem_base + TM_V + kk * 8, dsc_do + sto + ob, IDESC_S, kk != 0);
-          else umma_bf16(tmem_base + TM_S + buf * 128 + 64, dsc_v + oa, dsc_do + sto + ob, IDESC_S, kk != 0);
-        }
-        umma_commit(&s_full[buf]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(big_full, 0);
-    tc_fence_after();
-    if (n_steps > 0) {
-      mbar_wait(&sml_full[0], 0);
-      tc_fence_after();
-      issue_st_dpt(0, 0);
-    }
-    int st = 0; uint32_t ph = 0;
-    for (int i = 0; i < n_steps; ++i) {
-      int st1 = st + 1; uint32_t ph1 = ph;
-      if (st1 == STAGES) { st1 = 0; ph1 ^= 1; }
-      if (i + 1 < n_steps) {
-        mbar_wait(&sml_full[st1], ph1);
-        tc_fence_after();
-        issue_st_dpt((i + 1) & 1, st1);
-      }
-      mbar_wait(&t_ready[i & 1], (i >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        // P^T(i) / dS^T(i) are read from TENSOR MEMORY: query slice kk sits where column part kk read its S^T / dP^T values
-        const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
-        const uint32_t ta = tmem_base + TM_S + (i & 1) * 128;
-#pragma unroll
-        for (int kk = 0; kk < AB_BN / 16; ++kk)
-          umma_bf16_ts(tmem_base + TM_DV, ta + 16 * kk, dsc_domn + sto + ((kk * 2048) >> 4), IDESC_DKV, (i | kk) != 0);
-#pragma unroll
-        for (int kk = 0; kk < AB_BN / 16; ++kk)
-          umma_bf16_ts(tmem_base + TM_DK, ta + 64 + 16 * kk, dsc_qmn + sto + ((kk * 2048) >> 4), IDESC_DKV, (i | kk) != 0);
-        umma_commit(&sml_empty[st]);
-      }
-      __syncwarp();
-      st = st1; ph = ph1;
-    }
-    if (elect_one()) umma_commit(done);
-    __syncwarp();
-  } else {
-    // ---- math warps: four threads per KEY row (16 query columns each)
-    const int quad = warp & 3, part = warp >> 2;
-    const int r_in = quad * 32 + lane;
-    const int kv_row = kv0 + r_in;
-    const uint32_t t_lane = tmem_base + (uint32_t(quad * 32) << 16);
-    bool row_ok = kv_row < p.seq_kv;
-    const bool store_ok = row_ok;
-    if (row_ok && p.kv_mask) row_ok = p.kv_mask[int64_t(b) * p.seq_kv + kv_row] != 0;
-    const int64_t stat_base = (int64_t(b) * p.nheads + head) * p.seq_q;
-    const bool vec_stats = (p.seq_q % 4) == 0;   // 16-byte aligned rows of lse / delta
-    // relative-position bias: key row kv_row, query column qi -> entry (kv_row - qi + seq_q - 1) of the head's vector
-    const int n_rel = p.seq_q + p.seq_kv - 1;
-    const float* bkey = kBias ? p.rel_bias + int64_t(head) * n_rel + (min(kv_row, p.seq_kv - 1) + p.seq_q - 1) : nullptr;
-    if constexpr (kKT) {  // park this thread's quarter of its K and V rows in TMEM (A operands of S^T and dP^T)
-      constexpr int W = D / 2 / AB_PARTS;
-      uint32_t wk[W], wv[W];
-      const uint4* gk = reinterpret_cast<const uint4*>(p.k + (int64_t(b) * p.seq_kv + kv_row) * p.k_row_stride +
-                                                       int64_t(head) * p.k_head_stride + part * (2 * W));
-      const uint4* gv = reinterpret_cast<const uint4*>(p.v + (int64_t(b) * p.seq_kv + kv_row) * p.v_row_stride +
-                                                       int64_t(head) * p.v_head_stride + part * (2 * W));
-#pragma unroll
-      for (int i = 0; i < W / 4; ++i) {
-        const uint4 a = store_ok ? gk[i] : make_uint4(0, 0, 0, 0), c = store_ok ? gv[i] : make_uint4(0, 0, 0, 0);
-        wk[4 * i] = a.x; wk[4 * i + 1] = a.y; wk[4 * i + 2] = a.z; wk[4 * i + 3] = a.w;
-        wv[4 * i] = c.x; wv[4 * i + 1] = c.y; wv[4 * i + 2] = c.z; wv[4 * i + 3] = c.w;
-      }
-      if constexpr (W == 8) { tmem_st8(t_lane + TM_K + part * W, wk); tmem_st8(t_lane + TM_V + part * W, wv); }
-      else { tmem_st16(t_lane + TM_K + part * W, wk); tmem_st16(t_lane + TM_V + part * W, wv); }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(big_full);
-    }
-    for (int i = 0; i < n_steps; ++i) {
-      const int buf = i & 1;
-      const int qt0 = (i_start + i) * AB_BN;
-      // lse / delta of this thread's 16 query columns: same addresses in every lane (one broadcast transaction per load),
-      // issued before the wait on the tensor core so that their latency hides behind it
-      float lse_c[AB_PC], del_c[AB_PC];
-      const int qc0 = qt0 + part * AB_PC;
-      if (vec_stats && qc0 + AB_PC <= p.seq_q) {
-#pragma unroll
-        for (int c = 0; c < AB_PC; c += 4) {
-          const float4 l4 = __ldg(reinterpret_cast<const float4*>(p.lse + stat_base + qc0 + c));
-          const float4 d4 = __ldg(reinterpret_cast<const float4*>(p.delta + stat_base + qc0 + c));
-          lse_c[c] = l4.x; lse_c[c + 1] = l4.y; lse_c[c + 2] = l4.z; lse_c[c + 3] = l4.w;
-          del_c[c] = d4.x; del_c[c + 1] = d4.y; del_c[c + 2] = d4.z; del_c[c + 3] = d4.w;
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < AB_PC; ++c) {
-          const int qi = qc0 + c;
-          lse_c[c] = qi < p.seq_q ? __ldg(p.lse + stat_base + qi) : INFINITY;
-          del_c[c] = qi < p.seq_q ? __ldg(p.delta + stat_base + qi) : 0.f;
-        }
-      }
-      mbar_wait(&s_full[buf], (i >> 1) & 1);
-      tc_fence_after();
-      uint32_t s[AB_PC], d[AB_PC];
-      tmem_ld16(t_lane + TM_S + buf * 128 + part * AB_PC, s);
-      tmem_ld16(t_lane + TM_S + buf * 128 + 64 + part * AB_PC, d);
-      tmem_ld_wait();
-      const bool need_causal = p.causal && (qt0 < kv0 + AB_BM - 1);
-      uint32_t pp[AB_PC / 2], pd[AB_PC / 2];
-#pragma unroll
-      for (int c = 0; c < AB_PC; c += 2) {
-        float pv[2], dv[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float arg = __uint_as_float(s[c + e]) * p.scale_log2 - lse_c[c + e];
-          if constexpr (kBias) arg += __ldg(bkey - min(qc0 + c + e, p.seq_q - 1)) * 1.4426950408889634f;
-          float x = ex2_approx(arg);
-          const bool keep = row_ok && !(need_causal && (qc0 + c + e) < kv_row);
-          x = keep ? x : 0.f;
-          pv[e] = x;
-          dv[e] = x * (__uint_as_float(d[c + e]) - del_c[c + e]);
-        }
-        pp[c >> 1] = pack_bf16x2(pv[0], pv[1]);
-        pd[c >> 1] = pack_bf16x2(dv[0], dv[1]);
-      }
-      // P^T(i) / dS^T(i) go back to TMEM over the S^T / dP^T columns this thread has just consumed (A operands of dV / dK)
-      tmem_st8(t_lane + TM_S + buf * 128 + part * AB_PC, pp);
-      tmem_st8(t_lane + TM_S + buf * 128 + 64 + part * AB_PC, pd);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_ready[buf]);
-    }
-    // ---- epilogue: dV, dK; the four threads of a row take 16-column chunks (chunk index = cc * 4 + part)
-    mbar_wait(done, 0);
-    tc_fence_after();
-    __nv_bfloat16* dvp = p.dv + (int64_t(b) * p.seq_kv + kv_row) * p.dv_row_stride + int64_t(head) * p.dv_head_stride;
-    __nv_bfloat16* dkp = p.dk + (int64_t(b) * p.seq_kv + kv_row) * p.dk_row_stride + int64_t(head) * p.dk_head_stride;
-#pragma unroll
-    for (int which = 0; which < 2; ++which) {
-#pragma unroll
-      for (int cc = 0; cc < D / 64; ++cc) {
-        const int ch = cc * AB_PARTS + part;
-        uint32_t t[AB_PC];
-        if (n_steps > 0) {
-          tmem_ld16(t_lane + (which == 0 ? TM_DV : TM_DK) + ch * AB_PC, t);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int c = 0; c < AB_PC; ++c) t[c] = 0u;
-        }
-        if (store_ok) {
-          const float mul = which == 0 ? 1.f : p.scale;
-          __nv_bfloat16* dst = (which == 0 ? dvp : dkp) + ch * AB_PC;
-#pragma unroll
-          for (int c = 0; c < AB_PC; c += 8) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(t[c + e]) * mul;
-            *reinterpret_cast<uint4*>(dst + c) = pack8(f);
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == AB_W_MMA) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
+
+  reg_inc<240>();
+  const int wg = (threadIdx.x >> 7) - 1;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // key rows r_lo, r_lo + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG0) + wg * (64 * 128), 0, 1024);
+  const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_BIG1) + wg * (64 * 128), 0, 1024);
+  const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), 0, 1024);               // K-major view (S^T)
+  const uint64_t dsc_do = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), 0, 1024);
+  const uint64_t dsc_qmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);   // MN-major view (dK)
+  const uint64_t dsc_domn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), AB_BN * 128, 1024);  // MN-major view (dV)
+  const int64_t stat_base = (int64_t(b) * p.nheads + head) * p.seq_q;
+  const int n_rel = p.seq_q + p.seq_kv - 1;
+  int kv_row[2];
+  bool row_ok[2];
+  const float* bkey[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    kv_row[h] = kv0 + r_lo + 8 * h;
+    row_ok[h] = kv_row[h] < p.seq_kv && (p.kv_mask == nullptr || p.kv_mask[int64_t(b) * p.seq_kv + kv_row[h]] != 0);
+    // relative-position bias: key row kv_row, query column qi -> entry (kv_row - qi + seq_q - 1) of the head's vector
+    bkey[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (min(kv_row[h], p.seq_kv - 1) + p.seq_q - 1) : nullptr;
+  }
+  float dv[D / 2], dk[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+
+  mbar_wait(big_full, 0);
+  for (int i = 0; i < n_steps; ++i) {
+    const int st = i % STAGES;
+    const uint32_t ph = (i / STAGES) & 1;
+    const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
+    const int qt0 = (i_start + i) * AB_BN;
+    float s[32], dp[32];
+    mbar_wait(&sml_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss_n64<0, 0>(s, dsc_k + (kslice(kk, AB_BM) >> 4), dsc_q + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss_n64<0, 0>(dp, dsc_v + (kslice(kk, AB_BM) >> 4), dsc_do + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+    wgmma_fence_acc(dp);
+    const bool need_causal = p.causal && (qt0 < kv0 + AB_BM - 1);
+#pragma unroll
+    for (int ii = 0; ii < 8; ++ii) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int qi = qt0 + 8 * ii + cq + c;
+        const bool q_ok = qi < p.seq_q;
+        const float lse_c = q_ok ? __ldg(p.lse + stat_base + qi) : INFINITY;
+        const float del_c = q_ok ? __ldg(p.delta + stat_base + qi) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int e = 2 * h + c;
+          float arg = s[4 * ii + e] * p.scale_log2 - lse_c;
+          if constexpr (kBias) arg = fmaf(__ldg(bkey[h] - min(qi, p.seq_q - 1)), 1.4426950408889634f, arg);
+          float x = ex2_approx(arg);
+          const bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]);
+          x = keep ? x : 0.f;
+          s[4 * ii + e] = x;                                  // P^T
+          dp[4 * ii + e] = x * (dp[4 * ii + e] - del_c);      // dS^T
+        }
+      }
+    }
+    uint32_t pa[AB_BN / 16][4], da[AB_BN / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < AB_BN / 16; ++kk) { to_frag(s, kk, pa[kk]); to_frag(dp, kk, da[kk]); }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dv, pa[kk], dsc_domn + sto + ((kk * 2048) >> 4));
+#pragma unroll
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dk, da[kk], dsc_qmn + sto + ((kk * 2048) >> 4));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(dv);
+    wgmma_fence_acc(dk);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sml_empty[st]);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (kv_row[h] >= p.seq_kv) continue;
+    __nv_bfloat16* dvp = p.dv + (int64_t(b) * p.seq_kv + kv_row[h]) * p.dv_row_stride + int64_t(head) * p.dv_head_stride + cq;
+    __nv_bfloat16* dkp = p.dk + (int64_t(b) * p.seq_kv + kv_row[h]) * p.dk_row_stride + int64_t(head) * p.dk_head_stride + cq;
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i) {
+      *reinterpret_cast<uint32_t*>(dvp + 8 * i) = pack_bf16x2(dv[4 * i + 2 * h], dv[4 * i + 2 * h + 1]);
+      *reinterpret_cast<uint32_t*>(dkp + 8 * i) = pack_bf16x2(dk[4 * i + 2 * h] * p.scale, dk[4 * i + 2 * h + 1] * p.scale);
+    }
   }
 }
 
-// dBias[h, i] (+)= sum over (b, q tile, warp) of the per-warp diagonal sums the dQ kernel left in the workspace, in a FIXED
-// order (deterministic). i = (k - q) + seq_q - 1. Stage 1: grid (i chunks, heads, batch splits) -> part2[split][h][i];
-// stage 2 adds the splits onto the caller's fp32 vector.
+// dBias[h, i] (+)= sum over (b, q tile, step) of the diagonal sums the dQ kernel left in the workspace, in a FIXED order
+// (deterministic). i = (k - q) + seq_q - 1. Stage 1: grid (i chunks, heads, batch splits) -> part2[split][h][i]; stage 2 adds
+// the splits onto the caller's fp32 vector.
 __global__ void __launch_bounds__(128) attn_dbias_reduce_kernel(const float* __restrict__ part, float* __restrict__ part2,
                                                                 int batch, int nheads, int seq_q, int seq_kv, int causal,
-                                                                int n_qtiles, int64_t tstride, int bsplit) {
+                                                                int n_qtiles, int bsplit) {
   const int n_rel = seq_q + seq_kv - 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int h = blockIdx.y, sp = blockIdx.z;
@@ -722,13 +441,12 @@ __global__ void __launch_bounds__(128) attn_dbias_reduce_kernel(const float* __r
     for (int tile = 0; tile < n_qtiles; ++tile) {
       const int q0 = tile * AB_BM;
       const int n_steps = causal ? min(n_all, (min(q0 + AB_BM, seq_q) + AB_BN - 1) / AB_BN) : n_all;
-      const float* base = part + ((int64_t(b) * nheads + h) * n_qtiles + tile) * (AB_MATH / 32) * tstride;
-#pragma unroll 4
-      for (int w = 0; w < AB_MATH / 32; ++w) {
-        const int quad = w & 3, prt = w >> 2;
-        const int t = d + q0 + quad * 32 - prt * AB_PC + 31;
-        if (t >= 0 && (t & 63) < 47 && (t >> 6) < n_steps) acc += base[int64_t(w) * tstride + t];
-      }
+      const float* base = part + ((int64_t(b) * nheads + h) * n_qtiles + tile) * n_all * AB_DSTRIDE;
+      // step j holds the diagonal k - q = d in slot t = d + q0 - 64 j + 127 when 0 <= t < 191
+      const int hi = d + q0 + (AB_BM - 1), lo = d + q0 - (AB_BN - 1);
+      if (hi < 0) continue;
+      const int j_lo = lo <= 0 ? 0 : (lo + AB_BN - 1) / AB_BN, j_hi = min(n_steps - 1, hi / AB_BN);
+      for (int j = j_lo; j <= j_hi; ++j) acc += base[int64_t(j) * AB_DSTRIDE + (hi - j * AB_BN)];
     }
   }
   part2[(int64_t(sp) * nheads + h) * n_rel + i] = acc;
@@ -745,15 +463,15 @@ __global__ void __launch_bounds__(128) attn_dbias_final_kernel(const float* __re
 static inline int dbias_bsplit(int batch) { return batch < 16 ? batch : 16; }
 static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {
   const int64_t n_qt = (seq_q + AB_BM - 1) / AB_BM, n_all = (seq_kv + AB_BN - 1) / AB_BN;
-  return size_t(batch) * nheads * n_qt * (AB_MATH / 32) * n_all * 64;
+  return size_t(batch) * nheads * n_qt * n_all * AB_DSTRIDE;
 }
 
 template <int D, bool kBias>
 static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                            int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
                            float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
-  using SQ = AttBwdSmem<D, (D == 64 ? 6 : 4), 2>;
-  using SK = AttBwdSmem<D, (D == 64 ? 6 : 3), 4>;
+  using SQ = AttBwdSmem<D, kBias>;
+  using SK = AttBwdSmem<D, false>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<D, kBias>, cudaFuncAttributeMaxDynamicSharedMemorySize, SQ::TOTAL);
@@ -793,7 +511,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
     if (kBias && drel_bias != nullptr) {
       const int n_rel = p.seq_q + p.seq_kv - 1, bs = dbias_bsplit(p.batch);
       attn_dbias_reduce_kernel<<<dim3((n_rel + 127) / 128, p.nheads, bs), 128, 0, st>>>(
-          p.dbias_part, part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), p.dbias_tstride, bs);
+          p.dbias_part, part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), bs);
       FSB_CUDA_LAUNCH_CHECK();
       attn_dbias_final_kernel<<<dim3((n_rel + 127) / 128, p.nheads), 128, 0, st>>>(part2, drel_bias, p.nheads, n_rel, bs);
       FSB_CUDA_LAUNCH_CHECK();
@@ -811,12 +529,6 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
 }  // namespace fsb
 
 using namespace fsb;
-
-#ifdef FSB_ATTN_TRACE
-extern "C" int fsb_debug_attn_trace(long long* host_out /* [2][64][8] */) {
-  return cudaMemcpyFromSymbol(host_out, g_attn_trace, sizeof(long long) * 2 * 64 * 8) == cudaSuccess ? 0 : -2;
-}
-#endif
 
 extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                             const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q,
@@ -841,7 +553,7 @@ extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const v
   FSB_REQUIRE(drel_bias == nullptr || rel_bias != nullptr, "sdpa_bwd: drel_bias without rel_bias");
   AttBwdParams p;
   p.lse = lse; p.delta = delta; p.kv_mask = kv_mask;
-  p.rel_bias = rel_bias; p.dbias_part = nullptr; p.dbias_tstride = ((seq_kv + AB_BN - 1) / AB_BN) * 64;
+  p.rel_bias = rel_bias; p.dbias_part = nullptr;
   float* part2 = nullptr;
   if (drel_bias != nullptr) {
     const size_t need = fsb_sdpa_bwd_workspace_bytes(batch, seq_q, seq_kv, nheads);
@@ -851,8 +563,6 @@ extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const v
     p.dbias_part = static_cast<float*>(workspace);
     part2 = p.dbias_part + dbias_part_floats(batch, seq_q, seq_kv, nheads);
   }
-  p.q = (const __nv_bfloat16*)q; p.dout = (const __nv_bfloat16*)dout; p.q_row_stride = q_row_stride; p.do_row_stride = do_row_stride;
-  p.k = (const __nv_bfloat16*)k; p.v = (const __nv_bfloat16*)v; p.k_row_stride = k_row_stride; p.v_row_stride = v_row_stride;
   p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
   p.dq_row_stride = dq_row_stride; p.dk_row_stride = dk_row_stride; p.dv_row_stride = dv_row_stride;
   p.dq_head_stride = dq_head_stride; p.dk_head_stride = dk_head_stride; p.dv_head_stride = dv_head_stride;
@@ -870,7 +580,7 @@ extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const v
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {
   if (batch <= 0 || seq_q <= 0 || seq_kv <= 0 || nheads <= 0) return 0;
-  // per-warp diagonal sums of the dQ kernel + the batch-split partial vectors of the reduction
+  // per-step diagonal sums of the dQ kernel + the batch-split partial vectors of the reduction
   return (fsb::dbias_part_floats(batch, seq_q, seq_kv, nheads) +
           size_t(fsb::dbias_bsplit(int(batch))) * nheads * size_t(seq_q + seq_kv - 1)) * sizeof(float);
 }

@@ -1,22 +1,17 @@
-// fsb200 — fused scaled-dot-product attention, forward (flash-style online softmax on tcgen05 / TMEM).
+// fsb200 — fused scaled-dot-product attention, forward (flash-style online softmax on wgmma).
 // Replaces ParallelSelfAttention.flash_attention (fengshen/models/megatron/layers/transformer.py:410-456, 3P
 // flash_attn_cuda.fwd) and the baddbmm -> FusedScaleMaskSoftmax -> bmm path (transformer.py:307-408): same math,
 //   O = softmax(scale * Q K^T + mask) V,  mask = causal and/or key-padding,
 // without the three repacking copies of q/k/v (transformer.py:419-429): Q, K, V are read straight out of the packed
 // QKV projection output through TMA tensor maps (any row/head stride), O is written in [token, head*dim] layout.
 //
-// CTA = one (batch, head, pair of 128-row Q tiles), 12 warps (warps 10-11 only donate registers through setmaxnreg):
-//   warps 0-3 / 4-7 : softmax group of Q tile 0 / 1. TMEM lane == query row == thread: a thread owns the 64 scores of its
-//                     row for the step, so row max / row sum need no cross-thread exchange; S(j+1) is prefetched from
-//                     TMEM into a second register set while the exponentials of step j run.
-//   warp 8          : TMA producer (Q once; K and V tiles through multi-stage rings)
-//   warp 9          : tcgen05.mma issuer: S_i(j) = Q_i K_j^T (128 x 64 x D), O_i += P_i(j) V_j (128 x D x 64)
-// S is double-buffered in TMEM and P in shared memory, so the tensor core runs S(j+1)/S(j+2) while the softmax group
-// works on step j; the two Q tiles interleave on top of that.
-// O ACCUMULATES IN TMEM across the whole key loop. The running max used as exponent reference (m_ref) is only raised
-// when the true row max exceeds it by more than 2^8 (lazy rescaling): then — rarely — the group multiplies its O rows
-// in TMEM by 2^(m_ref_old - m_new) (tcgen05.ld / tcgen05.st). Probabilities are therefore <= 256 instead of <= 1, well
-// inside bf16/fp32 range; the final O / l is exact in the same way as with the eager rescale.
+// CTA = one (batch, head, 128-row Q tile), 3 warpgroups:
+//   warpgroup 0     : TMA producer (Q once; K and V tiles through a multi-stage ring, separate full barriers so that
+//                     S = Q K^T can start before V has landed)
+//   warpgroups 1, 2 : 64 query rows each. S(j) = Q K_j^T (wgmma, both operands in shared memory, fp32 in registers),
+//                     online softmax in registers (a row lives in the four lanes of a quad), then O += P(j) V_j with P as
+//                     the register A operand — P never touches shared memory.
+// The two consumer warpgroups run independently on the same K/V stage, so one's softmax overlaps the other's MMAs.
 #include <stdlib.h>
 
 #include "host_common.h"
@@ -24,51 +19,23 @@
 
 namespace fsb {
 
-constexpr int ATT_BQ = 128;   // rows per Q tile (= TMEM lanes)
-// Q tiles per CTA (template parameter NQ): 2 = one CTA per SM working on two tiles; 1 = one tile per CTA and TWO CTAs per SM
-// (256 TMEM columns, ~97 KB of shared memory, 256 threads each): the same two tiles per SM, but as independent CTAs — one CTA's
-// prologue (TMEM allocation, barrier set-up, Q / first K, V round trips) and epilogue overlap the other's key loop, and the
-// two softmax groups are no longer marched in lockstep by a shared MMA-issue warp. At S <= 1024 the per-CTA fixed cost is of
-// the order of the key loop itself (D = 64: 250 TFLOP/s at S = 1024 against 400 at S = 8192 with NQ = 2).
-constexpr int ATT_BKV = 64;   // keys per inner step
-constexpr int ATT_GROUP = 128;                       // softmax threads per Q tile (one per row)
-// threads = NQ * 128 softmax + one more warpgroup: TMA warp, MMA warp, two idle warps (setmaxnreg donors)
-constexpr float ATT_RESCALE_TAU = 8.0f;              // log2 units
-// setmaxnreg split (a warpgroup shares one value): 256 softmax threads x ATT_SM_REGS + 128 (TMA / MMA / idle) x ATT_WG2_REGS
-// <= 65536. The softmax threads hold two 64-score register sets (S(j) and the prefetched S(j+1)): every register they do not
-// get shows up as local-memory traffic in the hot loop.
-#ifndef ATT_WG2_REGS
-#define ATT_WG2_REGS 72
-#endif
-#ifndef ATT_SM_REGS
-#define ATT_SM_REGS 216
-#endif
-// 216 / 72 leaves 1024 registers of the SM unclaimed. Do NOT close that gap: 232 / 48 (exactly 65536) never gets its
-// setmaxnreg.inc granted and the kernel hangs (measured the hard way, round 2).
-static_assert(256 * ATT_SM_REGS + 128 * ATT_WG2_REGS <= 65536 - 1024, "register file (keep the launch-time slack)");
-// NQ = 1 (two CTAs per SM, 128 + 128 threads each): 2 * 128 * (192 + 48) = 61440
-constexpr int ATT1_SM_REGS = 192, ATT1_WG2_REGS = 48;
+constexpr int ATT_BQ = 128;   // rows per Q tile (two consumer warpgroups x 64)
+constexpr int ATT_BKV = 128;  // keys per inner step
+constexpr int ATT_THREADS = 384;
 
-template <int D, int NQ>
+template <int D>
 struct AttFwdSmem {
-  // K/V ring depth (must cover the TMA round trip); NQ = 1 has to fit twice into an SM's shared memory
-  static constexpr int STAGES = NQ == 2 ? ((D == 128) ? 3 : 6) : ((D == 128) ? 2 : 5);
-  static constexpr int Q_BYTES = ATT_BQ * D * 2;           // per slot
+  static constexpr int STAGES = D == 128 ? 2 : 3;          // K/V ring depth
+  static constexpr int Q_BYTES = ATT_BQ * D * 2;
   static constexpr int KV_BYTES = ATT_BKV * D * 2;         // per tensor per stage
-  static constexpr int P_BYTES = ATT_BQ * ATT_BKV * 2;     // per slot per buffer
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = OFF_Q + NQ * Q_BYTES;
+  static constexpr int OFF_K = OFF_Q + Q_BYTES;
   static constexpr int OFF_V = OFF_K + STAGES * KV_BYTES;
-  static constexpr int OFF_P = OFF_V + STAGES * KV_BYTES;  // [slot][buf]
-  static constexpr int OFF_BAR = OFF_P + (NQ == 2 ? NQ * 2 * P_BYTES : 0);   // NQ = 1: P only ever travels through TMEM
-  // relative-position bias window (kBias && kPT && NQ == 2): the P tiles are not used with the TMEM hand-over, so their 64 KB hold
-  // the fp32 window of the head's bias vector this CTA can touch (pre-multiplied by log2 e): NQ * 128 + seq_kv (+63) entries
-  static constexpr int BIAS_FLOATS = (NQ == 2) ? (NQ * 2 * P_BYTES) / 4 : 0;
-  // q_full, k_full[S], k_empty[S], v_full[S], v_empty[S], s_full[2][2], p_ready[2][2], o_done[2]
-  static constexpr int NBAR = 1 + 4 * STAGES + 10;
-  static constexpr int TOTAL = OFF_BAR + NBAR * 8 + 16 + 1024;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into on sm_100");
-  static_assert(NQ == 2 || TOTAL + 1024 <= 232448 / 2, "NQ = 1 is meant to run two CTAs per SM");
+  static constexpr int OFF_BAR = OFF_V + STAGES * KV_BYTES;
+  // q_full, k_full[S], v_full[S], kv_empty[S]
+  static constexpr int NBAR = 1 + 3 * STAGES;
+  static constexpr int TOTAL = OFF_BAR + NBAR * 8 + 1024;
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
 };
 
 struct AttFwdParams {
@@ -83,397 +50,184 @@ struct AttFwdParams {
   float scale_log2;  // softmax scale * log2(e)
 };
 
-// Optional cycle trace of one CTA (development aid; compiled in only with -DFSB_ATTN_TRACE)
-#ifdef FSB_ATTN_TRACE
-__device__ long long g_fwd_trace[2][64][8];
-#define FTRACE(role, step, k) do { if (ftrace_on && (step) < 64) g_fwd_trace[role][step][k] = clock64(); } while (0)
-#else
-#define FTRACE(role, step, k) do { } while (0)
-#endif
+template <int D>
+__device__ __forceinline__ void wgmma_rs_d(float (&o)[D / 2], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (D == 128) wgmma_rs_n128<1>(o, a, db, 1u);
+  else wgmma_rs_n64<1>(o, a, db, 1u);
+}
 
-// kPT: P(j) is handed to the PV product through TENSOR MEMORY — each softmax thread writes its row's 64 probabilities (bf16
-// pairs, 32 columns) over the first half of the S(j) columns it has just consumed and the tensor core reads the A operand
-// from there (tcgen05.mma with a TMEM A operand, as the backward kernels do for dS): per 64-key step and Q tile that removes a
-// 16 KB shared-memory write, a 16 KB operand read and the generic->async proxy fence from the shared-memory-bound loop.
-template <int D, bool kBias, bool kPT, int NQ>
-__global__ void __launch_bounds__(NQ * ATT_GROUP + 128, NQ == 1 ? 2 : 1)
+template <int D, bool kBias>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttFwdParams p) {
-  using S = AttFwdSmem<D, NQ>;
-  constexpr int ATT_NQ = NQ;
-  constexpr int ATT_W_TMA = NQ * 4, ATT_W_MMA = NQ * 4 + 1;
-  static_assert(NQ == 2 || kPT, "one Q tile per CTA relies on the TMEM hand-over of P (no P tile in shared memory)");
+  using S = AttFwdSmem<D>;
   constexpr int STAGES = S::STAGES;
-  constexpr int TMEM_COLS = NQ == 2 ? 512 : 256;
-  constexpr int SLOT_COLS = 2 * ATT_BKV + D;  // S[2] | O   per Q tile
-  constexpr uint32_t IDESC_S = make_idesc_bf16(ATT_BQ, ATT_BKV, 0, 0);
-  constexpr uint32_t IDESC_PV = make_idesc_bf16(ATT_BQ, D, 0, 1);
-  static_assert(ATT_NQ * SLOT_COLS <= TMEM_COLS, "TMEM budget");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
   uint64_t* q_full = bars;
   uint64_t* k_full = q_full + 1;
-  uint64_t* k_empty = k_full + STAGES;
-  uint64_t* v_full = k_empty + STAGES;
-  uint64_t* v_empty = v_full + STAGES;
-  uint64_t* s_full = v_empty + STAGES;  // [slot*2 + buf]
-  uint64_t* p_ready = s_full + 4;       // [slot*2 + buf]: per P buffer, because a softmax group may run one step ahead
-  uint64_t* o_done = p_ready + 4;       // [slot]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(o_done + 2);
+  uint64_t* v_full = k_full + STAGES;
+  uint64_t* kv_empty = v_full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int pair = gridDim.x - 1 - blockIdx.x;  // heavy (late) causal tiles first
+  const int tile = gridDim.x - 1 - blockIdx.x;  // heavy (late) causal tiles first
   const int head = blockIdx.y, b = blockIdx.z;
-  const int q0 = pair * (ATT_NQ * ATT_BQ);
-
+  const int q0 = tile * ATT_BQ;
   const int n_all = (p.seq_kv + ATT_BKV - 1) / ATT_BKV;
-  int n_kv[ATT_NQ];
-#pragma unroll
-  for (int i = 0; i < ATT_NQ; ++i) {
-    const int qs = q0 + i * ATT_BQ;
-    if (qs >= p.seq_q) n_kv[i] = 0;
-    else if (p.causal) n_kv[i] = min(n_all, (min(qs + ATT_BQ, p.seq_q) + ATT_BKV - 1) / ATT_BKV);
-    else n_kv[i] = n_all;
-  }
-  const int n_total = NQ == 2 ? max(n_kv[0], n_kv[NQ - 1]) : n_kv[0];
-#ifdef FSB_ATTN_TRACE
-  const bool ftrace_on = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && lane == 0 &&
-                         (warp == 4 || warp == ATT_W_MMA);   // slot-1 math warp (most steps) and the MMA warp
-#endif
+  const int n_kv = p.causal ? min(n_all, (min(q0 + ATT_BQ, p.seq_q) + ATT_BKV - 1) / ATT_BKV) : n_all;
 
-  if (warp == ATT_W_TMA && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1);
+      mbar_init(&k_full[i], 1); mbar_init(&v_full[i], 1);
+      mbar_init(&kv_empty[i], 8);   // one arrive per consumer warp
     }
-    for (int i = 0; i < 4; ++i) mbar_init(&s_full[i], 1);
-    for (int i = 0; i < 4; ++i) mbar_init(&p_ready[i], ATT_GROUP);
-    for (int i = 0; i < 2; ++i) mbar_init(&o_done[i], 1);
     fence_barrier_init();
   }
-  if (warp == ATT_W_MMA) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-  // bias window in shared memory: entries [b_lo, b_lo + b_len) of this head's vector cover every (row, key) of the CTA
-  [[maybe_unused]] const int n_rel_ = p.seq_q + p.seq_kv - 1;
-  [[maybe_unused]] const int b_lo = (p.seq_q - 1) - min(q0 + ATT_NQ * ATT_BQ - 1, p.seq_q - 1);
-  [[maybe_unused]] const int b_len = ATT_NQ * ATT_BQ + n_total * ATT_BKV;
-  constexpr bool kBiasSmem = kBias && kPT && NQ == 2;
-  [[maybe_unused]] const bool bias_in_smem = kBiasSmem && b_len <= S::BIAS_FLOATS;
-  if constexpr (kBiasSmem) {
-    if (bias_in_smem) {
-      float* bs = reinterpret_cast<float*>(smem + S::OFF_P);
-      const float* src = p.rel_bias + int64_t(head) * n_rel_ + b_lo;
-      for (int i = threadIdx.x; i < b_len; i += NQ * ATT_GROUP + 128)
-        bs[i] = (b_lo + i < n_rel_) ? __ldg(src + i) * 1.4426950408889634f : 0.f;
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  // register split: see ATT_SM_REGS / ATT_WG2_REGS
-  if (warp > ATT_W_MMA) {
-    reg_dec<(NQ == 2 ? ATT_WG2_REGS : ATT1_WG2_REGS)>();   // idle donor warps
-  } else if (warp == ATT_W_TMA) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    reg_dec<(NQ == 2 ? ATT_WG2_REGS : ATT1_WG2_REGS)>();
-    if (lane == 0) {
+    reg_dec<24>();
+    if (threadIdx.x == 0) {
       const int qc = head * p.q_head_stride, kc = head * p.k_head_stride, vc = head * p.v_head_stride;
-      const int active = (n_kv[0] > 0) + (NQ == 2 ? int(n_kv[NQ - 1] > 0) : 0);
-      mbar_expect_tx(q_full, active * S::Q_BYTES);
+      mbar_expect_tx(q_full, S::Q_BYTES);
 #pragma unroll
-      for (int i = 0; i < ATT_NQ; ++i) {
-        if (n_kv[i] == 0) continue;
-#pragma unroll
-        for (int h = 0; h < D / 64; ++h)
-          tma_load_3d(smem + S::OFF_Q + i * S::Q_BYTES + h * (ATT_BQ * 128), &tmQ, q_full, qc + h * 64, q0 + i * ATT_BQ, b);
-      }
+      for (int h = 0; h < D / 64; ++h) tma_load_3d(smem + S::OFF_Q + h * (ATT_BQ * 128), &tmQ, q_full, qc + h * 64, q0, b);
       int st = 0; uint32_t ph = 0;
-      for (int j = 0; j < n_total; ++j) {
-        mbar_wait(&k_empty[st], ph ^ 1);
+      for (int j = 0; j < n_kv; ++j) {
+        mbar_wait(&kv_empty[st], ph ^ 1);
         mbar_expect_tx(&k_full[st], S::KV_BYTES);
 #pragma unroll
         for (int h = 0; h < D / 64; ++h)
-          tma_load_3d(smem + S::OFF_K + st * S::KV_BYTES + h * (ATT_BKV * 128), &tmK, &k_full[st], kc + h * 64,
-                      j * ATT_BKV, b);
-        mbar_wait(&v_empty[st], ph ^ 1);
+          tma_load_3d(smem + S::OFF_K + st * S::KV_BYTES + h * (ATT_BKV * 128), &tmK, &k_full[st], kc + h * 64, j * ATT_BKV, b);
         mbar_expect_tx(&v_full[st], S::KV_BYTES);
 #pragma unroll
         for (int h = 0; h < D / 64; ++h)
-          tma_load_3d(smem + S::OFF_V + st * S::KV_BYTES + h * (ATT_BKV * 128), &tmV, &v_full[st], vc + h * 64,
-                      j * ATT_BKV, b);
+          tma_load_3d(smem + S::OFF_V + st * S::KV_BYTES + h * (ATT_BKV * 128), &tmV, &v_full[st], vc + h * 64, j * ATT_BKV, b);
         if (++st == STAGES) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp == ATT_W_MMA) {
-    // ===================== MMA issuer: warp-uniform loop, one elected lane issues =====================
-    reg_dec<(NQ == 2 ? ATT_WG2_REGS : ATT1_WG2_REGS)>();
-    const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_Q), 0, 1024);
-    const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_K), 0, 1024);
-    const uint64_t dsc_p = make_smem_desc_sw128(smem_u32(smem + S::OFF_P), 0, 1024);
-    const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_V), ATT_BKV * 128, 1024);  // MN-major
-    auto issue_S = [&](int slot, int buf, int st) {   // caller holds elect_one()
-      const uint64_t da = dsc_q + uint64_t(slot) * (S::Q_BYTES >> 4), db = dsc_k + uint64_t(st) * (S::KV_BYTES >> 4);
-#pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk)
-        umma_bf16(tmem_base + slot * SLOT_COLS + buf * ATT_BKV, da + (((kk / 4) * (ATT_BQ * 128) + (kk % 4) * 32) >> 4),
-                  db + (((kk / 4) * (ATT_BKV * 128) + (kk % 4) * 32) >> 4), IDESC_S, kk != 0);
-      umma_commit(&s_full[slot * 2 + buf]);
-    };
-    auto issue_PV = [&](int slot, int buf, int st, bool accumulate) {
-      const uint64_t da = dsc_p + uint64_t(slot * 2 + buf) * (S::P_BYTES >> 4), db = dsc_v + uint64_t(st) * (S::KV_BYTES >> 4);
-      const uint32_t ta = tmem_base + slot * SLOT_COLS + buf * ATT_BKV;   // P(j): 8 columns per 16-key slice
-#pragma unroll
-      for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
-        if constexpr (kPT)
-          umma_bf16_ts(tmem_base + slot * SLOT_COLS + 2 * ATT_BKV, ta + 8 * kk, db + ((kk * 2048) >> 4), IDESC_PV,
-                       (accumulate || kk != 0) ? 1u : 0u);
-        else
-          umma_bf16(tmem_base + slot * SLOT_COLS + 2 * ATT_BKV, da + ((kk * 32) >> 4), db + ((kk * 2048) >> 4), IDESC_PV,
-                    (accumulate || kk != 0) ? 1u : 0u);
-      }
-      umma_commit(&o_done[slot]);
-    };
-    mbar_wait(q_full, 0);
-    // prologue: S(0) and S(1) of every active slot
-    for (int t = 0; t < 2 && t < n_total; ++t) {
-      mbar_wait(&k_full[t % STAGES], (t / STAGES) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        for (int i = 0; i < ATT_NQ; ++i)
-          if (t < n_kv[i]) issue_S(i, t & 1, t % STAGES);
-        umma_commit(&k_empty[t % STAGES]);
-      }
-      __syncwarp();
-    }
-    for (int j = 0; j < n_total; ++j) {
-      const int st = j % STAGES;
-      const uint32_t ph = (j / STAGES) & 1;
-      const int t2 = j + 2, st2 = t2 % STAGES;
-      const uint32_t ph2 = (t2 / STAGES) & 1;
-      bool v_waited = false, k_waited = false;
-      for (int i = 0; i < ATT_NQ; ++i) {
-        if (j >= n_kv[i]) continue;
-        if (i == 1) FTRACE(1, j, 0);
-        mbar_wait(&p_ready[i * 2 + (j & 1)], (j >> 1) & 1);
-        if (i == 1) FTRACE(1, j, 1);
-        if (!v_waited) { mbar_wait(&v_full[st], ph); v_waited = true; }
-        const bool more = t2 < n_kv[i];
-        if (more && !k_waited) { mbar_wait(&k_full[st2], ph2); k_waited = true; }
-        tc_fence_after();
-        if (i == 1) FTRACE(1, j, 2);
-        if (elect_one()) {
-          issue_PV(i, j & 1, st, j > 0);
-          if (more) issue_S(i, j & 1, st2);   // S buffer (j & 1) was consumed by softmax step j
-        }
-        __syncwarp();
-        if (i == 1) FTRACE(1, j, 3);
-      }
-      if (elect_one()) {
-        umma_commit(&v_empty[st]);
-        if (t2 < n_total) umma_commit(&k_empty[st2]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================== softmax groups: one thread per query row =====================
-    reg_inc<(NQ == 2 ? ATT_SM_REGS : ATT1_SM_REGS)>();
-    const int slot = warp >> 2;
-    const int quad = warp & 3;                    // TMEM lane quadrant this warp may access (= warp id % 4)
-    const int r_in = quad * 32 + lane;            // row inside the tile == TMEM lane
-    const int q_row = q0 + slot * ATT_BQ + r_in;  // position in the sequence
-    const int n_mine = n_kv[slot];
-    const uint32_t t_slot = tmem_base + (uint32_t(quad * 32) << 16) + slot * SLOT_COLS;
-    const int sw = r_in & 7;
-    const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
-    const float sc = p.scale_log2;
-    const int kmax = p.causal ? min(q_row, p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
-    // T5 / mT5 relative-position bias (transformers mt5/modeling_mt5.py:181-235,:320): bias[h, q, k] depends on k - q only, so it
-    // arrives as one vector per head; this row reads the 64 consecutive entries starting at (c0 - q_row + seq_q - 1).
-    const int n_rel = p.seq_q + p.seq_kv - 1;
-    const float* brow = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row, p.seq_q - 1)) : nullptr;
-    const float sc_eff = kBias ? 1.f : sc;        // with a bias the scores are moved to the scaled log2 domain first
-    [[maybe_unused]] const int bias_k0 = (p.seq_q - 1 - min(q_row, p.seq_q - 1)) - b_lo;   // this row's offset into the smem window
-
-    float m_ref = -INFINITY;                      // exponent reference, scaled log2 domain
-    float l0 = 0.f, l1 = 0.f;                     // two partial row sums (shorter FADD chains)
-    uint32_t sa[64], sb[64];                      // S(j) and the prefetched S(j+1), raw fp32 scores
-
-    auto load_s = [&](int j, uint32_t (&dst)[64]) {   // asynchronous: tmem_ld_wait() before dst is read
-      mbar_wait(&s_full[slot * 2 + (j & 1)], (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t a = t_slot + (j & 1) * ATT_BKV;
-      tmem_ld32_at<0>(a, dst);
-      tmem_ld32_at<32>(a + 32, dst);
-    };
-    // Same, but only if S(j) has already landed (warp-uniform answer: tcgen05.ld is warp-collective). In steady state the
-    // tensor core is still busy with the other Q tile's products when this is asked, so the blocking form runs after the
-    // exponentials instead of in front of them (a cycle trace showed 250-420 cycles per step spent waiting here).
-    auto try_load_s = [&](int j, uint32_t (&dst)[64]) -> bool {
-      if (!__all_sync(0xffffffffu, mbar_test(&s_full[slot * 2 + (j & 1)], (j >> 1) & 1))) return false;
-      tc_fence_after();
-      const uint32_t a = t_slot + (j & 1) * ATT_BKV;
-      tmem_ld32_at<0>(a, dst);
-      tmem_ld32_at<32>(a + 32, dst);
-      return true;
-    };
-    auto step = [&](int j, uint32_t (&cur)[64], uint32_t (&nxt)[64]) {
-      const int buf = j & 1;
-      FTRACE(0, j, 0);
-      tmem_ld_wait();                             // S(j) is in cur[]
-      FTRACE(0, j, 1);
-      const int c0 = j * ATT_BKV;
-      if constexpr (kBias) {
-        constexpr float kLog2e = 1.4426950408889634f;
-        if (bias_in_smem) {
-          // 64 consecutive window entries of this row (lanes walk the window backwards by one: conflict-free), already in
-          // log2 units; the window is zero-padded past the vector, so the ragged last tile needs no clamp
-          const float* bs = reinterpret_cast<const float*>(smem + S::OFF_P) + bias_k0 + c0;
-#pragma unroll
-          for (int c = 0; c < 64; ++c) cur[c] = __float_as_uint(fmaf(__uint_as_float(cur[c]), sc, bs[c]));
-        } else if (c0 + ATT_BKV <= p.seq_kv) {
-#pragma unroll
-          for (int c = 0; c < 64; ++c)
-            cur[c] = __float_as_uint(fmaf(__ldg(brow + c0 + c), kLog2e, __uint_as_float(cur[c]) * sc));
-        } else {   // last, partial key tile: stay inside the vector (those columns are masked below anyway)
-#pragma unroll
-          for (int c = 0; c < 64; ++c)
-            cur[c] = __float_as_uint(fmaf(__ldg(brow + min(c0 + c, p.seq_kv - 1)), kLog2e, __uint_as_float(cur[c]) * sc));
-        }
-      }
-      const bool need_mask = (p.causal && c0 + ATT_BKV - 1 > q0 + slot * ATT_BQ) || (c0 + ATT_BKV > p.seq_kv) || mrow;
-      if (need_mask) {
-        if (mrow == nullptr) {
-          // causal / ragged-tail masking is a per-row column LIMIT: one compare + select per score. (At S <= 1024 a third or
-          // more of all steps touch the diagonal, so this path is as hot as the unmasked one.)
-          const int lim = kmax - c0;              // keep columns c <= lim
-#pragma unroll
-          for (int c = 0; c < 64; ++c) cur[c] = (c <= lim) ? cur[c] : 0xff800000u;   // -inf
-        } else {
-#pragma unroll
-          for (int c = 0; c < 64; ++c) {
-            const int col = c0 + c;
-            bool keep = col < p.seq_kv && !(p.causal && col > q_row);
-            if (keep) keep = mrow[col] != 0;
-            if (!keep) cur[c] = 0xff800000u;      // -inf
-          }
-        }
-      }
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 64; c += 4) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) mx4[e] = fmaxf(mx4[e], __uint_as_float(cur[c + e]));
-      }
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * sc_eff;   // scale > 0 (checked on the host)
-      FTRACE(0, j, 2);
-      // lazy reference update: raise m_ref only when the row max outgrew it by more than 2^tau
-      const bool raise = mx > m_ref + ATT_RESCALE_TAU;
-      const bool resc = raise && m_ref != -INFINITY;   // something was accumulated with the old reference
-      const float f = resc ? ex2_approx(m_ref - mx) : 1.f;
-      // TMEM ld/st are warp-collective (.sync.aligned): the whole warp takes the branch if ANY row needs it (factor 1 elsewhere)
-      if (j > 0 && __any_sync(0xffffffffu, resc)) {
-        mbar_wait(&o_done[slot], (j - 1) & 1);    // PV(j-1) must have landed in TMEM
-        tc_fence_after();
-#pragma unroll
-        for (int ch = 0; ch < D / 32; ++ch) {
-          uint32_t t[32];
-          const uint32_t addr = t_slot + 2 * ATT_BKV + ch * 32;
-          tmem_ld32(addr, t);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 32; ++c) t[c] = __float_as_uint(__uint_as_float(t[c]) * f);
-          tmem_st32(addr, t);
-        }
-        tmem_st_wait();
-      }
-      l0 *= f; l1 *= f;
-      if (raise) m_ref = mx;
-      const float neg_m = (m_ref == -INFINITY) ? 0.f : -m_ref;
-      FTRACE(0, j, 3);
-      // prefetch S(j+1) into the other register set while this step's exponentials run — if it is there already
-      const bool more = j + 1 < n_mine;
-      const bool prefetched = more && try_load_s(j + 1, nxt);
-      FTRACE(0, j, 4);
-      if constexpr (kPT) {
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {          // 32 keys -> 16 TMEM columns per store (keeps the register footprint low)
-          uint32_t pk[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float a = ex2_approx(fmaf(__uint_as_float(cur[hf * 32 + 2 * e]), sc_eff, neg_m));
-            const float bq = ex2_approx(fmaf(__uint_as_float(cur[hf * 32 + 2 * e + 1]), sc_eff, neg_m));
-            pk[e] = pack_bf16x2(a, bq);
-            l0 += a; l1 += bq;                    // fp32 sums of the unrounded probabilities (LSE exact to fp32)
-          }
-          tmem_st16(t_slot + buf * ATT_BKV + hf * 16, pk);   // over the S(j) columns this thread has already consumed
-        }
-        FTRACE(0, j, 5);
-        tmem_st_wait();
-      } else {
-        uint8_t* sP = smem + S::OFF_P + (slot * 2 + buf) * S::P_BYTES + r_in * 128;
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {            // 8 keys -> one 16-byte chunk of the 128B-swizzled P row
-          uint32_t pk[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float a = ex2_approx(fmaf(__uint_as_float(cur[ch * 8 + 2 * e]), sc_eff, neg_m));
-            const float bq = ex2_approx(fmaf(__uint_as_float(cur[ch * 8 + 2 * e + 1]), sc_eff, neg_m));
-            pk[e] = pack_bf16x2(a, bq);
-            l0 += a; l1 += bq;                      // fp32 sums of the unrounded probabilities (LSE exact to fp32)
-          }
-          *reinterpret_cast<uint4*>(sP + ((ch ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        }
-        FTRACE(0, j, 5);
-        fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      }
-      tc_fence_before();     // order our tcgen05.ld/st before the MMAs that read / overwrite TMEM
-      mbar_arrive(&p_ready[slot * 2 + buf]);
-      if (more && !prefetched) load_s(j + 1, nxt);   // its latency hides behind the next step's first instructions
-      FTRACE(0, j, 6);
-    };
-    if (n_mine > 0) load_s(0, sa);
-    for (int j = 0; j < n_mine; j += 2) {
-      step(j, sa, sb);
-      if (j + 1 < n_mine) step(j + 1, sb, sa);
-    }
-    // ---- epilogue: read O from TMEM, normalise, store O (bf16) and LSE (log2 domain)
-    if (n_mine > 0) {
-      mbar_wait(&o_done[slot], (n_mine - 1) & 1);
-      tc_fence_after();
-      const float l_run = l0 + l1;
-      const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-      const bool row_ok = q_row < p.seq_q;
-      __nv_bfloat16* op = p.o + (int64_t(b) * p.seq_q + q_row) * p.o_row_stride + int64_t(head) * p.o_head_stride;
-#pragma unroll
-      for (int cc = 0; cc < D / 32; ++cc) {
-        uint32_t t[32];
-        tmem_ld32(t_slot + 2 * ATT_BKV + cc * 32, t);
-        tmem_ld_wait();
-        if (row_ok) {
-#pragma unroll
-          for (int c = 0; c < 32; c += 8) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(t[c + e]) * inv;
-            *reinterpret_cast<uint4*>(op + cc * 32 + c) = pack8(f);
-          }
-        }
-      }
-      if (row_ok)
-        p.lse[(int64_t(b) * p.nheads + head) * p.seq_q + q_row] = l_run > 0.f ? m_ref + log2f(l_run) : INFINITY;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == ATT_W_MMA) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
+  // ===================== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of the tile =====================
+  reg_inc<240>();   // 256 * 240 + 128 * 24 = 64512
+  const int wg = (threadIdx.x >> 7) - 1;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8
+  const int cq = 2 * (lane & 3);                               // its columns inside every 8-column group: cq, cq + 1
+  const uint64_t dsc_q = make_smem_desc_sw128(smem_u32(smem + S::OFF_Q) + wg * (64 * 128), 0, 1024);
+  const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_K), 0, 1024);
+  const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_V), ATT_BKV * 128, 1024);   // MN-major (D contiguous)
+  const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
+  const float sc = p.scale_log2;
+  const int n_rel = p.seq_q + p.seq_kv - 1;
+  int q_row[2], kmax[2];
+  const float* brow[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    q_row[h] = q0 + r_lo + 8 * h;
+    kmax[h] = p.causal ? min(q_row[h], p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
+    // T5 / mT5 relative-position bias (transformers mt5/modeling_mt5.py:181-235,:320): bias[h, q, k] depends on k - q only, so
+    // it arrives as one vector per head; this row reads entries (k - q_row + seq_q - 1).
+    brow[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row[h], p.seq_q - 1)) : nullptr;
+  }
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // running max (scaled log2 domain), thread-partial row sums
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int st = j % STAGES;
+    const uint32_t ph = (j / STAGES) & 1;
+    float s[ATT_BKV / 2];
+    mbar_wait(&k_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss_n128<0, 0>(s, dsc_q + (((kk / 4) * (ATT_BQ * 128) + (kk % 4) * 32) >> 4),
+                          dsc_k + ((st * S::KV_BYTES + (kk / 4) * (ATT_BKV * 128) + (kk % 4) * 32) >> 4), kk != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+
+    // scores -> scaled log2 domain (+ bias), masked to -inf; s[4 i + e]: column 8 i + cq + (e & 1), row h = e >> 1
+    const int c0 = j * ATT_BKV;
+    const bool need_mask = (p.causal && c0 + ATT_BKV - 1 > q0 + wg * 64) || (c0 + ATT_BKV > p.seq_kv) || mrow;
+#pragma unroll
+    for (int i = 0; i < ATT_BKV / 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int h = e >> 1, col = c0 + 8 * i + cq + (e & 1);
+        float x;
+        if constexpr (kBias) x = fmaf(__ldg(brow[h] + min(col, p.seq_kv - 1)), 1.4426950408889634f, s[4 * i + e] * sc);
+        else x = s[4 * i + e] * sc;
+        if (need_mask) {
+          bool keep = col <= kmax[h];
+          if (mrow != nullptr && keep) keep = mrow[col] != 0;
+          x = keep ? x : -INFINITY;
+        }
+        s[4 * i + e] = x;
+      }
+    }
+    float neg_m[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < ATT_BKV / 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[h], mx);
+      const float f = (m_new == -INFINITY) ? 1.f : ex2_approx(m[h] - m_new);
+      l[h] *= f;
+#pragma unroll
+      for (int i = 0; i < D / 8; ++i) { o[4 * i + 2 * h] *= f; o[4 * i + 2 * h + 1] *= f; }
+      m[h] = m_new;
+      neg_m[h] = (m_new == -INFINITY) ? 0.f : -m_new;
+    }
+    // P(j) as register A fragments: 16-key slice kk = accumulator groups 2 kk and 2 kk + 1
+    uint32_t pa[ATT_BKV / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int h = r & 1, i = 2 * kk + (r >> 1);
+        const float a = ex2_approx(s[4 * i + 2 * h] + neg_m[h]), c = ex2_approx(s[4 * i + 2 * h + 1] + neg_m[h]);
+        l[h] += a + c;   // fp32 sums of the unrounded probabilities
+        pa[kk][r] = pack_bf16x2(a, c);
+      }
+    }
+    mbar_wait(&v_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATT_BKV / 16; ++kk)
+      wgmma_rs_d<D>(o, pa[kk], dsc_v + ((st * S::KV_BYTES + kk * 2048) >> 4));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+  }
+
+  // ---- epilogue: normalise, store O (bf16) and LSE (log2 domain)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lr = l[h];
+    lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+    lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+    if (q_row[h] >= p.seq_q) continue;
+    const float inv = lr > 0.f ? 1.f / lr : 0.f;
+    __nv_bfloat16* op = p.o + (int64_t(b) * p.seq_q + q_row[h]) * p.o_row_stride + int64_t(head) * p.o_head_stride + cq;
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i)
+      *reinterpret_cast<uint32_t*>(op + 8 * i) = pack_bf16x2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+    if ((lane & 3) == 0)
+      p.lse[(int64_t(b) * p.nheads + head) * p.seq_q + q_row[h]] = lr > 0.f ? m[h] + log2f(lr) : INFINITY;
   }
 }
 
@@ -486,25 +240,22 @@ int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_
   return make_tmap_bf16(tm, base, 3, dims, strides, box);
 }
 
-template <int D, bool kBias, bool kPT, int NQ>
+template <int D, bool kBias>
 static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttFwdParams& p,
                            cudaStream_t st) {
-  using S = AttFwdSmem<D, NQ>;
-  constexpr int ATT_NQ = NQ;
+  using S = AttFwdSmem<D>;
   static bool configured = false;
-  auto kern = attn_fwd_kernel<D, kBias, kPT, NQ>;
+  auto kern = attn_fwd_kernel<D, kBias>;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) {
       set_error("sdpa_fwd: cudaFuncSetAttribute(%d) failed: %s", S::TOTAL, cudaGetErrorString(e));
       return FSB_ERR_CUDA;
     }
-    if (NQ == 1)   // two CTAs per SM only fit with the largest shared-memory carve-out
-      cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     configured = true;
   }
-  dim3 grid((p.seq_q + ATT_NQ * ATT_BQ - 1) / (ATT_NQ * ATT_BQ), p.nheads, p.batch);
-  kern<<<grid, NQ * ATT_GROUP + 128, S::TOTAL, st>>>(tq, tk, tv, p);
+  dim3 grid((p.seq_q + ATT_BQ - 1) / ATT_BQ, p.nheads, p.batch);
+  kern<<<grid, ATT_THREADS, S::TOTAL, st>>>(tq, tk, tv, p);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
@@ -512,12 +263,6 @@ static int launch_attn_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const C
 }  // namespace fsb
 
 using namespace fsb;
-
-#ifdef FSB_ATTN_TRACE
-extern "C" int fsb_debug_attn_fwd_trace(long long* host_out /* [2][64][8] */) {
-  return cudaMemcpyFromSymbol(host_out, g_fwd_trace, sizeof(long long) * 2 * 64 * 8) == cudaSuccess ? 0 : 1;
-}
-#endif
 
 extern "C" int fsb_sdpa_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int64_t batch,
                             int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
@@ -545,15 +290,9 @@ extern "C" int fsb_sdpa_fwd(const void* q, const void* k, const void* v, void* o
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch);
   p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
-  // FSB_ATTN_P_TMEM=0 selects the shared-memory P hand-over (A/B measurements); default: through tensor memory
-  static const bool p_tmem = [] { const char* e = getenv("FSB_ATTN_P_TMEM"); return e ? atoi(e) != 0 : true; }();
-  // FSB_ATTN_NQ=1|2 forces one / two Q tiles per CTA (default below; see the NQ note at the top of the file)
-  static const int nq_env = [] { const char* e = getenv("FSB_ATTN_NQ"); return e ? atoi(e) : 0; }();
-  const int nq = (nq_env == 1 || nq_env == 2) ? nq_env : 2;
-#define FSB_FWD(DD, BB) (!p_tmem ? launch_attn_fwd<DD, BB, false, 2>(tq, tk, tv, p, (cudaStream_t)st)                 \
-                         : nq == 1 ? launch_attn_fwd<DD, BB, true, 1>(tq, tk, tv, p, (cudaStream_t)st)               \
-                                   : launch_attn_fwd<DD, BB, true, 2>(tq, tk, tv, p, (cudaStream_t)st))
-  if (rel_bias != nullptr) return head_dim == 128 ? FSB_FWD(128, true) : FSB_FWD(64, true);
-  return head_dim == 128 ? FSB_FWD(128, false) : FSB_FWD(64, false);
-#undef FSB_FWD
+  if (rel_bias != nullptr)
+    return head_dim == 128 ? launch_attn_fwd<128, true>(tq, tk, tv, p, (cudaStream_t)st)
+                           : launch_attn_fwd<64, true>(tq, tk, tv, p, (cudaStream_t)st);
+  return head_dim == 128 ? launch_attn_fwd<128, false>(tq, tk, tv, p, (cudaStream_t)st)
+                         : launch_attn_fwd<64, false>(tq, tk, tv, p, (cudaStream_t)st);
 }

@@ -1,7 +1,7 @@
 // Host-side MegatronBERT sample assembly: the per-document work of `ErLangShenCollator`
 // (fengshen/examples/pretrain_erlangshen_bert/pretrain_erlangshen.py:57-123 and the fengshen/data/data_utils helpers it calls:
 // sop_utils.py:2-32, truncate_utils.py:2-19, token_type_utils.py:1-25, mask_utils.py:19-285 with its defaults) in one C call over a
-// batch of ALREADY TOKENISED documents. At the B200's step rates the Python collator (~50 k tokens/s per core, DESIGN §6) is the
+// batch of ALREADY TOKENISED documents. At a GPU training step's rates the Python collator (~50 k tokens/s per core, DESIGN §6) is the
 // first thing to starve the step; this leaves tokenisation as the only Python-side cost.
 //
 // The batch is bit-identical to the Python path, including the state the numpy RandomState is left in: the generator is numpy's

@@ -1,17 +1,18 @@
-// fsb200 — persistent, warp-specialised bf16 GEMM for sm_100a: TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM
-// -> epilogue warps -> HBM. Replaces the cuBLAS calls behind F.linear on the reference hot path
+// fsb200 — persistent, warp-specialised bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem -> wgmma (fp32 accumulators in
+// registers) -> fused epilogue -> HBM. Replaces the cuBLAS calls behind F.linear on the reference hot path
 // (fengshen/models/megatron/mpu/layers.py:347-360, :451-470; layers/transformer.py:136-172) and their autograd
 // transposes. One kernel, three operand layouts:
 //   NT  D = A[M,K] B[N,K]^T   both operands K-major          (forward)
 //   NN  D = A[M,K] B[K,N]     B is MN-major in shared memory  (dgrad)
 //   TN  D = A[K,M]^T B[K,N]   A and B MN-major                (wgrad)
-// MN-major tiles are fetched as 64(mn) x 64(k) TMA boxes; the UMMA descriptor's leading-byte-offset walks the boxes.
+// MN-major tiles are fetched as 64(mn) x 64(k) TMA boxes; the wgmma descriptor's leading-byte-offset walks the boxes and
+// the instruction's transpose bit reads them as MN-major.
 //
-// Roles (384 threads = 3 warpgroups): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer, warps 2-3 idle (they only
-// donate registers: setmaxnreg moves the budget of warpgroup 0 to the epilogue), warps 4..11 = epilogue: TMEM lane
-// quadrant = warp_id % 4, and the two warps of a quadrant split the tile's 64-column groups between them (bias /
-// activation / bf16 conversion are instruction-bound with one warp per scheduler). Two TMEM accumulator stages let the
-// epilogue of tile i overlap the main loop of tile i+1. Grid = min(#tiles, #SMs); static round-robin tile order, grouped 8 m-tiles deep for L2.
+// Roles (384 threads = 3 warpgroups): warpgroup 0 = TMA producer (one thread issues; setmaxnreg gives its registers to the
+// others), warpgroups 1-2 = consumers: each owns 64 rows of the 128 x BN tile, issues m64nBNk16 wgmmas on the shared stage
+// and runs the epilogue (bias / activation / pre-activation copy / bf16 or fp32 store, optionally accumulating) straight from
+// its accumulator registers. The producer runs up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
+// operands stream in during the epilogue. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
 #include <stdlib.h>
 
 #include "host_common.h"
@@ -22,10 +23,6 @@ namespace fsb {
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_EPI_WARP0 = 4;   // first epilogue warp
-#ifndef FSB_GEMM_CTA2_DEFAULT
-#define FSB_GEMM_CTA2_DEFAULT true
-#endif
 
 struct GemmParams {
   void* D;
@@ -37,33 +34,21 @@ struct GemmParams {
   int bias_f32;    // bias dtype
   int epilogue;    // fsb_gemm_epilogue
   int accumulate;  // D += result
-  int tma_store;   // bf16 D without accumulate: stage through smem and write with cp.async.bulk.tensor (full lines)
   int tiles_m, tiles_n;
   int group_m;     // m-tiles per rasterisation group (see fsb_gemm_bf16)
-  int l2_hints;    // bit 0: A panels evict-last, bit 1: B panels evict-first, bit 2: D stores evict-first (FSB_GEMM_L2HINT)
+  int l2_hints;    // bit 0: A panels evict-last, bit 1: B panels evict-first (FSB_GEMM_L2HINT)
 };
 
-// kAux: the GEMM also writes the pre-activation (GELU MLPs): two bulk stores per column group. Their smem->global reads
-// queue behind the mainloop's TMA loads, so that variant trades one operand stage (K is the hidden size there, short
-// mainloops) for a four-deep staging ring per epilogue warp.
-// kCta2: CTA-pair variant (tcgen05 cta_group::2): the pair computes a 256 x BN tile; each CTA stages its own 128 rows of A and
-// HALF of B (BN/2 columns), so a stage is 32 KB instead of 48 KB and the per-SM shared-memory traffic (TMA fill + MMA operand
-// reads: 192 B/clk for a lone 128x256 tile, above the 128 B/clk an SM delivers) drops to 128 B/clk.
-template <int BN, bool kAux, bool kCta2>
+template <int BN>
 struct GemmSmem {
-  static constexpr int BNL = kCta2 ? BN / 2 : BN;                  // B columns staged by this CTA
-  static constexpr int STAGES = kCta2 ? (kAux ? 5 : 6) : BN == 256 ? (kAux ? 3 : 4) : (kAux ? 5 : 6);
-  static constexpr int NBUF = kAux ? 4 : 2;                        // staging tiles per epilogue warp
+  static constexpr int STAGES = BN == 256 ? 4 : 6;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_BYTES = BNL * GEMM_BK * 2;
+  static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STORE_OFFSET = STAGES * STAGE_BYTES;       // per epilogue warp: NBUF x [32 rows x 64 cols] bf16 staging tiles
-  static constexpr int STORE_WARP_BYTES = 32 * 64 * 2;
-  static constexpr int BIAS_OFFSET = STORE_OFFSET + 4 * NBUF * STORE_WARP_BYTES;   // 2 x [BN] bf16: this tile's bias slice
-  static constexpr int BAR_OFFSET = BIAS_OFFSET + 2 * BN * 2;
-  // full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], tmem_ptr
-  static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 4) * 8 + 16 + 1024 /*align slack*/;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into on sm_100");
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  // full[STAGES], empty[STAGES]
+  static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024 /*align slack*/;
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
 };
 
 // 0.5 x (1 + tanh(u)) == x * sigmoid(2u) == x / (1 + 2^(-2 u log2 e)): two MUFU ops instead of tanhf's ~25 instructions
@@ -101,88 +86,58 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   n_idx = in_g / gsize;
 }
 
-template <int kLayout, int BN, bool kAux, bool kCta2>
+template <int kLayout, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr bool A_MN = (kLayout == FSB_GEMM_TN);
   constexpr bool B_MN = (kLayout != FSB_GEMM_NT);
-  using S = GemmSmem<BN, kAux, kCta2>;
+  using S = GemmSmem<BN>;
   constexpr int STAGES = S::STAGES;
-  constexpr int BNL = S::BNL;
-  constexpr int TILE_M = kCta2 ? 2 * GEMM_BM : GEMM_BM;   // rows of one (cluster) tile
-  constexpr uint32_t IDESC = make_idesc_bf16(TILE_M, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-  constexpr int TMEM_COLS = 2 * BN;  // 512 or 256
-  const uint32_t cta_rank = kCta2 ? cluster_ctarank() : 0u;        // 0 = leader (issues the pair's MMAs)
-  const int tile_first = kCta2 ? int(blockIdx.x >> 1) : int(blockIdx.x);
-  const int tile_step = kCta2 ? int(gridDim.x >> 1) : int(gridDim.x);
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], (p.tma_store ? 8 : 4) * (kCta2 ? 2 : 1));  // one arrive per participating epilogue warp (of both CTAs)
+      mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (kCta2) tmem_alloc_2cta<TMEM_COLS>(tmem_ptr_smem); else tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (kCta2) cluster_sync_all();   // the peer's barriers are initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
     reg_dec<40>();
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      // (pair) both CTAs load their own halves; every transaction is credited to the LEADER's full barrier, on which the
-      // leader alone posts the expected byte count of the whole pair
-      // L2 policy: tiles are walked m-fastest inside a group of m-tiles, so a group's A panels are read again for every
-      // n-tile of the sweep (keep them: evict-last) while a B panel is used by the CTAs of one wave and then dead (evict-
-      // first); ncu showed the 8192x15360x5120 GEMM reading 738 MB for 241 MB of operands without the hints.
+      // L2 policy (FSB_GEMM_L2HINT): tiles are walked m-fastest inside a group of m-tiles, so a group's A panels are read
+      // again for every n-tile of the sweep (evict-last) while a B panel is used by the CTAs of one wave (evict-first).
       const uint64_t pol_a = (p.l2_hints & 1) ? kL2EvictLast : kL2EvictNormal, pol_b = (p.l2_hints & 2) ? kL2EvictFirst : kL2EvictNormal;
       const bool hints = (p.l2_hints & 3) != 0;
       auto load = [&](uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, uint64_t policy) {
-        if (hints) {
-          if constexpr (kCta2) tma_load_3d_2cta_hint(dst, tm, mapa_shared(smem_u32(bar), 0), c0, c1, c2, policy);
-          else tma_load_3d_hint(dst, tm, bar, c0, c1, c2, policy);
-        } else {
-          if constexpr (kCta2) tma_load_3d_2cta(dst, tm, mapa_shared(smem_u32(bar), 0), c0, c1, c2);
-          else tma_load_3d(dst, tm, bar, c0, c1, c2);
-        }
+        if (hints) tma_load_3d_hint(dst, tm, bar, c0, c1, c2, policy);
+        else tma_load_3d(dst, tm, bar, c0, c1, c2);
       };
-      for (int t = tile_first; t < num_tiles; t += tile_step) {
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int b, m_idx, n_idx;
         tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
-        const int m0 = m_idx * TILE_M + int(cta_rank) * GEMM_BM, n0 = n_idx * BN + int(cta_rank) * (kCta2 ? BNL : 0);
+        const int m0 = m_idx * GEMM_BM, n0 = n_idx * BN;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * S::STAGE_BYTES;
           uint8_t* sb = sa + S::A_BYTES;
-          if (!kCta2 || cta_rank == 0) mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES * (kCta2 ? 2 : 1));
+          mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES);
           const int k0 = kb * GEMM_BK;
           if constexpr (!A_MN) {
             load(sa, &tmA, &full_bar[stage], k0, m0, b, pol_a);
@@ -195,307 +150,121 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             load(sb, &tmB, &full_bar[stage], k0, n0, b, pol_b);
           } else {
 #pragma unroll
-            for (int c = 0; c < BNL / 64; ++c)
+            for (int c = 0; c < BN / 64; ++c)
               load(sb + c * (GEMM_BK * 128), &tmB, &full_bar[stage], n0 + c * 64, k0, b, pol_b);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: warp-uniform loop, one elected lane issues =====================
-    reg_dec<40>();
-    const uint64_t dsc_a = A_MN ? make_smem_desc_sw128(smem_u32(smem), GEMM_BK * 128, 1024)
-                                : make_smem_desc_sw128(smem_u32(smem), 0, 1024);
+  } else {
+    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====================
+    reg_inc<232>();  // 256 * 232 + 128 * 40 = 64512
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int wl = warp & 3;
+    // A: K-major -> the warpgroup's 64 rows start 64 * 128 B into the stage; MN-major -> its own 64-wide m chunk
+    const uint64_t dsc_a = A_MN ? make_smem_desc_sw128(smem_u32(smem) + wg * (GEMM_BK * 128), GEMM_BK * 128, 1024)
+                                : make_smem_desc_sw128(smem_u32(smem) + wg * (64 * 128), 0, 1024);
     const uint64_t dsc_b = B_MN ? make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, GEMM_BK * 128, 1024)
                                 : make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, 0, 1024);
+    float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    if (!kCta2 || cta_rank == 0)   // (pair) the leader issues for both SMs; commits are multicast to both CTAs' barriers
-    for (int t = tile_first; t < num_tiles; t += tile_step) {
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t so = uint64_t(stage) * (S::STAGE_BYTES >> 4);
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            const uint64_t da = dsc_a + so + ((A_MN ? k * 2048 : k * 32) >> 4), db = dsc_b + so + ((B_MN ? k * 2048 : k * 32) >> 4);
-            if constexpr (kCta2) umma_bf16_2cta(d_tmem, da, db, IDESC, (kb | k) != 0 ? 1u : 0u);
-            else umma_bf16(d_tmem, da, db, IDESC, (kb | k) != 0 ? 1u : 0u);
-          }
-          // frees this smem stage (in both CTAs) when the MMAs retire
-          if constexpr (kCta2) umma_commit_2cta(&empty_bar[stage], 3); else umma_commit(&empty_bar[stage]);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) {   // accumulator ready for the epilogue (of both CTAs)
-        if constexpr (kCta2) umma_commit_2cta(&tmem_full[acc], 3); else umma_commit(&tmem_full[acc]);
-      }
-      __syncwarp();
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp < GEMM_EPI_WARP0) {
-    reg_dec<40>();   // idle register donors
-  } else {
-    // ===================== epilogue (warps 4..11) =====================
-    reg_inc<232>();  // 256 * 232 + 128 * 40 = 384 * 168
-    const int quad = warp & 3;                        // TMEM lanes [32*quad, 32*quad+32)
-    const int half = (warp - GEMM_EPI_WARP0) >> 2;    // which of the quadrant's two warps
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    // hand an accumulator stage back to the MMA warp (the pair's leader owns the barrier)
-    auto release_acc = [&](int a) {
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (kCta2 && cta_rank != 0) mbar_arrive_cluster(mapa_shared(smem_u32(&tmem_empty[a]), 0));
-        else mbar_arrive(&tmem_empty[a]);
-      }
-    };
-    if (p.tma_store) {
-      // ---- bf16 D without accumulate (forward / dgrad GEMMs): every warp owns its 32 rows end to end.
-      // TMEM -> registers 64 columns at a time (the next group's tcgen05.ld is in flight while this one is converted),
-      // bias / activation in registers, bf16 rows into the warp's own 128B-swizzled [32 x 64] staging tile, one bulk tensor
-      // store per tile and warp: no CTA-wide barrier anywhere, and the accumulator is handed back to the MMA warp as soon
-      // as its last column has been read.
-      constexpr int NBW = S::NBUF / 2;             // staging tiles per warp
-      uint8_t* stg_w = smem + S::STORE_OFFSET + (half * 4 + quad) * (NBW * S::STORE_WARP_BYTES);
-      uint32_t item = 0;                           // bulk stores issued by this warp (staging buffer = item % NBW)
-      auto stage_store = [&](const uint32_t (&w)[32], const CUtensorMap* tm, int c0, int r0, int bz) {
-        uint8_t* stg = stg_w + (item % NBW) * S::STORE_WARP_BYTES;
-        if (lane == 0) tma_store_wait_read<NBW - 1>();   // the store issued NBW items ago has finished reading this buffer
-        __syncwarp();
-        const uint32_t row_addr = smem_u32(stg) + lane * 128;
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          st_shared_v4(row_addr + ((q ^ (lane & 7)) << 4), w[q * 4], w[q * 4 + 1], w[q * 4 + 2], w[q * 4 + 3]);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          if (p.l2_hints & 4) tma_store_3d_hint(tm, stg, c0, r0, bz, kL2EvictFirst);
-          else tma_store_3d(tm, stg, c0, r0, bz);
-          tma_store_commit();
-        }
-        ++item;
-      };
-      for (int t = tile_first; t < num_tiles; t += tile_step) {
-        int b, m_idx, n_idx;
-        tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
-        const int r0 = m_idx * TILE_M + int(cta_rank) * GEMM_BM + quad * 32;
-        const int n0 = n_idx * BN;
-        constexpr int NG = BN / 64;
-        const int ng = min(NG, (p.N - n0 + 63) / 64);     // column groups of this tile that exist
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t t_acc = tmem_base + (uint32_t(quad * 32) << 16) + acc * BN;
-        constexpr int NGW = NG / 2;                        // column groups per warp: g = 2 * i + half
-        if (half >= ng) {                                  // (ragged last tile) nothing for this warp: just release
-          release_acc(acc);
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-          continue;
-        }
-        uint32_t r[2][64];
-        tmem_ld32_at<0>(t_acc + half * 64, r[0]);
-        tmem_ld32_at<32>(t_acc + half * 64 + 32, r[0]);
-        // bias slice of this tile -> shared memory as bf16 (all epilogue warps write identical values, so only a
-        // __syncwarp is needed; two buffers because a warp may run one tile ahead of its slowest sibling)
-        __nv_bfloat16* sbias = reinterpret_cast<__nv_bfloat16*>(smem + S::BIAS_OFFSET) + acc * BN;
-        float bias_reg[NGW * 2];                   // fp32 bias: lane l keeps this warp's columns, broadcast by shuffle (exact)
-        if (p.bias != nullptr) {
-          if (p.bias_f32) {
-#pragma unroll
-            for (int c = 0; c < NGW * 2; ++c) {
-              const int col = n0 + (2 * (c >> 1) + half) * 64 + (c & 1) * 32 + lane;
-              bias_reg[c] = col < p.N ? __ldg(reinterpret_cast<const float*>(p.bias) + col) : 0.f;
-            }
-          } else {
-#pragma unroll
-            for (int c = 0; c < BN / 32; ++c) {
-              const int col = n0 + c * 32 + lane;
-              sbias[c * 32 + lane] = col < p.N ? __ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col) : __float2bfloat16(0.f);
-            }
-          }
-          __syncwarp();
-        }
-#pragma unroll
-        for (int i = 0; i < NGW; ++i) {
-          const int g = 2 * i + half;
-          if (g < ng) {                                    // warp-uniform
-            tmem_ld_wait();
-            if (i + 1 < NGW && g + 2 < ng) {
-              tmem_ld32_at<0>(t_acc + (g + 2) * 64, r[(i + 1) & 1]);
-              tmem_ld32_at<32>(t_acc + (g + 2) * 64 + 32, r[(i + 1) & 1]);
-            } else {                                       // last read of this accumulator: give it back to the MMA warp
-              release_acc(acc);
-            }
-            uint32_t (&v)[64] = r[i & 1];
-            const int col0 = n0 + g * 64;
-            if (p.bias != nullptr && p.bias_f32) {
-#pragma unroll
-              for (int j = 0; j < 64; ++j)
-                v[j] = __float_as_uint(__uint_as_float(v[j]) + __shfl_sync(0xffffffffu, bias_reg[i * 2 + (j >> 5)], j & 31));
-            } else if (p.bias != nullptr) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {                // broadcast 16-byte reads: 8 bias values each
-                const uint4 bq = *reinterpret_cast<const uint4*>(sbias + g * 64 + q * 8);
-                const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  v[q * 8 + 2 * e] = __float_as_uint(__uint_as_float(v[q * 8 + 2 * e]) + bf16lo(bw[e]));
-                  v[q * 8 + 2 * e + 1] = __float_as_uint(__uint_as_float(v[q * 8 + 2 * e + 1]) + bf16hi(bw[e]));
-                }
-              }
-            }
-            uint32_t w[32];
-            if (kAux && p.aux != nullptr) {                // pre-activation copy (bf16) through its own tensor map
-#pragma unroll
-              for (int j = 0; j < 32; ++j) w[j] = pack_bf16x2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-              stage_store(w, &tmAux, col0, r0, b);
-            }
-            if (p.epilogue == FSB_EPI_GELU_TANH) {
-#pragma unroll
-              for (int j = 0; j < 64; ++j) v[j] = __float_as_uint(gelu_tanh_f(__uint_as_float(v[j])));
-            } else if (p.epilogue == FSB_EPI_GELU_ERF) {
-#pragma unroll
-              for (int j = 0; j < 64; ++j) v[j] = __float_as_uint(gelu_erf_f(__uint_as_float(v[j])));
-            }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) w[j] = pack_bf16x2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-            stage_store(w, &tmD, col0, r0, b);
-          }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (lane == 0) tma_store_wait_read<0>();     // smem must outlive the last bulk stores' reads
-    } else if (half == 0)
-    for (int t = tile_first; t < num_tiles; t += tile_step) {
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       int b, m_idx, n_idx;
       tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
-      const int row = m_idx * TILE_M + int(cta_rank) * GEMM_BM + quad * 32 + lane;
-      const int n0 = n_idx * BN;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const bool row_ok = row < p.M;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= p.N) break;  // warp-uniform
-        uint32_t r[32];
-        tmem_ld32(tmem_base + (uint32_t(quad * 32) << 16) + acc * BN + c * 32, r);
-        tmem_ld_wait();
-        float v[32];
+      int prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t so = uint64_t(stage) * (S::STAGE_BYTES >> 4);
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        const bool full_cols = (col0 + 32 <= p.N);
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          const uint64_t da = dsc_a + so + ((A_MN ? k * 2048 : k * 32) >> 4), db = dsc_b + so + ((B_MN ? k * 2048 : k * 32) >> 4);
+          if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+          else wgmma_ss_n128<A_MN, B_MN>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage can be refilled
+        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue from registers: accumulator j covers columns 8 (j / 4) + 2 (lane % 4) + (j & 1), rows r and r + 8
+      const int row0 = m_idx * GEMM_BM + wg * 64 + wl * 16 + (lane >> 2);
+      const int colq = n_idx * BN + 2 * (lane & 3);
+      const int64_t d_off = int64_t(b) * p.stride_d, aux_off = int64_t(b) * p.stride_aux;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = colq + 8 * j;
+        if (col >= p.N) continue;
+        const bool two = col + 1 < p.N;
+        float bv0 = 0.f, bv1 = 0.f;
         if (p.bias != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (full_cols || col0 + j < p.N) {
-              float bv = p.bias_f32 ? __ldg(reinterpret_cast<const float*>(p.bias) + col0 + j)
-                                    : __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col0 + j));
-              v[j] += bv;
-            }
-          }
-        }
-        if (p.aux != nullptr && row_ok) {  // pre-activation copy (bf16)
-          __nv_bfloat16* ap = reinterpret_cast<__nv_bfloat16*>(p.aux) + int64_t(b) * p.stride_aux +
-                              int64_t(row) * p.ldaux + col0;
-          if (full_cols) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              uint4 q;
-              q.x = pack_bf16x2(v[j], v[j + 1]); q.y = pack_bf16x2(v[j + 2], v[j + 3]);
-              q.z = pack_bf16x2(v[j + 4], v[j + 5]); q.w = pack_bf16x2(v[j + 6], v[j + 7]);
-              *reinterpret_cast<uint4*>(ap + j) = q;
-            }
+          if (p.bias_f32) {
+            bv0 = __ldg(reinterpret_cast<const float*>(p.bias) + col);
+            if (two) bv1 = __ldg(reinterpret_cast<const float*>(p.bias) + col + 1);
           } else {
-            for (int j = 0; j < 32 && col0 + j < p.N; ++j) ap[j] = __float2bfloat16(v[j]);
+            bv0 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col));
+            if (two) bv1 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col + 1));
           }
         }
-        if (p.epilogue == FSB_EPI_GELU_TANH) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_tanh_f(v[j]);
-        } else if (p.epilogue == FSB_EPI_GELU_ERF) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf_f(v[j]);
-        }
-        if (row_ok) {
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row >= p.M) continue;
+          float v0 = acc[4 * j + 2 * h] + bv0, v1 = acc[4 * j + 2 * h + 1] + bv1;
+          if (p.aux != nullptr) {   // pre-activation copy (bf16)
+            __nv_bfloat16* ap = reinterpret_cast<__nv_bfloat16*>(p.aux) + aux_off + int64_t(row) * p.ldaux + col;
+            if (two) *reinterpret_cast<uint32_t*>(ap) = pack_bf16x2(v0, v1);
+            else *ap = __float2bfloat16(v0);
+          }
+          if (p.epilogue == FSB_EPI_GELU_TANH) { v0 = gelu_tanh_f(v0); v1 = gelu_tanh_f(v1); }
+          else if (p.epilogue == FSB_EPI_GELU_ERF) { v0 = gelu_erf_f(v0); v1 = gelu_erf_f(v1); }
           if (p.d_f32) {
-            float* dp = reinterpret_cast<float*>(p.D) + int64_t(b) * p.stride_d + int64_t(row) * p.ldd + col0;
-            if (full_cols) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 q = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                if (p.accumulate) {
-                  float4 o = *reinterpret_cast<const float4*>(dp + j);
-                  q.x += o.x; q.y += o.y; q.z += o.z; q.w += o.w;
-                }
-                *reinterpret_cast<float4*>(dp + j) = q;
-              }
+            float* dp = reinterpret_cast<float*>(p.D) + d_off + int64_t(row) * p.ldd + col;
+            if (two) {
+              float2 q = make_float2(v0, v1);
+              if (p.accumulate) { const float2 o = *reinterpret_cast<const float2*>(dp); q.x += o.x; q.y += o.y; }
+              *reinterpret_cast<float2*>(dp) = q;
             } else {
-              for (int j = 0; j < 32 && col0 + j < p.N; ++j) dp[j] = p.accumulate ? dp[j] + v[j] : v[j];
+              *dp = p.accumulate ? *dp + v0 : v0;
             }
           } else {
-            __nv_bfloat16* dp =
-                reinterpret_cast<__nv_bfloat16*>(p.D) + int64_t(b) * p.stride_d + int64_t(row) * p.ldd + col0;
-            if (full_cols) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                if (p.accumulate) {
-                  uint4 o = *reinterpret_cast<const uint4*>(dp + j);
-                  v[j] += bf16lo(o.x); v[j + 1] += bf16hi(o.x); v[j + 2] += bf16lo(o.y); v[j + 3] += bf16hi(o.y);
-                  v[j + 4] += bf16lo(o.z); v[j + 5] += bf16hi(o.z); v[j + 6] += bf16lo(o.w); v[j + 7] += bf16hi(o.w);
-                }
-                uint4 q;
-                q.x = pack_bf16x2(v[j], v[j + 1]); q.y = pack_bf16x2(v[j + 2], v[j + 3]);
-                q.z = pack_bf16x2(v[j + 4], v[j + 5]); q.w = pack_bf16x2(v[j + 6], v[j + 7]);
-                *reinterpret_cast<uint4*>(dp + j) = q;
+            __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D) + d_off + int64_t(row) * p.ldd + col;
+            if (two) {
+              if (p.accumulate) {
+                const uint32_t o = *reinterpret_cast<const uint32_t*>(dp);
+                v0 += bf16lo(o); v1 += bf16hi(o);
               }
+              *reinterpret_cast<uint32_t*>(dp) = pack_bf16x2(v0, v1);
             } else {
-              for (int j = 0; j < 32 && col0 + j < p.N; ++j) {
-                float o = p.accumulate ? __bfloat162float(dp[j]) : 0.f;
-                dp[j] = __float2bfloat16(v[j] + o);
-              }
+              *dp = __float2bfloat16(p.accumulate ? __bfloat162float(*dp) + v0 : v0);
             }
           }
         }
       }
-      release_acc(acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (kCta2) cluster_sync_all();   // the peer may still be reading TMEM / signalling our barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (kCta2) tmem_dealloc_2cta<TMEM_COLS>(tmem_base); else tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
 // SMs left to concurrently running communication kernels (fsb_set_reserved_sms): a persistent GEMM CTA fills an SM
 // (all of its registers), so a collective that overlaps backward would otherwise push GEMM CTAs into a second wave.
 static int g_reserved_sms = 0;
-static inline int gemm_sms(bool pairs) {
-  // a blocked SM blocks its whole CTA pair: pair kernels give up two SMs per reserved one
-  const int n = num_sms() - (pairs ? 2 : 1) * g_reserved_sms;
-  return n < 2 ? 2 : n;
+static inline int gemm_sms() {
+  const int n = num_sms() - g_reserved_sms;
+  return n < 1 ? 1 : n;
 }
 
-template <int kLayout, int BN, bool kAux, bool kCta2>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmAux,
-                       const GemmParams& p, cudaStream_t stream) {
-  using S = GemmSmem<BN, kAux, kCta2>;
+template <int kLayout, int BN>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+  using S = GemmSmem<BN>;
   static bool configured = false;
-  auto kern = gemm_bf16_kernel<kLayout, BN, kAux, kCta2>;
+  auto kern = gemm_bf16_kernel<kLayout, BN>;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
     if (e != cudaSuccess) {
@@ -505,26 +274,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
     configured = true;
   }
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
-  if constexpr (kCta2) {
-    const int pairs = gemm_sms(true) / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * (num_tiles < pairs ? num_tiles : pairs));
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = S::TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmD, tmAux, p);
-    if (e != cudaSuccess) {
-      set_error("gemm: cluster launch failed: %s", cudaGetErrorString(e));
-      return FSB_ERR_CUDA;
-    }
-  } else {
-    const int grid = num_tiles < gemm_sms(false) ? num_tiles : gemm_sms(false);
-    kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
-  }
+  const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
+  kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, p);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
@@ -558,7 +309,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
 static int gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                      int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_pair = false);
+                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_wide = false);
 
 }  // namespace fsb
 
@@ -570,19 +321,19 @@ extern "C" int fsb_set_reserved_sms(int n) {
   return FSB_OK;
 }
 
-// Split-K plan for weight-gradient GEMMs whose output has too few tiles to occupy the SMs (e.g. 768 x 768 x 32768: 36
+// Split-K plan for weight-gradient GEMMs whose output has too few tiles to occupy the SMs (e.g. 768 x 768 x 32768: 18
 // tiles): `splits` K-chunks run as a batched GEMM into an fp32 scratch and are summed in a fixed order (deterministic).
-// Preferred: 256 x 256 CTA-pair tiles (a lone 128 x 128 tile is shared-memory-bound at half the MMA rate), K split so that the
-// SM pairs are busy; small outputs (M or N < 256) keep 128 x 128 tiles. Returns 0 / 1 when the call does not split.
-static int splitk_plan(int layout, int64_t M, int64_t N, int64_t K, int64_t batch, bool plain, bool* pair_out) {
+// Preferred: 128 x 256 tiles (twice the operand reuse of 128 x 128), K split so that the SMs are busy; outputs narrower than
+// 256 keep 128 x 128 tiles. Returns 0 / 1 when the call does not split.
+static int splitk_plan(int layout, int64_t M, int64_t N, int64_t K, int64_t batch, bool plain, bool* wide_out) {
   if (!(layout == FSB_GEMM_TN && batch == 1 && plain && M > 0 && N > 0 && N % 4 == 0 && (M * N) % 8 == 0 && K >= 4096)) return 0;
-  const bool pair = M >= 256 && N >= 256;
-  const int64_t tiles = pair ? ((M + 255) / 256) * ((N + 255) / 256) : ((M + GEMM_BM - 1) / GEMM_BM) * ((N + 127) / 128);
-  const int64_t slots = pair ? num_sms() / 2 : num_sms();
+  const bool wide = N >= 256;
+  const int64_t tiles = ((M + GEMM_BM - 1) / GEMM_BM) * (wide ? (N + 255) / 256 : (N + 127) / 128);
+  const int64_t slots = num_sms();
   int splits = int(slots / tiles);
   if (splits > 16) splits = 16;
   while (splits > 1 && (K % (int64_t(splits) * GEMM_BK) != 0 || K / splits < 1024)) --splits;
-  if (pair_out) *pair_out = pair;
+  if (wide_out) *wide_out = wide;
   return (splits >= 2 && tiles * 2 <= slots) ? splits : 0;
 }
 
@@ -597,9 +348,9 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
                              int64_t stride_b, int64_t stride_d, int64_t stride_aux, void* workspace,
                              size_t workspace_bytes, fsb_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  bool pair = false;
+  bool wide = false;
   const int splits = (d_dtype == FSB_BF16 || d_dtype == FSB_F32)
-                         ? splitk_plan(layout, M, N, K, batch, bias == nullptr && aux == nullptr && epilogue == FSB_EPI_NONE, &pair)
+                         ? splitk_plan(layout, M, N, K, batch, bias == nullptr && aux == nullptr && epilogue == FSB_EPI_NONE, &wide)
                          : 0;
   if (splits >= 2) {
     // the scratch is the caller's (fsb_gemm_workspace_bytes): the library allocates nothing. Too small a workspace is an
@@ -613,7 +364,7 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
       float* ws = static_cast<float*>(workspace);
       const int64_t kc = K / splits;
       int rc = gemm_impl(layout, M, N, kc, A, lda, B, ldb, ws, N, FSB_F32, nullptr, FSB_BF16, FSB_EPI_NONE, 0, nullptr, 0,
-                         splits, kc * lda, kc * ldb, M * N, 0, stream, pair);
+                         splits, kc * lda, kc * ldb, M * N, 0, stream, wide);
       if (rc) return rc;
       FSB_REQUIRE(ldd % 4 == 0, "gemm: ldd=%ld not vector-aligned", (long)ldd);
       const int64_t work = M * (N / 4);
@@ -630,7 +381,7 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
 static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                           int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                           int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_pair) {
+                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_wide) {
   FSB_REQUIRE(layout >= 0 && layout <= 2, "gemm: bad layout %d", layout);
   FSB_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, "gemm: non-positive dims M=%ld N=%ld K=%ld batch=%ld", (long)M,
               (long)N, (long)K, (long)batch);
@@ -649,14 +400,10 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   // Tensor maps: always rank 3 (inner, outer, batch).
   CUtensorMap tmA, tmB;
   const bool a_mn = (layout == FSB_GEMM_TN), b_mn = (layout != FSB_GEMM_NT);
-  // 128 x 256 tiles unless they would leave a large part of the 148 SMs idle (weight-gradient GEMMs of small models:
+  // 128 x 256 tiles unless they would leave a large part of the SMs idle (weight-gradient GEMMs of small models:
   // e.g. 768 x 2304 x 32768 is only 54 such tiles) — then 128 x 128 tiles double the parallelism.
   const int64_t tiles256 = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + 255) / 256) * batch;
-  const int BN = (force_pair || (N > 128 && tiles256 * 10 >= int64_t(num_sms()) * 7)) ? 256 : 128;
-  // CTA pairs (cta_group::2, 256 x 256 tiles) once there is at least one pair tile per SM pair; FSB_GEMM_CTA2=0/1 overrides.
-  static const int cta2_env = [] { const char* e = getenv("FSB_GEMM_CTA2"); return e ? atoi(e) : -1; }();
-  const bool cta2 = force_pair || (BN == 256 && M > GEMM_BM && tiles256 >= num_sms() &&   // (M <= 128: the peer CTA would own no rows)
-                                   (cta2_env < 0 ? FSB_GEMM_CTA2_DEFAULT : cta2_env != 0));
+  const int BN = (force_wide || (N > 128 && tiles256 * 10 >= int64_t(num_sms()) * 7)) ? 256 : 128;
   {
     // A: K-major -> memory [M rows, K inner]; MN-major -> memory [K rows, M inner]
     uint64_t dims[3] = {uint64_t(a_mn ? M : K), uint64_t(a_mn ? K : M), uint64_t(batch)};
@@ -668,25 +415,11 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   {
     uint64_t dims[3] = {uint64_t(b_mn ? N : K), uint64_t(b_mn ? K : N), uint64_t(batch)};
     uint64_t strides[2] = {uint64_t(ldb) * 2, uint64_t(batch > 1 ? stride_b : (b_mn ? K : N) * ldb) * 2};
-    uint32_t box[3] = {64, uint32_t(b_mn ? GEMM_BK : (cta2 ? BN / 2 : BN)), 1};
+    uint32_t box[3] = {64, uint32_t(b_mn ? GEMM_BK : BN), 1};
     int rc = make_tmap_bf16(&tmB, B, 3, dims, strides, box);
     if (rc) return rc;
   }
   GemmParams p;
-  p.tma_store = (d_dtype == FSB_BF16 && !accumulate) ? 1 : 0;
-  CUtensorMap tmD = tmA, tmAux = tmA;  // placeholders when the bulk-store path is off / there is no aux output
-  if (p.tma_store) {
-    uint64_t dims[3] = {uint64_t(N), uint64_t(M), uint64_t(batch)};
-    uint64_t strides[2] = {uint64_t(ldd) * 2, uint64_t(batch > 1 ? stride_d : M * ldd) * 2};
-    uint32_t box[3] = {64, 32, 1};   // one epilogue warp's rows x one 128-byte column group
-    int rc = make_tmap_bf16(&tmD, D, 3, dims, strides, box);
-    if (rc) return rc;
-    if (aux != nullptr) {
-      uint64_t astrides[2] = {uint64_t(ldaux) * 2, uint64_t(batch > 1 ? stride_aux : M * ldaux) * 2};
-      rc = make_tmap_bf16(&tmAux, aux, 3, dims, astrides, box);
-      if (rc) return rc;
-    }
-  }
   p.D = D; p.aux = aux; p.bias = bias;
   p.ldd = ldd; p.ldaux = ldaux; p.stride_d = stride_d; p.stride_aux = stride_aux;
   p.M = int(M); p.N = int(N); p.K = int(K); p.batch = int(batch);
@@ -694,31 +427,23 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   p.epilogue = epilogue; p.accumulate = accumulate;
   static const int l2hint_env = [] { const char* e = getenv("FSB_GEMM_L2HINT"); return e ? atoi(e) : 0; }();
   p.l2_hints = l2hint_env;
-  p.tiles_m = cta2 ? int((M + 2 * GEMM_BM - 1) / (2 * GEMM_BM)) : int((M + GEMM_BM - 1) / GEMM_BM);
+  p.tiles_m = int((M + GEMM_BM - 1) / GEMM_BM);
   p.tiles_n = int((N + BN - 1) / BN);
   // Rasterisation: tiles are walked m-fastest inside groups of group_m m-tiles, so one wave of CTAs touches group_m A panels
-  // and #SMs/group_m B panels. HBM traffic per wave is minimal when both sides weigh the same (group_m ~ sqrt(#SMs * BN/BM):
-  // 16 for 256-wide tiles, 12 for 128-wide ones); measured with ncu, panels do not survive in the L2 from one wave to the next
-  // unless they are small (the two dies' L2 halves mirror shared lines), so the group only grows beyond that while its A panels
-  // (group_m x 128 x K bf16) stay under ~32 MB (ncu: 8192x15360x5120 reads 1379 MB at group_m 8, 584 MB at 24; 241 MB algorithmic).
+  // and #SMs/group_m B panels. HBM traffic per wave is least when both sides weigh about the same (group_m ~ sqrt(#SMs * BN/BM):
+  // 16 for 256-wide tiles, 12 for 128-wide ones); the group only grows beyond that while its A panels (group_m x 128 x K bf16)
+  // stay well inside the L2 (~32 MB of its 50 MB).
   {
     const int64_t a_panel = int64_t(GEMM_BM) * K * 2;
     const int64_t base = BN == 256 ? 16 : 12;
     int64_t gm = (int64_t(32) << 20) / a_panel;
     gm = gm < base ? base : (gm > 64 ? 64 : gm);
-    p.group_m = cta2 ? int((gm + 1) / 2) : int(gm);   // pair tiles are two A panels tall
+    p.group_m = int(gm);
   }
 
-#define FSB_GEMM_DISPATCH(L)                                                    \
-  case L:                                                                        \
-    if (cta2)                                                                                                    \
-      return (p.tma_store && aux != nullptr) ? launch_gemm<L, 256, true, true>(tmA, tmB, tmD, tmAux, p, stream)   \
-                                             : launch_gemm<L, 256, false, true>(tmA, tmB, tmD, tmAux, p, stream); \
-    if (p.tma_store && aux != nullptr)                                                                           \
-      return BN == 256 ? launch_gemm<L, 256, true, false>(tmA, tmB, tmD, tmAux, p, stream)                        \
-                       : launch_gemm<L, 128, true, false>(tmA, tmB, tmD, tmAux, p, stream);                       \
-    return BN == 256 ? launch_gemm<L, 256, false, false>(tmA, tmB, tmD, tmAux, p, stream)                         \
-                     : launch_gemm<L, 128, false, false>(tmA, tmB, tmD, tmAux, p, stream);
+#define FSB_GEMM_DISPATCH(L) \
+  case L:                    \
+    return BN == 256 ? launch_gemm<L, 256>(tmA, tmB, p, stream) : launch_gemm<L, 128>(tmA, tmB, p, stream);
   switch (layout) {
     FSB_GEMM_DISPATCH(FSB_GEMM_NT)
     FSB_GEMM_DISPATCH(FSB_GEMM_NN)

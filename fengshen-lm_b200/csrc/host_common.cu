@@ -23,7 +23,7 @@ int num_sms() {
   if (dev < 0 || dev >= 64) dev = 0;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];

@@ -1,4 +1,4 @@
-// fsb200 — the reference's two in-tree CUDA ops, re-designed for sm_100a (HBM-bound row softmax):
+// fsb200 — the reference's two in-tree CUDA ops, re-designed for sm_90a (HBM-bound row softmax):
 //   scaled_masked_softmax_cuda.{forward,backward}              fused_kernels/scaled_masked_softmax.h:117-335
 //       y = softmax(mask ? -10000 : scale * x) over the last dim;  x [b, np, sq, sk], mask uint8 [b|1, 1, sq, sk]
 //       dx = scale * (dy*y - y * sum(dy*y)), written IN PLACE over dy (scaled_masked_softmax_cuda.cu:95-105)

@@ -1,2 +1,2 @@
-"""fsb200 — B200-native backend for the Fengshen data-parallel pretraining step (see DESIGN.md)."""
+"""fsb200 — H100-native backend for the Fengshen data-parallel pretraining step (see DESIGN.md)."""
 __version__ = "0.1"

@@ -1,4 +1,4 @@
-/* fsb200 — C ABI of libfsb200.so, the B200 (sm_100a) backend for the Fengshen data-parallel pretraining step.
+/* fsb200 — C ABI of libfsb200.so, the H100 (sm_90a) backend for the Fengshen data-parallel pretraining step.
  *
  * This is the drop-in boundary (SURVEY.md §8b). The reference reaches its native code through pybind11
  * torch-extension modules that take torch::Tensor (fengshen/models/megatron/fused_kernels/
@@ -38,9 +38,9 @@ typedef enum { FSB_BF16 = 0, FSB_F32 = 1, FSB_U32 = 2, FSB_U64 = 3 /* index buil
 /* ---- library ---------------------------------------------------------------------------------------------- */
 int fsb_version(void);               /* 1000*major + minor */
 const char* fsb_last_error(void);    /* thread-local, never NULL */
-int fsb_num_sms(void);               /* SM count of the current device (148 on B200) */
+int fsb_num_sms(void);               /* SM count of the current device (132 on H100 SXM) */
 
-/* ---- GEMM (tcgen05 + TMA + TMEM) --------------------------------------------------------------------------
+/* ---- GEMM (wgmma + TMA) ------------------------------------------------------------------------------------
  * Replaces F.linear / torch.baddbmm / torch.bmm -> cuBLAS on the hot path:
  *   ColumnParallelLinear.forward  fengshen/models/megatron/mpu/layers.py:347-360  (Y = X W^T)
  *   RowParallelLinear.forward     fengshen/models/megatron/mpu/layers.py:451-470
@@ -57,12 +57,12 @@ int fsb_num_sms(void);               /* SM count of the current device (148 on B
  * Requirements: pointers 16-byte aligned; lda/ldb/ldd multiples of 8 elements.
  * aux (bf16, may be NULL): receives acc + bias BEFORE the activation (saved for the activation's backward).
  * `batch` > 1 runs independent GEMMs with element strides stride_a/b/d between them (use 1 and 0 otherwise).
- * Kernel selection is internal: CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles) when the output has at least one such tile
- * per SM pair, single-CTA 128 x 256 / 128 x 128 tiles otherwise. FSB_GEMM_TN calls whose output has few tiles and K >= 4096
+ * Kernel selection is internal: persistent 128 x 256 tiles, or 128 x 128 tiles when the wide ones would leave many SMs
+ * idle. FSB_GEMM_TN calls whose output has few tiles and K >= 4096
  * (weight gradients of small models) split K: the chunks are accumulated in fp32 in the caller's `workspace`
  * (fsb_gemm_workspace_bytes(layout, M, N, K) bytes; 0 when the call does not split) and reduced in a fixed order — results
  * are deterministic; a split call with too small a workspace is an error. Other calls ignore `workspace` (may be NULL).
- * fsb_set_reserved_sms(n): persistent GEMM grids leave n SMs (2n for CTA-pair kernels) to communication kernels that
+ * fsb_set_reserved_sms(n): persistent GEMM grids leave n SMs to communication kernels that
  * overlap them (the ZeRO engine's reduce-scatter / all-gather on the side stream); 0 restores the full grid.
  * FSB_EPI_GELU_ERF evaluates erf through Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, below the bf16 rounding of the output).
  */
@@ -203,7 +203,7 @@ int fsb_scaled_upper_triang_masked_softmax_bwd(void* dy_inplace, const void* y, 
                                                float scale, fsb_stream_t stream);
 int fsb_softmax_get_batch_per_block(int64_t sq, int64_t sk, int64_t batches, int64_t attn_heads);
 
-/* ---- fused scaled-dot-product attention (tcgen05, flash-style online softmax) ------------------------------
+/* ---- fused scaled-dot-product attention (wgmma, flash-style online softmax) ----------------------------------
  * Replaces ParallelSelfAttention.flash_attention (fengshen/models/megatron/layers/transformer.py:410-456; 3P
  * flash_attn_cuda.fwd/bwd, layers/flash_attention.py:31-47,81-101) and the legacy baddbmm -> FusedScaleMaskSoftmax ->
  * bmm path (transformer.py:307-408). q/k/v are read in place from the packed QKV projection output:
@@ -227,7 +227,7 @@ int fsb_sdpa_fwd(const void* q, const void* k, const void* v, void* o, float* ls
  * rel_bias as in the forward; drel_bias (fp32 [nheads, seq_q + seq_kv - 1], may be NULL) is ACCUMULATED into:
  *   drel_bias[h][r] += sum over (batch, q) of dS[q, q + r - (seq_q - 1)]   (gradient w.r.t. the bias vector; the
  * [buckets, heads] table gradient is its scatter over bucket(r), autograd of T5Attention.compute_bias). It needs a workspace of
- * fsb_sdpa_bwd_workspace_bytes(batch, seq_q, seq_kv, nheads) bytes: per-warp diagonal sums written by the dQ kernel and
+ * fsb_sdpa_bwd_workspace_bytes(batch, seq_q, seq_kv, nheads) bytes: per-step diagonal sums written by the dQ kernel and
  * reduced in a fixed order (no atomics). */
 size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads);
 int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,

@@ -1,4 +1,4 @@
-"""The two HF-backed recipes as test bodies, shared by tests/test_hf_scripts_gpu.py (real fsb200 models on a B200) and
+"""The two HF-backed recipes as test bodies, shared by tests/test_hf_scripts_gpu.py (real fsb200 models on a GPU) and
 tests/test_hf_trainer_flow_cpu.py (tests/toy_models.py doubles + tests/cpu_kernels.py): launcher -> transformers rebinding ->
 script -> compat Trainer -> ZeroEngine -> checkpoints -> resume -> export. Only the loss thresholds differ between the two."""
 import json

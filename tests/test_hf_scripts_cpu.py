@@ -1,9 +1,10 @@
 """CPU half of the HF-backed recipes (C2 / C3; SURVEY §8a row A16, §8f rank 3): everything the scripts do before the model
 touches CUDA — the launcher's sys.path / transformers rebinding, argument parsers, tokenizer, collator, data modules, batches —
-for fsb200's own example script and, where /root/reference exists, for the UNMODIFIED reference scripts
-(examples/pretrain_erlangshen_bert/pretrain_erlangshen.py, examples/wenzhong_qa/finetune_wenzhong.py). Building a model without
-a GPU must fail loudly (no CPU fallback on the product path)."""
+for fsb200's own example script, and the collator of the UNMODIFIED reference script
+(examples/pretrain_erlangshen_bert/pretrain_erlangshen.py) against a golden batch it produced. Building a model without a GPU
+must fail loudly (no CPU fallback on the product path)."""
 import argparse
+import json
 import os
 import runpy
 import sys
@@ -15,11 +16,7 @@ import torch
 import hf_fixtures as F
 
 ROOT = F.ROOT
-REF = os.environ.get("FSB_REFERENCE_ROOT", "/root/reference")
-ERLANGSHEN = os.path.join(REF, "fengshen", "examples", "pretrain_erlangshen_bert", "pretrain_erlangshen.py")
-WENZHONG = os.path.join(REF, "fengshen", "examples", "wenzhong_qa", "finetune_wenzhong.py")
 EXAMPLE = os.path.join(ROOT, "examples", "pretrain_erlangshen_bert.py")
-needs_ref = pytest.mark.skipif(not os.path.exists(ERLANGSHEN), reason="reference tree not present on this machine")
 
 
 @pytest.fixture
@@ -117,38 +114,26 @@ def test_example_script_cpu_half(launcher, tmp_path):
             ns["ErLangShenBert"](args, tokenizer=tok)
 
 
-@needs_ref
-def test_unmodified_erlangshen_script_cpu_half(launcher, tmp_path):
-    launcher(ERLANGSHEN)
-    ns = runpy.run_path(ERLANGSHEN, run_name="reference_not_main")      # module body: imports + class definitions, as written
-    assert ns["MegatronBertForPreTraining"].__module__ == "fsb200.hf"
-    assert os.path.join("fengshen-lm_b200", "compat") in sys.modules["fengshen.data.data_utils.mask_utils"].__file__
+def test_erlangshen_collator_matches_the_unmodified_script_golden(launcher, tmp_path):
+    """The collator of the UNMODIFIED reference script pretrain_erlangshen.py, run on these fixtures
+    (tests/golden/erlangshen_script_batch.npz, oracle/make_golden_erlangshen_script.py) == the library collator, draw for draw."""
+    launcher(EXAMPLE)
+    golden = np.load(os.path.join(ROOT, "tests", "golden", "erlangshen_script_batch.npz"))
     F.bert_dir(tmp_path / "m")
     corpus = F.bert_corpus(tmp_path / "train.json")
-    args = _erlangshen_args(ns, tmp_path, tmp_path / "m", corpus)
-    tok = ns["AutoTokenizer"].from_pretrained(args.model_path)
-    coll = ns["ErLangShenCollator"](tokenizer=tok, max_seq_length=args.max_seq_length, masked_lm_prob=args.masked_lm_prob,
-                                    content_key=args.sample_content_key)
-    coll.setup()
-    dm = ns["UniversalDataModule"](tokenizer=tok, args=args, collate_fn=coll)        # --train_file through `datasets`
-    ds = dm.datasets[args.train_datasets_field]
-    rows = [ds[i] for i in range(4)]
-    coll.np_rng = np.random.RandomState(5)
-    coll.vocab_id_list = sorted(coll.vocab_id_list)
-    theirs = coll(rows)
-    _check_mlm_batch(theirs, 4, 64, tok)
-    # the script's own collator (reference code) on the compat helpers == the library collator, draw for draw
+    rows = [json.loads(line) for line in open(corpus, encoding="utf8")][:4]
+    from transformers import AutoTokenizer
+    tok = AutoTokenizer.from_pretrained(str(tmp_path / "m"))
     from fengshen.data.data_utils.collators import ErLangShenCollator as Lib
-    lib = Lib(tokenizer=tok, max_seq_length=args.max_seq_length, masked_lm_prob=args.masked_lm_prob)
+    lib = Lib(tokenizer=tok, max_seq_length=64, masked_lm_prob=0.15)
     lib.setup()
     lib.np_rng = np.random.RandomState(5)
     lib.vocab_id_list = sorted(lib.vocab_id_list)
     ours = lib(rows)
-    for k in theirs:
-        assert torch.equal(theirs[k], ours[k]), k
-    if not torch.cuda.is_available():
-        with pytest.raises(RuntimeError, match="CUDA|NVIDIA"):
-            ns["ErLangShenBert"](args, tokenizer=tok)
+    _check_mlm_batch(ours, 4, 64, tok)
+    assert set(ours) == set(golden.files)
+    for k in golden.files:
+        assert np.array_equal(ours[k].numpy(), golden[k]), k
 
 
 def _qa_args(parser_owner, tmp, mdir):
@@ -175,31 +160,3 @@ def test_medical_qa_datamodule(launcher, tmp_path):
     n = int(b["attention_mask"][0].sum())
     text = rows[0]["Question"] + rows[0]["answer"]
     assert dm.train_data.tokenizer.decode(b["input_ids"][0, :n]) == text[:n]           # byte-level, ASCII: one token per char
-
-
-@needs_ref
-def test_unmodified_wenzhong_script_cpu_half(launcher, tmp_path):
-    launcher(WENZHONG)
-    ns = runpy.run_path(WENZHONG, run_name="reference_not_main")
-    assert ns["GPT2LMHeadModel"].__module__ == "fsb200.hf"
-    assert os.path.join("fengshen-lm_b200", "compat") in sys.modules[ns["GPT2QADataModel"].__module__].__file__
-    F.gpt2_tokenizer_dir(tmp_path / "m")
-    F.qa_files(tmp_path / "data")
-    p = argparse.ArgumentParser("QA Task")
-    p.add_argument('--do_eval_only', action='store_true', default=False)
-    p.add_argument('--pretrained_model_path', default='google/mt5-small', type=str)
-    p.add_argument('--output_save_path', default='./predict.json', type=str)
-    p = ns["GPT2QADataModel"].add_data_specific_args(p)
-    p = ns["Trainer"].add_argparse_args(p)
-    p = ns["GPT2FinetuneMedicalQAModelCheckpoint"].add_argparse_args(p)
-    p = ns["GPT2FinetuneMedicalQA"].add_model_specific_args(p)
-    args = p.parse_args(["--pretrained_model_path", str(tmp_path / "m"), "--data_dir", str(tmp_path / "data"),
-                         "--train_batchsize", "4", "--valid_batchsize", "4", "--max_seq_length", "64", "--num_workers", "0",
-                         "--max_epochs", "1", "--gpus", "1", "--default_root_dir", str(tmp_path),
-                         "--dirpath", str(tmp_path / "ckpt")])
-    dm = ns["GPT2QADataModel"](args)
-    assert len(dm.train_dataloader()) == 12
-    cb = ns["GPT2FinetuneMedicalQAModelCheckpoint"](args).callbacks
-    assert cb.save_last and cb.every_n_train_steps == 100
-    with pytest.raises((FileNotFoundError, RuntimeError)):      # no weights in the fixture directory / no GPU: loud either way
-        ns["GPT2FinetuneMedicalQA"](args, len(dm.train_dataloader()))

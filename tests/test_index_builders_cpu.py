@@ -140,33 +140,16 @@ def test_blending_follows_weights(H):
 
 
 def test_blendable_dataset_and_the_unmodified_reference_class_on_our_helpers(H):
-    """The caller of build_blending_indices. Where the reference tree exists, ITS BlendableDataset (loaded from its file, which
-    does `from fengshen.data.megatron_dataloader import helpers`) runs on the fsb200 helpers and yields the same items."""
+    """The caller of build_blending_indices: the compat BlendableDataset on the fsb200 helpers yields, item for item, what the
+    unmodified reference BlendableDataset on its own C++ helpers yielded for the same parts and weights
+    (tests/golden/blendable_dataset.json, oracle/make_golden_blendable_dataset.py)."""
+    import json
     from fengshen.data.megatron_dataloader.blendable_dataset import BlendableDataset
-    parts = [[("a", i) for i in range(70)], [("b", i) for i in range(20)], [("c", i) for i in range(10)]]
-    ds = BlendableDataset(parts, [7, 2, 1])
-    assert len(ds) == 100
-    items = [ds[i] for i in range(100)]
-    for name, n in (("a", 70), ("b", 20), ("c", 10)):
+    golden = json.load(open(os.path.join(ROOT, "tests", "golden", "blendable_dataset.json")))
+    parts = [[(name, i) for i in range(n)] for name, n in golden["sizes"]]
+    ds = BlendableDataset(parts, golden["weights"])
+    assert len(ds) == len(golden["items"]) == 100
+    items = [ds[i] for i in range(len(ds))]
+    for name, n in golden["sizes"]:
         assert [v for k, v in items if k == name] == list(range(n))          # everything consumed exactly once, in order
-    assert [k for k, _ in items[:10]].count("a") == 7
-    ref_file = os.path.join(os.environ.get("FSB_REFERENCE_ROOT", "/root/reference"),
-                            "fengshen/data/megatron_dataloader/blendable_dataset.py")
-    if not os.path.exists(ref_file):
-        return
-    import importlib.util
-    import torch.distributed as dist
-    spec = importlib.util.spec_from_file_location("ref_blendable_dataset", ref_file)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    started = False
-    if not dist.is_initialized():                       # the reference calls torch.distributed.get_rank() unconditionally
-        dist.init_process_group("gloo", init_method="tcp://127.0.0.1:29631", rank=0, world_size=1)
-        started = True
-    try:
-        with quiet_stdout():
-            theirs = mod.BlendableDataset(parts, [7, 2, 1])
-        assert [theirs[i] for i in range(100)] == items
-    finally:
-        if started:
-            dist.destroy_process_group()
+    assert [list(it) for it in items] == golden["items"]

@@ -92,8 +92,8 @@ def test_gemm_splitk_wgrad():
 
 @pytest.mark.parametrize("layout", [L.GEMM_NT, L.GEMM_NN, L.GEMM_TN])
 def test_gemm_cta_pair_tiles(layout):
-    """Shapes with >= one 256x256 tile per SM pair run the cta_group::2 kernel; ragged M / N edges, every epilogue."""
-    M, N, K = 2304 + 40, 4096 + 72, 320          # 10 x 17 pair tiles, both edges ragged (TMA zero-fill / clipped stores)
+    """Several waves of persistent 128 x 256 tiles with ragged M / N edges, every epilogue."""
+    M, N, K = 2304 + 40, 4096 + 72, 320          # 19 x 17 tiles, both edges ragged (TMA zero-fill / clipped stores)
     if layout == L.GEMM_NT:
         a, b = _rand(M, K, seed=11), _rand(N, K, seed=12, scale=0.1)
         ref = a.float() @ b.float().t()
@@ -104,19 +104,19 @@ def test_gemm_cta_pair_tiles(layout):
         a, b = _rand(K, M, seed=11), _rand(K, N, seed=12, scale=0.1)
         ref = a.float().t() @ b.float()
     out = ops.gemm(layout, a, b)
-    _close(out, ref, atol=2e-2 * math.sqrt(K / 64), rtol=1e-2, what="pair-tile bf16")
+    _close(out, ref, atol=2e-2 * math.sqrt(K / 64), rtol=1e-2, what="large-tile bf16")
     bias = _rand(N, seed=13)
     aux = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
     out = ops.gemm(layout, a, b, bias=bias, epilogue=L.EPI_GELU_TANH, aux=aux)
     pre = ref + bias.float()
-    _close(aux, pre, 3e-2, 1e-2, "pair-tile aux")
-    _close(out, torch.nn.functional.gelu(pre, approximate="tanh"), 3e-2, 1e-2, "pair-tile gelu")
+    _close(aux, pre, 3e-2, 1e-2, "large-tile aux")
+    _close(out, torch.nn.functional.gelu(pre, approximate="tanh"), 3e-2, 1e-2, "large-tile gelu")
     acc = torch.full((M, N), 0.5, dtype=torch.float32, device=DEV)
     ops.gemm(layout, a, b, out=acc, accumulate=True)
-    _close(acc, ref + 0.5, atol=1e-3 * math.sqrt(K / 64), rtol=1e-4, what="pair-tile fp32 accumulate")
+    _close(acc, ref + 0.5, atol=1e-3 * math.sqrt(K / 64), rtol=1e-4, what="large-tile fp32 accumulate")
     accb = torch.ones(M, N, dtype=torch.bfloat16, device=DEV)
     ops.gemm(layout, a, b, out=accb, accumulate=True)
-    _close(accb, ref + 1.0, atol=3e-2 * math.sqrt(K / 64), rtol=1e-2, what="pair-tile bf16 accumulate")
+    _close(accb, ref + 1.0, atol=3e-2 * math.sqrt(K / 64), rtol=1e-2, what="large-tile bf16 accumulate")
 
 
 @pytest.mark.parametrize("act", [L.ACT_GELU_TANH, L.ACT_GELU_ERF, L.ACT_TANH])

@@ -7,7 +7,7 @@ keeps bf16 activations with fp32 accumulation, the oracle is fp32 end to end):
   logits          |delta| <= 4 * 2^-8 * max|logit|
   gradients       cosine >= 0.999 and norm ratio within 2 % per parameter
   20-step curve   max |delta| <= 1e-2 against the reference's fp32 curve AND <= 1/3 of |reference bf16 - reference fp32|
-                  (measured 3e-3 / 6e-3 vs 4e-2 for the reference's own bf16 run; see the curve test)
+                  (the reference's own bf16 run is 4e-2 away from its fp32 run; see the curve test)
 """
 import glob
 import math
@@ -94,9 +94,8 @@ def test_loss_curve_vs_reference_golden(path):
     # north_star asks for 1e-3 against "the reference CPU run". The reference's OWN bf16 run on the CPU (its modules cast to
     # bfloat16, fp32 master AdamW: `loss_curve_bf16`, oracle/make_golden.py) sits 4.0e-2 / 4.1e-2 (max; 1.5e-2 / 1.7e-2 mean)
     # away from its fp32 run over these 20 steps — that is the noise floor of bf16 arithmetic on this problem, 40x the
-    # north_star figure. This path (bf16 storage, fp32 accumulation inside every kernel, fp32 master weights) measured
-    # 3.0e-3 (hn128) and 6.1e-3 (hn64) on B200 (tools/probe_loss_curve.py): 7-13x CLOSER to the fp32 reference than the
-    # reference's bf16 arithmetic is. Asserted: within 1e-2 absolute of the fp32 reference curve AND at most a third of the
+    # north_star figure. This path keeps bf16 storage with fp32 accumulation inside every kernel and fp32 master weights
+    # (tools/probe_loss_curve.py prints its distance). Asserted: within 1e-2 absolute of the fp32 reference curve AND at most a third of the
     # reference's own bf16-vs-fp32 distance; 1e-3 is not reachable by any bf16 step, and the test says so instead of hiding it.
     ref16 = np.abs(g["loss_curve_bf16"] - g["loss_curve"]).max()
     assert ref16 > 1e-2, ref16                      # the noise-floor claim itself is pinned

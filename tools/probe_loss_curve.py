@@ -1,4 +1,4 @@
-"""Dev tool: print the max |delta| between the bf16 B200 20-step loss curve and the reference's fp32 CPU curve (goldens)."""
+"""Dev tool: print the max |delta| between the bf16 GPU 20-step loss curve and the reference's fp32 CPU curve (goldens)."""
 import importlib.util, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
