@@ -10,9 +10,14 @@
 //
 // Roles (384 threads = 3 warpgroups): warpgroup 0 = TMA producer (one thread issues; setmaxnreg gives its registers to the
 // others), warpgroups 1-2 = consumers: each owns 64 rows of the 128 x BN tile, issues m64nBNk16 wgmmas on the shared stage
-// and runs the epilogue (bias / activation / pre-activation copy / bf16 or fp32 store, optionally accumulating) straight from
-// its accumulator registers. The producer runs up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
-// operands stream in during the epilogue. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
+// and runs the epilogue: bias / activation (and the optional accumulate into D) in registers, then 64-row x 128-byte
+// sub-tiles are written to a double-buffered, 128B-swizzled shared-memory staging area and leave by TMA bulk stores
+// (D and the pre-activation copy alike). The consumer does not wait for a store; it waits only before refilling a staging
+// buffer whose previous store has not yet been read out, so the global writes overlap the next tile's MMAs. Ragged tile
+// edges are clipped by the D / aux tensor maps. The producer runs up to STAGES k-blocks ahead, across tile boundaries, so the
+// next tile's operands stream in during the epilogue. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
+// K-split weight-gradient GEMMs carry the split as the batch coordinate of the tile: split s reads its own range of
+// k-blocks of the unbatched operands through full-K tensor maps and writes an fp32 partial product to D[s] (gemm_plan).
 #include <stdlib.h>
 
 #include "host_common.h"
@@ -37,15 +42,22 @@ struct GemmParams {
   int tiles_m, tiles_n;
   int group_m;     // m-tiles per rasterisation group (see fsb_gemm_bf16)
   int l2_hints;    // bit 0: A panels evict-last, bit 1: B panels evict-first (FSB_GEMM_L2HINT)
+  int ksplits;     // > 1: the batch index is a K-split of unbatched A / B (k_range)
 };
 
+// Shared memory: the operand stages, then the epilogue staging area, two 64-row x 128-byte sub-tile buffers (64 bf16 or 32
+// fp32 columns) per consumer warpgroup. Double-buffered 8 KB sub-tiles rather than a whole-tile buffer keep all 4 (6) operand
+// stages: a 128 x 256 bf16 tile would need 64 KB, i.e. one stage fewer, and the K = 768 GEMMs (12 k-blocks per tile) lean
+// on the producer running far ahead across the tile boundary.
 template <int BN>
 struct GemmSmem {
   static constexpr int STAGES = BN == 256 ? 4 : 6;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int EPI_BUF_BYTES = 64 * 128;
+  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = EPI_OFFSET + 2 /*warpgroups*/ * 2 /*buffers*/ * EPI_BUF_BYTES;
   // full[STAGES], empty[STAGES]
   static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024 /*align slack*/;
   static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
@@ -86,9 +98,28 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   n_idx = in_g / gsize;
 }
 
+// K range of a tile: the whole K, or for a K-split GEMM (p.ksplits > 1, batch index = split) the split's share of whole
+// k-blocks, [s * nkb / S, (s + 1) * nkb / S). `ab` is the operands' batch coordinate.
+__device__ __forceinline__ void k_range(const GemmParams& p, int b, int num_kb, int& kb_lo, int& kb_hi, int& ab) {
+  if (p.ksplits > 1) {
+    kb_lo = int(int64_t(b) * num_kb / p.ksplits);
+    kb_hi = int(int64_t(b + 1) * num_kb / p.ksplits);
+    ab = 0;
+  } else {
+    kb_lo = 0; kb_hi = num_kb; ab = b;
+  }
+}
+
+// Position of element (row, byte) of a 64-row x 128-byte sub-tile in the 128B-swizzled staging layout the D / aux tensor maps
+// declare: the 16-byte unit index is XORed with row % 8. A warp's 8 rows x 4 lanes then hit 32 distinct banks.
+__device__ __forceinline__ uint32_t epi_swz(int row, int byte) {
+  return uint32_t(row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15));
+}
+
 template <int kLayout, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
   constexpr bool A_MN = (kLayout == FSB_GEMM_TN);
   constexpr bool B_MN = (kLayout != FSB_GEMM_NT);
   using S = GemmSmem<BN>;
@@ -113,6 +144,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
     fence_barrier_init();
   }
+  if (threadIdx.x == 128) {
+    tma_prefetch_desc(&tmD);
+    if (p.aux != nullptr) tma_prefetch_desc(&tmAux);
+  }
   __syncthreads();
 
   if (warp < 4) {
@@ -130,28 +165,29 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         else tma_load_3d(dst, tm, bar, c0, c1, c2);
       };
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int b, m_idx, n_idx;
+        int b, m_idx, n_idx, kb_lo, kb_hi, ab;
         tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
+        k_range(p, b, num_kb, kb_lo, kb_hi, ab);
         const int m0 = m_idx * GEMM_BM, n0 = n_idx * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int kb = kb_lo; kb < kb_hi; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * S::STAGE_BYTES;
           uint8_t* sb = sa + S::A_BYTES;
           mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES);
           const int k0 = kb * GEMM_BK;
           if constexpr (!A_MN) {
-            load(sa, &tmA, &full_bar[stage], k0, m0, b, pol_a);
+            load(sa, &tmA, &full_bar[stage], k0, m0, ab, pol_a);
           } else {
 #pragma unroll
             for (int c = 0; c < GEMM_BM / 64; ++c)
-              load(sa + c * (GEMM_BK * 128), &tmA, &full_bar[stage], m0 + c * 64, k0, b, pol_a);
+              load(sa + c * (GEMM_BK * 128), &tmA, &full_bar[stage], m0 + c * 64, k0, ab, pol_a);
           }
           if constexpr (!B_MN) {
-            load(sb, &tmB, &full_bar[stage], k0, n0, b, pol_b);
+            load(sb, &tmB, &full_bar[stage], k0, n0, ab, pol_b);
           } else {
 #pragma unroll
             for (int c = 0; c < BN / 64; ++c)
-              load(sb + c * (GEMM_BK * 128), &tmB, &full_bar[stage], n0 + c * 64, k0, b, pol_b);
+              load(sb + c * (GEMM_BK * 128), &tmB, &full_bar[stage], n0 + c * 64, k0, ab, pol_b);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -162,31 +198,36 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     reg_inc<232>();  // 256 * 232 + 128 * 40 = 64512
     const int wg = (threadIdx.x >> 7) - 1;
     const int wl = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;   // issues this warpgroup's TMA stores and waits on them
     // A: K-major -> the warpgroup's 64 rows start 64 * 128 B into the stage; MN-major -> its own 64-wide m chunk
     const uint64_t dsc_a = A_MN ? make_smem_desc_sw128(smem_u32(smem) + wg * (GEMM_BK * 128), GEMM_BK * 128, 1024)
                                 : make_smem_desc_sw128(smem_u32(smem) + wg * (64 * 128), 0, 1024);
     const uint64_t dsc_b = B_MN ? make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, GEMM_BK * 128, 1024)
                                 : make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, 0, 1024);
+    uint8_t* const epi_buf = smem + S::EPI_OFFSET + wg * (2 * S::EPI_BUF_BYTES);
+    uint32_t n_stored = 0;   // sub-tiles this warpgroup has handed to the TMA unit (selects the staging buffer)
     float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int b, m_idx, n_idx;
+      int b, m_idx, n_idx, kb_lo, kb_hi, ab;
       tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
+      k_range(p, b, num_kb, kb_lo, kb_hi, ab);
       int prev = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      for (int kb = kb_lo; kb < kb_hi; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint64_t so = uint64_t(stage) * (S::STAGE_BYTES >> 4);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GEMM_BK / 16; ++k) {
           const uint64_t da = dsc_a + so + ((A_MN ? k * 2048 : k * 32) >> 4), db = dsc_b + so + ((B_MN ? k * 2048 : k * 32) >> 4);
-          if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
-          else wgmma_ss_n128<A_MN, B_MN>(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+          const uint32_t accum = (kb != kb_lo || k != 0) ? 1u : 0u;
+          if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc, da, db, accum);
+          else wgmma_ss_n128<A_MN, B_MN>(acc, da, db, accum);
         }
         wgmma_commit();
         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage can be refilled
-        if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (kb > kb_lo && lane == 0) mbar_arrive(&empty_bar[prev]);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
@@ -194,61 +235,111 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_fence_acc(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      // ---- epilogue from registers: accumulator j covers columns 8 (j / 4) + 2 (lane % 4) + (j & 1), rows r and r + 8
-      const int row0 = m_idx * GEMM_BM + wg * 64 + wl * 16 + (lane >> 2);
-      const int colq = n_idx * BN + 2 * (lane & 3);
-      const int64_t d_off = int64_t(b) * p.stride_d, aux_off = int64_t(b) * p.stride_aux;
+      // ---- epilogue: accumulator j covers columns 8 (j / 4) + 2 (lane % 4) + (j & 1), rows r and r + 8 (r = 16 wl + lane / 4)
+      const int r = wl * 16 + (lane >> 2);
+      const int m0 = m_idx * GEMM_BM + wg * 64, n0 = n_idx * BN;
+      const int64_t d_off = int64_t(b) * p.stride_d;
+      // One 64-row x 128-byte sub-tile: wait until the store that last used this buffer has read it, fill it, make the
+      // writes visible to the async proxy, and hand it to the TMA unit. The consumer never waits for a store to land.
+      auto stage_out = [&](const CUtensorMap* tm, int c0, auto&& fill) {
+        uint8_t* buf = epi_buf + (n_stored & 1) * S::EPI_BUF_BYTES;
+        if (leader) tma_store_wait_read<1>();
+        bar_sync(1 + wg, 128);
+        fill(buf);
+        fence_proxy_async();
+        bar_sync(1 + wg, 128);
+        if (leader) {
+          tma_store_3d(tm, buf, c0, m0, b);
+          tma_store_commit();
+        }
+        ++n_stored;
+      };
+      // bias (0 without one: the add is kept so that results do not depend on whether a bias was passed)
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
-        const int col = colq + 8 * j;
-        if (col >= p.N) continue;
-        const bool two = col + 1 < p.N;
+        const int col = n0 + 8 * j + 2 * (lane & 3);
         float bv0 = 0.f, bv1 = 0.f;
         if (p.bias != nullptr) {
           if (p.bias_f32) {
-            bv0 = __ldg(reinterpret_cast<const float*>(p.bias) + col);
-            if (two) bv1 = __ldg(reinterpret_cast<const float*>(p.bias) + col + 1);
+            if (col < p.N) bv0 = __ldg(reinterpret_cast<const float*>(p.bias) + col);
+            if (col + 1 < p.N) bv1 = __ldg(reinterpret_cast<const float*>(p.bias) + col + 1);
           } else {
-            bv0 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col));
-            if (two) bv1 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col + 1));
+            if (col < p.N) bv0 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col));
+            if (col + 1 < p.N) bv1 = __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col + 1));
           }
         }
+        acc[4 * j] += bv0; acc[4 * j + 1] += bv1; acc[4 * j + 2] += bv0; acc[4 * j + 3] += bv1;
+      }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
-          if (row >= p.M) continue;
-          float v0 = acc[4 * j + 2 * h] + bv0, v1 = acc[4 * j + 2 * h + 1] + bv1;
-          if (p.aux != nullptr) {   // pre-activation copy (bf16)
-            __nv_bfloat16* ap = reinterpret_cast<__nv_bfloat16*>(p.aux) + aux_off + int64_t(row) * p.ldaux + col;
-            if (two) *reinterpret_cast<uint32_t*>(ap) = pack_bf16x2(v0, v1);
-            else *ap = __float2bfloat16(v0);
-          }
-          if (p.epilogue == FSB_EPI_GELU_TANH) { v0 = gelu_tanh_f(v0); v1 = gelu_tanh_f(v1); }
-          else if (p.epilogue == FSB_EPI_GELU_ERF) { v0 = gelu_erf_f(v0); v1 = gelu_erf_f(v1); }
-          if (p.d_f32) {
-            float* dp = reinterpret_cast<float*>(p.D) + d_off + int64_t(row) * p.ldd + col;
-            if (two) {
-              float2 q = make_float2(v0, v1);
-              if (p.accumulate) { const float2 o = *reinterpret_cast<const float2*>(dp); q.x += o.x; q.y += o.y; }
-              *reinterpret_cast<float2*>(dp) = q;
-            } else {
-              *dp = p.accumulate ? *dp + v0 : v0;
-            }
-          } else {
-            __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D) + d_off + int64_t(row) * p.ldd + col;
-            if (two) {
-              if (p.accumulate) {
-                const uint32_t o = *reinterpret_cast<const uint32_t*>(dp);
-                v0 += bf16lo(o); v1 += bf16hi(o);
+      for (int g = 0; g < BN / 64; ++g) {   // 64 columns = accumulators j in [8 g, 8 g + 8)
+        if (p.aux != nullptr) {   // pre-activation copy (bf16)
+          stage_out(&tmAux, n0 + 64 * g, [&](uint8_t* buf) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int j = 8 * g + jj;
+                *reinterpret_cast<uint32_t*>(buf + epi_swz(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                    pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
               }
-              *reinterpret_cast<uint32_t*>(dp) = pack_bf16x2(v0, v1);
-            } else {
-              *dp = __float2bfloat16(p.accumulate ? __bfloat162float(*dp) + v0 : v0);
+          });
+        }
+#pragma unroll
+        for (int i = 32 * g; i < 32 * g + 32; ++i) {
+          if (p.epilogue == FSB_EPI_GELU_TANH) acc[i] = gelu_tanh_f(acc[i]);
+          else if (p.epilogue == FSB_EPI_GELU_ERF) acc[i] = gelu_erf_f(acc[i]);
+        }
+        if (p.accumulate) {   // D += result: fp32 sum with the old value, rounded once
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * g + jj;
+            const int col = n0 + 8 * j + 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = m0 + r + 8 * h;
+              if (row >= p.M || col >= p.N) continue;
+              const bool two = col + 1 < p.N;
+              const int64_t o = d_off + int64_t(row) * p.ldd + col;
+              if (p.d_f32) {
+                const float* dp = reinterpret_cast<const float*>(p.D) + o;
+                if (two) { const float2 q = *reinterpret_cast<const float2*>(dp); acc[4 * j + 2 * h] += q.x; acc[4 * j + 2 * h + 1] += q.y; }
+                else acc[4 * j + 2 * h] += *dp;
+              } else {
+                const __nv_bfloat16* dp = reinterpret_cast<const __nv_bfloat16*>(p.D) + o;
+                if (two) { const uint32_t q = *reinterpret_cast<const uint32_t*>(dp); acc[4 * j + 2 * h] += bf16lo(q); acc[4 * j + 2 * h + 1] += bf16hi(q); }
+                else acc[4 * j + 2 * h] += __bfloat162float(*dp);
+              }
             }
           }
+        }
+        if (p.d_f32) {   // two 32-column sub-tiles
+#pragma unroll
+          for (int q = 0; q < 2; ++q)
+            stage_out(&tmD, n0 + 64 * g + 32 * q, [&](uint8_t* buf) {
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int j = 8 * g + 4 * q + jj;
+                  *reinterpret_cast<float2*>(buf + epi_swz(r + 8 * h, 32 * jj + 8 * (lane & 3))) =
+                      make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                }
+            });
+        } else {
+          stage_out(&tmD, n0 + 64 * g, [&](uint8_t* buf) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int j = 8 * g + jj;
+                *reinterpret_cast<uint32_t*>(buf + epi_swz(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                    pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+              }
+          });
         }
       }
     }
+    if (leader) tma_store_wait<0>();   // every store has completed before the CTA (and its shared memory) goes away
   }
 }
 
@@ -261,7 +352,8 @@ static inline int gemm_sms() {
 }
 
 template <int kLayout, int BN>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmAux,
+                       const GemmParams& p, cudaStream_t stream) {
   using S = GemmSmem<BN>;
   static bool configured = false;
   auto kern = gemm_bf16_kernel<kLayout, BN>;
@@ -275,9 +367,30 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   }
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
   const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
-  kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, p);
+  kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
+}
+
+// Tile width and K-split count. 128 x 256 tiles unless they would leave a large part of the SMs idle (weight-gradient GEMMs
+// of small models: e.g. 768 x 2304 x 32768 is only 54 such tiles) — then 128 x 128 tiles double the parallelism.
+// Plain, unbatched TN GEMMs (weight gradients) whose output has too few tiles to occupy the SMs (e.g. 768 x 768 x 32768:
+// 18 tiles) split K instead: `splits` equal chunks of whole k-blocks, each >= 1024 deep, run as tiles of one launch into an
+// fp32 scratch and are summed in split order (deterministic). Outputs narrower than 256 keep 128 x 128 tiles.
+struct GemmPlan {
+  int bn, splits;
+};
+static GemmPlan gemm_plan(int layout, int64_t M, int64_t N, int64_t K, int64_t batch, bool plain, int sms) {
+  const int64_t tiles256 = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + 255) / 256) * batch;
+  const int bn = (N > 128 && tiles256 * 10 >= int64_t(sms) * 7) ? 256 : 128;
+  if (!(layout == FSB_GEMM_TN && batch == 1 && plain && N % 4 == 0 && (M * N) % 8 == 0 && K >= 4096)) return {bn, 1};
+  const bool wide = N >= 256;
+  const int64_t tiles = ((M + GEMM_BM - 1) / GEMM_BM) * (wide ? (N + 255) / 256 : (N + 127) / 128);
+  int splits = int(sms / tiles);
+  if (splits > 16) splits = 16;
+  while (splits > 1 && (K % (int64_t(splits) * GEMM_BK) != 0 || K / splits < 1024)) --splits;
+  if (splits >= 2 && tiles * 2 <= sms) return {wide ? 256 : bn, splits};
+  return {bn, 1};
 }
 
 // D (bf16 / fp32, optionally accumulated into) = sum over the K-splits of the fp32 partial products, in a fixed order
@@ -309,7 +422,8 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
 static int gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                      int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_wide = false);
+                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, int bn = 0,
+                     int ksplits = 1);
 
 }  // namespace fsb
 
@@ -321,25 +435,10 @@ extern "C" int fsb_set_reserved_sms(int n) {
   return FSB_OK;
 }
 
-// Split-K plan for weight-gradient GEMMs whose output has too few tiles to occupy the SMs (e.g. 768 x 768 x 32768: 18
-// tiles): `splits` K-chunks run as a batched GEMM into an fp32 scratch and are summed in a fixed order (deterministic).
-// Preferred: 128 x 256 tiles (twice the operand reuse of 128 x 128), K split so that the SMs are busy; outputs narrower than
-// 256 keep 128 x 128 tiles. Returns 0 / 1 when the call does not split.
-static int splitk_plan(int layout, int64_t M, int64_t N, int64_t K, int64_t batch, bool plain, bool* wide_out) {
-  if (!(layout == FSB_GEMM_TN && batch == 1 && plain && M > 0 && N > 0 && N % 4 == 0 && (M * N) % 8 == 0 && K >= 4096)) return 0;
-  const bool wide = N >= 256;
-  const int64_t tiles = ((M + GEMM_BM - 1) / GEMM_BM) * (wide ? (N + 255) / 256 : (N + 127) / 128);
-  const int64_t slots = num_sms();
-  int splits = int(slots / tiles);
-  if (splits > 16) splits = 16;
-  while (splits > 1 && (K % (int64_t(splits) * GEMM_BK) != 0 || K / splits < 1024)) --splits;
-  if (wide_out) *wide_out = wide;
-  return (splits >= 2 && tiles * 2 <= slots) ? splits : 0;
-}
-
 extern "C" size_t fsb_gemm_workspace_bytes(int layout, int64_t M, int64_t N, int64_t K) {
-  const int splits = splitk_plan(layout, M, N, K, 1, true, nullptr);
-  return splits ? size_t(splits) * size_t(M) * size_t(N) * sizeof(float) : 0;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  const int splits = gemm_plan(layout, M, N, K, 1, true, gemm_sms()).splits;
+  return splits > 1 ? size_t(splits) * size_t(M) * size_t(N) * sizeof(float) : 0;
 }
 
 extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
@@ -348,40 +447,40 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
                              int64_t stride_b, int64_t stride_d, int64_t stride_aux, void* workspace,
                              size_t workspace_bytes, fsb_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  bool wide = false;
-  const int splits = (d_dtype == FSB_BF16 || d_dtype == FSB_F32)
-                         ? splitk_plan(layout, M, N, K, batch, bias == nullptr && aux == nullptr && epilogue == FSB_EPI_NONE, &wide)
-                         : 0;
-  if (splits >= 2) {
+  FSB_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, "gemm: non-positive dims M=%ld N=%ld K=%ld batch=%ld", (long)M,
+              (long)N, (long)K, (long)batch);
+  const GemmPlan plan = gemm_plan(layout, M, N, K, batch, bias == nullptr && aux == nullptr && epilogue == FSB_EPI_NONE,
+                                  gemm_sms());
+  if (plan.splits > 1 && (d_dtype == FSB_BF16 || d_dtype == FSB_F32)) {
     // the scratch is the caller's (fsb_gemm_workspace_bytes): the library allocates nothing. Too small a workspace is an
     // error, not a silent change of algorithm (results would still be correct, but run-to-run timing / rounding would not be
     // what the same call gives with the workspace present).
+    const int splits = plan.splits;
     const size_t need = size_t(splits) * size_t(M) * size_t(N) * sizeof(float);
     FSB_REQUIRE(workspace != nullptr && workspace_bytes >= need && aligned16(workspace),
                 "gemm: this TN call splits K %d ways and needs a %zu-byte workspace (fsb_gemm_workspace_bytes); got %zu",
                 splits, need, workspace_bytes);
-    {
-      float* ws = static_cast<float*>(workspace);
-      const int64_t kc = K / splits;
-      int rc = gemm_impl(layout, M, N, kc, A, lda, B, ldb, ws, N, FSB_F32, nullptr, FSB_BF16, FSB_EPI_NONE, 0, nullptr, 0,
-                         splits, kc * lda, kc * ldb, M * N, 0, stream, wide);
-      if (rc) return rc;
-      FSB_REQUIRE(ldd % 4 == 0, "gemm: ldd=%ld not vector-aligned", (long)ldd);
-      const int64_t work = M * (N / 4);
-      const int blocks = int(work / 256 + 1 < 2 * num_sms() ? work / 256 + 1 : 2 * num_sms());
-      splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(ws, splits, M, N, D, ldd, d_dtype == FSB_F32, accumulate);
-      FSB_CUDA_LAUNCH_CHECK();
-      return FSB_OK;
-    }
+    FSB_REQUIRE(ldd % 4 == 0, "gemm: ldd=%ld not vector-aligned", (long)ldd);
+    float* ws = static_cast<float*>(workspace);
+    // split s: k-blocks k_range(s) of the whole (unbatched) A / B -> fp32 partial ws[s] (M x N, ld N)
+    int rc = gemm_impl(layout, M, N, K, A, lda, B, ldb, ws, N, FSB_F32, nullptr, FSB_BF16, FSB_EPI_NONE, 0, nullptr, 0,
+                       splits, 0, 0, M * N, 0, stream, plan.bn, splits);
+    if (rc) return rc;
+    const int64_t work = M * (N / 4);
+    const int blocks = int(work / 256 + 1 < 2 * num_sms() ? work / 256 + 1 : 2 * num_sms());
+    splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(ws, splits, M, N, D, ldd, d_dtype == FSB_F32, accumulate);
+    FSB_CUDA_LAUNCH_CHECK();
+    return FSB_OK;
   }
   return gemm_impl(layout, M, N, K, A, lda, B, ldb, D, ldd, d_dtype, bias, bias_dtype, epilogue, accumulate, aux, ldaux, batch,
-                   stride_a, stride_b, stride_d, stride_aux, stream);
+                   stride_a, stride_b, stride_d, stride_aux, stream, plan.bn, 1);
 }
 
 static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                           int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                           int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, bool force_wide) {
+                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, int bn,
+                          int ksplits) {
   FSB_REQUIRE(layout >= 0 && layout <= 2, "gemm: bad layout %d", layout);
   FSB_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, "gemm: non-positive dims M=%ld N=%ld K=%ld batch=%ld", (long)M,
               (long)N, (long)K, (long)batch);
@@ -396,28 +495,46 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   FSB_REQUIRE(aux == nullptr || (aligned16(aux) && ldaux % 8 == 0), "gemm: aux misaligned");
   FSB_REQUIRE(batch == 1 || (stride_a % 8 == 0 && stride_b % 8 == 0 && stride_d % 8 == 0),
               "gemm: batch strides must be multiples of 8");
+  FSB_REQUIRE(aux == nullptr || batch == 1 || stride_aux % 8 == 0, "gemm: aux batch stride must be a multiple of 8");
+  FSB_REQUIRE(ksplits == 1 || (ksplits > 1 && ksplits <= (K + GEMM_BK - 1) / GEMM_BK && ksplits == batch),
+              "gemm: bad K-split count %d", ksplits);
 
-  // Tensor maps: always rank 3 (inner, outer, batch).
-  CUtensorMap tmA, tmB;
+  // Tensor maps: always rank 3 (inner, outer, batch). A K-split GEMM reads unbatched operands and writes D[split].
+  CUtensorMap tmA, tmB, tmD, tmAux;
   const bool a_mn = (layout == FSB_GEMM_TN), b_mn = (layout != FSB_GEMM_NT);
-  // 128 x 256 tiles unless they would leave a large part of the SMs idle (weight-gradient GEMMs of small models:
-  // e.g. 768 x 2304 x 32768 is only 54 such tiles) — then 128 x 128 tiles double the parallelism.
-  const int64_t tiles256 = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + 255) / 256) * batch;
-  const int BN = (force_wide || (N > 128 && tiles256 * 10 >= int64_t(num_sms()) * 7)) ? 256 : 128;
+  const int BN = bn ? bn : gemm_plan(layout, M, N, K, batch, false, gemm_sms()).bn;
+  const int64_t ab = ksplits > 1 ? 1 : batch;
   {
     // A: K-major -> memory [M rows, K inner]; MN-major -> memory [K rows, M inner]
-    uint64_t dims[3] = {uint64_t(a_mn ? M : K), uint64_t(a_mn ? K : M), uint64_t(batch)};
-    uint64_t strides[2] = {uint64_t(lda) * 2, uint64_t(batch > 1 ? stride_a : (a_mn ? K : M) * lda) * 2};
+    uint64_t dims[3] = {uint64_t(a_mn ? M : K), uint64_t(a_mn ? K : M), uint64_t(ab)};
+    uint64_t strides[2] = {uint64_t(lda) * 2, uint64_t(ab > 1 ? stride_a : (a_mn ? K : M) * lda) * 2};
     uint32_t box[3] = {64, uint32_t(a_mn ? GEMM_BK : GEMM_BM), 1};
     int rc = make_tmap_bf16(&tmA, A, 3, dims, strides, box);
     if (rc) return rc;
   }
   {
-    uint64_t dims[3] = {uint64_t(b_mn ? N : K), uint64_t(b_mn ? K : N), uint64_t(batch)};
-    uint64_t strides[2] = {uint64_t(ldb) * 2, uint64_t(batch > 1 ? stride_b : (b_mn ? K : N) * ldb) * 2};
+    uint64_t dims[3] = {uint64_t(b_mn ? N : K), uint64_t(b_mn ? K : N), uint64_t(ab)};
+    uint64_t strides[2] = {uint64_t(ldb) * 2, uint64_t(ab > 1 ? stride_b : (b_mn ? K : N) * ldb) * 2};
     uint32_t box[3] = {64, uint32_t(b_mn ? GEMM_BK : BN), 1};
     int rc = make_tmap_bf16(&tmB, B, 3, dims, strides, box);
     if (rc) return rc;
+  }
+  {
+    // D / aux: [M rows, N inner], stored as 64-row x 128-byte boxes (64 bf16 or 32 fp32 columns); the map clips ragged edges
+    const int64_t es = d_dtype == FSB_F32 ? 4 : 2;
+    uint64_t dims[3] = {uint64_t(N), uint64_t(M), uint64_t(batch)};
+    uint64_t strides[2] = {uint64_t(ldd * es), uint64_t((batch > 1 ? stride_d : M * ldd) * es)};
+    uint32_t box[3] = {uint32_t(128 / es), 64, 1};
+    int rc = d_dtype == FSB_F32 ? make_tmap_f32(&tmD, D, 3, dims, strides, box) : make_tmap_bf16(&tmD, D, 3, dims, strides, box);
+    if (rc) return rc;
+    if (aux != nullptr) {
+      uint64_t astrides[2] = {uint64_t(ldaux * 2), uint64_t((batch > 1 ? stride_aux : M * ldaux) * 2)};
+      uint32_t abox[3] = {64, 64, 1};
+      rc = make_tmap_bf16(&tmAux, aux, 3, dims, astrides, abox);
+      if (rc) return rc;
+    } else {
+      tmAux = tmD;   // never read
+    }
   }
   GemmParams p;
   p.D = D; p.aux = aux; p.bias = bias;
@@ -425,6 +542,7 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   p.M = int(M); p.N = int(N); p.K = int(K); p.batch = int(batch);
   p.d_f32 = (d_dtype == FSB_F32); p.bias_f32 = (bias_dtype == FSB_F32);
   p.epilogue = epilogue; p.accumulate = accumulate;
+  p.ksplits = ksplits;
   static const int l2hint_env = [] { const char* e = getenv("FSB_GEMM_L2HINT"); return e ? atoi(e) : 0; }();
   p.l2_hints = l2hint_env;
   p.tiles_m = int((M + GEMM_BM - 1) / GEMM_BM);
@@ -434,7 +552,7 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   // 16 for 256-wide tiles, 12 for 128-wide ones); the group only grows beyond that while its A panels (group_m x 128 x K bf16)
   // stay well inside the L2 (~32 MB of its 50 MB).
   {
-    const int64_t a_panel = int64_t(GEMM_BM) * K * 2;
+    const int64_t a_panel = int64_t(GEMM_BM) * (K / ksplits) * 2;
     const int64_t base = BN == 256 ? 16 : 12;
     int64_t gm = (int64_t(32) << 20) / a_panel;
     gm = gm < base ? base : (gm > 64 ? 64 : gm);
@@ -443,7 +561,7 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
 
 #define FSB_GEMM_DISPATCH(L) \
   case L:                    \
-    return BN == 256 ? launch_gemm<L, 256>(tmA, tmB, p, stream) : launch_gemm<L, 128>(tmA, tmB, p, stream);
+    return BN == 256 ? launch_gemm<L, 256>(tmA, tmB, tmD, tmAux, p, stream) : launch_gemm<L, 128>(tmA, tmB, tmD, tmAux, p, stream);
   switch (layout) {
     FSB_GEMM_DISPATCH(FSB_GEMM_NT)
     FSB_GEMM_DISPATCH(FSB_GEMM_NN)

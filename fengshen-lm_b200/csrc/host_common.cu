@@ -47,13 +47,14 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// A tensor map is a pure function of (base, rank, dims, strides, box) — element type, swizzle, interleave, L2 promotion and
+// A tensor map is a pure function of (element type, base, rank, dims, strides, box) — swizzle, interleave, L2 promotion and
 // out-of-bounds fill are fixed below — and a training step presents the same few hundred operands every iteration (flat parameter
 // views, activation buffers the caching allocator hands back at the same addresses). The driver's encode call is memoised in a
 // per-thread direct-mapped table: a hit copies 128 bytes. FSB_TMAP_CACHE=0 disables it (A/B measurements).
 namespace {
 struct TmapKey {
   const void* base;
+  int32_t dtype;
   uint64_t dims[5];
   uint64_t strides[4];
   uint32_t box[5];
@@ -64,7 +65,7 @@ struct TmapSlot {
   CUtensorMap map;
   bool valid;
 };
-constexpr int kTmapSlots = 1024;   // power of two; ~210 KB per calling thread
+constexpr int kTmapSlots = 2048;   // power of two; ~0.6 MB per calling thread (a GEMM encodes four maps: A, B, D, aux)
 thread_local TmapSlot* t_tmap_cache = nullptr;
 
 bool tmap_cache_enabled() {
@@ -82,17 +83,17 @@ uint32_t tmap_hash(const TmapKey& k) {
   for (int i = 0; i < 5; ++i) mix(k.dims[i]);
   for (int i = 0; i < 4; ++i) mix(k.strides[i]);
   for (int i = 0; i < 5; ++i) mix(k.box[i]);
-  mix(static_cast<uint64_t>(k.rank));
+  mix(static_cast<uint64_t>(k.rank) | (static_cast<uint64_t>(k.dtype) << 8));
   return static_cast<uint32_t>(h ^ (h >> 32)) & (kTmapSlots - 1);
 }
 }  // namespace
 
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box) {
+static int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return FSB_ERR_CUDA;
   if (rank < 1 || rank > 5) {
-    set_error("make_tmap_bf16: rank %d outside 1..5", rank);
+    set_error("make_tmap: rank %d outside 1..5", rank);
     return FSB_ERR_INVALID;
   }
   TmapSlot* slot = nullptr;
@@ -100,6 +101,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   if (tmap_cache_enabled()) {
     memset(&key, 0, sizeof(key));
     key.base = base;
+    key.dtype = int32_t(dtype);
     key.rank = rank;
     for (int i = 0; i < rank; ++i) { key.dims[i] = dims[i]; key.box[i] = box[i]; }
     for (int i = 0; i + 1 < rank; ++i) key.strides[i] = strides_bytes[i];
@@ -122,7 +124,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
     estr[i] = 1;
   }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
+  CUresult r = fn(out, dtype, rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -138,6 +140,15 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
     slot->valid = true;
   }
   return FSB_OK;
+}
+
+int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                   const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box);
+}
+int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                  const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box);
 }
 
 }  // namespace fsb

@@ -32,10 +32,12 @@ void set_error(const char* fmt, ...);
 
 int num_sms();
 
-// 2-D / 3-D bf16 tensor map with 128B swizzle. dims/box innermost-first; strides (bytes) for dims 1.. .
+// 2-D / 3-D bf16 / fp32 tensor map with 128B swizzle. dims/box innermost-first; strides (bytes) for dims 1.. .
 // Returns 0 on success (error string set otherwise).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box);
+int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                  const uint32_t* box);
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

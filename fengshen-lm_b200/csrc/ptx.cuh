@@ -116,6 +116,10 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+template <int N>
+__device__ __forceinline__ void tma_store_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
 
 // ----------------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA, sm_90a): D[regs] (+)= A[smem desc | regs] * B[smem desc], issued by all 128 threads of a warpgroup
