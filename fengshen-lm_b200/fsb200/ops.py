@@ -77,10 +77,8 @@ def gemm(layout, a, b, out=None, out_dtype=_bf16, bias=None, epilogue=L.EPI_NONE
         _, _, ldaux = _rows2d(aux, "aux")
     ws, ws_bytes = None, 0
     if layout == L.GEMM_TN and bias is None and aux is None and epilogue == L.EPI_NONE:
-        key = (M, N, K)
-        ws_bytes = _splitk_bytes.get(key)
-        if ws_bytes is None:
-            ws_bytes = _splitk_bytes[key] = int(L.load().fsb_gemm_workspace_bytes(layout, M, N, K))
+        # asked on every call, not memoised per shape: the split plan follows fsb_set_reserved_sms
+        ws_bytes = int(L.load().fsb_gemm_workspace_bytes(layout, M, N, K))
         if ws_bytes:
             ws = workspace(ws_bytes, a.device, "gemm_splitk")   # one stream issues the step's GEMMs: a shared scratch is safe
     prof = _profiler
@@ -96,9 +94,6 @@ def gemm(layout, a, b, out=None, out_dtype=_bf16, bias=None, epilogue=L.EPI_NONE
         ev1 = torch.cuda.Event(enable_timing=True); ev1.record()
         prof.add("gemm_bf16_kernel", ev0, ev1, 2.0 * M * N * K)
     return out
-
-
-_splitk_bytes = {}
 
 
 def set_reserved_sms(n):
