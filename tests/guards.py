@@ -2,6 +2,7 @@
 
 A kernel under test writes into a view of a larger allocation. Everything outside the view is a guard: the test checks
 that the kernel wrote every element of the view (no NaN sentinel left) and that no guard element changed (bit equality).
+Also the bf16-ulp comparison for kernels that round their fp32 result to bf16 once.
 """
 import torch
 
@@ -53,3 +54,23 @@ def guarded_1d(n, dtype, fill=float("nan"), init=None, pad=8, device="cuda"):
     if init is not None:
         sel(buf).copy_(init)
     return Guarded(buf, sel)
+
+
+def bf16_ulp(ref):
+    """Spacing of bf16 numbers at |ref| (8 significant bits); the smallest normal spacing below 2^-126."""
+    _, e = torch.frexp(ref.double().abs().clamp_min(2.0 ** -126))
+    return torch.ldexp(torch.ones_like(ref, dtype=torch.float64), e - 8)
+
+
+def assert_ulp_close(got, ref, what="", ulps=1.0, floor=0.0):
+    """|got - ref| <= ulps * bf16_ulp(ref) + floor elementwise, ref in fp64. floor: a number or a tensor that broadcasts
+    against ref (an absolute allowance for fp32 cancellation, stated by the caller). NaN in got fails."""
+    ref = ref.double()
+    err = (got.double() - ref).abs()
+    tol = ulps * bf16_ulp(ref) + floor
+    bad = ~(err <= tol)
+    if bad.any():
+        i = int(bad.reshape(-1).nonzero()[0])
+        raise AssertionError(f"{what}: {int(bad.sum())}/{bad.numel()} elements beyond {ulps} bf16 ulp + floor; first at "
+                             f"flat index {i}: got {got.reshape(-1)[i].item():.6g}, want {ref.reshape(-1)[i].item():.6g}; "
+                             f"max err {err.max().item():.4g}")

@@ -55,8 +55,11 @@ def test_wenzhong_recipe_host_flow(launched_with_doubles, tmp_path):
 def _rank_main(rank, world, port, workdir, q):
     import json
     import runpy
+    # both ranks run on the CPU over gloo; hidden GPUs keep the trainer from picking NCCL and cuda:<rank> on a host with
+    # fewer GPUs than ranks
     os.environ.update(RANK=str(rank), LOCAL_RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1",
-                      MASTER_PORT=str(port), PL_DEEPSPEED_CONFIG_PATH=os.path.join(workdir, "ds_config.json"))
+                      MASTER_PORT=str(port), PL_DEEPSPEED_CONFIG_PATH=os.path.join(workdir, "ds_config.json"),
+                      CUDA_VISIBLE_DEVICES="")
     sys.path.insert(0, os.path.join(F.ROOT, "tests"))
     sys.path.insert(0, os.path.join(F.ROOT, "fengshen-lm_b200"))
     import torch
