@@ -82,7 +82,7 @@ class UniversalDataModule(LightningDataModule):
     def setup(self, stage=None):
         return
 
-    def _loader(self, ds, batch_size, custom_sampler):
+    def _loader(self, ds, batch_size, custom_sampler, data_parallel=False):
         collate_fn = getattr(ds, 'collate_fn', self.collate_fn)
         workers = getattr(self.hparams, 'dataloader_workers', 0)
         if custom_sampler:
@@ -90,8 +90,11 @@ class UniversalDataModule(LightningDataModule):
                               pin_memory=True)
         sampler = None
         if self.trainer is not None and self.trainer.world_size > 1:
-            sampler = DistributedSampler(ds, num_replicas=self.trainer.world_size, rank=self.trainer.global_rank,
-                                         shuffle=False)
+            # data_parallel: shard over the data-parallel group, so that the ranks of one tensor-parallel group read the same
+            # batch (without tensor parallelism that group is the whole world)
+            rank = mpu.get_data_parallel_rank() if data_parallel else self.trainer.global_rank
+            size = mpu.get_data_parallel_world_size() if data_parallel else self.trainer.world_size
+            sampler = DistributedSampler(ds, num_replicas=size, rank=rank, shuffle=False)
         return DataLoader(ds, batch_size=batch_size, sampler=sampler, num_workers=workers, collate_fn=collate_fn,
                           pin_memory=True)
 
@@ -101,7 +104,7 @@ class UniversalDataModule(LightningDataModule):
 
     def val_dataloader(self):
         ds = self.datasets[self.hparams.val_datasets_field]
-        return self._loader(ds, self.hparams.val_batchsize, False)
+        return self._loader(ds, self.hparams.val_batchsize, False, data_parallel=True)
 
     def test_dataloader(self):
         ds = self.datasets[self.hparams.test_datasets_field]

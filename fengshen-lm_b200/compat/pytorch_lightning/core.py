@@ -67,6 +67,10 @@ class LightningModule(_HParamsMixin, nn.Module):
 
     # ---- services
     def log(self, name, value, sync_dist=False, **_):
+        if self.trainer is not None and getattr(self.trainer, "_val_acc", None) is not None:
+            # inside a validation run: the run's batch-size-weighted mean, reported when the run ends
+            self.trainer._log_val(name, value, sync_dist, self.device)
+            return
         if isinstance(value, torch.Tensor):
             value = value.detach()
             if sync_dist and self.trainer is not None and self.trainer.world_size > 1:

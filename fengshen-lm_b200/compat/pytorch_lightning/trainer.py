@@ -5,23 +5,66 @@ Surface kept (SURVEY.md §8b): `add_argparse_args`, `from_argparse_args`, `fit`,
 checkpoint_callback, lightning_module, optimizers, callback_metrics`, and the two private paths the reference pokes:
 `_data_connector._train_dataloader_source.dataloader()` (fengshen/models/model_utils.py:195) and
 `fit_loop.epoch_loop._batches_that_stepped` (examples/pretrain_erlangshen_bert/pretrain_erlangshen.py:197).
+
+Validation inside `fit` restates PyTorch-Lightning 1.9 (the names in brackets are PL 1.9's, to check against an install):
+- Enabled (`Trainer.enable_validation`) only when the module overrides `validation_step` (`is_overridden`), a validation
+  loader exists (`datamodule.val_dataloader()` or `fit(val_dataloaders=...)`) and `limit_val_batches` is not 0. Otherwise
+  `fit` runs exactly as without validation, and `val_dataloader()` is never called. An error it raises propagates.
+- Cadence (`Trainer.val_check_batch`, `TrainingEpochLoop._should_check_val_fx`): a float `val_check_interval` f gives
+  `val_check_batch = max(1, int(n_train_batches * f))`, an int N gives N. An int above the epoch's batch count is a
+  `ValueError` unless `check_val_every_n_epoch` is None; a float with `check_val_every_n_epoch=None` is a `ValueError`
+  (PL's "should be an integer"). After training batch i, validation runs when
+  `(i + 1) % val_check_batch == 0`, where i is the batch index within the epoch, or the total batch index across epochs
+  when `check_val_every_n_epoch` is None (`total_batch_idx`). Batches are micro-batches, so a run may fall inside a
+  gradient-accumulation window. Only epochs with `(epoch + 1) % check_val_every_n_epoch == 0` validate
+  (`_should_check_val_epoch`).
+- Limits (`_parse_num_batches`): `limit_val_batches` is a fraction (float) or a count (int) of the loader's batches; a
+  fraction that leaves 0 batches of a non-empty loader is a `ValueError`; an empty loader means no validation. `num_sanity_val_steps` (default 2, -1 = all) batches run once before
+  the first training batch, also on resume (`_run_sanity_check`); their metrics are discarded.
+- Each run: `module.eval()`, `torch.no_grad()`, `validation_step(batch, batch_idx)` with batch_idx counted within the run,
+  then `module.train()`. PL wraps only the sanity pass in `isolate_rng`; here every run is, so that a validation run
+  leaves the training run bit-for-bit unchanged even when a collator draws random numbers.
+- Metrics (`ResultCollection`, `on_epoch=True`, mean reduction): `LightningModule.log` inside a run accumulates the
+  batch-size-weighted mean, the batch size being dim 0 of the batch's first tensor (`extract_batch_size`). `sync_dist=True`
+  makes it the global weighted mean (one all-reduce per metric per run). The result goes to `callback_metrics` and, from
+  rank 0, to the logger once at `step = global_step`; training log lines carry training metrics only.
 """
 import argparse
 import os
+import random
 from types import SimpleNamespace
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
 from .callbacks import ModelCheckpoint
+from .core import LightningModule
 from .strategies import DDPStrategy, DeepSpeedStrategy, strategy_from_string
+
+
+def _int_or_float(x):
+    """PL's `_int_or_float_type` (utilities/argparse.py): '100' is the int 100, '0.1' and '1.0' are floats."""
+    return float(x) if "." in str(x) else int(x)
+
+
+def _batch_limit(v, name):
+    """PL's `_determine_batch_limits`: None -> 1.0; a value in [0, 1] keeps its type; a whole float above 1 becomes an int."""
+    if v is None:
+        return 1.0
+    if 0 <= v <= 1:
+        return v
+    if v > 1 and v % 1.0 == 0:
+        return int(v)
+    raise ValueError(f"{name}={v!r}: expected a float in [0.0, 1.0] or an int >= 0")
+
 
 _ARGS = [  # the PL-1.x Trainer flags that the reference's launch scripts pass (examples/*/*.sh)
     ("--max_epochs", int, None), ("--max_steps", int, -1), ("--gpus", int, None), ("--devices", int, None),
     ("--num_nodes", int, 1), ("--strategy", str, None), ("--precision", str, "32"),
     ("--accumulate_grad_batches", int, 1), ("--gradient_clip_val", float, None), ("--default_root_dir", str, None),
-    ("--val_check_interval", float, None), ("--check_val_every_n_epoch", int, 1), ("--log_every_n_steps", int, 50),
-    ("--limit_val_batches", float, None), ("--num_sanity_val_steps", int, 0), ("--accelerator", str, None),
+    ("--val_check_interval", _int_or_float, None), ("--check_val_every_n_epoch", int, 1), ("--log_every_n_steps", int, 50),
+    ("--limit_val_batches", _int_or_float, None), ("--num_sanity_val_steps", int, 2), ("--accelerator", str, None),
     ("--resume_from_checkpoint", str, None), ("--enable_progress_bar", bool, True), ("--amp_backend", str, None),
     ("--profiler", str, None),
 ]
@@ -49,7 +92,8 @@ class Trainer:
     def __init__(self, max_epochs=None, max_steps=-1, gpus=None, devices=None, num_nodes=1, strategy=None,
                  precision="32", accumulate_grad_batches=1, gradient_clip_val=None, default_root_dir=None,
                  logger=None, callbacks=None, log_every_n_steps=50, replace_sampler_ddp=True,
-                 resume_from_checkpoint=None, **_):
+                 resume_from_checkpoint=None, val_check_interval=None, check_val_every_n_epoch=1,
+                 limit_val_batches=None, num_sanity_val_steps=2, **_):
         self.max_epochs = max_epochs if max_epochs is not None else (1000 if (max_steps or -1) < 0 else -1)
         self.max_steps = max_steps if max_steps is not None else -1
         self.gpus = gpus if gpus is not None else devices
@@ -63,6 +107,15 @@ class Trainer:
         self.log_every_n_steps = log_every_n_steps
         self.replace_sampler_ddp = replace_sampler_ddp
         self.resume_from_checkpoint = resume_from_checkpoint   # PL-1.x flag: same meaning as fit(ckpt_path=...)
+        self.val_check_interval = _batch_limit(val_check_interval, "val_check_interval")
+        self.limit_val_batches = _batch_limit(limit_val_batches, "limit_val_batches")
+        self.check_val_every_n_epoch = check_val_every_n_epoch
+        self.num_sanity_val_steps = int(num_sanity_val_steps)
+        self.val_check_batch = None       # set by fit() when validation is enabled
+        self.sanity_checking = False
+        self._val_acc = None              # name -> [device tensor (sum of v * batch size, sum of batch size), sync_dist]
+        self._val_batch_size = 0
+        self._val_names = set()           # metric names produced by validation, kept out of the training log lines
         if isinstance(strategy, str) or strategy is None:
             strategy = strategy_from_string(strategy)
         self.strategy = strategy
@@ -131,8 +184,122 @@ class Trainer:
                     opts.append(c)
         return opts, scheds
 
+    @staticmethod
+    def _to_device(batch, device):
+        return {k: (v.to(device, non_blocking=True) if isinstance(v, torch.Tensor) else v)
+                for k, v in batch.items()} if isinstance(batch, dict) else batch
+
+    # ---- validation ------------------------------------------------------------------------------------------------
+    def _val_loader(self, model, val_dataloaders):
+        """The validation loader when validation is enabled, else None (`val_dataloader()` is then not called)."""
+        if type(model).validation_step is LightningModule.validation_step or self.limit_val_batches == 0:
+            return None
+        if val_dataloaders is not None:
+            return val_dataloaders
+        return self.datamodule.val_dataloader() if self.datamodule is not None else None
+
+    @staticmethod
+    def _num_batches(loader, limit, name):
+        """PL's `_parse_num_batches`: the loader's batch count under an int (count) or float (fraction) limit."""
+        try:
+            n = len(loader)
+        except TypeError:
+            n = float("inf")
+        if isinstance(limit, int):
+            return min(n, limit)
+        if n == float("inf"):
+            if limit != 1.0:
+                raise ValueError(f"{name}={limit} needs a loader with a length")
+            return n
+        batches = int(n * limit)
+        if batches == 0 and limit > 0.0 and n > 0:
+            raise ValueError(f"{name}={limit} of {n} batches leaves none; use at least {1.0 / n} or an int")
+        return batches
+
+    def _val_check_batch(self, train_loader):
+        try:
+            n_train = len(train_loader)
+        except TypeError:
+            n_train = float("inf")
+        vci = self.val_check_interval
+        if isinstance(vci, int):
+            if vci > n_train and self.check_val_every_n_epoch is not None:
+                raise ValueError(f"val_check_interval ({vci}) must be less than or equal to the number of the training "
+                                 f"batches ({n_train}). To disable validation set limit_val_batches to 0; to validate "
+                                 "every N batches across epochs set check_val_every_n_epoch=None.")
+            return vci
+        if self.check_val_every_n_epoch is None:
+            raise ValueError(f"val_check_interval should be an integer when check_val_every_n_epoch=None, found {vci!r}")
+        if n_train == float("inf"):
+            if vci != 1.0:
+                raise ValueError(f"val_check_interval={vci} needs a training loader with a length")
+            return n_train       # validate once the epoch has ended
+        return max(1, int(n_train * vci))
+
+    def _should_check_val_epoch(self):
+        n = self.check_val_every_n_epoch
+        return n is None or (self.current_epoch + 1) % n == 0
+
+    @staticmethod
+    def _batch_size(batch):
+        """PL's `extract_batch_size`: dim 0 of the first tensor found in the batch."""
+        if isinstance(batch, torch.Tensor):
+            return batch.shape[0] if batch.dim() else 1
+        items = batch.values() if isinstance(batch, dict) else batch if isinstance(batch, (list, tuple)) else ()
+        for v in items:
+            bs = Trainer._batch_size(v)
+            if bs is not None:
+                return bs
+        return None
+
+    def _log_val(self, name, value, sync_dist, device):
+        """LightningModule.log inside a validation run: accumulate (v * batch size, batch size) on the device."""
+        v = value.detach() if isinstance(value, torch.Tensor) else torch.tensor(float(value))
+        v = v.to(device=device, dtype=torch.float64).reshape(())
+        bs = self._val_batch_size
+        entry = self._val_acc.get(name)
+        if entry is None:
+            entry = self._val_acc[name] = [torch.zeros(2, dtype=torch.float64, device=device), bool(sync_dist)]
+        entry[0][0] += v * bs
+        entry[0][1] += bs
+
+    def _run_validation(self, model, loader, n_batches, device, sanity=False):
+        rng = (random.getstate(), np.random.get_state(), torch.get_rng_state(),
+               torch.cuda.get_rng_state_all() if torch.cuda.is_available() and torch.cuda.is_initialized() else None)
+        self.sanity_checking = sanity
+        self._val_acc = {}
+        model.eval()
+        try:
+            with torch.no_grad():
+                for batch_idx, batch in enumerate(loader):
+                    if batch_idx >= n_batches:
+                        break
+                    self._val_batch_size = self._batch_size(batch) or 1
+                    model.validation_step(self._to_device(batch, device), batch_idx)
+            acc, self._val_acc = self._val_acc, None
+            for sums, sync in acc.values():
+                if sync and self.world_size > 1:
+                    dist.all_reduce(sums, op=dist.ReduceOp.SUM)
+            names = list(acc)
+            sums = torch.stack([acc[k][0] for k in names]).tolist() if names else []   # the run's one device->host read
+        finally:
+            self._val_acc = None
+            self.sanity_checking = False
+            model.train()
+            random.setstate(rng[0]); np.random.set_state(rng[1]); torch.set_rng_state(rng[2])
+            if rng[3] is not None:
+                torch.cuda.set_rng_state_all(rng[3])
+        if sanity:
+            return {}
+        metrics = {k: s / max(n, 1) for k, (s, n) in zip(names, sums)}
+        self._val_names.update(metrics)
+        self.callback_metrics.update(metrics)
+        if self.logger is not None and self.global_rank == 0 and metrics:
+            self.logger.log_metrics(metrics, self.global_step)
+        return metrics
+
     # ---- fit -----------------------------------------------------------------------------------------------------
-    def fit(self, model, datamodule=None, ckpt_path=None, train_dataloaders=None):
+    def fit(self, model, datamodule=None, ckpt_path=None, train_dataloaders=None, val_dataloaders=None):
         from fsb200.engine import ZeroEngine
         self.lightning_module, self.datamodule = model, datamodule
         model.trainer = self
@@ -176,6 +343,17 @@ class Trainer:
             cb.on_fit_start(self, model)
         loader = self._train_dl()
         device = fsb_model.flat.params.device
+        val_loader = self._val_loader(model, val_dataloaders)
+        if val_loader is not None:
+            self.val_check_batch = self._val_check_batch(loader)
+            n_val = self._num_batches(val_loader, self.limit_val_batches, "limit_val_batches")
+            if n_val == 0:       # an empty validation loader: no validation (PL's loop skips itself)
+                val_loader = None
+        if val_loader is not None:
+            n_sanity = n_val if self.num_sanity_val_steps == -1 else min(self.num_sanity_val_steps, n_val)
+            if n_sanity > 0:
+                self._run_validation(model, val_loader, n_sanity, device, sanity=True)
+        total_batch_idx = self.global_step * self.accumulate_grad_batches - 1   # counts across epochs, continues on resume
         done = False
         micro = 0
         while not done:
@@ -184,8 +362,7 @@ class Trainer:
             if hasattr(sampler, "set_epoch"):
                 sampler.set_epoch(self.current_epoch)
             for batch_idx, batch in enumerate(loader):
-                batch = {k: (v.to(device, non_blocking=True) if isinstance(v, torch.Tensor) else v)
-                         for k, v in batch.items()} if isinstance(batch, dict) else batch
+                batch = self._to_device(batch, device)
                 loss = model.training_step(batch, batch_idx)
                 loss = loss["loss"] if isinstance(loss, dict) else loss
                 loss.backward()
@@ -204,13 +381,21 @@ class Trainer:
                     if self.logger is not None and self.global_rank == 0 and \
                             self.global_step % max(1, self.log_every_n_steps) == 0:
                         self.logger.log_metrics({k: float(v) for k, v in self.callback_metrics.items()
-                                                 if not isinstance(v, str)}, self.global_step)
+                                                 if not isinstance(v, str) and k not in self._val_names}, self.global_step)
                 for cb in self.callbacks:
                     cb.on_train_batch_end(self, model, loss, batch, batch_idx)
+                total_batch_idx += 1
+                if val_loader is not None and self._should_check_val_epoch():
+                    i = total_batch_idx if self.check_val_every_n_epoch is None else batch_idx
+                    if (i + 1) % self.val_check_batch == 0:
+                        self._run_validation(model, val_loader, n_val, device)
                 if self.max_steps and self.max_steps > 0 and self.global_step >= self.max_steps:
                     done = True
                     stopped_mid_epoch = True
                     break
+            if val_loader is not None and self.val_check_batch == float("inf") and not stopped_mid_epoch and \
+                    self._should_check_val_epoch():   # a training loader without a length: validate at the epoch's end
+                self._run_validation(model, val_loader, n_val, device)
             for sc in self.lr_scheduler_configs:
                 if sc.get("interval", "epoch") == "epoch":
                     sc["scheduler"].step()
