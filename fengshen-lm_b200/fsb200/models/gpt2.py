@@ -14,6 +14,7 @@ from types import SimpleNamespace
 import torch
 from torch import nn
 
+from .. import generation
 from .. import lib as L
 from .. import ops
 from ..flat import FlatBuffers, FlatSpec
@@ -174,6 +175,81 @@ class GPT2LMHeadModel(nn.Module):
                 ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
+
+    # ---- KV-cache generation -----------------------------------------------------------------------------------------
+    # transformers' GenerationMixin on GPT-2 (wenzhong_qa/README.md:58-67: sampling with top_p, num_return_sequences,
+    # return_dict_in_generate, output_scores). The prompt is prefilled with the training kernels (causal attention under the
+    # left-padding key mask) and its keys / values land in a pre-allocated [rows, cap, 2, heads, head_dim] cache per layer;
+    # every later step feeds one token per row and attends with the split-KV decode kernel (ops.attn_decode). Position ids
+    # follow transformers 5.5.0 (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
+    @torch.no_grad()
+    def generate(self, input_ids=None, attention_mask=None, **kwargs):
+        """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded."""
+        dev = self.flat.params.device
+        ids = input_ids.to(device=dev, dtype=torch.int64)
+        B, S0 = ids.shape
+        c = generation.resolve(self.config, kwargs, S0, False)
+        if c.max_length > self.npos:
+            raise ValueError(f"fsb200 GPT2 generate: max_length {c.max_length} exceeds n_positions {self.npos}")
+        mask = generation.default_attention_mask(ids, c.pad, c.eos) if attention_mask is None else \
+            attention_mask.to(device=dev, dtype=torch.int64)
+        ids, mask = ids.repeat_interleave(c.expand, 0), mask.repeat_interleave(c.expand, 0)
+        R = ids.shape[0]
+        cap = (max(c.max_length, S0 + 1) + 63) // 64 * 64
+        st = SimpleNamespace(cache=[torch.zeros((R, cap, 2, self.nh, self.hn), dtype=torch.bfloat16, device=dev)
+                                    for _ in range(self.nl)],
+                             kv_mask=torch.zeros((R, cap), dtype=torch.uint8, device=dev),
+                             kv_len=torch.zeros(1, dtype=torch.int32, device=dev),
+                             count=mask.sum(-1), cur=S0)
+        st.kv_mask[:, :S0] = mask.to(torch.uint8)
+
+        def step(tokens, reorder):
+            if tokens is None:
+                pos = (mask.cumsum(-1) - 1).masked_fill(mask == 0, 0)
+                pre = None if bool(mask.all()) else st.kv_mask[:, :S0].contiguous()
+                return self._gen_forward(ids.reshape(-1), pos.reshape(-1), R, S0, st, pre)
+            if reorder is not None:
+                st.cache = [kv.index_select(0, reorder) for kv in st.cache]
+                st.kv_mask, st.count = st.kv_mask.index_select(0, reorder), st.count.index_select(0, reorder)
+            st.kv_mask[:, st.cur] = 1
+            st.kv_len.fill_(st.cur + 1)
+            logits = self._gen_forward(tokens, st.count, R, 1, st, None)
+            st.cur += 1
+            st.count = st.count + 1
+            return logits
+
+        return generation.run(step, ids, c)
+
+    def _gen_forward(self, ids, pos, B, S, st, prefill_mask):
+        """S > 1: prefill (writes cache slots [0, S)); S == 1: one decode step at slot st.cur. Returns fp32 logits [B, V]
+        of the last position."""
+        h, nh, hn = self.h, self.nh, self.hn
+        tr = self.transformer
+        self._need("no_decay"); self._need("wte")
+        x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
+        prev_m = None
+        scale = 1.0 / math.sqrt(hn)
+        at = 0 if S > 1 else st.cur
+        for i, blk in enumerate(tr.h):
+            self._need(f"layer{i}")
+            h1, _, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
+                                         self.eps, residual=None if prev_m is None else x)
+            qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
+            q5 = qkv.view(B, S, 3, nh, hn)
+            kv = st.cache[i]
+            kv[:, at:at + S].copy_(q5[:, :, 1:3])
+            if S > 1:
+                o, _ = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=prefill_mask)
+            else:
+                o, _ = ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], st.kv_len, scale, kv_mask=st.kv_mask)
+            a = ops.gemm(L.GEMM_NN, o.view(B * S, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
+            h2, _, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
+            f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data, epilogue=L.EPI_GELU_TANH)
+            m = ops.gemm(L.GEMM_NN, f, blk.mlp.c_proj.weight.data, bias=blk.mlp.c_proj.bias.data)
+            x, prev_m = x1, m
+        hf, _, _ = ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x)
+        last = hf.view(B, S, h)[:, -1].contiguous()
+        return ops.gemm(L.GEMM_NT, last, tr.wte.weight.data).float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):

@@ -19,6 +19,7 @@ from types import SimpleNamespace
 import torch
 from torch import nn
 
+from .. import generation
 from .. import lib as L
 from .. import ops
 from ..flat import FlatBuffers, FlatSpec
@@ -376,27 +377,7 @@ class LlamaForCausalLM(nn.Module):
             count = count + 1
         return seqs
 
-    @staticmethod
-    def _pick(logits, seqs, do_sample, temperature, top_k, top_p, repetition_penalty, generator):
-        """HF logits-processor order: repetition penalty -> temperature -> top-k -> top-p -> sample (or argmax)."""
-        if repetition_penalty != 1.0:
-            seen = torch.gather(logits, 1, seqs)
-            seen = torch.where(seen < 0, seen * repetition_penalty, seen / repetition_penalty)
-            logits = logits.scatter(1, seqs, seen)
-        if not do_sample:
-            return logits.argmax(-1)
-        if temperature != 1.0:
-            logits = logits / temperature
-        if top_k and top_k > 0:
-            kth = torch.topk(logits, min(top_k, logits.shape[-1]), dim=-1).values[:, -1:]
-            logits = logits.masked_fill(logits < kth, float("-inf"))
-        if top_p < 1.0:
-            srt, idx = torch.sort(logits, descending=False, dim=-1)
-            cum = torch.softmax(srt, -1).cumsum(-1)
-            remove = cum <= (1.0 - top_p)
-            remove[:, -1] = False
-            logits = logits.masked_fill(remove.scatter(1, idx, remove), float("-inf"))
-        return torch.multinomial(torch.softmax(logits, -1), 1, generator=generator).squeeze(1)
+    _pick = staticmethod(generation.pick)   # HF logits-processor order, then arg-max or one draw (fsb200/generation.py)
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):

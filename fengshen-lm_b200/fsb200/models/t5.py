@@ -26,6 +26,7 @@ from types import SimpleNamespace
 import torch
 from torch import nn
 
+from .. import generation
 from .. import lib as L
 from .. import ops
 from ..flat import FlatBuffers, FlatSpec
@@ -251,19 +252,12 @@ class MT5ForConditionalGeneration(nn.Module):
             return ops.rmsnorm_fwd(x, self.P(name).data, self.eps)
         return ops.rmsnorm_fwd(prev, self.P(name).data, self.eps, residual=x)
 
-    def _forward_impl(self, ids, dec_ids, mask, lab, B, Se, Sd, save, want_logits):
-        d, nh, dk, inner, ff = self.d, self.nh, self.dk, self.inner, self.ff
+    def _encode(self, ids, mask, B, Se, rel_e, save):
+        """Encoder stack over ids [B * Se]; returns (saved activations, final hidden states, their rstd, residual stream)."""
+        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
         P = self.P
-        Te, Td = B * Se, B * Sd
-        self._need("no_decay"); self._need("shared")
-        W = P("shared.weight").data
-        # relative-position bias vectors (fp32 [heads, 2S - 1]) from the two [buckets, heads] tables
-        rel_e = TB.rel_bias_vector(P("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Se, Se, True,
-                                   self.nbuckets, self.maxdist)
-        rel_d = TB.rel_bias_vector(P("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Sd, Sd, False,
-                                   self.nbuckets, self.maxdist)
-        # ---- encoder
-        x, prev = ops.embedding_fwd(ids, W), None
+        Te = B * Se
+        x, prev = ops.embedding_fwd(ids, P("shared.weight").data), None
         eacts = []
         for i in range(self.ne):
             p = f"encoder.block.{i}.layer."
@@ -282,6 +276,90 @@ class MT5ForConditionalGeneration(nn.Module):
             x, prev = x1, m
         self._need("head")
         enc_h, rfe, xfe = self._norm(prev, x, "encoder.final_layer_norm.weight")
+        return eacts, enc_h, rfe, xfe
+
+    # ---- KV-cache generation -----------------------------------------------------------------------------------------
+    # transformers' GenerationMixin on MT5 (mt5_summary.py:41-49,131-139; finetune_t5.py:66-71). The encoder runs once; every
+    # decoder layer projects its cross-attention K|V once from the encoder output; each step feeds one token per row, appends
+    # its self-attention K|V to a [rows, cap, 2, heads, d_kv] cache and runs the split-KV decode kernel twice per layer: self-
+    # attention with the relative-position bias at the query's slot, cross-attention under the encoder padding mask.
+    @torch.no_grad()
+    def generate(self, input_ids=None, attention_mask=None, **kwargs):
+        """HF `generate` semantics (fsb200/generation.py lists what is implemented); sequences start with
+        decoder_start_token_id."""
+        dev = self.flat.params.device
+        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        P = self.P
+        ids = input_ids.to(device=dev, dtype=torch.int64).contiguous()
+        B, Se = ids.shape
+        c = generation.resolve(self.config, kwargs, 1, True)
+        mask = generation.default_attention_mask(ids, c.pad, c.eos) if attention_mask is None else \
+            attention_mask.to(device=dev, dtype=torch.int64)
+        emask = None if bool(mask.all()) else mask.to(torch.uint8).contiguous()
+        self._need("no_decay"); self._need("shared")
+        rel_e = TB.rel_bias_vector(P("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Se, Se, True,
+                                   self.nbuckets, self.maxdist)
+        _, enc_h, _, _ = self._encode(ids.view(-1), emask, B, Se, rel_e, False)
+        R = B * c.expand
+        cross = []
+        for i in range(self.nd):
+            self._need(f"dec{i}")
+            kvc = ops.gemm(L.GEMM_NT, enc_h, self._d_kv[i]).view(B, Se, 2, nh, dk)
+            cross.append(kvc.repeat_interleave(c.expand, 0) if c.expand > 1 else kvc)
+        cmask = None if emask is None else emask.repeat_interleave(c.expand, 0).contiguous()
+        cap = (max(c.max_length, 2) + 63) // 64 * 64
+        rel_d = TB.rel_bias_vector(P("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, cap, cap,
+                                   False, self.nbuckets, self.maxdist)
+        enc_len = torch.full((1,), Se, dtype=torch.int32, device=dev)
+        start = torch.full((R, 1), c.start, dtype=torch.int64, device=dev)
+        st = SimpleNamespace(cache=[torch.zeros((R, cap, 2, nh, dk), dtype=torch.bfloat16, device=dev) for _ in range(self.nd)],
+                             kv_len=torch.zeros(1, dtype=torch.int32, device=dev), cur=0)
+
+        def step(tokens, reorder):
+            if reorder is not None:
+                st.cache = [kv.index_select(0, reorder) for kv in st.cache]
+            tok = start.view(-1) if tokens is None else tokens
+            st.kv_len.fill_(st.cur + 1)
+            self._need("no_decay"); self._need("shared")
+            y, prev = ops.embedding_fwd(tok, P("shared.weight").data), None
+            for i in range(self.nd):
+                p = f"decoder.block.{i}.layer."
+                self._need(f"dec{i}")
+                h1, _, y = self._norm(prev, y, p + "0.layer_norm.weight")
+                q3 = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i]).view(R, 3, nh, dk)
+                kv = st.cache[i]
+                kv[:, st.cur].copy_(q3[:, 1:3])
+                o, _ = ops.attn_decode(q3[:, 0], kv[:, :, 0], kv[:, :, 1], st.kv_len, 1.0, rel_bias=rel_d)
+                a = ops.gemm(L.GEMM_NT, o.view(R, inner), P(p + "0.SelfAttention.o.weight").data)
+                h2, _, y1 = self._norm(a, y, p + "1.layer_norm.weight")
+                qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
+                oc, _ = ops.attn_decode(qc.view(R, nh, dk), cross[i][:, :, 0], cross[i][:, :, 1], enc_len, 1.0,
+                                        kv_mask=cmask)
+                ac = ops.gemm(L.GEMM_NT, oc.view(R, inner), P(p + "1.EncDecAttention.o.weight").data)
+                h3, _, y2 = self._norm(ac, y1, p + "2.layer_norm.weight")
+                gu = ops.gemm(L.GEMM_NT, h3, self._d_wi[i])
+                act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
+                m = ops.gemm(L.GEMM_NT, act, P(p + "2.DenseReluDense.wo.weight").data)
+                y, prev = y2, m
+            self._need("head")
+            hf, _, _ = self._norm(prev, y, "decoder.final_layer_norm.weight")
+            st.cur += 1
+            return ops.gemm(L.GEMM_NT, hf, P(self._head).data).float()
+
+        return generation.run(step, start, c)
+
+    def _forward_impl(self, ids, dec_ids, mask, lab, B, Se, Sd, save, want_logits):
+        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        P = self.P
+        Td = B * Sd
+        self._need("no_decay"); self._need("shared")
+        W = P("shared.weight").data
+        # relative-position bias vectors (fp32 [heads, 2S - 1]) from the two [buckets, heads] tables
+        rel_e = TB.rel_bias_vector(P("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Se, Se, True,
+                                   self.nbuckets, self.maxdist)
+        rel_d = TB.rel_bias_vector(P("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Sd, Sd, False,
+                                   self.nbuckets, self.maxdist)
+        eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save)
         # ---- decoder
         y, prev = ops.embedding_fwd(dec_ids, W), None
         dacts = []

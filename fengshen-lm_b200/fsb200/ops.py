@@ -354,6 +354,46 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None):
     return out, lse
 
 
+def attn_decode(q, k_cache, v_cache, kv_len, scale, kv_mask=None, rel_bias=None, out=None):
+    """One decode step: q [B, H, D] (the newest token, at cache slot kv_len - 1) against k_cache / v_cache [B, cap, H, D]
+    (strided bf16 views, unit inner stride). kv_len: int32 CUDA scalar. kv_mask: uint8 [B, cap]. rel_bias: fp32
+    [H, 2 cap - 1] (sdpa_fwd's convention with seq_q = seq_kv = cap). Returns (out [B, H, D], lse [B, H] log2 domain)."""
+    for t, n in ((q, "q"), (k_cache, "k_cache"), (v_cache, "v_cache")):
+        _chk(t, _bf16, n)
+    if q.dim() != 3 or q.stride(2) != 1:
+        raise RuntimeError("fsb200 attn_decode: q must be [batch, heads, dim] with unit inner stride")
+    B, H, D = q.shape
+    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
+        if t.dim() != 4 or t.stride(3) != 1 or (t.shape[0], t.shape[2], t.shape[3]) != (B, H, D):
+            raise RuntimeError(f"fsb200 attn_decode: {n} must be [{B}, cap, {H}, {D}] with unit inner stride, "
+                               f"got {tuple(t.shape)} strides {t.stride()}")
+    cap = k_cache.shape[1]
+    if v_cache.shape[1] != cap:
+        raise RuntimeError("fsb200 attn_decode: k_cache and v_cache capacities differ")
+    _chk(kv_len, torch.int32, "kv_len")
+    if kv_len.numel() != 1:
+        raise RuntimeError("fsb200 attn_decode: kv_len must be a one-element int32 tensor")
+    if out is None:
+        out = torch.empty((B, H, D), dtype=_bf16, device=q.device)
+    _chk(out, _bf16, "out")
+    if tuple(out.shape) != (B, H, D) or out.stride(2) != 1:
+        raise RuntimeError("fsb200 attn_decode: out must be [batch, heads, dim] with unit inner stride")
+    if kv_mask is not None:
+        _chk(kv_mask, torch.uint8, "kv_mask")
+        if tuple(kv_mask.shape) != (B, cap) or not kv_mask.is_contiguous():
+            raise RuntimeError(f"fsb200 attn_decode: kv_mask must be contiguous uint8 [{B}, {cap}]")
+    if rel_bias is not None:
+        _chk_rel(rel_bias, H, cap, cap, "rel_bias")
+    lse = torch.empty((B, H), dtype=torch.float32, device=q.device)
+    ws_bytes = int(L.load().fsb_attn_decode_workspace_bytes(B, H, D, cap))
+    ws = workspace(ws_bytes, q.device, "attn_decode")
+    L.call("fsb_attn_decode", _p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), B, H, D, cap, _p(kv_len),
+           q.stride(0), q.stride(1), k_cache.stride(0), k_cache.stride(1), k_cache.stride(2),
+           v_cache.stride(0), v_cache.stride(1), v_cache.stride(2), out.stride(0), out.stride(1), float(scale),
+           _p(kv_mask), _p(rel_bias), _p(ws), ws_bytes, _stream())
+    return out, lse
+
+
 def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
     rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=), deterministically."""

@@ -240,6 +240,28 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
                  float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                  void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- decode attention over a KV cache (split-KV) -------------------------------------------------------------------
+ * One query row per (batch, head) — the newest token of a generation step, at cache slot *kv_len - 1 — attends to the cache
+ * slots [0, *kv_len):  O = softmax(scale * q.K^T + bias + mask) V. kv_len is a DEVICE int32 scalar, clamped to [0, kv_cap];
+ * no slot at or beyond it is ever read. Element addressing (elements, 16-byte aligned bases, strides multiples of 8):
+ *   q (b, head, d)       at q + b*q_batch_stride + head*q_head_stride + d        (o likewise with o_*_stride)
+ *   k (b, slot, head, d) at k + b*k_batch_stride + slot*k_row_stride + head*k_head_stride + d   (v likewise)
+ * lse: optional fp32 [batch, nheads], log2 domain as in fsb_sdpa_fwd. kv_mask: optional uint8 [batch, kv_cap], 1 = attend.
+ * rel_bias: optional fp32 [nheads, 2*kv_cap - 1] in fsb_sdpa_fwd's convention with seq_q = seq_kv = kv_cap, i.e. the bias of key
+ *   k is rel_bias[head][k - (*kv_len - 1) + kv_cap - 1] (T5 / mT5 decoder self-attention). A row that sees no key gets O = 0
+ *   and lse = +inf. head_dim in {64, 128}. The keys are split into chunks planned from (batch, nheads, kv_cap) alone; the fp32
+ * partials go to `workspace` (fsb_attn_decode_workspace_bytes bytes, 16-byte aligned) and are merged in a fixed order, so the
+ * result is deterministic. Two kernel launches. */
+size_t fsb_attn_decode_workspace_bytes(int64_t batch, int nheads, int head_dim, int64_t kv_cap);
+int fsb_attn_decode(const void* q, const void* k, const void* v, void* o, float* lse,
+                    int64_t batch, int nheads, int head_dim, int64_t kv_cap, const int32_t* kv_len,
+                    int64_t q_batch_stride, int64_t q_head_stride,
+                    int64_t k_batch_stride, int64_t k_row_stride, int64_t k_head_stride,
+                    int64_t v_batch_stride, int64_t v_row_stride, int64_t v_head_stride,
+                    int64_t o_batch_stride, int64_t o_head_stride,
+                    float scale, const uint8_t* kv_mask, const float* rel_bias,
+                    void* workspace, size_t workspace_bytes, fsb_stream_t stream);
+
 /* ---- communication (NCCL over NVLink / NVSwitch) --------------------------------------------------------------
  * The three exchange steps of the ZeRO-1/2 data path (SURVEY.md §8e) — the collectives the reference delegates to DeepSpeed
  * (fengshen/strategies/megatron_deepspeed.py:302-320; Appendix D): bucketed gradient reduce-scatter (SUM), the fp32 scalar
