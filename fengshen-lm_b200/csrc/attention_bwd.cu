@@ -13,6 +13,7 @@
 // S and dP are recomputed in both kernels (7 GEMMs instead of 5) — the price of determinism without a dQ reduction.
 // Both kernels: warpgroup 0 = TMA producer, warpgroups 1-2 = 64 resident rows each, working on the same streamed stage.
 #include "host_common.h"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace fsb {
@@ -37,6 +38,7 @@ struct AttBwdParams {
   int q_head_stride, k_head_stride, v_head_stride, do_head_stride;
   int seq_q, seq_kv, nheads, batch, causal;
   float scale, scale_log2;
+  DropArgs drop;             // attention-probability dropout (kDropout only): the forward's seed, stream base and site
 };
 
 // ------------------------------------------------------------------------------------------------ delta preprocess
@@ -104,7 +106,8 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 }
 
 // ================================================================================================ dQ kernel
-template <int D, bool kBias>
+// kDropout: dS = P * (dP * Z / (1 - p) - delta), Z regenerated from philox.cuh (delta = rowsum(dO * O) is unchanged).
+template <int D, bool kBias, bool kDropout>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -189,6 +192,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   float dq[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
+  DropKey dkey;
+  if constexpr (kDropout) dkey = drop_key(p.drop);
 
   mbar_wait(big_full, 0);
   for (int j = 0; j < n_steps; ++j) {
@@ -205,10 +210,12 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int kk = 0; kk < D / 16; ++kk)
       wgmma_ss_n64<0, 0>(dp, dsc_do + (kslice(kk, AB_BM) >> 4), dsc_v + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
     wgmma_commit();
+    const int c0 = j * AB_BN;
+    uint32_t dw[kDropout ? AB_BN / 16 : 1][2];   // the forward's keep bits, regenerated while the tensor cores work
+    if constexpr (kDropout) attn_drop_rows<AB_BN / 16>(dkey, uint32_t(b * p.nheads + head), q0 + r_lo, c0, lane, dw);
     wgmma_wait<0>();
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
-    const int c0 = j * AB_BN;
     const bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -223,7 +230,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           if (mrow != nullptr && keep) keep = mrow[col] != 0;
           pe = keep ? pe : 0.f;
         }
-        s[4 * i + e] = pe * (dp[4 * i + e] - delta[h]);   // dS
+        float dpe = dp[4 * i + e];
+        if constexpr (kDropout) dpe = drop_keep(dw[i >> 1][e & 1], 2 * h + (i & 1), dkey.thr) ? dpe * p.drop.keep_scale : 0.f;
+        s[4 * i + e] = pe * (dpe - delta[h]);   // dS
       }
     }
     if constexpr (kBias) {
@@ -270,7 +279,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 }
 
 // ================================================================================================ dK / dV kernel
-template <int D, bool kBias>
+// kDropout: dV += (P * Z / (1 - p))^T dO and dS^T = P^T * (dP^T * Z / (1 - p) - delta); a register row is a key row here, so
+// the mask comes from attn_drop_cols (same Philox calls as the row-major kernels, words picked along the other axis).
+template <int D, bool kBias, bool kDropout>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -353,6 +364,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  DropKey dkey;
+  if constexpr (kDropout) dkey = drop_key(p.drop);
 
   mbar_wait(big_full, 0);
   for (int i = 0; i < n_steps; ++i) {
@@ -370,6 +383,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     for (int kk = 0; kk < D / 16; ++kk)
       wgmma_ss_n64<0, 0>(dp, dsc_v + (kslice(kk, AB_BM) >> 4), dsc_do + sto + (kslice(kk, AB_BN) >> 4), kk != 0 ? 1u : 0u);
     wgmma_commit();
+    // the forward's keep bits, regenerated while the tensor cores work; one bit per element, so a single register carries
+    // them past the wait
+    uint32_t zbits = 0;
+    if constexpr (kDropout) zbits = attn_keep_cols<AB_BN / 16>(dkey, uint32_t(b * p.nheads + head), kv0 + r_lo, qt0, lane);
     wgmma_wait<0>();
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
@@ -390,8 +407,14 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
           float x = ex2_approx(arg);
           const bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]);
           x = keep ? x : 0.f;
-          s[4 * ii + e] = x;                                  // P^T
-          dp[4 * ii + e] = x * (dp[4 * ii + e] - del_c);      // dS^T
+          if constexpr (kDropout) {
+            const bool z = (zbits >> (4 * ii + e)) & 1u;
+            s[4 * ii + e] = z ? x * p.drop.keep_scale : 0.f;                                    // (P * Z / (1 - p))^T
+            dp[4 * ii + e] = x * ((z ? dp[4 * ii + e] * p.drop.keep_scale : 0.f) - del_c);      // dS^T
+          } else {
+            s[4 * ii + e] = x;                                  // P^T
+            dp[4 * ii + e] = x * (dp[4 * ii + e] - del_c);      // dS^T
+          }
         }
       }
     }
@@ -466,7 +489,7 @@ static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq
   return size_t(batch) * nheads * n_qt * n_all * AB_DSTRIDE;
 }
 
-template <int D, bool kBias>
+template <int D, bool kBias, bool kDropout>
 static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                            int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
                            float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
@@ -474,8 +497,10 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   using SK = AttBwdSmem<D, false>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<D, kBias>, cudaFuncAttributeMaxDynamicSharedMemorySize, SQ::TOTAL);
-    cudaError_t e2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<D, kBias>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK::TOTAL);
+    cudaError_t e1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<D, kBias, kDropout>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          SQ::TOTAL);
+    cudaError_t e2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<D, kBias, kDropout>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          SK::TOTAL);
     if (e1 != cudaSuccess || e2 != cudaSuccess) {
       set_error("sdpa_bwd: cudaFuncSetAttribute(%d / %d) failed", SQ::TOTAL, SK::TOTAL);
       return FSB_ERR_CUDA;
@@ -506,7 +531,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   // 2. dQ
   {
     dim3 grid((p.seq_q + AB_BM - 1) / AB_BM, p.nheads, p.batch);
-    attn_bwd_dq_kernel<D, kBias><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
+    attn_bwd_dq_kernel<D, kBias, kDropout><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
     FSB_CUDA_LAUNCH_CHECK();
     if (kBias && drel_bias != nullptr) {
       const int n_rel = p.seq_q + p.seq_kv - 1, bs = dbias_bsplit(p.batch);
@@ -520,7 +545,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   // 3. dK, dV
   {
     dim3 grid((p.seq_kv + AB_BM - 1) / AB_BM, p.nheads, p.batch);
-    attn_bwd_dkv_kernel<D, kBias><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
+    attn_bwd_dkv_kernel<D, kBias, kDropout><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
     FSB_CUDA_LAUNCH_CHECK();
   }
   return FSB_OK;
@@ -530,15 +555,14 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
 
 using namespace fsb;
 
-extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                            const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q,
-                            int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride, int64_t k_row_stride,
-                            int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
-                            int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                            int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                            int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
-                            int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias, void* workspace,
-                            size_t workspace_bytes, fsb_stream_t st) {
+static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                    float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads,
+                    int head_dim, int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                    int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                    int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                    int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                    float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
+                    void* workspace, size_t workspace_bytes, const DropArgs* drop, fsb_stream_t st) {
   FSB_REQUIRE(q && k && v && o && dout && lse && delta && dq && dk && dv, "sdpa_bwd: null pointer");
   FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd: head_dim %d unsupported (64 or 128)", head_dim);
   FSB_REQUIRE(batch > 0 && seq_q > 0 && seq_kv > 0 && nheads > 0 && batch < 65536 && nheads < 65536, "sdpa_bwd: bad dims");
@@ -570,12 +594,56 @@ extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const v
   p.do_head_stride = int(do_head_stride);
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-#define FSB_BWD(DD, BB)                                                                                                  \
-  launch_attn_bwd<DD, BB>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride, do_row_stride,       \
+#define FSB_BWD(DD, BB, DR)                                                                                              \
+  launch_attn_bwd<DD, BB, DR>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride, do_row_stride,       \
                           o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
-  if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true) : FSB_BWD(64, true);
-  return head_dim == 128 ? FSB_BWD(128, false) : FSB_BWD(64, false);
+  if (drop != nullptr) {
+    p.drop = *drop;
+    return head_dim == 128 ? FSB_BWD(128, false, true) : FSB_BWD(64, false, true);
+  }
+  if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, false) : FSB_BWD(64, true, false);
+  return head_dim == 128 ? FSB_BWD(128, false, false) : FSB_BWD(64, false, false);
 #undef FSB_BWD
+}
+
+extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                            const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q,
+                            int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride, int64_t k_row_stride,
+                            int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
+                            int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                            int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                            int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
+                            int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias, void* workspace,
+                            size_t workspace_bytes, fsb_stream_t st) {
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
+                  nullptr, st);
+}
+
+extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                    const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
+                                    int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
+                                    int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                    int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
+                                    int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                                    int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                                    int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
+                                    int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
+                                    void* workspace, size_t workspace_bytes, float p, uint64_t seed,
+                                    const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p > 0.f) {
+    FSB_REQUIRE(!causal && rel_bias == nullptr, "sdpa_bwd_dropout: causal masks and rel_bias are not supported with p > 0");
+    FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536, "sdpa_bwd_dropout: sequences longer than 65536 are not supported with p > 0");
+  }
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
+                  p > 0.f ? &d : nullptr, st);
 }
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {

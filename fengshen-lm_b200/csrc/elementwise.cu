@@ -8,7 +8,9 @@
 //   embedding   : VocabParallelEmbedding.forward mpu/layers.py:104-130 (+ learned position / token-type rows for
 //                 BERT / GPT-2: transformers bert/modeling_bert.py:53-112, gpt2/modeling_gpt2.py wte+wpe)
 //   add         : residual adds layers/transformer.py:775-788
+//   dropout     : y = x * Z / (1 - p) with the hidden-dropout mask of philox.cuh (BERT / MegatronBERT embedding sites)
 #include "host_common.h"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace fsb {
@@ -190,6 +192,37 @@ __global__ void __launch_bounds__(256) scale_inplace_kernel(uint4* __restrict__ 
     for (int j = 0; j < 8; ++j) f[j] *= s;
     x[i] = pack8(f);
   }
+}
+
+// y = x * Z / (1 - p) over [rows, cols]; one thread per 16-column group = one Philox call. The same op is the backward
+// (dx = dy * Z / (1 - p)).
+__global__ void __launch_bounds__(256) dropout_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int64_t rows,
+                                                      int cols, const DropArgs drop) {
+  const int nvec = cols >> 3, ngrp = (nvec + 1) >> 1;
+  const DropKey k = drop_key(drop);
+  for (int64_t g = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; g < rows * ngrp; g += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t row = g / ngrp;
+    const int c16 = int(g - row * ngrp);
+    const uint4 r = drop_hidden_bits(k, uint32_t(row), uint32_t(c16));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = 2 * c16 + h;
+      if (c >= nvec) break;
+      const uint32_t w0 = h ? r.z : r.x, w1 = h ? r.w : r.y;
+      float f[8];
+      unpack8(x[row * nvec + c], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = drop_keep(j < 4 ? w0 : w1, j & 3, k.thr) ? f[j] * drop.keep_scale : 0.f;
+      y[row * nvec + c] = pack8(f);
+    }
+  }
+}
+
+// saved = *base; *base += n — the dropout stream counter, advanced on the device once per training forward
+__global__ void dropout_advance_kernel(int64_t* __restrict__ base, int64_t* __restrict__ saved, int64_t n) {
+  const int64_t b = *base;
+  *saved = b;
+  *base = b + n;
 }
 
 // acc (fp32) += scale * x (bf16)   — gradient accumulation into the fp32 shard (ZeRO-2 per-micro-step reduce)
@@ -522,6 +555,34 @@ extern "C" int fsb_add(const void* a, const void* b, void* out, int64_t n, fsb_s
 extern "C" int fsb_scale_inplace(void* x, int64_t n, const float* scale_dev, fsb_stream_t st) {
   FSB_REQUIRE(x && scale_dev && n > 0 && n % 8 == 0 && aligned16(x), "scale_inplace: bad args (n %% 8 == 0, aligned)");
   scale_inplace_kernel<<<ew_grid(n / 8, 256), 256, 0, (cudaStream_t)st>>>((uint4*)x, n / 8, scale_dev);
+  FSB_CUDA_LAUNCH_CHECK();
+  return FSB_OK;
+}
+extern "C" int fsb_dropout(const void* x, void* y, int64_t rows, int64_t cols, float p, uint64_t seed,
+                           const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  FSB_REQUIRE(x && y && rows > 0 && cols > 0 && cols % 8 == 0 && cols <= (1 << 20) && aligned16(x) && aligned16(y),
+              "dropout: bad args (cols %% 8 == 0, aligned)");
+  FSB_REQUIRE(rows <= 0xffffffffll, "dropout: more than 2^32 rows");
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p == 0.f) {
+    if (x != y) {
+      cudaError_t e = cudaMemcpyAsync(y, x, size_t(rows) * size_t(cols) * 2, cudaMemcpyDeviceToDevice, (cudaStream_t)st);
+      if (e != cudaSuccess) {
+        set_error("dropout: copy failed: %s", cudaGetErrorString(e));
+        return FSB_ERR_CUDA;
+      }
+    }
+    return FSB_OK;
+  }
+  const int64_t groups = rows * ((cols / 8 + 1) / 2);
+  dropout_kernel<<<ew_grid(groups, 256), 256, 0, (cudaStream_t)st>>>((const uint4*)x, (uint4*)y, rows, int(cols), d);
+  FSB_CUDA_LAUNCH_CHECK();
+  return FSB_OK;
+}
+extern "C" int fsb_dropout_advance(int64_t* stream_base, int64_t* saved, int64_t n, fsb_stream_t st) {
+  FSB_REQUIRE(stream_base && saved && n >= 0, "dropout_advance: bad args");
+  dropout_advance_kernel<<<1, 1, 0, (cudaStream_t)st>>>(stream_base, saved, n);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }

@@ -10,9 +10,13 @@
 // Weight gradients: every thread accumulates fp32 partials over its rows; the CTA combines its RPC row slots through
 // shared memory in a fixed order and writes partial[cta, cols]; a second kernel reduces the partials column-wise
 // (deterministic, no atomics).
+// Dropout on the branch (kDrop, LayerNorm with a residual only): the forward computes x_sum = x * Z / (1 - p) + residual, Z the
+// hidden-dropout mask of philox.cuh at (row, col); the backward also writes dbranch = dx * Z / (1 - p) — the gradient of the
+// dropped branch beside the gradient of the sum.
 #include <stdlib.h>
 
 #include "host_common.h"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace fsb {
@@ -23,6 +27,36 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// x (8 columns 8 c .. 8 c + 7 of `row`) *= Z / (1 - p). One Philox call covers 16 columns; this vector uses half of it.
+// Everything arrives by value: the seed, threshold and scale straight from the kernel parameters (constant bank), the stream
+// from the one load each thread makes before its row loop — no copy of the parameter struct is ever addressed.
+__device__ __forceinline__ uint32_t keep_bits8(uint64_t seed, uint32_t s_lo, uint32_t s_hi, uint32_t thr, int row, int c) {
+  const DropKey k{uint32_t(seed), uint32_t(seed >> 32), s_lo, s_hi, thr};
+  const uint4 r = drop_hidden_bits(k, uint32_t(row), uint32_t(c >> 1));
+  const uint32_t w0 = (c & 1) ? r.z : r.x, w1 = (c & 1) ? r.w : r.y;
+  uint32_t bits = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) bits |= uint32_t(drop_keep(j < 4 ? w0 : w1, j & 3, thr)) << j;
+  return bits;
+}
+__device__ __forceinline__ void apply_keep8(uint32_t bits, float keep_scale, float (&x)[8]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) x[j] = (bits >> j) & 1u ? x[j] * keep_scale : 0.f;
+}
+// dropout on LayerNorm rows is instantiated up to this many 8-column vectors per thread (cols <= 12288): wider rows already
+// spill in the dropout-free backward
+constexpr int NORM_DROP_MAX_VPT = 6;
+// the stream number s = *stream_base + site of a dropout site, split in halves (0 without dropout: nothing is read)
+template <bool kDrop>
+__device__ __forceinline__ void drop_stream(const int64_t* stream_base, int64_t site, uint32_t& s_lo, uint32_t& s_hi) {
+  s_lo = s_hi = 0;
+  if constexpr (kDrop) {
+    const uint64_t s = uint64_t(*stream_base + site);
+    s_lo = uint32_t(s);
+    s_hi = uint32_t(s >> 32);
+  }
 }
 
 // Sum of (a, b) over the TPR threads that share a row; result broadcast to those threads.
@@ -47,15 +81,17 @@ __device__ __forceinline__ void row_sum2(float& a, float& b, float* red, int row
 // ------------------------------------------------------------------------------------------------------------
 // forward.  kLayer = false: RMSNorm (stats[row] = rstd). kLayer = true: LayerNorm (stats[2*row] = mean, [2*row+1] = rstd)
 // ------------------------------------------------------------------------------------------------------------
-template <bool kLayer, int TPR, int VPT>
+template <bool kLayer, int TPR, int VPT, bool kDrop>
 __global__ void __launch_bounds__(NORM_THREADS) norm_fwd_kernel(
     const uint4* __restrict__ x, const uint4* __restrict__ residual, const uint4* __restrict__ gamma,
     const uint4* __restrict__ beta, uint4* __restrict__ y, uint4* __restrict__ sum_out, float* __restrict__ stats,
-    int rows, int cols, float eps) {
+    int rows, int cols, float eps, const DropArgs drop) {
   constexpr int RPC = NORM_THREADS / TPR;
   __shared__ float red[RPC * 2 * (TPR / 32)];
   const int nvec = cols >> 3;
   const int row_slot = threadIdx.x / TPR, lir = threadIdx.x % TPR;
+  uint32_t s_lo, s_hi;
+  drop_stream<kDrop>(drop.stream_base, drop.site, s_lo, s_hi);
   for (int base_row = blockIdx.x * RPC; base_row < rows; base_row += gridDim.x * RPC) {
     const int row = base_row + row_slot;
     const bool rv = row < rows;
@@ -70,6 +106,7 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_fwd_kernel(
         if (residual != nullptr) {
           float r[8];
           unpack8(residual[base + c], r);
+          if constexpr (kDrop) apply_keep8(keep_bits8(drop.seed, s_lo, s_hi, drop.thr, row, c), drop.keep_scale, xv[i]);
 #pragma unroll
           for (int j = 0; j < 8; ++j) xv[i][j] = round_bf16(xv[i][j] + r[j]);  // the sum lives in bf16 in the reference
           sum_out[base + c] = pack8(xv[i]);
@@ -126,11 +163,12 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_fwd_kernel(
 // ------------------------------------------------------------------------------------------------------------
 // backward. dx = rstd * (g - xhat * mean(g*xhat) [- mean(g)])  with g = dy * gamma;  partial dgamma/dbeta per CTA.
 // ------------------------------------------------------------------------------------------------------------
-template <bool kLayer, int TPR, int VPT>
+template <bool kLayer, int TPR, int VPT, bool kDrop>
 __global__ void __launch_bounds__(NORM_THREADS) norm_bwd_kernel(
     const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint4* __restrict__ gamma,
     const float* __restrict__ stats, const uint4* __restrict__ dres, uint4* __restrict__ dx,
-    float* __restrict__ partial /* [grid, (kLayer?2:1) * cols] */, int rows, int cols) {
+    float* __restrict__ partial /* [grid, (kLayer?2:1) * cols] */, int rows, int cols, uint4* __restrict__ dbranch,
+    const DropArgs drop) {
   constexpr int RPC = NORM_THREADS / TPR;
   __shared__ float red[RPC * 2 * (TPR / 32)];
   extern __shared__ float comb[];  // [RPC][width] when RPC > 1
@@ -138,6 +176,8 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_bwd_kernel(
   const int row_slot = threadIdx.x / TPR, lir = threadIdx.x % TPR;
   const int width = cols * (kLayer ? 2 : 1);
   float dg[VPT][8], db[kLayer ? VPT : 1][8];
+  uint32_t s_lo, s_hi;
+  drop_stream<kDrop>(drop.stream_base, drop.site, s_lo, s_hi);
 #pragma unroll
   for (int i = 0; i < VPT; ++i)
 #pragma unroll
@@ -152,6 +192,15 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_bwd_kernel(
     float xh[VPT][8], g[VPT][8];
     uint4 rq[VPT];   // residual-branch gradient, fetched WITH x / dy (one memory round trip per row instead of two)
     float s_g = 0.f, s_gx = 0.f;
+    // keep bits of the row's vectors (8 per vector), drawn while the fewest values are live; applied to dbranch at the end
+    uint64_t keep = 0;
+    if constexpr (kDrop) {
+#pragma unroll
+      for (int i = 0; i < VPT; ++i) {
+        const int c = lir + i * TPR;
+        if (rv && c < nvec) keep |= uint64_t(keep_bits8(drop.seed, s_lo, s_hi, drop.thr, row, c)) << (8 * i);
+      }
+    }
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int c = lir + i * TPR;
@@ -196,6 +245,10 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_bwd_kernel(
           for (int j = 0; j < 8; ++j) o[j] += r[j];
         }
         dx[base + c] = pack8(o);
+        if constexpr (kDrop) {
+          apply_keep8(uint32_t(keep >> (8 * i)) & 0xffu, drop.keep_scale, o);
+          dbranch[base + c] = pack8(o);
+        }
       }
     }
   }
@@ -312,9 +365,9 @@ static int norm_grid(int64_t rows, int tpr) {
                              case 7: KERNEL_LAUNCH(256, 7); break; default: KERNEL_LAUNCH(256, 8); break; } break; \
   }
 
-template <bool kLayer>
+template <bool kLayer, bool kDrop = false>
 static int norm_fwd(const void* x, const void* residual, const void* gamma, const void* beta, void* y, void* sum_out,
-                    float* stats, int64_t rows, int64_t cols, float eps, cudaStream_t st) {
+                    float* stats, int64_t rows, int64_t cols, float eps, cudaStream_t st, const DropArgs& drop = DropArgs{}) {
   FSB_REQUIRE(rows > 0 && cols > 0 && cols % 8 == 0 && cols <= 16384 && rows < (1 << 30),
               "norm_fwd: bad shape rows=%ld cols=%ld", (long)rows, (long)cols);
   FSB_REQUIRE(x && gamma && y && stats && (!kLayer || beta), "norm_fwd: null pointer");
@@ -326,20 +379,21 @@ static int norm_fwd(const void* x, const void* residual, const void* gamma, cons
   norm_shape(cols, tpr, vpt);
   const int grid = norm_grid(rows, tpr);
 #define L(T, V)                                                                                                   \
-  norm_fwd_kernel<kLayer, T, V><<<grid, NORM_THREADS, 0, st>>>((const uint4*)x, (const uint4*)residual,          \
-                                                               (const uint4*)gamma, (const uint4*)beta, (uint4*)y, \
-                                                               (uint4*)sum_out, stats, int(rows), int(cols), eps)
+  if constexpr (!kDrop || V <= NORM_DROP_MAX_VPT)                                                                  \
+  norm_fwd_kernel<kLayer, T, V, kDrop><<<grid, NORM_THREADS, 0, st>>>(                                             \
+      (const uint4*)x, (const uint4*)residual, (const uint4*)gamma, (const uint4*)beta, (uint4*)y, (uint4*)sum_out, stats, \
+      int(rows), int(cols), eps, drop)
   FSB_NORM_DISPATCH(L)
 #undef L
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
 
-template <bool kLayer, int T, int V>
+template <bool kLayer, int T, int V, bool kDrop>
 static cudaError_t norm_bwd_smem_attr(size_t bytes) {
   static size_t configured = 0;
   if (bytes > 48 * 1024 && bytes > configured) {
-    cudaError_t e = cudaFuncSetAttribute(norm_bwd_kernel<kLayer, T, V>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(norm_bwd_kernel<kLayer, T, V, kDrop>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          int(bytes));
     if (e != cudaSuccess) return e;
     configured = bytes;
@@ -347,10 +401,10 @@ static cudaError_t norm_bwd_smem_attr(size_t bytes) {
   return cudaSuccess;
 }
 
-template <bool kLayer>
+template <bool kLayer, bool kDrop = false>
 static int norm_bwd(const void* dy, const void* x, const void* gamma, const float* stats, const void* dres, void* dx,
                     void* dgamma, void* dbeta, int wgrad_dtype, int accumulate, void* workspace, size_t ws_bytes,
-                    int64_t rows, int64_t cols, cudaStream_t st) {
+                    int64_t rows, int64_t cols, cudaStream_t st, void* dbranch = nullptr, const DropArgs& drop = DropArgs{}) {
   FSB_REQUIRE(rows > 0 && cols > 0 && cols % 8 == 0 && cols <= 16384 && rows < (1 << 30),
               "norm_bwd: bad shape rows=%ld cols=%ld", (long)rows, (long)cols);
   FSB_REQUIRE(dy && x && gamma && stats && dx && dgamma && workspace && (!kLayer || dbeta), "norm_bwd: null pointer");
@@ -366,11 +420,13 @@ static int norm_bwd(const void* dy, const void* x, const void* gamma, const floa
   const size_t smem = rpc > 1 ? size_t(rpc) * width * sizeof(float) : 0;
   cudaError_t e = cudaSuccess;
 #define L(T, V)                                                                                                    \
-  e = norm_bwd_smem_attr<kLayer, T, V>(smem);                                                                      \
-  if (e == cudaSuccess)                                                                                            \
-    norm_bwd_kernel<kLayer, T, V><<<grid, NORM_THREADS, smem, st>>>((const uint4*)dy, (const uint4*)x,             \
-                                                                    (const uint4*)gamma, stats, (const uint4*)dres, \
-                                                                    (uint4*)dx, (float*)workspace, int(rows), int(cols))
+  if constexpr (!kDrop || V <= NORM_DROP_MAX_VPT) {                                                                \
+    e = norm_bwd_smem_attr<kLayer, T, V, kDrop>(smem);                                                             \
+    if (e == cudaSuccess)                                                                                          \
+      norm_bwd_kernel<kLayer, T, V, kDrop><<<grid, NORM_THREADS, smem, st>>>(                                      \
+          (const uint4*)dy, (const uint4*)x, (const uint4*)gamma, stats, (const uint4*)dres, (uint4*)dx,               \
+          (float*)workspace, int(rows), int(cols), (uint4*)dbranch, drop);                                         \
+  }
   FSB_NORM_DISPATCH(L)
 #undef L
   if (e != cudaSuccess) {
@@ -414,4 +470,39 @@ extern "C" int fsb_layernorm_bwd(const void* dy, const void* x, const void* gamm
                                  fsb_stream_t st) {
   return norm_bwd<true>(dy, x, gamma, mean_rstd, dres, dx, dgamma, dbeta, wgrad_dtype, accumulate, workspace,
                         workspace_bytes, rows, cols, (cudaStream_t)st);
+}
+extern "C" int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
+                                         void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps, float p,
+                                         uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p == 0.f) return norm_fwd<true>(x, residual, gamma, beta, y, sum_out, mean_rstd, rows, cols, eps, (cudaStream_t)st);
+  FSB_REQUIRE(residual != nullptr, "layernorm_fwd_dropout: the dropped branch needs a residual");
+  FSB_REQUIRE(cols <= 8 * 256 * NORM_DROP_MAX_VPT, "layernorm_fwd_dropout: cols %ld > %d with p > 0", (long)cols,
+              8 * 256 * NORM_DROP_MAX_VPT);
+  return norm_fwd<true, true>(x, residual, gamma, beta, y, sum_out, mean_rstd, rows, cols, eps, (cudaStream_t)st, d);
+}
+extern "C" int fsb_layernorm_bwd_dropout(const void* dy, const void* x, const void* gamma, const float* mean_rstd,
+                                         const void* dres, void* dx, void* dbranch, void* dgamma, void* dbeta,
+                                         int wgrad_dtype, int accumulate, void* workspace, size_t workspace_bytes,
+                                         int64_t rows, int64_t cols, float p, uint64_t seed, const int64_t* stream_base,
+                                         int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(dbranch != nullptr && aligned16(dbranch), "layernorm_bwd_dropout: dbranch must be a 16-byte aligned buffer");
+  if (p == 0.f) {   // no mask: the branch gradient is the gradient of the sum
+    if (int rc = norm_bwd<true>(dy, x, gamma, mean_rstd, dres, dx, dgamma, dbeta, wgrad_dtype, accumulate, workspace,
+                                workspace_bytes, rows, cols, (cudaStream_t)st))
+      return rc;
+    cudaError_t e = cudaMemcpyAsync(dbranch, dx, size_t(rows) * size_t(cols) * 2, cudaMemcpyDeviceToDevice, (cudaStream_t)st);
+    if (e != cudaSuccess) {
+      set_error("layernorm_bwd_dropout: copy of dx failed: %s", cudaGetErrorString(e));
+      return FSB_ERR_CUDA;
+    }
+    return FSB_OK;
+  }
+  FSB_REQUIRE(cols <= 8 * 256 * NORM_DROP_MAX_VPT, "layernorm_bwd_dropout: cols %ld > %d with p > 0", (long)cols,
+              8 * 256 * NORM_DROP_MAX_VPT);
+  return norm_bwd<true, true>(dy, x, gamma, mean_rstd, dres, dx, dgamma, dbeta, wgrad_dtype, accumulate, workspace,
+                              workspace_bytes, rows, cols, (cudaStream_t)st, dbranch, d);
 }

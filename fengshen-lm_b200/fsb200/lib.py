@@ -15,6 +15,7 @@ c_int = ctypes.c_int
 c_i64 = ctypes.c_int64
 c_f32 = ctypes.c_float
 c_size = ctypes.c_size_t
+c_u64 = ctypes.c_uint64
 
 BF16, F32, U32, U64 = 0, 1, 2, 3
 GEMM_NT, GEMM_NN, GEMM_TN = 0, 1, 2
@@ -93,6 +94,19 @@ SIGNATURES = {
     "fsb_sdpa_bwd_workspace_bytes": (c_size, [c_i64, c_i64, c_i64, c_int]),
     "fsb_sdpa_bwd": (c_int, [c_void_p] * 10 + [c_i64, c_i64, c_i64, c_int, c_int] + [c_i64] * 16 +
                      [c_f32, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size, c_void_p]),
+    "fsb_sdpa_fwd_dropout": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_int, c_int,
+                                     c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f32, c_int, c_void_p, c_void_p,
+                                     c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_sdpa_bwd_dropout": (c_int, [c_void_p] * 10 + [c_i64, c_i64, c_i64, c_int, c_int] + [c_i64] * 16 +
+                             [c_f32, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size,
+                              c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_layernorm_fwd_dropout": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64,
+                                          c_f32, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_layernorm_bwd_dropout": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_int, c_int, c_void_p, c_size, c_i64, c_i64,
+                                          c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_dropout": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_dropout_advance": (c_int, [c_void_p, c_void_p, c_i64, c_void_p]),
     "fsb_attn_decode_workspace_bytes": (c_size, [c_i64, c_int, c_int, c_i64]),
     "fsb_attn_decode": (c_int, [c_void_p] * 5 + [c_i64, c_int, c_int, c_i64, c_void_p] + [c_i64] * 10 +
                         [c_f32, c_void_p, c_void_p, c_void_p, c_size, c_void_p]),
@@ -138,6 +152,7 @@ _NO_KERNEL = {"fsb_set_reserved_sms", "fsb_comm_unique_id", "fsb_comm_init", "fs
               "fsb_comm_all_gather", "fsb_comm_all_reduce", "fsb_index_build_sample_idx", "fsb_index_build_mapping",
               "fsb_index_build_blocks_mapping", "fsb_index_build_blending_indices", "fsb_bert_collate"}   # host-only calls / NCCL's kernels, not ours
 _KERNELS_PER_CALL = {"fsb_rmsnorm_bwd": 2, "fsb_layernorm_bwd": 2, "fsb_softmax_xent_fwd_bwd": 3, "fsb_sdpa_bwd": 3,
+                     "fsb_layernorm_bwd_dropout": 2, "fsb_sdpa_bwd_dropout": 3,
                      "fsb_sumsq": 2, "fsb_colsum": 2, "fsb_act_bwd_bias": 2, "fsb_attn_decode": 2}
 
 

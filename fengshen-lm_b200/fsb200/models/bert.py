@@ -8,7 +8,14 @@ The arithmetic restated here lives in 3P `transformers` (SURVEY.md Appendix C):
                 pooler tanh(W x[:,0]) + NSP head; loss = CE(mlm) + CE(nsp).
 Both: separate q/k/v Linear(h,h)+bias (laid out adjacently -> one [3h,h] GEMM), softmax(QK^T/sqrt(hn) + padding mask),
 LayerNorm eps 1e-12, MLM head = dense + act + LN + decoder tied to the word embeddings + bias, CE ignore_index -100.
-State-dict keys follow HF. Dropout must be 0 (rejected loudly otherwise).
+State-dict keys follow HF.
+Dropout (hidden_dropout_prob, attention_probs_dropout_prob; the two may differ) applies in training mode (`model.training`,
+also under no_grad), at HF's sites: the embeddings (BERT: after the LN; MegatronBERT: the sum, no LN), the attention
+probabilities, and the attention-output and FFN-output branches before their residual add — fused into the attention kernels
+and the LayerNorms that add the branch to the residual. Masks come from Philox (include/fsb200.h): a seed drawn once from
+torch.default_generator at construction (only when a probability is > 0) and a stream counter on the device that every training
+forward advances by its number of sites, so eager runs and replayed CUDA graphs draw the same fresh masks. In eval mode, or
+with both probabilities 0, the forward and backward are the dropout-free kernels.
 """
 import math
 from types import SimpleNamespace
@@ -52,9 +59,11 @@ class _BertFamily(nn.Module):
         self.h, self.nl, self.nh, self.V = g("hidden_size"), g("num_hidden_layers"), g("num_attention_heads"), g("vocab_size")
         self.ff, self.npos, self.ntype = g("intermediate_size"), g("max_position_embeddings", 512), g("type_vocab_size", 2)
         self.eps = g("layer_norm_eps", 1e-12)
-        for k in ("hidden_dropout_prob", "attention_probs_dropout_prob"):
-            if g(k, 0.0) not in (0, 0.0):
-                raise RuntimeError(f"fsb200 BERT: {k}={g(k)} — dropout is not implemented; set it to 0")
+        self.p_hidden = float(g("hidden_dropout_prob", 0.0) or 0.0)
+        self.p_attn = float(g("attention_probs_dropout_prob", 0.0) or 0.0)
+        for k, v in (("hidden_dropout_prob", self.p_hidden), ("attention_probs_dropout_prob", self.p_attn)):
+            if not 0.0 <= v < 1.0:
+                raise RuntimeError(f"fsb200 BERT: {k}={v} outside [0, 1)")
         act = g("hidden_act", "gelu")
         if act not in ("gelu", "gelu_new"):
             raise RuntimeError(f"fsb200 BERT: hidden_act={act!r} not implemented (gelu, gelu_new)")
@@ -126,9 +135,20 @@ class _BertFamily(nn.Module):
             self._nsp_b = torch.full((8,), -30000.0, dtype=torch.bfloat16, device=dev)
         self.reset_parameters(seed)
         self.accumulate_grads, self.loss_scale, self.grad_hook = False, 1.0, None
+        # dropout sites of one forward: 0 embeddings; for layer i, 1 + 3i attention probabilities, 2 + 3i attention output,
+        # 3 + 3i FFN output
+        self.dropout_sites = 1 + 3 * self.nl
+        self.dropout_seed, self.dropout_counter = None, None
+        if self.p_hidden > 0 or self.p_attn > 0:
+            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
+            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=dev)
 
     def P(self, name):
         return self._p[name]
+
+    def _drop(self, base, p, site):
+        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
+        return None if base is None or p == 0.0 else ops.Dropout(p, self.dropout_seed, base, site)
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -184,6 +204,11 @@ class _BertFamily(nn.Module):
         E = "bert.embeddings."
         scale = 1.0 / math.sqrt(hn)
         self._need("no_decay"); self._need("emb")
+        base = None
+        if self.training and self.dropout_seed is not None:
+            base = ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+        ph, pa = self.p_hidden, self.p_attn
+        D = lambda p, site: self._drop(base, p, site)
         emb = ops.embedding_fwd(ids, P(E + "word_embeddings.weight").data, pos=pos,
                                 P=P(E + "position_embeddings.weight").data, token_type=tt,
                                 T=P(E + "token_type_embeddings.weight").data, seq_len=S)
@@ -193,26 +218,31 @@ class _BertFamily(nn.Module):
         else:
             x, st_e, _ = ops.layernorm_fwd(emb, P(E + "LayerNorm.weight").data, P(E + "LayerNorm.bias").data, self.eps)
             emb_ctx = (emb, st_e)
+        if D(ph, 0) is not None:
+            x = ops.dropout(x, D(ph, 0))
         for i in range(self.nl):
             p = f"bert.encoder.layer.{i}."
             self._need(f"layer{i}")
             if pre:
                 h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, P(p + "attention.ln.weight").data,
                                                P(p + "attention.ln.bias").data, self.eps,
-                                               residual=None if prev_m is None else x)
+                                               residual=None if prev_m is None else x,
+                                               drop=None if prev_m is None else D(ph, 3 * i))   # layer i-1's FFN output
                 attn_in = h1
             else:
                 attn_in = x
             qkv = ops.gemm(L.GEMM_NT, attn_in, self._wqkv[i], bias=self._bqkv[i])
             q5 = qkv.view(B, S, 3, nh, hn)
-            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, False, kv_mask=mask)
+            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, False, kv_mask=mask, drop=D(pa, 1 + 3 * i))
             a = ops.gemm(L.GEMM_NT, o.view(T, h), P(p + "attention.output.dense.weight").data,
                          bias=P(p + "attention.output.dense.bias").data)
             if pre:
-                h2, st2, x1 = ops.layernorm_fwd(a, P(p + "ln.weight").data, P(p + "ln.bias").data, self.eps, residual=x)
+                h2, st2, x1 = ops.layernorm_fwd(a, P(p + "ln.weight").data, P(p + "ln.bias").data, self.eps, residual=x,
+                                                drop=D(ph, 2 + 3 * i))
             else:
                 h2, st2, x1 = ops.layernorm_fwd(a, P(p + "attention.output.LayerNorm.weight").data,
-                                                P(p + "attention.output.LayerNorm.bias").data, self.eps, residual=x)
+                                                P(p + "attention.output.LayerNorm.bias").data, self.eps, residual=x,
+                                                drop=D(ph, 2 + 3 * i))
             prea = torch.empty((T, self.ff), dtype=torch.bfloat16, device=x.device) if save else None
             f = ops.gemm(L.GEMM_NT, h2, P(p + "intermediate.dense.weight").data, bias=P(p + "intermediate.dense.bias").data,
                          epilogue=self.epi, aux=prea)
@@ -223,14 +253,15 @@ class _BertFamily(nn.Module):
                 x, prev_m = x1, m
             else:
                 xo, st3, s2 = ops.layernorm_fwd(m, P(p + "output.LayerNorm.weight").data,
-                                                P(p + "output.LayerNorm.bias").data, self.eps, residual=h2)
+                                                P(p + "output.LayerNorm.bias").data, self.eps, residual=h2,
+                                                drop=D(ph, 3 + 3 * i))
                 if save:
                     acts.append((x, qkv, o, lse, x1, st2, h2, prea, f, s2, st3))
                 x = xo
         self._need("head")
         if pre:
             hf, stf, xf = ops.layernorm_fwd(prev_m, P("bert.encoder.ln.weight").data, P("bert.encoder.ln.bias").data,
-                                            self.eps, residual=x)
+                                            self.eps, residual=x, drop=D(ph, 3 * self.nl))
         else:
             hf, stf, xf = x, None, None
         # MLM head: dense + act + LN + tied decoder + bias (on every position)
@@ -263,13 +294,23 @@ class _BertFamily(nn.Module):
                 loss = loss + nloss                               # modeling_megatron_bert.py:776-779
                 nsp_logits = keep_nsp
             if save:
-                ctx = (acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S)
+                ctx = (acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base)
                 logits = keep
         return loss, (logits if want_logits else None), nsp_logits, ctx
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S = ctx
+        acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base = ctx
+        ph, pa = self.p_hidden, self.p_attn
+        D = lambda p, site: self._drop(base, p, site)
+
+        def ln_bwd(dy, x, w, b, st, drop, dres=None):
+            """(gradient of the LN input sum, gradient of its dropped branch) — the same tensor without dropout."""
+            if drop is None:
+                d = ops.layernorm_bwd(dy, x, w.data, st, w.main_grad, b.main_grad, accumulate=acc, dres=dres)
+                return d, d
+            return ops.layernorm_bwd_dropout(dy, x, w.data, st, w.main_grad, b.main_grad, drop, accumulate=acc, dres=dres)
+
         h, nh, hn, pre = self.h, self.nh, self.hn, self.PRE_LN
         T = B * S
         P = self.P
@@ -317,7 +358,7 @@ class _BertFamily(nn.Module):
         self._done("head")
         if pre:
             ew, eb = P("bert.encoder.ln.weight"), P("bert.encoder.ln.bias")
-            dx = ops.layernorm_bwd(dhf, xf, ew.data, stf, ew.main_grad, eb.main_grad, accumulate=acc)
+            dx, dmb = ln_bwd(dhf, xf, ew, eb, stf, D(ph, 3 * self.nl))
         else:
             dx = dhf
         for i in reversed(range(self.nl)):
@@ -327,11 +368,11 @@ class _BertFamily(nn.Module):
             wo, bo = P(p + "attention.output.dense.weight"), P(p + "attention.output.dense.bias")
             if pre:
                 x, st1, h1, qkv, o, lse, x1, st2, h2, prea, f = acts[i]
-                dm, dres_in = dx, dx                       # x_next = x1 + m
+                dm, dres_in = dmb, dx                      # x_next = x1 + drop(m)
             else:
                 x, qkv, o, lse, x1, st2, h2, prea, f, s2, st3 = acts[i]
                 lw, lb = P(p + "output.LayerNorm.weight"), P(p + "output.LayerNorm.bias")
-                dm = ops.layernorm_bwd(dx, s2, lw.data, st3, lw.main_grad, lb.main_grad, accumulate=acc)  # d(h2 + m)
+                dsum, dm = ln_bwd(dx, s2, lw, lb, st3, D(ph, 3 + 3 * i))   # d(h2 + drop(m)), d(m)
                 dres_in = None
             acts[i] = None
             df = ops.gemm(L.GEMM_NN, dm, w2.data)
@@ -342,30 +383,32 @@ class _BertFamily(nn.Module):
             if pre:
                 dh2 = ops.gemm(L.GEMM_NN, dprea, w1.data)
                 lw, lb = P(p + "ln.weight"), P(p + "ln.bias")
-                dx1 = ops.layernorm_bwd(dh2, x1, lw.data, st2, lw.main_grad, lb.main_grad, accumulate=acc, dres=dres_in)
-                da = dx1
+                dx1, da = ln_bwd(dh2, x1, lw, lb, st2, D(ph, 2 + 3 * i), dres=dres_in)
             else:
-                ops.gemm(L.GEMM_NN, dprea, w1.data, out=dm, accumulate=True)      # dh2 = d(h2+m) + dgrad(fc1)
+                ops.gemm(L.GEMM_NN, dprea, w1.data, out=dsum, accumulate=True)    # dh2 = d(h2+m) + dgrad(fc1)
                 lw, lb = P(p + "attention.output.LayerNorm.weight"), P(p + "attention.output.LayerNorm.bias")
-                da = ops.layernorm_bwd(dm, x1, lw.data, st2, lw.main_grad, lb.main_grad, accumulate=acc)  # d(x + a)
+                dsum, da = ln_bwd(dsum, x1, lw, lb, st2, D(ph, 2 + 3 * i))       # d(x + drop(a)), d(a)
             do = ops.gemm(L.GEMM_NN, da, wo.data)
             ops.gemm(L.GEMM_TN, da, o.view(T, h), out=wo.main_grad, accumulate=acc)
             ops.colsum(da, bo.main_grad, accumulate=acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, False,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask)
+                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
             attn_in = h1 if pre else x
             ops.gemm(L.GEMM_TN, dqkv, attn_in, out=self._dwqkv[i], accumulate=acc)
             ops.colsum(dqkv, self._dbqkv[i], accumulate=acc)
             if pre:
                 dh1 = ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i])
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")
-                dx = ops.layernorm_bwd(dh1, x, lw.data, st1, lw.main_grad, lb.main_grad, accumulate=acc, dres=dx1)
+                # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped FFN output into x
+                dx, dmb = ln_bwd(dh1, x, lw, lb, st1, D(ph, 3 * i) if i > 0 else None, dres=dx1)
             else:
-                ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i], out=da, accumulate=True)  # dx_in = d(x+a) + dgrad(qkv)
-                dx = da
+                ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i], out=dsum, accumulate=True)  # dx_in = d(x+a) + dgrad(qkv)
+                dx = dsum
             self._done(f"layer{i}")
+        if D(ph, 0) is not None:
+            dx = ops.dropout(dx, D(ph, 0))
         if not pre:
             emb, st_e = emb_ctx
             lw, lb = P(E + "LayerNorm.weight"), P(E + "LayerNorm.bias")

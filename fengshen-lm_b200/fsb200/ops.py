@@ -149,14 +149,19 @@ def rmsnorm_bwd(dy, x, scale, rstd, dscale_out, accumulate=False, dres=None):
     return dx
 
 
-def layernorm_fwd(x, gamma, beta, eps, residual=None):
+def layernorm_fwd(x, gamma, beta, eps, residual=None, drop=None):
+    """drop: optional Dropout (see `Dropout`): x_sum = dropout(x) + residual (the dropped branch of a residual block)."""
     _chk(x, _bf16, "x"); _chk(gamma, _bf16, "gamma"); _chk(beta, _bf16, "beta")
     rows, cols = x.shape
     y = torch.empty_like(x)
     stats = torch.empty(rows, 2, dtype=torch.float32, device=x.device)
     xs = torch.empty_like(x) if residual is not None else None
-    L.call("fsb_layernorm_fwd", _p(x), _p(residual), _p(gamma), _p(beta), _p(y), _p(xs), _p(stats), rows, cols,
-           float(eps), _stream())
+    if drop is None:
+        L.call("fsb_layernorm_fwd", _p(x), _p(residual), _p(gamma), _p(beta), _p(y), _p(xs), _p(stats), rows, cols,
+               float(eps), _stream())
+    else:
+        L.call("fsb_layernorm_fwd_dropout", _p(x), _p(residual), _p(gamma), _p(beta), _p(y), _p(xs), _p(stats), rows, cols,
+               float(eps), *drop.args(), _stream())
     return y, stats, (xs if residual is not None else x)
 
 
@@ -169,6 +174,58 @@ def layernorm_bwd(dy, x, gamma, stats, dgamma_out, dbeta_out, accumulate=False, 
            L.F32 if dgamma_out.dtype == torch.float32 else L.BF16, int(bool(accumulate)), _p(ws), ws.numel(), rows, cols,
            _stream())
     return dx
+
+
+def layernorm_bwd_dropout(dy, x, gamma, stats, dgamma_out, dbeta_out, drop, accumulate=False, dres=None):
+    """Backward of layernorm_fwd(..., residual, drop): returns (dx, dbranch) — the gradient of the sum (= of the residual)
+    and the gradient of the dropped branch, dx * Z / (1 - p)."""
+    rows, cols = x.shape
+    dx = torch.empty_like(x)
+    dbranch = torch.empty_like(x)
+    nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 1)
+    ws = workspace(nbytes, x.device, "norm")
+    L.call("fsb_layernorm_bwd_dropout", _p(dy), _p(x), _p(gamma), _p(stats), _p(dres), _p(dx), _p(dbranch), _p(dgamma_out),
+           _p(dbeta_out), L.F32 if dgamma_out.dtype == torch.float32 else L.BF16, int(bool(accumulate)), _p(ws), ws.numel(),
+           rows, cols, *drop.args(), _stream())
+    return dx, dbranch
+
+
+# ------------------------------------------------------------------------------------------------------ dropout
+class Dropout:
+    """One dropout site of one forward: probability p, the model's seed, the forward's stream base (int64 [1] on the
+    device, from dropout_advance) and the site number. The keep mask is a function of these and of the element's coordinates
+    only (include/fsb200.h), so the backward passes the same object."""
+    __slots__ = ("p", "seed", "base", "site")
+
+    def __init__(self, p, seed, base, site):
+        if not 0.0 <= float(p) < 1.0:
+            raise RuntimeError(f"fsb200 dropout: p = {p} outside [0, 1)")
+        _chk(base, torch.int64, "dropout stream base")
+        self.p, self.seed, self.base, self.site = float(p), int(seed), base, int(site)
+
+    def args(self):
+        return self.p, self.seed, _p(self.base), self.site
+
+
+def dropout_advance(counter, n):
+    """Advance the device stream counter (int64 [1]) by n streams, on the device; returns the base this forward uses (a new
+    int64 [1] device tensor, saved with the activations for the backward)."""
+    _chk(counter, torch.int64, "dropout counter")
+    saved = torch.empty(1, dtype=torch.int64, device=counter.device)
+    L.call("fsb_dropout_advance", _p(counter), _p(saved), int(n), _stream())
+    return saved
+
+
+def dropout(x, drop, out=None):
+    """out = x * Z / (1 - p) over bf16 [rows, cols]; also the backward (pass dy, get dx)."""
+    _chk(x, _bf16, "x")
+    rows, cols, ld = _rows2d(x, "x")
+    if ld != cols:
+        raise RuntimeError("fsb200 dropout: x must be contiguous")
+    if out is None:
+        out = torch.empty_like(x)
+    L.call("fsb_dropout", _p(x), _p(out), rows, cols, *drop.args(), _stream())
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------ pointwise
@@ -332,9 +389,10 @@ def _chk_rel(rel, H, Sq, Skv, name):
                            f"got {tuple(rel.shape)}")
 
 
-def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None):
+def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop=None):
     """q,k,v: strided [B,S,H,D] bf16 views (e.g. slices of the packed QKV projection). Returns (out [B,Sq,H,D], lse).
-    rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias over the offset k - q (T5 relative-position bias)."""
+    rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias over the offset k - q (T5 relative-position bias).
+    drop: optional Dropout on the attention probabilities (not with causal or rel_bias when p > 0)."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -349,8 +407,12 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None):
             raise RuntimeError("fsb200: kv_mask must be contiguous uint8 [batch, seq_kv]")
     if rel_bias is not None:
         _chk_rel(rel_bias, H, Sq, Skv, "rel_bias")
-    L.call("fsb_sdpa_fwd", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs,
-           v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _stream())
+    if drop is None:
+        L.call("fsb_sdpa_fwd", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs,
+               v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _stream())
+    else:
+        L.call("fsb_sdpa_fwd_dropout", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs,
+               k_hs, v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), *drop.args(), _stream())
     return out, lse
 
 
@@ -394,9 +456,10 @@ def attn_decode(q, k_cache, v_cache, kv_len, scale, kv_mask=None, rel_bias=None,
     return out, lse
 
 
-def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None):
+def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None, drop=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
-    rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=), deterministically."""
+    rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=), deterministically.
+    drop: the forward's Dropout (same seed, base and site)."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")
@@ -415,6 +478,10 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
         _chk_rel(drel_bias, H, Sq, Skv, "drel_bias")
         ws_bytes = int(L.load().fsb_sdpa_bwd_workspace_bytes(B, Sq, Skv, H))
         ws = workspace(ws_bytes, q.device, "sdpa_dbias")
-    L.call("fsb_sdpa_bwd", _p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv,
-           H, D, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs,
-           float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes, _stream())
+    args = (_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv,
+            H, D, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs,
+            float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes)
+    if drop is None:
+        L.call("fsb_sdpa_bwd", *args, _stream())
+    else:
+        L.call("fsb_sdpa_bwd_dropout", *args, *drop.args(), _stream())

@@ -70,10 +70,14 @@ class PretrainStep:
         eng = self.engine
         if self.cuda_graph:
             if self._graph is None:
-                snap = (eng.master.clone(), eng.exp_avg.clone(), eng.exp_avg_sq.clone(), self.model.flat.params.clone())
+                state = [eng.master, eng.exp_avg, eng.exp_avg_sq, self.model.flat.params]
+                counter = getattr(self.model, "dropout_counter", None)
+                if counter is not None:    # the dropout stream counter advances on the device in every training forward
+                    state.append(counter)
+                snap = [t.clone() for t in state]
                 self._capture(device_batches)
-                for dst, src in zip((eng.master, eng.exp_avg, eng.exp_avg_sq, self.model.flat.params), snap):
-                    dst.copy_(src)     # the warm-up + capture passes must leave no trace in the optimizer state
+                for dst, src in zip(state, snap):
+                    dst.copy_(src)     # the warm-up + capture passes must leave no trace in the optimizer or dropout state
             for dst, src in zip(self._static, device_batches):
                 for k, v in src.items():
                     dst[k].copy_(v, non_blocking=True)

@@ -240,6 +240,56 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
                  float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                  void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- dropout (BERT / MegatronBERT training) -------------------------------------------------------------------------
+ * torch.nn.functional.dropout semantics: an element is dropped with probability p and every kept element is scaled by
+ * 1 / (1 - p). The keep bit is a pure function of (seed, stream, coordinates) through Philox4x32-10 (Random123; key =
+ * (seed & 0xffffffff, seed >> 32)), so no mask is stored: the backward kernels regenerate it.
+ *   threshold : thr = floor(p * 256 + 0.5) (fp32 arithmetic); an element whose 8-bit random value r < thr is dropped. The
+ *               effective rate thr / 256 is within 2^-9 of p. p outside [0, 1) is an error; p == 0 runs the kernels without
+ *               dropout (fsb_sdpa_fwd, fsb_layernorm_fwd, ...) and does not read the stream counter.
+ *   stream    : s = *stream_base + site (int64 read on the device; per-site stream numbers of one forward).
+ *   hidden    : element (row, col): counter (col / 16, row, s & 0xffffffff, s >> 32); r = byte (col % 16) % 4 (bits 8 (col % 4))
+ *               of output word (col % 16) / 4.
+ *   attention : element (b, head, q, k) with q = 16 qa + 8 qh + 2 qs + qp and k = 16 ka + 8 kh + 2 ks + kp:
+ *               counter ((4 ka + ks) | (4 qa + qs) << 16, b * nheads + head, s & 0xffffffff, s >> 32); r = byte 2 qh + kh of
+ *               output word 2 qp + kp. seq_q, seq_kv <= 65536.
+ * fsb_sdpa_fwd_dropout / fsb_sdpa_bwd_dropout: fsb_sdpa_fwd / fsb_sdpa_bwd with dropout on the attention probabilities,
+ *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. With p > 0, causal and
+ *   rel_bias are rejected. The backward must get the forward's seed, stream_base value and site.
+ * fsb_layernorm_fwd_dropout: fsb_layernorm_fwd with sum_out = x * Z / (1 - p) + residual (residual required when p > 0): the
+ *   dropped branch of a residual block. With p > 0 both LayerNorm entries take cols <= 12288. fsb_layernorm_bwd_dropout: fsb_layernorm_bwd that also writes dbranch = dx * Z / (1 - p)
+ *   (dx already includes dres), the gradient of the branch x, beside dx, the gradient of the sum (and of the residual).
+ * fsb_dropout: y = x * Z / (1 - p) over bf16 [rows, cols] (cols % 8 == 0, rows < 2^32); also the backward (dx = dy * Z / (1 - p)).
+ *   x == y is allowed.
+ * fsb_dropout_advance: *saved = *stream_base; *stream_base += n (one thread on the device). A training forward calls it once
+ *   and hands `saved` to every dropout call of that forward and of its backward, so a replayed CUDA graph draws new masks. */
+int fsb_sdpa_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse,
+                         int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                         int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                         int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                         float scale, int causal, const uint8_t* kv_mask, const float* rel_bias,
+                         float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                         const float* lse, float* delta, void* dq, void* dk, void* dv,
+                         int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                         int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                         int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                         int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                         int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                         float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
+                         void* workspace, size_t workspace_bytes,
+                         float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
+                              void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
+                              float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_layernorm_bwd_dropout(const void* dy, const void* x, const void* gamma, const float* mean_rstd, const void* dres,
+                              void* dx, void* dbranch, void* dgamma, void* dbeta, int wgrad_dtype, int accumulate,
+                              void* workspace, size_t workspace_bytes, int64_t rows, int64_t cols,
+                              float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_dropout(const void* x, void* y, int64_t rows, int64_t cols, float p, uint64_t seed, const int64_t* stream_base,
+                int64_t site, fsb_stream_t stream);
+int fsb_dropout_advance(int64_t* stream_base, int64_t* saved, int64_t n, fsb_stream_t stream);
+
 /* ---- decode attention over a KV cache (split-KV) -------------------------------------------------------------------
  * One query row per (batch, head) — the newest token of a generation step, at cache slot *kv_len - 1 — attends to the cache
  * slots [0, *kv_len):  O = softmax(scale * q.K^T + bias + mask) V. kv_len is a DEVICE int32 scalar, clamped to [0, kv_cap];

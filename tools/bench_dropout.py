@@ -1,0 +1,136 @@
+"""Cost of dropout on an H100: attention forward / backward device time with p = 0 and p = 0.1, and BERT / MegatronBERT
+training-step throughput with dropout-0 and dropout-0.1 configs, alternated in one process (median of 3 windows each). Attention times are kernel
+times from torch.profiler; step throughput is wall time over device-synchronised windows.
+
+    python tools/bench_dropout.py [--steps 20] [--out result.json]
+
+Shapes: C3 attention = micro-batch 32 x 512, 32 heads, head dim 64; C1 attention = 8 x 128, 12 heads. Steps: C1 = BERT-base
+(12 layers, hidden 768) at 8 x 128; C3 = the Erlangshen MegatronBERT width (hidden 2048, 32 heads) at 32 x 512 with 4 layers
+(the full 24-layer model's optimizer state and activations are not needed to price the per-layer dropout work). Prints one
+JSON line; card name and power limit come from nvidia-smi in the same process."""
+import argparse
+import json
+import math
+import os
+import statistics
+import subprocess
+import sys
+from types import SimpleNamespace
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "fengshen-lm_b200"))
+
+import torch  # noqa: E402
+
+from fsb200 import ops  # noqa: E402
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+
+
+def kernel_ms(fn, iters):
+    """Device time per call of the attention kernels fn launches (attn_fwd / attn_delta / attn_bwd_dq / attn_bwd_dkv), from
+    torch.profiler's CUDA activity records: kernel execution only, not the host time of the call."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+    us = 0.0
+    for evt in prof.key_averages():
+        if "attn_" in evt.key:
+            us += getattr(evt, "self_device_time_total", None) or evt.self_cuda_time_total
+    if us == 0.0:
+        raise RuntimeError("bench_dropout: the profiler recorded no attention kernel")
+    return us / 1e3 / iters
+
+
+def attention(B, S, H, D, iters=50):
+    g = torch.Generator().manual_seed(0)
+    qkv = torch.randn(B, S, 3, H, D, generator=g).to(torch.bfloat16).cuda()
+    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+    dout = torch.randn(B, S, H, D, generator=g).to(torch.bfloat16).cuda()
+    mask = torch.ones(B, S, dtype=torch.uint8, device="cuda")
+    mask[:, S - S // 8:] = 0
+    dq = torch.empty_like(qkv)
+    base = torch.zeros(1, dtype=torch.int64, device="cuda")
+    scale = 1.0 / math.sqrt(D)
+    res = {}
+    for _ in range(3):   # alternate p = 0 / 0.1 windows
+        for p in (0.0, 0.1):
+            drop = None if p == 0 else ops.Dropout(p, 1, base, 0)
+            o, lse = ops.sdpa_fwd(q, k, v, scale, False, kv_mask=mask, drop=drop)
+            f = kernel_ms(lambda: ops.sdpa_fwd(q, k, v, scale, False, kv_mask=mask, drop=drop), iters)
+            b = kernel_ms(lambda: ops.sdpa_bwd(q, k, v, o, dout, lse, scale, False, dq[:, :, 0], dq[:, :, 1], dq[:, :, 2],
+                                             kv_mask=mask, drop=drop), iters)
+            res.setdefault(p, []).append((f, b))
+    return {f"p={p}": {"fwd_ms": statistics.median(x[0] for x in v), "bwd_ms": statistics.median(x[1] for x in v)}
+            for p, v in res.items()}
+
+
+def step_throughput(kind, B, S, steps):
+    from fsb200.models.bert import BertForMaskedLM, MegatronBertForPreTraining
+    from fsb200.trainer import PretrainStep
+    if kind == "C1":
+        cfg = dict(vocab_size=21128, hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
+                   max_position_embeddings=512, type_vocab_size=2, hidden_act="gelu", layer_norm_eps=1e-12)
+        cls = BertForMaskedLM
+    else:
+        cfg = dict(vocab_size=21248, hidden_size=2048, num_hidden_layers=4, num_attention_heads=32, intermediate_size=8192,
+                   max_position_embeddings=512, type_vocab_size=2, hidden_act="gelu_new", layer_norm_eps=1e-12)
+        cls = MegatronBertForPreTraining
+    g = torch.Generator().manual_seed(1)
+    ids = torch.randint(1, cfg["vocab_size"], (B, S), generator=g)
+    labels = torch.where(torch.rand(B, S, generator=g) < 0.15, ids, torch.full_like(ids, -100))
+    batch = {"input_ids": ids.cuda(), "token_type_ids": torch.zeros_like(ids).cuda(), "labels": labels.cuda()}
+    if kind == "C3":
+        batch["next_sentence_label"] = torch.randint(0, 2, (B,), generator=g).cuda()
+    runs = {}
+    for p in (0.0, 0.1):
+        torch.manual_seed(0)
+        model = cls(SimpleNamespace(hidden_dropout_prob=p, attention_probs_dropout_prob=p, **cfg), device="cuda")
+        runs[p] = PretrainStep(model, lambda s_: 1e-4, lr=1e-4, weight_decay=0.01, grad_clip=1.0)
+        for _ in range(3):
+            runs[p].step_device([batch])
+    torch.cuda.synchronize()
+    res = {}
+    for _ in range(3):
+        for p in (0.0, 0.1):
+            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev0.record()
+            for _ in range(steps):
+                runs[p].step_device([batch])
+            ev1.record()
+            torch.cuda.synchronize()
+            res.setdefault(p, []).append(B * S * steps / (ev0.elapsed_time(ev1) / 1e3))
+    del runs
+    torch.cuda.empty_cache()
+    return {f"p={p}": {"tokens_per_s": statistics.median(v)} for p, v in res.items()}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_dropout: needs a GPU (no CPU timing is meaningful)")
+    out = {"card": card(),
+           "attention_C3_32x512_h32_d64": attention(32, 512, 32, 64),
+           "attention_C1_8x128_h12_d64": attention(8, 128, 12, 64),
+           "step_C1_bert_base_8x128": step_throughput("C1", 8, 128, a.steps),
+           "step_C3_width_4_layers_32x512": step_throughput("C3", 32, 512, max(3, a.steps // 4))}
+    line = json.dumps(out)
+    print(line)
+    if a.out:
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
