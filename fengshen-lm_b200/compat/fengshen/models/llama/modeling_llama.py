@@ -5,6 +5,7 @@ import os
 
 import torch
 
+from fsb200.models.export import wait_params
 from fsb200.models.llama import LlamaForCausalLM as _FsbLlama
 from .configuration_llama import LlamaConfig
 
@@ -49,9 +50,6 @@ class LlamaForCausalLM(_FsbLlama):
         model): config.json + pytorch_model.bin in the reference's key layout; `from_pretrained(path)` reads it back, and
         `fengshen.utils.llama_convert.fs_to_hf_state_dict` turns it into a transformers LLaMA checkpoint."""
         from fengshen.utils.llama_convert import save_pretrained_fs
-        hook = getattr(self, "param_hook", None)
-        eng = getattr(hook, "__self__", None)
-        if eng is not None and hasattr(eng, "wait_params"):
-            eng.wait_params()
+        wait_params(self)
         cfg = self.config.to_dict() if hasattr(self.config, "to_dict") else vars(self.config)
         save_pretrained_fs({k: v for k, v in self.state_dict().items()}, cfg, path)

@@ -1,0 +1,162 @@
+"""What the fsb200 model classes share with the ZeRO engine (fsb200/engine.py) and with each other, so that a model file holds
+only its own maths:
+  * parameters are views into one flat bf16 buffer (fsb200/flat.py), registered under the HF dotted names of the class the
+    model stands in for, each with `.main_grad` over its slice of the flat gradient buffer;
+  * the engine drives a model through `param_hook` / `grad_hook` / `backward_begin_hook`, `accumulate_grads` and `loss_scale`;
+  * a training forward is ONE autograd node: it runs the model's `_forward_impl(save=True)` and `loss.backward()` runs its
+    hand-written `_backward_impl`, which writes every gradient into the flat gradient buffer."""
+import torch
+from torch import nn
+
+from .. import ops
+from ..flat import FlatBuffers
+from . import export
+
+
+class _Holder(nn.Module):
+    """Bare container so that named_parameters() / state_dict() reproduce the reference's key names."""
+
+
+def bind_flat_parameters(module, flat):
+    """Register every entry of `flat` on `module`, in flat-layout order, as an nn.Parameter over its view with `.main_grad`
+    over its gradient view, under its dotted name: `a.b.weight` becomes module.a.b.weight, and an integer component an
+    nn.ModuleList entry (`transformer.h.3.*` -> module.transformer.h[3]). The parameters are also kept by name in module._p."""
+    module._p = {}
+    for name in flat.offsets:
+        prm = nn.Parameter(flat.view(name))
+        prm.main_grad = flat.view(name, grad=True)
+        module._p[name] = prm
+        parts = name.split(".")
+        mod = module
+        for part, nxt in zip(parts[:-1], parts[1:]):
+            if part not in mod._modules:   # a ModuleList's entries are named "0", "1", ...: they arrive in index order
+                mod.add_module(part, nn.ModuleList() if nxt.isdigit() else _Holder())
+            mod = mod._modules[part]
+        setattr(mod, parts[-1], prm)
+
+
+def flat_ids(t, dev):
+    """Integer inputs (token ids, labels, position or token-type ids) as contiguous int64 [B * S] on `dev`; None stays None."""
+    return None if t is None else t.to(device=dev, dtype=torch.int64).contiguous().view(-1)
+
+
+def key_mask(attention_mask, dev):
+    """The attention kernels' key-padding mask: uint8 [B, S] on `dev`, or None when there is no mask or no padding."""
+    if attention_mask is None or bool(attention_mask.all()):
+        return None
+    return attention_mask.to(device=dev, dtype=torch.uint8).contiguous()
+
+
+def learned_pos_emb_bwd(pos, dx, grad, B, S, accumulate):
+    """Gradient of a learned absolute position table ([positions, h], `grad` = its main_grad) from the gradient dx [B * S, h]
+    of the embedding sum. Without position ids row s is sum_b dx[b, s] (a column sum of dx viewed as [B, S * h]); with them,
+    a scatter-add by id. Rows no token used are zeroed unless gradients accumulate."""
+    if pos is None:
+        ops.colsum(dx.view(B, S * grad.shape[1]), grad[:S].reshape(-1), accumulate=accumulate)
+        if not accumulate and S < grad.shape[0]:
+            grad[S:].zero_()
+    else:
+        if not accumulate:
+            grad.zero_()
+        ops.embedding_bwd(pos, dx, grad)
+
+
+class FlatModel(nn.Module):
+    """Base of the fsb200 model classes. A subclass parses its config, builds its FlatSpec, calls `_bind_flat`, and implements
+    `_forward_impl(*inputs, save, want_logits) -> (loss, *outputs, saved)` and `_backward_impl(saved, gloss)`."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = config
+        self.accumulate_grads = False   # set by the engine for micro-batches after the first
+        self.loss_scale = 1.0           # 1 / (gradient_accumulation_steps * world_size), folded into dlogits
+        self.grad_hook = None           # engine callback: grad_hook(bucket) when a bucket's gradients are final
+
+    def _bind_flat(self, spec, device=None, world_size=None, tp=1):
+        """Allocate the flat buffers for `spec` and bind every entry. `world_size` is the data-parallel size the buckets are
+        padded for: by default the initialised process group's size over the tensor-parallel size `tp`."""
+        if world_size is None:   # laid out for the job's data-parallel world (the scripts build the model in setup())
+            import torch.distributed as dist
+            world_size = (dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1) // tp
+        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}"
+                           if torch.cuda.is_available() else "cuda")
+        if dev.type != "cuda":
+            raise RuntimeError(f"fsb200 {type(self).__name__} runs on CUDA only (no CPU fallback on the product path)")
+        self.flat = FlatBuffers(spec, dev, world_size=world_size)
+        bind_flat_parameters(self, self.flat)
+
+    def P(self, name):
+        return self._p[name]
+
+    # The reference scripts call `.from_pretrained(..., torch_dtype=torch.half).cuda()`; parameters here are views into the
+    # flat bf16 CUDA buffer and must never be re-allocated by nn.Module._apply.
+    def cuda(self, device=None):
+        return self
+
+    def half(self):
+        return self
+
+    def bfloat16(self):
+        return self
+
+    def to(self, *args, **kwargs):
+        return self
+
+    @torch.no_grad()
+    def load_reference_state_dict(self, sd):
+        """Copy a reference state dict (HF key names; fp32 / fp16 / bf16 tensors on any device) into the parameters. Every
+        parameter's key must be present with its shape; other keys (tied aliases, buffers) are ignored."""
+        for k, prm in self._p.items():
+            if k not in sd:
+                raise KeyError(f"missing key in state dict: {k}")
+            if tuple(sd[k].shape) != tuple(prm.shape):
+                raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(prm.shape)}")
+        for k, prm in self._p.items():
+            prm.copy_(sd[k].to(device=prm.device, dtype=prm.dtype))
+
+    def save_pretrained(self, path, **_):
+        """HF-style export (config.json + pytorch_model.bin with this class's HF key names): fsb200/models/export.py."""
+        export.save_pretrained(self, path)
+
+    # ---- engine hooks -----------------------------------------------------------------------------------------------
+    def _need(self, bucket):
+        """Forward is about to read this bucket's parameters (the engine may still be all-gathering them)."""
+        hook = getattr(self, "param_hook", None)
+        if hook is not None:
+            hook(bucket)
+
+    def _done(self, bucket):
+        """This bucket's gradients are final. A bucket the layout lacks (mT5's "head" with a tied LM head) is skipped."""
+        if self.grad_hook is not None and bucket in self.flat.bucket_index:
+            self.grad_hook(bucket)
+
+    def _begin_backward(self):
+        hook = getattr(self, "backward_begin_hook", None)
+        if hook is not None:
+            hook()
+
+    # ---- forward ----------------------------------------------------------------------------------------------------
+    def _step_or_forward(self, has_labels, want_logits, *inputs):
+        """-> (loss, *outputs). With labels under grad mode, the step node: `loss.backward()` then runs `_backward_impl`.
+        Otherwise a forward that keeps no activations (and always returns the logits)."""
+        if has_labels and torch.is_grad_enabled():
+            return _Step.apply(self, want_logits, next(iter(self._p.values())), *inputs)
+        return self._forward_impl(*inputs, save=False, want_logits=True)[:-1]
+
+
+class _Step(torch.autograd.Function):
+    """The whole network as one autograd node. `anchor`, a parameter, makes the node differentiable; its .grad is never
+    materialised: the kernels write the gradients into model.flat.grads."""
+
+    @staticmethod
+    def forward(ctx, model, want_logits, anchor, *inputs):
+        loss, *outputs, saved = model._forward_impl(*inputs, save=True, want_logits=want_logits)
+        ctx.model, ctx.saved, ctx.n_args = model, saved, 3 + len(inputs)
+        ctx.mark_non_differentiable(*[t for t in outputs if t is not None])
+        return (loss, *outputs)
+
+    @staticmethod
+    def backward(ctx, gloss, *_):
+        saved, ctx.saved = ctx.saved, None
+        ctx.model._backward_impl(saved, gloss)
+        return (None,) * ctx.n_args

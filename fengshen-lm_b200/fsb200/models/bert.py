@@ -21,40 +21,18 @@ import math
 from types import SimpleNamespace
 
 import torch
-from torch import nn
 
 from .. import lib as L
 from .. import ops
-from ..flat import FlatBuffers, FlatSpec
+from ..flat import FlatSpec
+from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd
 
 
-class _Holder(nn.Module):
-    pass
-
-
-def _set(root, dotted, value):
-    parts = dotted.split(".")
-    mod = root
-    for p in parts[:-1]:
-        if not hasattr(mod, p):
-            setattr(mod, p, nn.ModuleList() if False else _Holder())
-        mod = getattr(mod, p)
-    setattr(mod, parts[-1], value)
-
-
-class _BertFamily(nn.Module):
+class _BertFamily(FlatModel):
     PRE_LN = False
 
     def __init__(self, config, device=None, world_size=None, seed=0):
-        super().__init__()
-        self.config = config
-        if world_size is None:
-            import torch.distributed as dist
-            world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}"
-                           if torch.cuda.is_available() else "cuda")
-        if dev.type != "cuda":
-            raise RuntimeError("fsb200 BERT models run on CUDA only (no CPU fallback on the product path)")
+        super().__init__(config)
         g = lambda k, d=None: getattr(config, k, d)
         self.h, self.nl, self.nh, self.V = g("hidden_size"), g("num_hidden_layers"), g("num_attention_heads"), g("vocab_size")
         self.ff, self.npos, self.ntype = g("intermediate_size"), g("max_position_embeddings", 512), g("type_vocab_size", 2)
@@ -109,19 +87,8 @@ class _BertFamily(nn.Module):
         spec.add("cls.predictions.transform.LayerNorm.bias", (h,), "head")
         if pre:
             spec.add("cls.seq_relationship.weight", (2, h), "head"); spec.add("cls.seq_relationship.bias", (2,), "head")
-        self.flat = FlatBuffers(spec, dev, world_size=world_size)
-        self._p = {}
-        for name in self.flat.offsets:
-            prm = nn.Parameter(self.flat.view(name), requires_grad=True)
-            prm.main_grad = self.flat.view(name, grad=True)
-            self._p[name] = prm
-            parts = name.split(".")
-            mod = self
-            for j, part in enumerate(parts[:-1]):
-                if not hasattr(mod, part):
-                    setattr(mod, part, _Holder())
-                mod = getattr(mod, part)
-            setattr(mod, parts[-1], prm)
+        self._bind_flat(spec, device, world_size)
+        dev = self.flat.params.device
         # fused q|k|v operands
         self._wqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.weight", 3 * h, h) for i in range(self.nl)]
         self._dwqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.weight", 3 * h, h, grad=True)
@@ -134,7 +101,6 @@ class _BertFamily(nn.Module):
             self._nsp_w = torch.zeros(8, h, dtype=torch.bfloat16, device=dev)
             self._nsp_b = torch.full((8,), -30000.0, dtype=torch.bfloat16, device=dev)
         self.reset_parameters(seed)
-        self.accumulate_grads, self.loss_scale, self.grad_hook = False, 1.0, None
         # dropout sites of one forward: 0 embeddings; for layer i, 1 + 3i attention probabilities, 2 + 3i attention output,
         # 3 + 3i FFN output
         self.dropout_sites = 1 + 3 * self.nl
@@ -142,9 +108,6 @@ class _BertFamily(nn.Module):
         if self.p_hidden > 0 or self.p_attn > 0:
             self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
             self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=dev)
-
-    def P(self, name):
-        return self._p[name]
 
     def _drop(self, base, p, site):
         """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
@@ -162,35 +125,16 @@ class _BertFamily(nn.Module):
             else:
                 prm.normal_(0.0, std, generator=gen)
 
-    @torch.no_grad()
-    def load_reference_state_dict(self, sd):
-        for k, prm in self._p.items():
-            if tuple(sd[k].shape) != tuple(prm.shape):
-                raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(prm.shape)}")
-            prm.copy_(sd[k].to(device=prm.device, dtype=prm.dtype))
-
-    def cuda(self, device=None):
-        return self
-
-    def to(self, *a, **k):
-        return self
-
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, token_type_ids=None, position_ids=None, labels=None,
                 next_sentence_label=None, return_logits=False, **_):
         B, S = input_ids.shape
         dev = self.flat.params.device
-        c = lambda t: None if t is None else t.to(device=dev, dtype=torch.int64).contiguous().view(-1)
+        c = lambda t: flat_ids(t, dev)
         ids, tt, pos, lab = c(input_ids), c(token_type_ids), c(position_ids), c(labels)
         nsl = c(next_sentence_label)
-        mask = None
-        if attention_mask is not None and not bool(attention_mask.all()):
-            mask = attention_mask.to(device=dev, dtype=torch.uint8).contiguous()
-        if lab is not None and torch.is_grad_enabled():
-            anchor = self.P("cls.predictions.transform.LayerNorm.weight")
-            loss, logits, nsp = _BertStep.apply(self, ids, tt, pos, mask, lab, nsl, B, S, return_logits, anchor)
-        else:
-            loss, logits, nsp, _ = self._forward_impl(ids, tt, pos, mask, lab, nsl, B, S, save=False, want_logits=True)
+        mask = key_mask(attention_mask, dev)
+        loss, logits, nsp = self._step_or_forward(lab is not None, return_logits, ids, tt, pos, mask, lab, nsl, B, S)
         out = SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                               hidden_states=None, attentions=None)
         out.prediction_logits = out.logits
@@ -414,15 +358,8 @@ class _BertFamily(nn.Module):
             lw, lb = P(E + "LayerNorm.weight"), P(E + "LayerNorm.bias")
             dx = ops.layernorm_bwd(dx, emb, lw.data, st_e, lw.main_grad, lb.main_grad, accumulate=acc)
         ops.embedding_bwd(ids, dx, wte.main_grad)           # adds onto the tied decoder's weight gradient
-        wpe, wtt = P(E + "position_embeddings.weight"), P(E + "token_type_embeddings.weight")
-        if pos is None:
-            ops.colsum(dx.view(B, S * h), wpe.main_grad[:S].reshape(-1), accumulate=acc)
-            if not acc and S < self.npos:
-                wpe.main_grad[S:].zero_()
-        else:
-            if not acc:
-                wpe.main_grad.zero_()
-            ops.embedding_bwd(pos, dx, wpe.main_grad)
+        learned_pos_emb_bwd(pos, dx, P(E + "position_embeddings.weight").main_grad, B, S, acc)
+        wtt = P(E + "token_type_embeddings.weight")
         # token types: dT = onehot(tt)^T dx as a (tiny-M) GEMM; all-zero types reduce to a column sum
         if tt is None:
             ops.colsum(dx, wtt.main_grad[0], accumulate=acc)
@@ -439,26 +376,6 @@ class _BertFamily(nn.Module):
         self._done("emb")
         self._done("no_decay")
 
-    def save_pretrained(self, path, **_):
-        """HF-style export (config.json + pytorch_model.bin with this class's HF key names): fsb200/models/export.py."""
-        from .export import save_pretrained
-        save_pretrained(self, path)
-
-    def _done(self, bucket):
-        if self.grad_hook is not None:
-            self.grad_hook(bucket)
-
-    def _need(self, bucket):
-        """Forward is about to read this bucket's parameters (the engine may still be all-gathering them)."""
-        hook = getattr(self, "param_hook", None)
-        if hook is not None:
-            hook(bucket)
-
-    def _begin_backward(self):
-        hook = getattr(self, "backward_begin_hook", None)
-        if hook is not None:
-            hook()
-
 
 class BertForMaskedLM(_BertFamily):
     PRE_LN = False
@@ -466,21 +383,3 @@ class BertForMaskedLM(_BertFamily):
 
 class MegatronBertForPreTraining(_BertFamily):
     PRE_LN = True
-
-
-class _BertStep(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, model, ids, tt, pos, mask, lab, nsl, B, S, want_logits, _anchor):
-        loss, logits, nsp, saved = model._forward_impl(ids, tt, pos, mask, lab, nsl, B, S, save=True,
-                                                       want_logits=want_logits)
-        ctx.model, ctx.saved = model, saved
-        nd = [t for t in (logits, nsp) if t is not None]
-        ctx.mark_non_differentiable(*nd)
-        return loss, logits, nsp
-
-    @staticmethod
-    def backward(ctx, gloss, _gl, _gn):
-        model, saved = ctx.model, ctx.saved
-        ctx.saved = None
-        model._backward_impl(saved, gloss)
-        return (None,) * 11

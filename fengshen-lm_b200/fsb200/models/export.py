@@ -17,12 +17,17 @@ def _config_dict(cfg):
     return {k: v for k, v in d.items() if isinstance(v, (int, float, str, bool, list, dict, type(None)))}
 
 
-def save_pretrained(model, path, extra_config=None):
-    """config.json + pytorch_model.bin (bf16 tensors, HF key names). Waits for an in-flight parameter all-gather first."""
-    hook = getattr(model, "param_hook", None)
-    eng = getattr(hook, "__self__", None)
+def wait_params(model):
+    """Join the parameter all-gather the engine driving `model` (if any) may still have in flight, before the parameters are
+    read from the host."""
+    eng = getattr(getattr(model, "param_hook", None), "__self__", None)
     if eng is not None and hasattr(eng, "wait_params"):
         eng.wait_params()
+
+
+def save_pretrained(model, path, extra_config=None):
+    """config.json + pytorch_model.bin (bf16 tensors, HF key names). Waits for an in-flight parameter all-gather first."""
+    wait_params(model)
     os.makedirs(path, exist_ok=True)
     cfg = _config_dict(model.config)
     cfg.update(extra_config or {})

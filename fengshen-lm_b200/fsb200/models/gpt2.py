@@ -12,29 +12,17 @@ import math
 from types import SimpleNamespace
 
 import torch
-from torch import nn
 
 from .. import generation
 from .. import lib as L
 from .. import ops
-from ..flat import FlatBuffers, FlatSpec
+from ..flat import FlatSpec
+from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd
 
 
-class _Holder(nn.Module):
-    pass
-
-
-class GPT2LMHeadModel(nn.Module):
+class GPT2LMHeadModel(FlatModel):
     def __init__(self, config, device=None, world_size=None, seed=0):
-        super().__init__()
-        self.config = config
-        if world_size is None:
-            import torch.distributed as dist
-            world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}"
-                           if torch.cuda.is_available() else "cuda")
-        if dev.type != "cuda":
-            raise RuntimeError("fsb200 GPT2LMHeadModel runs on CUDA only (no CPU fallback on the product path)")
+        super().__init__(config)
         g = lambda k, d=None: getattr(config, k, d)
         self.h, self.nl, self.nh = g("n_embd", g("hidden_size")), g("n_layer", g("num_hidden_layers")), \
             g("n_head", g("num_attention_heads"))
@@ -64,41 +52,10 @@ class GPT2LMHeadModel(nn.Module):
                 spec.add(p + n, s, bk)
         spec.add("transformer.ln_f.weight", (h,), "wte")
         spec.add("transformer.ln_f.bias", (h,), "wte")
-        self.flat = FlatBuffers(spec, dev, world_size=world_size)
-
-        def P(name):
-            prm = nn.Parameter(self.flat.view(name), requires_grad=True)
-            prm.main_grad = self.flat.view(name, grad=True)
-            return prm
-
-        tr = self.transformer = _Holder()
-        tr.wte = _Holder(); tr.wte.weight = P("transformer.wte.weight")
-        tr.wpe = _Holder(); tr.wpe.weight = P("transformer.wpe.weight")
-        tr.h = nn.ModuleList()
-        for i in range(self.nl):
-            p = f"transformer.h.{i}."
-            blk = _Holder()
-            blk.ln_1 = _Holder(); blk.ln_1.weight = P(p + "ln_1.weight"); blk.ln_1.bias = P(p + "ln_1.bias")
-            blk.attn = _Holder()
-            blk.attn.c_attn = _Holder()
-            blk.attn.c_attn.weight = P(p + "attn.c_attn.weight"); blk.attn.c_attn.bias = P(p + "attn.c_attn.bias")
-            blk.attn.c_proj = _Holder()
-            blk.attn.c_proj.weight = P(p + "attn.c_proj.weight"); blk.attn.c_proj.bias = P(p + "attn.c_proj.bias")
-            blk.ln_2 = _Holder(); blk.ln_2.weight = P(p + "ln_2.weight"); blk.ln_2.bias = P(p + "ln_2.bias")
-            blk.mlp = _Holder()
-            blk.mlp.c_fc = _Holder()
-            blk.mlp.c_fc.weight = P(p + "mlp.c_fc.weight"); blk.mlp.c_fc.bias = P(p + "mlp.c_fc.bias")
-            blk.mlp.c_proj = _Holder()
-            blk.mlp.c_proj.weight = P(p + "mlp.c_proj.weight"); blk.mlp.c_proj.bias = P(p + "mlp.c_proj.bias")
-            tr.h.append(blk)
-        tr.ln_f = _Holder(); tr.ln_f.weight = P("transformer.ln_f.weight"); tr.ln_f.bias = P("transformer.ln_f.bias")
+        self._bind_flat(spec, device, world_size)
         self.lm_head = _Holder()
-        self.lm_head.weight = tr.wte.weight  # tied (modeling_gpt2.py:646)
-
+        self.lm_head.weight = self.transformer.wte.weight  # tied (modeling_gpt2.py:646)
         self.reset_parameters(seed)
-        self.accumulate_grads = False
-        self.loss_scale = 1.0
-        self.grad_hook = None
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -115,28 +72,13 @@ class GPT2LMHeadModel(nn.Module):
                 s = std / math.sqrt(2 * self.nl) if name.endswith("c_proj.weight") else std
                 prm.normal_(0.0, s, generator=gen)
 
-    @torch.no_grad()
-    def load_reference_state_dict(self, sd):
-        for k, prm in self.named_parameters():
-            if tuple(sd[k].shape) != tuple(prm.shape):
-                raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(prm.shape)}")
-            prm.copy_(sd[k].to(device=prm.device, dtype=prm.dtype))
-
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, labels=None, position_ids=None, return_logits=False, **_):
         B, S = input_ids.shape
         dev = self.flat.params.device
-        ids = input_ids.to(device=dev, dtype=torch.int64).contiguous().view(-1)
-        pos = None if position_ids is None else \
-            position_ids.to(device=dev, dtype=torch.int64).expand(B, S).contiguous().view(-1)
-        mask = None
-        if attention_mask is not None and not bool(attention_mask.all()):
-            mask = attention_mask.to(device=dev, dtype=torch.uint8).contiguous()
-        lab = None if labels is None else labels.to(device=dev, dtype=torch.int64).contiguous().view(-1)
-        if lab is not None and torch.is_grad_enabled():
-            loss, logits = _GPT2Step.apply(self, ids, pos, mask, lab, B, S, return_logits, self.transformer.ln_f.weight)
-        else:
-            loss, logits, _ = self._forward_impl(ids, pos, mask, lab, B, S, save=False, want_logits=True)
+        ids, lab, mask = flat_ids(input_ids, dev), flat_ids(labels, dev), key_mask(attention_mask, dev)
+        pos = None if position_ids is None else flat_ids(position_ids.expand(B, S), dev)
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, mask, lab, B, S)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
 
@@ -298,51 +240,6 @@ class GPT2LMHeadModel(nn.Module):
                                    blk.ln_1.bias.main_grad, accumulate=acc, dres=dx1)
             self._done(f"layer{i}")
         ops.embedding_bwd(ids, dx, wte.main_grad)  # accumulates onto the LM-head wgrad (tied weights)
-        wpe = tr.wpe.weight
-        if pos is None:
-            # dP[s] = sum_b dx[b, s]: column sum of dx viewed as [B, S*h]
-            ops.colsum(dx.view(B, S * h), wpe.main_grad[:S].reshape(-1), accumulate=acc)
-            if not acc and S < self.npos:
-                wpe.main_grad[S:].zero_()
-        else:
-            if not acc:
-                wpe.main_grad.zero_()
-            ops.embedding_bwd(pos, dx, wpe.main_grad)
+        learned_pos_emb_bwd(pos, dx, tr.wpe.weight.main_grad, B, S, acc)
         self._done("wte")
         self._done("no_decay")
-
-    def save_pretrained(self, path, **_):
-        """HF-style export (config.json + pytorch_model.bin with this class's HF key names): fsb200/models/export.py."""
-        from .export import save_pretrained
-        save_pretrained(self, path)
-
-    def _done(self, bucket):
-        if self.grad_hook is not None:
-            self.grad_hook(bucket)
-
-    def _need(self, bucket):
-        """Forward is about to read this bucket's parameters (the engine may still be all-gathering them)."""
-        hook = getattr(self, "param_hook", None)
-        if hook is not None:
-            hook(bucket)
-
-    def _begin_backward(self):
-        hook = getattr(self, "backward_begin_hook", None)
-        if hook is not None:
-            hook()
-
-
-class _GPT2Step(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, model, ids, pos, mask, lab, B, S, want_logits, _anchor):
-        loss, logits, saved = model._forward_impl(ids, pos, mask, lab, B, S, save=True, want_logits=want_logits)
-        ctx.model, ctx.saved = model, saved
-        ctx.mark_non_differentiable(*([logits] if logits is not None else []))
-        return loss, logits
-
-    @staticmethod
-    def backward(ctx, gloss, _glogits):
-        model, saved = ctx.model, ctx.saved
-        ctx.saved = None
-        model._backward_impl(saved, gloss)
-        return (None,) * 9

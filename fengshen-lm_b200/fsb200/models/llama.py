@@ -7,7 +7,7 @@ names (`llama.embed_in.word_embeddings.weight`, `llama.layers.N.attention.query_
 (layers/transformer.py:488-497). What differs is everything underneath:
   * activations stay [b, s, h] token-major — no [s, b, h] transposes (modeling_llama.py:201,222), no q/k/v repacking;
   * all parameters are views into one flat bf16 buffer, gradients go straight into the parallel flat grad buffer;
-  * the whole network is ONE autograd node (`_LlamaStep`): forward runs the hand-scheduled kernel sequence and keeps
+  * the whole network is ONE autograd node (fsb200/models/base.py): forward runs the hand-scheduled kernel sequence and keeps
     the activations it needs; `loss.backward()` runs the matching hand-written backward (dgrad / wgrad GEMMs, fused
     attention backward, norm backward with the residual-gradient add fused in).
 The causal mask is implicit (flash path semantics, transformer.py:441-448: `attention_mask` is not applied; identical to
@@ -17,12 +17,12 @@ import math
 from types import SimpleNamespace
 
 import torch
-from torch import nn
 
 from .. import generation
 from .. import lib as L
 from .. import ops
-from ..flat import FlatBuffers, FlatSpec
+from ..flat import FlatSpec
+from .base import FlatModel, _Holder, flat_ids
 
 
 def llama_ff_dim(hidden_size, multiple_of=256):
@@ -30,34 +30,22 @@ def llama_ff_dim(hidden_size, multiple_of=256):
     return multiple_of * ((ff + multiple_of - 1) // multiple_of)
 
 
-class _Holder(nn.Module):
-    """Bare container so that named_parameters()/state_dict() reproduce the reference's key names."""
-
-
 def _init_normal_(t, std, gen):
     t.copy_(torch.empty(t.shape, dtype=torch.float32).normal_(0.0, std, generator=gen).to(t.dtype))
 
 
-class LlamaForCausalLM(nn.Module):
+class LlamaForCausalLM(FlatModel):
     def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None):
         """tp_group: the tensor-model-parallel process group (mpu.get_model_parallel_group()) or None. With t = its size > 1
         this rank holds the shard the reference's `part_{rank}` checkpoints hold (utils/llama_convert/convert_fs_llama_tp.py
         :143-181): heads / ff columns / vocabulary rows split t ways (ColumnParallelLinear mpu/layers.py:261-360 for QKV,
         w1, w3 and the LM head; RowParallelLinear :363-470 for dense and w2; VocabParallelEmbedding :62-130), norms replicated.
         `world_size` is then the DATA-parallel size (ranks that share a tensor-parallel rank)."""
-        super().__init__()
-        self.config = config
+        super().__init__(config)
         import torch.distributed as dist
         self.tp_group = tp_group
         self.tp = dist.get_world_size(tp_group) if tp_group is not None else 1
         self.tp_rank = dist.get_rank(tp_group) if tp_group is not None else 0
-        if world_size is None:  # laid out for the job's data-parallel world (the scripts build the model in setup())
-            world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-            world_size //= self.tp
-        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}"
-                           if torch.cuda.is_available() else "cuda")
-        if dev.type != "cuda":
-            raise RuntimeError("fsb200 LlamaForCausalLM runs on CUDA only (no CPU fallback on the product path)")
         h, V, nl, nh = config.hidden_size, config.vocab_size, config.num_hidden_layers, config.num_attention_heads
         self.h, self.V, self.nl, self.nh = h, V, nl, nh
         self.hn = h // nh
@@ -88,65 +76,27 @@ class LlamaForCausalLM(nn.Module):
             spec.add(p + "mlp.w2.weight", (h, self.ff_l), bk)
         spec.add("llama.final_layer_norm.scale", (h,), "head")
         spec.add("embed_out.final_linear.weight", (self.V_l, h), "head")
-        self.flat = FlatBuffers(spec, dev, world_size=world_size)
-
-        # module tree mirroring the reference (modeling_llama.py:97-127, :239-252)
-        def P(name):
-            prm = nn.Parameter(self.flat.view(name), requires_grad=True)
-            prm.main_grad = self.flat.view(name, grad=True)
-            prm.fsb_name = name
-            return prm
-
-        self.llama = _Holder()
-        self.llama.embed_in = _Holder()
-        self.llama.embed_in.word_embeddings = _Holder()
-        self.llama.embed_in.word_embeddings.weight = P("llama.embed_in.word_embeddings.weight")
-        self.llama.layers = nn.ModuleList()
-        inv_freq = 1.0 / (getattr(config, "rotary_emb_base", 10000) ** (torch.arange(0, self.hn, 2).float() / self.hn))
-        for i in range(nl):
-            p = f"llama.layers.{i}."
-            lyr = _Holder()
-            lyr.input_layernorm = _Holder(); lyr.input_layernorm.scale = P(p + "input_layernorm.scale")
-            lyr.attention = _Holder()
-            lyr.attention.query_key_value = _Holder()
-            lyr.attention.query_key_value.weight = P(p + "attention.query_key_value.weight")
-            lyr.attention.rotary_emb = _Holder()
-            lyr.attention.rotary_emb.register_buffer("inv_freq", inv_freq.clone().to(dev))
-            lyr.attention.dense = _Holder(); lyr.attention.dense.weight = P(p + "attention.dense.weight")
-            lyr.post_attention_layernorm = _Holder()
-            lyr.post_attention_layernorm.scale = P(p + "post_attention_layernorm.scale")
-            lyr.mlp = _Holder()
-            lyr.mlp.w1 = _Holder(); lyr.mlp.w1.weight = P(p + "mlp.w1.weight")
-            lyr.mlp.w3 = _Holder(); lyr.mlp.w3.weight = P(p + "mlp.w3.weight")
-            lyr.mlp.w2 = _Holder(); lyr.mlp.w2.weight = P(p + "mlp.w2.weight")
-            lyr.w13 = None  # filled below (non-parameter view)
-            self.llama.layers.append(lyr)
-        self.llama.final_layer_norm = _Holder()
-        self.llama.final_layer_norm.scale = P("llama.final_layer_norm.scale")
-        self.embed_out = _Holder()
-        self.embed_out.final_linear = _Holder()
-        self.embed_out.final_linear.weight = P("embed_out.final_linear.weight")
-
+        self._bind_flat(spec, device, world_size, tp=self.tp)
         self._w13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h)
                      for i in range(nl)]
         self._dw13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h, grad=True) for i in range(nl)]
 
-        # RoPE tables exactly as RotaryEmbedding builds them (layers/positional_embeddings.py:38-52), fp32
-        self._inv_freq = inv_freq
+        # RoPE tables exactly as RotaryEmbedding builds them (layers/positional_embeddings.py:38-52), fp32; inv_freq is also a
+        # buffer of every layer in the reference's module tree (modeling_llama.py:97-127), hence in its state dict
+        self._inv_freq = 1.0 / (getattr(config, "rotary_emb_base", 10000) ** (torch.arange(0, self.hn, 2).float() / self.hn))
+        for lyr in self.llama.layers:
+            lyr.attention.rotary_emb = _Holder()
+            lyr.attention.rotary_emb.register_buffer("inv_freq", self._inv_freq.clone().to(self.flat.params.device))
         self._rope_rows = 0
-        self._ensure_rope(getattr(config, "max_position_embeddings", 2048), dev)
-
+        self._ensure_rope(getattr(config, "max_position_embeddings", 2048))
         self.reset_parameters(seed)
-        self.accumulate_grads = False   # set by the engine for micro-batches after the first
-        self.loss_scale = 1.0           # 1 / (gradient_accumulation_steps * world_size), folded into dlogits
-        self.grad_hook = None           # engine callback: grad_hook(bucket_name) when a bucket's gradients are final
 
-    def _ensure_rope(self, n, dev=None):
+    def _ensure_rope(self, n):
         """cos/sin tables with at least n rows. RotaryEmbedding regrows its cache when a longer sequence arrives
         (positional_embeddings.py:54-68); fsb_rope_inplace never reads past the table (rows beyond it become NaN)."""
         if n <= self._rope_rows:
             return
-        dev = dev if dev is not None else self.flat.params.device
+        dev = self.flat.params.device
         t = torch.arange(n, dtype=self._inv_freq.dtype)
         freqs = torch.einsum("i,j->ij", t, self._inv_freq)
         self._cos = freqs.cos().contiguous().to(dev)
@@ -171,40 +121,11 @@ class LlamaForCausalLM(nn.Module):
             else:
                 _init_normal_(prm.data, std, gen)
 
-    # The reference scripts call `.from_pretrained(..., torch_dtype=torch.half).cuda()`; parameters here are views into the
-    # flat bf16 CUDA buffer and must never be re-allocated by nn.Module._apply.
-    def cuda(self, device=None):
-        return self
-
-    def half(self):
-        return self
-
-    def bfloat16(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        return self
-
-    def train(self, mode=True):   # reference defect (modeling_llama.py:257-260: `mode` is required there); accept both
-        return super().train(mode)
-
-    # HF-style loading of a reference state dict (fp32/fp16/bf16 tensors on any device)
-    @torch.no_grad()
-    def load_reference_state_dict(self, sd):
-        own = dict(self.named_parameters())
-        missing = [k for k in own if k not in sd]
-        if missing:
-            raise KeyError(f"missing keys in state dict: {missing[:4]}...")
-        for k, prm in own.items():
-            if tuple(sd[k].shape) != tuple(prm.shape):
-                raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(prm.shape)}")
-            prm.copy_(sd[k].to(device=prm.device, dtype=prm.dtype))
-
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, labels=None, return_logits=False, **_):
         B, S = input_ids.shape
         dev = self.flat.params.device
-        ids = input_ids.to(device=dev, dtype=torch.int64).contiguous().view(-1)
+        ids = flat_ids(input_ids, dev)
         if position_ids is None:
             self._ensure_rope(S)
             pos = torch.arange(S, device=dev, dtype=torch.int64).repeat(B)
@@ -220,13 +141,8 @@ class LlamaForCausalLM(nn.Module):
                 torch._assert_async(((pos >= 0) & (pos < self._rope_rows)).all(),
                                     "fsb200 LlamaForCausalLM: position_ids outside [0, rope table rows); pass them on the "
                                     "host or raise config.max_position_embeddings")
-        lab = None if labels is None else labels.to(device=dev, dtype=torch.int64).contiguous().view(-1)
-        if lab is not None and torch.is_grad_enabled():
-            # a leaf that requires grad makes the node differentiable; real gradients go to the flat grad buffer
-            loss, logits = _LlamaStep.apply(self, ids, pos, lab, B, S, return_logits,
-                                            self.llama.final_layer_norm.scale)
-        else:
-            loss, logits, _ = self._forward_impl(ids, pos, lab, B, S, save=False, want_logits=True)
+        lab = flat_ids(labels, dev)
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
 
@@ -464,38 +380,3 @@ class LlamaForCausalLM(nn.Module):
         lo = self.tp_rank * self.V_l
         mine = (ids >= lo) & (ids < lo + self.V_l)
         return torch.where(mine, ids - lo, torch.zeros_like(ids)), mine.to(torch.bfloat16)[:, None]
-
-    def _done(self, bucket):
-        if self.grad_hook is not None:
-            self.grad_hook(bucket)
-
-    def _need(self, bucket):
-        """Forward is about to read this bucket's parameters (the engine may still be all-gathering them)."""
-        hook = getattr(self, "param_hook", None)
-        if hook is not None:
-            hook(bucket)
-
-    def _begin_backward(self):
-        hook = getattr(self, "backward_begin_hook", None)
-        if hook is not None:
-            hook()
-
-
-class _LlamaStep(torch.autograd.Function):
-    """The whole network as one autograd node; `flat_params` is the differentiable handle (its .grad is never
-    materialised: gradients are written into model.flat.grads by the kernels)."""
-
-    @staticmethod
-    def forward(ctx, model, ids, pos, lab, B, S, want_logits, flat_params):
-        loss, logits, saved = model._forward_impl(ids, pos, lab, B, S, save=True, want_logits=want_logits)
-        ctx.model = model
-        ctx.saved = saved
-        ctx.mark_non_differentiable(*([logits] if logits is not None else []))
-        return loss, logits
-
-    @staticmethod
-    def backward(ctx, gloss, _glogits):
-        model, saved = ctx.model, ctx.saved
-        ctx.saved = None
-        model._backward_impl(saved, None if gloss is None else gloss)
-        return (None,) * 8

@@ -24,30 +24,18 @@ import math
 from types import SimpleNamespace
 
 import torch
-from torch import nn
 
 from .. import generation
 from .. import lib as L
 from .. import ops
-from ..flat import FlatBuffers, FlatSpec
+from ..flat import FlatSpec
 from . import t5_bias as TB
+from .base import FlatModel, _Holder, flat_ids, key_mask
 
 
-class _Holder(nn.Module):
-    pass
-
-
-class MT5ForConditionalGeneration(nn.Module):
+class MT5ForConditionalGeneration(FlatModel):
     def __init__(self, config, device=None, world_size=None, seed=0):
-        super().__init__()
-        self.config = config
-        if world_size is None:
-            import torch.distributed as dist
-            world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}"
-                           if torch.cuda.is_available() else "cuda")
-        if dev.type != "cuda":
-            raise RuntimeError("fsb200 MT5ForConditionalGeneration runs on CUDA only (no CPU fallback on the product path)")
+        super().__init__(config)
         g = lambda k, d=None: getattr(config, k, d)
         self.d, self.dk, self.nh, self.ff = g("d_model"), g("d_kv"), g("num_heads"), g("d_ff")
         self.ne = g("num_layers")
@@ -109,22 +97,7 @@ class MT5ForConditionalGeneration(nn.Module):
         spec.add("decoder.final_layer_norm.weight", (d,), "head")
         if not self.tied:
             spec.add("lm_head.weight", (V, d), "head")
-        self.flat = FlatBuffers(spec, dev, world_size=world_size)
-
-        # module tree mirroring HF's parameter names (state_dict / named_parameters / weight-decay grouping BY NAME)
-        self._p = {}
-        for name in self.flat.offsets:
-            prm = nn.Parameter(self.flat.view(name), requires_grad=True)
-            prm.main_grad = self.flat.view(name, grad=True)
-            self._p[name] = prm
-            mod = self
-            parts = name.split(".")
-            for part in parts[:-1]:
-                if not hasattr(mod, part):
-                    setattr(mod, part, _Holder())
-                mod = getattr(mod, part)
-            setattr(mod, parts[-1], prm)
-
+        self._bind_flat(spec, device, world_size)
         if self.tied:
             self.lm_head = _Holder()
             self.lm_head.weight = self._p["shared.weight"]      # same Parameter object: named_parameters() lists it once
@@ -143,10 +116,6 @@ class MT5ForConditionalGeneration(nn.Module):
         self._d_dwi = [fl.span(D.format(i) + "2.DenseReluDense.wi_0.weight", 2 * ff, d, grad=True) for i in range(self.nd)]
 
         self.reset_parameters(seed)
-        self.accumulate_grads, self.loss_scale, self.grad_hook = False, 1.0, None
-
-    def P(self, name):
-        return self._p[name]
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -171,49 +140,6 @@ class MT5ForConditionalGeneration(nn.Module):
                 std = ff ** -0.5
             prm.normal_(0.0, std, generator=gen)
 
-    def cuda(self, device=None):
-        return self
-
-    def half(self):
-        return self
-
-    def bfloat16(self):
-        return self
-
-    def to(self, *args, **kwargs):
-        return self
-
-    @torch.no_grad()
-    def load_reference_state_dict(self, sd):
-        """HF state dict (fp32 / bf16, any device). `encoder.embed_tokens.weight` / `decoder.embed_tokens.weight` are aliases
-        of `shared.weight` in HF and are ignored."""
-        for k, prm in self._p.items():
-            if k not in sd:
-                raise KeyError(f"missing key in state dict: {k}")
-            if tuple(sd[k].shape) != tuple(prm.shape):
-                raise ValueError(f"shape mismatch for {k}: {tuple(sd[k].shape)} vs {tuple(prm.shape)}")
-            prm.copy_(sd[k].to(device=prm.device, dtype=prm.dtype))
-
-    def save_pretrained(self, path, **_):
-        """HF-style export (config.json + pytorch_model.bin with this class's HF key names): fsb200/models/export.py."""
-        from .export import save_pretrained
-        save_pretrained(self, path)
-
-    # ---- engine hooks -----------------------------------------------------------------------------------------------
-    def _done(self, bucket):
-        if self.grad_hook is not None and bucket in self.flat.bucket_index:   # "head" does not exist with a tied LM head
-            self.grad_hook(bucket)
-
-    def _need(self, bucket):
-        hook = getattr(self, "param_hook", None)
-        if hook is not None:
-            hook(bucket)
-
-    def _begin_backward(self):
-        hook = getattr(self, "backward_begin_hook", None)
-        if hook is not None:
-            hook()
-
     # ---- forward ----------------------------------------------------------------------------------------------------
     def _shift_right(self, labels):
         """MT5 _shift_right (:592): decoder_input_ids = [start] + labels[:-1], with -100 replaced by the pad id."""
@@ -225,24 +151,14 @@ class MT5ForConditionalGeneration(nn.Module):
     def forward(self, input_ids=None, attention_mask=None, labels=None, decoder_input_ids=None, return_logits=False, **_):
         dev = self.flat.params.device
         B, Se = input_ids.shape
-        ids = input_ids.to(device=dev, dtype=torch.int64).contiguous()
-        mask = None
-        if attention_mask is not None and not bool(attention_mask.all()):
-            mask = attention_mask.to(device=dev, dtype=torch.uint8).contiguous()
-        lab = None if labels is None else labels.to(device=dev, dtype=torch.int64).contiguous()
         if decoder_input_ids is None:
-            if lab is None:
+            if labels is None:
                 raise ValueError("fsb200 MT5: pass labels or decoder_input_ids")
-            dec_ids = self._shift_right(lab)
-        else:
-            dec_ids = decoder_input_ids.to(device=dev, dtype=torch.int64).contiguous()
-        Sd = dec_ids.shape[1]
-        if lab is not None and torch.is_grad_enabled():
-            loss, logits = _T5Step.apply(self, ids.view(-1), dec_ids.view(-1), mask, lab.view(-1), B, Se, Sd, return_logits,
-                                         self.P("decoder.final_layer_norm.weight"))
-        else:
-            loss, logits, _ = self._forward_impl(ids.view(-1), dec_ids.view(-1), mask, None if lab is None else lab.view(-1),
-                                                 B, Se, Sd, save=False, want_logits=True)
+            decoder_input_ids = self._shift_right(labels.to(device=dev, dtype=torch.int64))
+        Sd = decoder_input_ids.shape[1]
+        ids, dec_ids, lab = flat_ids(input_ids, dev), flat_ids(decoder_input_ids, dev), flat_ids(labels, dev)
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, dec_ids, key_mask(attention_mask, dev), lab,
+                                             B, Se, Sd)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, Sd, self.V),
                                past_key_values=None, encoder_last_hidden_state=None)
 
@@ -514,24 +430,6 @@ class MT5ForConditionalGeneration(nn.Module):
             mg.copy_((mg.float() + g).to(mg.dtype))
         else:
             mg.copy_(g.to(mg.dtype))
-
-
-class _T5Step(torch.autograd.Function):
-    """The whole encoder-decoder as one autograd node (cf. _LlamaStep)."""
-
-    @staticmethod
-    def forward(ctx, model, ids, dec_ids, mask, lab, B, Se, Sd, want_logits, anchor):
-        loss, logits, saved = model._forward_impl(ids, dec_ids, mask, lab, B, Se, Sd, save=True, want_logits=want_logits)
-        ctx.model, ctx.saved = model, saved
-        ctx.mark_non_differentiable(*([logits] if logits is not None else []))
-        return loss, logits
-
-    @staticmethod
-    def backward(ctx, gloss, _glogits):
-        model, saved = ctx.model, ctx.saved
-        ctx.saved = None
-        model._backward_impl(saved, None if gloss is None else gloss)
-        return (None,) * 10
 
 
 def t5_flops_per_step(cfg, B, Se, Sd):

@@ -9,10 +9,7 @@ import torch
 from torch import nn
 
 from fsb200.flat import FlatBuffers, FlatSpec
-
-
-class _Holder(nn.Module):
-    pass
+from fsb200.models.base import bind_flat_parameters
 
 
 class _ToyBase(nn.Module):
@@ -29,24 +26,13 @@ class _ToyBase(nn.Module):
             import torch.distributed as dist
             world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.flat = FlatBuffers(self._spec(self.V, self.H), "cpu", world_size=world_size)
-        self._p = {}
+        bind_flat_parameters(self, self.flat)
         g = torch.Generator().manual_seed(seed)
-        for name, (_, shape) in self.flat.offsets.items():
-            self.flat.view(name).copy_((torch.randn(shape, generator=g) * 0.02).to(torch.bfloat16))
-            prm = nn.Parameter(self.flat.view(name), requires_grad=True)
-            self._p[name] = prm
-            mod = self
-            parts = name.split(".")
-            for part in parts[:-1]:
-                if not hasattr(mod, part):
-                    setattr(mod, part, _Holder())
-                mod = getattr(mod, part)
-            setattr(mod, parts[-1], prm)
         with torch.no_grad():
             for name, prm in self._p.items():
+                prm.copy_((torch.randn(prm.shape, generator=g) * 0.02).to(torch.bfloat16))
                 if name.endswith("layer_norm.weight"):
                     prm.fill_(1.0)
-        self._gviews = {name: self.flat.view(name, grad=True) for name in self.flat.offsets}
         self.accumulate_grads, self.loss_scale, self.grad_hook = False, 1.0, None
 
     def load_reference_state_dict(self, sd):
@@ -106,8 +92,8 @@ class _ToyStep(torch.autograd.Function):
             for name, (off, _) in fb.offsets.items():
                 if start <= off < start + length:
                     g = gmap[name]
-                    g16 = torch.zeros_like(model._gviews[name]) if g is None else g.to(torch.bfloat16)
-                    gv = model._gviews[name]
+                    gv = model._p[name].main_grad
+                    g16 = torch.zeros_like(gv) if g is None else g.to(torch.bfloat16)
                     if model.accumulate_grads:
                         gv.copy_((gv.float() + g16.float()).to(torch.bfloat16))
                     else:
