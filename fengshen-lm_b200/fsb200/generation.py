@@ -8,6 +8,10 @@ calls `run(step, seqs, cfg)`. The step contract is
       * step(None, None): the prefill (the prompt rows, already expanded);
       * step(tokens [rows], reorder [rows] or None): first gather every cache row from `reorder` (beam search), then append
         `tokens` and return the next logits.
+      * the returned logits are a FRESH tensor that the model never writes again: the loop keeps them (`scores`, and greedy
+        without a penalty processes them into the very same tensor), so a step that computes into a static buffer (a
+        CUDA-graph replay, fsb200/decode_graph.py) returns a clone of it. `tokens` and `reorder` are only read during the
+        call; the step copies what it needs.
 
 Everything here is host-side PyTorch on whatever device the logits live on; the model does the GPU work.
 

@@ -110,6 +110,8 @@ SIGNATURES = {
     "fsb_attn_decode_workspace_bytes": (c_size, [c_i64, c_int, c_int, c_i64]),
     "fsb_attn_decode": (c_int, [c_void_p] * 5 + [c_i64, c_int, c_int, c_i64, c_void_p] + [c_i64] * 10 +
                         [c_f32, c_void_p, c_void_p, c_void_p, c_size, c_void_p]),
+    "fsb_kv_append": (c_int, [c_void_p] * 5 + [c_i64, c_int, c_int, c_i64, c_void_p] + [c_i64] * 10 + [c_void_p]),
+    "fsb_kv_reorder": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -16,6 +16,7 @@ import torch
 from .. import generation
 from .. import lib as L
 from .. import ops
+from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd
 
@@ -121,9 +122,11 @@ class GPT2LMHeadModel(FlatModel):
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on GPT-2 (wenzhong_qa/README.md:58-67: sampling with top_p, num_return_sequences,
     # return_dict_in_generate, output_scores). The prompt is prefilled with the training kernels (causal attention under the
-    # left-padding key mask) and its keys / values land in a pre-allocated [rows, cap, 2, heads, head_dim] cache per layer;
-    # every later step feeds one token per row and attends with the split-KV decode kernel (ops.attn_decode). Position ids
-    # follow transformers 5.5.0 (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
+    # left-padding key mask) and its keys / values land in a pre-allocated cache, one [layers, rows, cap, 2, heads, head_dim]
+    # allocation; every later step feeds one token per row, appends its keys / values at the device-side slot kv_len - 1
+    # (ops.kv_append) and attends with the split-KV decode kernel (ops.attn_decode). The decode step is one CUDA-graph replay
+    # (fsb200/decode_graph.py); beam search gathers the cache, key mask and positions into a twin (ops.kv_reorder) and the two
+    # directions alternate. Position ids follow transformers 5.5.0 (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded."""
@@ -138,40 +141,55 @@ class GPT2LMHeadModel(FlatModel):
         ids, mask = ids.repeat_interleave(c.expand, 0), mask.repeat_interleave(c.expand, 0)
         R = ids.shape[0]
         cap = (max(c.max_length, S0 + 1) + 63) // 64 * 64
-        st = SimpleNamespace(cache=[torch.zeros((R, cap, 2, self.nh, self.hn), dtype=torch.bfloat16, device=dev)
-                                    for _ in range(self.nl)],
-                             kv_mask=torch.zeros((R, cap), dtype=torch.uint8, device=dev),
-                             kv_len=torch.zeros(1, dtype=torch.int32, device=dev),
-                             count=mask.sum(-1), cur=S0)
-        st.kv_mask[:, :S0] = mask.to(torch.uint8)
+        # per cache twin (a second one for beam search): keys / values, key mask, next position id of every row
+        st = [SimpleNamespace(cache=torch.zeros((self.nl, R, cap, 2, self.nh, self.hn), dtype=torch.bfloat16, device=dev),
+                              kv_mask=torch.zeros((R, cap), dtype=torch.uint8, device=dev),
+                              count=torch.zeros(R, dtype=torch.int64, device=dev))
+              for _ in range(2 if c.num_beams > 1 else 1)]
+        st[0].kv_mask[:, :S0] = mask.to(torch.uint8)
+        st[0].count.copy_(mask.sum(-1))
+        kv_len = torch.full((1,), S0, dtype=torch.int32, device=dev)
+        tok, index = torch.zeros(R, dtype=torch.int64, device=dev), torch.zeros(R, dtype=torch.int64, device=dev)
+
+        def body(key):
+            src, reorder = key
+            a = st[src]
+            b = st[1 - src] if reorder else a
+            if reorder:
+                ops.kv_reorder(a.cache, b.cache, index, kv_len)
+                torch.index_select(a.kv_mask, 0, index, out=b.kv_mask)
+                torch.index_select(a.count, 0, index, out=b.count)
+            kv_len.add_(1)
+            logits = self._gen_forward(tok, b.count, R, 1, b, kv_len, None)
+            b.count.add_(1)
+            return logits
+
+        graphs = DecodeGraphs(self, body)
+        live = [0]   # the twin holding the current cache
 
         def step(tokens, reorder):
             if tokens is None:
                 pos = (mask.cumsum(-1) - 1).masked_fill(mask == 0, 0)
-                pre = None if bool(mask.all()) else st.kv_mask[:, :S0].contiguous()
-                return self._gen_forward(ids.reshape(-1), pos.reshape(-1), R, S0, st, pre)
+                pre = None if bool(mask.all()) else st[0].kv_mask[:, :S0].contiguous()
+                return self._gen_forward(ids.reshape(-1), pos.reshape(-1), R, S0, st[0], None, pre)
+            tok.copy_(tokens)
+            src = live[0]
             if reorder is not None:
-                st.cache = [kv.index_select(0, reorder) for kv in st.cache]
-                st.kv_mask, st.count = st.kv_mask.index_select(0, reorder), st.count.index_select(0, reorder)
-            st.kv_mask[:, st.cur] = 1
-            st.kv_len.fill_(st.cur + 1)
-            logits = self._gen_forward(tokens, st.count, R, 1, st, None)
-            st.cur += 1
-            st.count = st.count + 1
-            return logits
+                index.copy_(reorder)
+                live[0] = 1 - src
+            return graphs((src, reorder is not None))
 
         return generation.run(step, ids, c)
 
-    def _gen_forward(self, ids, pos, B, S, st, prefill_mask):
-        """S > 1: prefill (writes cache slots [0, S)); S == 1: one decode step at slot st.cur. Returns fp32 logits [B, V]
-        of the last position."""
+    def _gen_forward(self, ids, pos, B, S, st, kv_len, prefill_mask):
+        """S > 1: prefill (writes cache slots [0, S)); S == 1: one decode step at the device-side slot kv_len - 1. Returns fp32
+        logits [B, V] of the last position."""
         h, nh, hn = self.h, self.nh, self.hn
         tr = self.transformer
         self._need("no_decay"); self._need("wte")
         x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
         prev_m = None
         scale = 1.0 / math.sqrt(hn)
-        at = 0 if S > 1 else st.cur
         for i, blk in enumerate(tr.h):
             self._need(f"layer{i}")
             h1, _, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
@@ -179,11 +197,13 @@ class GPT2LMHeadModel(FlatModel):
             qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
             q5 = qkv.view(B, S, 3, nh, hn)
             kv = st.cache[i]
-            kv[:, at:at + S].copy_(q5[:, :, 1:3])
             if S > 1:
+                kv[:, :S].copy_(q5[:, :, 1:3])
                 o, _ = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=prefill_mask)
-            else:
-                o, _ = ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], st.kv_len, scale, kv_mask=st.kv_mask)
+            else:   # the key mask is shared by the layers: the first one sets the new slot's bit
+                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len,
+                              kv_mask=st.kv_mask if i == 0 else None)
+                o, _ = ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=st.kv_mask)
             a = ops.gemm(L.GEMM_NN, o.view(B * S, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
             h2, _, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
             f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data, epilogue=L.EPI_GELU_TANH)

@@ -21,6 +21,7 @@ import torch
 from .. import generation
 from .. import lib as L
 from .. import ops
+from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids
 
@@ -199,13 +200,16 @@ class LlamaForCausalLM(FlatModel):
     # (layers/transformer.py:529-537) and `llama_generate.generate` (examples/ziya_llama/llama_generate.py:16-39) left-pads the
     # prompts. Here the cache is a pre-allocated [batch, max_length, heads, head_dim] pair per layer; a decode step runs the
     # same kernels as training with one query row per sequence, the unused tail of the cache (and the left padding) hidden by
-    # the key mask. Padded keys ARE masked (the reference's `global` attention path; its flash path ignores the mask).
+    # the key mask. Padded keys ARE masked (the reference's `global` attention path; its flash path ignores the mask). The
+    # decode step keeps its position on the device (kv_len, the position ids; the new keys / values land at slot kv_len - 1
+    # through ops.kv_append) and runs as one CUDA-graph replay (fsb200/decode_graph.py).
     @property
     def device(self):
         return self.flat.params.device
 
-    def _layer_infer(self, i, x, prev_m, pos, B, S, kc, vc, at, kv_mask, causal):
-        """One layer forward without saving activations; writes this call's keys / values into the cache at [at, at + S)."""
+    def _layer_infer(self, i, x, prev_m, pos, B, S, kc, vc, kv_len, kv_mask, causal):
+        """One layer forward without saving activations; writes this call's keys / values into the cache: slots [0, S) in the
+        prefill (causal), slot kv_len - 1 in a decode step (S == 1; the first layer also sets that slot's kv_mask bit)."""
         if self.tp > 1:
             raise NotImplementedError("fsb200: KV-cache decoding under tensor parallelism is not implemented")
         h, nh, hn, ff = self.h, self.nh, self.hn, self.ff
@@ -216,12 +220,13 @@ class LlamaForCausalLM(FlatModel):
         ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * h, 3 * hn, offset=0)
         ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * h, 3 * hn, offset=hn)
         q5 = qkv.view(B, S, nh, 3, hn)
-        kc[:, at:at + S].copy_(q5[:, :, :, 1])
-        vc[:, at:at + S].copy_(q5[:, :, :, 2])
         if causal:   # prefill: attend inside the prompt (causal + left-padding mask)
+            kc[:, :S].copy_(q5[:, :, :, 1])
+            vc[:, :S].copy_(q5[:, :, :, 2])
             o, _ = ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], 1.0 / math.sqrt(hn), True,
                                 kv_mask=None if kv_mask is None else kv_mask[:, :S].contiguous())
         else:        # decode: one query row per sequence against the whole cache; unwritten slots are masked
+            ops.kv_append(q5[:, 0, :, 1], q5[:, 0, :, 2], kc, vc, kv_len, kv_mask=kv_mask if i == 0 else None)
             o, _ = ops.sdpa_fwd(q5[:, :, :, 0], kc, vc, 1.0 / math.sqrt(hn), False, kv_mask=kv_mask)
         a = ops.gemm(L.GEMM_NT, o.view(B * S, h), lyr.attention.dense.weight.data)
         h2, _, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
@@ -230,14 +235,14 @@ class LlamaForCausalLM(FlatModel):
         m = ops.gemm(L.GEMM_NT, act, lyr.mlp.w2.weight.data)
         return x1, m
 
-    def _infer(self, ids, pos, B, S, cache, at, kv_mask, causal):
+    def _infer(self, ids, pos, B, S, cache, kv_len, kv_mask, causal):
         """ids / pos flattened [B*S]; returns fp32 logits of the LAST position of every sequence, [B, V]."""
         for b in ("no_decay", "embed_in"):
             self._need(b)
         x, prev_m = ops.embedding_fwd(ids, self.llama.embed_in.word_embeddings.weight.data), None
         for i in range(self.nl):
             self._need(f"layer{i}")
-            x, prev_m = self._layer_infer(i, x, prev_m, pos, B, S, cache[i][0], cache[i][1], at, kv_mask, causal)
+            x, prev_m = self._layer_infer(i, x, prev_m, pos, B, S, cache[i][0], cache[i][1], kv_len, kv_mask, causal)
         self._need("head")
         hf, _, _ = ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
         last = hf.view(B, S, self.h)[:, -1].contiguous()                       # [B, h]
@@ -275,9 +280,19 @@ class LlamaForCausalLM(FlatModel):
         # position_ids = cumsum(mask) - 1, pads -> 1 (prepare_inputs_for_generation, modeling_llama.py:360-366)
         pos = mask.long().cumsum(-1) - 1
         pos = pos.masked_fill(mask == 0, 1)
-        logits = self._infer(ids.reshape(-1), pos.reshape(-1).contiguous(), B, S0, cache, 0, kv_mask if not bool(mask.all()) else None,
-                             True)
+        logits = self._infer(ids.reshape(-1), pos.reshape(-1).contiguous(), B, S0, cache, None,
+                             kv_mask if not bool(mask.all()) else None, True)
         count = mask.long().sum(-1)                                             # real tokens so far = next position id
+        kv_len = torch.full((1,), S0, dtype=torch.int32, device=dev)
+        tok = torch.zeros(B, dtype=torch.int64, device=dev)
+
+        def body(_):
+            kv_len.add_(1)
+            out = self._infer(tok, count, B, 1, cache, kv_len, kv_mask, False)
+            count.add_(1)
+            return out
+
+        graphs = DecodeGraphs(self, body)
         seqs = ids
         done = torch.zeros(B, dtype=torch.bool, device=dev)
         for cur in range(S0, max_length):
@@ -288,9 +303,8 @@ class LlamaForCausalLM(FlatModel):
             seqs = torch.cat([seqs, nxt[:, None]], dim=1)
             if cur + 1 >= max_length or bool(done.all()):
                 break
-            kv_mask[:, cur] = 1
-            logits = self._infer(nxt, count.clone(), B, 1, cache, cur, kv_mask, False)
-            count = count + 1
+            tok.copy_(nxt)
+            logits = graphs()
         return seqs
 
     _pick = staticmethod(generation.pick)   # HF logits-processor order, then arg-max or one draw (fsb200/generation.py)

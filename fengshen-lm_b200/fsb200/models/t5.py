@@ -28,6 +28,7 @@ import torch
 from .. import generation
 from .. import lib as L
 from .. import ops
+from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from . import t5_bias as TB
 from .base import FlatModel, _Holder, flat_ids, key_mask
@@ -197,8 +198,11 @@ class MT5ForConditionalGeneration(FlatModel):
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on MT5 (mt5_summary.py:41-49,131-139; finetune_t5.py:66-71). The encoder runs once; every
     # decoder layer projects its cross-attention K|V once from the encoder output; each step feeds one token per row, appends
-    # its self-attention K|V to a [rows, cap, 2, heads, d_kv] cache and runs the split-KV decode kernel twice per layer: self-
-    # attention with the relative-position bias at the query's slot, cross-attention under the encoder padding mask.
+    # its self-attention K|V at the device-side slot kv_len - 1 (ops.kv_append) of a [layers, rows, cap, 2, heads, d_kv]
+    # cache and runs the split-KV decode kernel twice per layer: self-attention with the relative-position bias at the
+    # query's slot, cross-attention under the encoder padding mask. Every decode step is one CUDA-graph replay
+    # (fsb200/decode_graph.py); beam search gathers the self-attention cache into a twin (ops.kv_reorder) and the two
+    # directions alternate. The cross-attention K|V is the same for every beam of an item and is not reordered.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); sequences start with
@@ -228,14 +232,18 @@ class MT5ForConditionalGeneration(FlatModel):
                                    False, self.nbuckets, self.maxdist)
         enc_len = torch.full((1,), Se, dtype=torch.int32, device=dev)
         start = torch.full((R, 1), c.start, dtype=torch.int64, device=dev)
-        st = SimpleNamespace(cache=[torch.zeros((R, cap, 2, nh, dk), dtype=torch.bfloat16, device=dev) for _ in range(self.nd)],
-                             kv_len=torch.zeros(1, dtype=torch.int32, device=dev), cur=0)
+        # the self-attention cache, and its twin for beam search
+        caches = [torch.zeros((self.nd, R, cap, 2, nh, dk), dtype=torch.bfloat16, device=dev)
+                  for _ in range(2 if c.num_beams > 1 else 1)]
+        kv_len = torch.zeros(1, dtype=torch.int32, device=dev)
+        tok, index = start.view(-1).clone(), torch.zeros(R, dtype=torch.int64, device=dev)
 
-        def step(tokens, reorder):
-            if reorder is not None:
-                st.cache = [kv.index_select(0, reorder) for kv in st.cache]
-            tok = start.view(-1) if tokens is None else tokens
-            st.kv_len.fill_(st.cur + 1)
+        def body(key):
+            src, reorder = key
+            cache = caches[1 - src] if reorder else caches[src]
+            if reorder:
+                ops.kv_reorder(caches[src], cache, index, kv_len)
+            kv_len.add_(1)
             self._need("no_decay"); self._need("shared")
             y, prev = ops.embedding_fwd(tok, P("shared.weight").data), None
             for i in range(self.nd):
@@ -243,9 +251,9 @@ class MT5ForConditionalGeneration(FlatModel):
                 self._need(f"dec{i}")
                 h1, _, y = self._norm(prev, y, p + "0.layer_norm.weight")
                 q3 = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i]).view(R, 3, nh, dk)
-                kv = st.cache[i]
-                kv[:, st.cur].copy_(q3[:, 1:3])
-                o, _ = ops.attn_decode(q3[:, 0], kv[:, :, 0], kv[:, :, 1], st.kv_len, 1.0, rel_bias=rel_d)
+                kv = cache[i]
+                ops.kv_append(q3[:, 1], q3[:, 2], kv[:, :, 0], kv[:, :, 1], kv_len)
+                o, _ = ops.attn_decode(q3[:, 0], kv[:, :, 0], kv[:, :, 1], kv_len, 1.0, rel_bias=rel_d)
                 a = ops.gemm(L.GEMM_NT, o.view(R, inner), P(p + "0.SelfAttention.o.weight").data)
                 h2, _, y1 = self._norm(a, y, p + "1.layer_norm.weight")
                 qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
@@ -259,8 +267,19 @@ class MT5ForConditionalGeneration(FlatModel):
                 y, prev = y2, m
             self._need("head")
             hf, _, _ = self._norm(prev, y, "decoder.final_layer_norm.weight")
-            st.cur += 1
             return ops.gemm(L.GEMM_NT, hf, P(self._head).data).float()
+
+        graphs = DecodeGraphs(self, body)
+        live = [0]   # the twin holding the current cache
+
+        def step(tokens, reorder):
+            if tokens is not None:
+                tok.copy_(tokens)
+            src = live[0]
+            if reorder is not None:
+                index.copy_(reorder)
+                live[0] = 1 - src
+            return graphs((src, reorder is not None))
 
         return generation.run(step, start, c)
 

@@ -456,6 +456,58 @@ def attn_decode(q, k_cache, v_cache, kv_len, scale, kv_mask=None, rel_bias=None,
     return out, lse
 
 
+def _chk_kv_len(kv_len, what):
+    _chk(kv_len, torch.int32, "kv_len")
+    if kv_len.numel() != 1:
+        raise RuntimeError(f"fsb200 {what}: kv_len must be a one-element int32 tensor")
+
+
+def kv_append(k_new, v_new, k_cache, v_cache, kv_len, kv_mask=None):
+    """Write the newest token's keys / values k_new, v_new [B, H, D] (strided bf16 views, unit inner stride) into slot
+    kv_len - 1 of k_cache / v_cache [B, cap, H, D] (strided views, e.g. the K and V halves of a [B, cap, 2, H, D] cache).
+    kv_len: int32 CUDA scalar (read on the device). kv_mask: optional uint8 [B, cap]; its bit at that slot is set to 1.
+    A slot outside [0, cap) writes nothing."""
+    for t, n in ((k_new, "k_new"), (v_new, "v_new"), (k_cache, "k_cache"), (v_cache, "v_cache")):
+        _chk(t, _bf16, n)
+    if k_new.dim() != 3 or k_new.stride(2) != 1:
+        raise RuntimeError("fsb200 kv_append: k_new must be [batch, heads, dim] with unit inner stride")
+    B, H, D = k_new.shape
+    if tuple(v_new.shape) != (B, H, D) or v_new.stride(2) != 1:
+        raise RuntimeError(f"fsb200 kv_append: v_new must be [{B}, {H}, {D}] with unit inner stride")
+    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
+        if t.dim() != 4 or t.stride(3) != 1 or (t.shape[0], t.shape[2], t.shape[3]) != (B, H, D):
+            raise RuntimeError(f"fsb200 kv_append: {n} must be [{B}, cap, {H}, {D}] with unit inner stride, "
+                               f"got {tuple(t.shape)} strides {t.stride()}")
+    cap = k_cache.shape[1]
+    if v_cache.shape[1] != cap:
+        raise RuntimeError("fsb200 kv_append: k_cache and v_cache capacities differ")
+    _chk_kv_len(kv_len, "kv_append")
+    if kv_mask is not None:
+        _chk(kv_mask, torch.uint8, "kv_mask")
+        if tuple(kv_mask.shape) != (B, cap) or not kv_mask.is_contiguous():
+            raise RuntimeError(f"fsb200 kv_append: kv_mask must be contiguous uint8 [{B}, {cap}]")
+    L.call("fsb_kv_append", _p(k_new), _p(v_new), _p(k_cache), _p(v_cache), _p(kv_mask), B, H, D, cap, _p(kv_len),
+           k_new.stride(0), k_new.stride(1), v_new.stride(0), v_new.stride(1), k_cache.stride(0), k_cache.stride(1),
+           k_cache.stride(2), v_cache.stride(0), v_cache.stride(1), v_cache.stride(2), _stream())
+
+
+def kv_reorder(src, dst, index, kv_len):
+    """Beam-search gather of the caches of every layer, one launch: dst[l, r, s] = src[l, index[r], s] for the live slots
+    s < kv_len (device int32 scalar); slots at or beyond it are neither read nor written. src / dst: contiguous bf16
+    [layers, rows, cap, ...], distinct buffers. index: int64 [rows] on the device."""
+    _chk(src, _bf16, "src"); _chk(dst, _bf16, "dst")
+    if src.dim() < 3 or not src.is_contiguous() or not dst.is_contiguous() or src.shape != dst.shape:
+        raise RuntimeError(f"fsb200 kv_reorder: src and dst must be contiguous bf16 [layers, rows, cap, ...] of one shape, "
+                           f"got {tuple(src.shape)} and {tuple(dst.shape)}")
+    layers, rows, cap = src.shape[:3]
+    _chk(index, torch.int64, "index")
+    if tuple(index.shape) != (rows,) or not index.is_contiguous():
+        raise RuntimeError(f"fsb200 kv_reorder: index must be contiguous int64 [{rows}]")
+    _chk_kv_len(kv_len, "kv_reorder")
+    slot = src[0, 0, 0].numel()
+    L.call("fsb_kv_reorder", _p(src), _p(dst), _p(index), layers, rows, cap, slot, _p(kv_len), _stream())
+
+
 def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None, drop=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
     rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=), deterministically.

@@ -312,6 +312,36 @@ int fsb_attn_decode(const void* q, const void* k, const void* v, void* o, float*
                     float scale, const uint8_t* kv_mask, const float* rel_bias,
                     void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- KV-cache maintenance of a decode step (device-side position) ------------------------------------------------------
+ * Both entries read the cache length from the same DEVICE int32 scalar `kv_len` as fsb_attn_decode and take no host-side
+ * slot, so a decode step built from them issues identical launches at every position and can be captured in a CUDA graph.
+ *
+ * fsb_kv_append: copies the newest token's keys and values into cache slot *kv_len - 1, for every row and head (16-byte
+ *   vector accesses). It replaces the per-step concatenation of the new key / value onto the layer's past (transformers'
+ *   cache update, `layer_past` in the reference) and a slot copy at a host index. Element addressing (elements; 16-byte
+ *   aligned bases; strides multiples of 8; head_dim a multiple of 8):
+ *     new key   (row, head, d)       at k_new + row*k_new_row_stride + head*k_new_head_stride + d        (v_new likewise)
+ *     cache key (row, slot, head, d) at k_cache + row*k_batch_stride + slot*k_row_stride + head*k_head_stride + d
+ *                                                                                                          (v_cache likewise)
+ *   e.g. GPT-2 / mT5: the new keys are the K third of the packed [t, {q,k,v}, heads, d] projection and the cache is
+ *   [rows, kv_cap, {k,v}, heads, d]; LLaMA: the K slice of the interleaved [t, heads, {q,k,v}, d] projection into a separate
+ *   [rows, kv_cap, heads, d] K cache. kv_mask: optional contiguous uint8 [rows, kv_cap]; kv_mask[row, slot] is set to 1.
+ *   A slot outside [0, kv_cap) writes nothing. One kernel launch.
+ *
+ * fsb_kv_reorder: the beam-search gather dst[l, r, s, :] = src[l, index[r], s, :] over the caches of all `layers` in one
+ *   launch, for the live slots s < *kv_len only (clamped to [0, kv_cap]); slots at or beyond it are neither read nor written.
+ *   It replaces transformers' `_reorder_cache` (an index_select of every layer's full capacity). src and dst are contiguous
+ *   bf16 [layers, rows, kv_cap, slot_elems] (slot_elems = the elements of one slot of one row, a multiple of 8, e.g.
+ *   2 * heads * head_dim), 16-byte aligned and disjoint. index: int64 [rows] on the device; a row whose index lies outside
+ *   [0, rows) is left untouched. One kernel launch. */
+int fsb_kv_append(const void* k_new, const void* v_new, void* k_cache, void* v_cache, uint8_t* kv_mask,
+                  int64_t rows, int nheads, int head_dim, int64_t kv_cap, const int32_t* kv_len,
+                  int64_t k_new_row_stride, int64_t k_new_head_stride, int64_t v_new_row_stride, int64_t v_new_head_stride,
+                  int64_t k_batch_stride, int64_t k_row_stride, int64_t k_head_stride,
+                  int64_t v_batch_stride, int64_t v_row_stride, int64_t v_head_stride, fsb_stream_t stream);
+int fsb_kv_reorder(const void* src, void* dst, const int64_t* index, int64_t layers, int64_t rows, int64_t kv_cap,
+                   int64_t slot_elems, const int32_t* kv_len, fsb_stream_t stream);
+
 /* ---- communication (NCCL over NVLink / NVSwitch) --------------------------------------------------------------
  * The three exchange steps of the ZeRO-1/2 data path (SURVEY.md §8e) — the collectives the reference delegates to DeepSpeed
  * (fengshen/strategies/megatron_deepspeed.py:302-320; Appendix D): bucketed gradient reduce-scatter (SUM), the fp32 scalar
