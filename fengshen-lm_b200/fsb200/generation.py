@@ -1,8 +1,8 @@
 """Model-agnostic generation controller: the token-selection loop of transformers' `GenerationMixin.generate` (HF 5.5.0,
 generation/utils.py `_sample` and `_beam_search`) on top of a model-provided step function.
 
-A model's `generate` resolves the options with `resolve(...)`, prepares its caches for `rows = batch * cfg.expand` sequences, and
-calls `run(step, seqs, cfg)`. The step contract is
+A model's `generate` resolves the options with `resolve(...)` (LLaMA: from its own keyword defaults), prepares its caches
+for `rows = batch * cfg.expand` sequences, and calls `run(step, seqs, cfg)`. The step contract is
 
     step(next_tokens, beam_reorder) -> fp32 logits [rows, V] of the last position of every row
       * step(None, None): the prefill (the prompt rows, already expanded);
@@ -114,14 +114,6 @@ def process(logits, seqs, do_sample, temperature, top_k, top_p, repetition_penal
         remove[:, -min_keep:] = False
         logits = logits.masked_fill(remove.scatter(1, idx, remove), float("-inf"))
     return logits
-
-
-def pick(logits, seqs, do_sample, temperature, top_k, top_p, repetition_penalty, generator):
-    """Process the logits (`process`) and select the next token: arg-max, or one draw from the softmax."""
-    logits = process(logits, seqs, do_sample, temperature, top_k, top_p, repetition_penalty)
-    if not do_sample:
-        return logits.argmax(-1)
-    return torch.multinomial(torch.softmax(logits, -1), 1, generator=generator).squeeze(1)
 
 
 def run(step, seqs, c, generator=None):

@@ -84,31 +84,11 @@ class GPT2LMHeadModel(FlatModel):
                                past_key_values=None, hidden_states=None, attentions=None)
 
     def _forward_impl(self, ids, pos, mask, lab, B, S, save, want_logits):
-        h, nh, hn = self.h, self.nh, self.hn
-        T = B * S
-        tr = self.transformer
-        self._need("no_decay"); self._need("wte")
-        x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
-        acts, prev_m = [], None
-        scale = 1.0 / math.sqrt(hn)
-        for i, blk in enumerate(tr.h):
-            self._need(f"layer{i}")
-            h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
-                                           self.eps, residual=None if prev_m is None else x)
-            qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
-            q5 = qkv.view(B, S, 3, nh, hn)
-            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask)
-            a = ops.gemm(L.GEMM_NN, o.view(T, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
-            h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
-            pre = torch.empty((T, self.inner), dtype=torch.bfloat16, device=x.device) if save else None
-            f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data,
-                         epilogue=L.EPI_GELU_TANH, aux=pre)
-            m = ops.gemm(L.GEMM_NN, f, blk.mlp.c_proj.weight.data, bias=blk.mlp.c_proj.bias.data)
-            if save:
-                acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f))
-            x, prev_m = x1, m
-        hf, stf, xf = ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x)
-        logits = ops.gemm(L.GEMM_NT, hf, tr.wte.weight.data)
+        scale = 1.0 / math.sqrt(self.hn)
+        acts = [] if save else None
+        hf, stf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale,
+                                                                             True, kv_mask=mask), acts)
+        logits = ops.gemm(L.GEMM_NT, hf, self.transformer.wte.weight.data)
         loss, ctx = None, None
         if lab is not None:
             keep = logits.clone() if (want_logits and save) else None
@@ -119,14 +99,43 @@ class GPT2LMHeadModel(FlatModel):
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
+    def _stack(self, ids, pos, B, S, attend, acts=None):
+        """Embedding, the blocks and ln_f over ids [B * S] -> (hidden states, ln_f stats, residual stream). attend(i, q5) is
+        block i's attention over the packed q|k|v view [B, S, 3, heads, head_dim] -> (out, lse); `acts`, when given,
+        collects what the backward reads."""
+        h, nh, hn = self.h, self.nh, self.hn
+        tr = self.transformer
+        self._need("no_decay"); self._need("wte")
+        x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
+        prev_m = None
+        for i, blk in enumerate(tr.h):
+            self._need(f"layer{i}")
+            h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
+                                           self.eps, residual=None if prev_m is None else x)
+            qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
+            o, lse = attend(i, qkv.view(B, S, 3, nh, hn))
+            a = ops.gemm(L.GEMM_NN, o.view(B * S, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
+            h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
+            pre = None if acts is None else torch.empty((B * S, self.inner), dtype=torch.bfloat16, device=x.device)
+            f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data,
+                         epilogue=L.EPI_GELU_TANH, aux=pre)
+            m = ops.gemm(L.GEMM_NN, f, blk.mlp.c_proj.weight.data, bias=blk.mlp.c_proj.bias.data)
+            if acts is not None:
+                acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f))
+            # free this block's temporaries before the next block allocates its own (the peak of a long prompt's prefill)
+            del st1, h1, qkv, o, lse, a, st2, h2, pre, f
+            x, prev_m = x1, m
+        return ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x)
+
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on GPT-2 (wenzhong_qa/README.md:58-67: sampling with top_p, num_return_sequences,
-    # return_dict_in_generate, output_scores). The prompt is prefilled with the training kernels (causal attention under the
-    # left-padding key mask) and its keys / values land in a pre-allocated cache, one [layers, rows, cap, 2, heads, head_dim]
-    # allocation; every later step feeds one token per row, appends its keys / values at the device-side slot kv_len - 1
-    # (ops.kv_append) and attends with the split-KV decode kernel (ops.attn_decode). The decode step is one CUDA-graph replay
-    # (fsb200/decode_graph.py); beam search gathers the cache, key mask and positions into a twin (ops.kv_reorder) and the two
-    # directions alternate. Position ids follow transformers 5.5.0 (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
+    # return_dict_in_generate, output_scores). Prefill and decode steps run the training layer stack (`_stack`) with their
+    # own attention: the prefill writes the prompt's keys / values into a pre-allocated cache, one [layers, rows, cap, 2,
+    # heads, head_dim] allocation, and attends causally under the left-padding key mask; a decode step feeds one token per
+    # row, appends its keys / values at the device-side slot kv_len - 1 (ops.kv_append) and attends with the split-KV decode
+    # kernel (ops.attn_decode). The decode step is one CUDA-graph replay (fsb200/decode_graph.py); beam search gathers the
+    # cache, key mask and positions into the twin (ops.kv_reorder). Position ids follow transformers 5.5.0
+    # (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded."""
@@ -141,7 +150,8 @@ class GPT2LMHeadModel(FlatModel):
         ids, mask = ids.repeat_interleave(c.expand, 0), mask.repeat_interleave(c.expand, 0)
         R = ids.shape[0]
         cap = (max(c.max_length, S0 + 1) + 63) // 64 * 64
-        # per cache twin (a second one for beam search): keys / values, key mask, next position id of every row
+        scale = 1.0 / math.sqrt(self.hn)
+        # per cache: keys / values, key mask, next position id of every row
         st = [SimpleNamespace(cache=torch.zeros((self.nl, R, cap, 2, self.nh, self.hn), dtype=torch.bfloat16, device=dev),
                               kv_mask=torch.zeros((R, cap), dtype=torch.uint8, device=dev),
                               count=torch.zeros(R, dtype=torch.int64, device=dev))
@@ -149,69 +159,38 @@ class GPT2LMHeadModel(FlatModel):
         st[0].kv_mask[:, :S0] = mask.to(torch.uint8)
         st[0].count.copy_(mask.sum(-1))
         kv_len = torch.full((1,), S0, dtype=torch.int32, device=dev)
-        tok, index = torch.zeros(R, dtype=torch.int64, device=dev), torch.zeros(R, dtype=torch.int64, device=dev)
 
-        def body(key):
-            src, reorder = key
-            a = st[src]
-            b = st[1 - src] if reorder else a
-            if reorder:
+        def prefill():
+            pos = (mask.cumsum(-1) - 1).masked_fill(mask == 0, 0)
+            pre = None if bool(mask.all()) else st[0].kv_mask[:, :S0].contiguous()
+
+            def attend(i, q5):
+                st[0].cache[i][:, :S0].copy_(q5[:, :, 1:3])
+                return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=pre)
+            return self._last_logits(ids.reshape(-1), pos.reshape(-1), R, S0, attend)
+
+        def body(tok, index, a, b):
+            if b is not a:
                 ops.kv_reorder(a.cache, b.cache, index, kv_len)
                 torch.index_select(a.kv_mask, 0, index, out=b.kv_mask)
                 torch.index_select(a.count, 0, index, out=b.count)
             kv_len.add_(1)
-            logits = self._gen_forward(tok, b.count, R, 1, b, kv_len, None)
+
+            def attend(i, q5):   # the key mask is shared by the layers: the first one sets the new slot's bit
+                kv = b.cache[i]
+                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len,
+                              kv_mask=b.kv_mask if i == 0 else None)
+                return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=b.kv_mask)
+            logits = self._last_logits(tok, b.count, R, 1, attend)
             b.count.add_(1)
             return logits
 
-        graphs = DecodeGraphs(self, body)
-        live = [0]   # the twin holding the current cache
+        return generation.run(DecodeGraphs(self, R, st, body, prefill), ids, c)
 
-        def step(tokens, reorder):
-            if tokens is None:
-                pos = (mask.cumsum(-1) - 1).masked_fill(mask == 0, 0)
-                pre = None if bool(mask.all()) else st[0].kv_mask[:, :S0].contiguous()
-                return self._gen_forward(ids.reshape(-1), pos.reshape(-1), R, S0, st[0], None, pre)
-            tok.copy_(tokens)
-            src = live[0]
-            if reorder is not None:
-                index.copy_(reorder)
-                live[0] = 1 - src
-            return graphs((src, reorder is not None))
-
-        return generation.run(step, ids, c)
-
-    def _gen_forward(self, ids, pos, B, S, st, kv_len, prefill_mask):
-        """S > 1: prefill (writes cache slots [0, S)); S == 1: one decode step at the device-side slot kv_len - 1. Returns fp32
-        logits [B, V] of the last position."""
-        h, nh, hn = self.h, self.nh, self.hn
-        tr = self.transformer
-        self._need("no_decay"); self._need("wte")
-        x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
-        prev_m = None
-        scale = 1.0 / math.sqrt(hn)
-        for i, blk in enumerate(tr.h):
-            self._need(f"layer{i}")
-            h1, _, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
-                                         self.eps, residual=None if prev_m is None else x)
-            qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
-            q5 = qkv.view(B, S, 3, nh, hn)
-            kv = st.cache[i]
-            if S > 1:
-                kv[:, :S].copy_(q5[:, :, 1:3])
-                o, _ = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=prefill_mask)
-            else:   # the key mask is shared by the layers: the first one sets the new slot's bit
-                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len,
-                              kv_mask=st.kv_mask if i == 0 else None)
-                o, _ = ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=st.kv_mask)
-            a = ops.gemm(L.GEMM_NN, o.view(B * S, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
-            h2, _, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
-            f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data, epilogue=L.EPI_GELU_TANH)
-            m = ops.gemm(L.GEMM_NN, f, blk.mlp.c_proj.weight.data, bias=blk.mlp.c_proj.bias.data)
-            x, prev_m = x1, m
-        hf, _, _ = ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x)
-        last = hf.view(B, S, h)[:, -1].contiguous()
-        return ops.gemm(L.GEMM_NT, last, tr.wte.weight.data).float()
+    def _last_logits(self, ids, pos, B, S, attend):
+        """fp32 logits [B, V] of the last position of every sequence."""
+        hf, _, _ = self._stack(ids, pos, B, S, attend)
+        return ops.gemm(L.GEMM_NT, hf.view(B, S, self.h)[:, -1].contiguous(), self.transformer.wte.weight.data).float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):

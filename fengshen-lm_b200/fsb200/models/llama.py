@@ -148,10 +148,28 @@ class LlamaForCausalLM(FlatModel):
                                past_key_values=None, hidden_states=None, attentions=None)
 
     def _forward_impl(self, ids, pos, lab, B, S, save, want_logits):
-        h, nh, hn, ff = self.h, self.nh_l, self.hn, self.ff_l          # LOCAL heads / ff columns under tensor parallelism
-        hl = self.h_l
-        T = B * S
-        acts = []
+        scale = 1.0 / math.sqrt(self.hn)
+        acts = [] if save else None
+        hf, rstdf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2],
+                                                                               scale, True), acts)
+        logits = ops.gemm(L.GEMM_NT, hf, self.embed_out.final_linear.weight.data)
+        logits = self._tp_gather_columns(logits)   # ParallelLinear(parallel_output=False): full-vocabulary logits on every rank
+        loss = None
+        ctx = None
+        if lab is not None:
+            keep = logits.clone() if (want_logits and save) else None
+            loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
+                                                dlogits="inplace" if save else None)
+            if save:
+                ctx = (acts, hf, rstdf, xf, dlogits, ids, pos, B, S)
+                logits = keep
+        return loss, (logits if want_logits else None), ctx
+
+    def _stack(self, ids, pos, B, S, attend, acts=None):
+        """Embedding, the layers and the final norm over ids [B * S] -> (hidden states, their rstd, residual stream).
+        attend(i, q5) is layer i's attention over the per-head interleaved q|k|v view [B, S, heads, 3, head_dim] (rotary
+        embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads."""
+        nh, hn, ff, hl = self.nh_l, self.hn, self.ff_l, self.h_l      # LOCAL heads / ff columns under tensor parallelism
         self._need("no_decay"); self._need("embed_in")
         ids_l, emb_keep = self._local_ids(ids)
         x = ops.embedding_fwd(ids_l, self.llama.embed_in.word_embeddings.weight.data)
@@ -166,92 +184,34 @@ class LlamaForCausalLM(FlatModel):
             qkv = ops.gemm(L.GEMM_NT, h1, lyr.attention.query_key_value.weight.data)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
-            q5 = qkv.view(B, S, nh, 3, hn)
-            o, lse = ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], 1.0 / math.sqrt(hn), True)
-            o2 = o.view(T, hl)
-            a = ops.gemm(L.GEMM_NT, o2, lyr.attention.dense.weight.data)
+            o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
+            a = ops.gemm(L.GEMM_NT, o.view(B * S, hl), lyr.attention.dense.weight.data)
             self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
             h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
             gu = ops.gemm(L.GEMM_NT, h2, self._w13[i])
             act = ops.glu_fwd(L.ACT_SILU, gu[:, :ff], gu[:, ff:])
             m = ops.gemm(L.GEMM_NT, act, lyr.mlp.w2.weight.data)
             self._tp_all_reduce(m)        # RowParallelLinear (w2)
-            if save:
+            if acts is not None:
                 acts.append((x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, gu, act))
+            # free this layer's temporaries before the next layer allocates its own (the peak of a long prompt's prefill)
+            del rstd1, h1, qkv, o, lse, a, rstd2, h2, gu, act
             x, prev_m = x1, m
         self._need("head")
-        hf, rstdf, xf = ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
-        logits = ops.gemm(L.GEMM_NT, hf, self.embed_out.final_linear.weight.data)
-        logits = self._tp_gather_columns(logits)   # ParallelLinear(parallel_output=False): full-vocabulary logits on every rank
-        loss = None
-        ctx = None
-        if lab is not None:
-            keep = logits.clone() if (want_logits and save) else None
-            loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
-                                                dlogits="inplace" if save else None)
-            if save:
-                ctx = (acts, hf, rstdf, xf, dlogits, ids, pos, B, S)
-                logits = keep
-        return loss, (logits if want_logits else None), ctx
+        return ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
 
     # ---- KV-cache inference (SURVEY.md §8f rank 4) -----------------------------------------------------------------------
     # The reference decodes through HF's GenerationMixin: `prepare_inputs_for_generation` (modeling_llama.py:353-377) feeds the
     # last token with position_ids = cumsum(attention_mask) - 1, every layer concatenates the new key / value onto `layer_past`
     # (layers/transformer.py:529-537) and `llama_generate.generate` (examples/ziya_llama/llama_generate.py:16-39) left-pads the
-    # prompts. Here the cache is a pre-allocated [batch, max_length, heads, head_dim] pair per layer; a decode step runs the
-    # same kernels as training with one query row per sequence, the unused tail of the cache (and the left padding) hidden by
-    # the key mask. Padded keys ARE masked (the reference's `global` attention path; its flash path ignores the mask). The
-    # decode step keeps its position on the device (kv_len, the position ids; the new keys / values land at slot kv_len - 1
-    # through ops.kv_append) and runs as one CUDA-graph replay (fsb200/decode_graph.py).
+    # prompts. Here the cache is a pre-allocated [batch, max_length, heads, head_dim] pair per layer; prefill and decode steps
+    # run the training layer stack (`_stack`), a decode step with one query row per sequence, the unused tail of the cache (and
+    # the left padding) hidden by the key mask. Padded keys ARE masked (the reference's `global` attention path; its flash
+    # path ignores the mask). The decode step keeps its position on the device (kv_len, the position ids; the new keys /
+    # values land at slot kv_len - 1 through ops.kv_append) and runs as one CUDA-graph replay (fsb200/decode_graph.py).
     @property
     def device(self):
         return self.flat.params.device
-
-    def _layer_infer(self, i, x, prev_m, pos, B, S, kc, vc, kv_len, kv_mask, causal):
-        """One layer forward without saving activations; writes this call's keys / values into the cache: slots [0, S) in the
-        prefill (causal), slot kv_len - 1 in a decode step (S == 1; the first layer also sets that slot's kv_mask bit)."""
-        if self.tp > 1:
-            raise NotImplementedError("fsb200: KV-cache decoding under tensor parallelism is not implemented")
-        h, nh, hn, ff = self.h, self.nh, self.hn, self.ff
-        lyr = self.llama.layers[i]
-        h1, _, x = ops.rmsnorm_fwd(x if prev_m is None else prev_m, lyr.input_layernorm.scale.data, self.eps,
-                                   residual=None if prev_m is None else x)
-        qkv = ops.gemm(L.GEMM_NT, h1, lyr.attention.query_key_value.weight.data)
-        ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * h, 3 * hn, offset=0)
-        ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * h, 3 * hn, offset=hn)
-        q5 = qkv.view(B, S, nh, 3, hn)
-        if causal:   # prefill: attend inside the prompt (causal + left-padding mask)
-            kc[:, :S].copy_(q5[:, :, :, 1])
-            vc[:, :S].copy_(q5[:, :, :, 2])
-            o, _ = ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], 1.0 / math.sqrt(hn), True,
-                                kv_mask=None if kv_mask is None else kv_mask[:, :S].contiguous())
-        else:        # decode: one query row per sequence against the whole cache; unwritten slots are masked
-            ops.kv_append(q5[:, 0, :, 1], q5[:, 0, :, 2], kc, vc, kv_len, kv_mask=kv_mask if i == 0 else None)
-            o, _ = ops.sdpa_fwd(q5[:, :, :, 0], kc, vc, 1.0 / math.sqrt(hn), False, kv_mask=kv_mask)
-        a = ops.gemm(L.GEMM_NT, o.view(B * S, h), lyr.attention.dense.weight.data)
-        h2, _, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
-        gu = ops.gemm(L.GEMM_NT, h2, self._w13[i])
-        act = ops.glu_fwd(L.ACT_SILU, gu[:, :ff], gu[:, ff:])
-        m = ops.gemm(L.GEMM_NT, act, lyr.mlp.w2.weight.data)
-        return x1, m
-
-    def _infer(self, ids, pos, B, S, cache, kv_len, kv_mask, causal):
-        """ids / pos flattened [B*S]; returns fp32 logits of the LAST position of every sequence, [B, V]."""
-        for b in ("no_decay", "embed_in"):
-            self._need(b)
-        x, prev_m = ops.embedding_fwd(ids, self.llama.embed_in.word_embeddings.weight.data), None
-        for i in range(self.nl):
-            self._need(f"layer{i}")
-            x, prev_m = self._layer_infer(i, x, prev_m, pos, B, S, cache[i][0], cache[i][1], kv_len, kv_mask, causal)
-        self._need("head")
-        hf, _, _ = ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
-        last = hf.view(B, S, self.h)[:, -1].contiguous()                       # [B, h]
-        rows = max(8, B)                                                        # the GEMM wants >= 8 aligned rows
-        if rows != B:
-            pad = torch.zeros((rows, self.h), dtype=last.dtype, device=last.device)
-            pad[:B] = last
-            last = pad
-        return ops.gemm(L.GEMM_NT, last, self.embed_out.final_linear.weight.data)[:B].float()
 
     @torch.no_grad()
     def generate(self, input_ids, attention_mask=None, max_length=None, max_new_tokens=None, do_sample=False,
@@ -260,7 +220,9 @@ class LlamaForCausalLM(FlatModel):
         """Greedy / sampling decode with a KV cache; the keyword surface `llama_generate.generate` passes to HF's
         `model.generate` (do_sample, top_p, top_k, max_length, repetition_penalty, temperature, pad_token_id, eos_token_id).
         Prompts are LEFT-padded (attention_mask 0 on the pads). Returns [batch, <= max_length] token ids, prompt included,
-        finished rows filled with pad_token_id — HF's GenerationMixin conventions."""
+        finished rows filled with pad_token_id — HF's GenerationMixin conventions, selected by fsb200/generation.py."""
+        if self.tp > 1:
+            raise NotImplementedError("fsb200: KV-cache decoding under tensor parallelism is not implemented")
         dev = self.device
         ids = input_ids.to(device=dev, dtype=torch.int64)
         B, S0 = ids.shape
@@ -270,44 +232,55 @@ class LlamaForCausalLM(FlatModel):
             max_length = S0 + (max_new_tokens if max_new_tokens is not None else 20)
         if max_length <= S0:
             return ids
-        pad_id = pad_token_id if pad_token_id is not None else (eos_token_id if eos_token_id is not None else 0)
+        c = SimpleNamespace(num_beams=1, do_sample=do_sample, temperature=temperature, top_k=top_k, top_p=top_p,
+                            repetition_penalty=repetition_penalty, max_length=max_length, output_scores=False,
+                            return_dict=False, eos=None if eos_token_id is None else [eos_token_id],
+                            pad=pad_token_id if pad_token_id is not None else (eos_token_id if eos_token_id is not None else 0))
         Lmax = (max_length + 63) // 64 * 64
         self._ensure_rope(max_length)
+        scale = 1.0 / math.sqrt(self.hn)
         cache = [(torch.zeros((B, Lmax, self.nh, self.hn), dtype=torch.bfloat16, device=dev),
                   torch.zeros((B, Lmax, self.nh, self.hn), dtype=torch.bfloat16, device=dev)) for _ in range(self.nl)]
         kv_mask = torch.zeros((B, Lmax), dtype=torch.uint8, device=dev)
         kv_mask[:, :S0] = mask
-        # position_ids = cumsum(mask) - 1, pads -> 1 (prepare_inputs_for_generation, modeling_llama.py:360-366)
-        pos = mask.long().cumsum(-1) - 1
-        pos = pos.masked_fill(mask == 0, 1)
-        logits = self._infer(ids.reshape(-1), pos.reshape(-1).contiguous(), B, S0, cache, None,
-                             kv_mask if not bool(mask.all()) else None, True)
         count = mask.long().sum(-1)                                             # real tokens so far = next position id
         kv_len = torch.full((1,), S0, dtype=torch.int32, device=dev)
-        tok = torch.zeros(B, dtype=torch.int64, device=dev)
 
-        def body(_):
+        def prefill():
+            # position_ids = cumsum(mask) - 1, pads -> 1 (prepare_inputs_for_generation, modeling_llama.py:360-366)
+            pos = (mask.long().cumsum(-1) - 1).masked_fill(mask == 0, 1)
+            pre = None if bool(mask.all()) else kv_mask[:, :S0].contiguous()
+
+            def attend(i, q5):   # attend inside the prompt (causal + left-padding mask)
+                kc, vc = cache[i]
+                kc[:, :S0].copy_(q5[:, :, :, 1])
+                vc[:, :S0].copy_(q5[:, :, :, 2])
+                return ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, True, kv_mask=pre)
+            return self._last_logits(ids.reshape(-1), pos.reshape(-1).contiguous(), B, S0, attend)
+
+        def body(tok, *_):
             kv_len.add_(1)
-            out = self._infer(tok, count, B, 1, cache, kv_len, kv_mask, False)
+
+            def attend(i, q5):   # one query row per sequence against the whole cache; unwritten slots are masked
+                kc, vc = cache[i]
+                ops.kv_append(q5[:, 0, :, 1], q5[:, 0, :, 2], kc, vc, kv_len, kv_mask=kv_mask if i == 0 else None)
+                return ops.sdpa_fwd(q5[:, :, :, 0], kc, vc, scale, False, kv_mask=kv_mask)
+            out = self._last_logits(tok, count, B, 1, attend)
             count.add_(1)
             return out
 
-        graphs = DecodeGraphs(self, body)
-        seqs = ids
-        done = torch.zeros(B, dtype=torch.bool, device=dev)
-        for cur in range(S0, max_length):
-            nxt = self._pick(logits, seqs, do_sample, temperature, top_k, top_p, repetition_penalty, generator)
-            if eos_token_id is not None:
-                nxt = torch.where(done, torch.full_like(nxt, pad_id), nxt)
-                done = done | (nxt == eos_token_id)
-            seqs = torch.cat([seqs, nxt[:, None]], dim=1)
-            if cur + 1 >= max_length or bool(done.all()):
-                break
-            tok.copy_(nxt)
-            logits = graphs()
-        return seqs
+        return generation.run(DecodeGraphs(self, B, [cache], body, prefill), ids, c, generator)
 
-    _pick = staticmethod(generation.pick)   # HF logits-processor order, then arg-max or one draw (fsb200/generation.py)
+    def _last_logits(self, ids, pos, B, S, attend):
+        """fp32 logits [B, V] of the last position of every sequence."""
+        hf, _, _ = self._stack(ids, pos, B, S, attend)
+        last = hf.view(B, S, self.h)[:, -1].contiguous()                       # [B, h]
+        rows = max(8, B)                                                        # the GEMM wants >= 8 aligned rows
+        if rows != B:
+            pad = torch.zeros((rows, self.h), dtype=last.dtype, device=last.device)
+            pad[:B] = last
+            last = pad
+        return ops.gemm(L.GEMM_NT, last, self.embed_out.final_linear.weight.data)[:B].float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):

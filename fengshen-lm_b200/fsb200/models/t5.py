@@ -195,20 +195,51 @@ class MT5ForConditionalGeneration(FlatModel):
         enc_h, rfe, xfe = self._norm(prev, x, "encoder.final_layer_norm.weight")
         return eacts, enc_h, rfe, xfe
 
+    def _decode(self, dec_ids, B, S, attend, cross_attend, acts=None):
+        """Decoder stack over dec_ids [B * S] -> (final hidden states, their rstd, residual stream). attend(i, q5) is layer i's
+        self-attention over the packed q|k|v view [B, S, 3, heads, d_kv] -> (out, lse); cross_attend(i, qc) its
+        cross-attention from the query projection [B * S, inner] -> (out, lse, the encoder's K|V or None); `acts`, when given,
+        collects what the backward reads."""
+        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        P = self.P
+        T = B * S
+        self._need("no_decay"); self._need("shared")
+        y, prev = ops.embedding_fwd(dec_ids, P("shared.weight").data), None
+        for i in range(self.nd):
+            p = f"decoder.block.{i}.layer."
+            self._need(f"dec{i}")
+            h1, r1, y = self._norm(prev, y, p + "0.layer_norm.weight")
+            qkv = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i])
+            o, lse = attend(i, qkv.view(B, S, 3, nh, dk))
+            a = ops.gemm(L.GEMM_NT, o.view(T, inner), P(p + "0.SelfAttention.o.weight").data)
+            h2, r2, y1 = self._norm(a, y, p + "1.layer_norm.weight")
+            qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
+            oc, lsec, kvc = cross_attend(i, qc)
+            ac = ops.gemm(L.GEMM_NT, oc.view(T, inner), P(p + "1.EncDecAttention.o.weight").data)
+            h3, r3, y2 = self._norm(ac, y1, p + "2.layer_norm.weight")
+            gu = ops.gemm(L.GEMM_NT, h3, self._d_wi[i])
+            act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
+            m = ops.gemm(L.GEMM_NT, act, P(p + "2.DenseReluDense.wo.weight").data)
+            if acts is not None:
+                acts.append((y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, gu, act))
+            y, prev = y2, m
+        self._need("head")
+        return self._norm(prev, y, "decoder.final_layer_norm.weight")
+
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on MT5 (mt5_summary.py:41-49,131-139; finetune_t5.py:66-71). The encoder runs once; every
-    # decoder layer projects its cross-attention K|V once from the encoder output; each step feeds one token per row, appends
-    # its self-attention K|V at the device-side slot kv_len - 1 (ops.kv_append) of a [layers, rows, cap, 2, heads, d_kv]
-    # cache and runs the split-KV decode kernel twice per layer: self-attention with the relative-position bias at the
-    # query's slot, cross-attention under the encoder padding mask. Every decode step is one CUDA-graph replay
-    # (fsb200/decode_graph.py); beam search gathers the self-attention cache into a twin (ops.kv_reorder) and the two
-    # directions alternate. The cross-attention K|V is the same for every beam of an item and is not reordered.
+    # decoder layer projects its cross-attention K|V once from the encoder output; each step runs the training decoder stack
+    # (`_decode`) on one token per row, appends its self-attention K|V at the device-side slot kv_len - 1 (ops.kv_append) of
+    # a [layers, rows, cap, 2, heads, d_kv] cache and runs the split-KV decode kernel twice per layer: self-attention with
+    # the relative-position bias at the query's slot, cross-attention under the encoder padding mask. Every decode step is
+    # one CUDA-graph replay (fsb200/decode_graph.py); beam search gathers the self-attention cache into the twin
+    # (ops.kv_reorder). The cross-attention K|V is the same for every beam of an item and is not reordered.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); sequences start with
         decoder_start_token_id."""
         dev = self.flat.params.device
-        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        nh, dk = self.nh, self.dk
         P = self.P
         ids = input_ids.to(device=dev, dtype=torch.int64).contiguous()
         B, Se = ids.shape
@@ -232,94 +263,49 @@ class MT5ForConditionalGeneration(FlatModel):
                                    False, self.nbuckets, self.maxdist)
         enc_len = torch.full((1,), Se, dtype=torch.int32, device=dev)
         start = torch.full((R, 1), c.start, dtype=torch.int64, device=dev)
-        # the self-attention cache, and its twin for beam search
         caches = [torch.zeros((self.nd, R, cap, 2, nh, dk), dtype=torch.bfloat16, device=dev)
                   for _ in range(2 if c.num_beams > 1 else 1)]
         kv_len = torch.zeros(1, dtype=torch.int32, device=dev)
-        tok, index = start.view(-1).clone(), torch.zeros(R, dtype=torch.int64, device=dev)
 
-        def body(key):
-            src, reorder = key
-            cache = caches[1 - src] if reorder else caches[src]
-            if reorder:
-                ops.kv_reorder(caches[src], cache, index, kv_len)
+        def cross_attend(i, qc):
+            oc, lsec = ops.attn_decode(qc.view(R, nh, dk), cross[i][:, :, 0], cross[i][:, :, 1], enc_len, 1.0, kv_mask=cmask)
+            return oc, lsec, None
+
+        def body(tok, index, a, b):
+            if b is not a:
+                ops.kv_reorder(a, b, index, kv_len)
             kv_len.add_(1)
-            self._need("no_decay"); self._need("shared")
-            y, prev = ops.embedding_fwd(tok, P("shared.weight").data), None
-            for i in range(self.nd):
-                p = f"decoder.block.{i}.layer."
-                self._need(f"dec{i}")
-                h1, _, y = self._norm(prev, y, p + "0.layer_norm.weight")
-                q3 = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i]).view(R, 3, nh, dk)
-                kv = cache[i]
-                ops.kv_append(q3[:, 1], q3[:, 2], kv[:, :, 0], kv[:, :, 1], kv_len)
-                o, _ = ops.attn_decode(q3[:, 0], kv[:, :, 0], kv[:, :, 1], kv_len, 1.0, rel_bias=rel_d)
-                a = ops.gemm(L.GEMM_NT, o.view(R, inner), P(p + "0.SelfAttention.o.weight").data)
-                h2, _, y1 = self._norm(a, y, p + "1.layer_norm.weight")
-                qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
-                oc, _ = ops.attn_decode(qc.view(R, nh, dk), cross[i][:, :, 0], cross[i][:, :, 1], enc_len, 1.0,
-                                        kv_mask=cmask)
-                ac = ops.gemm(L.GEMM_NT, oc.view(R, inner), P(p + "1.EncDecAttention.o.weight").data)
-                h3, _, y2 = self._norm(ac, y1, p + "2.layer_norm.weight")
-                gu = ops.gemm(L.GEMM_NT, h3, self._d_wi[i])
-                act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
-                m = ops.gemm(L.GEMM_NT, act, P(p + "2.DenseReluDense.wo.weight").data)
-                y, prev = y2, m
-            self._need("head")
-            hf, _, _ = self._norm(prev, y, "decoder.final_layer_norm.weight")
+
+            def attend(i, q5):
+                kv = b[i]
+                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len)
+                return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, 1.0, rel_bias=rel_d)
+            hf, _, _ = self._decode(tok, R, 1, attend, cross_attend)
             return ops.gemm(L.GEMM_NT, hf, P(self._head).data).float()
 
-        graphs = DecodeGraphs(self, body)
-        live = [0]   # the twin holding the current cache
-
-        def step(tokens, reorder):
-            if tokens is not None:
-                tok.copy_(tokens)
-            src = live[0]
-            if reorder is not None:
-                index.copy_(reorder)
-                live[0] = 1 - src
-            return graphs((src, reorder is not None))
-
-        return generation.run(step, start, c)
+        graphs = DecodeGraphs(self, R, caches, body)
+        graphs.tok.copy_(start.view(-1))      # the first step decodes the start token
+        return generation.run(graphs, start, c)
 
     def _forward_impl(self, ids, dec_ids, mask, lab, B, Se, Sd, save, want_logits):
-        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        nh, dk = self.nh, self.dk
         P = self.P
-        Td = B * Sd
         self._need("no_decay"); self._need("shared")
-        W = P("shared.weight").data
         # relative-position bias vectors (fp32 [heads, 2S - 1]) from the two [buckets, heads] tables
         rel_e = TB.rel_bias_vector(P("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Se, Se, True,
                                    self.nbuckets, self.maxdist)
         rel_d = TB.rel_bias_vector(P("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Sd, Sd, False,
                                    self.nbuckets, self.maxdist)
         eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save)
-        # ---- decoder
-        y, prev = ops.embedding_fwd(dec_ids, W), None
-        dacts = []
-        for i in range(self.nd):
-            p = f"decoder.block.{i}.layer."
-            self._need(f"dec{i}")
-            h1, r1, y = self._norm(prev, y, p + "0.layer_norm.weight")
-            qkv = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i])
-            q5 = qkv.view(B, Sd, 3, nh, dk)
-            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True, rel_bias=rel_d)
-            a = ops.gemm(L.GEMM_NT, o.view(Td, inner), P(p + "0.SelfAttention.o.weight").data)
-            h2, r2, y1 = self._norm(a, y, p + "1.layer_norm.weight")
-            qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
+
+        def cross_attend(i, qc):
             kvc = ops.gemm(L.GEMM_NT, enc_h, self._d_kv[i])
             kv5 = kvc.view(B, Se, 2, nh, dk)
             oc, lsec = ops.sdpa_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, False, kv_mask=mask)
-            ac = ops.gemm(L.GEMM_NT, oc.view(Td, inner), P(p + "1.EncDecAttention.o.weight").data)
-            h3, r3, y2 = self._norm(ac, y1, p + "2.layer_norm.weight")
-            gu = ops.gemm(L.GEMM_NT, h3, self._d_wi[i])
-            act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
-            m = ops.gemm(L.GEMM_NT, act, P(p + "2.DenseReluDense.wo.weight").data)
-            if save:
-                dacts.append((y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, gu, act))
-            y, prev = y2, m
-        hf, rfd, xfd = self._norm(prev, y, "decoder.final_layer_norm.weight")
+            return oc, lsec, kvc
+        dacts = [] if save else None
+        hf, rfd, xfd = self._decode(dec_ids, B, Sd, lambda i, q5: ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True,
+                                                                              rel_bias=rel_d), cross_attend, dacts)
         logits = ops.gemm(L.GEMM_NT, hf, P(self._head).data)
         loss, ctx = None, None
         if lab is not None:

@@ -425,25 +425,12 @@ def attn_decode(q, k_cache, v_cache, kv_len, scale, kv_mask=None, rel_bias=None,
     if q.dim() != 3 or q.stride(2) != 1:
         raise RuntimeError("fsb200 attn_decode: q must be [batch, heads, dim] with unit inner stride")
     B, H, D = q.shape
-    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
-        if t.dim() != 4 or t.stride(3) != 1 or (t.shape[0], t.shape[2], t.shape[3]) != (B, H, D):
-            raise RuntimeError(f"fsb200 attn_decode: {n} must be [{B}, cap, {H}, {D}] with unit inner stride, "
-                               f"got {tuple(t.shape)} strides {t.stride()}")
-    cap = k_cache.shape[1]
-    if v_cache.shape[1] != cap:
-        raise RuntimeError("fsb200 attn_decode: k_cache and v_cache capacities differ")
-    _chk(kv_len, torch.int32, "kv_len")
-    if kv_len.numel() != 1:
-        raise RuntimeError("fsb200 attn_decode: kv_len must be a one-element int32 tensor")
+    cap = _chk_cache(k_cache, v_cache, kv_mask, kv_len, B, H, D, "attn_decode")
     if out is None:
         out = torch.empty((B, H, D), dtype=_bf16, device=q.device)
     _chk(out, _bf16, "out")
     if tuple(out.shape) != (B, H, D) or out.stride(2) != 1:
         raise RuntimeError("fsb200 attn_decode: out must be [batch, heads, dim] with unit inner stride")
-    if kv_mask is not None:
-        _chk(kv_mask, torch.uint8, "kv_mask")
-        if tuple(kv_mask.shape) != (B, cap) or not kv_mask.is_contiguous():
-            raise RuntimeError(f"fsb200 attn_decode: kv_mask must be contiguous uint8 [{B}, {cap}]")
     if rel_bias is not None:
         _chk_rel(rel_bias, H, cap, cap, "rel_bias")
     lse = torch.empty((B, H), dtype=torch.float32, device=q.device)
@@ -462,6 +449,24 @@ def _chk_kv_len(kv_len, what):
         raise RuntimeError(f"fsb200 {what}: kv_len must be a one-element int32 tensor")
 
 
+def _chk_cache(k_cache, v_cache, kv_mask, kv_len, B, H, D, what):
+    """The decode ops' cache operands: k_cache / v_cache [B, cap, H, D] (unit inner stride), kv_mask None or contiguous
+    uint8 [B, cap], kv_len a one-element int32 tensor. Returns cap."""
+    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
+        if t.dim() != 4 or t.stride(3) != 1 or (t.shape[0], t.shape[2], t.shape[3]) != (B, H, D):
+            raise RuntimeError(f"fsb200 {what}: {n} must be [{B}, cap, {H}, {D}] with unit inner stride, "
+                               f"got {tuple(t.shape)} strides {t.stride()}")
+    cap = k_cache.shape[1]
+    if v_cache.shape[1] != cap:
+        raise RuntimeError(f"fsb200 {what}: k_cache and v_cache capacities differ")
+    _chk_kv_len(kv_len, what)
+    if kv_mask is not None:
+        _chk(kv_mask, torch.uint8, "kv_mask")
+        if tuple(kv_mask.shape) != (B, cap) or not kv_mask.is_contiguous():
+            raise RuntimeError(f"fsb200 {what}: kv_mask must be contiguous uint8 [{B}, {cap}]")
+    return cap
+
+
 def kv_append(k_new, v_new, k_cache, v_cache, kv_len, kv_mask=None):
     """Write the newest token's keys / values k_new, v_new [B, H, D] (strided bf16 views, unit inner stride) into slot
     kv_len - 1 of k_cache / v_cache [B, cap, H, D] (strided views, e.g. the K and V halves of a [B, cap, 2, H, D] cache).
@@ -474,18 +479,7 @@ def kv_append(k_new, v_new, k_cache, v_cache, kv_len, kv_mask=None):
     B, H, D = k_new.shape
     if tuple(v_new.shape) != (B, H, D) or v_new.stride(2) != 1:
         raise RuntimeError(f"fsb200 kv_append: v_new must be [{B}, {H}, {D}] with unit inner stride")
-    for t, n in ((k_cache, "k_cache"), (v_cache, "v_cache")):
-        if t.dim() != 4 or t.stride(3) != 1 or (t.shape[0], t.shape[2], t.shape[3]) != (B, H, D):
-            raise RuntimeError(f"fsb200 kv_append: {n} must be [{B}, cap, {H}, {D}] with unit inner stride, "
-                               f"got {tuple(t.shape)} strides {t.stride()}")
-    cap = k_cache.shape[1]
-    if v_cache.shape[1] != cap:
-        raise RuntimeError("fsb200 kv_append: k_cache and v_cache capacities differ")
-    _chk_kv_len(kv_len, "kv_append")
-    if kv_mask is not None:
-        _chk(kv_mask, torch.uint8, "kv_mask")
-        if tuple(kv_mask.shape) != (B, cap) or not kv_mask.is_contiguous():
-            raise RuntimeError(f"fsb200 kv_append: kv_mask must be contiguous uint8 [{B}, {cap}]")
+    cap = _chk_cache(k_cache, v_cache, kv_mask, kv_len, B, H, D, "kv_append")
     L.call("fsb_kv_append", _p(k_new), _p(v_new), _p(k_cache), _p(v_cache), _p(kv_mask), B, H, D, cap, _p(kv_len),
            k_new.stride(0), k_new.stride(1), v_new.stride(0), v_new.stride(1), k_cache.stride(0), k_cache.stride(1),
            k_cache.stride(2), v_cache.stride(0), v_cache.stride(1), v_cache.stride(2), _stream())

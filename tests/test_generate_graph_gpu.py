@@ -240,6 +240,31 @@ def test_host_calls_do_not_grow_with_new_tokens(kind, monkeypatch):
     assert counts["1"][1] < counts["0"][1] - 15 * per_step
 
 
+@pytest.mark.parametrize("kind", ["gpt2", "mt5", "llama"])
+def test_generate_releases_its_memory_on_return(kind, monkeypatch):
+    """The caches (the beam twin included), the static buffers and the graphs of a `generate` call are freed when it
+    returns, by reference counting alone: no reference cycle holds them until the garbage collector runs."""
+    import gc
+    m = {"gpt2": _gpt2, "mt5": _mt5, "llama": _llama}[kind]()
+    ids = torch.randint(4, V, (2, 16), generator=torch.Generator().manual_seed(3)).cuda()
+    if kind == "llama":
+        gen = lambda: m.generate(ids, max_length=16 + 8)                                          # noqa: E731
+    else:
+        gen = lambda: m.generate(input_ids=ids, max_new_tokens=8, num_beams=2, eos_token_id=V)   # noqa: E731
+    monkeypatch.setenv("FSB_GENERATE_GRAPH", "1")
+    gen()                              # workspaces and tables that persist across calls
+    torch.cuda.synchronize()
+    gc.collect()
+    gc.disable()
+    try:
+        base = torch.cuda.memory_allocated()
+        gen()
+        torch.cuda.synchronize()
+        assert torch.cuda.memory_allocated() == base
+    finally:
+        gc.enable()
+
+
 def test_parameters_updated_between_calls_are_seen(monkeypatch):
     """A training step between two generate calls: the graphed decode reads the updated weights (it equals the eager decode
     after the step, and differs from the decode before it)."""

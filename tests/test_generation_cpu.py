@@ -213,11 +213,6 @@ def test_unsupported_keywords_raise(kw, t5):
     G.resolve(t5.config, dict(num_beam_groups=1, no_repeat_ngram_size=0, force_words_ids=None), 1, True)
 
 
-def test_llama_pick_is_the_controller_pick():
-    from fsb200.models.llama import LlamaForCausalLM
-    assert LlamaForCausalLM._pick is G.pick
-
-
 def test_fixtures_are_not_echoes(t5, gpt2):
     """The parity cases above only test something when the fixtures' continuations depend on their input: greedy rows that
     are not a repeat of their last input token and several distinct tokens per batch, beams whose scores are not 0 (a certain continuation), and sampling distributions that
