@@ -150,6 +150,10 @@ int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* 
                   const uint32_t* box) {
   return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box);
 }
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box);
+}
 
 }  // namespace fsb
 

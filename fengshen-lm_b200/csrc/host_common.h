@@ -38,6 +38,8 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
                    const uint32_t* box);
 int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                   const uint32_t* box);
+int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box);
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

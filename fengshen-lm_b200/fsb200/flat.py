@@ -60,13 +60,14 @@ class FlatSpec:
 
 
 class FlatBuffers:
-    """Owns the flat bf16 parameter and gradient buffers and hands out views."""
+    """Owns the flat bf16 parameter and gradient buffers and hands out views. grads=False allocates no gradient buffer
+    (`grads` is None): a model that only runs inference (an int8 LLaMA) then holds its parameters alone."""
 
-    def __init__(self, spec, device, world_size=1, grad_dtype=torch.bfloat16):
+    def __init__(self, spec, device, world_size=1, grad_dtype=torch.bfloat16, grads=True):
         self.offsets, self.buckets, self.total = spec.plan(world_size)
         self.world_size = world_size
         self.params = torch.zeros(self.total, dtype=torch.bfloat16, device=device)
-        self.grads = torch.zeros(self.total, dtype=grad_dtype, device=device)
+        self.grads = torch.zeros(self.total, dtype=grad_dtype, device=device) if grads else None
         self.bucket_index = {b: i for i, (b, _, _, _) in enumerate(self.buckets)}
         # gradient-space layout: identical to the parameter layout until compact_grads() folds the per-layer buckets
         # onto rotating slots (ZeRO-2: a full-size gradient buffer never exists)
@@ -92,6 +93,8 @@ class FlatBuffers:
         return self.grad_bucket_start[i] + (off - self.buckets[i][1])
 
     def _grad_view(self, off, shape):
+        if self.grads is None:
+            raise RuntimeError("fsb200: these flat buffers were built without a gradient buffer")
         g = self._grad_off(off)
         t = self.grads[g:g + _numel(shape)].view(shape)
         self._grad_views.append((t, off, tuple(shape)))
@@ -144,6 +147,8 @@ class FlatBuffers:
         "gradients are partitioned as they are produced" (SURVEY.md Appendix D) instead of a full-size buffer. Every grad view
         handed out so far (prm.main_grad, fused-operand spans) is re-pointed in place. Returns the bytes released."""
         import re
+        if self.grads is None:
+            return 0
         fam = {}
         for i, (name, _, length, _) in enumerate(self.buckets):
             m = re.fullmatch(r"(.*?)(\d+)", name)

@@ -19,12 +19,14 @@ class _Holder(nn.Module):
 
 def bind_flat_parameters(module, flat):
     """Register every entry of `flat` on `module`, in flat-layout order, as an nn.Parameter over its view with `.main_grad`
-    over its gradient view, under its dotted name: `a.b.weight` becomes module.a.b.weight, and an integer component an
-    nn.ModuleList entry (`transformer.h.3.*` -> module.transformer.h[3]). The parameters are also kept by name in module._p."""
+    over its gradient view (when `flat` has a gradient buffer), under its dotted name: `a.b.weight` becomes module.a.b.weight,
+    and an integer component an nn.ModuleList entry (`transformer.h.3.*` -> module.transformer.h[3]). The parameters are also
+    kept by name in module._p."""
     module._p = {}
     for name in flat.offsets:
-        prm = nn.Parameter(flat.view(name))
-        prm.main_grad = flat.view(name, grad=True)
+        prm = nn.Parameter(flat.view(name), requires_grad=flat.grads is not None)
+        if flat.grads is not None:
+            prm.main_grad = flat.view(name, grad=True)
         module._p[name] = prm
         parts = name.split(".")
         mod = module
@@ -72,9 +74,10 @@ class FlatModel(nn.Module):
         self.loss_scale = 1.0           # 1 / (gradient_accumulation_steps * world_size), folded into dlogits
         self.grad_hook = None           # engine callback: grad_hook(bucket) when a bucket's gradients are final
 
-    def _bind_flat(self, spec, device=None, world_size=None, tp=1):
+    def _bind_flat(self, spec, device=None, world_size=None, tp=1, grads=True):
         """Allocate the flat buffers for `spec` and bind every entry. `world_size` is the data-parallel size the buckets are
-        padded for: by default the initialised process group's size over the tensor-parallel size `tp`."""
+        padded for: by default the initialised process group's size over the tensor-parallel size `tp`. grads=False: no
+        gradient buffer (inference-only models)."""
         if world_size is None:   # laid out for the job's data-parallel world (the scripts build the model in setup())
             import torch.distributed as dist
             world_size = (dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1) // tp
@@ -82,7 +85,7 @@ class FlatModel(nn.Module):
                            if torch.cuda.is_available() else "cuda")
         if dev.type != "cuda":
             raise RuntimeError(f"fsb200 {type(self).__name__} runs on CUDA only (no CPU fallback on the product path)")
-        self.flat = FlatBuffers(spec, dev, world_size=world_size)
+        self.flat = FlatBuffers(spec, dev, world_size=world_size, grads=grads)
         bind_flat_parameters(self, self.flat)
 
     def P(self, name):

@@ -35,18 +35,34 @@ def _init_normal_(t, std, gen):
     t.copy_(torch.empty(t.shape, dtype=torch.float32).normal_(0.0, std, generator=gen).to(t.dtype))
 
 
+_W8_NAMES = ("attention.query_key_value.weight", "attention.dense.weight", "mlp.w1.weight", "mlp.w3.weight", "mlp.w2.weight")
+
+
+def _int8_unsupported(what):
+    return NotImplementedError(f"fsb200 LlamaForCausalLM: {what} is not implemented for an int8 (load_in_8bit=True) model; "
+                               "it only runs inference")
+
+
 class LlamaForCausalLM(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None):
+    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False):
         """tp_group: the tensor-model-parallel process group (mpu.get_model_parallel_group()) or None. With t = its size > 1
         this rank holds the shard the reference's `part_{rank}` checkpoints hold (utils/llama_convert/convert_fs_llama_tp.py
         :143-181): heads / ff columns / vocabulary rows split t ways (ColumnParallelLinear mpu/layers.py:261-360 for QKV,
         w1, w3 and the LM head; RowParallelLinear :363-470 for dense and w2; VocabParallelEmbedding :62-130), norms replicated.
-        `world_size` is then the DATA-parallel size (ranks that share a tensor-parallel rank)."""
+        `world_size` is then the DATA-parallel size (ranks that share a tensor-parallel rank).
+
+        load_in_8bit: an inference-only model (`from_pretrained(..., load_in_8bit=True)`, examples/ziya_inference/
+        hf_quantizatin_inference.py:20-22). Each layer's four projections (query_key_value, dense, w1 | w3, w2) are held as
+        int8 q [n, k] + fp32 per-row scales s [n] and run through the W8A16 GEMM; the embedding, the norm scales and the LM
+        head stay bf16 in flat buffers without a gradient buffer. Training, tensor parallelism and save_pretrained raise."""
         super().__init__(config)
         import torch.distributed as dist
+        self.load_in_8bit = bool(load_in_8bit)
         self.tp_group = tp_group
         self.tp = dist.get_world_size(tp_group) if tp_group is not None else 1
         self.tp_rank = dist.get_rank(tp_group) if tp_group is not None else 0
+        if self.load_in_8bit and self.tp > 1:
+            raise _int8_unsupported("tensor parallelism")
         h, V, nl, nh = config.hidden_size, config.vocab_size, config.num_hidden_layers, config.num_attention_heads
         self.h, self.V, self.nl, self.nh = h, V, nl, nh
         self.hn = h // nh
@@ -69,23 +85,34 @@ class LlamaForCausalLM(FlatModel):
         for i in range(nl):
             p, bk = f"llama.layers.{i}.", f"layer{i}"
             spec.add(p + "input_layernorm.scale", (h,), bk)          # *.scale names match 'layernorm.' -> no-decay bucket
-            spec.add(p + "attention.query_key_value.weight", (3 * self.h_l, h), bk)
-            spec.add(p + "attention.dense.weight", (h, self.h_l), bk)
+            if not self.load_in_8bit:
+                spec.add(p + "attention.query_key_value.weight", (3 * self.h_l, h), bk)
+                spec.add(p + "attention.dense.weight", (h, self.h_l), bk)
             spec.add(p + "post_attention_layernorm.scale", (h,), bk)
-            spec.add(p + "mlp.w1.weight", (self.ff_l, h), bk)   # w1 | w3 adjacent: one [2ff, h] GEMM operand
-            spec.add(p + "mlp.w3.weight", (self.ff_l, h), bk)
-            spec.add(p + "mlp.w2.weight", (h, self.ff_l), bk)
+            if not self.load_in_8bit:
+                spec.add(p + "mlp.w1.weight", (self.ff_l, h), bk)   # w1 | w3 adjacent: one [2ff, h] GEMM operand
+                spec.add(p + "mlp.w3.weight", (self.ff_l, h), bk)
+                spec.add(p + "mlp.w2.weight", (h, self.ff_l), bk)
         spec.add("llama.final_layer_norm.scale", (h,), "head")
         spec.add("embed_out.final_linear.weight", (self.V_l, h), "head")
-        self._bind_flat(spec, device, world_size, tp=self.tp)
-        self._w13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h)
-                     for i in range(nl)]
-        self._dw13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h, grad=True) for i in range(nl)]
+        self._bind_flat(spec, device, world_size, tp=self.tp, grads=not self.load_in_8bit)
+        if self.load_in_8bit:
+            # per layer {projection: (q int8 [n, k], s fp32 [n])}; w1 | w3 is one [2ff, h] operand as in the bf16 layout
+            dev = self.flat.params.device
+            shapes = {"qkv": (3 * h, h), "dense": (h, h), "w13": (2 * self.ff, h), "w2": (h, self.ff)}
+            self._w8 = [{k: (torch.zeros(n_k, dtype=torch.int8, device=dev), torch.zeros(n_k[0], dtype=torch.float32, device=dev))
+                         for k, n_k in shapes.items()} for _ in range(nl)]
+        else:
+            self._w13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h)
+                         for i in range(nl)]
+            self._dw13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h, grad=True) for i in range(nl)]
 
         # RoPE tables exactly as RotaryEmbedding builds them (layers/positional_embeddings.py:38-52), fp32; inv_freq is also a
         # buffer of every layer in the reference's module tree (modeling_llama.py:97-127), hence in its state dict
         self._inv_freq = 1.0 / (getattr(config, "rotary_emb_base", 10000) ** (torch.arange(0, self.hn, 2).float() / self.hn))
         for lyr in self.llama.layers:
+            if "attention" not in lyr._modules:    # int8: the projections live outside the flat buffers
+                lyr.attention = _Holder()
             lyr.attention.rotary_emb = _Holder()
             lyr.attention.rotary_emb.register_buffer("inv_freq", self._inv_freq.clone().to(self.flat.params.device))
         self._rope_rows = 0
@@ -121,6 +148,94 @@ class LlamaForCausalLM(FlatModel):
                 prm.normal_(0.0, std, generator=gen)
             else:
                 _init_normal_(prm.data, std, gen)
+        if self.load_in_8bit:   # each int8 matrix: drawn in bf16 on the device and quantised, one temporary at a time
+            dgen = torch.Generator(device=self.flat.params.device).manual_seed(seed + 104729)
+            for w8 in self._w8:
+                for key, (q, s) in w8.items():
+                    tmp = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
+                    tmp.normal_(0.0, wang if key in ("dense", "w2") else small, generator=dgen)
+                    ops.quantize_w8(tmp, q, s)
+                    del tmp
+
+    # ---- int8 (load_in_8bit) ------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def load_reference_state_dict(self, sd):
+        """As FlatModel.load_reference_state_dict; an int8 model quantises each projection on the device as it arrives."""
+        if not self.load_in_8bit:
+            return super().load_reference_state_dict(sd)
+        targets = set(self._p) | set(self._w8_targets())
+        missing = targets - set(sd)
+        if missing:
+            raise KeyError(f"missing key in state dict: {sorted(missing)[0]}")
+        self._load_w8_shard(sd, set())
+
+    def _w8_targets(self):
+        """{state-dict key: (q, s) row slice it quantises into} of every int8 projection."""
+        out, ff = {}, self.ff
+        for i, w8 in enumerate(self._w8):
+            p = f"llama.layers.{i}."
+            (qq, sq), (qd, sd_), (q13, s13), (q2, s2) = w8["qkv"], w8["dense"], w8["w13"], w8["w2"]
+            out[p + _W8_NAMES[0]] = (qq, sq)
+            out[p + _W8_NAMES[1]] = (qd, sd_)
+            out[p + _W8_NAMES[2]] = (q13[:ff], s13[:ff])
+            out[p + _W8_NAMES[3]] = (q13[ff:], s13[ff:])
+            out[p + _W8_NAMES[4]] = (q2, s2)
+        return out
+
+    @torch.no_grad()
+    def _load_w8_shard(self, sd, loaded):
+        """Load the keys of `sd` (a whole state dict or one checkpoint shard) this int8 model holds: bf16 parameters are
+        copied, projections quantised on the device (one bf16 temporary at a time). The shard's shapes are checked before
+        anything is written. Adds the loaded keys to the set `loaded` and returns the keys it does not yet hold."""
+        targets = self._w8_targets()
+        for k, v in sd.items():
+            want = tuple(self._p[k].shape) if k in self._p else tuple(targets[k][0].shape) if k in targets else None
+            if want is not None and tuple(v.shape) != want:
+                raise ValueError(f"shape mismatch for {k}: {tuple(v.shape)} vs {want}")
+        for k, v in sd.items():
+            v = v if v.dtype == torch.bfloat16 else v.to(torch.bfloat16)   # converted where it lies: one bf16 copy on the device
+            if k in self._p:
+                self._p[k].copy_(v)
+            elif k in targets:
+                q, s = targets[k]
+                tmp = v.to(q.device).contiguous()
+                ops.quantize_w8(tmp, q, s)
+                del tmp
+            else:
+                continue
+            loaded.add(k)
+        return (set(self._p) | set(targets)) - loaded
+
+    def get_memory_footprint(self):
+        """Bytes held by the model's tensors: parameters (and their gradient buffer, if any), int8 weights and scales, and
+        buffers (transformers' `PreTrainedModel.get_memory_footprint`, which hf_quantizatin_inference.py prints)."""
+        n = self.flat.params.numel() * self.flat.params.element_size()
+        if self.flat.grads is not None:
+            n += self.flat.grads.numel() * self.flat.grads.element_size()
+        for w8 in getattr(self, "_w8", ()):
+            n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in w8.values())
+        return n + sum(b.numel() * b.element_size() for b in self.buffers())
+
+    def save_pretrained(self, path, **kw):
+        if self.load_in_8bit:
+            raise _int8_unsupported("save_pretrained (int8 export)")
+        return super().save_pretrained(path, **kw)
+
+    def _linear(self, i, name, x):
+        """x @ W^T for layer i's projection `name` (qkv, dense, w13, w2): the bf16 GEMM, or the W8A16 GEMM of an int8 model."""
+        if self.load_in_8bit:
+            q, s = self._w8[i][name]
+            return ops.gemm_w8a16(x, q, s)
+        lyr = self.llama.layers[i]
+        if name == "qkv":
+            w = lyr.attention.query_key_value.weight.data
+        elif name == "dense":
+            w = lyr.attention.dense.weight.data
+        elif name == "w13":
+            w = self._w13[i]
+        else:
+            w = lyr.mlp.w2.weight.data
+        return ops.gemm(L.GEMM_NT, x, w)
 
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, labels=None, return_logits=False, **_):
@@ -143,6 +258,8 @@ class LlamaForCausalLM(FlatModel):
                                     "fsb200 LlamaForCausalLM: position_ids outside [0, rope table rows); pass them on the "
                                     "host or raise config.max_position_embeddings")
         lab = flat_ids(labels, dev)
+        if self.load_in_8bit and lab is not None and torch.is_grad_enabled():
+            raise _int8_unsupported("a training forward (labels under grad mode)")
         loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
@@ -181,16 +298,16 @@ class LlamaForCausalLM(FlatModel):
             self._need(f"layer{i}")
             h1, rstd1, x = ops.rmsnorm_fwd(x if prev_m is None else prev_m, lyr.input_layernorm.scale.data, self.eps,
                                            residual=None if prev_m is None else x)
-            qkv = ops.gemm(L.GEMM_NT, h1, lyr.attention.query_key_value.weight.data)
+            qkv = self._linear(i, "qkv", h1)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
             o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
-            a = ops.gemm(L.GEMM_NT, o.view(B * S, hl), lyr.attention.dense.weight.data)
+            a = self._linear(i, "dense", o.view(B * S, hl))
             self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
             h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
-            gu = ops.gemm(L.GEMM_NT, h2, self._w13[i])
+            gu = self._linear(i, "w13", h2)
             act = ops.glu_fwd(L.ACT_SILU, gu[:, :ff], gu[:, ff:])
-            m = ops.gemm(L.GEMM_NT, act, lyr.mlp.w2.weight.data)
+            m = self._linear(i, "w2", act)
             self._tp_all_reduce(m)        # RowParallelLinear (w2)
             if acts is not None:
                 acts.append((x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, gu, act))
@@ -216,18 +333,27 @@ class LlamaForCausalLM(FlatModel):
     @torch.no_grad()
     def generate(self, input_ids, attention_mask=None, max_length=None, max_new_tokens=None, do_sample=False,
                  temperature=1.0, top_k=0, top_p=1.0, repetition_penalty=1.0, pad_token_id=None, eos_token_id=None,
-                 generator=None, **_):
+                 generator=None, num_return_sequences=1, **_):
         """Greedy / sampling decode with a KV cache; the keyword surface `llama_generate.generate` passes to HF's
-        `model.generate` (do_sample, top_p, top_k, max_length, repetition_penalty, temperature, pad_token_id, eos_token_id).
-        Prompts are LEFT-padded (attention_mask 0 on the pads). Returns [batch, <= max_length] token ids, prompt included,
-        finished rows filled with pad_token_id — HF's GenerationMixin conventions, selected by fsb200/generation.py."""
+        `model.generate` (do_sample, top_p, top_k, max_length, repetition_penalty, temperature, pad_token_id, eos_token_id),
+        plus num_return_sequences (sampling only; each prompt repeated in place, HF's `_expand_inputs_for_generation`), which
+        hf_quantizatin_inference.py passes. Prompts are LEFT-padded (attention_mask 0 on the pads). Returns
+        [batch * num_return_sequences, <= max_length] token ids, prompt included, finished rows filled with pad_token_id —
+        HF's GenerationMixin conventions, selected by fsb200/generation.py."""
         if self.tp > 1:
             raise NotImplementedError("fsb200: KV-cache decoding under tensor parallelism is not implemented")
+        nrs = int(num_return_sequences or 1)
+        if nrs > 1 and not do_sample:
+            raise ValueError("fsb200 generate: greedy search with `num_return_sequences` > 1 returns identical rows; "
+                             "set do_sample=True")
         dev = self.device
         ids = input_ids.to(device=dev, dtype=torch.int64)
         B, S0 = ids.shape
         mask = torch.ones((B, S0), dtype=torch.uint8, device=dev) if attention_mask is None else \
             attention_mask.to(device=dev).to(torch.uint8)
+        if nrs > 1:
+            ids, mask = ids.repeat_interleave(nrs, 0), mask.repeat_interleave(nrs, 0)
+            B *= nrs
         if max_length is None:
             max_length = S0 + (max_new_tokens if max_new_tokens is not None else 20)
         if max_length <= S0:

@@ -96,6 +96,42 @@ def gemm(layout, a, b, out=None, out_dtype=_bf16, bias=None, epilogue=L.EPI_NONE
     return out
 
 
+def quantize_w8(w, q=None, s=None):
+    """Symmetric per-output-channel int8 quantisation of a bf16 weight w[n, k] (unit inner stride) -> (q int8 [n, k]
+    contiguous, s fp32 [n]) with s = absmax / 127 and q = clamp(rint(w / s), -127, 127) (include/fsb200.h). q and s may be
+    given (contiguous, e.g. row slices of a larger operand) to quantise in place of a new allocation."""
+    _chk(w, _bf16, "w")
+    n, k, ldw = _rows2d(w, "w")
+    q = torch.empty((n, k), dtype=torch.int8, device=w.device) if q is None else q
+    s = torch.empty((n,), dtype=torch.float32, device=w.device) if s is None else s
+    _chk(q, torch.int8, "q"); _chk(s, torch.float32, "s")
+    if tuple(q.shape) != (n, k) or not q.is_contiguous() or tuple(s.shape) != (n,) or not s.is_contiguous():
+        raise RuntimeError(f"fsb200 quantize_w8: q must be contiguous [{n}, {k}] and s contiguous [{n}]")
+    L.call("fsb_quantize_w8", _p(w), ldw, n, k, _p(q), _p(s), _stream())
+    return q, s
+
+
+def gemm_w8a16(a, q, s, out=None):
+    """out[m, n] = bf16(s[n] * (a[m, k] @ q[n, k]^T)), fp32 accumulation: a bf16 (unit inner stride), q int8 [n, k]
+    contiguous and s fp32 [n] as quantize_w8 returns them. `out` (bf16, unit inner stride) may be a strided view."""
+    _chk(a, _bf16, "a"); _chk(q, torch.int8, "q"); _chk(s, torch.float32, "s")
+    m, k, lda = _rows2d(a, "a")
+    if q.dim() != 2 or not q.is_contiguous(): raise RuntimeError("fsb200 gemm_w8a16: q must be contiguous [n, k]")
+    n = q.shape[0]
+    if q.shape[1] != k: raise RuntimeError(f"fsb200 gemm_w8a16: K mismatch {k} vs {q.shape[1]}")
+    if tuple(s.shape) != (n,) or not s.is_contiguous(): raise RuntimeError("fsb200 gemm_w8a16: s must be contiguous [n]")
+    if out is None:
+        out = torch.empty((m, n), dtype=_bf16, device=a.device)
+    _chk(out, _bf16, "out")
+    orr, occ, ldd = _rows2d(out, "out")
+    if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_w8a16: out shape {tuple(out.shape)} != ({m},{n})")
+    ws_bytes = int(L.load().fsb_gemm_w8a16_workspace_bytes(m, n, k))
+    ws = workspace(ws_bytes, a.device, "gemm_w8a16") if ws_bytes else None
+    L.call("fsb_gemm_w8a16", m, n, k, _p(a), lda, _p(q), _p(s), _p(out), ldd, _p(ws), ws_bytes, _stream(),
+           tag=f"{m}x{n}x{k}" if L.call_profiler is not None else None)
+    return out
+
+
 def set_reserved_sms(n):
     """Leave n SMs (2n for CTA-pair kernels) of every persistent GEMM grid to overlapping communication kernels."""
     L.call("fsb_set_reserved_sms", int(n))

@@ -83,6 +83,26 @@ int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K,
 size_t fsb_gemm_workspace_bytes(int layout, int64_t M, int64_t N, int64_t K);
 int fsb_set_reserved_sms(int n);
 
+/* ---- int8 weight-only inference (W8A16) ------------------------------------------------------------------------
+ * Stand in for `from_pretrained(..., load_in_8bit=True)` (fengshen/examples/ziya_inference/hf_quantizatin_inference.py:20-22),
+ * whose Linear layers bitsandbytes replaces with Linear8bitLt (third party). Weight-only: activations stay bf16, there is
+ * no outlier decomposition, so results are not bit-comparable with bitsandbytes.
+ *
+ * fsb_quantize_w8: symmetric per-output-channel quantisation of W bf16 [n, k] (row stride ldw >= k):
+ *   s[r] = absmax(W[r, :]) / 127.0f (IEEE fp32 division); q[r, c] = clamp(rint(W[r, c] / s[r]), -127, 127), rint rounding
+ *   half to even, the division IEEE fp32. A zero row gives s = 0, q = 0. q: int8 [n, k] row-major contiguous; s: fp32 [n].
+ * fsb_gemm_w8a16: D[m, n] = bf16(s[n] * sum_k A[m, k] q[n, k]), fp32 accumulation. A bf16 [m, k] (row stride lda), q / s as
+ *   fsb_quantize_w8 writes them, D bf16 [m, n] (row stride ldd); rows of D at or beyond m and columns beyond n are not
+ *   written. Requirements: k % 16 == 0, n % 8 == 0, lda >= k and ldd >= n multiples of 8, a / q / s / d 16-byte aligned.
+ *   Any m >= 1; one kernel serves decode (m of 1-32) and prefill. Calls whose output tiles leave SMs idle split K: fp32
+ *   partials go to the caller's `workspace` (fsb_gemm_w8a16_workspace_bytes(m, n, k) bytes, 0 when the call does not split)
+ *   and are summed in a fixed order. The plan depends on (m, n, k) and the SM count only: results are deterministic. A
+ *   split call with too small a workspace is an error. */
+int fsb_quantize_w8(const void* w, int64_t ldw, int64_t n, int64_t k, int8_t* q, float* s, fsb_stream_t stream);
+size_t fsb_gemm_w8a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
+int fsb_gemm_w8a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const int8_t* q, const float* s,
+                   void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
+
 /* ---- RMSNorm / LayerNorm ------------------------------------------------------------------------------------
  * RMSNorm.forward fengshen/models/megatron/layers/norms.py:44-52 (y = scale * cast(x * rsqrt(mean(x^2) + eps)), the cast to
  * 16 bit happening BEFORE the scale multiply); LayerNorm = torch.nn.LayerNorm (norms.py:16; HF BERT/GPT-2 eps 1e-12/1e-5).

@@ -1,0 +1,190 @@
+"""Int8 weight-only (W8A16) LLaMA inference on one GPU.
+
+1. Kernel A/B: fsb_gemm_w8a16 against fsb_gemm_bf16 (NT) on the Ziya-LLaMA-13B projection shapes (n, k) = (15360, 5120)
+   query_key_value, (5120, 5120) dense, (27648, 5120) w1|w3, (5120, 13824) w2, at m = 1, 8, 32 token rows (decode) and 4096
+   (prefill). Device time per call: 50 calls captured in one CUDA graph, the graph replayed under CUDA events; the two
+   kernels alternated `--reps` times, medians reported. Bytes per call: int8 n*k + 4n (weights and scales) + 2mk + 2mn,
+   bf16 2nk + 2mk + 2mn; GB/s and the share of the 3.35 TB/s HBM3 data-sheet figure for m <= 32, TFLOP/s (2mnk) at 4096.
+2. End to end: `generate` at Ziya width (hidden 5120, 40 heads, ff 13824, vocabulary 39424), prompt 512, 128 new tokens,
+   batch 1 and 8, greedy, random weights: bf16 and int8 at 8 of the 40 layers, int8 at all 40. Tokens/s (host wall clock,
+   median of `--reps`), device time per new token (torch.profiler, prefill included, separate run), host `fsb_*` calls per
+   new token, and the peak of torch.cuda.max_memory_allocated over building the model and generating, above what was
+   allocated before.
+
+  python tools/bench_int8.py [--reps 3] [--skip-e2e] [--out DIR]
+
+Prints one JSON line per measurement, the card's name, power limit and max SM clock first; --out also writes them to
+DIR/bench_int8.jsonl."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from types import SimpleNamespace
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+import __graft_entry__  # noqa: E402,F401  (puts the package on sys.path)
+from fsb200 import lib as L  # noqa: E402
+from fsb200 import ops  # noqa: E402
+from fsb200.models.llama import LlamaForCausalLM  # noqa: E402
+
+HBM = 3.35e12
+ZIYA = dict(vocab_size=39424, hidden_size=5120, num_attention_heads=40)
+SHAPES = (("qkv", 15360, 5120), ("dense", 5120, 5120), ("w1w3", 27648, 5120), ("w2", 5120, 13824))
+
+
+def card():
+    p = torch.cuda.get_device_properties(torch.cuda.current_device())
+    bus = f"{p.pci_domain_id:08X}:{p.pci_bus_id:02X}:{p.pci_device_id:02X}.0"
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", bus],
+                       capture_output=True, text=True, check=True)
+    name, power, clock = (s.strip() for s in q.stdout.strip().split(","))
+    return dict(gpu=name, power_limit=power, max_sm_clock=clock)
+
+
+def graph_us(fn, calls=50, reps=20):
+    """Device time of one call: `calls` calls captured in a CUDA graph, replayed `reps` times between CUDA events."""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(calls):
+            fn()
+    g.replay()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        g.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return 1e3 * e0.elapsed_time(e1) / (reps * calls)
+
+
+def kernel_ab(reps, emit):
+    gen = torch.Generator(device="cuda").manual_seed(0)
+    for name, n, k in SHAPES:
+        w = (torch.randn((n, k), generator=gen, device="cuda") * 0.02).to(torch.bfloat16)
+        q, s = ops.quantize_w8(w)
+        for m in (1, 8, 32, 4096):
+            a = torch.randn((m, k), generator=gen, device="cuda").to(torch.bfloat16)
+            d8 = torch.empty((m, n), dtype=torch.bfloat16, device="cuda")
+            d16 = torch.empty((m, n), dtype=torch.bfloat16, device="cuda")
+            f16 = lambda: ops.gemm(L.GEMM_NT, a, w, out=d16)            # noqa: E731  (the decode step's bf16 call)
+            f8 = lambda: ops.gemm_w8a16(a, q, s, out=d8)                # noqa: E731
+            t16, t8 = [], []
+            for _ in range(reps):
+                t16.append(graph_us(f16))
+                t8.append(graph_us(f8))
+            t16, t8 = sorted(t16)[reps // 2], sorted(t8)[reps // 2]
+            # the int8 result against the bf16 GEMM of the dequantised weight (a sanity figure, not a test)
+            ref = ops.gemm(L.GEMM_NT, a, (q.float() * s[:, None]).to(torch.bfloat16)).float()
+            rel = float((d8.float() - ref).abs().max() / ref.abs().max().clamp_min(1e-30))
+            b8 = n * k + 4 * n + 2 * m * k + 2 * m * n
+            b16 = 2 * n * k + 2 * m * k + 2 * m * n
+            line = dict(bench="gemm_w8a16_ab", shape=name, m=m, n=n, k=k, bf16_us=round(t16, 2), int8_us=round(t8, 2),
+                        speedup=round(t16 / t8, 3), splitk_workspace_bytes=int(L.load().fsb_gemm_w8a16_workspace_bytes(m, n, k)),
+                        max_rel_diff_vs_dequantised_bf16=rel, reps=reps)
+            if m <= 32:
+                line.update(int8_GBps=round(b8 / t8 / 1e3, 1), bf16_GBps=round(b16 / t16 / 1e3, 1),
+                            int8_share_of_hbm=round(b8 / (t8 * 1e-6) / HBM, 3), bf16_share_of_hbm=round(b16 / (t16 * 1e-6) / HBM, 3))
+            else:
+                line.update(int8_TFLOPs=round(2 * m * n * k / t8 / 1e6, 1), bf16_TFLOPs=round(2 * m * n * k / t16 / 1e6, 1))
+            emit(line)
+            del a, d8, d16, ref
+        del w, q, s
+        torch.cuda.empty_cache()
+
+
+def _count_calls():
+    n = [0]
+    real = L.call
+
+    def counted(name, *args, **kw):
+        n[0] += 1
+        return real(name, *args, **kw)
+    L.call = counted
+    return n
+
+
+def end_to_end(reps, emit, S=512, new=128):
+    calls = _count_calls()
+    for layers, int8 in ((8, False), (8, True), (40, True)):
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
+        base = torch.cuda.memory_allocated()
+        torch.cuda.reset_peak_memory_stats()
+        cfg = SimpleNamespace(num_hidden_layers=layers, rms_norm_epsilon=1e-6, max_position_embeddings=2048,
+                              rotary_emb_base=10000, llama_mlp_multiple_of=256, **ZIYA)
+        t0 = time.perf_counter()
+        model = LlamaForCausalLM(cfg, device="cuda", world_size=1, load_in_8bit=int8)
+        torch.cuda.synchronize()
+        build_s = time.perf_counter() - t0
+        for B in (1, 8):
+            ids = torch.randint(2, ZIYA["vocab_size"] - 8, (B, S), generator=torch.Generator().manual_seed(1)).cuda()
+            gen = lambda: model.generate(ids, max_length=S + new)     # noqa: E731
+            out = gen()                                                # warm-up: workspaces, graph capture paths
+            assert out.shape == (B, S + new), out.shape
+            wall = []
+            for _ in range(reps):
+                torch.cuda.synchronize()
+                calls[0] = 0
+                t0 = time.perf_counter()
+                gen()
+                torch.cuda.synchronize()
+                wall.append(time.perf_counter() - t0)
+            ncalls = calls[0]
+            from torch.profiler import ProfilerActivity, profile
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                gen()
+                torch.cuda.synchronize()
+            dev_us = sum(e.self_device_time_total for e in prof.key_averages())
+            w = sorted(wall)[len(wall) // 2]
+            emit(dict(bench="generate_int8", model=f"ziya-llama-13b-L{layers}", weights="int8" if int8 else "bf16", batch=B,
+                      prompt=S, new_tokens=new, reps=reps, tokens_per_s=round(B * new / w, 1),
+                      wall_ms_per_token=round(1e3 * w / new, 3), device_ms_per_token=round(dev_us / 1e3 / new, 3),
+                      host_calls_per_token=round(ncalls / new, 2),
+                      peak_mem_GiB=round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 3),
+                      model_footprint_GiB=round(model.get_memory_footprint() / 2 ** 30, 3), build_s=round(build_s, 1)))
+            del ids, gen, out
+        del model
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_int8: needs a CUDA GPU")
+    info = card()
+    lines = []
+
+    def emit(d):
+        d.update(info)
+        lines.append(d)
+        print(json.dumps(d), flush=True)
+    emit(dict(bench="card"))
+    kernel_ab(args.reps, emit)
+    if not args.skip_e2e:
+        end_to_end(args.reps, emit)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "bench_int8.jsonl"), "w") as f:
+            for d in lines:
+                f.write(json.dumps(d) + "\n")
+
+
+if __name__ == "__main__":
+    main()
