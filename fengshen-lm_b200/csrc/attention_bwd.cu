@@ -18,9 +18,6 @@
 
 namespace fsb {
 
-int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
-                   int box_rows);
-
 constexpr int AB_THREADS = 384;
 constexpr int AB_BM = 128;       // rows owned by the CTA (queries for dQ, keys for dKV)
 constexpr int AB_BN = 64;        // streamed tile (keys for dQ, queries for dKV)
@@ -86,14 +83,9 @@ struct AttBwdSmem {
   static constexpr int OFF_BAR = OFF_DS + (kDS ? (AB_BM * (AB_BN + 1) * 4 + 15) / 16 * 16 : 0);
   static constexpr int NBAR = 1 + 2 * STAGES;  // big_full, sml_full[S], sml_empty[S]
   static constexpr int TOTAL = OFF_BAR + NBAR * 8 + 1024;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
+  static_assert(TOTAL <= kSmemOptIn, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
 };
 
-template <int D>
-__device__ __forceinline__ void wgmma_rs_acc(float (&o)[D / 2], const uint32_t (&a)[4], uint64_t db) {
-  if constexpr (D == 128) wgmma_rs_n128<1>(o, a, db, 1u);
-  else wgmma_rs_n64<1>(o, a, db, 1u);
-}
 // shared-memory byte offset of the 16-wide K slice kk of a K-major tile with `rows` rows (64-column swizzle chunks)
 __device__ __forceinline__ uint32_t kslice(int kk, int rows) { return (kk / 4) * (rows * 128) + (kk % 4) * 32; }
 // 16-key slice kk of a [64 x 64] fp32 accumulator as bf16 register A fragments
@@ -113,13 +105,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                    const AttBwdParams p) {
   using S = AttBwdSmem<D, kBias>;
-  constexpr int STAGES = S::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
-  uint64_t* big_full = bars;
-  uint64_t* sml_full = big_full + 1;
-  uint64_t* sml_empty = sml_full + STAGES;
+  uint8_t* smem = align_smem_1024(smem_raw);
+  uint64_t* big_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
+  TmaRing<S::STAGES> ring(big_full + 1);   // the streamed tiles
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = gridDim.x - 1 - blockIdx.x;
@@ -131,7 +120,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     mbar_init(big_full, 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 8); }
+    ring.init();
     fence_barrier_init();
   }
   __syncthreads();
@@ -147,16 +136,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmQ, big_full, qc + h * 64, q0, b);
         tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmdO, big_full, dc + h * 64, q0, b);
       }
-      int st = 0; uint32_t ph = 0;
       for (int j = 0; j < n_steps; ++j) {
-        mbar_wait(&sml_empty[st], ph ^ 1);
-        mbar_expect_tx(&sml_full[st], 2 * S::SML_BYTES);
+        const int st = ring.stage;
+        ring.acquire();
+        uint64_t* bar = ring.expect(2 * S::SML_BYTES);
 #pragma unroll
         for (int h = 0; h < D / 64; ++h) {
-          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmK, &sml_full[st], kc + h * 64, j * AB_BN, b);
-          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmV, &sml_full[st], vc + h * 64, j * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmK, bar, kc + h * 64, j * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmV, bar, vc + h * 64, j * AB_BN, b);
         }
-        if (++st == STAGES) { st = 0; ph ^= 1; }
+        ring.advance();
       }
     }
     return;
@@ -197,11 +186,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   mbar_wait(big_full, 0);
   for (int j = 0; j < n_steps; ++j) {
-    const int st = j % STAGES;
-    const uint32_t ph = (j / STAGES) & 1;
-    const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
+    const auto step = ring.at(j);
+    const uint64_t sto = uint64_t(step.stage) * (S::SML_BYTES >> 4);
     float s[32], dp[32];
-    mbar_wait(&sml_full[st], ph);
+    step.wait();
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)
@@ -261,12 +249,12 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int kk = 0; kk < AB_BN / 16; ++kk) to_frag(s, kk, a[kk]);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dq, a[kk], dsc_kmn + sto + ((kk * 2048) >> 4));
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dq, a[kk], dsc_kmn + sto + ((kk * 2048) >> 4), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(dq);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&sml_empty[st]);
+    step.release(lane);
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -287,13 +275,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                     const AttBwdParams p) {
   using S = AttBwdSmem<D, false>;
-  constexpr int STAGES = S::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
-  uint64_t* big_full = bars;
-  uint64_t* sml_full = big_full + 1;
-  uint64_t* sml_empty = sml_full + STAGES;
+  uint8_t* smem = align_smem_1024(smem_raw);
+  uint64_t* big_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
+  TmaRing<S::STAGES> ring(big_full + 1);   // the streamed tiles
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x;  // early key tiles see the most queries under a causal mask: they come first already
@@ -306,7 +291,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     mbar_init(big_full, 1);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&sml_full[i], 1); mbar_init(&sml_empty[i], 8); }
+    ring.init();
     fence_barrier_init();
   }
   __syncthreads();
@@ -322,18 +307,16 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmK, big_full, kc + h * 64, kv0, b);
         tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmV, big_full, vc + h * 64, kv0, b);
       }
-      int st = 0; uint32_t ph = 0;
       for (int i = 0; i < n_steps; ++i) {
-        mbar_wait(&sml_empty[st], ph ^ 1);
-        mbar_expect_tx(&sml_full[st], 2 * S::SML_BYTES);
+        const int st = ring.stage;
+        ring.acquire();
+        uint64_t* bar = ring.expect(2 * S::SML_BYTES);
 #pragma unroll
         for (int h = 0; h < D / 64; ++h) {
-          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmQ, &sml_full[st], qc + h * 64,
-                      (i_start + i) * AB_BN, b);
-          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmdO, &sml_full[st], dc + h * 64,
-                      (i_start + i) * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmQ, bar, qc + h * 64, (i_start + i) * AB_BN, b);
+          tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmdO, bar, dc + h * 64, (i_start + i) * AB_BN, b);
         }
-        if (++st == STAGES) { st = 0; ph ^= 1; }
+        ring.advance();
       }
     }
     return;
@@ -369,12 +352,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 
   mbar_wait(big_full, 0);
   for (int i = 0; i < n_steps; ++i) {
-    const int st = i % STAGES;
-    const uint32_t ph = (i / STAGES) & 1;
-    const uint64_t sto = uint64_t(st) * (S::SML_BYTES >> 4);
+    const auto step = ring.at(i);
+    const uint64_t sto = uint64_t(step.stage) * (S::SML_BYTES >> 4);
     const int qt0 = (i_start + i) * AB_BN;
     float s[32], dp[32];
-    mbar_wait(&sml_full[st], ph);
+    step.wait();
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)
@@ -423,15 +405,15 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     for (int kk = 0; kk < AB_BN / 16; ++kk) { to_frag(s, kk, pa[kk]); to_frag(dp, kk, da[kk]); }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dv, pa[kk], dsc_domn + sto + ((kk * 2048) >> 4));
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dv, pa[kk], dsc_domn + sto + ((kk * 2048) >> 4), 1u);
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_acc<D>(dk, da[kk], dsc_qmn + sto + ((kk * 2048) >> 4));
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dk, da[kk], dsc_qmn + sto + ((kk * 2048) >> 4), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&sml_empty[st]);
+    step.release(lane);
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -495,18 +477,8 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
                            float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
   using SQ = AttBwdSmem<D, kBias>;
   using SK = AttBwdSmem<D, false>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<D, kBias, kDropout>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          SQ::TOTAL);
-    cudaError_t e2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<D, kBias, kDropout>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          SK::TOTAL);
-    if (e1 != cudaSuccess || e2 != cudaSuccess) {
-      set_error("sdpa_bwd: cudaFuncSetAttribute(%d / %d) failed", SQ::TOTAL, SK::TOTAL);
-      return FSB_ERR_CUDA;
-    }
-    configured = true;
-  }
+  if (int rc = ensure_smem<attn_bwd_dq_kernel<D, kBias, kDropout>>(SQ::TOTAL, "sdpa_bwd")) return rc;
+  if (int rc = ensure_smem<attn_bwd_dkv_kernel<D, kBias, kDropout>>(SK::TOTAL, "sdpa_bwd")) return rc;
   // 1. delta
   {
     const int64_t groups = int64_t(p.batch) * p.seq_q * p.nheads;

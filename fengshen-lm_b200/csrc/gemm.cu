@@ -18,8 +18,6 @@
 // next tile's operands stream in during the epilogue. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
 // K-split weight-gradient GEMMs carry the split as the batch coordinate of the tile: split s reads its own range of
 // k-blocks of the unbatched operands through full-K tensor maps and writes an fp32 partial product to D[s] (gemm_plan).
-#include <stdlib.h>
-
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -41,7 +39,6 @@ struct GemmParams {
   int accumulate;  // D += result
   int tiles_m, tiles_n;
   int group_m;     // m-tiles per rasterisation group (see fsb_gemm_bf16)
-  int l2_hints;    // bit 0: A panels evict-last, bit 1: B panels evict-first (FSB_GEMM_L2HINT)
   int ksplits;     // > 1: the batch index is a K-split of unbatched A / B (k_range)
 };
 
@@ -60,7 +57,7 @@ struct GemmSmem {
   static constexpr int BAR_OFFSET = EPI_OFFSET + 2 /*warpgroups*/ * 2 /*buffers*/ * EPI_BUF_BYTES;
   // full[STAGES], empty[STAGES]
   static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024 /*align slack*/;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
+  static_assert(TOTAL <= kSmemOptIn, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
 };
 
 // 0.5 x (1 + tanh(u)) == x * sigmoid(2u) == x / (1 + 2^(-2 u log2 e)): two MUFU ops instead of tanhf's ~25 instructions
@@ -110,12 +107,6 @@ __device__ __forceinline__ void k_range(const GemmParams& p, int b, int num_kb, 
   }
 }
 
-// Position of element (row, byte) of a 64-row x 128-byte sub-tile in the 128B-swizzled staging layout the D / aux tensor maps
-// declare: the 16-byte unit index is XORed with row % 8. A warp's 8 rows x 4 lanes then hit 32 distinct banks.
-__device__ __forceinline__ uint32_t epi_swz(int row, int byte) {
-  return uint32_t(row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15));
-}
-
 template <int kLayout, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -123,12 +114,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr bool A_MN = (kLayout == FSB_GEMM_TN);
   constexpr bool B_MN = (kLayout != FSB_GEMM_NT);
   using S = GemmSmem<BN>;
-  constexpr int STAGES = S::STAGES;
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
+  uint8_t* smem = align_smem_1024(smem_raw);
+  TmaRing<S::STAGES> ring(reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -138,10 +127,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
-    }
+    ring.init();
     fence_barrier_init();
   }
   if (threadIdx.x == 128) {
@@ -154,42 +140,32 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // ===================== TMA producer =====================
     reg_dec<40>();
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      // L2 policy (FSB_GEMM_L2HINT): tiles are walked m-fastest inside a group of m-tiles, so a group's A panels are read
-      // again for every n-tile of the sweep (evict-last) while a B panel is used by the CTAs of one wave (evict-first).
-      const uint64_t pol_a = (p.l2_hints & 1) ? kL2EvictLast : kL2EvictNormal, pol_b = (p.l2_hints & 2) ? kL2EvictFirst : kL2EvictNormal;
-      const bool hints = (p.l2_hints & 3) != 0;
-      auto load = [&](uint8_t* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, uint64_t policy) {
-        if (hints) tma_load_3d_hint(dst, tm, bar, c0, c1, c2, policy);
-        else tma_load_3d(dst, tm, bar, c0, c1, c2);
-      };
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int b, m_idx, n_idx, kb_lo, kb_hi, ab;
         tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
         k_range(p, b, num_kb, kb_lo, kb_hi, ab);
         const int m0 = m_idx * GEMM_BM, n0 = n_idx * BN;
         for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * S::STAGE_BYTES;
+          ring.acquire();
+          uint8_t* sa = smem + ring.stage * S::STAGE_BYTES;
           uint8_t* sb = sa + S::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES);
+          uint64_t* bar = ring.expect(S::STAGE_BYTES);
           const int k0 = kb * GEMM_BK;
           if constexpr (!A_MN) {
-            load(sa, &tmA, &full_bar[stage], k0, m0, ab, pol_a);
+            tma_load_3d(sa, &tmA, bar, k0, m0, ab);
           } else {
 #pragma unroll
             for (int c = 0; c < GEMM_BM / 64; ++c)
-              load(sa + c * (GEMM_BK * 128), &tmA, &full_bar[stage], m0 + c * 64, k0, ab, pol_a);
+              tma_load_3d(sa + c * (GEMM_BK * 128), &tmA, bar, m0 + c * 64, k0, ab);
           }
           if constexpr (!B_MN) {
-            load(sb, &tmB, &full_bar[stage], k0, n0, ab, pol_b);
+            tma_load_3d(sb, &tmB, bar, k0, n0, ab);
           } else {
 #pragma unroll
             for (int c = 0; c < BN / 64; ++c)
-              load(sb + c * (GEMM_BK * 128), &tmB, &full_bar[stage], n0 + c * 64, k0, ab, pol_b);
+              tma_load_3d(sb + c * (GEMM_BK * 128), &tmB, bar, n0 + c * 64, k0, ab);
           }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          ring.advance();
         }
       }
     }
@@ -207,16 +183,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint8_t* const epi_buf = smem + S::EPI_OFFSET + wg * (2 * S::EPI_BUF_BYTES);
     uint32_t n_stored = 0;   // sub-tiles this warpgroup has handed to the TMA unit (selects the staging buffer)
     float acc[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       int b, m_idx, n_idx, kb_lo, kb_hi, ab;
       tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
       k_range(p, b, num_kb, kb_lo, kb_hi, ab);
       int prev = 0;
       for (int kb = kb_lo; kb < kb_hi; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint64_t so = uint64_t(stage) * (S::STAGE_BYTES >> 4);
+        ring.wait();
+        const uint64_t so = uint64_t(ring.stage) * (S::STAGE_BYTES >> 4);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GEMM_BK / 16; ++k) {
@@ -227,13 +201,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         wgmma_commit();
         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage can be refilled
-        if (kb > kb_lo && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (kb > kb_lo) ring.release(prev, lane);
+        prev = ring.stage;
+        ring.advance();
       }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      ring.release(prev, lane);
 
       // ---- epilogue: accumulator j covers columns 8 (j / 4) + 2 (lane % 4) + (j & 1), rows r and r + 8 (r = 16 wl + lane / 4)
       const int r = wl * 16 + (lane >> 2);
@@ -279,7 +253,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const int j = 8 * g + jj;
-                *reinterpret_cast<uint32_t*>(buf + epi_swz(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                *reinterpret_cast<uint32_t*>(buf + swz128(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
                     pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
               }
           });
@@ -321,7 +295,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int j = 8 * g + 4 * q + jj;
-                  *reinterpret_cast<float2*>(buf + epi_swz(r + 8 * h, 32 * jj + 8 * (lane & 3))) =
+                  *reinterpret_cast<float2*>(buf + swz128(r + 8 * h, 32 * jj + 8 * (lane & 3))) =
                       make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
                 }
             });
@@ -332,7 +306,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const int j = 8 * g + jj;
-                *reinterpret_cast<uint32_t*>(buf + epi_swz(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                *reinterpret_cast<uint32_t*>(buf + swz128(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
                     pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
               }
           });
@@ -355,19 +329,10 @@ template <int kLayout, int BN>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmAux,
                        const GemmParams& p, cudaStream_t stream) {
   using S = GemmSmem<BN>;
-  static bool configured = false;
-  auto kern = gemm_bf16_kernel<kLayout, BN>;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL);
-    if (e != cudaSuccess) {
-      set_error("gemm: cudaFuncSetAttribute(%d B smem) failed: %s", S::TOTAL, cudaGetErrorString(e));
-      return FSB_ERR_CUDA;
-    }
-    configured = true;
-  }
+  if (int rc = ensure_smem<gemm_bf16_kernel<kLayout, BN>>(S::TOTAL, "gemm")) return rc;
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
   const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
-  kern<<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
+  gemm_bf16_kernel<kLayout, BN><<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
@@ -543,8 +508,6 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   p.d_f32 = (d_dtype == FSB_F32); p.bias_f32 = (bias_dtype == FSB_F32);
   p.epilogue = epilogue; p.accumulate = accumulate;
   p.ksplits = ksplits;
-  static const int l2hint_env = [] { const char* e = getenv("FSB_GEMM_L2HINT"); return e ? atoi(e) : 0; }();
-  p.l2_hints = l2hint_env;
   p.tiles_m = int((M + GEMM_BM - 1) / GEMM_BM);
   p.tiles_n = int((N + BN - 1) / BN);
   // Rasterisation: tiles are walked m-fastest inside groups of group_m m-tiles, so one wave of CTAs touches group_m A panels

@@ -155,6 +155,14 @@ int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* d
   return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box);
 }
 
+int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
+                   int box_rows) {
+  uint64_t dims[3] = {uint64_t(width), uint64_t(seq), uint64_t(batch)};
+  uint64_t strides[2] = {uint64_t(row_stride) * 2, uint64_t(seq) * uint64_t(row_stride) * 2};
+  uint32_t box[3] = {64, uint32_t(box_rows), 1};
+  return make_tmap_bf16(tm, base, 3, dims, strides, box);
+}
+
 }  // namespace fsb
 
 extern "C" int fsb_version(void) { return 1000 * 0 + 1; }

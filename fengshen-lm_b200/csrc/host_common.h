@@ -40,7 +40,28 @@ int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* 
                   const uint32_t* box);
 int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                  const uint32_t* box);
+// bf16 map over a packed attention activation buffer: dims {width, seq, batch} with rows row_stride elements apart; box
+// {64, box_rows, 1}
+int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
+                   int box_rows);
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Lets kKernel launch with `bytes` of dynamic shared memory (above the 48 KB default); the attribute is set on the first
+// successful call only. The kernel is a template argument so that every kernel has its own flag: kernels of one signature
+// share a function-pointer type.
+template <auto kKernel>
+int ensure_smem(int bytes, const char* what) {
+  static bool configured = false;
+  if (!configured) {
+    const cudaError_t e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaFuncSetAttribute(%d B smem) failed: %s", what, bytes, cudaGetErrorString(e));
+      return FSB_ERR_CUDA;
+    }
+    configured = true;
+  }
+  return FSB_OK;
+}
 
 }  // namespace fsb

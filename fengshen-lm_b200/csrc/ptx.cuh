@@ -64,6 +64,68 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------------------------
+// warp-specialised TMA pipeline: one producer thread fills a ring of shared-memory stages, the consumer warpgroups drain it
+// ----------------------------------------------------------------------------------------------
+// dynamic shared memory a block can opt into on sm_90 (227 KB)
+constexpr int kSmemOptIn = 232448;
+
+// SWIZZLE_128B tiles must start on a 1024-byte boundary; every kernel reserves 1024 bytes of slack for this
+__device__ __forceinline__ uint8_t* align_smem_1024(uint8_t* smem_raw) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
+
+// Position in a ring of STAGES stages and its barriers, laid out in shared memory as full[NFULL][STAGES], empty[STAGES].
+// The producer arms a full barrier (count 1) with the bytes its TMA loads will deliver; lane 0 of each of the 8 consumer
+// warps arrives on the empty barrier once the warp's MMAs on the stage have retired. Both sides visit the stages in the same
+// order; `phase` is the parity of the current pass over the ring. With NFULL > 1 a stage lands in parts that the consumers
+// wait for separately (attention's K and V).
+template <int STAGES, int NFULL = 1>
+struct TmaRing {
+  uint64_t* const bar;
+  uint64_t* const empty_bar;
+  int stage = 0;
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ explicit TmaRing(uint64_t* bars) : bar(bars), empty_bar(bars + NFULL * STAGES) {}
+  __device__ __forceinline__ uint64_t* full(int f) const { return bar + f * STAGES + stage; }
+  __device__ __forceinline__ uint64_t* empty(int s) const { return empty_bar + s; }
+
+  // one thread, before the __syncthreads that publishes the barriers
+  __device__ __forceinline__ void init() const {
+    for (int s = 0; s < STAGES; ++s) {
+      for (int f = 0; f < NFULL; ++f) mbar_init(bar + f * STAGES + s, 1);
+      mbar_init(empty(s), 8);
+    }
+  }
+  // producer: wait until the consumers have released the current stage (on the first pass every stage is free)
+  __device__ __forceinline__ void acquire() const { mbar_wait(empty(stage), phase ^ 1); }
+  // producer: arm full barrier f of the current stage for `bytes`; the loads into that part of the stage complete on the
+  // barrier returned
+  __device__ __forceinline__ uint64_t* expect(uint32_t bytes, int f = 0) const {
+    mbar_expect_tx(full(f), bytes);
+    return full(f);
+  }
+  // consumer: wait until full barrier f of the current stage has received its bytes
+  __device__ __forceinline__ void wait(int f = 0) const { mbar_wait(full(f), phase); }
+  // consumer: the warp is done with stage s (its MMAs on it have retired); lane 0 hands it back to the producer
+  __device__ __forceinline__ void release(int s, int lane) const {
+    if (lane == 0) mbar_arrive(empty(s));
+  }
+  // consumer: the same for the current stage
+  __device__ __forceinline__ void release(int lane) const { release(stage, lane); }
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  // the ring as it stands after j advances from the start
+  __device__ __forceinline__ TmaRing at(int j) const {
+    TmaRing r(bar);
+    r.stage = j % STAGES;
+    r.phase = (j / STAGES) & 1;
+    return r;
+  }
+};
+
+// ----------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor); coordinates are innermost-first
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -81,23 +143,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-// L2 eviction-priority hints for bulk tensor copies (the 64-bit policy words CUTLASS uses, cute/arch/copy_sm90_desc.hpp)
-constexpr uint64_t kL2EvictNormal = 0x1000000000000000ull, kL2EvictFirst = 0x12F0000000000000ull,
-                   kL2EvictLast = 0x14F0000000000000ull;
-__device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                 uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_3d_hint(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2,
-                                                  uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-               : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
@@ -158,10 +203,39 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_
   d |= static_cast<uint64_t>(1) << 62;                       // [62,64) layout type: SWIZZLE_128B
   return d;
 }
+// Byte offset of element (row, byte) of a tile of 128-byte rows in the SWIZZLE_128B layout (the one TMA reads and writes):
+// the 16-byte unit index is XORed with row % 8, so a warp's 8 rows x 4 lanes hit 32 distinct banks.
+__device__ __forceinline__ uint32_t swz128(int row, int byte) {
+  return uint32_t(row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15));
+}
 
 // m64nNk16, bf16 x bf16 -> fp32. kTA / kTB = 1: that operand is MN-major in shared memory. Register A operand (_rs): the
 // fragment of one 64 x 16 slice, four bf16 pairs per thread — (row, k..k+1), (row+8, k..k+1), (row, k+8..), (row+8, k+8..)
 // with row = 16 * warp + lane / 4, k = 2 * (lane % 4): the same positions the fp32 accumulator uses for two 8-column groups.
+template <int kTB>
+__device__ __forceinline__ void wgmma_rs_n8(float (&d)[4], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %9, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, %10;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(kTB));
+}
+template <int kTB>
+__device__ __forceinline__ void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(kTB));
+}
+template <int kTB>
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(kTB));
+}
 template <int kTA, int kTB>
 __device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
@@ -210,6 +284,17 @@ __device__ __forceinline__ void wgmma_rs_n256(float (&d)[128], const uint32_t (&
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(kTB));
 }
+// register-A m64nNk16 for N = 8, 16, 32, 64, 128, 256
+template <int N, int kTB>
+__device__ __forceinline__ void wgmma_rs_dim(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  static_assert(N == 8 || N == 16 || N == 32 || N == 64 || N == 128 || N == 256, "no m64nNk16 wgmma for this N");
+  if constexpr (N == 8) wgmma_rs_n8<kTB>(d, a, db, accumulate);
+  else if constexpr (N == 16) wgmma_rs_n16<kTB>(d, a, db, accumulate);
+  else if constexpr (N == 32) wgmma_rs_n32<kTB>(d, a, db, accumulate);
+  else if constexpr (N == 64) wgmma_rs_n64<kTB>(d, a, db, accumulate);
+  else if constexpr (N == 128) wgmma_rs_n128<kTB>(d, a, db, accumulate);
+  else wgmma_rs_n256<kTB>(d, a, db, accumulate);
+}
 
 // ----------------------------------------------------------------------------------------------
 // misc
@@ -232,5 +317,10 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   return q;
 }
 __device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16(x)); }
+__device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
+  uint16_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+  return v;
+}
 
 }  // namespace fsb
