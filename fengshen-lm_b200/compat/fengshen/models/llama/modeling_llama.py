@@ -27,7 +27,7 @@ class LlamaForCausalLM(_FsbLlama):
         super().__init__(config, **kw)
 
     @classmethod
-    def from_pretrained(cls, path, torch_dtype=None, load_in_8bit=False, device_map=None, **kw):
+    def from_pretrained(cls, path, torch_dtype=None, load_in_8bit=False, device_map=None, load_in_4bit=False, **kw):
         """Loads config.json + pytorch_model.bin (or the sharded index) written by the reference's save_pretrained /
         hf_to_fs.py. torch_dtype is accepted for signature parity; parameters are stored in bf16.
 
@@ -35,6 +35,8 @@ class LlamaForCausalLM(_FsbLlama):
         projections are int8 (fsb200/models/llama.py). The checkpoint is read one shard file at a time and each shard's
         matrices are quantised on the device before the next file is read, so host memory holds one shard. HF-format
         directories are converted first with `fengshen.utils.llama_convert.hf_to_fs_state_dict`.
+        load_in_4bit=True (hf_quantizatin_inference.py:3,16): the same with int4 projections (one bf16 scale per row and
+        group of 128 k), loaded the same way. Passing both flags raises ValueError.
         device_map: None, "auto" or one device (the model lives on one GPU); a map over several devices raises."""
         if device_map is not None and device_map != "auto":
             if isinstance(device_map, dict):
@@ -48,17 +50,17 @@ class LlamaForCausalLM(_FsbLlama):
         with open(os.path.join(path, "config.json")) as f:
             raw = json.load(f)
         raw.pop("torch_dtype", None); raw.pop("architectures", None); raw.pop("model_type", None)
-        model = cls(LlamaConfig(**raw), load_in_8bit=load_in_8bit, **kw)
+        model = cls(LlamaConfig(**raw), load_in_8bit=load_in_8bit, load_in_4bit=load_in_4bit, **kw)
         idx = os.path.join(path, "pytorch_model.bin.index.json")
         files = [os.path.join(path, "pytorch_model.bin")]
         if os.path.exists(idx):
             with open(idx) as f:
                 files = sorted({os.path.join(path, v) for v in json.load(f)["weight_map"].values()})
-        if load_in_8bit:
+        if model.weight_format != "bf16":
             loaded, missing = set(), None
             for fn in files:
                 shard = torch.load(fn, map_location="cpu", weights_only=True)
-                missing = model._load_w8_shard(shard, loaded)
+                missing = model._load_quantized_shard(shard, loaded)
                 del shard
             if missing:
                 raise KeyError(f"missing key in checkpoint {path}: {sorted(missing)[0]}")
@@ -73,8 +75,8 @@ class LlamaForCausalLM(_FsbLlama):
         """HF-style export (what the scripts call after training, e.g. examples/pretrain_t5/pretrain_t5.py:105-112 for its
         model): config.json + pytorch_model.bin in the reference's key layout; `from_pretrained(path)` reads it back, and
         `fengshen.utils.llama_convert.fs_to_hf_state_dict` turns it into a transformers LLaMA checkpoint."""
-        if self.load_in_8bit:
-            return super().save_pretrained(path)   # raises: int8 export is not implemented
+        if self.weight_format != "bf16":
+            return super().save_pretrained(path)   # raises: int8 / int4 export is not implemented
         from fengshen.utils.llama_convert import save_pretrained_fs
         wait_params(self)
         cfg = self.config.to_dict() if hasattr(self.config, "to_dict") else vars(self.config)

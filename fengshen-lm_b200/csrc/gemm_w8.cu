@@ -1,50 +1,79 @@
-// fsb200 — int8 weight-only GEMM (W8A16) and its quantiser for sm_90a: the inference layers behind `load_in_8bit=True`
-// (fengshen/examples/ziya_inference/hf_quantizatin_inference.py:20-22, which hands the Linear layers to bitsandbytes'
-// Linear8bitLt). Weights are stored as int8 q[n, k] with one fp32 scale per output channel, s[n] = absmax(W[n, :]) / 127;
-// the GEMM computes D[m, n] = bf16(s[n] * sum_k A[m, k] q[n, k]) with fp32 accumulation.
+// fsb200 — weight-only GEMMs (W8A16, W4A16) and their quantisers for sm_90a: the inference layers behind `load_in_8bit=True`
+// and `load_in_4bit=True` (fengshen/examples/ziya_inference/hf_quantizatin_inference.py). The formats (include/fsb200.h):
+//   * int8: q int8 [n, k] with one fp32 scale per output channel, s[n] = absmax(W[n, :]) / 127; the GEMM computes
+//     D[m, n] = bf16(s[n] * sum_k A[m, k] q[n, k]) with fp32 accumulation.
+//   * int4: q in [-7, 7], two per byte, with one bf16 scale per output channel and group of 128 k; the GEMM computes
+//     D[m, n] = bf16(sum_k A[m, k] bf16(q[n, k] s[n, k / 128])) with fp32 accumulation.
 //
 // The operands are swapped against gemm.cu: decode has 1-32 token rows, far below the 64-row minimum of a wgmma A operand, so
-// the WEIGHT tile is the A operand and the token tile the B operand (n = 8..128 tokens per tile).
+// the WEIGHT tile is the A operand and the token tile the B operand (n = 8..128 tokens per tile). One kernel template serves
+// both formats; the format decides the weight tile's layout, how a fragment is converted and where the scale is applied.
 //   * Roles (384 threads = 3 warpgroups): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each owning
 //     64 of the tile's 128 weight rows.
-//   * Per stage the producer loads a 128-row x 128-byte int8 weight tile and two 64-wide bf16 token boxes, all 128B-swizzled;
-//     TMA zero-fills token rows at or beyond m and weight rows at or beyond n.
-//   * Each consumer thread reads its fragment of the int8 tile (2-byte pieces: (row, k..k+1) as the register-A layout places
-//     them), converts it to bf16 in registers (exact: every int8 is a bf16) and issues wgmma in the register-A form against
-//     the token tile in shared memory. Two fragment buffers let one stage's conversion overlap the previous stage's MMAs.
-//   * Epilogue: each accumulator row (one weight row) is multiplied by s[n], rounded to bf16 and staged transposed
-//     ([token][weight row], 128B-swizzled) in shared memory; a TMA store writes D row-major and clips rows >= m, columns >= n.
+//   * Per stage (128 k) the producer loads the tile's 128 weight rows of quantised weights (int8: 128 rows x 128 bytes; int4:
+//     64 row pairs x 128 bytes) and two 64-wide bf16 token boxes, all 128B-swizzled; TMA zero-fills token rows at or beyond m
+//     and weight rows at or beyond n.
+//   * Each consumer thread reads its fragment of the weight tile, converts it to bf16 in registers and issues wgmma in the
+//     register-A form against the token tile in shared memory. Two fragment buffers let one stage's conversion overlap the
+//     previous stage's MMAs.
+//       int8: 2-byte pieces ((row, k..k+1) as the register-A layout places them), converted exactly (every int8 is a bf16).
+//       int4: the whole fragment of a k16 step is one 32-bit word: a warp's wgmma rows g and g + 8 are weight rows 2g and
+//       2g + 1 of its 16, and one 128-byte line holds a row pair. Each pair of codes becomes bf16(q * s) with the stage's
+//       group scale (a stage is one group) before the MMA.
+//   * Epilogue: each accumulator row (one weight row) is multiplied by s[n] (int8 only), rounded to bf16 and staged
+//     transposed ([token][weight row], 128B-swizzled) in shared memory; a TMA store writes D row-major and clips rows >= m,
+//     columns >= n.
 //   * When the output tiles leave SMs idle (decode), K is split: split j writes its fp32 partial product to the caller's
-//     workspace and a second kernel sums the splits in order, scales, rounds and stores D. The plan is a function of (m, n, k)
-//     and the SM count only, so graph replays equal eager calls bit for bit.
+//     workspace and a second kernel sums the splits in order, scales (int8), rounds and stores D. The plan is a function of
+//     (m, n, k) and the SM count only, so graph replays equal eager calls bit for bit.
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace fsb {
 
 constexpr int W8_BM = 128;        // weight rows per tile (2 consumer warpgroups x 64)
-constexpr int W8_BK = 128;        // k per stage: one 128-byte swizzle row of int8
+constexpr int W8_BK = 128;        // k per stage: one 128-byte swizzle line of int8 per row, of int4 per row pair
 constexpr int W8_THREADS = 384;
+constexpr int W4_GROUP = 128;     // int4: k per scale group (= W8_BK: one group per stage)
 
-template <int BT>
-struct W8Smem {
-  static constexpr int W_BYTES = W8_BM * W8_BK;                // int8 weight tile
+// int8: a 128-byte line of the weight tile is one weight row; a thread's fragment rows are `row` and `row + 8`; the fp32
+// per-row scale is applied after the sum.
+struct FmtW8 {
+  static constexpr int kRowsPerLine = 1;
+  static constexpr int kPartner = 8;        // the thread's second weight row is row + kPartner
+  static constexpr int kMaxStages = 8;
+  static constexpr bool kRowScale = true;
+};
+// int4: a line is a row pair (2p, 2p + 1) and a thread's fragment rows are `row` (even) and `row + 1`; the group scales are
+// applied to the fragments, so the sum is stored as it is. Half the bytes per stage: up to twice the stages keeps as many
+// weight bytes in flight as int8.
+struct FmtW4 {
+  static constexpr int kRowsPerLine = 2;
+  static constexpr int kPartner = 1;
+  static constexpr int kMaxStages = 16;
+  static constexpr bool kRowScale = false;
+};
+
+template <class F, int BT>
+struct WqSmem {
+  static constexpr int W_BYTES = W8_BM / F::kRowsPerLine * 128;  // quantised weight tile
   static constexpr int T_BYTES = BT * W8_BK * 2;               // two 64-wide bf16 token boxes
   static constexpr int STAGE_BYTES = W_BYTES + T_BYTES;
   static constexpr int EPI_BYTES = 2 * BT * 128;               // per consumer warpgroup: BT tokens x 64 bf16 weight rows
   static constexpr int BUDGET = kSmemOptIn - 1024 - 256;
   static constexpr int FIT = (BUDGET - EPI_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = FIT > 8 ? 8 : FIT;
+  static constexpr int STAGES = FIT > F::kMaxStages ? F::kMaxStages : FIT;
   static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFFSET = EPI_OFFSET + EPI_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024 /*align slack*/;
   static_assert(STAGES >= 3, "too few pipeline stages");
+  static_assert(2 * STAGES * 8 <= 256, "barriers exceed their reserve");
   static_assert(TOTAL <= kSmemOptIn, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
   static_assert(STAGE_BYTES % 1024 == 0 && (BT * 128) % 1024 == 0, "swizzled tiles must stay 1024-byte aligned");
 };
 
-struct W8Params {
-  const float* scale;
+struct WqParams {
+  const void* scale;  // int8: fp32 [N]; int4: bf16 [N, K / 128]
   float* ws;          // split-K partials [splits, M, N] fp32, or nullptr
   int M, N, K;
   int tiles_t, tiles_n, splits, num_kb;
@@ -63,11 +92,21 @@ __device__ __forceinline__ void i8x4_to_bf16x4(uint32_t x, uint32_t& lo, uint32_
   hi = __byte_perm(__float_as_uint(f2), __float_as_uint(f3), 0x7632);
 }
 
-template <int BT>
+// Two int4 codes (bits 0-3 and 16-19 of x, each q + 8) -> the bf16x2 pair bf16(q * s), s2 holding s twice. 0x4300 | code is
+// the bf16 128 + code; subtracting 136 gives q exactly, and one bf16 multiply rounds the exact product q * s once.
+__device__ __forceinline__ uint32_t i4x2_to_bf16x2(uint32_t x, uint32_t s2) {
+  const uint32_t v = (x & 0x000F000Fu) | 0x43004300u;
+  uint32_t q, w;
+  asm("fma.rn.bf16x2 %0, %1, %2, %3;" : "=r"(q) : "r"(v), "r"(0x3F803F80u), "r"(0xC308C308u));   // v * 1 - 136
+  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(w) : "r"(q), "r"(s2));
+  return w;
+}
+
+template <class F, int BT>
 __global__ void __launch_bounds__(W8_THREADS, 1)
-gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA,
-                  const __grid_constant__ CUtensorMap tmD, const W8Params p) {
-  using S = W8Smem<BT>;
+gemm_wq_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA,
+               const __grid_constant__ CUtensorMap tmD, const WqParams p) {
+  using S = WqSmem<F, BT>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   TmaRing<S::STAGES> ring(reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET));
@@ -100,7 +139,7 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         const int k0 = kb * W8_BK;
         const bool second = k0 + 64 < p.K;   // the upper 64-wide token box holds real columns
         uint64_t* bar = ring.expect(S::W_BYTES + (second ? 2 : 1) * BT * 128);
-        tma_load_2d(sw, &tmW, bar, k0, n0);
+        tma_load_2d(sw, &tmW, bar, k0, n0 / F::kRowsPerLine);   // int4: a byte line of q holds a row pair's k values
         tma_load_2d(st, &tmA, bar, k0, t0);
         if (second) tma_load_2d(st + BT * 128, &tmA, bar, k0 + 64, t0);
         ring.advance();
@@ -111,7 +150,7 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     reg_inc<232>();
     const int wg = (threadIdx.x >> 7) - 1;
     const int wl = warp & 3, g = lane >> 2, tq = lane & 3;
-    const int row = wg * 64 + wl * 16 + g;           // this thread's weight rows in the tile: row and row + 8
+    const int row = wg * 64 + wl * 16 + F::kRowsPerLine * g;   // this thread's weight rows in the tile: row, row + kPartner
     const uint32_t smem_base = smem_u32(smem);
     const uint64_t dsc_t = make_smem_desc_sw128(smem_base + S::W_BYTES, 0, 1024);
     float acc[BT / 2];
@@ -123,23 +162,49 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     uint64_t* const empty_bar = ring.empty_bar;
     int stage = 0, prev = -1;
     uint32_t phase = 0;
+    // int4: the group scales of rows `row` and `row + 1` (bf16 bits), loaded one stage ahead. Rows at or beyond N read row
+    // N - 2's scales: their sums are never stored.
+    const uint16_t* s_row = nullptr;
+    uint32_t s_next0 = 0, s_next1 = 0;
+    if constexpr (!F::kRowScale) {
+      s_row = static_cast<const uint16_t*>(p.scale) + int64_t(min(n0 + row, p.N - 2)) * p.num_kb;
+      s_next0 = __ldg(s_row + kb_lo);
+      s_next1 = __ldg(s_row + p.num_kb + kb_lo);
+    }
 
-    // One stage: convert this thread's fragments of the int8 tile into `fr`, issue the stage's MMAs, then wait until the
+    // One stage: convert this thread's fragments of the weight tile into `fr`, issue the stage's MMAs, then wait until the
     // PREVIOUS stage's MMAs have retired (its token tile and its fragment buffer, the other one, are then free).
     auto run_stage = [&](uint32_t (&fr)[8][4], int kb) {
+      uint32_t sc0 = 0, sc1 = 0;
+      if constexpr (!F::kRowScale) {
+        sc0 = s_next0 * 0x10001u;
+        sc1 = s_next1 * 0x10001u;
+        const int nk = min(kb + 1, kb_hi - 1);
+        s_next0 = __ldg(s_row + nk);
+        s_next1 = __ldg(s_row + p.num_kb + nk);
+      }
       mbar_wait(&full_bar[stage], phase);
       const int steps = min(8, (p.K - kb * W8_BK) >> 4);   // k16 steps inside K (K % 16 == 0)
       const uint32_t w0 = smem_base + stage * S::STAGE_BYTES;
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) {
         if (kk < steps) {
-          const uint32_t a = w0 + swz128(row, 16 * kk + 2 * tq);   // row + 8 is 1024 bytes on, same swizzle phase
-          const uint32_t x = __byte_perm(lds_u16(a), lds_u16(a + 1024), 0x5410);
-          const uint32_t y = __byte_perm(lds_u16(a + 8), lds_u16(a + 1024 + 8), 0x5410);
-          uint32_t r0, r1, r2, r3;
-          i8x4_to_bf16x4(x, r0, r1);
-          i8x4_to_bf16x4(y, r2, r3);
-          fr[kk][0] = r0; fr[kk][1] = r1; fr[kk][2] = r2; fr[kk][3] = r3;
+          if constexpr (F::kRowScale) {
+            const uint32_t a = w0 + swz128(row, 16 * kk + 2 * tq);   // row + 8 is 1024 bytes on, same swizzle phase
+            const uint32_t x = __byte_perm(lds_u16(a), lds_u16(a + 1024), 0x5410);
+            const uint32_t y = __byte_perm(lds_u16(a + 8), lds_u16(a + 1024 + 8), 0x5410);
+            uint32_t r0, r1, r2, r3;
+            i8x4_to_bf16x4(x, r0, r1);
+            i8x4_to_bf16x4(y, r2, r3);
+            fr[kk][0] = r0; fr[kk][1] = r1; fr[kk][2] = r2; fr[kk][3] = r3;
+          } else {
+            // the row pair's line is row / 2 of the tile; a warp's 8 lines x 4 lanes hit 32 distinct banks
+            const uint32_t x = lds_u32(w0 + swz128(row >> 1, 16 * kk + 4 * tq));
+            fr[kk][0] = i4x2_to_bf16x2(x, sc0);         // (row, k..k+1)
+            fr[kk][1] = i4x2_to_bf16x2(x >> 4, sc1);    // (row + 1, k..k+1)
+            fr[kk][2] = i4x2_to_bf16x2(x >> 8, sc0);    // (row, k+8..k+9)
+            fr[kk][3] = i4x2_to_bf16x2(x >> 12, sc1);   // (row + 1, k+8..k+9)
+          }
         }
       }
       wgmma_fence();
@@ -168,10 +233,10 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
     wgmma_fence_acc(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-    // ---- epilogue: acc[4 j + 2 h + e] is (weight row `row + 8 h`, token 8 j + 2 tq + e) of the tile
-    const int nrow0 = n0 + row, nrow1 = nrow0 + 8;
+    // ---- epilogue: acc[4 j + 2 h + e] is (weight row `row + kPartner h`, token 8 j + 2 tq + e) of the tile
+    const int nrow0 = n0 + row, nrow1 = nrow0 + F::kPartner;
     if (p.ws != nullptr) {
-      // K-split: unscaled fp32 partial to ws[split, token, n]; a warp's 8 consecutive rows are 32 contiguous bytes per token
+      // K-split: unscaled fp32 partial to ws[split, token, n]
       float* ws = p.ws + int64_t(split) * p.M * p.N;
 #pragma unroll
       for (int j = 0; j < BT / 8; ++j)
@@ -183,17 +248,22 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
           if (nrow1 < p.N) ws[int64_t(tok) * p.N + nrow1] = acc[4 * j + 2 + e];
         }
     } else {
-      const float s0 = nrow0 < p.N ? __ldg(p.scale + nrow0) : 0.f;
-      const float s1 = nrow1 < p.N ? __ldg(p.scale + nrow1) : 0.f;
+      float s0 = 1.f, s1 = 1.f;
+      if constexpr (F::kRowScale) {
+        const float* scale = static_cast<const float*>(p.scale);
+        s0 = nrow0 < p.N ? __ldg(scale + nrow0) : 0.f;
+        s1 = nrow1 < p.N ? __ldg(scale + nrow1) : 0.f;
+      }
       uint8_t* buf = smem + S::EPI_OFFSET + wg * (BT * 128);
-      const int lr = wl * 16 + g;   // weight row inside the warpgroup's 64 (the staging tile's column)
+      const int lr = wl * 16 + F::kRowsPerLine * g;   // weight row inside the warpgroup's 64 (the staging tile's column)
 #pragma unroll
       for (int j = 0; j < BT / 8; ++j)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int tok = 8 * j + 2 * tq + e;
           *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * lr)) = __float2bfloat16_rn(acc[4 * j + e] * s0);
-          *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * (lr + 8))) = __float2bfloat16_rn(acc[4 * j + 2 + e] * s1);
+          *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * (lr + F::kPartner))) =
+              __float2bfloat16_rn(acc[4 * j + 2 + e] * s1);
         }
       fence_proxy_async();
       bar_sync(1 + wg, 128);
@@ -206,8 +276,10 @@ gemm_w8a16_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
   }
 }
 
-// D[m, n:n+8] = bf16(s[n:n+8] * sum over splits of ws[split, m, n:n+8]), splits summed in order
-__global__ void w8_splitk_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ scale, int splits, int64_t M,
+// D[m, n:n+8] = bf16(s[n:n+8] * sum over splits of ws[split, m, n:n+8]), splits summed in order; int4 (kRowScale false)
+// stores the sum unscaled
+template <bool kRowScale>
+__global__ void wq_splitk_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ scale, int splits, int64_t M,
                                         int64_t N, __nv_bfloat16* __restrict__ D, int64_t ldd) {
   const int64_t n8 = N / 8;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < M * n8; i += int64_t(gridDim.x) * blockDim.x) {
@@ -221,8 +293,10 @@ __global__ void w8_splitk_reduce_kernel(const float* __restrict__ ws, const floa
       a = q[0]; b = q[1];
       v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
     }
-    const float4 s0 = *reinterpret_cast<const float4*>(scale + n), s1 = *reinterpret_cast<const float4*>(scale + n + 4);
-    v[0] *= s0.x; v[1] *= s0.y; v[2] *= s0.z; v[3] *= s0.w; v[4] *= s1.x; v[5] *= s1.y; v[6] *= s1.z; v[7] *= s1.w;
+    if constexpr (kRowScale) {
+      const float4 s0 = *reinterpret_cast<const float4*>(scale + n), s1 = *reinterpret_cast<const float4*>(scale + n + 4);
+      v[0] *= s0.x; v[1] *= s0.y; v[2] *= s0.z; v[3] *= s0.w; v[4] *= s1.x; v[5] *= s1.y; v[6] *= s1.z; v[7] *= s1.w;
+    }
     *reinterpret_cast<uint4*>(D + m * ldd + n) = pack8(v);
   }
 }
@@ -255,10 +329,52 @@ __global__ void quantize_w8_kernel(const __nv_bfloat16* __restrict__ W, int64_t 
   }
 }
 
+// One warp per (row pair 2p, 2p + 1; group of 128 k), 8 groups per block: per row s = bf16(absmax / 7) (IEEE division, then
+// round to nearest even), q = clamp(rint(w / s), -7, 7) (0 where s == 0), packed as include/fsb200.h lays it out: in each
+// 16-k block, byte 4t + 2b + h holds k = 8h + 2t + b, row 2p in the low nibble and row 2p + 1 in the high one, each q + 8.
+__global__ void quantize_w4_kernel(const __nv_bfloat16* __restrict__ W, int64_t ldw, int64_t K, int groups,
+                                   uint8_t* __restrict__ q, __nv_bfloat16* __restrict__ s) {
+  __shared__ int8_t qs[8][2][W4_GROUP];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int grp = blockIdx.y * 8 + warp;
+  if (grp >= groups) return;
+  const int64_t pr = blockIdx.x;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const __nv_bfloat16* w = W + (2 * pr + e) * ldw + int64_t(grp) * W4_GROUP + 4 * lane;
+    float v[4], amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      v[i] = __bfloat162float(w[i]);
+      amax = fmaxf(amax, fabsf(v[i]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const __nv_bfloat16 sb = __float2bfloat16_rn(__fdiv_rn(amax, 7.0f));
+    const float sc = __bfloat162float(sb);
+    if (lane == 0) s[(2 * pr + e) * groups + grp] = sb;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float r = 0.f;
+      if (sc != 0.f) r = fminf(fmaxf(rintf(__fdiv_rn(v[i], sc)), -7.f), 7.f);
+      qs[warp][e][4 * lane + i] = static_cast<int8_t>(r);
+    }
+  }
+  __syncwarp();
+  // this lane writes bytes 4 lane .. 4 lane + 3 of the group: 16-k block lane / 4, t = lane % 4, byte i = 2b + h
+  uint32_t word = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = 16 * (lane >> 2) + 8 * (i & 1) + 2 * (lane & 3) + (i >> 1);
+    word |= uint32_t((qs[warp][0][c] + 8) | ((qs[warp][1][c] + 8) << 4)) << (8 * i);
+  }
+  reinterpret_cast<uint32_t*>(q + pr * K + int64_t(grp) * W4_GROUP)[lane] = word;
+}
+
 // Token-tile width and K-split count, from (m, n, k) and the SM count only. Tiles are 128 weight rows x BT tokens, BT the
 // smallest of 8, 16, 32, 64, 128 that holds m (decode fits in one token tile). Too few tiles for the SMs (decode: n = 5120
 // is 40 tiles) split K into equal runs of whole 128-deep blocks, the smallest count whose waves keep >= 90% of the SMs busy
-// (else the best), each run at least 2 blocks deep.
+// (else the best), each run at least 2 blocks deep. Both weight formats use the same plan.
 struct W8Plan {
   int bt, splits;
 };
@@ -278,13 +394,85 @@ static W8Plan w8_plan(int64_t M, int64_t N, int64_t K, int sms) {
   return {bt, best};
 }
 
-template <int BT>
-static int launch_w8(const CUtensorMap& tmW, const CUtensorMap& tmA, const CUtensorMap& tmD, const W8Params& p,
-                     cudaStream_t stream) {
-  using S = W8Smem<BT>;
-  if (int rc = ensure_smem<gemm_w8a16_kernel<BT>>(S::TOTAL, "gemm_w8a16")) return rc;
+static size_t wq_workspace_bytes(int64_t m, int64_t n, int64_t k) {
+  if (m <= 0 || n <= 0 || k <= 0) return 0;
+  const W8Plan plan = w8_plan(m, n, k, num_sms());
+  return plan.splits > 1 ? size_t(plan.splits) * size_t(m) * size_t(n) * sizeof(float) : 0;
+}
+
+template <class F, int BT>
+static int launch_wq(const CUtensorMap& tmW, const CUtensorMap& tmA, const CUtensorMap& tmD, const WqParams& p,
+                     cudaStream_t stream, const char* what) {
+  using S = WqSmem<F, BT>;
+  if (int rc = ensure_smem<gemm_wq_kernel<F, BT>>(S::TOTAL, what)) return rc;
   const int64_t grid = int64_t(p.tiles_t) * p.tiles_n * p.splits;
-  gemm_w8a16_kernel<BT><<<unsigned(grid), W8_THREADS, S::TOTAL, stream>>>(tmW, tmA, tmD, p);
+  gemm_wq_kernel<F, BT><<<unsigned(grid), W8_THREADS, S::TOTAL, stream>>>(tmW, tmA, tmD, p);
+  FSB_CUDA_LAUNCH_CHECK();
+  return FSB_OK;
+}
+
+// The checks and launch shared by fsb_gemm_w8a16 and fsb_gemm_w4a16 (`what` names the entry in messages). The format's own
+// k requirement is checked by the caller.
+template <class F>
+static int gemm_wq(const char* what, int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const void* q,
+                   const void* s, void* d, int64_t ldd, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  FSB_REQUIRE(n % 8 == 0, "%s: n=%ld must be a multiple of 8", what, (long)n);
+  FSB_REQUIRE(a && q && s && d, "%s: null operand", what);
+  FSB_REQUIRE(aligned16(a) && aligned16(q) && aligned16(s) && aligned16(d), "%s: a, q, s and d must be 16-byte aligned",
+              what);
+  FSB_REQUIRE(lda >= k && lda % 8 == 0, "%s: lda=%ld must be >= k and a multiple of 8", what, (long)lda);
+  FSB_REQUIRE(ldd >= n && ldd % 8 == 0, "%s: ldd=%ld must be >= n and a multiple of 8", what, (long)ldd);
+  const W8Plan plan = w8_plan(m, n, k, num_sms());
+  const size_t need = plan.splits > 1 ? size_t(plan.splits) * size_t(m) * size_t(n) * sizeof(float) : 0;
+  FSB_REQUIRE(need == 0 || (workspace != nullptr && workspace_bytes >= need && aligned16(workspace)),
+              "%s: this call splits K %d ways and needs a 16-byte aligned %zu-byte workspace "
+              "(fsb_%s_workspace_bytes); got %zu",
+              what, plan.splits, need, what, workspace_bytes);
+
+  CUtensorMap tmW, tmA, tmD;
+  {
+    // int8: [n, k] bytes; int4: [n / 2, k] bytes, a line per row pair
+    uint64_t dims[2] = {uint64_t(k), uint64_t(n / F::kRowsPerLine)};
+    uint64_t strides[1] = {uint64_t(k)};
+    uint32_t box[2] = {uint32_t(W8_BK), uint32_t(W8_BM / F::kRowsPerLine)};
+    int rc = make_tmap_u8(&tmW, q, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[2] = {uint64_t(k), uint64_t(m)};
+    uint64_t strides[1] = {uint64_t(lda) * 2};
+    uint32_t box[2] = {64, uint32_t(plan.bt)};
+    int rc = make_tmap_bf16(&tmA, a, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  {
+    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
+    uint64_t strides[1] = {uint64_t(ldd) * 2};
+    uint32_t box[2] = {64, uint32_t(plan.bt)};
+    int rc = make_tmap_bf16(&tmD, d, 2, dims, strides, box);
+    if (rc) return rc;
+  }
+  WqParams p;
+  p.scale = s;
+  p.ws = plan.splits > 1 ? static_cast<float*>(workspace) : nullptr;
+  p.M = int(m); p.N = int(n); p.K = int(k);
+  p.tiles_t = int((m + plan.bt - 1) / plan.bt);
+  p.tiles_n = int((n + W8_BM - 1) / W8_BM);
+  p.splits = plan.splits;
+  p.num_kb = int((k + W8_BK - 1) / W8_BK);
+  int rc = FSB_ERR_INVALID;
+  switch (plan.bt) {
+    case 8: rc = launch_wq<F, 8>(tmW, tmA, tmD, p, stream, what); break;
+    case 16: rc = launch_wq<F, 16>(tmW, tmA, tmD, p, stream, what); break;
+    case 32: rc = launch_wq<F, 32>(tmW, tmA, tmD, p, stream, what); break;
+    case 64: rc = launch_wq<F, 64>(tmW, tmA, tmD, p, stream, what); break;
+    default: rc = launch_wq<F, 128>(tmW, tmA, tmD, p, stream, what); break;
+  }
+  if (rc || plan.splits == 1) return rc;
+  const int64_t work = m * (n / 8);
+  const int blocks = int(work / 256 + 1 < 4 * num_sms() ? work / 256 + 1 : 4 * num_sms());
+  wq_splitk_reduce_kernel<F::kRowScale><<<blocks, 256, 0, stream>>>(p.ws, static_cast<const float*>(F::kRowScale ? s : nullptr),
+                                                                   plan.splits, m, n, static_cast<__nv_bfloat16*>(d), ldd);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
@@ -306,74 +494,46 @@ extern "C" int fsb_quantize_w8(const void* w, int64_t ldw, int64_t n, int64_t k,
   return FSB_OK;
 }
 
-extern "C" size_t fsb_gemm_w8a16_workspace_bytes(int64_t m, int64_t n, int64_t k) {
-  if (m <= 0 || n <= 0 || k <= 0) return 0;
-  const W8Plan plan = w8_plan(m, n, k, num_sms());
-  return plan.splits > 1 ? size_t(plan.splits) * size_t(m) * size_t(n) * sizeof(float) : 0;
-}
+extern "C" size_t fsb_gemm_w8a16_workspace_bytes(int64_t m, int64_t n, int64_t k) { return wq_workspace_bytes(m, n, k); }
 
 extern "C" int fsb_gemm_w8a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const int8_t* q,
                               const float* s, void* d, int64_t ldd, void* workspace, size_t workspace_bytes,
                               fsb_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w8a16: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
   FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w8a16: dims too large");
   FSB_REQUIRE(k % 16 == 0, "gemm_w8a16: k=%ld must be a multiple of 16", (long)k);
-  FSB_REQUIRE(n % 8 == 0, "gemm_w8a16: n=%ld must be a multiple of 8", (long)n);
-  FSB_REQUIRE(a && q && s && d, "gemm_w8a16: null operand");
-  FSB_REQUIRE(aligned16(a) && aligned16(q) && aligned16(s) && aligned16(d),
-              "gemm_w8a16: a, q, s and d must be 16-byte aligned");
-  FSB_REQUIRE(lda >= k && lda % 8 == 0, "gemm_w8a16: lda=%ld must be >= k and a multiple of 8", (long)lda);
-  FSB_REQUIRE(ldd >= n && ldd % 8 == 0, "gemm_w8a16: ldd=%ld must be >= n and a multiple of 8", (long)ldd);
-  const W8Plan plan = w8_plan(m, n, k, num_sms());
-  const size_t need = plan.splits > 1 ? size_t(plan.splits) * size_t(m) * size_t(n) * sizeof(float) : 0;
-  FSB_REQUIRE(need == 0 || (workspace != nullptr && workspace_bytes >= need && aligned16(workspace)),
-              "gemm_w8a16: this call splits K %d ways and needs a 16-byte aligned %zu-byte workspace "
-              "(fsb_gemm_w8a16_workspace_bytes); got %zu",
-              plan.splits, need, workspace_bytes);
+  return gemm_wq<FmtW8>("gemm_w8a16", m, n, k, a, lda, q, s, d, ldd, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream_));
+}
 
-  CUtensorMap tmW, tmA, tmD;
-  {
-    uint64_t dims[2] = {uint64_t(k), uint64_t(n)};
-    uint64_t strides[1] = {uint64_t(k)};
-    uint32_t box[2] = {uint32_t(W8_BK), uint32_t(W8_BM)};
-    int rc = make_tmap_u8(&tmW, q, 2, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {uint64_t(k), uint64_t(m)};
-    uint64_t strides[1] = {uint64_t(lda) * 2};
-    uint32_t box[2] = {64, uint32_t(plan.bt)};
-    int rc = make_tmap_bf16(&tmA, a, 2, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
-    uint64_t strides[1] = {uint64_t(ldd) * 2};
-    uint32_t box[2] = {64, uint32_t(plan.bt)};
-    int rc = make_tmap_bf16(&tmD, d, 2, dims, strides, box);
-    if (rc) return rc;
-  }
-  W8Params p;
-  p.scale = s;
-  p.ws = plan.splits > 1 ? static_cast<float*>(workspace) : nullptr;
-  p.M = int(m); p.N = int(n); p.K = int(k);
-  p.tiles_t = int((m + plan.bt - 1) / plan.bt);
-  p.tiles_n = int((n + W8_BM - 1) / W8_BM);
-  p.splits = plan.splits;
-  p.num_kb = int((k + W8_BK - 1) / W8_BK);
-  int rc = FSB_ERR_INVALID;
-  switch (plan.bt) {
-    case 8: rc = launch_w8<8>(tmW, tmA, tmD, p, stream); break;
-    case 16: rc = launch_w8<16>(tmW, tmA, tmD, p, stream); break;
-    case 32: rc = launch_w8<32>(tmW, tmA, tmD, p, stream); break;
-    case 64: rc = launch_w8<64>(tmW, tmA, tmD, p, stream); break;
-    default: rc = launch_w8<128>(tmW, tmA, tmD, p, stream); break;
-  }
-  if (rc || plan.splits == 1) return rc;
-  const int64_t work = m * (n / 8);
-  const int blocks = int(work / 256 + 1 < 4 * num_sms() ? work / 256 + 1 : 4 * num_sms());
-  w8_splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(p.ws, s, plan.splits, m, n, static_cast<__nv_bfloat16*>(d), ldd);
+extern "C" int fsb_quantize_w4(const void* w, int64_t ldw, int64_t n, int64_t k, uint8_t* q, void* s,
+                               fsb_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  FSB_REQUIRE(n > 0 && k > 0, "quantize_w4: non-positive dims n=%ld k=%ld", (long)n, (long)k);
+  FSB_REQUIRE(n < (int64_t(1) << 31) && k < (int64_t(1) << 30), "quantize_w4: n=%ld or k=%ld too large", (long)n, (long)k);
+  FSB_REQUIRE(k % W4_GROUP == 0, "quantize_w4: k=%ld must be a multiple of %d (the scale group)", (long)k, W4_GROUP);
+  FSB_REQUIRE(n % 8 == 0, "quantize_w4: n=%ld must be a multiple of 8", (long)n);
+  FSB_REQUIRE(ldw >= k, "quantize_w4: ldw=%ld < k=%ld", (long)ldw, (long)k);
+  FSB_REQUIRE(w && q && s, "quantize_w4: null pointer");
+  FSB_REQUIRE((reinterpret_cast<uintptr_t>(w) & 1) == 0 && (reinterpret_cast<uintptr_t>(q) & 3) == 0 &&
+                  (reinterpret_cast<uintptr_t>(s) & 1) == 0,
+              "quantize_w4: misaligned w, q or s");
+  const int groups = int(k / W4_GROUP);
+  const dim3 grid(unsigned(n / 2), unsigned((groups + 7) / 8));
+  quantize_w4_kernel<<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(w), ldw, k, groups, q,
+                                               static_cast<__nv_bfloat16*>(s));
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
+}
+
+extern "C" size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k) { return wq_workspace_bytes(m, n, k); }
+
+extern "C" int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q,
+                              const void* s, void* d, int64_t ldd, void* workspace, size_t workspace_bytes,
+                              fsb_stream_t stream_) {
+  FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w4a16: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
+  FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w4a16: dims too large");
+  FSB_REQUIRE(k % W4_GROUP == 0, "gemm_w4a16: k=%ld must be a multiple of %d (the scale group)", (long)k, W4_GROUP);
+  return gemm_wq<FmtW4>("gemm_w4a16", m, n, k, a, lda, q, s, d, ldd, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream_));
 }

@@ -322,5 +322,10 @@ __device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
   asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 }  // namespace fsb

@@ -31,9 +31,10 @@ import torch.distributed as dist
 class ZeroEngine:
     def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.1, grad_clip=0.0, ga_steps=1,
                  process_group=None, stage=2, kernels=None, overlap_comm=True, comm_sms=None, comm_backend="torch", tp_group=None):
-        if getattr(model, "load_in_8bit", False):
-            raise NotImplementedError("fsb200 ZeroEngine: an int8 (load_in_8bit=True) model only runs inference; training it "
-                                      "is not implemented")
+        fmt = getattr(model, "weight_format", "bf16")   # "int8" / "int4": a load_in_8bit / load_in_4bit model
+        if fmt != "bf16":
+            raise NotImplementedError(f"fsb200 ZeroEngine: an {fmt} (load_in_{fmt[3:]}bit=True) model only runs inference; "
+                                      "training it is not implemented")
         self.model = model
         self.flat = model.flat
         self.lr, self.betas, self.eps, self.weight_decay = lr, betas, eps, weight_decay

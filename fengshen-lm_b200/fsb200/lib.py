@@ -36,6 +36,10 @@ SIGNATURES = {
     "fsb_gemm_w8a16_workspace_bytes": (c_size, [c_i64, c_i64, c_i64]),
     "fsb_gemm_w8a16": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_size,
                                c_void_p]),
+    "fsb_quantize_w4": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_void_p]),
+    "fsb_gemm_w4a16_workspace_bytes": (c_size, [c_i64, c_i64, c_i64]),
+    "fsb_gemm_w4a16": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_size,
+                               c_void_p]),
     "fsb_norm_bwd_workspace_bytes": (c_size, [c_i64, c_i64, c_int]),
     "fsb_rmsnorm_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_f32,
                                 c_void_p]),

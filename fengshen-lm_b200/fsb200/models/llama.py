@@ -37,14 +37,20 @@ def _init_normal_(t, std, gen):
 
 _W8_NAMES = ("attention.query_key_value.weight", "attention.dense.weight", "mlp.w1.weight", "mlp.w3.weight", "mlp.w2.weight")
 
+# weight format -> (quantiser, GEMM, (q dtype, q shape, s dtype, s shape) of an [n, k] weight)
+_WQ = {
+    "int8": (ops.quantize_w8, ops.gemm_w8a16, lambda n, k: (torch.int8, (n, k), torch.float32, (n,))),
+    "int4": (ops.quantize_w4, ops.gemm_w4a16, lambda n, k: (torch.uint8, (n // 2, k), torch.bfloat16, (n, k // 128))),
+}
 
-def _int8_unsupported(what):
-    return NotImplementedError(f"fsb200 LlamaForCausalLM: {what} is not implemented for an int8 (load_in_8bit=True) model; "
-                               "it only runs inference")
+
+def _quantized_unsupported(fmt, what):
+    return NotImplementedError(f"fsb200 LlamaForCausalLM: {what} is not implemented for an {fmt} (load_in_{fmt[3:]}bit=True) "
+                               "model; it only runs inference")
 
 
 class LlamaForCausalLM(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False):
+    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False, load_in_4bit=False):
         """tp_group: the tensor-model-parallel process group (mpu.get_model_parallel_group()) or None. With t = its size > 1
         this rank holds the shard the reference's `part_{rank}` checkpoints hold (utils/llama_convert/convert_fs_llama_tp.py
         :143-181): heads / ff columns / vocabulary rows split t ways (ColumnParallelLinear mpu/layers.py:261-360 for QKV,
@@ -54,15 +60,25 @@ class LlamaForCausalLM(FlatModel):
         load_in_8bit: an inference-only model (`from_pretrained(..., load_in_8bit=True)`, examples/ziya_inference/
         hf_quantizatin_inference.py:20-22). Each layer's four projections (query_key_value, dense, w1 | w3, w2) are held as
         int8 q [n, k] + fp32 per-row scales s [n] and run through the W8A16 GEMM; the embedding, the norm scales and the LM
-        head stay bf16 in flat buffers without a gradient buffer. Training, tensor parallelism and save_pretrained raise."""
+        head stay bf16 in flat buffers without a gradient buffer. Training, tensor parallelism and save_pretrained raise.
+
+        load_in_4bit: the same with int4 projections (examples/ziya_inference/hf_quantizatin_inference.py:3,16): q packed two
+        per byte [n / 2, k] + bf16 scales [n, k / 128], one per row and group of 128 k, run through the W4A16 GEMM.
+        hidden_size and the MLP width must then be multiples of 128."""
         super().__init__(config)
         import torch.distributed as dist
-        self.load_in_8bit = bool(load_in_8bit)
+        if load_in_8bit and load_in_4bit:
+            raise ValueError("fsb200 LlamaForCausalLM: load_in_8bit and load_in_4bit are mutually exclusive; pass one")
+        # the layer projections' weight format; load_in_8bit / load_in_4bit are kept as the public flags
+        self.weight_format = "int8" if load_in_8bit else "int4" if load_in_4bit else "bf16"
+        self.load_in_8bit = self.weight_format == "int8"
+        self.load_in_4bit = self.weight_format == "int4"
+        quantized = self.weight_format != "bf16"
         self.tp_group = tp_group
         self.tp = dist.get_world_size(tp_group) if tp_group is not None else 1
         self.tp_rank = dist.get_rank(tp_group) if tp_group is not None else 0
-        if self.load_in_8bit and self.tp > 1:
-            raise _int8_unsupported("tensor parallelism")
+        if quantized and self.tp > 1:
+            raise _quantized_unsupported(self.weight_format, "tensor parallelism")
         h, V, nl, nh = config.hidden_size, config.vocab_size, config.num_hidden_layers, config.num_attention_heads
         self.h, self.V, self.nl, self.nh = h, V, nl, nh
         self.hn = h // nh
@@ -75,6 +91,9 @@ class LlamaForCausalLM(FlatModel):
         t = self.tp
         if nh % t or self.ff % (8 * t) or V % (8 * t):
             raise RuntimeError(f"fsb200: heads {nh}, ff {self.ff} and vocab {V} must split evenly over tensor-parallel size {t}")
+        if self.load_in_4bit and (h % 128 or self.ff % 128):
+            raise RuntimeError(f"fsb200: an int4 model needs hidden_size ({h}) and the MLP width ({self.ff}) to be multiples "
+                               "of 128 (the scale group)")
         # local (per tensor-parallel rank) extents
         self.nh_l, self.ff_l, self.V_l = nh // t, self.ff // t, V // t
         self.h_l = self.nh_l * self.hn
@@ -85,23 +104,29 @@ class LlamaForCausalLM(FlatModel):
         for i in range(nl):
             p, bk = f"llama.layers.{i}.", f"layer{i}"
             spec.add(p + "input_layernorm.scale", (h,), bk)          # *.scale names match 'layernorm.' -> no-decay bucket
-            if not self.load_in_8bit:
+            if not quantized:
                 spec.add(p + "attention.query_key_value.weight", (3 * self.h_l, h), bk)
                 spec.add(p + "attention.dense.weight", (h, self.h_l), bk)
             spec.add(p + "post_attention_layernorm.scale", (h,), bk)
-            if not self.load_in_8bit:
+            if not quantized:
                 spec.add(p + "mlp.w1.weight", (self.ff_l, h), bk)   # w1 | w3 adjacent: one [2ff, h] GEMM operand
                 spec.add(p + "mlp.w3.weight", (self.ff_l, h), bk)
                 spec.add(p + "mlp.w2.weight", (h, self.ff_l), bk)
         spec.add("llama.final_layer_norm.scale", (h,), "head")
         spec.add("embed_out.final_linear.weight", (self.V_l, h), "head")
-        self._bind_flat(spec, device, world_size, tp=self.tp, grads=not self.load_in_8bit)
-        if self.load_in_8bit:
-            # per layer {projection: (q int8 [n, k], s fp32 [n])}; w1 | w3 is one [2ff, h] operand as in the bf16 layout
+        self._bind_flat(spec, device, world_size, tp=self.tp, grads=not quantized)
+        if quantized:
+            # per layer {projection: (q, s)} in the format's layout (_WQ); w1 | w3 is one [2ff, h] operand as in the bf16
+            # layout. The int8 model keeps them in self._w8, the int4 one in self._w4; self._wq is the model's own.
             dev = self.flat.params.device
             shapes = {"qkv": (3 * h, h), "dense": (h, h), "w13": (2 * self.ff, h), "w2": (h, self.ff)}
-            self._w8 = [{k: (torch.zeros(n_k, dtype=torch.int8, device=dev), torch.zeros(n_k[0], dtype=torch.float32, device=dev))
-                         for k, n_k in shapes.items()} for _ in range(nl)]
+            layout = _WQ[self.weight_format][2]
+
+            def zeros(n, k):
+                qd, qs, sd, ss = layout(n, k)
+                return torch.zeros(qs, dtype=qd, device=dev), torch.zeros(ss, dtype=sd, device=dev)
+            self._wq = [{key: zeros(*n_k) for key, n_k in shapes.items()} for _ in range(nl)]
+            setattr(self, "_w8" if self.load_in_8bit else "_w4", self._wq)
         else:
             self._w13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h)
                          for i in range(nl)]
@@ -111,7 +136,7 @@ class LlamaForCausalLM(FlatModel):
         # buffer of every layer in the reference's module tree (modeling_llama.py:97-127), hence in its state dict
         self._inv_freq = 1.0 / (getattr(config, "rotary_emb_base", 10000) ** (torch.arange(0, self.hn, 2).float() / self.hn))
         for lyr in self.llama.layers:
-            if "attention" not in lyr._modules:    # int8: the projections live outside the flat buffers
+            if "attention" not in lyr._modules:    # int8 / int4: the projections live outside the flat buffers
                 lyr.attention = _Holder()
             lyr.attention.rotary_emb = _Holder()
             lyr.attention.rotary_emb.register_buffer("inv_freq", self._inv_freq.clone().to(self.flat.params.device))
@@ -148,48 +173,57 @@ class LlamaForCausalLM(FlatModel):
                 prm.normal_(0.0, std, generator=gen)
             else:
                 _init_normal_(prm.data, std, gen)
-        if self.load_in_8bit:   # each int8 matrix: drawn in bf16 on the device and quantised, one temporary at a time
+        if self.weight_format != "bf16":   # each quantised matrix: drawn in bf16 on the device and quantised, one at a time
             dgen = torch.Generator(device=self.flat.params.device).manual_seed(seed + 104729)
-            for w8 in self._w8:
-                for key, (q, s) in w8.items():
-                    tmp = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
+            for wq in self._wq:
+                for key, (q, s) in wq.items():
+                    tmp = torch.empty(self._weight_shape(q, s), dtype=torch.bfloat16, device=q.device)
                     tmp.normal_(0.0, wang if key in ("dense", "w2") else small, generator=dgen)
-                    ops.quantize_w8(tmp, q, s)
+                    self._quantize(tmp, q, s)
                     del tmp
 
-    # ---- int8 (load_in_8bit) ------------------------------------------------------------------------------------------
+    # ---- int8 / int4 (load_in_8bit / load_in_4bit) ---------------------------------------------------------------------
+    def _quantize(self, w, q, s):
+        _WQ[self.weight_format][0](w, q, s)
+
+    @staticmethod
+    def _weight_shape(q, s):
+        """[n, k] of the bf16 weight that (q, s) holds: s has one row per weight row in both formats, q the k columns."""
+        return s.shape[0], q.shape[1]
+
     @torch.no_grad()
     def load_reference_state_dict(self, sd):
-        """As FlatModel.load_reference_state_dict; an int8 model quantises each projection on the device as it arrives."""
-        if not self.load_in_8bit:
+        """As FlatModel.load_reference_state_dict; a quantised model quantises each projection on the device as it arrives."""
+        if self.weight_format == "bf16":
             return super().load_reference_state_dict(sd)
-        targets = set(self._p) | set(self._w8_targets())
+        targets = set(self._p) | set(self._wq_targets())
         missing = targets - set(sd)
         if missing:
             raise KeyError(f"missing key in state dict: {sorted(missing)[0]}")
-        self._load_w8_shard(sd, set())
+        self._load_quantized_shard(sd, set())
 
-    def _w8_targets(self):
-        """{state-dict key: (q, s) row slice it quantises into} of every int8 projection."""
-        out, ff = {}, self.ff
-        for i, w8 in enumerate(self._w8):
+    def _wq_targets(self):
+        """{state-dict key: (q, s) row slice it quantises into} of every quantised projection."""
+        out = {}
+        for i, wq in enumerate(self._wq):
             p = f"llama.layers.{i}."
-            (qq, sq), (qd, sd_), (q13, s13), (q2, s2) = w8["qkv"], w8["dense"], w8["w13"], w8["w2"]
+            (qq, sq), (qd, sd_), (q13, s13), (q2, s2) = wq["qkv"], wq["dense"], wq["w13"], wq["w2"]
+            hq, hs = q13.shape[0] // 2, s13.shape[0] // 2     # w1 is the upper half of the [2ff, h] operand, w3 the lower
             out[p + _W8_NAMES[0]] = (qq, sq)
             out[p + _W8_NAMES[1]] = (qd, sd_)
-            out[p + _W8_NAMES[2]] = (q13[:ff], s13[:ff])
-            out[p + _W8_NAMES[3]] = (q13[ff:], s13[ff:])
+            out[p + _W8_NAMES[2]] = (q13[:hq], s13[:hs])
+            out[p + _W8_NAMES[3]] = (q13[hq:], s13[hs:])
             out[p + _W8_NAMES[4]] = (q2, s2)
         return out
 
     @torch.no_grad()
-    def _load_w8_shard(self, sd, loaded):
-        """Load the keys of `sd` (a whole state dict or one checkpoint shard) this int8 model holds: bf16 parameters are
-        copied, projections quantised on the device (one bf16 temporary at a time). The shard's shapes are checked before
+    def _load_quantized_shard(self, sd, loaded):
+        """Load the keys of `sd` (a whole state dict or one checkpoint shard) this int8 / int4 model holds: bf16 parameters
+        are copied, projections quantised on the device (one bf16 temporary at a time). The shard's shapes are checked before
         anything is written. Adds the loaded keys to the set `loaded` and returns the keys it does not yet hold."""
-        targets = self._w8_targets()
+        targets = self._wq_targets()
         for k, v in sd.items():
-            want = tuple(self._p[k].shape) if k in self._p else tuple(targets[k][0].shape) if k in targets else None
+            want = tuple(self._p[k].shape) if k in self._p else tuple(self._weight_shape(*targets[k])) if k in targets else None
             if want is not None and tuple(v.shape) != want:
                 raise ValueError(f"shape mismatch for {k}: {tuple(v.shape)} vs {want}")
         for k, v in sd.items():
@@ -199,7 +233,7 @@ class LlamaForCausalLM(FlatModel):
             elif k in targets:
                 q, s = targets[k]
                 tmp = v.to(q.device).contiguous()
-                ops.quantize_w8(tmp, q, s)
+                self._quantize(tmp, q, s)
                 del tmp
             else:
                 continue
@@ -207,25 +241,26 @@ class LlamaForCausalLM(FlatModel):
         return (set(self._p) | set(targets)) - loaded
 
     def get_memory_footprint(self):
-        """Bytes held by the model's tensors: parameters (and their gradient buffer, if any), int8 weights and scales, and
+        """Bytes held by the model's tensors: parameters (and their gradient buffer, if any), int8 / int4 weights and scales, and
         buffers (transformers' `PreTrainedModel.get_memory_footprint`, which hf_quantizatin_inference.py prints)."""
         n = self.flat.params.numel() * self.flat.params.element_size()
         if self.flat.grads is not None:
             n += self.flat.grads.numel() * self.flat.grads.element_size()
-        for w8 in getattr(self, "_w8", ()):
-            n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in w8.values())
+        for wq in getattr(self, "_wq", ()):
+            n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in wq.values())
         return n + sum(b.numel() * b.element_size() for b in self.buffers())
 
     def save_pretrained(self, path, **kw):
-        if self.load_in_8bit:
-            raise _int8_unsupported("save_pretrained (int8 export)")
+        if self.weight_format != "bf16":
+            raise _quantized_unsupported(self.weight_format, f"save_pretrained ({self.weight_format} export)")
         return super().save_pretrained(path, **kw)
 
     def _linear(self, i, name, x):
-        """x @ W^T for layer i's projection `name` (qkv, dense, w13, w2): the bf16 GEMM, or the W8A16 GEMM of an int8 model."""
-        if self.load_in_8bit:
-            q, s = self._w8[i][name]
-            return ops.gemm_w8a16(x, q, s)
+        """x @ W^T for layer i's projection `name` (qkv, dense, w13, w2): the bf16 GEMM, or the W8A16 / W4A16 GEMM of an
+        int8 / int4 model."""
+        if self.weight_format != "bf16":
+            q, s = self._wq[i][name]
+            return _WQ[self.weight_format][1](x, q, s)
         lyr = self.llama.layers[i]
         if name == "qkv":
             w = lyr.attention.query_key_value.weight.data
@@ -258,8 +293,8 @@ class LlamaForCausalLM(FlatModel):
                                     "fsb200 LlamaForCausalLM: position_ids outside [0, rope table rows); pass them on the "
                                     "host or raise config.max_position_embeddings")
         lab = flat_ids(labels, dev)
-        if self.load_in_8bit and lab is not None and torch.is_grad_enabled():
-            raise _int8_unsupported("a training forward (labels under grad mode)")
+        if self.weight_format != "bf16" and lab is not None and torch.is_grad_enabled():
+            raise _quantized_unsupported(self.weight_format, "a training forward (labels under grad mode)")
         loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)

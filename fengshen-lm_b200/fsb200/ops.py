@@ -132,6 +132,47 @@ def gemm_w8a16(a, q, s, out=None):
     return out
 
 
+def quantize_w4(w, q=None, s=None):
+    """Symmetric int4 quantisation of a bf16 weight w[n, k] (unit inner stride) with one scale per row and group of 128 k
+    -> (q uint8 [n / 2, k] contiguous, two 4-bit codes per byte, s bf16 [n, k / 128] contiguous) with
+    s = bf16(absmax / 7) and q = clamp(rint(w / s), -7, 7); include/fsb200.h gives the packed layout. q and s may be given
+    (contiguous, e.g. row slices of a larger operand: an even number of rows) to quantise in place of a new allocation."""
+    _chk(w, _bf16, "w")
+    n, k, ldw = _rows2d(w, "w")
+    if n % 2 or k % 128:
+        raise RuntimeError(f"fsb200 quantize_w4: w [{n}, {k}] needs k a multiple of 128 and n a multiple of 8")
+    q = torch.empty((n // 2, k), dtype=torch.uint8, device=w.device) if q is None else q
+    s = torch.empty((n, k // 128), dtype=_bf16, device=w.device) if s is None else s
+    _chk(q, torch.uint8, "q"); _chk(s, _bf16, "s")
+    if tuple(q.shape) != (n // 2, k) or not q.is_contiguous() or tuple(s.shape) != (n, k // 128) or not s.is_contiguous():
+        raise RuntimeError(f"fsb200 quantize_w4: q must be contiguous [{n // 2}, {k}] and s contiguous [{n}, {k // 128}]")
+    L.call("fsb_quantize_w4", _p(w), ldw, n, k, _p(q), _p(s), _stream())
+    return q, s
+
+
+def gemm_w4a16(a, q, s, out=None):
+    """out[m, n] = bf16(a[m, k] @ W^[n, k]^T), fp32 accumulation, W^ = bf16(q * s) the dequantised int4 weight: a bf16
+    (unit inner stride), q uint8 [n / 2, k] and s bf16 [n, k / 128] contiguous as quantize_w4 returns them. `out` (bf16,
+    unit inner stride) may be a strided view."""
+    _chk(a, _bf16, "a"); _chk(q, torch.uint8, "q"); _chk(s, _bf16, "s")
+    m, k, lda = _rows2d(a, "a")
+    if q.dim() != 2 or not q.is_contiguous(): raise RuntimeError("fsb200 gemm_w4a16: q must be contiguous [n / 2, k]")
+    n = 2 * q.shape[0]
+    if q.shape[1] != k: raise RuntimeError(f"fsb200 gemm_w4a16: K mismatch {k} vs {q.shape[1]}")
+    if s.dim() != 2 or s.shape[0] != n or s.shape[1] * 128 != k or not s.is_contiguous():
+        raise RuntimeError(f"fsb200 gemm_w4a16: s must be contiguous [{n}, k / 128] for k = {k}")
+    if out is None:
+        out = torch.empty((m, n), dtype=_bf16, device=a.device)
+    _chk(out, _bf16, "out")
+    orr, occ, ldd = _rows2d(out, "out")
+    if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_w4a16: out shape {tuple(out.shape)} != ({m},{n})")
+    ws_bytes = int(L.load().fsb_gemm_w4a16_workspace_bytes(m, n, k))
+    ws = workspace(ws_bytes, a.device, "gemm_w4a16") if ws_bytes else None
+    L.call("fsb_gemm_w4a16", m, n, k, _p(a), lda, _p(q), _p(s), _p(out), ldd, _p(ws), ws_bytes, _stream(),
+           tag=f"{m}x{n}x{k}" if L.call_profiler is not None else None)
+    return out
+
+
 def set_reserved_sms(n):
     """Leave n SMs (2n for CTA-pair kernels) of every persistent GEMM grid to overlapping communication kernels."""
     L.call("fsb_set_reserved_sms", int(n))

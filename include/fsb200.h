@@ -103,6 +103,32 @@ size_t fsb_gemm_w8a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int fsb_gemm_w8a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const int8_t* q, const float* s,
                    void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- int4 weight-only inference (W4A16) ------------------------------------------------------------------------
+ * Stand in for `from_pretrained(..., load_in_4bit=True)` (fengshen/examples/ziya_inference/hf_quantizatin_inference.py:3,16).
+ * Symmetric round-to-nearest with one scale per output row and group of 128 consecutive k, no calibration and no zero
+ * point: results are not bit-comparable with bitsandbytes NF4/FP4 or llama.cpp q4_*.
+ *
+ * fsb_quantize_w4: W bf16 [n, k] (row stride ldw >= k). For row r and group g (columns 128g .. 128g + 127):
+ *   a = absmax(W[r, group]) over the fp32 values; s[r, g] = bf16_rne(a / 7.0f), the division IEEE fp32;
+ *   q[r, c] = clamp(rint(W[r, c] / float(s[r, g])), -7, 7), rint rounding half to even, the division IEEE fp32; where
+ *   s == 0 (a zero group, or an underflow) q = 0. The dequantised weight is W^[r, c] = bf16_rne(q[r, c] * s[r, g]), the
+ *   exact product rounded once.
+ *   s: bf16 [n, k / 128] row-major contiguous.
+ *   q: n * k / 2 bytes, packed as [n / 2, k] bytes, row-major contiguous. Byte line p holds rows 2p and 2p + 1: row 2p in
+ *   the low nibble, row 2p + 1 in the high nibble, each as the 4-bit code q + 8 (1 .. 15). Along the line, k runs in blocks
+ *   of 16; inside block j (bytes 16j .. 16j + 15) the byte at 16j + 4t + 2b + h (t < 4, b < 2, h < 2) holds
+ *   k = 16j + 8h + 2t + b. Each 32-bit word is then one thread's wgmma register-A fragment for one k16 step.
+ *   Requirements: k % 128 == 0, n % 8 == 0, w 2-byte, q 4-byte and s 2-byte aligned. fsb_quantize_w4 is the only writer of
+ *   this layout.
+ * fsb_gemm_w4a16: D[m, n] = bf16(sum_k A[m, k] W^[n, k]), fp32 accumulation. A bf16 [m, k] (row stride lda), q / s as
+ *   fsb_quantize_w4 writes them, D bf16 [m, n] (row stride ldd). Requirements: k % 128 == 0 and otherwise as fsb_gemm_w8a16
+ *   (n % 8 == 0, lda >= k and ldd >= n multiples of 8, a / q / s / d 16-byte aligned). Tiles, K-split plan, workspace
+ *   (fsb_gemm_w4a16_workspace_bytes) and determinism as fsb_gemm_w8a16. */
+int fsb_quantize_w4(const void* w, int64_t ldw, int64_t n, int64_t k, uint8_t* q, void* s, fsb_stream_t stream);
+size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
+int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
+                   void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
+
 /* ---- RMSNorm / LayerNorm ------------------------------------------------------------------------------------
  * RMSNorm.forward fengshen/models/megatron/layers/norms.py:44-52 (y = scale * cast(x * rsqrt(mean(x^2) + eps)), the cast to
  * 16 bit happening BEFORE the scale multiply); LayerNorm = torch.nn.LayerNorm (norms.py:16; HF BERT/GPT-2 eps 1e-12/1e-5).

@@ -1,17 +1,18 @@
-"""Int8 weight-only (W8A16) LLaMA inference on one GPU.
+"""Int8 (W8A16) and int4 (W4A16) weight-only LLaMA inference on one GPU.
 
-1. Kernel A/B: fsb_gemm_w8a16 against fsb_gemm_bf16 (NT) on the Ziya-LLaMA-13B projection shapes (n, k) = (15360, 5120)
-   query_key_value, (5120, 5120) dense, (27648, 5120) w1|w3, (5120, 13824) w2, at m = 1, 8, 32 token rows (decode) and 4096
-   (prefill). Device time per call: 50 calls captured in one CUDA graph, the graph replayed under CUDA events; the two
-   kernels alternated `--reps` times, medians reported. Bytes per call: int8 n*k + 4n (weights and scales) + 2mk + 2mn,
-   bf16 2nk + 2mk + 2mn; GB/s and the share of the 3.35 TB/s HBM3 data-sheet figure for m <= 32, TFLOP/s (2mnk) at 4096.
+1. Kernel A/B/C: fsb_gemm_w8a16 and fsb_gemm_w4a16 against fsb_gemm_bf16 (NT) on the Ziya-LLaMA-13B projection shapes
+   (n, k) = (15360, 5120) query_key_value, (5120, 5120) dense, (27648, 5120) w1|w3, (5120, 13824) w2, at m = 1, 8, 32 token
+   rows (decode) and 4096 (prefill). Device time per call: 50 calls captured in one CUDA graph, the graph replayed under
+   CUDA events; the three kernels alternated `--reps` times, medians reported. Bytes per call: int8 n*k + 4n (weights and
+   scales) + 2mk + 2mn, int4 n*k/2 + 2n*k/128 + 2mk + 2mn, bf16 2nk + 2mk + 2mn; GB/s and the share of the 3.35 TB/s HBM3
+   data-sheet figure for m <= 32, TFLOP/s (2mnk) at 4096.
 2. End to end: `generate` at Ziya width (hidden 5120, 40 heads, ff 13824, vocabulary 39424), prompt 512, 128 new tokens,
-   batch 1 and 8, greedy, random weights: bf16 and int8 at 8 of the 40 layers, int8 at all 40. Tokens/s (host wall clock,
+   batch 1 and 8, greedy, random weights: bf16, int8 and int4 at 8 of the 40 layers, int8 and int4 at all 40. Tokens/s (host wall clock,
    median of `--reps`), device time per new token (torch.profiler, prefill included, separate run), host `fsb_*` calls per
    new token, and the peak of torch.cuda.max_memory_allocated over building the model and generating, above what was
    allocated before.
 
-  python tools/bench_int8.py [--reps 3] [--skip-e2e] [--out DIR]
+  python tools/bench_int8.py [--reps 3] [--skip-e2e] [--skip-40] [--out DIR]
 
 Prints one JSON line per measurement, the card's name, power limit and max SM clock first; --out also writes them to
 DIR/bench_int8.jsonl."""
@@ -74,34 +75,55 @@ def kernel_ab(reps, emit):
     for name, n, k in SHAPES:
         w = (torch.randn((n, k), generator=gen, device="cuda") * 0.02).to(torch.bfloat16)
         q, s = ops.quantize_w8(w)
+        q4, s4 = ops.quantize_w4(w)
+        w4 = dequantize_w4(q4, s4)
         for m in (1, 8, 32, 4096):
             a = torch.randn((m, k), generator=gen, device="cuda").to(torch.bfloat16)
             d8 = torch.empty((m, n), dtype=torch.bfloat16, device="cuda")
+            d4 = torch.empty((m, n), dtype=torch.bfloat16, device="cuda")
             d16 = torch.empty((m, n), dtype=torch.bfloat16, device="cuda")
             f16 = lambda: ops.gemm(L.GEMM_NT, a, w, out=d16)            # noqa: E731  (the decode step's bf16 call)
             f8 = lambda: ops.gemm_w8a16(a, q, s, out=d8)                # noqa: E731
-            t16, t8 = [], []
+            f4 = lambda: ops.gemm_w4a16(a, q4, s4, out=d4)              # noqa: E731
+            t16, t8, t4 = [], [], []
             for _ in range(reps):
                 t16.append(graph_us(f16))
                 t8.append(graph_us(f8))
-            t16, t8 = sorted(t16)[reps // 2], sorted(t8)[reps // 2]
-            # the int8 result against the bf16 GEMM of the dequantised weight (a sanity figure, not a test)
+                t4.append(graph_us(f4))
+            t16, t8, t4 = sorted(t16)[reps // 2], sorted(t8)[reps // 2], sorted(t4)[reps // 2]
+            # each result against the bf16 GEMM of its dequantised weight (a sanity figure, not a test)
             ref = ops.gemm(L.GEMM_NT, a, (q.float() * s[:, None]).to(torch.bfloat16)).float()
             rel = float((d8.float() - ref).abs().max() / ref.abs().max().clamp_min(1e-30))
+            ref4 = ops.gemm(L.GEMM_NT, a, w4).float()
+            rel4 = float((d4.float() - ref4).abs().max() / ref4.abs().max().clamp_min(1e-30))
             b8 = n * k + 4 * n + 2 * m * k + 2 * m * n
+            b4 = n * k // 2 + 2 * n * (k // 128) + 2 * m * k + 2 * m * n
             b16 = 2 * n * k + 2 * m * k + 2 * m * n
-            line = dict(bench="gemm_w8a16_ab", shape=name, m=m, n=n, k=k, bf16_us=round(t16, 2), int8_us=round(t8, 2),
-                        speedup=round(t16 / t8, 3), splitk_workspace_bytes=int(L.load().fsb_gemm_w8a16_workspace_bytes(m, n, k)),
-                        max_rel_diff_vs_dequantised_bf16=rel, reps=reps)
+            line = dict(bench="gemm_weight_only_ab", shape=name, m=m, n=n, k=k, bf16_us=round(t16, 2), int8_us=round(t8, 2),
+                        int4_us=round(t4, 2), speedup=round(t16 / t8, 3), int4_speedup=round(t16 / t4, 3),
+                        int4_over_int8=round(t8 / t4, 3),
+                        splitk_workspace_bytes=int(L.load().fsb_gemm_w8a16_workspace_bytes(m, n, k)),
+                        max_rel_diff_vs_dequantised_bf16=rel, int4_max_rel_diff_vs_dequantised_bf16=rel4, reps=reps)
             if m <= 32:
-                line.update(int8_GBps=round(b8 / t8 / 1e3, 1), bf16_GBps=round(b16 / t16 / 1e3, 1),
-                            int8_share_of_hbm=round(b8 / (t8 * 1e-6) / HBM, 3), bf16_share_of_hbm=round(b16 / (t16 * 1e-6) / HBM, 3))
+                line.update(int8_GBps=round(b8 / t8 / 1e3, 1), int4_GBps=round(b4 / t4 / 1e3, 1), bf16_GBps=round(b16 / t16 / 1e3, 1),
+                            int8_share_of_hbm=round(b8 / (t8 * 1e-6) / HBM, 3), int4_share_of_hbm=round(b4 / (t4 * 1e-6) / HBM, 3),
+                            bf16_share_of_hbm=round(b16 / (t16 * 1e-6) / HBM, 3))
             else:
-                line.update(int8_TFLOPs=round(2 * m * n * k / t8 / 1e6, 1), bf16_TFLOPs=round(2 * m * n * k / t16 / 1e6, 1))
+                line.update(int8_TFLOPs=round(2 * m * n * k / t8 / 1e6, 1), int4_TFLOPs=round(2 * m * n * k / t4 / 1e6, 1),
+                            bf16_TFLOPs=round(2 * m * n * k / t16 / 1e6, 1))
             emit(line)
-            del a, d8, d16, ref
-        del w, q, s
+            del a, d8, d4, d16, ref, ref4
+        del w, q, s, q4, s4, w4
         torch.cuda.empty_cache()
+
+
+def dequantize_w4(q, s):
+    """W^ = bf16(q * s) of an int4 weight, unpacked on the device by the layout of include/fsb200.h (bench sanity check)."""
+    n2, k = q.shape
+    b = q.view(n2, k // 16, 4, 2, 2).to(torch.int16)                          # [p, block, t, b, h]
+    u = torch.stack([b & 0xF, b >> 4], dim=-1) - 8                           # [p, block, t, b, h, row]
+    qi = u.permute(0, 5, 1, 4, 2, 3).reshape(2 * n2, k).float()
+    return (qi.view(2 * n2, k // 128, 128) * s.float()[:, :, None]).view(2 * n2, k).to(torch.bfloat16)
 
 
 def _count_calls():
@@ -115,9 +137,10 @@ def _count_calls():
     return n
 
 
-def end_to_end(reps, emit, S=512, new=128):
+def end_to_end(reps, emit, S=512, new=128, full=True):
     calls = _count_calls()
-    for layers, int8 in ((8, False), (8, True), (40, True)):
+    runs = [(8, "bf16"), (8, "int8"), (8, "int4")] + ([(40, "int8"), (40, "int4")] if full else [])
+    for layers, fmt in runs:
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
         base = torch.cuda.memory_allocated()
@@ -125,7 +148,7 @@ def end_to_end(reps, emit, S=512, new=128):
         cfg = SimpleNamespace(num_hidden_layers=layers, rms_norm_epsilon=1e-6, max_position_embeddings=2048,
                               rotary_emb_base=10000, llama_mlp_multiple_of=256, **ZIYA)
         t0 = time.perf_counter()
-        model = LlamaForCausalLM(cfg, device="cuda", world_size=1, load_in_8bit=int8)
+        model = LlamaForCausalLM(cfg, device="cuda", world_size=1, load_in_8bit=fmt == "int8", load_in_4bit=fmt == "int4")
         torch.cuda.synchronize()
         build_s = time.perf_counter() - t0
         for B in (1, 8):
@@ -148,7 +171,7 @@ def end_to_end(reps, emit, S=512, new=128):
                 torch.cuda.synchronize()
             dev_us = sum(e.self_device_time_total for e in prof.key_averages())
             w = sorted(wall)[len(wall) // 2]
-            emit(dict(bench="generate_int8", model=f"ziya-llama-13b-L{layers}", weights="int8" if int8 else "bf16", batch=B,
+            emit(dict(bench="generate_weight_only", model=f"ziya-llama-13b-L{layers}", weights=fmt, batch=B,
                       prompt=S, new_tokens=new, reps=reps, tokens_per_s=round(B * new / w, 1),
                       wall_ms_per_token=round(1e3 * w / new, 3), device_ms_per_token=round(dev_us / 1e3 / new, 3),
                       host_calls_per_token=round(ncalls / new, 2),
@@ -164,6 +187,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--skip-40", action="store_true", help="end to end at 8 layers only")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -178,7 +202,7 @@ def main():
     emit(dict(bench="card"))
     kernel_ab(args.reps, emit)
     if not args.skip_e2e:
-        end_to_end(args.reps, emit)
+        end_to_end(args.reps, emit, full=not args.skip_40)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, "bench_int8.jsonl"), "w") as f:
