@@ -145,7 +145,9 @@ class FlatBuffers:
         gradient slots: bucket k of a family writes slot k % slots. The engine reduce-scatters a slot before backward reaches
         the layer that reuses it, so gradients of at most `slots` layers of a family exist at any time — DeepSpeed ZeRO-2's
         "gradients are partitioned as they are produced" (SURVEY.md Appendix D) instead of a full-size buffer. Every grad view
-        handed out so far (prm.main_grad, fused-operand spans) is re-pointed in place. Returns the bytes released."""
+        handed out so far (prm.main_grad, fused-operand spans) is re-pointed in place. A tensor derived from such a view
+        (`.view(-1)`, a slice) is not re-pointed and keeps writing the released buffer, so a model must not keep one across
+        construction: it keeps the view and derives at the point of use. Returns the bytes released."""
         import re
         if self.grads is None:
             return 0

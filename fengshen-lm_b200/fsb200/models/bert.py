@@ -95,7 +95,9 @@ class _BertFamily(FlatModel):
                        for i in range(self.nl)]
         self._bqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.bias", 1, 3 * h).view(-1)
                       for i in range(self.nl)]
-        self._dbqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.bias", 1, 3 * h, grad=True).view(-1)
+        # kept as the [1, 3h] span itself (flattened where it is written): ZeRO-2's compact_grads re-points the gradient
+        # views the flat buffers handed out, not tensors derived from them
+        self._dbqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.bias", 1, 3 * h, grad=True)
                        for i in range(self.nl)]
         if pre:  # NSP classifier padded to 8 outputs (pad logits = -30000 -> zero probability); parameters stay [2, h]
             self._nsp_w = torch.zeros(8, h, dtype=torch.bfloat16, device=dev)
@@ -299,12 +301,12 @@ class _BertFamily(FlatModel):
                       "bert.pooler.dense.bias"):
                 if not acc:
                     P(n).main_grad.zero_()
-        self._done("head")
         if pre:
             ew, eb = P("bert.encoder.ln.weight"), P("bert.encoder.ln.bias")
             dx, dmb = ln_bwd(dhf, xf, ew, eb, stf, D(ph, 3 * self.nl))
         else:
             dx = dhf
+        self._done("head")          # after the final encoder LN: its weight gradient is in the head bucket
         for i in reversed(range(self.nl)):
             p = f"bert.encoder.layer.{i}."
             w1, b1 = P(p + "intermediate.dense.weight"), P(p + "intermediate.dense.bias")
@@ -341,7 +343,7 @@ class _BertFamily(FlatModel):
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
             attn_in = h1 if pre else x
             ops.gemm(L.GEMM_TN, dqkv, attn_in, out=self._dwqkv[i], accumulate=acc)
-            ops.colsum(dqkv, self._dbqkv[i], accumulate=acc)
+            ops.colsum(dqkv, self._dbqkv[i].view(-1), accumulate=acc)
             if pre:
                 dh1 = ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i])
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")
