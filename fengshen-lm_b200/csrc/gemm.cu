@@ -456,6 +456,11 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
               (long)ldb);
   FSB_REQUIRE(d_dtype == FSB_BF16 || d_dtype == FSB_F32, "gemm: bad d_dtype");
   FSB_REQUIRE(ldd % (d_dtype == FSB_F32 ? 4 : 8) == 0, "gemm: ldd=%ld not vector-aligned", (long)ldd);
+  // D and aux leave through TMA stores, which clip a ragged row end only at 16-byte granularity: an N that ends inside a
+  // 16-byte chunk would have the rest of that chunk (columns N.. of the row) overwritten with zeros.
+  FSB_REQUIRE(N % (d_dtype == FSB_F32 && aux == nullptr ? 4 : 8) == 0,
+              "gemm: N=%ld must be a multiple of %d (8 for a bf16 D or aux, 4 for an fp32 D)", (long)N,
+              d_dtype == FSB_F32 && aux == nullptr ? 4 : 8);
   FSB_REQUIRE(epilogue >= 0 && epilogue <= 2, "gemm: bad epilogue %d", epilogue);
   FSB_REQUIRE(aux == nullptr || (aligned16(aux) && ldaux % 8 == 0), "gemm: aux misaligned");
   FSB_REQUIRE(batch == 1 || (stride_a % 8 == 0 && stride_b % 8 == 0 && stride_d % 8 == 0),

@@ -54,7 +54,8 @@ int fsb_num_sms(void);               /* SM count of the current device (132 on H
  * A, B bf16. D bf16 or fp32 (d_dtype). Optional fused epilogue, applied in this order:
  *   acc (+ bias[N]) -> activation -> (+ D_old if accumulate) -> store.
  * bias: fp32 or bf16 vector of length N (bias_dtype), may be NULL.
- * Requirements: pointers 16-byte aligned; lda/ldb/ldd multiples of 8 elements.
+ * Requirements: pointers 16-byte aligned; lda/ldb/ldd multiples of 8 elements; N a multiple of 8 (of 4 for an fp32 D
+ * without aux): D and aux are stored in whole 16-byte chunks, so a row may not end inside one. M and K are free.
  * aux (bf16, may be NULL): receives acc + bias BEFORE the activation (saved for the activation's backward).
  * `batch` > 1 runs independent GEMMs with element strides stride_a/b/d between them (use 1 and 0 otherwise).
  * Kernel selection is internal: persistent 128 x 256 tiles, or 128 x 128 tiles when the wide ones would leave many SMs
