@@ -18,6 +18,7 @@ forward advances by its number of sites, so eager runs and replayed CUDA graphs 
 with both probabilities 0, the forward and backward are the dropout-free kernels.
 """
 import math
+from collections import namedtuple
 from types import SimpleNamespace
 
 import torch
@@ -26,6 +27,9 @@ from .. import lib as L
 from .. import ops
 from ..flat import FlatSpec
 from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd
+from .layers import Linear
+
+_Layer = namedtuple("_Layer", "qkv attn_out inter out")   # attention.self q|k|v, attention.output.dense, intermediate, output
 
 
 class _BertFamily(FlatModel):
@@ -89,17 +93,16 @@ class _BertFamily(FlatModel):
             spec.add("cls.seq_relationship.weight", (2, h), "head"); spec.add("cls.seq_relationship.bias", (2,), "head")
         self._bind_flat(spec, device, world_size)
         dev = self.flat.params.device
-        # fused q|k|v operands
-        self._wqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.weight", 3 * h, h) for i in range(self.nl)]
-        self._dwqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.weight", 3 * h, h, grad=True)
-                       for i in range(self.nl)]
-        self._bqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.bias", 1, 3 * h).view(-1)
-                      for i in range(self.nl)]
-        # kept as the [1, 3h] span itself (flattened where it is written): ZeRO-2's compact_grads re-points the gradient
-        # views the flat buffers handed out, not tensors derived from them
-        self._dbqkv = [self.flat.span(f"bert.encoder.layer.{i}.attention.self.query.bias", 1, 3 * h, grad=True)
-                       for i in range(self.nl)]
-        if pre:  # NSP classifier padded to 8 outputs (pad logits = -30000 -> zero probability); parameters stay [2, h]
+        P = self.P
+        lin = lambda n: Linear.of(P(n + ".weight"), P(n + ".bias"))
+        self._proj = [_Layer(Linear.span(self.flat, p + "attention.self.query.weight", 3 * h, h, p + "attention.self.query.bias"),
+                             lin(p + "attention.output.dense"), lin(p + "intermediate.dense"), lin(p + "output.dense"))
+                      for p in (f"bert.encoder.layer.{i}." for i in range(self.nl))]
+        self._transform = lin("cls.predictions.transform.dense")
+        self._decoder = Linear.of(P(E + "word_embeddings.weight"), P("cls.predictions.bias"))   # tied to the word embeddings
+        if pre:
+            self._pooler = lin("bert.pooler.dense")
+            # NSP classifier padded to 8 outputs (pad logits = -30000 -> zero probability); parameters stay [2, h]
             self._nsp_w = torch.zeros(8, h, dtype=torch.bfloat16, device=dev)
             self._nsp_b = torch.full((8,), -30000.0, dtype=torch.bfloat16, device=dev)
         self.reset_parameters(seed)
@@ -166,7 +169,7 @@ class _BertFamily(FlatModel):
             emb_ctx = (emb, st_e)
         if D(ph, 0) is not None:
             x = ops.dropout(x, D(ph, 0))
-        for i in range(self.nl):
+        for i, pj in enumerate(self._proj):
             p = f"bert.encoder.layer.{i}."
             self._need(f"layer{i}")
             if pre:
@@ -177,11 +180,10 @@ class _BertFamily(FlatModel):
                 attn_in = h1
             else:
                 attn_in = x
-            qkv = ops.gemm(L.GEMM_NT, attn_in, self._wqkv[i], bias=self._bqkv[i])
+            qkv = pj.qkv(attn_in)
             q5 = qkv.view(B, S, 3, nh, hn)
             o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, False, kv_mask=mask, drop=D(pa, 1 + 3 * i))
-            a = ops.gemm(L.GEMM_NT, o.view(T, h), P(p + "attention.output.dense.weight").data,
-                         bias=P(p + "attention.output.dense.bias").data)
+            a = pj.attn_out(o.view(T, h))
             if pre:
                 h2, st2, x1 = ops.layernorm_fwd(a, P(p + "ln.weight").data, P(p + "ln.bias").data, self.eps, residual=x,
                                                 drop=D(ph, 2 + 3 * i))
@@ -190,9 +192,8 @@ class _BertFamily(FlatModel):
                                                 P(p + "attention.output.LayerNorm.bias").data, self.eps, residual=x,
                                                 drop=D(ph, 2 + 3 * i))
             prea = torch.empty((T, self.ff), dtype=torch.bfloat16, device=x.device) if save else None
-            f = ops.gemm(L.GEMM_NT, h2, P(p + "intermediate.dense.weight").data, bias=P(p + "intermediate.dense.bias").data,
-                         epilogue=self.epi, aux=prea)
-            m = ops.gemm(L.GEMM_NT, f, P(p + "output.dense.weight").data, bias=P(p + "output.dense.bias").data)
+            f = pj.inter(h2, epilogue=self.epi, aux=prea)
+            m = pj.out(f)
             if pre:
                 if save:
                     acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, prea, f))
@@ -212,17 +213,15 @@ class _BertFamily(FlatModel):
             hf, stf, xf = x, None, None
         # MLM head: dense + act + LN + tied decoder + bias (on every position)
         tpre = torch.empty((T, h), dtype=torch.bfloat16, device=hf.device) if save else None
-        tf = ops.gemm(L.GEMM_NT, hf, P("cls.predictions.transform.dense.weight").data,
-                      bias=P("cls.predictions.transform.dense.bias").data, epilogue=self.epi, aux=tpre)
+        tf = self._transform(hf, epilogue=self.epi, aux=tpre)
         tn, stt, _ = ops.layernorm_fwd(tf, P("cls.predictions.transform.LayerNorm.weight").data,
                                        P("cls.predictions.transform.LayerNorm.bias").data, self.eps)
-        logits = ops.gemm(L.GEMM_NT, tn, P(E + "word_embeddings.weight").data, bias=P("cls.predictions.bias").data)
+        logits = self._decoder(tn)
         loss, ctx, nsp_logits = None, None, None
         nsp_ctx = None
         if pre:
             first = hf.view(B, S, h)[:, 0, :]                     # strided [B, h] view, row stride S*h
-            ppre = torch.empty((B, h), dtype=torch.bfloat16, device=hf.device)
-            ops.gemm(L.GEMM_NT, first, P("bert.pooler.dense.weight").data, bias=P("bert.pooler.dense.bias").data, out=ppre)
+            ppre = self._pooler(first)
             pooled = ops.act_fwd(L.ACT_TANH, ppre)
             self._nsp_w[:2].copy_(P("cls.seq_relationship.weight").data)
             self._nsp_b[:2].copy_(P("cls.seq_relationship.bias").data)
@@ -268,18 +267,12 @@ class _BertFamily(FlatModel):
             ops.scale_inplace(dlogits, gloss)
             if dnsp is not None:
                 ops.scale_inplace(dnsp, gloss)
-        wte = P(E + "word_embeddings.weight")
-        dtn = ops.gemm(L.GEMM_NN, dlogits, wte.data)
-        ops.gemm(L.GEMM_TN, dlogits, tn, out=wte.main_grad, accumulate=acc)    # tied decoder: written first
-        ops.colsum(dlogits, P("cls.predictions.bias").main_grad, accumulate=acc)
+        dtn = self._decoder.backward(dlogits, tn, acc)     # tied decoder: written first, the embedding adds later
         del dlogits
         lnw, lnb = P("cls.predictions.transform.LayerNorm.weight"), P("cls.predictions.transform.LayerNorm.bias")
         dtf = ops.layernorm_bwd(dtn, tf, lnw.data, stt, lnw.main_grad, lnb.main_grad, accumulate=acc)
         dtpre = ops.act_bwd(self.act, dtf, tpre)
-        tw, tb = P("cls.predictions.transform.dense.weight"), P("cls.predictions.transform.dense.bias")
-        dhf = ops.gemm(L.GEMM_NN, dtpre, tw.data)
-        ops.gemm(L.GEMM_TN, dtpre, hf, out=tw.main_grad, accumulate=acc)
-        ops.colsum(dtpre, tb.main_grad, accumulate=acc)
+        dhf = self._transform.backward(dtpre, hf, acc)
         if pre and dnsp is not None:
             first, ppre, pooled = nsp_ctx
             sw, sb = P("cls.seq_relationship.weight"), P("cls.seq_relationship.bias")
@@ -292,10 +285,7 @@ class _BertFamily(FlatModel):
             else:
                 sw.main_grad.copy_(dw8[:2]); sb.main_grad.copy_(db8[:2])
             dppre = ops.act_bwd(L.ACT_TANH, dpooled, ppre)
-            pw, pb = P("bert.pooler.dense.weight"), P("bert.pooler.dense.bias")
-            ops.gemm(L.GEMM_TN, dppre, first, out=pw.main_grad, accumulate=acc)
-            ops.colsum(dppre, pb.main_grad, accumulate=acc)
-            ops.gemm(L.GEMM_NN, dppre, pw.data, out=dhf.view(B, S, h)[:, 0, :], accumulate=True)   # += into token 0 rows
+            self._pooler.backward(dppre, first, acc, dx=dhf.view(B, S, h)[:, 0, :], dx_accumulate=True)   # += into token 0 rows
         elif pre:
             for n in ("cls.seq_relationship.weight", "cls.seq_relationship.bias", "bert.pooler.dense.weight",
                       "bert.pooler.dense.bias"):
@@ -308,10 +298,7 @@ class _BertFamily(FlatModel):
             dx = dhf
         self._done("head")          # after the final encoder LN: its weight gradient is in the head bucket
         for i in reversed(range(self.nl)):
-            p = f"bert.encoder.layer.{i}."
-            w1, b1 = P(p + "intermediate.dense.weight"), P(p + "intermediate.dense.bias")
-            w2, b2 = P(p + "output.dense.weight"), P(p + "output.dense.bias")
-            wo, bo = P(p + "attention.output.dense.weight"), P(p + "attention.output.dense.bias")
+            p, pj = f"bert.encoder.layer.{i}.", self._proj[i]
             if pre:
                 x, st1, h1, qkv, o, lse, x1, st2, h2, prea, f = acts[i]
                 dm, dres_in = dmb, dx                      # x_next = x1 + drop(m)
@@ -321,37 +308,28 @@ class _BertFamily(FlatModel):
                 dsum, dm = ln_bwd(dx, s2, lw, lb, st3, D(ph, 3 + 3 * i))   # d(h2 + drop(m)), d(m)
                 dres_in = None
             acts[i] = None
-            df = ops.gemm(L.GEMM_NN, dm, w2.data)
-            ops.gemm(L.GEMM_TN, dm, f, out=w2.main_grad, accumulate=acc)
-            ops.colsum(dm, b2.main_grad, accumulate=acc)
-            dprea = ops.act_bwd_bias(self.act, df, prea, b1.main_grad, accumulate=acc)   # dGELU + intermediate.dense bias grad
-            ops.gemm(L.GEMM_TN, dprea, h2, out=w1.main_grad, accumulate=acc)
+            df = pj.out.backward(dm, f, acc)
+            dprea = ops.act_bwd_bias(self.act, df, prea, pj.inter.bias_grad, accumulate=acc)   # dGELU + its bias grad
             if pre:
-                dh2 = ops.gemm(L.GEMM_NN, dprea, w1.data)
+                dh2 = pj.inter.backward(dprea, h2, acc, colsum=False)
                 lw, lb = P(p + "ln.weight"), P(p + "ln.bias")
                 dx1, da = ln_bwd(dh2, x1, lw, lb, st2, D(ph, 2 + 3 * i), dres=dres_in)
             else:
-                ops.gemm(L.GEMM_NN, dprea, w1.data, out=dsum, accumulate=True)    # dh2 = d(h2+m) + dgrad(fc1)
+                pj.inter.backward(dprea, h2, acc, dx=dsum, dx_accumulate=True, colsum=False)   # dh2 = d(h2+m) + dgrad(fc1)
                 lw, lb = P(p + "attention.output.LayerNorm.weight"), P(p + "attention.output.LayerNorm.bias")
                 dsum, da = ln_bwd(dsum, x1, lw, lb, st2, D(ph, 2 + 3 * i))       # d(x + drop(a)), d(a)
-            do = ops.gemm(L.GEMM_NN, da, wo.data)
-            ops.gemm(L.GEMM_TN, da, o.view(T, h), out=wo.main_grad, accumulate=acc)
-            ops.colsum(da, bo.main_grad, accumulate=acc)
+            do = pj.attn_out.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, False,
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
-            attn_in = h1 if pre else x
-            ops.gemm(L.GEMM_TN, dqkv, attn_in, out=self._dwqkv[i], accumulate=acc)
-            ops.colsum(dqkv, self._dbqkv[i].view(-1), accumulate=acc)
             if pre:
-                dh1 = ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i])
+                dh1 = pj.qkv.backward(dqkv, h1, acc)
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")
                 # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped FFN output into x
                 dx, dmb = ln_bwd(dh1, x, lw, lb, st1, D(ph, 3 * i) if i > 0 else None, dres=dx1)
             else:
-                ops.gemm(L.GEMM_NN, dqkv, self._wqkv[i], out=dsum, accumulate=True)  # dx_in = d(x+a) + dgrad(qkv)
-                dx = dsum
+                dx = pj.qkv.backward(dqkv, x, acc, dx=dsum, dx_accumulate=True)   # dx_in = d(x+a) + dgrad(qkv)
             self._done(f"layer{i}")
         if D(ph, 0) is not None:
             dx = ops.dropout(dx, D(ph, 0))
@@ -359,7 +337,7 @@ class _BertFamily(FlatModel):
             emb, st_e = emb_ctx
             lw, lb = P(E + "LayerNorm.weight"), P(E + "LayerNorm.bias")
             dx = ops.layernorm_bwd(dx, emb, lw.data, st_e, lw.main_grad, lb.main_grad, accumulate=acc)
-        ops.embedding_bwd(ids, dx, wte.main_grad)           # adds onto the tied decoder's weight gradient
+        ops.embedding_bwd(ids, dx, P(E + "word_embeddings.weight").main_grad)   # adds onto the tied decoder's weight gradient
         learned_pos_emb_bwd(pos, dx, P(E + "position_embeddings.weight").main_grad, B, S, acc)
         wtt = P(E + "token_type_embeddings.weight")
         # token types: dT = onehot(tt)^T dx as a (tiny-M) GEMM; all-zero types reduce to a column sum

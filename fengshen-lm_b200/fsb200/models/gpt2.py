@@ -9,6 +9,7 @@ Conv1D's [in, out] layout maps onto the GEMM layouts without any transpose: forw
 Dropout probabilities must be 0 (parity / benchmark setting, SURVEY.md §8d); a non-zero value is rejected loudly.
 """
 import math
+from collections import namedtuple
 from types import SimpleNamespace
 
 import torch
@@ -19,6 +20,9 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd
+from .layers import Linear
+
+_Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
 
 
 class GPT2LMHeadModel(FlatModel):
@@ -56,6 +60,10 @@ class GPT2LMHeadModel(FlatModel):
         self._bind_flat(spec, device, world_size)
         self.lm_head = _Holder()
         self.lm_head.weight = self.transformer.wte.weight  # tied (modeling_gpt2.py:646)
+        self._head = Linear.of(self.lm_head.weight)
+        conv1d = lambda m: Linear.of(m.weight, m.bias, conv1d=True)
+        self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
+                      for b in self.transformer.h]
         self.reset_parameters(seed)
 
     @torch.no_grad()
@@ -88,7 +96,7 @@ class GPT2LMHeadModel(FlatModel):
         acts = [] if save else None
         hf, stf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale,
                                                                              True, kv_mask=mask), acts)
-        logits = ops.gemm(L.GEMM_NT, hf, self.transformer.wte.weight.data)
+        logits = self._head(hf)
         loss, ctx = None, None
         if lab is not None:
             keep = logits.clone() if (want_logits and save) else None
@@ -108,18 +116,17 @@ class GPT2LMHeadModel(FlatModel):
         self._need("no_decay"); self._need("wte")
         x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
         prev_m = None
-        for i, blk in enumerate(tr.h):
+        for i, (blk, pj) in enumerate(zip(tr.h, self._proj)):
             self._need(f"layer{i}")
             h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
                                            self.eps, residual=None if prev_m is None else x)
-            qkv = ops.gemm(L.GEMM_NN, h1, blk.attn.c_attn.weight.data, bias=blk.attn.c_attn.bias.data)
+            qkv = pj.c_attn(h1)
             o, lse = attend(i, qkv.view(B, S, 3, nh, hn))
-            a = ops.gemm(L.GEMM_NN, o.view(B * S, h), blk.attn.c_proj.weight.data, bias=blk.attn.c_proj.bias.data)
+            a = pj.attn_proj(o.view(B * S, h))
             h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
             pre = None if acts is None else torch.empty((B * S, self.inner), dtype=torch.bfloat16, device=x.device)
-            f = ops.gemm(L.GEMM_NN, h2, blk.mlp.c_fc.weight.data, bias=blk.mlp.c_fc.bias.data,
-                         epilogue=L.EPI_GELU_TANH, aux=pre)
-            m = ops.gemm(L.GEMM_NN, f, blk.mlp.c_proj.weight.data, bias=blk.mlp.c_proj.bias.data)
+            f = pj.c_fc(h2, epilogue=L.EPI_GELU_TANH, aux=pre)
+            m = pj.mlp_proj(f)
             if acts is not None:
                 acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f))
             # free this block's temporaries before the next block allocates its own (the peak of a long prompt's prefill)
@@ -190,7 +197,7 @@ class GPT2LMHeadModel(FlatModel):
     def _last_logits(self, ids, pos, B, S, attend):
         """fp32 logits [B, V] of the last position of every sequence."""
         hf, _, _ = self._stack(ids, pos, B, S, attend)
-        return ops.gemm(L.GEMM_NT, hf.view(B, S, self.h)[:, -1].contiguous(), self.transformer.wte.weight.data).float()
+        return self._head(hf.view(B, S, self.h)[:, -1].contiguous()).float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
@@ -203,42 +210,29 @@ class GPT2LMHeadModel(FlatModel):
         scale = 1.0 / math.sqrt(hn)
         if gloss is not None:
             ops.scale_inplace(dlogits, gloss)  # upstream scalar; the kernel exits immediately when it is 1.0
-        wte = tr.wte.weight
-        dhf = ops.gemm(L.GEMM_NN, dlogits, wte.data)
-        ops.gemm(L.GEMM_TN, dlogits, hf, out=wte.main_grad, accumulate=acc)   # tied head: written first, embedding adds later
+        dhf = self._head.backward(dlogits, hf, acc)   # tied head: written first, the embedding adds later
         del dlogits
         dx = ops.layernorm_bwd(dhf, xf, tr.ln_f.weight.data, stf, tr.ln_f.weight.main_grad, tr.ln_f.bias.main_grad,
                                accumulate=acc)
         for i in reversed(range(self.nl)):
-            blk = tr.h[i]
+            blk, pj = tr.h[i], self._proj[i]
             x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f = acts[i]
             acts[i] = None
-            w = blk.mlp.c_proj
-            df = ops.gemm(L.GEMM_NT, dx, w.weight.data)
-            ops.gemm(L.GEMM_TN, f, dx, out=w.weight.main_grad, accumulate=acc)
-            ops.colsum(dx, w.bias.main_grad, accumulate=acc)
-            w = blk.mlp.c_fc
-            dpre = ops.act_bwd_bias(L.ACT_GELU_TANH, df, pre, w.bias.main_grad, accumulate=acc)   # dGELU + c_fc bias grad
-            dh2 = ops.gemm(L.GEMM_NT, dpre, w.weight.data)
-            ops.gemm(L.GEMM_TN, h2, dpre, out=w.weight.main_grad, accumulate=acc)
+            df = pj.mlp_proj.backward(dx, f, acc)
+            dpre = ops.act_bwd_bias(L.ACT_GELU_TANH, df, pre, pj.c_fc.bias_grad, accumulate=acc)   # dGELU + c_fc bias grad
+            dh2 = pj.c_fc.backward(dpre, h2, acc, colsum=False)
             dx1 = ops.layernorm_bwd(dh2, x1, blk.ln_2.weight.data, st2, blk.ln_2.weight.main_grad,
                                     blk.ln_2.bias.main_grad, accumulate=acc, dres=dx)
-            w = blk.attn.c_proj
-            do = ops.gemm(L.GEMM_NT, dx1, w.weight.data)
-            ops.gemm(L.GEMM_TN, o.view(T, h), dx1, out=w.weight.main_grad, accumulate=acc)
-            ops.colsum(dx1, w.bias.main_grad, accumulate=acc)
+            do = pj.attn_proj.backward(dx1, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask)
-            w = blk.attn.c_attn
-            dh1 = ops.gemm(L.GEMM_NT, dqkv, w.weight.data)
-            ops.gemm(L.GEMM_TN, h1, dqkv, out=w.weight.main_grad, accumulate=acc)
-            ops.colsum(dqkv, w.bias.main_grad, accumulate=acc)
+            dh1 = pj.c_attn.backward(dqkv, h1, acc)
             dx = ops.layernorm_bwd(dh1, x, blk.ln_1.weight.data, st1, blk.ln_1.weight.main_grad,
                                    blk.ln_1.bias.main_grad, accumulate=acc, dres=dx1)
             self._done(f"layer{i}")
-        ops.embedding_bwd(ids, dx, wte.main_grad)  # accumulates onto the LM-head wgrad (tied weights)
+        ops.embedding_bwd(ids, dx, tr.wte.weight.main_grad)  # accumulates onto the LM-head wgrad (tied weights)
         learned_pos_emb_bwd(pos, dx, tr.wpe.weight.main_grad, B, S, acc)
         self._done("wte")
         self._done("no_decay")

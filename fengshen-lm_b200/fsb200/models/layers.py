@@ -1,0 +1,73 @@
+"""The linear maps and the gated MLP the fsb200 models share: forward and hand-written backward over views into the flat
+buffers (fsb200/flat.py)."""
+import torch
+
+from .. import lib as L
+from .. import ops
+
+
+class Linear:
+    """One linear map of a model: the weight (one parameter, or a fused span of adjacent ones such as q|k|v or w1|w3), its
+    gradient view exactly as the flat buffers handed it out, and optionally a bias and its gradient view. ZeRO-2's compaction
+    re-points those views in place, not tensors derived from them (`.view(-1)`, a slice), so none is kept here.
+    An HF `Linear` weight is [out, in] (forward NT, dgrad NN, wgrad TN(dy, x)); a GPT-2 `Conv1D` weight (conv1d=True) is
+    [in, out] (forward NN, dgrad NT, wgrad TN(x, dy))."""
+
+    def __init__(self, weight, weight_grad=None, bias=None, bias_grad=None, conv1d=False):
+        self.weight, self.weight_grad, self.bias, self.bias_grad = weight, weight_grad, bias, bias_grad
+        self.conv1d = conv1d
+
+    @classmethod
+    def of(cls, weight, bias=None, conv1d=False):
+        """Over parameters bound to the flat buffers (.main_grad, if any, is the gradient view)."""
+        grad = lambda p: getattr(p, "main_grad", None)
+        return cls(weight.data, grad(weight), None if bias is None else bias.data, None if bias is None else grad(bias), conv1d)
+
+    @classmethod
+    def span(cls, flat, first, rows, cols, first_bias=None):
+        """The [rows, cols] weight starting at parameter `first` and covering the adjacent ones after it; first_bias: the same
+        for the bias, a [1, rows] span (the kernels read its `rows` contiguous elements)."""
+        return cls(flat.span(first, rows, cols), flat.span(first, rows, cols, grad=True),
+                   None if first_bias is None else flat.span(first_bias, 1, rows),
+                   None if first_bias is None else flat.span(first_bias, 1, rows, grad=True))
+
+    def __call__(self, x, epilogue=L.EPI_NONE, aux=None):
+        return ops.gemm(L.GEMM_NN if self.conv1d else L.GEMM_NT, x, self.weight, bias=self.bias, epilogue=epilogue, aux=aux)
+
+    def backward(self, dy, x, accumulate, dx=None, dx_accumulate=False, colsum=True):
+        """-> the gradient of the input x, given dy, the gradient of the output. Writes the weight's gradient (and the bias's)
+        into the flat gradient buffer, adding to it when `accumulate`. dx: write the input gradient into this buffer instead,
+        adding to it when dx_accumulate. colsum=False: the bias gradient is already written (ops.act_bwd_bias)."""
+        if self.conv1d:
+            dx = ops.gemm(L.GEMM_NT, dy, self.weight, out=dx, accumulate=dx_accumulate)
+            ops.gemm(L.GEMM_TN, x, dy, out=self.weight_grad, accumulate=accumulate)
+        else:
+            dx = ops.gemm(L.GEMM_NN, dy, self.weight, out=dx, accumulate=dx_accumulate)
+            ops.gemm(L.GEMM_TN, dy, x, out=self.weight_grad, accumulate=accumulate)
+        if self.bias is not None and colsum:
+            ops.colsum(dy, self.bias_grad, accumulate=accumulate)
+        return dx
+
+
+class GatedMLP:
+    """m = wo(act(gate) * up) with [gate | up] = wi(h): wi is one projection over the adjacent gate and up weights, `act` the
+    gate's activation (L.ACT_SILU for LLaMA, L.ACT_GELU_TANH for mT5)."""
+
+    def __init__(self, wi, wo, act):
+        self.wi, self.wo, self.act = wi, wo, act
+
+    def __call__(self, h):
+        """-> (m, what the backward reads)."""
+        gu = self.wi(h)
+        f = gu.shape[1] // 2
+        act = ops.glu_fwd(self.act, gu[:, :f], gu[:, f:])
+        return self.wo(act), (gu, act)
+
+    def backward(self, dm, h, saved, accumulate):
+        """-> the gradient of h; writes the weight gradients as Linear.backward does."""
+        gu, act = saved
+        f = gu.shape[1] // 2
+        dact = self.wo.backward(dm, act, accumulate)
+        dgu = torch.empty_like(gu)
+        ops.glu_bwd(self.act, dact, gu[:, :f], gu[:, f:], dgu[:, :f], dgu[:, f:])
+        return self.wi.backward(dgu, h, accumulate)

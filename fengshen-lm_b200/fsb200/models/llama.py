@@ -14,6 +14,7 @@ The causal mask is implicit (flash path semantics, transformer.py:441-448: `atte
 the `global` path when the mask is all ones — SURVEY.md Appendix B).
 """
 import math
+from collections import namedtuple
 from types import SimpleNamespace
 
 import torch
@@ -24,6 +25,7 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids
+from .layers import GatedMLP, Linear
 
 
 def llama_ff_dim(hidden_size, multiple_of=256):
@@ -35,18 +37,34 @@ def _init_normal_(t, std, gen):
     t.copy_(torch.empty(t.shape, dtype=torch.float32).normal_(0.0, std, generator=gen).to(t.dtype))
 
 
-_W8_NAMES = ("attention.query_key_value.weight", "attention.dense.weight", "mlp.w1.weight", "mlp.w3.weight", "mlp.w2.weight")
-
-# weight format -> (quantiser, GEMM, (q dtype, q shape, s dtype, s shape) of an [n, k] weight)
+# weight format -> (quantiser, (q dtype, q shape, s dtype, s shape) of an [n, k] weight)
 _WQ = {
-    "int8": (ops.quantize_w8, ops.gemm_w8a16, lambda n, k: (torch.int8, (n, k), torch.float32, (n,))),
-    "int4": (ops.quantize_w4, ops.gemm_w4a16, lambda n, k: (torch.uint8, (n // 2, k), torch.bfloat16, (n, k // 128))),
+    "int8": (ops.quantize_w8, lambda n, k: (torch.int8, (n, k), torch.float32, (n,))),
+    "int4": (ops.quantize_w4, lambda n, k: (torch.uint8, (n // 2, k), torch.bfloat16, (n, k // 128))),
 }
+
+_Layer = namedtuple("_Layer", "qkv dense mlp")   # a layer's projections: query_key_value, dense, the gated MLP (w1 | w3, w2)
 
 
 def _quantized_unsupported(fmt, what):
     return NotImplementedError(f"fsb200 LlamaForCausalLM: {what} is not implemented for an {fmt} (load_in_{fmt[3:]}bit=True) "
                                "model; it only runs inference")
+
+
+class QuantizedLinear:
+    """A layer projection of an int8 / int4 model, with Linear's call surface: the [n, k] weight held as q + scales s in the
+    format's layout (_WQ) and run through the W8A16 / W4A16 GEMM. Inference only: its backward raises."""
+
+    def __init__(self, fmt, n, k, device):
+        qd, qs, sd, ss = _WQ[fmt][1](n, k)
+        self.fmt = fmt
+        self.q, self.s = torch.zeros(qs, dtype=qd, device=device), torch.zeros(ss, dtype=sd, device=device)
+
+    def __call__(self, x):
+        return (ops.gemm_w8a16 if self.fmt == "int8" else ops.gemm_w4a16)(x, self.q, self.s)
+
+    def backward(self, *_, **__):
+        raise _quantized_unsupported(self.fmt, "backward")
 
 
 class LlamaForCausalLM(FlatModel):
@@ -115,22 +133,16 @@ class LlamaForCausalLM(FlatModel):
         spec.add("llama.final_layer_norm.scale", (h,), "head")
         spec.add("embed_out.final_linear.weight", (self.V_l, h), "head")
         self._bind_flat(spec, device, world_size, tp=self.tp, grads=not quantized)
-        if quantized:
-            # per layer {projection: (q, s)} in the format's layout (_WQ); w1 | w3 is one [2ff, h] operand as in the bf16
-            # layout. The int8 model keeps them in self._w8, the int4 one in self._w4; self._wq is the model's own.
-            dev = self.flat.params.device
-            shapes = {"qkv": (3 * h, h), "dense": (h, h), "w13": (2 * self.ff, h), "w2": (h, self.ff)}
-            layout = _WQ[self.weight_format][2]
-
-            def zeros(n, k):
-                qd, qs, sd, ss = layout(n, k)
-                return torch.zeros(qs, dtype=qd, device=dev), torch.zeros(ss, dtype=sd, device=dev)
-            self._wq = [{key: zeros(*n_k) for key, n_k in shapes.items()} for _ in range(nl)]
-            setattr(self, "_w8" if self.load_in_8bit else "_w4", self._wq)
+        if quantized:   # w1 | w3 is one [2ff, h] operand as in the bf16 layout
+            qlin = lambda n, k: QuantizedLinear(self.weight_format, n, k, self.flat.params.device)
+            self._proj = [_Layer(qlin(3 * h, h), qlin(h, h), GatedMLP(qlin(2 * self.ff, h), qlin(h, self.ff), L.ACT_SILU))
+                          for _ in range(nl)]
         else:
-            self._w13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h)
-                         for i in range(nl)]
-            self._dw13 = [self.flat.span(f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h, grad=True) for i in range(nl)]
+            self._proj = [_Layer(Linear.of(lyr.attention.query_key_value.weight), Linear.of(lyr.attention.dense.weight),
+                                 GatedMLP(Linear.span(self.flat, f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h),
+                                          Linear.of(lyr.mlp.w2.weight), L.ACT_SILU))
+                          for i, lyr in enumerate(self.llama.layers)]
+        self._head = Linear.of(self.embed_out.final_linear.weight)
 
         # RoPE tables exactly as RotaryEmbedding builds them (layers/positional_embeddings.py:38-52), fp32; inv_freq is also a
         # buffer of every layer in the reference's module tree (modeling_llama.py:97-127), hence in its state dict
@@ -179,13 +191,10 @@ class LlamaForCausalLM(FlatModel):
                 for key, (q, s) in wq.items():
                     tmp = torch.empty(self._weight_shape(q, s), dtype=torch.bfloat16, device=q.device)
                     tmp.normal_(0.0, wang if key in ("dense", "w2") else small, generator=dgen)
-                    self._quantize(tmp, q, s)
+                    _WQ[self.weight_format][0](tmp, q, s)
                     del tmp
 
     # ---- int8 / int4 (load_in_8bit / load_in_4bit) ---------------------------------------------------------------------
-    def _quantize(self, w, q, s):
-        _WQ[self.weight_format][0](w, q, s)
-
     @staticmethod
     def _weight_shape(q, s):
         """[n, k] of the bf16 weight that (q, s) holds: s has one row per weight row in both formats, q the k columns."""
@@ -202,18 +211,27 @@ class LlamaForCausalLM(FlatModel):
             raise KeyError(f"missing key in state dict: {sorted(missing)[0]}")
         self._load_quantized_shard(sd, set())
 
+    @property
+    def _wq(self):
+        """Per layer {projection: (q, s)} of an int8 / int4 model (w13: the w1 | w3 operand), as `_w8` / `_w4` name them."""
+        return [{"qkv": (lp.qkv.q, lp.qkv.s), "dense": (lp.dense.q, lp.dense.s), "w13": (lp.mlp.wi.q, lp.mlp.wi.s),
+                 "w2": (lp.mlp.wo.q, lp.mlp.wo.s)} for lp in self._proj]
+    _w8 = _w4 = _wq
+
+    @property
+    def _w13(self):
+        """Per layer the [2ff, h] w1 | w3 operand of a bf16 model."""
+        return [lp.mlp.wi.weight for lp in self._proj]
+
     def _wq_targets(self):
-        """{state-dict key: (q, s) row slice it quantises into} of every quantised projection."""
+        """{state-dict key: (q, s) it quantises into} of every quantised projection. w1 and w3 are the upper and lower
+        halves of the w1 | w3 projection, in q (whose int4 rows pack two weight rows) as in s."""
         out = {}
-        for i, wq in enumerate(self._wq):
+        for i, (qkv, dense, mlp) in enumerate(self._proj):
             p = f"llama.layers.{i}."
-            (qq, sq), (qd, sd_), (q13, s13), (q2, s2) = wq["qkv"], wq["dense"], wq["w13"], wq["w2"]
-            hq, hs = q13.shape[0] // 2, s13.shape[0] // 2     # w1 is the upper half of the [2ff, h] operand, w3 the lower
-            out[p + _W8_NAMES[0]] = (qq, sq)
-            out[p + _W8_NAMES[1]] = (qd, sd_)
-            out[p + _W8_NAMES[2]] = (q13[:hq], s13[:hs])
-            out[p + _W8_NAMES[3]] = (q13[hq:], s13[hs:])
-            out[p + _W8_NAMES[4]] = (q2, s2)
+            (q1, q3), (s1, s3) = mlp.wi.q.chunk(2), mlp.wi.s.chunk(2)
+            out.update({p + "attention.query_key_value.weight": (qkv.q, qkv.s), p + "attention.dense.weight": (dense.q, dense.s),
+                        p + "mlp.w1.weight": (q1, s1), p + "mlp.w3.weight": (q3, s3), p + "mlp.w2.weight": (mlp.wo.q, mlp.wo.s)})
         return out
 
     @torch.no_grad()
@@ -233,7 +251,7 @@ class LlamaForCausalLM(FlatModel):
             elif k in targets:
                 q, s = targets[k]
                 tmp = v.to(q.device).contiguous()
-                self._quantize(tmp, q, s)
+                _WQ[self.weight_format][0](tmp, q, s)
                 del tmp
             else:
                 continue
@@ -246,7 +264,7 @@ class LlamaForCausalLM(FlatModel):
         n = self.flat.params.numel() * self.flat.params.element_size()
         if self.flat.grads is not None:
             n += self.flat.grads.numel() * self.flat.grads.element_size()
-        for wq in getattr(self, "_wq", ()):
+        for wq in self._wq if self.weight_format != "bf16" else ():
             n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in wq.values())
         return n + sum(b.numel() * b.element_size() for b in self.buffers())
 
@@ -254,23 +272,6 @@ class LlamaForCausalLM(FlatModel):
         if self.weight_format != "bf16":
             raise _quantized_unsupported(self.weight_format, f"save_pretrained ({self.weight_format} export)")
         return super().save_pretrained(path, **kw)
-
-    def _linear(self, i, name, x):
-        """x @ W^T for layer i's projection `name` (qkv, dense, w13, w2): the bf16 GEMM, or the W8A16 / W4A16 GEMM of an
-        int8 / int4 model."""
-        if self.weight_format != "bf16":
-            q, s = self._wq[i][name]
-            return _WQ[self.weight_format][1](x, q, s)
-        lyr = self.llama.layers[i]
-        if name == "qkv":
-            w = lyr.attention.query_key_value.weight.data
-        elif name == "dense":
-            w = lyr.attention.dense.weight.data
-        elif name == "w13":
-            w = self._w13[i]
-        else:
-            w = lyr.mlp.w2.weight.data
-        return ops.gemm(L.GEMM_NT, x, w)
 
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, labels=None, return_logits=False, **_):
@@ -304,7 +305,7 @@ class LlamaForCausalLM(FlatModel):
         acts = [] if save else None
         hf, rstdf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2],
                                                                                scale, True), acts)
-        logits = ops.gemm(L.GEMM_NT, hf, self.embed_out.final_linear.weight.data)
+        logits = self._head(hf)
         logits = self._tp_gather_columns(logits)   # ParallelLinear(parallel_output=False): full-vocabulary logits on every rank
         loss = None
         ctx = None
@@ -321,7 +322,7 @@ class LlamaForCausalLM(FlatModel):
         """Embedding, the layers and the final norm over ids [B * S] -> (hidden states, their rstd, residual stream).
         attend(i, q5) is layer i's attention over the per-head interleaved q|k|v view [B, S, heads, 3, head_dim] (rotary
         embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads."""
-        nh, hn, ff, hl = self.nh_l, self.hn, self.ff_l, self.h_l      # LOCAL heads / ff columns under tensor parallelism
+        nh, hn, hl = self.nh_l, self.hn, self.h_l      # LOCAL heads under tensor parallelism
         self._need("no_decay"); self._need("embed_in")
         ids_l, emb_keep = self._local_ids(ids)
         x = ops.embedding_fwd(ids_l, self.llama.embed_in.word_embeddings.weight.data)
@@ -329,25 +330,23 @@ class LlamaForCausalLM(FlatModel):
             x.mul_(emb_keep)
             self._tp_all_reduce(x)
         prev_m = None
-        for i, lyr in enumerate(self.llama.layers):
+        for i, (lyr, lp) in enumerate(zip(self.llama.layers, self._proj)):
             self._need(f"layer{i}")
             h1, rstd1, x = ops.rmsnorm_fwd(x if prev_m is None else prev_m, lyr.input_layernorm.scale.data, self.eps,
                                            residual=None if prev_m is None else x)
-            qkv = self._linear(i, "qkv", h1)
+            qkv = lp.qkv(h1)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
             o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
-            a = self._linear(i, "dense", o.view(B * S, hl))
+            a = lp.dense(o.view(B * S, hl))
             self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
             h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
-            gu = self._linear(i, "w13", h2)
-            act = ops.glu_fwd(L.ACT_SILU, gu[:, :ff], gu[:, ff:])
-            m = self._linear(i, "w2", act)
+            m, ms = lp.mlp(h2)
             self._tp_all_reduce(m)        # RowParallelLinear (w2)
             if acts is not None:
-                acts.append((x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, gu, act))
+                acts.append((x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, ms))
             # free this layer's temporaries before the next layer allocates its own (the peak of a long prompt's prefill)
-            del rstd1, h1, qkv, o, lse, a, rstd2, h2, gu, act
+            del rstd1, h1, qkv, o, lse, a, rstd2, h2, ms
             x, prev_m = x1, m
         self._need("head")
         return ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
@@ -441,13 +440,12 @@ class LlamaForCausalLM(FlatModel):
             pad = torch.zeros((rows, self.h), dtype=last.dtype, device=last.device)
             pad[:B] = last
             last = pad
-        return ops.gemm(L.GEMM_NT, last, self.embed_out.final_linear.weight.data)[:B].float()
+        return self._head(last)[:B].float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
         acts, hf, rstdf, xf, dlogits, ids, pos, B, S = ctx
-        h, nh, hn, ff = self.h, self.nh_l, self.hn, self.ff_l
-        hl = self.h_l
+        nh, hn, hl = self.nh_l, self.hn, self.h_l
         T = B * S
         acc = self.accumulate_grads
         self._begin_backward()
@@ -455,43 +453,31 @@ class LlamaForCausalLM(FlatModel):
             ops.scale_inplace(dlogits, gloss)  # upstream scalar; the kernel exits immediately when it is 1.0
         if self.tp > 1:   # this rank's vocabulary columns of dlogits (a strided view: the GEMMs take the row stride)
             dlogits = dlogits[:, self.tp_rank * self.V_l:(self.tp_rank + 1) * self.V_l]
-        W_out = self.embed_out.final_linear.weight
-        dhf = ops.gemm(L.GEMM_NN, dlogits, W_out.data)
+        dhf = self._head.backward(dlogits, hf, acc)
         self._tp_all_reduce(dhf)          # backward of copy_to_model_parallel_region (mpu/mappings.py): sum the partial dgrads
-        ops.gemm(L.GEMM_TN, dlogits, hf, out=W_out.main_grad, accumulate=acc)
         del dlogits
         self._done("head")
         fscale = self.llama.final_layer_norm.scale
         dx = ops.rmsnorm_bwd(dhf, xf, fscale.data, rstdf, fscale.main_grad, accumulate=acc)
         for i in reversed(range(self.nl)):
-            lyr = self.llama.layers[i]
-            x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, gu, act = acts[i]
+            lyr, lp = self.llama.layers[i], self._proj[i]
+            x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, ms = acts[i]
             acts[i] = None
             # x_next = x1 + m  ->  dm = dx, residual gradient into x1 = dx
-            w2 = lyr.mlp.w2.weight
-            dact = ops.gemm(L.GEMM_NN, dx, w2.data)
-            ops.gemm(L.GEMM_TN, dx, act, out=w2.main_grad, accumulate=acc)
-            dgu = torch.empty_like(gu)
-            ops.glu_bwd(L.ACT_SILU, dact, gu[:, :ff], gu[:, ff:], dgu[:, :ff], dgu[:, ff:])
-            dh2 = ops.gemm(L.GEMM_NN, dgu, self._w13[i])
+            dh2 = lp.mlp.backward(dx, h2, ms, acc)
             self._tp_all_reduce(dh2)      # column-parallel w1|w3: dgrad partial sums
-            ops.gemm(L.GEMM_TN, dgu, h2, out=self._dw13[i], accumulate=acc)
             s2 = lyr.post_attention_layernorm.scale
             dx1 = ops.rmsnorm_bwd(dh2, x1, s2.data, rstd2, s2.main_grad, accumulate=acc, dres=dx)
             # x1 = x + a  ->  da = dx1
-            wd = lyr.attention.dense.weight
-            do = ops.gemm(L.GEMM_NN, dx1, wd.data)
-            ops.gemm(L.GEMM_TN, dx1, o.view(T, hl), out=wd.main_grad, accumulate=acc)
+            do = lp.dense.backward(dx1, o.view(T, hl), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, nh, 3, hn), dqkv.view(B, S, nh, 3, hn)
             ops.sdpa_bwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o, do.view(B, S, nh, hn), lse,
                          1.0 / math.sqrt(hn), True, d5[:, :, :, 0], d5[:, :, :, 1], d5[:, :, :, 2])
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=0)
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=hn)
-            wq = lyr.attention.query_key_value.weight
-            dh1 = ops.gemm(L.GEMM_NN, dqkv, wq.data)
+            dh1 = lp.qkv.backward(dqkv, h1, acc)
             self._tp_all_reduce(dh1)      # column-parallel QKV: dgrad partial sums
-            ops.gemm(L.GEMM_TN, dqkv, h1, out=wq.main_grad, accumulate=acc)
             s1 = lyr.input_layernorm.scale
             dx = ops.rmsnorm_bwd(dh1, x, s1.data, rstd1, s1.main_grad, accumulate=acc, dres=dx1)
             self._done(f"layer{i}")

@@ -21,6 +21,7 @@ every decoder layer's K|V-projection dgrad: accumulated in fp32 by the GEMM epil
 Dropout must be 0 (parity / benchmark setting, SURVEY.md §8d); a non-zero value is rejected loudly.
 """
 import math
+from collections import namedtuple
 from types import SimpleNamespace
 
 import torch
@@ -32,6 +33,10 @@ from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from . import t5_bias as TB
 from .base import FlatModel, _Holder, flat_ids, key_mask
+from .layers import GatedMLP, Linear
+
+_Enc = namedtuple("_Enc", "qkv o mlp")             # a layer's projections: self-attention q|k|v and o, the gated FFN
+_Dec = namedtuple("_Dec", "qkv o cq ckv co mlp")   # ... and between them cross-attention q, k|v and o
 
 
 class MT5ForConditionalGeneration(FlatModel):
@@ -102,19 +107,15 @@ class MT5ForConditionalGeneration(FlatModel):
         if self.tied:
             self.lm_head = _Holder()
             self.lm_head.weight = self._p["shared.weight"]      # same Parameter object: named_parameters() lists it once
-        self._head = "shared.weight" if self.tied else "lm_head.weight"
-        fl = self.flat
-        E, D = "encoder.block.{}.layer.", "decoder.block.{}.layer."
-        self._e_qkv = [fl.span(E.format(i) + "0.SelfAttention.q.weight", 3 * inner, d) for i in range(self.ne)]
-        self._e_dqkv = [fl.span(E.format(i) + "0.SelfAttention.q.weight", 3 * inner, d, grad=True) for i in range(self.ne)]
-        self._e_wi = [fl.span(E.format(i) + "1.DenseReluDense.wi_0.weight", 2 * ff, d) for i in range(self.ne)]
-        self._e_dwi = [fl.span(E.format(i) + "1.DenseReluDense.wi_0.weight", 2 * ff, d, grad=True) for i in range(self.ne)]
-        self._d_qkv = [fl.span(D.format(i) + "0.SelfAttention.q.weight", 3 * inner, d) for i in range(self.nd)]
-        self._d_dqkv = [fl.span(D.format(i) + "0.SelfAttention.q.weight", 3 * inner, d, grad=True) for i in range(self.nd)]
-        self._d_kv = [fl.span(D.format(i) + "1.EncDecAttention.k.weight", 2 * inner, d) for i in range(self.nd)]
-        self._d_dkv = [fl.span(D.format(i) + "1.EncDecAttention.k.weight", 2 * inner, d, grad=True) for i in range(self.nd)]
-        self._d_wi = [fl.span(D.format(i) + "2.DenseReluDense.wi_0.weight", 2 * ff, d) for i in range(self.nd)]
-        self._d_dwi = [fl.span(D.format(i) + "2.DenseReluDense.wi_0.weight", 2 * ff, d, grad=True) for i in range(self.nd)]
+        self._head = Linear.of(self._p["shared.weight" if self.tied else "lm_head.weight"])
+        lin = lambda name: Linear.of(self.P(name + ".weight"))
+        span = lambda first, rows: Linear.span(self.flat, first + ".weight", rows, d)
+        mlp = lambda p: GatedMLP(span(p + "DenseReluDense.wi_0", 2 * ff), lin(p + "DenseReluDense.wo"), L.ACT_GELU_TANH)
+        self._enc = [_Enc(span(p + "0.SelfAttention.q", 3 * inner), lin(p + "0.SelfAttention.o"), mlp(p + "1."))
+                     for p in (f"encoder.block.{i}.layer." for i in range(self.ne))]
+        self._dec = [_Dec(span(p + "0.SelfAttention.q", 3 * inner), lin(p + "0.SelfAttention.o"), lin(p + "1.EncDecAttention.q"),
+                          span(p + "1.EncDecAttention.k", 2 * inner), lin(p + "1.EncDecAttention.o"), mlp(p + "2."))
+                     for p in (f"decoder.block.{i}.layer." for i in range(self.nd))]
 
         self.reset_parameters(seed)
 
@@ -171,25 +172,23 @@ class MT5ForConditionalGeneration(FlatModel):
 
     def _encode(self, ids, mask, B, Se, rel_e, save):
         """Encoder stack over ids [B * Se]; returns (saved activations, final hidden states, their rstd, residual stream)."""
-        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         Te = B * Se
         x, prev = ops.embedding_fwd(ids, P("shared.weight").data), None
         eacts = []
-        for i in range(self.ne):
+        for i, pj in enumerate(self._enc):
             p = f"encoder.block.{i}.layer."
             self._need(f"enc{i}")
             h1, r1, x = self._norm(prev, x, p + "0.layer_norm.weight")
-            qkv = ops.gemm(L.GEMM_NT, h1, self._e_qkv[i])
+            qkv = pj.qkv(h1)
             q5 = qkv.view(B, Se, 3, nh, dk)
             o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, False, kv_mask=mask, rel_bias=rel_e)
-            a = ops.gemm(L.GEMM_NT, o.view(Te, inner), P(p + "0.SelfAttention.o.weight").data)
+            a = pj.o(o.view(Te, inner))
             h2, r2, x1 = self._norm(a, x, p + "1.layer_norm.weight")
-            gu = ops.gemm(L.GEMM_NT, h2, self._e_wi[i])
-            act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
-            m = ops.gemm(L.GEMM_NT, act, P(p + "1.DenseReluDense.wo.weight").data)
+            m, ms = pj.mlp(h2)
             if save:
-                eacts.append((x, r1, h1, qkv, o, lse, x1, r2, h2, gu, act))
+                eacts.append((x, r1, h1, qkv, o, lse, x1, r2, h2, ms))
             x, prev = x1, m
         self._need("head")
         enc_h, rfe, xfe = self._norm(prev, x, "encoder.final_layer_norm.weight")
@@ -200,28 +199,26 @@ class MT5ForConditionalGeneration(FlatModel):
         self-attention over the packed q|k|v view [B, S, 3, heads, d_kv] -> (out, lse); cross_attend(i, qc) its
         cross-attention from the query projection [B * S, inner] -> (out, lse, the encoder's K|V or None); `acts`, when given,
         collects what the backward reads."""
-        nh, dk, inner, ff = self.nh, self.dk, self.inner, self.ff
+        nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         T = B * S
         self._need("no_decay"); self._need("shared")
         y, prev = ops.embedding_fwd(dec_ids, P("shared.weight").data), None
-        for i in range(self.nd):
+        for i, pj in enumerate(self._dec):
             p = f"decoder.block.{i}.layer."
             self._need(f"dec{i}")
             h1, r1, y = self._norm(prev, y, p + "0.layer_norm.weight")
-            qkv = ops.gemm(L.GEMM_NT, h1, self._d_qkv[i])
+            qkv = pj.qkv(h1)
             o, lse = attend(i, qkv.view(B, S, 3, nh, dk))
-            a = ops.gemm(L.GEMM_NT, o.view(T, inner), P(p + "0.SelfAttention.o.weight").data)
+            a = pj.o(o.view(T, inner))
             h2, r2, y1 = self._norm(a, y, p + "1.layer_norm.weight")
-            qc = ops.gemm(L.GEMM_NT, h2, P(p + "1.EncDecAttention.q.weight").data)
+            qc = pj.cq(h2)
             oc, lsec, kvc = cross_attend(i, qc)
-            ac = ops.gemm(L.GEMM_NT, oc.view(T, inner), P(p + "1.EncDecAttention.o.weight").data)
+            ac = pj.co(oc.view(T, inner))
             h3, r3, y2 = self._norm(ac, y1, p + "2.layer_norm.weight")
-            gu = ops.gemm(L.GEMM_NT, h3, self._d_wi[i])
-            act = ops.glu_fwd(L.ACT_GELU_TANH, gu[:, :ff], gu[:, ff:])
-            m = ops.gemm(L.GEMM_NT, act, P(p + "2.DenseReluDense.wo.weight").data)
+            m, ms = pj.mlp(h3)
             if acts is not None:
-                acts.append((y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, gu, act))
+                acts.append((y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms))
             y, prev = y2, m
         self._need("head")
         return self._norm(prev, y, "decoder.final_layer_norm.weight")
@@ -255,7 +252,7 @@ class MT5ForConditionalGeneration(FlatModel):
         cross = []
         for i in range(self.nd):
             self._need(f"dec{i}")
-            kvc = ops.gemm(L.GEMM_NT, enc_h, self._d_kv[i]).view(B, Se, 2, nh, dk)
+            kvc = self._dec[i].ckv(enc_h).view(B, Se, 2, nh, dk)
             cross.append(kvc.repeat_interleave(c.expand, 0) if c.expand > 1 else kvc)
         cmask = None if emask is None else emask.repeat_interleave(c.expand, 0).contiguous()
         cap = (max(c.max_length, 2) + 63) // 64 * 64
@@ -281,7 +278,7 @@ class MT5ForConditionalGeneration(FlatModel):
                 ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len)
                 return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, 1.0, rel_bias=rel_d)
             hf, _, _ = self._decode(tok, R, 1, attend, cross_attend)
-            return ops.gemm(L.GEMM_NT, hf, P(self._head).data).float()
+            return self._head(hf).float()
 
         graphs = DecodeGraphs(self, R, caches, body)
         graphs.tok.copy_(start.view(-1))      # the first step decodes the start token
@@ -299,14 +296,14 @@ class MT5ForConditionalGeneration(FlatModel):
         eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save)
 
         def cross_attend(i, qc):
-            kvc = ops.gemm(L.GEMM_NT, enc_h, self._d_kv[i])
+            kvc = self._dec[i].ckv(enc_h)
             kv5 = kvc.view(B, Se, 2, nh, dk)
             oc, lsec = ops.sdpa_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, False, kv_mask=mask)
             return oc, lsec, kvc
         dacts = [] if save else None
         hf, rfd, xfd = self._decode(dec_ids, B, Sd, lambda i, q5: ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True,
                                                                               rel_bias=rel_d), cross_attend, dacts)
-        logits = ops.gemm(L.GEMM_NT, hf, P(self._head).data)
+        logits = self._head(hf)
         loss, ctx = None, None
         if lab is not None:
             keep = logits.clone() if (want_logits and save) else None
@@ -320,7 +317,7 @@ class MT5ForConditionalGeneration(FlatModel):
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
         eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd = ctx
-        d, nh, dk, inner, ff = self.d, self.nh, self.dk, self.inner, self.ff
+        d, nh, dk, inner = self.d, self.nh, self.dk, self.inner
         P = self.P
         Te, Td = B * Se, B * Sd
         acc = self.accumulate_grads
@@ -328,9 +325,7 @@ class MT5ForConditionalGeneration(FlatModel):
         self._begin_backward()
         if gloss is not None:
             ops.scale_inplace(dlogits, gloss)
-        Wlm = P(self._head)
-        dhf = ops.gemm(L.GEMM_NN, dlogits, Wlm.data)
-        ops.gemm(L.GEMM_TN, dlogits, hf, out=Wlm.main_grad, accumulate=acc)   # tied head: written first, the embeddings add later
+        dhf = self._head.backward(dlogits, hf, acc)   # tied head: written first, the embeddings add later
         del dlogits
         self._done("head")                      # lm_head is the bucket's only decayed parameter (the norms are no-decay)
         fs = P("decoder.final_layer_norm.weight")
@@ -339,44 +334,30 @@ class MT5ForConditionalGeneration(FlatModel):
         drel_d = torch.zeros_like(rel_d)
         denc32 = torch.empty((Te, d), dtype=torch.float32, device=dev)   # sum over decoder layers of the K|V dgrads
         for i in reversed(range(self.nd)):
-            p = f"decoder.block.{i}.layer."
-            y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, gu, act = dacts[i]
+            p, pj = f"decoder.block.{i}.layer.", self._dec[i]
+            y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms = dacts[i]
             dacts[i] = None
-            wo = P(p + "2.DenseReluDense.wo.weight")
-            dact = ops.gemm(L.GEMM_NN, dy, wo.data)
-            ops.gemm(L.GEMM_TN, dy, act, out=wo.main_grad, accumulate=acc)
-            dgu = torch.empty_like(gu)
-            ops.glu_bwd(L.ACT_GELU_TANH, dact, gu[:, :ff], gu[:, ff:], dgu[:, :ff], dgu[:, ff:])
-            dh3 = ops.gemm(L.GEMM_NN, dgu, self._d_wi[i])
-            ops.gemm(L.GEMM_TN, dgu, h3, out=self._d_dwi[i], accumulate=acc)
+            dh3 = pj.mlp.backward(dy, h3, ms, acc)
             s3 = P(p + "2.layer_norm.weight")
             dy2 = ops.rmsnorm_bwd(dh3, y2, s3.data, r3, s3.main_grad, accumulate=acc, dres=dy)
             # cross-attention
-            woc = P(p + "1.EncDecAttention.o.weight")
-            doc = ops.gemm(L.GEMM_NN, dy2, woc.data)
-            ops.gemm(L.GEMM_TN, dy2, oc.view(Td, inner), out=woc.main_grad, accumulate=acc)
+            doc = pj.co.backward(dy2, oc.view(Td, inner), acc)
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             kv5, dkv5 = kvc.view(B, Se, 2, nh, dk), dkvc.view(B, Se, 2, nh, dk)
             ops.sdpa_bwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], oc, doc.view(B, Sd, nh, dk), lsec, 1.0, False,
                          dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1], kv_mask=mask)
-            wqc = P(p + "1.EncDecAttention.q.weight")
-            dh2 = ops.gemm(L.GEMM_NN, dqc, wqc.data)
-            ops.gemm(L.GEMM_TN, dqc, h2, out=wqc.main_grad, accumulate=acc)
-            ops.gemm(L.GEMM_NN, dkvc, self._d_kv[i], out=denc32, accumulate=(i != self.nd - 1))
-            ops.gemm(L.GEMM_TN, dkvc, enc_h, out=self._d_dkv[i], accumulate=acc)
+            dh2 = pj.cq.backward(dqc, h2, acc)
+            pj.ckv.backward(dkvc, enc_h, acc, dx=denc32, dx_accumulate=(i != self.nd - 1))
             s2 = P(p + "1.layer_norm.weight")
             dy1 = ops.rmsnorm_bwd(dh2, y1, s2.data, r2, s2.main_grad, accumulate=acc, dres=dy2)
             # causal self-attention with the decoder's relative-position bias
-            wos = P(p + "0.SelfAttention.o.weight")
-            do = ops.gemm(L.GEMM_NN, dy1, wos.data)
-            ops.gemm(L.GEMM_TN, dy1, o.view(Td, inner), out=wos.main_grad, accumulate=acc)
+            do = pj.o.backward(dy1, o.view(Td, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Sd, 3, nh, dk), dqkv.view(B, Sd, 3, nh, dk)
             ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, True,
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], rel_bias=rel_d, drel_bias=drel_d)
-            dh1 = ops.gemm(L.GEMM_NN, dqkv, self._d_qkv[i])
-            ops.gemm(L.GEMM_TN, dqkv, h1, out=self._d_dqkv[i], accumulate=acc)
+            dh1 = pj.qkv.backward(dqkv, h1, acc)
             s1 = P(p + "0.layer_norm.weight")
             dy = ops.rmsnorm_bwd(dh1, y, s1.data, r1, s1.main_grad, accumulate=acc, dres=dy1)
             if i == 0:
@@ -392,27 +373,18 @@ class MT5ForConditionalGeneration(FlatModel):
         es = P("encoder.final_layer_norm.weight")
         dx = ops.rmsnorm_bwd(denc, xfe, es.data, rfe, es.main_grad, accumulate=acc)
         for i in reversed(range(self.ne)):
-            p = f"encoder.block.{i}.layer."
-            x, r1, h1, qkv, o, lse, x1, r2, h2, gu, act = eacts[i]
+            p, pj = f"encoder.block.{i}.layer.", self._enc[i]
+            x, r1, h1, qkv, o, lse, x1, r2, h2, ms = eacts[i]
             eacts[i] = None
-            wo = P(p + "1.DenseReluDense.wo.weight")
-            dact = ops.gemm(L.GEMM_NN, dx, wo.data)
-            ops.gemm(L.GEMM_TN, dx, act, out=wo.main_grad, accumulate=acc)
-            dgu = torch.empty_like(gu)
-            ops.glu_bwd(L.ACT_GELU_TANH, dact, gu[:, :ff], gu[:, ff:], dgu[:, :ff], dgu[:, ff:])
-            dh2 = ops.gemm(L.GEMM_NN, dgu, self._e_wi[i])
-            ops.gemm(L.GEMM_TN, dgu, h2, out=self._e_dwi[i], accumulate=acc)
+            dh2 = pj.mlp.backward(dx, h2, ms, acc)
             s2 = P(p + "1.layer_norm.weight")
             dx1 = ops.rmsnorm_bwd(dh2, x1, s2.data, r2, s2.main_grad, accumulate=acc, dres=dx)
-            wos = P(p + "0.SelfAttention.o.weight")
-            do = ops.gemm(L.GEMM_NN, dx1, wos.data)
-            ops.gemm(L.GEMM_TN, dx1, o.view(Te, inner), out=wos.main_grad, accumulate=acc)
+            do = pj.o.backward(dx1, o.view(Te, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Se, 3, nh, dk), dqkv.view(B, Se, 3, nh, dk)
             ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Se, nh, dk), lse, 1.0, False,
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, rel_bias=rel_e, drel_bias=drel_e)
-            dh1 = ops.gemm(L.GEMM_NN, dqkv, self._e_qkv[i])
-            ops.gemm(L.GEMM_TN, dqkv, h1, out=self._e_dqkv[i], accumulate=acc)
+            dh1 = pj.qkv.backward(dqkv, h1, acc)
             s1 = P(p + "0.layer_norm.weight")
             dx = ops.rmsnorm_bwd(dh1, x, s1.data, r1, s1.main_grad, accumulate=acc, dres=dx1)
             if i == 0:

@@ -20,6 +20,7 @@ from fsb200.engine import ZeroEngine
 from fsb200.flat import FlatBuffers
 from fsb200.models.bert import BertForMaskedLM, MegatronBertForPreTraining
 from fsb200.models.gpt2 import GPT2LMHeadModel
+from fsb200.models.layers import GatedMLP, Linear
 from fsb200.models.llama import LlamaForCausalLM
 from fsb200.models.t5 import MT5ForConditionalGeneration
 from fsb200.trainer import PretrainStep
@@ -163,8 +164,8 @@ def _tied_writes(flat):
 
 
 def _tensors(obj, path, seen):
-    """(attribute path, tensor) of every tensor reachable from obj through attributes (of modules and flat buffers), lists,
-    tuples, dicts and a parameter's .main_grad."""
+    """(attribute path, tensor) of every tensor reachable from obj through attributes (of modules, flat buffers and the
+    models' projections), lists, tuples, dicts and a parameter's .main_grad."""
     if id(obj) in seen:
         return
     seen.add(id(obj))
@@ -178,7 +179,7 @@ def _tensors(obj, path, seen):
         items = [(f"{path}[{k!r}]", v) for k, v in obj.items()]
     elif isinstance(obj, (list, tuple)):
         items = [(f"{path}[{i}]", v) for i, v in enumerate(obj)]
-    elif isinstance(obj, (nn.Module, FlatBuffers)):
+    elif isinstance(obj, (nn.Module, FlatBuffers, Linear, GatedMLP)):
         items = [(f"{path}.{k}", v) for k, v in vars(obj).items()]
     else:
         return
@@ -195,6 +196,12 @@ def test_zero2_compaction_leaves_no_stale_gradient_alias(name):
     assert model.flat.grads.numel() < model.flat.total, "the layer buckets were not folded onto rotating gradient slots"
     stale = [p for p, t in _tensors(model, "model", set()) if t.untyped_storage().data_ptr() == old.data_ptr()]
     assert not stale, f"still on the released gradient buffer: {stale}"
+    # every gradient view the flat buffers handed out is held where the walk sees it, not only by the flat buffers' own list
+    reached = {id(model.flat)}
+    for _ in _tensors(model, "model", reached):
+        pass
+    unseen = [(off, shape) for t, off, shape in model.flat._grad_views if id(t) not in reached]
+    assert not unseen, f"gradient views the walk does not reach outside the flat buffers (offset, shape): {unseen}"
 
 
 # ---- B: the gradient the engine hands to AdamW, exactly --------------------------------------------------------------------
