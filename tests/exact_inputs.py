@@ -373,3 +373,303 @@ def selector_bias(H, Sq, Skv, deltas):
         for d in (dl if isinstance(dl, (tuple, list)) else (dl,)):
             rel[h, d + Sq - 1] = SELECT
     return rel
+
+
+# ================================================================================ the training step's looping kernels
+# Constructions for tests/test_exact_step_gpu.py: the fused cross-entropy, AdamW, the sum of squares, the vector helpers,
+# the column sums and the embedding gather / sorted backward. Each is a function of the element, row or token index, so the
+# GPU tests build multi-GB inputs on the device chunk by chunk and name the index a defect touched.
+LN2 = math.log(2.0)
+XENT_GAP = 128            # least gap between a dead logit and its row maximum: __expf(-128) = ex2.approx(-184.7) flushes to 0
+XENT_MAX_J = 6            # a row has 2^j live logits, j <= 6
+
+
+def xent_special_columns(V):
+    """Columns where a vector, an unrolled load or a loop iteration of the 512-thread row loop begins or ends: 0, V - 1, the
+    8-column vector edges around 8, the 4096-column edges of the four loads in flight and the 16384-column iteration edges."""
+    cand = [0, V - 1, V - 8, 7, 8, 4095, 4096, 8191, 8192, 16383, 16384, 32767, 32768, 49151, 49152]
+    return [c for c in dict.fromkeys(cand) if 0 <= c < V]
+
+
+def xent_strides(V):
+    """Distances between the live columns of a row: neighbours, one lane of consecutive vectors, and wide spreads; every one
+    small enough that 64 of them stay distinct modulo V."""
+    return [1, 7, 8, 9, 257, V // (2 ** XENT_MAX_J + 1)]
+
+
+def xent_rows(t, V, S, shift, ignore=None, ignore_index=-100):
+    """Per-row description of the exact cross-entropy input, for the int64 row indices t (any device).
+
+    Row t has 2^j live logits equal to its maximum M, at columns base + k stride (mod V), k < 2^j; every other logit is
+    M - 128, M - 136 or M - 144 (by column mod 3) for the rows with M in [-80, 80] (even), and M - 128 (1 + column mod 3) for
+    the rows with M = 2048 + 128 u in the thousands. The label of row t is a live column (the first or the last), a special
+    dead column, or a plain dead column; or ignore_index where ignore(t) holds and on the last `shift` rows of a sequence.
+    Returns a dict of tensors shaped like t: j, M, base, stride, n_live, label (ignore_index when ignored), valid."""
+    dev = t.device
+    sp = torch.tensor(xent_special_columns(V), device=dev)
+    st = torch.tensor(xent_strides(V), device=dev)
+    j = (t * 5 + t // 3) % (XENT_MAX_J + 1)
+    big = t % 11 == 0
+    M = torch.where(big, 2048 + 128 * ((t // 11) % 8), 2 * ((t * 37) % 81) - 80)
+    base = torch.where(t % 3 == 0, sp[(t // 3) % len(sp)], (t * 7919) % V)
+    stride = st[(t // 3) % len(st)]
+    n_live = torch.ones_like(j) << j
+    kind = (t // 7) % 4
+    plain_dead = (base + n_live * stride) % V
+    special = sp[(t // 4) % len(sp)]
+    special_is_live = xent_is_live(special, base, stride, n_live, V)
+    label = torch.where(kind == 0, base, torch.where(kind == 1, (base + (n_live - 1) * stride) % V,
+                        torch.where((kind == 2) & ~special_is_live, special, plain_dead)))
+    s = t % S
+    valid = s + shift < S
+    if ignore is not None:
+        valid &= ~ignore(t)
+    label = torch.where(valid, label, torch.full_like(label, ignore_index))
+    return {"j": j, "M": M, "base": base, "stride": stride, "n_live": n_live, "label": label, "valid": valid}
+
+
+def xent_is_live(c, base, stride, n_live, V):
+    """Whether column c is one of the live columns base + k stride (mod V), k < n_live (all broadcast)."""
+    d = (c - base) % V
+    return (d % stride == 0) & (d // stride < n_live)
+
+
+def xent_labels_array(rows_desc, S, shift, V):
+    """labels[rows] as the kernel reads them (labels[t + shift] for row t): the label of row t stored at t + shift; the first
+    `shift` entries of each sequence, which no row reads, hold a plain column."""
+    label = rows_desc["label"]
+    rows = label.numel()
+    arr = torch.full_like(label, V // 2)
+    if shift == 0:
+        return label.clone()
+    s = torch.arange(rows, device=label.device) % S
+    keep = s + shift < S
+    idx = torch.arange(rows, device=label.device)[keep]
+    arr[idx + shift] = label[keep]
+    return arr
+
+
+def xent_logits(t, V, desc_fn):
+    """Logits of rows t ([len(t), V] fp32 on t's device, every value a bf16 value)."""
+    d = desc_fn(t)
+    c = torch.arange(V, device=t.device)[None, :]
+    M = d["M"][:, None]
+    small = M.abs() <= 80
+    dead = torch.where(small, M - XENT_GAP - 8 * (c % 3), M - XENT_GAP * (1 + c % 3))
+    live = xent_is_live(c, d["base"][:, None], d["stride"][:, None], d["n_live"][:, None], V)
+    return torch.where(live, M, dead).float(), live, d
+
+
+def xent_grad_scale_f32(grad_scale, n_valid):
+    """The kernel's fp32 factor grad_scale / n_valid: one IEEE division of two fp32 values."""
+    return float(np.float32(grad_scale) / np.float32(n_valid))
+
+
+def xent_row_loss_exact(M, j, lab_logit):
+    """fp64 M + log(2^j) - logit[label] (the true loss of a row whose row sum is 2^j)."""
+    return M.double() + j.double() * LN2 - lab_logit.double()
+
+
+def xent_row_loss_bound(M, j, ref):
+    """What the kernel's lse = M + logf(2^j) then lse - logit[label] may be off by in fp32: logf within 1 ulp of j ln2, and
+    one rounding of each of the two additions (ulp(x) <= 2^-23 |x|), doubled."""
+    lg = j.double() * LN2
+    return 2.0 ** -22 * lg + 2.0 ** -22 * (M.double().abs() + lg) + 2.0 ** -22 * ref.abs()
+
+
+XENT_MEAN_DEPTH = 42      # longest fp32 addition chain of loss_reduce_kernel: 32 strided terms (rows <= 32768), 5 + 5 tree levels
+
+
+# ------------------------------------------------------------------------------------------------------------- AdamW
+ADAM_LR = 0.25            # a power of two: master moves by exactly +-lr per step
+ADAM_EXP_SPAN = 121       # gradient magnitude 2^((i mod 121) - 60): names the element class a thread read
+
+
+def adam_p0(i):
+    """Initial master weight of element i: an integer below 2^19 in magnitude (exact in fp32 with two fraction bits to spare)."""
+    return ((i % (1 << 20)) - (1 << 19)).float()
+
+
+def adam_exponent(i):
+    return (i % ADAM_EXP_SPAN) - 60
+
+
+def adam_sign(i, step):
+    """+1 or -1: bit (step + 7) of a multiplicative hash of i, so neighbouring elements and steps differ."""
+    return 1 - 2 * (((i * 2654435761) >> (step + 7)) & 1)
+
+
+def adam_grad(i, step):
+    """Gradient of element i at `step`: +-2^e, e in [-60, 60]: exact in bf16 and fp32, and its square (times a grad_scale of
+    2^-3 .. 2^2) stays a normal fp32 number."""
+    return torch.ldexp(adam_sign(i, step).float(), adam_exponent(i).int())
+
+
+def adam_master(i, steps):
+    """master after `steps` updates with beta1 = beta2 = eps = wd = 0: m = g, v = g^2, denom = |g|, so p -= lr sign(g)."""
+    acc = torch.zeros_like(i, dtype=torch.float32)
+    for s in range(steps):
+        acc += adam_sign(i, s).float()
+    return adam_p0(i) - ADAM_LR * acc
+
+
+# --------------------------------------------------------------------------------------------------------- sum of squares
+SUMSQ_FIELDS = 12         # rounds named per launch: value 2^(f - 11), square 2^(2f - 22), f < 12: bits -22 .. 0
+
+
+def sumsq_field_positions(round_lo, n_rounds, threads, nvec):
+    """(flat element index, field f) of the one non-zero element of each grid-stride round round_lo .. round_lo + 11 that
+    exists: round r reads vectors r * threads .. (r + 1) * threads - 1; the element sits at a thread that moves with r and
+    in vector slot r mod 4. Returns a list of (index, round, field)."""
+    out = []
+    for f in range(SUMSQ_FIELDS):
+        r = round_lo + f
+        if r >= n_rounds:
+            break
+        width = min(threads, nvec - r * threads)
+        th = (r * 7919 + 13) % width
+        out.append(((r * threads + th) * 4 + r % 4, r, f))
+    return out
+
+
+def sumsq_field_value(f):
+    return 2.0 ** (f - 11)
+
+
+def sumsq_count_pattern(i):
+    """+-1 at the elements with i mod 8 == (i // 8) mod 8 (every vector slot and thread over the rounds), 0 elsewhere."""
+    on = (i % 8) == ((i // 8) % 8)
+    return torch.where(on, 1 - 2 * ((i // 64) % 2), 0).float()
+
+
+def sumsq_count(n):
+    """Number of non-zero elements of sumsq_count_pattern over [0, n)."""
+    full, rem = divmod(n, 64)
+    return full * 8 + sum(1 for k in range(rem) if k % 8 == k // 8)
+
+
+# ---------------------------------------------------------------------------------------------------------- column sums
+COLSUM_BITS = 22          # rows coded per column: row j of a window adds 2^j, so a column sum has at most 22 bits
+
+
+def colsum_plan(rows, cols, sms):
+    """(strips, rows per strip) as elementwise.cu's colsum_plan picks them."""
+    col_tiles = (cols + 63) // 64
+    want = (4 * sms + col_tiles - 1) // col_tiles
+    want = max(1, min(want, (rows + 31) // 32, 1024))
+    rps = ((rows + want - 1) // want + 31) // 32 * 32
+    return (rows + rps - 1) // rps, rps
+
+
+def colsum_focus(rows, cols, rps, pass_idx=0):
+    """Column c watches one window of COLSUM_BITS consecutive rows of one strip: rows strip * rps + 22 w .. + 21 (clipped to
+    the strip and the matrix), row k of the window holding 2^k in that column and every other row 0. The (strip, window)
+    pairs are dealt out to the columns cyclically, shifted by pass_idx * cols, so that n_passes(...) passes cover every row.
+    Returns (row index [cols, 22] int64 with -1 where the window is short, strip [cols], window [cols])."""
+    ns = (rows + rps - 1) // rps
+    nw = (rps + COLSUM_BITS - 1) // COLSUM_BITS
+    tup = (torch.arange(cols) + pass_idx * cols) % (ns * nw)
+    strip, win = tup // nw, tup % nw
+    k = torch.arange(COLSUM_BITS)
+    r = strip[:, None] * rps + win[:, None] * COLSUM_BITS + k[None, :]
+    ok = (win[:, None] * COLSUM_BITS + k[None, :] < rps) & (r < rows)
+    return torch.where(ok, r, torch.full_like(r, -1)), strip, win
+
+
+def colsum_passes(rows, cols, rps):
+    ns = (rows + rps - 1) // rps
+    return -(-(ns * ((rps + COLSUM_BITS - 1) // COLSUM_BITS)) // cols)
+
+
+def colsum_matrix(rows, cols, rr, device=None):
+    """The bf16 [rows, cols] matrix of colsum_focus rows rr, and its exact column sums (fp64)."""
+    x = torch.zeros(rows, cols, dtype=torch.float32, device=device)
+    k = torch.arange(COLSUM_BITS, device=device).expand_as(rr)
+    c = torch.arange(cols, device=device)[:, None].expand_as(rr)
+    ok = rr >= 0
+    x[rr[ok], c[ok]] = torch.ldexp(torch.ones(int(ok.sum()), device=device), k[ok].int())
+    want = torch.where(ok, torch.ldexp(torch.ones_like(rr, dtype=torch.float64), k), 0.0).sum(1)
+    return x.to(torch.bfloat16), want
+
+
+def colsum_missing_rows(got, want, rr_col):
+    """The rows of one column whose bit is set in want but not in got (both integers), and those set only in got."""
+    g, w = int(got), int(want)
+    lost = [int(rr_col[k]) for k in range(COLSUM_BITS) if (w >> k) & 1 and not (g >> k) & 1]
+    extra = [k for k in range(COLSUM_BITS + 2) if (g >> k) & 1 and not (w >> k) & 1]
+    return lost, extra
+
+
+# ------------------------------------------------------------------------------------------------ sorted embedding backward
+EMB_CODED_MAX = 8         # a short run has 1..8 occurrences; occurrence q adds +-2^q: a run sum fits bf16's 8 bits
+EMB_BIG_COLS = 384        # the long run: columns c < 384 count occurrences q = c mod 384; 384 + b counts block q // 384
+
+
+def embedding_bwd_ids(tokens, V, big_id, seed):
+    """ids [tokens] int64: half the tokens carry big_id (one long run), the other half runs of 1..8 occurrences over distinct
+    ids that include 0 (the run at sorted position 0) and V - 1 (the run that ends at the last sorted position), token order
+    shuffled. Returns (ids, short_ids, short_lengths)."""
+    g = torch.Generator().manual_seed(seed)
+    half = tokens // 2
+    lengths = []
+    total = 0
+    while total < tokens - half:
+        ln = 1 + len(lengths) % EMB_CODED_MAX
+        ln = min(ln, tokens - half - total)
+        lengths.append(ln)
+        total += ln
+    nrun = len(lengths)
+    pool = torch.randperm(V - 2, generator=g)[:nrun + 1] + 1
+    pool = pool[pool != big_id][:nrun - 2]
+    short_ids = torch.cat([torch.tensor([0]), pool, torch.tensor([V - 1])])
+    lens = torch.tensor(lengths)
+    ids = torch.cat([torch.full((half,), big_id), short_ids.repeat_interleave(lens)])
+    perm = torch.randperm(tokens, generator=g)
+    return ids[perm].contiguous(), short_ids, lens
+
+
+def occurrence_index(ids):
+    """For each token, how many earlier tokens (in token order) carry the same id: its place in a stable sort's run."""
+    order = torch.sort(ids, stable=True).indices
+    sorted_ids = ids[order]
+    start = torch.ones_like(sorted_ids, dtype=torch.bool)
+    start[1:] = sorted_ids[1:] != sorted_ids[:-1]
+    pos = torch.arange(len(ids))
+    run_start = torch.cummax(torch.where(start, pos, torch.zeros_like(pos)), 0).values
+    occ = torch.empty_like(ids)
+    occ[order] = pos - run_start
+    return occ
+
+
+def embedding_bwd_dout(ids, occ, cols, big_id, seed):
+    """dout [tokens, cols] fp32 (bf16 values) and the old dW rows of the touched ids:
+    - short runs: occurrence q adds s 2^q in column c, s = +1 on even 8-column vectors and -1 on odd ones; the old value is
+      -256 s, so old + run sum is in [-256, 256] in magnitude: a bf16 integer, and a lost or doubled occurrence flips its bit;
+    - the long run: columns c < 384 hold 1 where q mod 384 == c, columns 384 + b hold 1 where q // 384 == b (old -256), so one
+      lost occurrence q is named by the pair of columns it leaves short; the remaining columns hold integers in [-3, 3] (old
+      a small integer), summed exactly in fp32 and rounded once to bf16."""
+    g = torch.Generator().manual_seed(seed)
+    T = len(ids)
+    c = torch.arange(cols)[None, :]
+    sgn = 1.0 - 2.0 * ((c // 8) % 2).double()
+    short = (ids != big_id)[:, None]
+    q = occ[:, None]
+    d_short = sgn * torch.ldexp(torch.ones(T, 1, dtype=torch.float64), q.clamp(max=30))
+    nb = -(-int((ids == big_id).sum()) // EMB_BIG_COLS)
+    d_big = torch.where(c < EMB_BIG_COLS, (q % EMB_BIG_COLS == c).double(),
+                        torch.where(c < EMB_BIG_COLS + nb, (q // EMB_BIG_COLS == c - EMB_BIG_COLS).double(),
+                                    torch.randint(-3, 4, (T, cols), generator=g).double()))
+    dout = torch.where(short, d_short, d_big)
+    return dout
+
+
+def embedding_bwd_old(V, cols, big_id, n_big, short_ids, seed):
+    """Initial dW [V, cols] fp64: random integers in [-50, 50] on the rows no id hits, -256 s on the short runs' rows, -256 on
+    the long run's counting columns and a small integer elsewhere on its row."""
+    g = torch.Generator().manual_seed(seed)
+    old = torch.randint(-50, 51, (V, cols), generator=g).double()
+    c = torch.arange(cols)
+    sgn = 1.0 - 2.0 * ((c // 8) % 2).double()
+    old[short_ids] = -256.0 * sgn
+    old[big_id, c < EMB_BIG_COLS + -(-n_big // EMB_BIG_COLS)] = -256.0
+    return old

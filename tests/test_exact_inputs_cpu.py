@@ -5,6 +5,7 @@ against these references; this file keeps the references honest without a device
 import math
 
 import numpy as np
+import pytest
 import torch
 
 import exact_inputs as X
@@ -243,3 +244,194 @@ def test_selector_bias_winners_and_exact_diagonals():
     ref = X.attention_ref(torch.zeros(1, 130, 3, 64, dtype=torch.float64), V, V, X.LN2_SCALE, False, None, rel=rel)
     assert torch.equal(ref["O"][0, 129, 0], V[0, 0, 0]) and torch.equal(ref["O"][0, :, 1], V[0, :130, 1])
     assert torch.equal(ref["O"][0, 0, 2], V[0, 390, 2]) and int(ref["nwin"][0, 2, 1]) == 391
+
+
+# ================================================================================ the training step's looping kernels
+def _f32(x):
+    return np.float32(x)
+
+
+@pytest.mark.parametrize("V,S,shift,ignore", [(50264, 1024, 1, lambda t: t % 5 == 3), (32600, 512, 0, lambda t: t % 4 >= 2),
+                                              (21128, 128, 1, lambda t: t % 9 == 4)])
+def test_xent_rows_are_exact(V, S, shift, ignore):
+    rows = {50264: 32768, 32600: 16384, 21128: 3200}[V]
+    t = torch.arange(rows)
+    d = X.xent_rows(t, V, S, shift, ignore=ignore)
+    # every row: 2^j distinct live columns; dead labels are dead and live labels live; special columns are used
+    assert max(X.xent_strides(V)) * (2 ** X.XENT_MAX_J + 1) <= V
+    valid = d["valid"]
+    lab = d["label"]
+    assert bool((lab[~valid] == -100).all()) and bool(((lab[valid] >= 0) & (lab[valid] < V)).all())
+    live_lab = X.xent_is_live(lab, d["base"], d["stride"], d["n_live"], V) & valid
+    kind = (t // 7) % 4
+    assert bool(live_lab[valid & (kind <= 1)].all()) and not bool(live_lab[valid & (kind == 3)].any())
+    assert live_lab[valid].any() and (~live_lab[valid]).any()
+    sp = set(X.xent_special_columns(V))
+    assert {0, V - 1} <= set(d["base"].tolist()) and {0, V - 1} <= set(lab[valid & live_lab].tolist())
+    assert len(sp & set(lab[valid & ~live_lab].tolist())) >= len(sp) // 2, "dead labels on the special columns"
+    labels = X.xent_labels_array(d, S, shift, V)
+    s = t % S
+    read = s + shift < S
+    assert torch.equal(labels[(t + shift)[read]], lab[read]), "labels[t + shift] is row t's label"
+    n_valid = int(valid.sum())
+    if V == 32600:
+        assert n_valid == 8192
+    else:
+        assert n_valid & (n_valid - 1) != 0
+    # logits of a spread of rows: bf16 values, 2^j at the maximum, the rest >= 128 below; exp of the gap flushes to 0
+    pick = torch.cat([torch.arange(0, 600), torch.arange(rows - 300, rows), torch.randperm(rows)[:300]])
+    x, live, dd = X.xent_logits(pick, V, lambda tt: X.xent_rows(tt, V, S, shift, ignore=ignore))
+    assert X.is_bf16(x)
+    assert torch.equal(live.sum(1), dd["n_live"])
+    mx = x.max(1).values
+    assert torch.equal(mx, dd["M"].float()) and set(dd["M"].tolist()) >= {-80, 80, 2048 + 128 * 7}
+    assert bool(((x[~live] <= (mx[:, None].expand_as(x))[~live] - X.XENT_GAP)).all())
+    assert _f32(-X.XENT_GAP) * X.LOG2E_F32 < -126, "ex2.approx.ftz of the scaled gap is below 2^-126: exactly 0"
+    for c in X.xent_special_columns(V):
+        assert live[:, c].any(), f"special column {c} is live in some row"
+
+
+def test_xent_gradient_and_loss_references():
+    for gs, nv in ((1.0, 26214), (1.0, 8192), (3.0, 2791)):
+        sc = X.xent_grad_scale_f32(gs, nv)
+        assert sc == float(np.float32(gs) / np.float32(nv))
+        for j in range(X.XENT_MAX_J + 1):
+            p = 2.0 ** -j
+            for v in (p, p - 1, -1.0, 0.0):
+                assert float(_f32(v)) == v, "p - onehot is exact in fp32 before the one product"
+    M, j = torch.tensor([-80, 80, 2944]), torch.tensor([0, 6, 3])
+    lab = torch.tensor([-80, -64, 2944 - 256])
+    ref = X.xent_row_loss_exact(M, j, lab)
+    assert torch.allclose(ref, torch.tensor([0.0, 144 + 6 * math.log(2), 256 + 3 * math.log(2)], dtype=torch.float64))
+    # the kernel's fp32 chain, with logf off by one ulp, stays inside the bound
+    for m, jj, lb in zip(M.tolist(), j.tolist(), lab.tolist()):
+        lg = np.float32(math.log(2.0 ** jj))
+        lg = np.nextafter(lg, np.float32(np.inf))
+        got = float(np.float32(np.float32(m) + lg) - np.float32(lb))
+        r = m + jj * math.log(2) - lb
+        assert abs(got - r) <= float(X.xent_row_loss_bound(torch.tensor(m), torch.tensor(jj), torch.tensor(r)))
+
+
+def test_adamw_trajectory_is_exact_in_fp32():
+    """The kernel's fp32 operations with beta1 = beta2 = eps = wd = 0 on the coded gradients, simulated in numpy fp32 over
+    every exponent class and the grad scales used, give m = g, v = g^2 and the closed-form master, bit for bit."""
+    i = torch.cat([torch.arange(0, 5000), torch.arange(2 ** 29 - 2000, 2 ** 29 + 4), torch.tensor([124_445_183])])
+    p = X.adam_p0(i).numpy()
+    assert np.array_equal(p.astype(np.float64), X.adam_p0(i).double().numpy())
+    lr = np.float32(X.ADAM_LR)
+    for s, gs in enumerate((2.0 ** -3, 1.0, 4.0, 1.0)):
+        g16 = X.adam_grad(i, s)
+        assert X.is_bf16(g16.double())
+        gj = g16.numpy().astype(np.float32) * np.float32(gs)
+        m = np.float32(0) * np.float32(5) + np.float32(1) * gj
+        v = np.float32(0) * np.float32(5) + np.float32(1) * gj * gj
+        assert np.all(np.abs(v) >= np.float32(2.0 ** -126)) and np.all(np.isfinite(v))
+        denom = np.sqrt(v) / np.float32(1) + np.float32(0)
+        p = p * np.float32(1) - (lr / np.float32(1)) * (m / denom)
+        assert np.array_equal(m, gj) and np.array_equal(v, gj * gj) and np.array_equal(denom, np.abs(gj))
+        assert np.array_equal(p, X.adam_master(i, s + 1).numpy())
+    # the exponent names the element class: every class occurs among any 121 neighbours
+    assert len(set(X.adam_exponent(torch.arange(7, 7 + X.ADAM_EXP_SPAN)).tolist())) == X.ADAM_EXP_SPAN
+
+
+def test_sumsq_fields_and_count():
+    threads = 8 * 132 * 256
+    n = 124_445_184
+    nvec = n // 4
+    R = -(-nvec // threads)
+    seen = []
+    for lo in range(0, R, X.SUMSQ_FIELDS):
+        pos = X.sumsq_field_positions(lo, R, threads, nvec)
+        vals = [X.sumsq_field_value(f) for _, _, f in pos]
+        assert all(X.is_bf16(torch.tensor([v], dtype=torch.float64)) for v in vals)
+        for p, r, f in pos:
+            assert p < n and (p // 4) // threads == r and p % 4 == r % 4
+        sq = [v * v for v in vals]
+        # partial sums in any order, on top of 0 or 2: dyadic multiples of 2^-22 below 4 (24 bits): exact in fp32
+        total = sum(sq) + 2.0
+        assert total < 4 and all((x * 2 ** 22).is_integer() for x in sq)
+        perm = np.random.default_rng(lo).permutation(len(sq))
+        acc = np.float32(2.0)
+        for k in perm:
+            acc = np.float32(acc + np.float32(sq[k]))
+        assert float(acc) == total
+        # a lost field clears exactly its bit
+        code = round((total - 2.0 - sq[-1]) * 2 ** 22)
+        assert [f for _, _, f in pos if not (code >> (2 * f)) & 1] == [pos[-1][2]]
+        seen += [r for _, r, _ in pos]
+    assert seen == list(range(R))
+    i = torch.arange(0, 64 * 1000 + 37)
+    x = X.sumsq_count_pattern(i)
+    assert int((x != 0).sum()) == X.sumsq_count(len(i)) and set(x.unique().tolist()) == {-1.0, 0.0, 1.0}
+    assert set((i[x != 0] % 4).tolist()) == {0, 1, 2, 3}
+    assert X.sumsq_count(n) + 3 < 2 ** 24
+
+
+@pytest.mark.parametrize("rows,cols", [(32768, 768), (32768, 3072), (16384, 2048), (16384, 8192), (32, 786432),
+                                       (8, 98304), (777, 1032)])
+def test_colsum_windows_cover_every_row(rows, cols):
+    ns, rps = X.colsum_plan(rows, cols, 132)
+    covered = torch.zeros(rows, dtype=torch.bool)
+    for p in range(X.colsum_passes(rows, cols, rps)):
+        rr, strip, win = X.colsum_focus(rows, cols, rps, p)
+        ok = rr >= 0
+        covered[rr[ok]] = True
+        assert bool(((rr[ok] // rps) == strip[:, None].expand_as(rr)[ok]).all()), "a window stays inside its strip"
+        if cols <= 8192:
+            x, want = X.colsum_matrix(rows, cols, rr)
+            assert X.is_bf16(x.double()) and torch.equal(x.double().sum(0), want)
+            assert want.max() < 2 ** X.COLSUM_BITS and (want + 500).max() < 2 ** 24
+            # drop one row: the decoder names it
+            c = int(ok.sum(1).argmax())
+            k = int(ok[c].nonzero()[-1])
+            lost, extra = X.colsum_missing_rows(want[c] - 2 ** k, want[c], rr[c])
+            assert lost == [int(rr[c, k])] and extra == []
+    assert covered.all(), "every row is watched by some column in some pass"
+
+
+def test_embedding_bwd_runs_are_exact():
+    T, V, h, big = 32768, 50264, 768, 50256
+    ids, short_ids, lens = X.embedding_bwd_ids(T, V, big, seed=1)
+    n_big = int((ids == big).sum())
+    assert n_big == T // 2 and int(lens.sum()) == T - n_big and int(lens.max()) == X.EMB_CODED_MAX
+    assert len(set(short_ids.tolist())) == len(short_ids) and big not in set(short_ids.tolist())
+    srt = torch.sort(ids, stable=True).values
+    assert int(srt[0]) == 0 and int(srt[-1]) == V - 1
+    occ = X.occurrence_index(ids)
+    assert int(occ[ids == big].max()) == n_big - 1
+    for sid, ln in list(zip(short_ids.tolist(), lens.tolist()))[:50]:
+        assert sorted(occ[ids == sid].tolist()) == list(range(ln))
+    dout = X.embedding_bwd_dout(ids, occ, h, big, seed=2)
+    old = X.embedding_bwd_old(V, h, big, n_big, short_ids, seed=3)
+    assert X.is_bf16(dout) and X.is_bf16(old)
+    # per id and column: sum |terms| + |old| < 2^24, so any order of fp32 additions is exact
+    absum = old.abs().index_add(0, ids, dout.abs())
+    assert absum.max() < 2 ** 24
+    want = old.index_add(0, ids, dout)
+    touched = torch.unique(ids)
+    coded = torch.cat([short_ids])
+    assert X.is_bf16(want[coded]), "short runs: old + run sum is a bf16 integer, so a lost bit shows"
+    nb = -(-n_big // X.EMB_BIG_COLS)
+    assert X.is_bf16(want[big, :X.EMB_BIG_COLS + nb])
+    # a lost occurrence of the long run is named by its two counting columns
+    q = 5000
+    tok = int(((ids == big) & (occ == q)).nonzero())
+    drop = want[big] - dout[tok]
+    short_cols = (want[big, :X.EMB_BIG_COLS + nb] != drop[:X.EMB_BIG_COLS + nb]).nonzero().view(-1).tolist()
+    assert short_cols == [q % X.EMB_BIG_COLS, X.EMB_BIG_COLS + q // X.EMB_BIG_COLS]
+    # a lost occurrence of a short run clears its bit
+    sid = int(short_ids[lens == X.EMB_CODED_MAX][0])
+    tok = int(((ids == sid) & (occ == 3)).nonzero())
+    assert int(abs((want[sid, 0] - dout[tok, 0]) - old[sid, 0])) == 255 - 8
+    assert len(touched) == len(short_ids) + 1
+
+
+def test_vector_helper_values_are_exact():
+    i = torch.arange(0, 10 ** 8, 9973)
+    x16 = (((i * 3) % 255) - 127).double()
+    old = ((i % (1 << 20)) - (1 << 19)).double()
+    assert X.is_bf16(x16) and torch.equal((old.float() + 0.25 * x16.float()).double(), old + 0.25 * x16)
+    b = (((i * 7) % 253) - 126).double() * torch.ldexp(torch.ones(len(i), dtype=torch.float64), -(i % 3))
+    assert X.is_bf16(b) and X.is_bf16(x16 * 0.125)
+    x32 = (i % (1 << 24)).float() * torch.ldexp(torch.ones(len(i)), -(i % 5).int())
+    assert not X.is_bf16(x32.double()), "the cast inputs need rounding"
