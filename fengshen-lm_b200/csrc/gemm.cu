@@ -82,19 +82,6 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   return x >= 0.f ? fmaf(-hx, erfc_z, x) : hx * erfc_z;
 }
 
-__device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int group_m, int& b, int& m_idx, int& n_idx) {
-  const int per = tiles_m * tiles_n;
-  b = t / per;
-  int r = t - b * per;
-  const int group_span = group_m * tiles_n;
-  const int g = r / group_span;
-  const int first_m = g * group_m;
-  const int gsize = min(tiles_m - first_m, group_m);
-  const int in_g = r - g * group_span;
-  m_idx = first_m + in_g % gsize;
-  n_idx = in_g / gsize;
-}
-
 // K range of a tile: the whole K, or for a K-split GEMM (p.ksplits > 1, batch index = split) the split's share of whole
 // k-blocks, [s * nkb / S, (s + 1) * nkb / S). `ab` is the operands' batch coordinate.
 __device__ __forceinline__ void k_range(const GemmParams& p, int b, int num_kb, int& kb_lo, int& kb_hi, int& ab) {
@@ -315,14 +302,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
     if (leader) tma_store_wait<0>();   // every store has completed before the CTA (and its shared memory) goes away
   }
-}
-
-// SMs left to concurrently running communication kernels (fsb_set_reserved_sms): a persistent GEMM CTA fills an SM
-// (all of its registers), so a collective that overlaps backward would otherwise push GEMM CTAs into a second wave.
-static int g_reserved_sms = 0;
-static inline int gemm_sms() {
-  const int n = num_sms() - g_reserved_sms;
-  return n < 1 ? 1 : n;
 }
 
 template <int kLayout, int BN>

@@ -16,6 +16,8 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int g_reserved_sms = 0;
+
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;

@@ -32,6 +32,15 @@ void set_error(const char* fmt, ...);
 
 int num_sms();
 
+// SMs left to concurrently running communication kernels (fsb_set_reserved_sms): a persistent GEMM CTA fills an SM
+// (all of its registers), so a collective that overlaps backward would otherwise push GEMM CTAs into a second wave.
+// Every persistent GEMM (gemm.cu, gemm_fp8.cu) sizes its grid with gemm_sms().
+extern int g_reserved_sms;
+static inline int gemm_sms() {
+  const int n = num_sms() - g_reserved_sms;
+  return n < 1 ? 1 : n;
+}
+
 // 2-D / 3-D bf16 / fp32 tensor map with 128B swizzle. dims/box innermost-first; strides (bytes) for dims 1.. .
 // Returns 0 on success (error string set otherwise).
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,

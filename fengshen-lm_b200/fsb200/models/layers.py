@@ -34,6 +34,10 @@ class Linear:
     def __call__(self, x, epilogue=L.EPI_NONE, aux=None):
         return ops.gemm(L.GEMM_NN if self.conv1d else L.GEMM_NT, x, self.weight, bias=self.bias, epilogue=epilogue, aux=aux)
 
+    def forward(self, x, save):
+        """-> (the output, what backward reads of the input: x itself when `save`, else None)."""
+        return self(x), (x if save else None)
+
     def backward(self, dy, x, accumulate, dx=None, dx_accumulate=False, colsum=True):
         """-> the gradient of the input x, given dy, the gradient of the output. Writes the weight's gradient (and the bias's)
         into the flat gradient buffer, adding to it when `accumulate`. dx: write the input gradient into this buffer instead,
@@ -51,23 +55,55 @@ class Linear:
 
 class GatedMLP:
     """m = wo(act(gate) * up) with [gate | up] = wi(h): wi is one projection over the adjacent gate and up weights, `act` the
-    gate's activation (L.ACT_SILU for LLaMA, L.ACT_GELU_TANH for mT5)."""
+    gate's activation (L.ACT_SILU for LLaMA, L.ACT_GELU_TANH for mT5). wi and wo are Linear or Fp8Linear."""
 
     def __init__(self, wi, wo, act):
         self.wi, self.wo, self.act = wi, wo, act
 
-    def __call__(self, h):
-        """-> (m, what the backward reads)."""
-        gu = self.wi(h)
+    def __call__(self, h, save=True):
+        """-> (m, what the backward reads; with save=False, only what a forward needs is computed)."""
+        gu, hs = self.wi.forward(h, save)
         f = gu.shape[1] // 2
         act = ops.glu_fwd(self.act, gu[:, :f], gu[:, f:])
-        return self.wo(act), (gu, act)
+        m, acts = self.wo.forward(act, save)
+        return m, (hs, gu, acts)
 
-    def backward(self, dm, h, saved, accumulate):
+    def backward(self, dm, saved, accumulate):
         """-> the gradient of h; writes the weight gradients as Linear.backward does."""
-        gu, act = saved
+        hs, gu, act = saved
         f = gu.shape[1] // 2
         dact = self.wo.backward(dm, act, accumulate)
         dgu = torch.empty_like(gu)
         ops.glu_bwd(self.act, dact, gu[:, :f], gu[:, f:], dgu[:, :f], dgu[:, f:])
-        return self.wi.backward(dgu, h, accumulate)
+        return self.wi.backward(dgu, hs, accumulate)
+
+
+class Fp8Linear:
+    """A Linear (HF layout, no bias) run in FP8 with just-in-time per-tensor scaling, with Linear's call surface. The weight
+    and its gradient stay the bf16 flat-buffer views of `lin`; the weight is cast on every call, so nothing goes stale after
+    an optimizer step.
+      forward: y = x W^T from x e4m3 and W e4m3, both row-major; when saving, x's transposed codes and scale are kept for the
+               weight gradient instead of x.
+      backward: dy e5m2 (both layouts) and W e4m3 (transposed): dx = dy (W^T)^T, dW (+)= dy^T (x^T)^T into the flat gradient.
+    The token count and both extents of W must be multiples of 16."""
+
+    def __init__(self, lin):
+        if lin.conv1d or lin.bias is not None:
+            raise ValueError("fsb200 Fp8Linear: only bias-free [out, in] projections run in FP8")
+        self.lin = lin
+
+    def __call__(self, x):
+        return self.forward(x, False)[0]
+
+    def forward(self, x, save):
+        xq, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=save)
+        wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
+        return ops.gemm_fp8(xq, sx, wq, sw), ((xt, sx) if save else None)
+
+    def backward(self, dy, saved, accumulate, dx=None, dx_accumulate=False):
+        xt, sx = saved
+        dyq, dyt, sdy = ops.fp8_quantize(dy, "e5m2", rowwise=True, colwise=True)
+        _, wt, sw = ops.fp8_quantize(self.lin.weight, "e4m3", rowwise=False, colwise=True)
+        dx = ops.gemm_fp8(dyq, sdy, wt, sw, out=dx, accumulate=dx_accumulate)
+        ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate)
+        return dx

@@ -25,7 +25,7 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids
-from .layers import GatedMLP, Linear
+from .layers import Fp8Linear, GatedMLP, Linear
 
 
 def llama_ff_dim(hidden_size, multiple_of=256):
@@ -63,12 +63,16 @@ class QuantizedLinear:
     def __call__(self, x):
         return (ops.gemm_w8a16 if self.fmt == "int8" else ops.gemm_w4a16)(x, self.q, self.s)
 
+    def forward(self, x, save):
+        return self(x), None
+
     def backward(self, *_, **__):
         raise _quantized_unsupported(self.fmt, "backward")
 
 
 class LlamaForCausalLM(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False, load_in_4bit=False):
+    def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False, load_in_4bit=False,
+                 fp8=False):
         """tp_group: the tensor-model-parallel process group (mpu.get_model_parallel_group()) or None. With t = its size > 1
         this rank holds the shard the reference's `part_{rank}` checkpoints hold (utils/llama_convert/convert_fs_llama_tp.py
         :143-181): heads / ff columns / vocabulary rows split t ways (ColumnParallelLinear mpu/layers.py:261-360 for QKV,
@@ -82,11 +86,23 @@ class LlamaForCausalLM(FlatModel):
 
         load_in_4bit: the same with int4 projections (examples/ziya_inference/hf_quantizatin_inference.py:3,16): q packed two
         per byte [n / 2, k] + bf16 scales [n, k / 128], one per row and group of 128 k, run through the W4A16 GEMM.
-        hidden_size and the MLP width must then be multiples of 128."""
+        hidden_size and the MLP width must then be multiples of 128.
+
+        fp8: train in FP8 (include/fsb200.h, fsb_gemm_fp8). Each layer's four projections (query_key_value, dense, w1 | w3,
+        w2) run as Fp8Linear: e4m3 activations and weights, e5m2 gradients, per-tensor power-of-two scales computed from each
+        tensor's amax just before its cast, fp32 accumulation. The embedding, the LM head, the norms and attention stay bf16,
+        as do the master weights, the gradients and the optimizer state, so checkpoints and resume are unchanged. The training
+        and no-grad (validation) forwards run FP8; `generate` runs the bf16 layer stack on the same weights. Results differ from
+        bf16 by design. hidden_size, the MLP width and the tokens per micro-batch must be multiples of 16 (checked at the first
+        forward); tensor parallelism and load_in_8bit / load_in_4bit are refused."""
         super().__init__(config)
         import torch.distributed as dist
         if load_in_8bit and load_in_4bit:
             raise ValueError("fsb200 LlamaForCausalLM: load_in_8bit and load_in_4bit are mutually exclusive; pass one")
+        if fp8 and (load_in_8bit or load_in_4bit):
+            raise ValueError("fsb200 LlamaForCausalLM: fp8=True trains in FP8; it cannot be combined with load_in_8bit or "
+                             "load_in_4bit (inference-only weight formats)")
+        self.fp8 = bool(fp8)
         # the layer projections' weight format; load_in_8bit / load_in_4bit are kept as the public flags
         self.weight_format = "int8" if load_in_8bit else "int4" if load_in_4bit else "bf16"
         self.load_in_8bit = self.weight_format == "int8"
@@ -97,6 +113,9 @@ class LlamaForCausalLM(FlatModel):
         self.tp_rank = dist.get_rank(tp_group) if tp_group is not None else 0
         if quantized and self.tp > 1:
             raise _quantized_unsupported(self.weight_format, "tensor parallelism")
+        if self.fp8 and self.tp > 1:
+            raise NotImplementedError("fsb200 LlamaForCausalLM: fp8=True under tensor parallelism is not implemented (the "
+                                      "per-tensor scales of the shards differ from one GPU's)")
         h, V, nl, nh = config.hidden_size, config.vocab_size, config.num_hidden_layers, config.num_attention_heads
         self.h, self.V, self.nl, self.nh = h, V, nl, nh
         self.hn = h // nh
@@ -142,6 +161,11 @@ class LlamaForCausalLM(FlatModel):
                                  GatedMLP(Linear.span(self.flat, f"llama.layers.{i}.mlp.w1.weight", 2 * self.ff_l, h),
                                           Linear.of(lyr.mlp.w2.weight), L.ACT_SILU))
                           for i, lyr in enumerate(self.llama.layers)]
+        self._proj_bf16 = self._proj   # what generate runs
+        if self.fp8:
+            self._proj = [_Layer(Fp8Linear(lp.qkv), Fp8Linear(lp.dense),
+                                 GatedMLP(Fp8Linear(lp.mlp.wi), Fp8Linear(lp.mlp.wo), L.ACT_SILU))
+                          for lp in self._proj_bf16]
         self._head = Linear.of(self.embed_out.final_linear.weight)
 
         # RoPE tables exactly as RotaryEmbedding builds them (layers/positional_embeddings.py:38-52), fp32; inv_freq is also a
@@ -221,7 +245,7 @@ class LlamaForCausalLM(FlatModel):
     @property
     def _w13(self):
         """Per layer the [2ff, h] w1 | w3 operand of a bf16 model."""
-        return [lp.mlp.wi.weight for lp in self._proj]
+        return [lp.mlp.wi.weight for lp in self._proj_bf16]
 
     def _wq_targets(self):
         """{state-dict key: (q, s) it quantises into} of every quantised projection. w1 and w3 are the upper and lower
@@ -293,6 +317,10 @@ class LlamaForCausalLM(FlatModel):
                 torch._assert_async(((pos >= 0) & (pos < self._rope_rows)).all(),
                                     "fsb200 LlamaForCausalLM: position_ids outside [0, rope table rows); pass them on the "
                                     "host or raise config.max_position_embeddings")
+        if self.fp8 and (self.h % 16 or self.ff % 16 or (B * S) % 16):
+            raise ValueError(f"fsb200 LlamaForCausalLM(fp8=True): hidden_size ({self.h}), the MLP width ({self.ff}) and the "
+                             f"tokens per micro-batch (batch {B} x sequence {S}) must be multiples of 16 (the FP8 GEMM "
+                             "operands need 16-byte rows in both layouts)")
         lab = flat_ids(labels, dev)
         if self.weight_format != "bf16" and lab is not None and torch.is_grad_enabled():
             raise _quantized_unsupported(self.weight_format, "a training forward (labels under grad mode)")
@@ -318,11 +346,13 @@ class LlamaForCausalLM(FlatModel):
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
-    def _stack(self, ids, pos, B, S, attend, acts=None):
+    def _stack(self, ids, pos, B, S, attend, acts=None, proj=None):
         """Embedding, the layers and the final norm over ids [B * S] -> (hidden states, their rstd, residual stream).
         attend(i, q5) is layer i's attention over the per-head interleaved q|k|v view [B, S, heads, 3, head_dim] (rotary
-        embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads."""
+        embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads. proj: the layers'
+        projections (default self._proj)."""
         nh, hn, hl = self.nh_l, self.hn, self.h_l      # LOCAL heads under tensor parallelism
+        save = acts is not None
         self._need("no_decay"); self._need("embed_in")
         ids_l, emb_keep = self._local_ids(ids)
         x = ops.embedding_fwd(ids_l, self.llama.embed_in.word_embeddings.weight.data)
@@ -330,23 +360,23 @@ class LlamaForCausalLM(FlatModel):
             x.mul_(emb_keep)
             self._tp_all_reduce(x)
         prev_m = None
-        for i, (lyr, lp) in enumerate(zip(self.llama.layers, self._proj)):
+        for i, (lyr, lp) in enumerate(zip(self.llama.layers, self._proj if proj is None else proj)):
             self._need(f"layer{i}")
             h1, rstd1, x = ops.rmsnorm_fwd(x if prev_m is None else prev_m, lyr.input_layernorm.scale.data, self.eps,
                                            residual=None if prev_m is None else x)
-            qkv = lp.qkv(h1)
+            qkv, h1s = lp.qkv.forward(h1, save)   # h1s: what the QKV weight gradient reads of h1
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
             ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
             o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
-            a = lp.dense(o.view(B * S, hl))
+            a, os_ = lp.dense.forward(o.view(B * S, hl), save)
             self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
             h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
-            m, ms = lp.mlp(h2)
+            m, ms = lp.mlp(h2, save)
             self._tp_all_reduce(m)        # RowParallelLinear (w2)
             if acts is not None:
-                acts.append((x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, ms))
+                acts.append((x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms))
             # free this layer's temporaries before the next layer allocates its own (the peak of a long prompt's prefill)
-            del rstd1, h1, qkv, o, lse, a, rstd2, h2, ms
+            del rstd1, h1, h1s, qkv, o, os_, lse, a, rstd2, h2, ms
             x, prev_m = x1, m
         self._need("head")
         return ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
@@ -433,7 +463,7 @@ class LlamaForCausalLM(FlatModel):
 
     def _last_logits(self, ids, pos, B, S, attend):
         """fp32 logits [B, V] of the last position of every sequence."""
-        hf, _, _ = self._stack(ids, pos, B, S, attend)
+        hf, _, _ = self._stack(ids, pos, B, S, attend, proj=self._proj_bf16)   # fp8=True: generate runs in bf16
         last = hf.view(B, S, self.h)[:, -1].contiguous()                       # [B, h]
         rows = max(8, B)                                                        # the GEMM wants >= 8 aligned rows
         if rows != B:
@@ -461,22 +491,22 @@ class LlamaForCausalLM(FlatModel):
         dx = ops.rmsnorm_bwd(dhf, xf, fscale.data, rstdf, fscale.main_grad, accumulate=acc)
         for i in reversed(range(self.nl)):
             lyr, lp = self.llama.layers[i], self._proj[i]
-            x, rstd1, h1, qkv, o, lse, x1, rstd2, h2, ms = acts[i]
+            x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms = acts[i]
             acts[i] = None
             # x_next = x1 + m  ->  dm = dx, residual gradient into x1 = dx
-            dh2 = lp.mlp.backward(dx, h2, ms, acc)
+            dh2 = lp.mlp.backward(dx, ms, acc)
             self._tp_all_reduce(dh2)      # column-parallel w1|w3: dgrad partial sums
             s2 = lyr.post_attention_layernorm.scale
             dx1 = ops.rmsnorm_bwd(dh2, x1, s2.data, rstd2, s2.main_grad, accumulate=acc, dres=dx)
             # x1 = x + a  ->  da = dx1
-            do = lp.dense.backward(dx1, o.view(T, hl), acc)
+            do = lp.dense.backward(dx1, os_, acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, nh, 3, hn), dqkv.view(B, S, nh, 3, hn)
             ops.sdpa_bwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o, do.view(B, S, nh, hn), lse,
                          1.0 / math.sqrt(hn), True, d5[:, :, :, 0], d5[:, :, :, 1], d5[:, :, :, 2])
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=0)
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=hn)
-            dh1 = lp.qkv.backward(dqkv, h1, acc)
+            dh1 = lp.qkv.backward(dqkv, h1s, acc)
             self._tp_all_reduce(dh1)      # column-parallel QKV: dgrad partial sums
             s1 = lyr.input_layernorm.scale
             dx = ops.rmsnorm_bwd(dh1, x, s1.data, rstd1, s1.main_grad, accumulate=acc, dres=dx1)

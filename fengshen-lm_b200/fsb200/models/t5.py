@@ -337,7 +337,7 @@ class MT5ForConditionalGeneration(FlatModel):
             p, pj = f"decoder.block.{i}.layer.", self._dec[i]
             y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms = dacts[i]
             dacts[i] = None
-            dh3 = pj.mlp.backward(dy, h3, ms, acc)
+            dh3 = pj.mlp.backward(dy, ms, acc)
             s3 = P(p + "2.layer_norm.weight")
             dy2 = ops.rmsnorm_bwd(dh3, y2, s3.data, r3, s3.main_grad, accumulate=acc, dres=dy)
             # cross-attention
@@ -376,7 +376,7 @@ class MT5ForConditionalGeneration(FlatModel):
             p, pj = f"encoder.block.{i}.layer.", self._enc[i]
             x, r1, h1, qkv, o, lse, x1, r2, h2, ms = eacts[i]
             eacts[i] = None
-            dh2 = pj.mlp.backward(dx, h2, ms, acc)
+            dh2 = pj.mlp.backward(dx, ms, acc)
             s2 = P(p + "1.layer_norm.weight")
             dx1 = ops.rmsnorm_bwd(dh2, x1, s2.data, r2, s2.main_grad, accumulate=acc, dres=dx)
             do = pj.o.backward(dx1, o.view(Te, inner), acc)

@@ -173,6 +173,52 @@ def gemm_w4a16(a, q, s, out=None):
     return out
 
 
+FP8_FORMATS = {"e4m3": (0, torch.float8_e4m3fn), "e5m2": (1, torch.float8_e5m2)}   # name -> (fsb_fp8_format, code dtype)
+_FP8_CODE = {dt: code for code, dt in FP8_FORMATS.values()}
+
+
+def fp8_quantize(x, fmt, rowwise=True, colwise=False):
+    """Per-tensor FP8 quantisation of a bf16 x [rows, cols] (unit inner stride, row stride a multiple of 8; rows and cols
+    multiples of 16) in format `fmt` ("e4m3" or "e5m2") -> (y [rows, cols] or None, yt [cols, rows] or None, scale_inv fp32
+    [1]): the row-major codes if `rowwise`, the transposed codes if `colwise` (torch.float8_e4m3fn / float8_e5m2 tensors), and
+    1 / scale, the scale being the power of two 2^floor(log2(fmax / amax)); include/fsb200.h gives the rule, the rounding and
+    the NaN convention."""
+    _chk(x, _bf16, "x")
+    if fmt not in FP8_FORMATS:
+        raise RuntimeError(f"fsb200 fp8_quantize: format {fmt!r} is not one of {sorted(FP8_FORMATS)}")
+    code, dt = FP8_FORMATS[fmt]
+    rows, cols, ldx = _rows2d(x, "x")
+    y = torch.empty((rows, cols), dtype=dt, device=x.device) if rowwise else None
+    yt = torch.empty((cols, rows), dtype=dt, device=x.device) if colwise else None
+    sinv = torch.empty(2, dtype=torch.float32, device=x.device)   # [scale_inv, amax]
+    L.call("fsb_fp8_quantize", _p(x), ldx, rows, cols, code, _p(y), _p(yt), _p(sinv), _p(sinv[1:]), _stream())
+    return y, yt, sinv[:1]
+
+
+def gemm_fp8(a, a_scale_inv, b, b_scale_inv, out=None, accumulate=False):
+    """out[m, n] (+)= bf16((a[m, k] @ b[n, k]^T) * a_scale_inv * b_scale_inv), fp32 accumulation: a and b contiguous FP8
+    codes as fp8_quantize returns them, (e4m3, e4m3) or (e5m2, e4m3); the scales fp32 [1] device tensors. `out` (bf16, unit
+    inner stride) may be a strided view; `accumulate` adds into it with one rounding."""
+    _chk(a_scale_inv, torch.float32, "a_scale_inv"); _chk(b_scale_inv, torch.float32, "b_scale_inv")
+    for t, name in ((a, "a"), (b, "b")):
+        _chk(t, None, name)
+        if t.dtype not in _FP8_CODE: raise RuntimeError(f"fsb200 gemm_fp8: {name} must hold FP8 codes, got {t.dtype}")
+        if t.dim() != 2 or not t.is_contiguous(): raise RuntimeError(f"fsb200 gemm_fp8: {name} must be contiguous 2-D")
+    m, k = a.shape
+    n = b.shape[0]
+    if b.shape[1] != k: raise RuntimeError(f"fsb200 gemm_fp8: K mismatch {k} vs {b.shape[1]}")
+    if out is None:
+        if accumulate: raise RuntimeError("fsb200 gemm_fp8: accumulate needs an existing `out`")
+        out = torch.empty((m, n), dtype=_bf16, device=a.device)
+    _chk(out, _bf16, "out")
+    orr, occ, ldd = _rows2d(out, "out")
+    if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_fp8: out shape {tuple(out.shape)} != ({m},{n})")
+    L.call("fsb_gemm_fp8", m, n, k, _p(a), _FP8_CODE[a.dtype], _p(a_scale_inv), _p(b), _FP8_CODE[b.dtype], _p(b_scale_inv),
+           _p(out), ldd, int(bool(accumulate)), _stream(),
+           tag=f"{m}x{n}x{k} acc{int(bool(accumulate))}" if L.call_profiler is not None else None)
+    return out
+
+
 def set_reserved_sms(n):
     """Leave n SMs (2n for CTA-pair kernels) of every persistent GEMM grid to overlapping communication kernels."""
     L.call("fsb_set_reserved_sms", int(n))

@@ -130,6 +130,34 @@ size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
                    void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- FP8 training GEMM (opt-in LLaMA precision, `fp8=True`) -------------------------------------------------------
+ * The "hybrid" recipe with just-in-time ("current") per-tensor scaling: activations and weights are e4m3 (largest finite
+ * value 448), gradients e5m2 (57344); accumulation is fp32, outputs bf16.
+ *
+ * fsb_fp8_quantize: x bf16 [rows, cols] (row stride ldx >= cols, a multiple of 8) -> FP8 codes in format `fmt`.
+ *   amax = max |x| over the whole tensor, written to the caller's device fp32 scalar `amax` (scratch and output).
+ *   scale = 2^e with e = floor(log2(fmax / amax)) clamped to [-126, 126], so that scale and 1 / scale are normal fp32 numbers;
+ *   amax == 0 gives scale = 1. code = cvt.rn.satfinite(x * scale): round to nearest even, magnitudes beyond fmax (and inf)
+ *   saturate to +-fmax, NaN stays NaN. scale_inv = 1 / scale, except when amax is not finite (a NaN or inf in x): then
+ *   scale_inv = NaN, so everything computed from the codes is NaN rather than a clipped finite value.
+ *   Outputs, each optional (NULL: not written): y uint8 [rows, cols] row-major contiguous; yt uint8 [cols, rows], the
+ *   transposed codes, contiguous; scale_inv one device fp32. Requirements: rows % 16 == 0 and cols % 16 == 0 (both layouts
+ *   need 16-byte row strides for TMA), x / y / yt 16-byte aligned. Two kernel launches (amax, then cast and transpose) after
+ *   an asynchronous clear of amax; deterministic (the maximum does not depend on order).
+ * fsb_gemm_fp8: D[m, n] = bf16((sum_k A[m, k] B[n, k]) * a_scale_inv * b_scale_inv), the product accumulated in fp32 and
+ *   promoted into a separate fp32 accumulator after every 128 k; with `accumulate`, D[m, n] = bf16(that fp32 value + D[m, n])
+ *   with one rounding. A uint8 codes [m, k] and B uint8 codes [n, k], both contiguous (K-major), as fsb_fp8_quantize writes y
+ *   or yt; a_scale_inv / b_scale_inv: device fp32 scalars (read by the kernel, so a captured graph stays valid). Format pairs
+ *   (a_fmt, b_fmt): (E4M3, E4M3) forward, (E5M2, E4M3) data and weight gradients; any other pair is an error.
+ *   D bf16 [m, n], row stride ldd >= n a multiple of 8. Requirements: k % 16 == 0, n % 8 == 0, a / b / d 16-byte aligned;
+ *   any m >= 1; rows of D at or beyond m and columns beyond n are not written. Persistent 128 x 128 tiles on the SMs that
+ *   fsb_set_reserved_sms leaves to GEMMs, no K-split: deterministic (the result does not depend on the grid). */
+typedef enum { FSB_FP8_E4M3 = 0, FSB_FP8_E5M2 = 1 } fsb_fp8_format;
+int fsb_fp8_quantize(const void* x, int64_t ldx, int64_t rows, int64_t cols, int fmt, void* y, void* yt, float* scale_inv,
+                     float* amax, fsb_stream_t stream);
+int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv, const void* b,
+                 int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, int accumulate, fsb_stream_t stream);
+
 /* ---- RMSNorm / LayerNorm ------------------------------------------------------------------------------------
  * RMSNorm.forward fengshen/models/megatron/layers/norms.py:44-52 (y = scale * cast(x * rsqrt(mean(x^2) + eps)), the cast to
  * 16 bit happening BEFORE the scale multiply); LayerNorm = torch.nn.LayerNorm (norms.py:16; HF BERT/GPT-2 eps 1e-12/1e-5).
