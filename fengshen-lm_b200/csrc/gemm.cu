@@ -1,7 +1,7 @@
 // fsb200 — persistent, warp-specialised bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem -> wgmma (fp32 accumulators in
 // registers) -> fused epilogue -> HBM. Replaces the cuBLAS calls behind F.linear on the reference hot path
 // (fengshen/models/megatron/mpu/layers.py:347-360, :451-470; layers/transformer.py:136-172) and their autograd
-// transposes. One kernel, three operand layouts:
+// transposes. Three operand layouts:
 //   NT  D = A[M,K] B[N,K]^T   both operands K-major          (forward)
 //   NN  D = A[M,K] B[K,N]     B is MN-major in shared memory  (dgrad)
 //   TN  D = A[K,M]^T B[K,N]   A and B MN-major                (wgrad)
@@ -9,13 +9,19 @@
 // the instruction's transpose bit reads them as MN-major.
 //
 // Roles (384 threads = 3 warpgroups): warpgroup 0 = TMA producer (one thread issues; setmaxnreg gives its registers to the
-// others), warpgroups 1-2 = consumers: each owns 64 rows of the 128 x BN tile, issues m64nBNk16 wgmmas on the shared stage
-// and runs the epilogue: bias / activation (and the optional accumulate into D) in registers, then 64-row x 128-byte
-// sub-tiles are written to a double-buffered, 128B-swizzled shared-memory staging area and leave by TMA bulk stores
-// (D and the pre-activation copy alike). The consumer does not wait for a store; it waits only before refilling a staging
-// buffer whose previous store has not yet been read out, so the global writes overlap the next tile's MMAs. Ragged tile
-// edges are clipped by the D / aux tensor maps. The producer runs up to STAGES k-blocks ahead, across tile boundaries, so the
-// next tile's operands stream in during the epilogue. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
+// others), warpgroups 1-2 = consumers. Each consumer accumulates 64 rows x BN columns with m64nBNk16 wgmmas and runs the
+// epilogue: bias / activation (and the optional accumulate into D) in registers, then 64-row x 128-byte sub-tiles are
+// written to a double-buffered, 128B-swizzled shared-memory staging area of its own and leave by TMA bulk stores (D and the
+// pre-activation copy alike). The consumer does not wait for a store; it waits only before refilling a staging buffer whose
+// previous store has not yet been read out. Ragged tile edges are clipped by the D / aux tensor maps. The producer runs up
+// to STAGES k-blocks ahead, across tile boundaries. Grid = min(#tiles, #SMs); static round-robin tile order, grouped for L2.
+// Two schedules (gemm_plan picks one per call; each has its own kernel name):
+//   cooperative (gemm_bf16_kernel): both consumers work on one 128 x BN tile (BN = 128, 192 or 256), 64 rows each, on the
+//     same stages. Long-K and weight-gradient GEMMs.
+//   ping-pong (gemm_bf16_pingpong_kernel): each consumer owns whole 64 x 256 tiles and the two take turns on the tensor
+//     cores, so one's epilogue runs while the other's mainloop issues MMAs. Short-K GEMMs (K <= 1024), whose 128 x 256
+//     epilogue would otherwise leave the tensor cores idle for a visible share of each tile.
+// Both issue the same k16 MMA steps per output element in the same order, so the schedule and tile shape never change a bit.
 // K-split weight-gradient GEMMs carry the split as the batch coordinate of the tile: split s reads its own range of
 // k-blocks of the unbatched operands through full-K tensor maps and writes an fp32 partial product to D[s] (gemm_plan).
 #include "host_common.h"
@@ -45,16 +51,19 @@ struct GemmParams {
 // Shared memory: the operand stages, then the epilogue staging area, two 64-row x 128-byte sub-tile buffers (64 bf16 or 32
 // fp32 columns) per consumer warpgroup. Double-buffered 8 KB sub-tiles rather than a whole-tile buffer keep all 4 (6) operand
 // stages: a 128 x 256 bf16 tile would need 64 KB, i.e. one stage fewer, and the K = 768 GEMMs (12 k-blocks per tile) lean
-// on the producer running far ahead across the tile boundary.
-template <int BN>
+// on the producer running far ahead across the tile boundary. As many stages as fit, at most 6: 4 for 128 x 256, 128 x 192
+// and 64 x 256 tiles, 6 for 128 x 128.
+template <int TM, int BN>
 struct GemmSmem {
-  static constexpr int STAGES = BN == 256 ? 4 : 6;
-  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
+  static constexpr int A_BYTES = TM * GEMM_BK * 2;
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int EPI_BUF_BYTES = 64 * 128;
+  static constexpr int EPI_BYTES = 2 /*warpgroups*/ * 2 /*buffers*/ * EPI_BUF_BYTES;
+  static constexpr int FIT = (kSmemOptIn - 1024 /*align slack*/ - EPI_BYTES - 2 * 6 * 8) / STAGE_BYTES;
+  static constexpr int STAGES = FIT < 6 ? FIT : 6;
   static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = EPI_OFFSET + 2 /*warpgroups*/ * 2 /*buffers*/ * EPI_BUF_BYTES;
+  static constexpr int BAR_OFFSET = EPI_OFFSET + EPI_BYTES;
   // full[STAGES], empty[STAGES]
   static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024 /*align slack*/;
   static_assert(TOTAL <= kSmemOptIn, "exceeds the 227 KB of shared memory a block can opt into on sm_90");
@@ -94,13 +103,21 @@ __device__ __forceinline__ void k_range(const GemmParams& p, int b, int num_kb, 
   }
 }
 
-template <int kLayout, int BN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+// The kernel body. Cooperative (kPP = false): both consumer warpgroups work on one 128 x BN tile, warpgroup wg on rows
+// [64 wg, 64 wg + 64), and every stage is read by both. Ping-pong (kPP = true): each warpgroup owns whole TM x BN tiles, the
+// CTA's even tiles going to warpgroup 0 and its odd tiles to warpgroup 1, and each stage is read by one warpgroup only. The
+// two take turns on the tensor cores: a warpgroup waits for its turn (named barrier 3 + wg), issues its tile's mainloop, and
+// hands the turn over (barrier 3 + other) before it drains its MMAs and runs the epilogue, so one warpgroup's epilogue runs
+// under the other's mainloop. The turn also keeps the ring sound: a warpgroup only waits on its tile's stages once the other
+// has waited on everything before them, so no waiter is ever more than one pass over the ring ahead. The epilogues need no
+// ordering of their own: each warpgroup has its own staging buffers and its own TMA store groups.
+template <int kLayout, int TM, int BN, bool kPP>
+__device__ __forceinline__ void gemm_bf16_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
+                                               const CUtensorMap& tmAux, const GemmParams& p) {
   constexpr bool A_MN = (kLayout == FSB_GEMM_TN);
   constexpr bool B_MN = (kLayout != FSB_GEMM_NT);
-  using S = GemmSmem<BN>;
+  static_assert(TM == (kPP ? 64 : 128), "each warpgroup accumulates 64 rows of the tile");
+  using S = GemmSmem<TM, BN>;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
@@ -114,7 +131,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    ring.init();
+    ring.init(kPP ? 4 : 8);
     fence_barrier_init();
   }
   if (threadIdx.x == 128) {
@@ -124,14 +141,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   __syncthreads();
 
   if (warp < 4) {
-    // ===================== TMA producer =====================
+    // ===================== TMA producer: the CTA's tiles in order, each tile's k-blocks in order =====================
     reg_dec<40>();
     if (threadIdx.x == 0) {
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int b, m_idx, n_idx, kb_lo, kb_hi, ab;
         tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
         k_range(p, b, num_kb, kb_lo, kb_hi, ab);
-        const int m0 = m_idx * GEMM_BM, n0 = n_idx * BN;
+        const int m0 = m_idx * TM, n0 = n_idx * BN;
         for (int kb = kb_lo; kb < kb_hi; ++kb) {
           ring.acquire();
           uint8_t* sa = smem + ring.stage * S::STAGE_BYTES;
@@ -142,7 +159,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             tma_load_3d(sa, &tmA, bar, k0, m0, ab);
           } else {
 #pragma unroll
-            for (int c = 0; c < GEMM_BM / 64; ++c)
+            for (int c = 0; c < TM / 64; ++c)
               tma_load_3d(sa + c * (GEMM_BK * 128), &tmA, bar, m0 + c * 64, k0, ab);
           }
           if constexpr (!B_MN) {
@@ -157,23 +174,31 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   } else {
-    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====================
+    // ===================== consumers =====================
     reg_inc<232>();  // 256 * 232 + 128 * 40 = 64512
     const int wg = (threadIdx.x >> 7) - 1;
     const int wl = warp & 3;
     const bool leader = (threadIdx.x & 127) == 0;   // issues this warpgroup's TMA stores and waits on them
-    // A: K-major -> the warpgroup's 64 rows start 64 * 128 B into the stage; MN-major -> its own 64-wide m chunk
-    const uint64_t dsc_a = A_MN ? make_smem_desc_sw128(smem_u32(smem) + wg * (GEMM_BK * 128), GEMM_BK * 128, 1024)
-                                : make_smem_desc_sw128(smem_u32(smem) + wg * (64 * 128), 0, 1024);
+    // The warpgroup's 64 rows of the stage's A: 64 K-major rows or one 64-wide MN-major chunk, 8 KB either way
+    const uint32_t a_base = smem_u32(smem) + (kPP ? 0 : wg * 8192);
+    const uint64_t dsc_a = A_MN ? make_smem_desc_sw128(a_base, GEMM_BK * 128, 1024) : make_smem_desc_sw128(a_base, 0, 1024);
     const uint64_t dsc_b = B_MN ? make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, GEMM_BK * 128, 1024)
                                 : make_smem_desc_sw128(smem_u32(smem) + S::A_BYTES, 0, 1024);
     uint8_t* const epi_buf = smem + S::EPI_OFFSET + wg * (2 * S::EPI_BUF_BYTES);
     uint32_t n_stored = 0;   // sub-tiles this warpgroup has handed to the TMA unit (selects the staging buffer)
     float acc[BN / 2];
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    int i = kPP ? wg : 0;    // the CTA's i-th tile
+    for (int t = blockIdx.x + i * gridDim.x; t < num_tiles; t += (kPP ? 2 : 1) * gridDim.x, i += kPP ? 2 : 1) {
       int b, m_idx, n_idx, kb_lo, kb_hi, ab;
       tile_coords(t, p.tiles_m, p.tiles_n, p.group_m, b, m_idx, n_idx);
       k_range(p, b, num_kb, kb_lo, kb_hi, ab);
+      if constexpr (kPP) {
+        // every tile has num_kb k-blocks (ping-pong runs no K-split): the tile's first stage is the ring's i * num_kb-th
+        const int64_t pos = int64_t(i) * num_kb;
+        ring.stage = int(pos % S::STAGES);
+        ring.phase = uint32_t(pos / S::STAGES) & 1u;
+        if (i > 0) bar_sync(3 + wg, 256);   // wait for the turn on the tensor cores
+      }
       int prev = 0;
       for (int kb = kb_lo; kb < kb_hi; ++kb) {
         ring.wait();
@@ -184,6 +209,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const uint64_t da = dsc_a + so + ((A_MN ? k * 2048 : k * 32) >> 4), db = dsc_b + so + ((B_MN ? k * 2048 : k * 32) >> 4);
           const uint32_t accum = (kb != kb_lo || k != 0) ? 1u : 0u;
           if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc, da, db, accum);
+          else if constexpr (BN == 192) wgmma_ss_n192<A_MN, B_MN>(acc, da, db, accum);
           else wgmma_ss_n128<A_MN, B_MN>(acc, da, db, accum);
         }
         wgmma_commit();
@@ -192,13 +218,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         prev = ring.stage;
         ring.advance();
       }
+      if constexpr (kPP) {
+        if (t + gridDim.x < num_tiles) bar_arrive(3 + (wg ^ 1), 256);   // the other warpgroup's next tile may start
+      }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       ring.release(prev, lane);
 
       // ---- epilogue: accumulator j covers columns 8 (j / 4) + 2 (lane % 4) + (j & 1), rows r and r + 8 (r = 16 wl + lane / 4)
       const int r = wl * 16 + (lane >> 2);
-      const int m0 = m_idx * GEMM_BM + wg * 64, n0 = n_idx * BN;
+      const int m0 = m_idx * TM + (kPP ? 0 : 64 * wg), n0 = n_idx * BN;
       const int64_t d_off = int64_t(b) * p.stride_d;
       // One 64-row x 128-byte sub-tile: wait until the store that last used this buffer has read it, fill it, make the
       // writes visible to the async proxy, and hand it to the TMA unit. The consumer never waits for a store to land.
@@ -304,37 +333,81 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
+// Two entry points so that profiles tell the schedules apart.
 template <int kLayout, int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+  gemm_bf16_body<kLayout, GEMM_BM, BN, false>(tmA, tmB, tmD, tmAux, p);
+}
+template <int kLayout, int TM, int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                          const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux,
+                          const GemmParams p) {
+  gemm_bf16_body<kLayout, TM, BN, true>(tmA, tmB, tmD, tmAux, p);
+}
+
+template <int kLayout, int TM, int BN, bool kPP>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmAux,
                        const GemmParams& p, cudaStream_t stream) {
-  using S = GemmSmem<BN>;
-  if (int rc = ensure_smem<gemm_bf16_kernel<kLayout, BN>>(S::TOTAL, "gemm")) return rc;
+  using S = GemmSmem<TM, BN>;
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
   const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
-  gemm_bf16_kernel<kLayout, BN><<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
+  if constexpr (kPP) {
+    if (int rc = ensure_smem<gemm_bf16_pingpong_kernel<kLayout, TM, BN>>(S::TOTAL, "gemm")) return rc;
+    gemm_bf16_pingpong_kernel<kLayout, TM, BN><<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
+  } else {
+    if (int rc = ensure_smem<gemm_bf16_kernel<kLayout, BN>>(S::TOTAL, "gemm")) return rc;
+    gemm_bf16_kernel<kLayout, BN><<<grid, GEMM_THREADS, S::TOTAL, stream>>>(tmA, tmB, tmD, tmAux, p);
+  }
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
 
-// Tile width and K-split count. 128 x 256 tiles unless they would leave a large part of the SMs idle (weight-gradient GEMMs
-// of small models: e.g. 768 x 2304 x 32768 is only 54 such tiles) — then 128 x 128 tiles double the parallelism.
-// Plain, unbatched TN GEMMs (weight gradients) whose output has too few tiles to occupy the SMs (e.g. 768 x 768 x 32768:
-// 18 tiles) split K instead: `splits` equal chunks of whole k-blocks, each >= 1024 deep, run as tiles of one launch into an
-// fp32 scratch and are summed in split order (deterministic). Outputs narrower than 256 keep 128 x 128 tiles.
+// Tile shape, schedule and K-split count.
+// - Width: 128 x 256 tiles unless they would leave a large part of the SMs idle (weight-gradient GEMMs of small models: e.g.
+//   768 x 2304 x 32768 is only 54 such tiles); then 128 x 128 tiles double the parallelism.
+// - K-split: plain, unbatched TN GEMMs (weight gradients) whose output has too few tiles to occupy the SMs (e.g.
+//   768 x 768 x 32768: 18 tiles) split K instead: `splits` equal chunks of whole k-blocks, each >= 1024 deep, run as tiles
+//   of one launch into an fp32 scratch and are summed in split order (deterministic). Outputs narrower than 256 keep
+//   128 x 128 tiles.
+// - Ping-pong: an unsplit call that would run 128 x 256 tiles at K <= 1024 runs the ping-pong kernel on 64 x 256 tiles.
+//   Short-K tiles spend a visible share of their time in the epilogue (K = 768: 12 k-blocks), which ping-pong hides under
+//   the other warpgroup's mainloop. Longer K has less epilogue to hide and keeps the cooperative tile, which loads each B
+//   k-block for 128 rows instead of 64. Measured on one H100 80GB HBM3 at 700 W (tools/bench_gemm.py gpt2): 64 x 256
+//   ping-pong took c_fc fwd 0.288 -> 0.253 ms and head fwd 4.98 -> 4.63 ms, but c_fc dgrad (K = 3072) 0.223 -> 0.261 and
+//   c_attn dgrad (K = 2304) 0.178 -> 0.191; 128 x 128 ping-pong tiles (two m64n128 per k16) were no faster at K = 768
+//   (c_fc fwd 0.252, head fwd 4.71 ms) and slower still at K = 3072 (0.304 ms).
+// - Wave-aware width: an unsplit TN call on 128 x 128 tiles whose last wave would be less than half full runs 128 x 192
+//   tiles if that takes fewer waves (c_fc / mlp_proj wgrad of GPT-2 small on 132 SMs: 144 tiles = 2 waves -> 96 tiles = 1).
+// None of these choices changes a result bit: each output element is accumulated by the same k16 MMA steps in the same
+// k-block order, and only the K-split (whose count and boundaries these rules leave alone) regroups the sum.
+constexpr int GEMM_PP_BM = 64;
+constexpr int64_t kPingPongMaxK = 1024;
 struct GemmPlan {
   int bn, splits;
+  bool pingpong;   // ping-pong kernel on GEMM_PP_BM x bn tiles
 };
 static GemmPlan gemm_plan(int layout, int64_t M, int64_t N, int64_t K, int64_t batch, bool plain, int sms) {
-  const int64_t tiles256 = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + 255) / 256) * batch;
+  const int64_t tiles_m = (M + GEMM_BM - 1) / GEMM_BM;
+  const int64_t tiles256 = tiles_m * ((N + 255) / 256) * batch;
   const int bn = (N > 128 && tiles256 * 10 >= int64_t(sms) * 7) ? 256 : 128;
-  if (!(layout == FSB_GEMM_TN && batch == 1 && plain && N % 4 == 0 && (M * N) % 8 == 0 && K >= 4096)) return {bn, 1};
-  const bool wide = N >= 256;
-  const int64_t tiles = ((M + GEMM_BM - 1) / GEMM_BM) * (wide ? (N + 255) / 256 : (N + 127) / 128);
-  int splits = int(sms / tiles);
-  if (splits > 16) splits = 16;
-  while (splits > 1 && (K % (int64_t(splits) * GEMM_BK) != 0 || K / splits < 1024)) --splits;
-  if (splits >= 2 && tiles * 2 <= sms) return {wide ? 256 : bn, splits};
-  return {bn, 1};
+  if (layout == FSB_GEMM_TN && batch == 1 && plain && N % 4 == 0 && (M * N) % 8 == 0 && K >= 4096) {
+    const bool wide = N >= 256;
+    const int64_t tiles = tiles_m * (wide ? (N + 255) / 256 : (N + 127) / 128);
+    int splits = int(sms / tiles);
+    if (splits > 16) splits = 16;
+    while (splits > 1 && (K % (int64_t(splits) * GEMM_BK) != 0 || K / splits < 1024)) --splits;
+    if (splits >= 2 && tiles * 2 <= sms) return {wide ? 256 : bn, splits, false};
+  }
+  if (bn == 256 && K <= kPingPongMaxK) return {256, 1, true};
+  if (bn == 128 && layout == FSB_GEMM_TN && N > 128) {
+    const int64_t tiles128 = tiles_m * ((N + 127) / 128) * batch, tiles192 = tiles_m * ((N + 191) / 192) * batch;
+    const int64_t last = tiles128 % sms;
+    if (last != 0 && last * 2 < sms && (tiles192 + sms - 1) / sms < (tiles128 + sms - 1) / sms) return {192, 1, false};
+  }
+  return {bn, 1, false};
 }
 
 // D (bf16 / fp32, optionally accumulated into) = sum over the K-splits of the fp32 partial products, in a fixed order
@@ -366,8 +439,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
 static int gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                      int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                      int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, int bn = 0,
-                     int ksplits = 1);
+                     int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, const GemmPlan& plan);
 
 }  // namespace fsb
 
@@ -408,7 +480,7 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
     float* ws = static_cast<float*>(workspace);
     // split s: k-blocks k_range(s) of the whole (unbatched) A / B -> fp32 partial ws[s] (M x N, ld N)
     int rc = gemm_impl(layout, M, N, K, A, lda, B, ldb, ws, N, FSB_F32, nullptr, FSB_BF16, FSB_EPI_NONE, 0, nullptr, 0,
-                       splits, 0, 0, M * N, 0, stream, plan.bn, splits);
+                       splits, 0, 0, M * N, 0, stream, GemmPlan{plan.bn, splits, false});
     if (rc) return rc;
     const int64_t work = M * (N / 4);
     const int blocks = int(work / 256 + 1 < 2 * num_sms() ? work / 256 + 1 : 2 * num_sms());
@@ -417,14 +489,15 @@ extern "C" int fsb_gemm_bf16(int layout, int64_t M, int64_t N, int64_t K, const 
     return FSB_OK;
   }
   return gemm_impl(layout, M, N, K, A, lda, B, ldb, D, ldd, d_dtype, bias, bias_dtype, epilogue, accumulate, aux, ldaux, batch,
-                   stride_a, stride_b, stride_d, stride_aux, stream, plan.bn, 1);
+                   stride_a, stride_b, stride_d, stride_aux, stream, plan);
 }
 
 static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda, const void* B,
                           int64_t ldb, void* D, int64_t ldd, int d_dtype, const void* bias, int bias_dtype,
                           int epilogue, int accumulate, void* aux, int64_t ldaux, int64_t batch, int64_t stride_a,
-                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream, int bn,
-                          int ksplits) {
+                          int64_t stride_b, int64_t stride_d, int64_t stride_aux, cudaStream_t stream,
+                          const GemmPlan& plan) {
+  const int ksplits = plan.splits;
   FSB_REQUIRE(layout >= 0 && layout <= 2, "gemm: bad layout %d", layout);
   FSB_REQUIRE(M > 0 && N > 0 && K > 0 && batch > 0, "gemm: non-positive dims M=%ld N=%ld K=%ld batch=%ld", (long)M,
               (long)N, (long)K, (long)batch);
@@ -451,13 +524,13 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   // Tensor maps: always rank 3 (inner, outer, batch). A K-split GEMM reads unbatched operands and writes D[split].
   CUtensorMap tmA, tmB, tmD, tmAux;
   const bool a_mn = (layout == FSB_GEMM_TN), b_mn = (layout != FSB_GEMM_NT);
-  const int BN = bn ? bn : gemm_plan(layout, M, N, K, batch, false, gemm_sms()).bn;
+  const int BN = plan.bn, TM = plan.pingpong ? GEMM_PP_BM : GEMM_BM;
   const int64_t ab = ksplits > 1 ? 1 : batch;
   {
     // A: K-major -> memory [M rows, K inner]; MN-major -> memory [K rows, M inner]
     uint64_t dims[3] = {uint64_t(a_mn ? M : K), uint64_t(a_mn ? K : M), uint64_t(ab)};
     uint64_t strides[2] = {uint64_t(lda) * 2, uint64_t(ab > 1 ? stride_a : (a_mn ? K : M) * lda) * 2};
-    uint32_t box[3] = {64, uint32_t(a_mn ? GEMM_BK : GEMM_BM), 1};
+    uint32_t box[3] = {64, uint32_t(a_mn ? GEMM_BK : TM), 1};
     int rc = make_tmap_bf16(&tmA, A, 3, dims, strides, box);
     if (rc) return rc;
   }
@@ -492,23 +565,26 @@ static int fsb::gemm_impl(int layout, int64_t M, int64_t N, int64_t K, const voi
   p.d_f32 = (d_dtype == FSB_F32); p.bias_f32 = (bias_dtype == FSB_F32);
   p.epilogue = epilogue; p.accumulate = accumulate;
   p.ksplits = ksplits;
-  p.tiles_m = int((M + GEMM_BM - 1) / GEMM_BM);
+  p.tiles_m = int((M + TM - 1) / TM);
   p.tiles_n = int((N + BN - 1) / BN);
   // Rasterisation: tiles are walked m-fastest inside groups of group_m m-tiles, so one wave of CTAs touches group_m A panels
-  // and #SMs/group_m B panels. HBM traffic per wave is least when both sides weigh about the same (group_m ~ sqrt(#SMs * BN/BM):
-  // 16 for 256-wide tiles, 12 for 128-wide ones); the group only grows beyond that while its A panels (group_m x 128 x K bf16)
-  // stay well inside the L2 (~32 MB of its 50 MB).
+  // and #SMs/group_m B panels. HBM traffic per wave is least when both sides weigh about the same (group_m ~ sqrt(#SMs * BN/TM):
+  // 16 for 128 x 256 tiles, 12 for 128 x 128 and 128 x 192, 24 for 64 x 256); the group only grows beyond that while its A
+  // panels (group_m x TM x K bf16) stay well inside the L2 (~32 MB of its 50 MB).
   {
-    const int64_t a_panel = int64_t(GEMM_BM) * (K / ksplits) * 2;
-    const int64_t base = BN == 256 ? 16 : 12;
+    const int64_t a_panel = int64_t(TM) * (K / ksplits) * 2;
+    const int64_t base = TM == 64 ? 24 : (BN == 256 ? 16 : 12);
     int64_t gm = (int64_t(32) << 20) / a_panel;
     gm = gm < base ? base : (gm > 64 ? 64 : gm);
     p.group_m = int(gm);
   }
 
-#define FSB_GEMM_DISPATCH(L) \
-  case L:                    \
-    return BN == 256 ? launch_gemm<L, 256>(tmA, tmB, tmD, tmAux, p, stream) : launch_gemm<L, 128>(tmA, tmB, tmD, tmAux, p, stream);
+#define FSB_GEMM_DISPATCH(L)                                                                                              \
+  case L:                                                                                                                 \
+    if (plan.pingpong) return launch_gemm<L, GEMM_PP_BM, 256, true>(tmA, tmB, tmD, tmAux, p, stream);                    \
+    if (BN == 256) return launch_gemm<L, GEMM_BM, 256, false>(tmA, tmB, tmD, tmAux, p, stream);                           \
+    if (BN == 192 && L == FSB_GEMM_TN) return launch_gemm<FSB_GEMM_TN, GEMM_BM, 192, false>(tmA, tmB, tmD, tmAux, p, stream); \
+    return launch_gemm<L, GEMM_BM, 128, false>(tmA, tmB, tmD, tmAux, p, stream);
   switch (layout) {
     FSB_GEMM_DISPATCH(FSB_GEMM_NT)
     FSB_GEMM_DISPATCH(FSB_GEMM_NN)
