@@ -571,6 +571,7 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
                           o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
   if (drop != nullptr) {
     p.drop = *drop;
+    if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, true) : FSB_BWD(64, true, true);
     return head_dim == 128 ? FSB_BWD(128, false, true) : FSB_BWD(64, false, true);
   }
   if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, false) : FSB_BWD(64, true, false);
@@ -608,7 +609,7 @@ extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v,
   DropArgs d;
   if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
   if (p > 0.f) {
-    FSB_REQUIRE(!causal && rel_bias == nullptr, "sdpa_bwd_dropout: causal masks and rel_bias are not supported with p > 0");
+    FSB_REQUIRE(!causal, "sdpa_bwd_dropout: the causal flag is not supported with p > 0; fold the mask into rel_bias");
     FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536, "sdpa_bwd_dropout: sequences longer than 65536 are not supported with p > 0");
   }
   return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,

@@ -8,7 +8,7 @@
 //   embedding   : VocabParallelEmbedding.forward mpu/layers.py:104-130 (+ learned position / token-type rows for
 //                 BERT / GPT-2: transformers bert/modeling_bert.py:53-112, gpt2/modeling_gpt2.py wte+wpe)
 //   add         : residual adds layers/transformer.py:775-788
-//   dropout     : y = x * Z / (1 - p) with the hidden-dropout mask of philox.cuh (BERT / MegatronBERT embedding sites)
+//   dropout     : y = x * Z / (1 - p) with the hidden-dropout mask of philox.cuh (BERT / MegatronBERT / mT5 embedding sites)
 #include "host_common.h"
 #include "philox.cuh"
 #include "ptx.cuh"
@@ -99,13 +99,17 @@ __device__ __forceinline__ float dact_f(float x) {
 }
 
 // out[t, c] = act(gate[t, c]) * up[t, c]; gate/up/out have independent row strides (elements).
-template <int ACT>
+// kDrop: out[t, c] = act(gate[t, c]) * up[t, c] * Z / (1 - p), Z the hidden-dropout mask of philox.cuh at (t, c) of out; the
+// backward applies the same mask to dout first (MT5DenseGatedActDense's dropout between the product and wo).
+template <int ACT, bool kDrop>
 __global__ void __launch_bounds__(256) glu_fwd_kernel(const __nv_bfloat16* __restrict__ gate,
                                                       const __nv_bfloat16* __restrict__ up,
                                                       __nv_bfloat16* __restrict__ out, int64_t rows, int cols,
-                                                      int64_t ld_gate, int64_t ld_up, int64_t ld_out) {
+                                                      int64_t ld_gate, int64_t ld_up, int64_t ld_out, const DropArgs drop) {
   const int vpr = cols >> 3;
   const int64_t total = rows * vpr;
+  uint32_t s_lo, s_hi;
+  drop_stream<kDrop>(drop.stream_base, drop.site, s_lo, s_hi);
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t t = i / vpr;
     const int c = int(i % vpr) * 8;
@@ -114,23 +118,27 @@ __global__ void __launch_bounds__(256) glu_fwd_kernel(const __nv_bfloat16* __res
     unpack8(*reinterpret_cast<const uint4*>(up + t * ld_up + c), u);
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = act_f<ACT>(g[j]) * u[j];
+    if constexpr (kDrop) apply_keep8(keep_bits8(drop.seed, s_lo, s_hi, drop.thr, int(t), c >> 3), drop.keep_scale, o);
     *reinterpret_cast<uint4*>(out + t * ld_out + c) = pack8(o);
   }
 }
-template <int ACT>
+template <int ACT, bool kDrop>
 __global__ void __launch_bounds__(256) glu_bwd_kernel(const __nv_bfloat16* __restrict__ dout,
                                                       const __nv_bfloat16* __restrict__ gate,
                                                       const __nv_bfloat16* __restrict__ up,
                                                       __nv_bfloat16* __restrict__ dgate, __nv_bfloat16* __restrict__ dup,
                                                       int64_t rows, int cols, int64_t ld_dout, int64_t ld_gate,
-                                                      int64_t ld_up, int64_t ld_dgate, int64_t ld_dup) {
+                                                      int64_t ld_up, int64_t ld_dgate, int64_t ld_dup, const DropArgs drop) {
   const int vpr = cols >> 3;
   const int64_t total = rows * vpr;
+  uint32_t s_lo, s_hi;
+  drop_stream<kDrop>(drop.stream_base, drop.site, s_lo, s_hi);
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t t = i / vpr;
     const int c = int(i % vpr) * 8;
     float d[8], g[8], u[8], og[8], ou[8];
     unpack8(*reinterpret_cast<const uint4*>(dout + t * ld_dout + c), d);
+    if constexpr (kDrop) apply_keep8(keep_bits8(drop.seed, s_lo, s_hi, drop.thr, int(t), c >> 3), drop.keep_scale, d);
     unpack8(*reinterpret_cast<const uint4*>(gate + t * ld_gate + c), g);
     unpack8(*reinterpret_cast<const uint4*>(up + t * ld_up + c), u);
 #pragma unroll
@@ -496,36 +504,73 @@ extern "C" int fsb_rope_inplace(void* x, const float* cos_table, const float* si
   return FSB_OK;
 }
 
-extern "C" int fsb_glu_fwd(int act, const void* gate, const void* up, void* out, int64_t rows, int64_t cols,
-                           int64_t ld_gate, int64_t ld_up, int64_t ld_out, fsb_stream_t st) {
+static int glu_fwd(int act, const void* gate, const void* up, void* out, int64_t rows, int64_t cols, int64_t ld_gate,
+                   int64_t ld_up, int64_t ld_out, const DropArgs* drop, cudaStream_t st) {
   FSB_REQUIRE(act >= 0 && act <= 2, "glu_fwd: bad act %d", act);
   FSB_REQUIRE(gate && up && out && rows > 0 && cols > 0 && cols % 8 == 0, "glu_fwd: bad args");
   FSB_REQUIRE(ld_gate % 8 == 0 && ld_up % 8 == 0 && ld_out % 8 == 0 && aligned16(gate) && aligned16(up) && aligned16(out),
               "glu_fwd: alignment");
   const int g = ew_grid(rows * (cols / 8), 256);
-#define L(A) glu_fwd_kernel<A><<<g, 256, 0, (cudaStream_t)st>>>((const __nv_bfloat16*)gate, (const __nv_bfloat16*)up, \
-                                                               (__nv_bfloat16*)out, rows, int(cols), ld_gate, ld_up, ld_out)
-  if (act == 0) L(0); else if (act == 1) L(1); else L(2);
+#define L(A, D) glu_fwd_kernel<A, D><<<g, 256, 0, st>>>((const __nv_bfloat16*)gate, (const __nv_bfloat16*)up,       \
+                                                        (__nv_bfloat16*)out, rows, int(cols), ld_gate, ld_up, ld_out, \
+                                                        drop ? *drop : DropArgs{})
+  if (drop != nullptr) {
+    if (act == 0) L(0, true); else if (act == 1) L(1, true); else L(2, true);
+  } else {
+    if (act == 0) L(0, false); else if (act == 1) L(1, false); else L(2, false);
+  }
 #undef L
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
-extern "C" int fsb_glu_bwd(int act, const void* dout, const void* gate, const void* up, void* dgate, void* dup,
-                           int64_t rows, int64_t cols, int64_t ld_dout, int64_t ld_gate, int64_t ld_up,
-                           int64_t ld_dgate, int64_t ld_dup, fsb_stream_t st) {
+static int glu_bwd(int act, const void* dout, const void* gate, const void* up, void* dgate, void* dup, int64_t rows,
+                   int64_t cols, int64_t ld_dout, int64_t ld_gate, int64_t ld_up, int64_t ld_dgate, int64_t ld_dup,
+                   const DropArgs* drop, cudaStream_t st) {
   FSB_REQUIRE(act >= 0 && act <= 2, "glu_bwd: bad act %d", act);
   FSB_REQUIRE(dout && gate && up && dgate && dup && rows > 0 && cols > 0 && cols % 8 == 0, "glu_bwd: bad args");
   FSB_REQUIRE((ld_dout | ld_gate | ld_up | ld_dgate | ld_dup) % 8 == 0 && aligned16(dout) && aligned16(gate) &&
                   aligned16(up) && aligned16(dgate) && aligned16(dup),
               "glu_bwd: alignment");
   const int g = ew_grid(rows * (cols / 8), 256);
-#define L(A) glu_bwd_kernel<A><<<g, 256, 0, (cudaStream_t)st>>>(                                                    \
+#define L(A, D) glu_bwd_kernel<A, D><<<g, 256, 0, st>>>(                                                           \
       (const __nv_bfloat16*)dout, (const __nv_bfloat16*)gate, (const __nv_bfloat16*)up, (__nv_bfloat16*)dgate,       \
-      (__nv_bfloat16*)dup, rows, int(cols), ld_dout, ld_gate, ld_up, ld_dgate, ld_dup)
-  if (act == 0) L(0); else if (act == 1) L(1); else L(2);
+      (__nv_bfloat16*)dup, rows, int(cols), ld_dout, ld_gate, ld_up, ld_dgate, ld_dup, drop ? *drop : DropArgs{})
+  if (drop != nullptr) {
+    if (act == 0) L(0, true); else if (act == 1) L(1, true); else L(2, true);
+  } else {
+    if (act == 0) L(0, false); else if (act == 1) L(1, false); else L(2, false);
+  }
 #undef L
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
+}
+extern "C" int fsb_glu_fwd(int act, const void* gate, const void* up, void* out, int64_t rows, int64_t cols,
+                           int64_t ld_gate, int64_t ld_up, int64_t ld_out, fsb_stream_t st) {
+  return glu_fwd(act, gate, up, out, rows, cols, ld_gate, ld_up, ld_out, nullptr, (cudaStream_t)st);
+}
+extern "C" int fsb_glu_bwd(int act, const void* dout, const void* gate, const void* up, void* dgate, void* dup,
+                           int64_t rows, int64_t cols, int64_t ld_dout, int64_t ld_gate, int64_t ld_up,
+                           int64_t ld_dgate, int64_t ld_dup, fsb_stream_t st) {
+  return glu_bwd(act, dout, gate, up, dgate, dup, rows, cols, ld_dout, ld_gate, ld_up, ld_dgate, ld_dup, nullptr,
+                 (cudaStream_t)st);
+}
+extern "C" int fsb_glu_fwd_dropout(int act, const void* gate, const void* up, void* out, int64_t rows, int64_t cols,
+                                   int64_t ld_gate, int64_t ld_up, int64_t ld_out, float p, uint64_t seed,
+                                   const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p > 0.f) FSB_REQUIRE(rows <= 0x7fffffffll, "glu_fwd_dropout: more than 2^31 - 1 rows with p > 0");
+  return glu_fwd(act, gate, up, out, rows, cols, ld_gate, ld_up, ld_out, p > 0.f ? &d : nullptr, (cudaStream_t)st);
+}
+extern "C" int fsb_glu_bwd_dropout(int act, const void* dout, const void* gate, const void* up, void* dgate, void* dup,
+                                   int64_t rows, int64_t cols, int64_t ld_dout, int64_t ld_gate, int64_t ld_up,
+                                   int64_t ld_dgate, int64_t ld_dup, float p, uint64_t seed, const int64_t* stream_base,
+                                   int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p > 0.f) FSB_REQUIRE(rows <= 0x7fffffffll, "glu_bwd_dropout: more than 2^31 - 1 rows with p > 0");
+  return glu_bwd(act, dout, gate, up, dgate, dup, rows, cols, ld_dout, ld_gate, ld_up, ld_dgate, ld_dup,
+                 p > 0.f ? &d : nullptr, (cudaStream_t)st);
 }
 extern "C" int fsb_act_fwd(int act, const void* x, void* y, int64_t n, fsb_stream_t st) {
   FSB_REQUIRE(act >= 0 && act <= 3 && x && y && n > 0 && n % 8 == 0 && aligned16(x) && aligned16(y), "act_fwd: bad args");

@@ -10,7 +10,7 @@
 // Weight gradients: every thread accumulates fp32 partials over its rows; the CTA combines its RPC row slots through
 // shared memory in a fixed order and writes partial[cta, cols]; a second kernel reduces the partials column-wise
 // (deterministic, no atomics).
-// Dropout on the branch (kDrop, LayerNorm with a residual only): the forward computes x_sum = x * Z / (1 - p) + residual, Z the
+// Dropout on the branch (kDrop, with a residual only): the forward computes x_sum = x * Z / (1 - p) + residual, Z the
 // hidden-dropout mask of philox.cuh at (row, col); the backward also writes dbranch = dx * Z / (1 - p) — the gradient of the
 // dropped branch beside the gradient of the sum.
 #include <stdlib.h>
@@ -29,35 +29,9 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// x (8 columns 8 c .. 8 c + 7 of `row`) *= Z / (1 - p). One Philox call covers 16 columns; this vector uses half of it.
-// Everything arrives by value: the seed, threshold and scale straight from the kernel parameters (constant bank), the stream
-// from the one load each thread makes before its row loop — no copy of the parameter struct is ever addressed.
-__device__ __forceinline__ uint32_t keep_bits8(uint64_t seed, uint32_t s_lo, uint32_t s_hi, uint32_t thr, int row, int c) {
-  const DropKey k{uint32_t(seed), uint32_t(seed >> 32), s_lo, s_hi, thr};
-  const uint4 r = drop_hidden_bits(k, uint32_t(row), uint32_t(c >> 1));
-  const uint32_t w0 = (c & 1) ? r.z : r.x, w1 = (c & 1) ? r.w : r.y;
-  uint32_t bits = 0;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) bits |= uint32_t(drop_keep(j < 4 ? w0 : w1, j & 3, thr)) << j;
-  return bits;
-}
-__device__ __forceinline__ void apply_keep8(uint32_t bits, float keep_scale, float (&x)[8]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) x[j] = (bits >> j) & 1u ? x[j] * keep_scale : 0.f;
-}
-// dropout on LayerNorm rows is instantiated up to this many 8-column vectors per thread (cols <= 12288): wider rows already
+// dropout on norm rows is instantiated up to this many 8-column vectors per thread (cols <= 12288): wider rows already
 // spill in the dropout-free backward
 constexpr int NORM_DROP_MAX_VPT = 6;
-// the stream number s = *stream_base + site of a dropout site, split in halves (0 without dropout: nothing is read)
-template <bool kDrop>
-__device__ __forceinline__ void drop_stream(const int64_t* stream_base, int64_t site, uint32_t& s_lo, uint32_t& s_hi) {
-  s_lo = s_hi = 0;
-  if constexpr (kDrop) {
-    const uint64_t s = uint64_t(*stream_base + site);
-    s_lo = uint32_t(s);
-    s_hi = uint32_t(s >> 32);
-  }
-}
 
 // Sum of (a, b) over the TPR threads that share a row; result broadcast to those threads.
 // red: [RPC][2][TPR/32] floats of shared memory. Every thread of the CTA must call (contains __syncthreads).
@@ -505,4 +479,38 @@ extern "C" int fsb_layernorm_bwd_dropout(const void* dy, const void* x, const vo
               8 * 256 * NORM_DROP_MAX_VPT);
   return norm_bwd<true, true>(dy, x, gamma, mean_rstd, dres, dx, dgamma, dbeta, wgrad_dtype, accumulate, workspace,
                               workspace_bytes, rows, cols, (cudaStream_t)st, dbranch, d);
+}
+extern "C" int fsb_rmsnorm_fwd_dropout(const void* x, const void* residual, const void* scale, void* y, void* sum_out,
+                                       float* rstd, int64_t rows, int64_t cols, float eps, float p, uint64_t seed,
+                                       const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  if (p == 0.f) return norm_fwd<false>(x, residual, scale, nullptr, y, sum_out, rstd, rows, cols, eps, (cudaStream_t)st);
+  FSB_REQUIRE(residual != nullptr, "rmsnorm_fwd_dropout: the dropped branch needs a residual");
+  FSB_REQUIRE(cols <= 8 * 256 * NORM_DROP_MAX_VPT, "rmsnorm_fwd_dropout: cols %ld > %d with p > 0", (long)cols,
+              8 * 256 * NORM_DROP_MAX_VPT);
+  return norm_fwd<false, true>(x, residual, scale, nullptr, y, sum_out, rstd, rows, cols, eps, (cudaStream_t)st, d);
+}
+extern "C" int fsb_rmsnorm_bwd_dropout(const void* dy, const void* x, const void* scale, const float* rstd, const void* dres,
+                                       void* dx, void* dbranch, void* dscale, int wgrad_dtype, int accumulate, void* workspace,
+                                       size_t workspace_bytes, int64_t rows, int64_t cols, float p, uint64_t seed,
+                                       const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(dbranch != nullptr && aligned16(dbranch), "rmsnorm_bwd_dropout: dbranch must be a 16-byte aligned buffer");
+  if (p == 0.f) {   // no mask: the branch gradient is the gradient of the sum
+    if (int rc = norm_bwd<false>(dy, x, scale, rstd, dres, dx, dscale, nullptr, wgrad_dtype, accumulate, workspace,
+                                 workspace_bytes, rows, cols, (cudaStream_t)st))
+      return rc;
+    cudaError_t e = cudaMemcpyAsync(dbranch, dx, size_t(rows) * size_t(cols) * 2, cudaMemcpyDeviceToDevice, (cudaStream_t)st);
+    if (e != cudaSuccess) {
+      set_error("rmsnorm_bwd_dropout: copy of dx failed: %s", cudaGetErrorString(e));
+      return FSB_ERR_CUDA;
+    }
+    return FSB_OK;
+  }
+  FSB_REQUIRE(cols <= 8 * 256 * NORM_DROP_MAX_VPT, "rmsnorm_bwd_dropout: cols %ld > %d with p > 0", (long)cols,
+              8 * 256 * NORM_DROP_MAX_VPT);
+  return norm_bwd<false, true>(dy, x, scale, rstd, dres, dx, dscale, nullptr, wgrad_dtype, accumulate, workspace,
+                               workspace_bytes, rows, cols, (cudaStream_t)st, dbranch, d);
 }

@@ -59,6 +59,35 @@ __device__ __forceinline__ uint4 drop_hidden_bits(const DropKey& k, uint32_t row
   return philox4x32_10(make_uint4(col16, row, k.s_lo, k.s_hi), k.k0, k.k1);
 }
 
+// The hidden-layout keep bits of the 8 columns 8 c .. 8 c + 7 of `row` (bit j: column 8 c + j). One Philox call covers 16
+// columns; this vector uses half of it. Everything arrives by value: the seed, threshold and scale straight from the kernel
+// parameters (constant bank), the stream from the one load each thread makes before its loop — no copy of the parameter
+// struct is ever addressed.
+__device__ __forceinline__ uint32_t keep_bits8(uint64_t seed, uint32_t s_lo, uint32_t s_hi, uint32_t thr, int row, int c) {
+  const DropKey k{uint32_t(seed), uint32_t(seed >> 32), s_lo, s_hi, thr};
+  const uint4 r = drop_hidden_bits(k, uint32_t(row), uint32_t(c >> 1));
+  const uint32_t w0 = (c & 1) ? r.z : r.x, w1 = (c & 1) ? r.w : r.y;
+  uint32_t bits = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) bits |= uint32_t(drop_keep(j < 4 ? w0 : w1, j & 3, thr)) << j;
+  return bits;
+}
+// x *= Z / (1 - p) over the 8 columns of keep_bits8
+__device__ __forceinline__ void apply_keep8(uint32_t bits, float keep_scale, float (&x)[8]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) x[j] = (bits >> j) & 1u ? x[j] * keep_scale : 0.f;
+}
+// the stream number s = *stream_base + site of a dropout site, split in halves (0 without dropout: nothing is read)
+template <bool kDrop>
+__device__ __forceinline__ void drop_stream(const int64_t* stream_base, int64_t site, uint32_t& s_lo, uint32_t& s_hi) {
+  s_lo = s_hi = 0;
+  if constexpr (kDrop) {
+    const uint64_t s = uint64_t(*stream_base + site);
+    s_lo = uint32_t(s);
+    s_hi = uint32_t(s >> 32);
+  }
+}
+
 // Attention dropout, element (b, head, q, k), with q = 16 qa + 8 qh + 2 qs + qp and k = 16 ka + 8 kh + 2 ks + kp:
 // counter ((ka * 4 + ks) | (qa * 4 + qs) << 16, b * nheads + head, stream lo, stream hi); word 2 qp + kp, byte 2 qh + kh.
 // One call covers the 4 x 4 block q in {16 qa + 2 qs + {0, 1, 8, 9}}, k likewise. In the wgmma accumulator layout a thread owns

@@ -60,21 +60,22 @@ class GatedMLP:
     def __init__(self, wi, wo, act):
         self.wi, self.wo, self.act = wi, wo, act
 
-    def __call__(self, h, save=True):
-        """-> (m, what the backward reads; with save=False, only what a forward needs is computed)."""
+    def __call__(self, h, save=True, drop=None):
+        """-> (m, what the backward reads; with save=False, only what a forward needs is computed). drop: optional
+        ops.Dropout on act(gate) * up, the input of wo (mT5's dropout inside the FFN)."""
         gu, hs = self.wi.forward(h, save)
         f = gu.shape[1] // 2
-        act = ops.glu_fwd(self.act, gu[:, :f], gu[:, f:])
+        act = ops.glu_fwd(self.act, gu[:, :f], gu[:, f:], drop=drop)
         m, acts = self.wo.forward(act, save)
         return m, (hs, gu, acts)
 
-    def backward(self, dm, saved, accumulate):
-        """-> the gradient of h; writes the weight gradients as Linear.backward does."""
+    def backward(self, dm, saved, accumulate, drop=None):
+        """-> the gradient of h; writes the weight gradients as Linear.backward does. drop: the forward's Dropout."""
         hs, gu, act = saved
         f = gu.shape[1] // 2
         dact = self.wo.backward(dm, act, accumulate)
         dgu = torch.empty_like(gu)
-        ops.glu_bwd(self.act, dact, gu[:, :f], gu[:, f:], dgu[:, :f], dgu[:, f:])
+        ops.glu_bwd(self.act, dact, gu[:, :f], gu[:, f:], dgu[:, :f], dgu[:, f:], drop=drop)
         return self.wi.backward(dgu, hs, accumulate)
 
 

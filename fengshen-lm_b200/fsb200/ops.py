@@ -250,14 +250,19 @@ def set_profiler(p):
 
 
 # ------------------------------------------------------------------------------------------------------ norms
-def rmsnorm_fwd(x, scale, eps, residual=None):
-    """x [rows, cols] bf16. Returns (y, rstd, x_sum) where x_sum = x + residual (or x itself when residual is None)."""
+def rmsnorm_fwd(x, scale, eps, residual=None, drop=None):
+    """x [rows, cols] bf16. Returns (y, rstd, x_sum) where x_sum = x + residual (or x itself when residual is None).
+    drop: optional Dropout (see `Dropout`): x_sum = dropout(x) + residual (the dropped branch of a residual block)."""
     _chk(x, _bf16, "x"); _chk(scale, _bf16, "scale")
     rows, cols = x.shape
     y = torch.empty_like(x)
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
     xs = torch.empty_like(x) if residual is not None else None
-    L.call("fsb_rmsnorm_fwd", _p(x), _p(residual), _p(scale), _p(y), _p(xs), _p(rstd), rows, cols, float(eps), _stream())
+    if drop is None:
+        L.call("fsb_rmsnorm_fwd", _p(x), _p(residual), _p(scale), _p(y), _p(xs), _p(rstd), rows, cols, float(eps), _stream())
+    else:
+        L.call("fsb_rmsnorm_fwd_dropout", _p(x), _p(residual), _p(scale), _p(y), _p(xs), _p(rstd), rows, cols, float(eps),
+               *drop.args(), _stream())
     return y, rstd, (xs if residual is not None else x)
 
 
@@ -270,6 +275,20 @@ def rmsnorm_bwd(dy, x, scale, rstd, dscale_out, accumulate=False, dres=None):
            L.F32 if dscale_out.dtype == torch.float32 else L.BF16, int(bool(accumulate)), _p(ws), ws.numel(), rows, cols,
            _stream())
     return dx
+
+
+def rmsnorm_bwd_dropout(dy, x, scale, rstd, dscale_out, drop, accumulate=False, dres=None):
+    """Backward of rmsnorm_fwd(..., residual, drop): returns (dx, dbranch) — the gradient of the sum (= of the residual)
+    and the gradient of the dropped branch, dx * Z / (1 - p)."""
+    rows, cols = x.shape
+    dx = torch.empty_like(x)
+    dbranch = torch.empty_like(x)
+    nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 0)
+    ws = workspace(nbytes, x.device, "norm")
+    L.call("fsb_rmsnorm_bwd_dropout", _p(dy), _p(x), _p(scale), _p(rstd), _p(dres), _p(dx), _p(dbranch), _p(dscale_out),
+           L.F32 if dscale_out.dtype == torch.float32 else L.BF16, int(bool(accumulate)), _p(ws), ws.numel(), rows, cols,
+           *drop.args(), _stream())
+    return dx, dbranch
 
 
 def layernorm_fwd(x, gamma, beta, eps, residual=None, drop=None):
@@ -360,22 +379,30 @@ def rope_inplace(x, cos, sin, positions, nheads, head_dim, row_stride, head_stri
            row_stride, head_stride, cos.shape[0], int(bool(backward)), _stream())
 
 
-def glu_fwd(act, gate, up):
+def glu_fwd(act, gate, up, drop=None):
+    """out = act(gate) * up; drop: optional Dropout on out (out * Z / (1 - p))."""
     rows, cols, ldg = _rows2d(gate, "gate")
     _, _, ldu = _rows2d(up, "up")
     out = torch.empty((rows, cols), dtype=_bf16, device=gate.device)
-    L.call("fsb_glu_fwd", act, _p(gate), _p(up), _p(out), rows, cols, ldg, ldu, cols, _stream())
+    if drop is None:
+        L.call("fsb_glu_fwd", act, _p(gate), _p(up), _p(out), rows, cols, ldg, ldu, cols, _stream())
+    else:
+        L.call("fsb_glu_fwd_dropout", act, _p(gate), _p(up), _p(out), rows, cols, ldg, ldu, cols, *drop.args(), _stream())
     return out
 
 
-def glu_bwd(act, dout, gate, up, dgate, dup):
+def glu_bwd(act, dout, gate, up, dgate, dup, drop=None):
+    """drop: the forward's Dropout (the mask is applied to dout first)."""
     rows, cols, ldg = _rows2d(gate, "gate")
     _, _, ldu = _rows2d(up, "up")
     _, _, ldo = _rows2d(dout, "dout")
     _, _, ldg2 = _rows2d(dgate, "dgate")
     _, _, ldu2 = _rows2d(dup, "dup")
-    L.call("fsb_glu_bwd", act, _p(dout), _p(gate), _p(up), _p(dgate), _p(dup), rows, cols, ldo, ldg, ldu, ldg2, ldu2,
-           _stream())
+    args = (act, _p(dout), _p(gate), _p(up), _p(dgate), _p(dup), rows, cols, ldo, ldg, ldu, ldg2, ldu2)
+    if drop is None:
+        L.call("fsb_glu_bwd", *args, _stream())
+    else:
+        L.call("fsb_glu_bwd_dropout", *args, *drop.args(), _stream())
 
 
 def act_fwd(act, x):
@@ -515,7 +542,8 @@ def _chk_rel(rel, H, Sq, Skv, name):
 def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop=None):
     """q,k,v: strided [B,S,H,D] bf16 views (e.g. slices of the packed QKV projection). Returns (out [B,Sq,H,D], lse).
     rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias over the offset k - q (T5 relative-position bias).
-    drop: optional Dropout on the attention probabilities (not with causal or rel_bias when p > 0)."""
+    drop: optional Dropout on the attention probabilities. With p > 0 causal must be False: a causal rel_bias (-inf at
+    offsets k - q > 0) expresses the same mask."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")

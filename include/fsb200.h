@@ -315,7 +315,7 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
                  float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                  void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
-/* ---- dropout (BERT / MegatronBERT training) -------------------------------------------------------------------------
+/* ---- dropout (BERT / MegatronBERT / mT5 training) -------------------------------------------------------------------
  * torch.nn.functional.dropout semantics: an element is dropped with probability p and every kept element is scaled by
  * 1 / (1 - p). The keep bit is a pure function of (seed, stream, coordinates) through Philox4x32-10 (Random123; key =
  * (seed & 0xffffffff, seed >> 32)), so no mask is stored: the backward kernels regenerate it.
@@ -329,11 +329,16 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
  *               counter ((4 ka + ks) | (4 qa + qs) << 16, b * nheads + head, s & 0xffffffff, s >> 32); r = byte 2 qh + kh of
  *               output word 2 qp + kp. seq_q, seq_kv <= 65536.
  * fsb_sdpa_fwd_dropout / fsb_sdpa_bwd_dropout: fsb_sdpa_fwd / fsb_sdpa_bwd with dropout on the attention probabilities,
- *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. With p > 0, causal and
- *   rel_bias are rejected. The backward must get the forward's seed, stream_base value and site.
+ *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. rel_bias composes with
+ *   dropout; with p > 0 the causal flag is rejected: fold the causal mask into rel_bias instead (-inf at offsets k - q > 0,
+ *   as T5's decoder adds its causal mask to the position bias). The backward must get the forward's seed, stream_base value
+ *   and site.
  * fsb_layernorm_fwd_dropout: fsb_layernorm_fwd with sum_out = x * Z / (1 - p) + residual (residual required when p > 0): the
  *   dropped branch of a residual block. With p > 0 both LayerNorm entries take cols <= 12288. fsb_layernorm_bwd_dropout: fsb_layernorm_bwd that also writes dbranch = dx * Z / (1 - p)
  *   (dx already includes dres), the gradient of the branch x, beside dx, the gradient of the sum (and of the residual).
+ * fsb_rmsnorm_fwd_dropout / fsb_rmsnorm_bwd_dropout: the same contract over fsb_rmsnorm_fwd / fsb_rmsnorm_bwd.
+ * fsb_glu_fwd_dropout: fsb_glu_fwd with out = act(gate) * up * Z / (1 - p), Z the hidden mask at (row, col) of out
+ *   (rows < 2^31 when p > 0). fsb_glu_bwd_dropout: fsb_glu_bwd with the same mask applied to dout first.
  * fsb_dropout: y = x * Z / (1 - p) over bf16 [rows, cols] (cols % 8 == 0, rows < 2^32); also the backward (dx = dy * Z / (1 - p)).
  *   x == y is allowed.
  * fsb_dropout_advance: *saved = *stream_base; *stream_base += n (one thread on the device). A training forward calls it once
@@ -361,6 +366,19 @@ int fsb_layernorm_bwd_dropout(const void* dy, const void* x, const void* gamma, 
                               void* dx, void* dbranch, void* dgamma, void* dbeta, int wgrad_dtype, int accumulate,
                               void* workspace, size_t workspace_bytes, int64_t rows, int64_t cols,
                               float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_rmsnorm_fwd_dropout(const void* x, const void* residual, const void* scale, void* y, void* sum_out, float* rstd,
+                            int64_t rows, int64_t cols, float eps,
+                            float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_rmsnorm_bwd_dropout(const void* dy, const void* x, const void* scale, const float* rstd, const void* dres, void* dx,
+                            void* dbranch, void* dscale, int wgrad_dtype, int accumulate, void* workspace,
+                            size_t workspace_bytes, int64_t rows, int64_t cols,
+                            float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_glu_fwd_dropout(int act, const void* gate, const void* up, void* out, int64_t rows, int64_t cols, int64_t ld_gate,
+                        int64_t ld_up, int64_t ld_out,
+                        float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_glu_bwd_dropout(int act, const void* dout, const void* gate, const void* up, void* dgate, void* dup, int64_t rows,
+                        int64_t cols, int64_t ld_dout, int64_t ld_gate, int64_t ld_up, int64_t ld_dgate, int64_t ld_dup,
+                        float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
 int fsb_dropout(const void* x, void* y, int64_t rows, int64_t cols, float p, uint64_t seed, const int64_t* stream_base,
                 int64_t site, fsb_stream_t stream);
 int fsb_dropout_advance(int64_t* stream_base, int64_t* saved, int64_t n, fsb_stream_t stream);
