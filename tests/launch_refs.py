@@ -15,9 +15,15 @@ sum|terms| is used (`_sum_close` there). A K-deep fp32 dot product is bounded by
 test_fp8_gpu / test_int8_gpu.
 """
 import math
+from typing import NamedTuple
 
+import numpy as np
 import torch
 
+import fp8_ref
+import int4_ref
+import int8_ref
+import philox_ref
 from guards import bf16_ulp, bits
 
 U16 = 2.0 ** -8
@@ -73,6 +79,74 @@ def _chunks(n, bytes_per_item):
 def _ulp_tol(ref, dtype):
     """The storage rounding of a value computed in fp32: 1 bf16 ulp, or 2 u32 relative for an fp32 result."""
     return bf16_ulp(ref) if dtype == BF16 else 2 * U32 * ref.abs()
+
+
+# ----------------------------------------------------------------------------------------------------------- dropout
+class DropSpec(NamedTuple):
+    """What a dropout mask is a function of (include/fsb200.h): the rate, the model's seed and the stream number
+    s = *stream_base + site."""
+    p: float
+    seed: int
+    stream: int
+
+
+def drop_spec(drop):
+    """The DropSpec of an ops.Dropout: its base is read from the device."""
+    return None if drop is None else DropSpec(drop.p, drop.seed, int(drop.base.item()) + drop.site)
+
+
+def keep_scale(p):
+    """1 / (1 - p) as the kernels form it: fp32 p, fp32 subtraction and IEEE division (philox.cuh make_drop_args)."""
+    one = torch.tensor(1.0, dtype=F32)
+    return float(one / (one - torch.tensor(p, dtype=F32)))
+
+
+def hidden_mult(d, rows, cols, device):
+    """Z / (1 - p) of the hidden layout for the rows in range `rows`: fp64 [len(rows), cols] (0 where dropped)."""
+    keep = philox_ref.hidden_keep_t(d.seed, d.stream, rows, cols, d.p, device)
+    return keep.double() * keep_scale(d.p)
+
+
+def attn_mult(d, batches, nheads, seq_q, seq_kv, device):
+    """Z / (1 - p) of the attention layout for the batch rows in range `batches`: fp64 [nb, nheads, seq_q, seq_kv]."""
+    keep = philox_ref.attn_keep_t(d.seed, d.stream, batches, nheads, seq_q, seq_kv, d.p, device)
+    return keep.double() * keep_scale(d.p)
+
+
+def _range(sl):
+    return range(sl.start, sl.stop)
+
+
+def verify_dropout(bound, x, d, out):
+    """out = bf16(fp32(x) * fp32(1 / (1 - p))) where the hidden mask keeps, +0 where it drops: one fp32 product rounded
+    once, bit for bit."""
+    rows, cols = x.shape
+    ks = torch.tensor(keep_scale(d.p), dtype=F32)
+    for rs in _chunks(rows, cols * 8 * 6):
+        keep = philox_ref.hidden_keep_t(d.seed, d.stream, _range(rs), cols, d.p, x.device)
+        want = torch.where(keep, x[rs].float() * ks.to(x.device), torch.zeros((), dtype=F32, device=x.device)).to(BF16)
+        bound.exact("x * Z / (1 - p)", out[rs], want)
+
+
+def check_dropout(real, bound, x, drop, out=None):
+    x0 = x.clone() if out is not None else x        # out may alias x
+    d = drop_spec(drop)
+    ret = real(x, drop, out=out)
+    verify_dropout(bound, x0, d, ret)
+    return ret
+
+
+def verify_dropout_advance(bound, old, n, saved, counter):
+    """saved = the old counter and counter = old + n, exactly."""
+    bound.equal("saved stream base", saved.reshape(-1).cpu(), torch.tensor([old]))
+    bound.equal("advanced counter", counter.reshape(-1).cpu(), torch.tensor([old + n]))
+
+
+def check_dropout_advance(real, bound, counter, n):
+    old = int(counter.item())
+    saved = real(counter, n)
+    verify_dropout_advance(bound, old, int(n), saved, counter)
+    return saved
 
 
 # ------------------------------------------------------------------------------------------------------- activations
@@ -179,18 +253,25 @@ def _sum_tol(abs_sum, ref, dtype):
     return tol + bf16_ulp(ref) if dtype == BF16 else tol
 
 
-def verify_norm_fwd(bound, layer, x, residual, w, beta, eps, y, stats, xsum):
-    """x_sum = bf16(x + residual): the fp32 sum of two bf16 values rounded once, compared bit for bit.
+def verify_norm_fwd(bound, layer, x, residual, w, beta, eps, y, stats, xsum, drop=None):
+    """x_sum = bf16(x + residual): the fp32 sum of two bf16 values rounded once, compared bit for bit. With dropout (a
+    DropSpec) x_sum = bf16(t + residual), t = fp32(x * fp32(1 / (1 - p))) where the hidden mask keeps and 0 where it drops
+    (norm.cu's apply_keep8 before the add), bit for bit.
     Statistics against fp64 on x_sum: rstd within 1e-5 relative (rsqrtf, 2 ulp, and a per-row fp32 sum of at most
     8 VPT + log2 TPR <= 72 levels: (72 u32 / 2 + 2^-22) < 1e-5); LayerNorm's mean within 72 u32 mean|x| + 1e-30.
     RMSNorm: y = bf16(bf16(x rstd) * scale) with the kernel's rstd, bit for bit (norms.py casts before the scale multiply).
     LayerNorm: y = bf16((x - mean) rstd gamma + beta) with the kernel's statistics: four fp32 roundings, 2^-22
     (|xhat gamma| + |beta|), and 1 ulp."""
     rows, cols = x.shape
-    if residual is not None:
-        bound.exact("x + residual", xsum, (x.float() + residual.float()).to(BF16))
     xs = xsum
     for rs in _chunks(rows, cols * 8 * 10):
+        if residual is not None:
+            xf = x[rs].float()
+            if drop is not None:
+                keep = philox_ref.hidden_keep_t(drop.seed, drop.stream, _range(rs), cols, drop.p, x.device)
+                ks = torch.tensor(keep_scale(drop.p), dtype=F32, device=x.device)
+                xf = torch.where(keep, xf * ks, torch.zeros((), dtype=F32, device=x.device))
+            bound.exact("x + residual", xsum[rs], (xf + residual[rs].float()).to(BF16))
         xd = xs[rs].double()
         if layer:
             mean_g, rstd_g = stats[rs, 0].double(), stats[rs, 1].double()
@@ -211,27 +292,27 @@ def verify_norm_fwd(bound, layer, x, residual, w, beta, eps, y, stats, xsum):
 
 
 def check_rmsnorm_fwd(real, bound, x, scale, eps, residual=None, drop=None):
-    if drop is not None:
-        raise AssertionError("rmsnorm_fwd with dropout has no launch reference (the benchmark step runs at p = 0)")
-    y, rstd, xs = ret = real(x, scale, eps, residual=residual)
-    verify_norm_fwd(bound, False, x, residual, scale, None, eps, y, rstd, xs)
+    d = drop_spec(drop)
+    y, rstd, xs = ret = real(x, scale, eps, residual=residual, drop=drop)
+    verify_norm_fwd(bound, False, x, residual, scale, None, eps, y, rstd, xs, d)
     return ret
 
 
 def check_layernorm_fwd(real, bound, x, gamma, beta, eps, residual=None, drop=None):
-    if drop is not None:
-        raise AssertionError("layernorm_fwd with dropout has no launch reference (the benchmark step runs at p = 0)")
-    y, stats, xs = ret = real(x, gamma, beta, eps, residual=residual)
-    verify_norm_fwd(bound, True, x, residual, gamma, beta, eps, y, stats, xs)
+    d = drop_spec(drop)
+    y, stats, xs = ret = real(x, gamma, beta, eps, residual=residual, drop=drop)
+    verify_norm_fwd(bound, True, x, residual, gamma, beta, eps, y, stats, xs, d)
     return ret
 
 
-def verify_norm_bwd(bound, layer, dy, x, w, stats, dres, dx, dw, dw_old, db=None, db_old=None):
+def verify_norm_bwd(bound, layer, dy, x, w, stats, dres, dx, dw, dw_old, db=None, db_old=None, drop=None, dbranch=None):
     """With the forward's statistics (the call's own operands): xhat = (x - mean) rstd, g = dy w,
     dx = rstd (g - [mean(g)] - xhat mean(g xhat)) (+ dres), rounded once: 1 ulp plus test_layer_ops_gpu's floor
     1e-5 max_row |rstd (g - ...)| for the fp32 row sums inside the means.
     dw = sum_rows dy * xhat (RMSNorm: dy * bf16(x rstd), the rounded value the forward multiplied), db = sum_rows dy, each
-    (+ the old value when accumulating): ACC_REL of sum|terms| (+ 1 ulp in bf16)."""
+    (+ the old value when accumulating): ACC_REL of sum|terms| (+ 1 ulp in bf16).
+    With dropout (a DropSpec): dbranch = bf16(dx32 Z / (1 - p)) from the kernel's unrounded fp32 dx (norm.cu applies the
+    mask after dx is stored): M = Z / (1 - p) times dx's bound, plus 1 ulp of the product."""
     rows, cols = x.shape
     wd = w.double()
     gw = torch.zeros(cols, dtype=torch.float64, device=x.device)
@@ -253,7 +334,11 @@ def verify_norm_bwd(bound, layer, dy, x, w, stats, dres, dx, dw, dw_old, db=None
             core = core - g.mean(1, keepdim=True)
         core = rstd * core
         ref = core + (dres[rs].double() if dres is not None else 0.0)
-        bound.close("dx", dx[rs], ref, 1e-5 * core.abs().amax(1, keepdim=True) + bf16_ulp(ref))
+        tol = 1e-5 * core.abs().amax(1, keepdim=True) + bf16_ulp(ref)
+        bound.close("dx", dx[rs], ref, tol)
+        if drop is not None:
+            m = hidden_mult(drop, _range(rs), cols, x.device)
+            bound.close("dbranch", dbranch[rs], m * ref, m * tol + bf16_ulp(m * ref))
         t = dyd * xw
         gw += t.sum(0); aw += t.abs().sum(0)
         if layer:
@@ -271,6 +356,24 @@ def check_rmsnorm_bwd(real, bound, dy, x, scale, rstd, dscale_out, accumulate=Fa
     dx = real(dy, x, scale, rstd, dscale_out, accumulate=accumulate, dres=dres)
     verify_norm_bwd(bound, False, dy, x, scale, rstd, dres, dx, dscale_out, old)
     return dx
+
+
+def check_rmsnorm_bwd_dropout(real, bound, dy, x, scale, rstd, dscale_out, drop, accumulate=False, dres=None):
+    old = dscale_out.clone() if accumulate else None
+    d = drop_spec(drop)
+    dx, dbr = ret = real(dy, x, scale, rstd, dscale_out, drop, accumulate=accumulate, dres=dres)
+    verify_norm_bwd(bound, False, dy, x, scale, rstd, dres, dx, dscale_out, old, drop=d, dbranch=dbr)
+    return ret
+
+
+def check_layernorm_bwd_dropout(real, bound, dy, x, gamma, stats, dgamma_out, dbeta_out, drop, accumulate=False,
+                                dres=None):
+    og = dgamma_out.clone() if accumulate else None
+    ob = dbeta_out.clone() if accumulate else None
+    d = drop_spec(drop)
+    dx, dbr = ret = real(dy, x, gamma, stats, dgamma_out, dbeta_out, drop, accumulate=accumulate, dres=dres)
+    verify_norm_bwd(bound, True, dy, x, gamma, stats, dres, dx, dgamma_out, og, dbeta_out, ob, drop=d, dbranch=dbr)
+    return ret
 
 
 def check_layernorm_bwd(real, bound, dy, x, gamma, stats, dgamma_out, dbeta_out, accumulate=False, dres=None):
@@ -315,39 +418,50 @@ def check_rope_inplace(real, bound, x, cos, sin, positions, nheads, head_dim, ro
 
 
 # ------------------------------------------------------------------------------------------------------ activations
-def verify_glu_fwd(bound, act, gate, up, out):
-    """out = act(gate) * up rounded once: 1 ulp plus ACT_FLOOR |up|."""
-    for rs in _chunks(gate.shape[0], gate.shape[1] * 8 * 10):
+def verify_glu_fwd(bound, act, gate, up, out, drop=None):
+    """out = act(gate) * up rounded once: 1 ulp plus ACT_FLOOR |up|. With dropout (a DropSpec) the fp32 product is
+    multiplied by M = Z / (1 - p) of the hidden layout before the rounding: M ACT_FLOOR |up| plus 2 u32 |ref| for the extra
+    fp32 product."""
+    cols = gate.shape[1]
+    for rs in _chunks(gate.shape[0], cols * 8 * 12):
         g, u = gate[rs].double(), up[rs].double()
         ref = act64(act, g) * u
-        bound.close("out", out[rs], ref, bf16_ulp(ref) + ACT_FLOOR * u.abs())
+        tol = ACT_FLOOR * u.abs()
+        if drop is not None:
+            m = hidden_mult(drop, _range(rs), cols, gate.device)
+            ref, tol = ref * m, tol * m + 2 * U32 * (ref * m).abs()
+        bound.close("out", out[rs], ref, bf16_ulp(ref) + tol)
 
 
 def check_glu_fwd(real, bound, act, gate, up, drop=None):
-    if drop is not None:
-        raise AssertionError("glu_fwd with dropout has no launch reference (the benchmark step runs at p = 0)")
-    out = real(act, gate, up)
-    verify_glu_fwd(bound, act, gate, up, out)
+    d = drop_spec(drop)
+    out = real(act, gate, up, drop=drop)
+    verify_glu_fwd(bound, act, gate, up, out, d)
     return out
 
 
-def verify_glu_bwd(bound, act, dout, gate, up, dgate, dup):
+def verify_glu_bwd(bound, act, dout, gate, up, dgate, dup, drop=None):
     """dgate = dout * up * act'(gate), dup = dout * act(gate), each rounded once: 1 ulp plus ACT_FLOOR |dout up| and
-    ACT_FLOOR |dout|."""
-    for rs in _chunks(gate.shape[0], gate.shape[1] * 8 * 16):
+    ACT_FLOOR |dout|. With dropout (a DropSpec) dout is first multiplied by M = Z / (1 - p) in fp32 (elementwise.cu):
+    the same bounds on M dout, plus 2 u32 |ref| for that product."""
+    cols = gate.shape[1]
+    for rs in _chunks(gate.shape[0], cols * 8 * 18):
         d, g, u = dout[rs].double(), gate[rs].double(), up[rs].double()
+        extra = 0.0
+        if drop is not None:
+            d = d * hidden_mult(drop, _range(rs), cols, gate.device)
+            extra = 2 * U32
         rg = d * u * dact64(act, g)
         ru = d * act64(act, g)
-        bound.close("dgate", dgate[rs], rg, bf16_ulp(rg) + ACT_FLOOR * (d * u).abs())
-        bound.close("dup", dup[rs], ru, bf16_ulp(ru) + ACT_FLOOR * d.abs())
+        bound.close("dgate", dgate[rs], rg, bf16_ulp(rg) + ACT_FLOOR * (d * u).abs() + extra * rg.abs())
+        bound.close("dup", dup[rs], ru, bf16_ulp(ru) + ACT_FLOOR * d.abs() + extra * ru.abs())
 
 
 def check_glu_bwd(real, bound, act, dout, gate, up, dgate, dup, drop=None):
-    if drop is not None:
-        raise AssertionError("glu_bwd with dropout has no launch reference (the benchmark step runs at p = 0)")
     d0, g0, u0 = dout.clone(), gate.clone(), up.clone()     # dgate / dup may overwrite them
-    ret = real(act, dout, gate, up, dgate, dup)
-    verify_glu_bwd(bound, act, d0, g0, u0, dgate, dup)
+    d = drop_spec(drop)
+    ret = real(act, dout, gate, up, dgate, dup, drop=drop)
+    verify_glu_bwd(bound, act, d0, g0, u0, dgate, dup, d)
     return ret
 
 
@@ -684,18 +798,22 @@ def _bhsd(t):
 def _scores(q, k, scale, causal, kv_mask, rel_bias, bs):
     """fp64 scores [nb, H, Sq, Skv] in natural-log units (masked: -inf) and the fp32 score error e_s of each: the D-deep
     fp32 dot product, D 2^-23 scale (|q||k|), plus 2^-22 (|scale q.k| + |bias|) for the scale, the bias fma and the
-    conversion to the log2 domain."""
+    conversion to the log2 domain. A -inf bias (T5's causal mask folded into rel_bias under dropout) masks its position like
+    kv_mask does: score -inf, error 0."""
     qd, kd = _bhsd(q[bs]).double(), _bhsd(k[bs]).double()
     D, Sq, Skv = q.shape[3], q.shape[1], k.shape[1]
     s = scale * (qd @ kd.transpose(-1, -2))
     e = D * 2.0 ** -23 * scale * (qd.abs() @ kd.abs().transpose(-1, -2)) + 2.0 ** -22 * s.abs()
+    keep = torch.ones((1, 1, Sq, Skv), dtype=torch.bool, device=q.device)
     if rel_bias is not None:
         qi = torch.arange(Sq, device=q.device)[:, None]
         ki = torch.arange(Skv, device=q.device)[None, :]
         bias = rel_bias.double()[:, ki - qi + Sq - 1]           # [H, Sq, Skv]
+        fin = torch.isfinite(bias)                              # a folded causal mask: -inf, p = 0 and no error there
+        bias = torch.where(fin, bias, 0.0)
         s = s + bias
         e = e + 2.0 ** -22 * bias.abs()
-    keep = torch.ones((1, 1, Sq, Skv), dtype=torch.bool, device=q.device)
+        keep = keep & fin[None]
     if causal:
         keep = keep & torch.ones((Sq, Skv), dtype=torch.bool, device=q.device).tril()
     if kv_mask is not None:
@@ -717,23 +835,29 @@ def _softmax(s):
 
 def _batch_chunks(q, k):
     B, Sq, H, _ = q.shape
-    return _chunks(B, H * Sq * k.shape[1] * 8 * 14)
+    return _chunks(B, H * Sq * k.shape[1] * 8 * 16)
 
 
-def verify_sdpa_fwd(bound, q, k, v, scale, causal, kv_mask, rel_bias, out, lse):
+def verify_sdpa_fwd(bound, q, k, v, scale, causal, kv_mask, rel_bias, out, lse, drop=None):
     """O = softmax(scale q k^T + bias) V. The kernel rounds each unnormalised probability exp2(x - m) <= 1 to bf16 before
     the PV MMA and O once at the end, dividing by the fp32 sum of the unrounded probabilities. With the per-row score error
     E = max_k e_s (see _scores) + (2 + Skv / 64) 2^-22 (ex2.approx per probability and per online-softmax rescale), each
     probability is within E relative before the bf16 rounding, so
     |O - O_ref| <= (u16 + 2 E + Skv 2^-23) (P |V|) + 1 ulp(O) (u16 for the rounded P, 2 E through numerator and
     denominator, the Skv-deep fp32 PV accumulation). P |V| <= max|V|: the issue's 2^-8 max|V| + 1 ulp, per element.
-    lse (log2 domain) within (E + 2^-22 (1 + |lse|)) / ln 2. Rows with no key attended: O = 0, lse = +inf."""
+    lse (log2 domain) within (E + 2^-22 (1 + |lse|)) / ln 2. Rows with no key attended: O = 0, lse = +inf.
+    With dropout (a DropSpec): O = (P M) V, M = Z / (1 - p) of the attention layout; the kernel multiplies each fp32
+    probability by the fp32 1 / (1 - p) before the bf16 rounding (2^-23 more in E); the lse is that of the undropped P."""
+    B, Sq, H, _ = q.shape
     Skv = k.shape[1]
     ln2 = math.log(2.0)
     for bs in _batch_chunks(q, k):
         s, e, keep = _scores(q, k, scale, causal, kv_mask, rel_bias, bs)
         p, lse_ref = _softmax(s)
         E = e.amax(-1, keepdim=True) + (2 + Skv / 64) * 2.0 ** -22
+        if drop is not None:
+            p = p * attn_mult(drop, _range(bs), H, Sq, Skv, q.device)
+            E = E + 2.0 ** -23
         vd = _bhsd(v[bs]).double()
         ref = p @ vd
         mag = p @ vd.abs()
@@ -747,10 +871,9 @@ def verify_sdpa_fwd(bound, q, k, v, scale, causal, kv_mask, rel_bias, out, lse):
 
 
 def check_sdpa_fwd(real, bound, q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop=None):
-    if drop is not None:
-        raise AssertionError("sdpa_fwd with dropout has no launch reference (the benchmark step runs at p = 0)")
-    o, lse = ret = real(q, k, v, scale, causal, kv_mask=kv_mask, out=out, rel_bias=rel_bias)
-    verify_sdpa_fwd(bound, q, k, v, scale, causal, kv_mask, rel_bias, o, lse)
+    d = drop_spec(drop)
+    o, lse = ret = real(q, k, v, scale, causal, kv_mask=kv_mask, out=out, rel_bias=rel_bias, drop=drop)
+    verify_sdpa_fwd(bound, q, k, v, scale, causal, kv_mask, rel_bias, o, lse, d)
     return ret
 
 
@@ -766,7 +889,7 @@ def _diag_sums(m, Sq):
 
 
 def verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None,
-                    drel_bias=None, drel_old=None):
+                    drel_bias=None, drel_old=None, drop=None):
     """The exact gradients of O = softmax(scale q k^T + bias) V for the given dO, in fp64: dV = P^T dO, dS = P (dP - delta)
     with dP = dO V^T and delta = rowsum(dO O), dQ = scale dS K, dK = scale dS^T Q, dbias[h, r] += sum over (b, q) of dS on
     diagonal r.
@@ -776,7 +899,10 @@ def verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, k
     the call's own operands). Hence the fp32 dS is within E = P (eps_P |dP - delta| + (1 + eps_P)(e_dP + e_delta)).
     dQ, dK multiply bf16(dS) (u16 relative): |dQ - ref| <= scale ((u16 + Skv 2^-23)(|dS| + E) + E) |K| + 1 ulp, dK the
     same with Sq and |Q|; dV multiplies bf16(P): ((1 + u16)(eps_P + u16) + Sq 2^-23) P^T |dO| + 1 ulp. dbias sums the fp32
-    dS: diagonal sums of E + B Sq 2^-23 |dS|, plus 2 u32 |dbias| for the add onto the old value."""
+    dS: diagonal sums of E + B Sq 2^-23 |dS|, plus 2 u32 |dbias| for the add onto the old value.
+    With dropout (a DropSpec, M = Z / (1 - p)): O = (P M) V, so dV = (P M)^T dO and dS = P (M dP - delta), delta still
+    rowsum(dO O) of the dropped O (attention_bwd.cu multiplies dP by the fp32 M before subtracting delta): the bounds above
+    with P M in dV's and M dP, M e_dP in dS's, and 2^-23 more in eps_P for the fp32 products with 1 / (1 - p)."""
     B, Sq, H, D = q.shape
     Skv = k.shape[1]
     ln2 = math.log(2.0)
@@ -788,16 +914,19 @@ def verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, k
         del s
         vd, dod, qd, kd = (_bhsd(t[bs]).double() for t in (v, dout, q, k))
         od = _bhsd(out[bs]).double()
-        o_ref = p @ vd
+        m = None if drop is None else attn_mult(drop, _range(bs), H, Sq, Skv, q.device)
+        o_ref = (p if m is None else p * m) @ vd
         delta = (dod * o_ref).sum(-1, keepdim=True)
         e_delta = (dod.abs() * (od - o_ref).abs()).sum(-1, keepdim=True) + D * 2.0 ** -23 * (dod * od).abs().sum(-1, keepdim=True)
         del o_ref
         lg = lse[bs].double()
         dl = torch.where(torch.isfinite(lse_ref), (lg * ln2 - lse_ref).abs(), torch.zeros_like(lse_ref))
-        eps_p = (dl[..., None] + e.amax(-1, keepdim=True) + 3 * 2.0 ** -22)
+        eps_p = (dl[..., None] + e.amax(-1, keepdim=True) + 3 * 2.0 ** -22 + (0.0 if m is None else 2.0 ** -23))
         del e
         dP = dod @ vd.transpose(-1, -2)
         e_dp = D * 2.0 ** -23 * (dod.abs() @ vd.abs().transpose(-1, -2))
+        if m is not None:
+            dP, e_dp = dP * m, e_dp * m
         dS = p * (dP - delta)
         E = p * (eps_p * (dP - delta).abs() + (1 + eps_p) * (e_dp + e_delta))
         del dP, e_dp
@@ -808,8 +937,11 @@ def verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, k
         ref = scale * (dS.transpose(-1, -2) @ qd)
         tol = scale * (((U16 + Sq * 2.0 ** -23) * (aS + E) + E).transpose(-1, -2) @ qd.abs()) + bf16_ulp(ref)
         bound.close("dK", _bhsd(dk[bs]), ref, tol)
-        ref = p.transpose(-1, -2) @ dod
-        w = ((1 + U16) * (eps_p + U16) + Sq * 2.0 ** -23) * p
+        pm = p if m is None else p * m
+        del m
+        ref = pm.transpose(-1, -2) @ dod
+        w = ((1 + U16) * (eps_p + U16) + Sq * 2.0 ** -23) * pm
+        del pm
         tol = w.transpose(-1, -2) @ dod.abs() + bf16_ulp(ref)
         bound.close("dV", _bhsd(dv[bs]), ref, tol)
         if dsum is not None:
@@ -825,11 +957,242 @@ def verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, k
 
 def check_sdpa_bwd(real, bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None,
                    drel_bias=None, drop=None):
-    if drop is not None:
-        raise AssertionError("sdpa_bwd with dropout has no launch reference (the benchmark step runs at p = 0)")
     old = None if drel_bias is None else drel_bias.clone()
-    ret = real(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=kv_mask, rel_bias=rel_bias, drel_bias=drel_bias)
-    verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, old)
+    d = drop_spec(drop)
+    ret = real(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=kv_mask, rel_bias=rel_bias, drel_bias=drel_bias,
+               drop=drop)
+    verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, old, d)
+    return ret
+
+
+# ------------------------------------------------------------------------------------------------ weight-only int8 / int4
+def verify_quantize_w8(bound, w, q, s):
+    """q and s bit for bit as int8_ref.quantize (the numpy float32 restatement of include/fsb200.h) gives them."""
+    n, k = w.shape
+    for rs in _chunks(n, k * 4 * 8):
+        qn, sn = int8_ref.quantize(w[rs].float().cpu().numpy())
+        bound.equal("int8 codes", q[rs].cpu(), torch.from_numpy(qn))
+        bound.equal("row scales (bits)", s[rs].cpu().view(torch.int32), torch.from_numpy(sn).view(torch.int32))
+
+
+def check_quantize_w8(real, bound, w, q=None, s=None):
+    ret = real(w, q=q, s=s)
+    verify_quantize_w8(bound, w, *ret)
+    return ret
+
+
+def verify_quantize_w4(bound, w, q, s):
+    """The packed codes and the bf16 group scales bit for bit as int4_ref.quantize and int4_ref.pack give them."""
+    n, k = w.shape
+    for rs in _chunks(n // 2, 2 * k * 4 * 8):
+        rows = slice(2 * rs.start, 2 * rs.stop)
+        qn, sn = int4_ref.quantize(w[rows].float().cpu().numpy())
+        bound.equal("packed int4 codes", q[rs].cpu(), torch.from_numpy(int4_ref.pack(qn)))
+        bound.exact("group scales", s[rows].cpu(), torch.from_numpy(sn).to(BF16))
+
+
+def check_quantize_w4(real, bound, w, q=None, s=None):
+    ret = real(w, q=q, s=s)
+    verify_quantize_w4(bound, w, *ret)
+    return ret
+
+
+def unpack_w4(q, s):
+    """W^ = bf16(q * s) [n, k] from the packed codes and the group scales (int4_ref.unpack / dequantize in torch, so it
+    runs on the operands' device)."""
+    p2, k = q.shape
+    b = q.reshape(p2, k // 16, 4, 2, 2).to(torch.int16)                        # [p, block, t, b, h]
+    u = torch.stack([b & 0xF, b >> 4], -1) - 8                                 # [p, block, t, b, h, row]
+    codes = u.permute(0, 5, 1, 4, 2, 3).reshape(2 * p2, k)
+    return (codes.float() * s.float().repeat_interleave(int4_ref.GROUP, 1)).to(BF16)
+
+
+def _verify_scaled_gemm(bound, what, a64_of, b64_of, m, n, k, out, old=None, acc_rel=None):
+    """out[m, n] = bf16(A B^T (+ old)), fp32 accumulation of exact products: 2^-8 |ref| for the rounding (and the scale
+    products), K 2^-23 (|A||B|^T) for the accumulation, 2 u32 |old| for the add (test_fp8_gpu / test_int8_gpu's bound).
+    `acc_rel` replaces K 2^-23 where the accumulation is not plain fp32."""
+    for cs in _chunks(n, 8 * 2 * k):
+        B64 = b64_of(cs)
+        Babs = B64.abs()
+        for rs in _chunks(m, 8 * (2 * k + 6 * (cs.stop - cs.start))):
+            A64 = a64_of(rs)
+            ref = A64 @ B64.t()
+            tol = (k * 2.0 ** -23 if acc_rel is None else acc_rel) * (A64.abs() @ Babs.t())
+            del A64
+            if old is not None:
+                o = old[rs, cs].double()
+                ref, tol = ref + o, tol + 2 * U32 * o.abs()
+            bound.close(what, out[rs, cs], ref, tol + 2.0 ** -8 * ref.abs())
+            del ref, tol
+        del B64, Babs
+
+
+def verify_gemm_w8a16(bound, a, q, s, out):
+    """out = bf16(s[n] (A q^T)): the fp64 product with the dequantised weight q s, at the bound of test_int8_gpu."""
+    m, k = a.shape
+    _verify_scaled_gemm(bound, "W8A16 D", lambda rs: a[rs].double(), lambda cs: q[cs].double() * s[cs].double()[:, None],
+                        m, q.shape[0], k, out)
+
+
+def check_gemm_w8a16(real, bound, a, q, s, out=None):
+    ret = real(a, q, s, out=out)
+    verify_gemm_w8a16(bound, a, q, s, ret)
+    return ret
+
+
+def verify_gemm_w4a16(bound, a, q, s, out):
+    """out = bf16(A W^T), W^ = bf16(q s) the dequantised int4 weight: fp64 over W^ at the bound of test_int4_gpu."""
+    m, k = a.shape
+    n = 2 * q.shape[0]
+
+    def b64(cs):
+        lines = slice(cs.start // 2, (cs.stop + 1) // 2)
+        w = unpack_w4(q[lines], s[2 * lines.start:2 * lines.stop]).double()
+        return w[cs.start - 2 * lines.start:cs.stop - 2 * lines.start]
+    _verify_scaled_gemm(bound, "W4A16 D", lambda rs: a[rs].double(), b64, m, n, k, out)
+
+
+def check_gemm_w4a16(real, bound, a, q, s, out=None):
+    ret = real(a, q, s, out=out)
+    verify_gemm_w4a16(bound, a, q, s, ret)
+    return ret
+
+
+# ------------------------------------------------------------------------------------------------------------- FP8
+def verify_fp8_quantize(bound, x, fmt, y, yt, scale_inv):
+    """The codes (row-major and transposed) and 1 / scale bit for bit as tests/fp8_ref.py gives them: amax over the whole
+    tensor, scale = 2^e, each code the satfinite round-to-nearest-even cast of x scale."""
+    rows, cols = x.shape
+    amax = float(x.float().abs().max()) if x.numel() else 0.0
+    e, sinv = fp8_ref.scale_exp(amax, fmt)
+    bound.equal("scale_inv (bits)", scale_inv.reshape(-1).cpu().view(torch.int32),
+                torch.tensor([sinv], dtype=torch.float32).view(torch.int32))
+    sc = np.float32(np.ldexp(1.0, e))
+    for rs in _chunks(rows, cols * 8 * 16):
+        codes = torch.from_numpy(fp8_ref.encode(x[rs].float().cpu().numpy() * sc, fmt))
+        if y is not None:
+            bound.equal("row-major codes", y[rs].view(torch.uint8).cpu(), codes)
+        if yt is not None:
+            bound.equal("transposed codes", yt[:, rs].view(torch.uint8).cpu(), codes.t())
+
+
+def check_fp8_quantize(real, bound, x, fmt, rowwise=True, colwise=False):
+    ret = real(x, fmt, rowwise=rowwise, colwise=colwise)
+    verify_fp8_quantize(bound, x, fmt, *ret)
+    return ret
+
+
+FP8_MMA_REL = 2.0 ** -9    # the FP8 tensor-core accumulation error of one 128-deep block, relative to its sum |A||B|
+
+
+def verify_gemm_fp8(bound, a, a_scale_inv, b, b_scale_inv, out, old=None):
+    """out (+)= bf16((A B^T) a_scale_inv b_scale_inv) over the decoded codes, on the scaled operands: 2^-8 |ref| for the
+    rounding, 2 u32 |old| for the accumulate add, and (FP8_MMA_REL + K / 128 2^-23) (|A||B|^T) for the accumulation.
+    The FP8 wgmma does not accumulate in full fp32: inside the tensor core the sum keeps about 14 significant bits (the
+    DeepSeek-V3 report, section 3.3.2, measured it on Hopper), which is why gemm_fp8.cu promotes the partial of every
+    128-deep block into an fp32 accumulator (K / 128 fp32 adds, 2^-23 each). NVIDIA does not document how the tensor core
+    aligns and truncates, so the in-block term is not derived: FP8_MMA_REL = 2^-9 allows each of a block's four k32 wgmma
+    steps to lose 2^-11 of the block's sum |A||B|. On one H100 80GB HBM3 the census's weight-gradient GEMMs (K = 1024
+    tokens) measured up to 8e-4 = 2^-10.3 of sum |A||B| beyond the bf16 rounding, more than an fp32 sum of 1024 terms can
+    lose (1024 2^-24 = 6e-5); test_fp8_gpu.test_gemm_vs_fp64's fp32 bound K 2^-23 (|A||B|^T) fails there."""
+    sa, sb = float(a_scale_inv.double()), float(b_scale_inv.double())
+    m, k = a.shape
+    _verify_scaled_gemm(bound, "FP8 D", lambda rs: a[rs].float().double() * sa, lambda cs: b[cs].float().double() * sb,
+                        m, b.shape[0], k, out, old, acc_rel=FP8_MMA_REL + -(-k // 128) * 2.0 ** -23)
+
+
+def check_gemm_fp8(real, bound, a, a_scale_inv, b, b_scale_inv, out=None, accumulate=False):
+    old = out.clone() if accumulate else None
+    ret = real(a, a_scale_inv, b, b_scale_inv, out=out, accumulate=accumulate)
+    verify_gemm_fp8(bound, a, a_scale_inv, b, b_scale_inv, ret, old)
+    return ret
+
+
+# --------------------------------------------------------------------------------------------------------- decoding
+def verify_attn_decode(bound, q, k_cache, v_cache, kv_len, scale, kv_mask, rel_bias, out, lse):
+    """One query per (batch, head) against the slots [0, kv_len) only: scores scale q.k + rel_bias[h, k - (kv_len - 1) +
+    cap - 1], masked where kv_mask is 0 (or the bias -inf), softmax and P V in fp64. The kernel keeps every probability in
+    fp32 (no bf16 rounding of P) and merges the split partials in fp32, so with E = max_k e_s (_scores' error) +
+    (3 + cap / 32) 2^-22 (ex2.approx per probability, per rescale and per merged split)
+    |O - O_ref| <= (2 E + kv_len 2^-23) (P |V|) + 1 ulp(O); lse (log2 domain) within (E + 2^-22 (1 + |lse|)) / ln 2. A row
+    that sees no key: O = 0, lse = +inf."""
+    B, H, D = q.shape
+    cap = k_cache.shape[1]
+    L = max(0, min(int(kv_len), cap))
+    ln2 = math.log(2.0)
+    for bs in _chunks(B, H * max(L, 1) * 8 * (12 + 4 * D)):
+        qd = q[bs].double()                                         # [b, H, D]
+        kd = k_cache[bs, :L].double().permute(0, 2, 1, 3)           # [b, H, L, D]
+        vd = v_cache[bs, :L].double().permute(0, 2, 1, 3)
+        s = scale * torch.einsum("bhd,bhld->bhl", qd, kd)
+        e = D * 2.0 ** -23 * scale * torch.einsum("bhd,bhld->bhl", qd.abs(), kd.abs()) + 2.0 ** -22 * s.abs()
+        keep = torch.ones_like(s, dtype=torch.bool)
+        if rel_bias is not None:
+            bias = rel_bias.double()[:, torch.arange(L, device=q.device) - (L - 1) + cap - 1][None]   # [1, H, L]
+            fin = torch.isfinite(bias)
+            bias = torch.where(fin, bias, 0.0)
+            s, e, keep = s + bias, e + 2.0 ** -22 * bias.abs(), keep & fin
+        if kv_mask is not None:
+            keep = keep & (kv_mask[bs, :L] != 0)[:, None, :]
+        s = s.masked_fill(~keep, float("-inf"))
+        e = e.masked_fill(~keep, 0.0)
+        p, lse_ref = _softmax(s)
+        E = (e.amax(-1, keepdim=True) if L else torch.zeros_like(s[..., :1])) + (3 + cap / 32) * 2.0 ** -22
+        ref = torch.einsum("bhl,bhld->bhd", p, vd)
+        mag = torch.einsum("bhl,bhld->bhd", p, vd.abs())
+        bound.close("O", out[bs], ref, (2 * E + L * 2.0 ** -23) * mag + bf16_ulp(ref))
+        if lse is not None:
+            lg = lse[bs].double()
+            fin = torch.isfinite(lse_ref)
+            bound.equal("rows without keys (lse = inf)", torch.isinf(lg) & (lg > 0), ~fin)
+            ltol = (E[..., 0] + 2.0 ** -22 * (1 + lse_ref.abs())) / ln2
+            bound.close("lse", torch.where(fin, lg, 0.0), torch.where(fin, lse_ref / ln2, 0.0), torch.where(fin, ltol, 0.0))
+
+
+def check_attn_decode(real, bound, q, k_cache, v_cache, kv_len, scale, kv_mask=None, rel_bias=None, out=None):
+    o, lse = ret = real(q, k_cache, v_cache, kv_len, scale, kv_mask=kv_mask, rel_bias=rel_bias, out=out)
+    verify_attn_decode(bound, q, k_cache, v_cache, int(kv_len.item()), scale, kv_mask, rel_bias, o, lse)
+    return ret
+
+
+def verify_kv_append(bound, k_new, v_new, kv_len, k_before, v_before, m_before, k_cache, v_cache, kv_mask):
+    """Slot kv_len - 1 of both caches holds k_new / v_new bit for bit and its kv_mask bit is 1; every other element of both
+    caches and of the mask is unchanged (a slot outside the cache: nothing changes)."""
+    cap = k_cache.shape[1]
+    slot = int(kv_len) - 1
+    for name, new, before, after in (("K cache", k_new, k_before, k_cache), ("V cache", v_new, v_before, v_cache)):
+        want = before.clone()
+        if 0 <= slot < cap:
+            want[:, slot] = new
+        bound.exact(name, after, want)
+    if kv_mask is not None:
+        want = m_before.clone()
+        if 0 <= slot < cap:
+            want[:, slot] = 1
+        bound.equal("kv_mask", kv_mask, want)
+
+
+def check_kv_append(real, bound, k_new, v_new, k_cache, v_cache, kv_len, kv_mask=None):
+    kb, vb = k_cache.clone(), v_cache.clone()
+    mb = None if kv_mask is None else kv_mask.clone()
+    ret = real(k_new, v_new, k_cache, v_cache, kv_len, kv_mask=kv_mask)
+    verify_kv_append(bound, k_new, v_new, int(kv_len.item()), kb, vb, mb, k_cache, v_cache, kv_mask)
+    return ret
+
+
+def verify_kv_reorder(bound, src, index, kv_len, dst_before, dst):
+    """dst[l, r, :kv_len] = src[l, index[r], :kv_len] bit for bit; dst's slots at or beyond kv_len are unchanged."""
+    cap = src.shape[2]
+    L = max(0, min(int(kv_len), cap))
+    want = dst_before.clone()
+    want[:, :, :L] = src[:, index.to(src.device), :L]
+    bound.exact("reordered cache", dst, want)
+
+
+def check_kv_reorder(real, bound, src, dst, index, kv_len):
+    before = dst.clone()
+    ret = real(src, dst, index, kv_len)
+    verify_kv_reorder(bound, src, index, int(kv_len.item()), before, dst)
     return ret
 
 
@@ -847,4 +1210,10 @@ CHECKERS = {
     "accumulate": check_accumulate, "scale_inplace": check_scale_inplace, "cast_f32_to_bf16": check_cast_f32_to_bf16,
     "add": check_add,
     "sumsq": check_sumsq, "clip_coef": check_clip_coef, "adamw_flat": check_adamw_flat,
+    "dropout": check_dropout, "dropout_advance": check_dropout_advance,
+    "layernorm_bwd_dropout": check_layernorm_bwd_dropout, "rmsnorm_bwd_dropout": check_rmsnorm_bwd_dropout,
+    "fp8_quantize": check_fp8_quantize, "gemm_fp8": check_gemm_fp8,
+    "quantize_w8": check_quantize_w8, "quantize_w4": check_quantize_w4,
+    "gemm_w8a16": check_gemm_w8a16, "gemm_w4a16": check_gemm_w4a16,
+    "attn_decode": check_attn_decode, "kv_append": check_kv_append, "kv_reorder": check_kv_reorder,
 }

@@ -17,6 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "fengshen-lm_b200", "compat"))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
+import int8_ref  # noqa: E402
 import llama_oracle as O  # noqa: E402
 from fsb200 import lib as L  # noqa: E402
 from fsb200 import ops  # noqa: E402
@@ -26,15 +27,7 @@ V = 512
 PROJ = ("attention.query_key_value.weight", "attention.dense.weight", "mlp.w1.weight", "mlp.w3.weight", "mlp.w2.weight")
 
 
-def np_quantize(w):
-    """The quantiser's contract in numpy float32: s = absmax / 127, q = clamp(rint(w / s), -127, 127), zero rows 0."""
-    w = np.asarray(w, dtype=np.float32)
-    s = (np.abs(w).max(axis=1) / np.float32(127.0)).astype(np.float32)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        r = np.rint(w / s[:, None])
-    q = np.clip(r, -127, 127)
-    q[s == 0] = 0
-    return q.astype(np.int8), s
+np_quantize = int8_ref.quantize
 
 
 def _bf16(x):

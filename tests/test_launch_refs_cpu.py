@@ -2,14 +2,23 @@
 the fp64 forward (the bf16 rounding of the autograd result is accepted, at bounds about one ulp wide), and the bound
 rejects the faults a kernel makes: one 64 x 64 block replaced by its neighbour's values, one row dropped from a column
 sum, one 128-deep k-block missing from a GEMM, one head's O swapped with another's, one row's term dropped from a norm
-backward. The census on the GPU (test_workload_launches_gpu.py) is only as strong as these proofs.
+backward. The dropout, quantisation, FP8 and decode checkers reject the mask of site + 1, a mask transposed in (q, k),
+a mask without its 1 / (1 - p), a stream that lost its high word, an off-by-one counter, kv_append at slot kv_len,
+attn_decode reading one slot past kv_len, kv_reorder writing past kv_len or gathering another layer, the neighbouring
+channel's or group's scale, and an FP8 scale used uninverted. The censuses on the GPU (test_workload_launches_gpu.py,
+test_path_launches_gpu.py) are only as strong as these proofs.
 """
 import math
 
+import numpy as np
 import pytest
 import torch
 
+import fp8_ref
+import int4_ref
+import int8_ref
 import launch_refs as R
+import philox_ref
 
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 
@@ -413,3 +422,336 @@ def test_gemm_reference_in_small_chunks(monkeypatch):
         _rejects(R.verify_gemm, layout, a, b, _swap_block(ref.to(BF16), 128, 192), bias, R.EPI_GELU_TANH, None, aux, aux)
         lost = R.act64(R.ACT_GELU_TANH, pre - A[:, 128:256].double() @ B[128:256].double())
         _rejects(R.verify_gemm, layout, a, b, lost.to(BF16), bias, R.EPI_GELU_TANH, None, aux, aux)
+
+
+# ---------------------------------------------------------------------------------------------------- dropout masks
+SEED = 0x1234_5678_9ABC_DEF
+HI = 2 ** 32 + 1        # a stream in the high word: base 2^32 - 5 plus site 6, as the GPU census draws them
+
+
+def test_torch_philox_matches_numpy():
+    """philox_ref's torch port gives the numpy masks bit for bit, in both layouts, for row / batch windows and for streams
+    that carry into the high word."""
+    for stream in (0, 5, 2 ** 32 - 1, 2 ** 32, 2 ** 32 + 3, 2 ** 45 + 2 ** 32 - 1):
+        hk = philox_ref.hidden_keep(SEED, stream, 40, 88, 0.1)
+        assert np.array_equal(philox_ref.hidden_keep_t(SEED, stream, range(0, 40), 88, 0.1).numpy(), hk)
+        assert np.array_equal(philox_ref.hidden_keep_t(SEED, stream, range(7, 19), 88, 0.1).numpy(), hk[7:19])
+        ak = philox_ref.attn_keep(SEED, stream, 3, 2, 40, 72, 0.1)
+        assert np.array_equal(philox_ref.attn_keep_t(SEED, stream, range(0, 3), 2, 40, 72, 0.1).numpy(), ak)
+        assert np.array_equal(philox_ref.attn_keep_t(SEED, stream, range(2, 3), 2, 40, 72, 0.1).numpy(), ak[2:])
+    w = philox_ref.philox4x32_10_t((torch.tensor([0xFFFFFFFF, 0]), 0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFFF), (0xFFFFFFFF, 0))
+    wn = philox_ref.philox4x32_10((np.array([0xFFFFFFFF, 0]), 0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFFF), (0xFFFFFFFF, 0))
+    assert all(np.array_equal(a.numpy(), b.astype(np.int64)) for a, b in zip(w, wn))
+
+
+def _spec(stream, p=0.1):
+    return R.DropSpec(p, SEED, stream)
+
+
+def _hmask(d, rows, cols, scaled=True):
+    k = philox_ref.hidden_keep_t(d.seed, d.stream, range(rows), cols, d.p).double()
+    return k * R.keep_scale(d.p) if scaled else k
+
+
+FAULTS = {   # the masks a kernel could draw by mistake, as (spec, scaled) of the right spec d
+    "site + 1": lambda d: (d._replace(stream=d.stream + 1), True),
+    "no 1 / (1 - p)": lambda d: (d, False),
+    "high word lost": lambda d: (d._replace(stream=d.stream & 0xFFFFFFFF), True),
+}
+
+
+def test_dropout_and_advance():
+    rows, cols = 96, 264
+    x = _randn(rows, cols, seed=1)
+    d = _spec(HI + 1)
+    ks = torch.tensor(R.keep_scale(d.p))
+    good = torch.where(_hmask(d, rows, cols, False) > 0, x.float() * ks, torch.zeros(())).to(BF16)
+    _ok(R.verify_dropout, x, d, good)
+    for name, f in FAULTS.items():
+        fd, scaled = f(d)
+        _rejects(R.verify_dropout, x, d, (x.double() * _hmask(fd, rows, cols, scaled)).to(BF16))
+    _ok(R.verify_dropout_advance, HI, 7, torch.tensor([HI]), torch.tensor([HI + 7]))
+    _rejects(R.verify_dropout_advance, HI, 7, torch.tensor([HI]), torch.tensor([HI + 6]))
+    _rejects(R.verify_dropout_advance, HI, 7, torch.tensor([HI + 1]), torch.tensor([HI + 7]))
+
+
+@pytest.mark.parametrize("layer", [False, True], ids=["rmsnorm", "layernorm"])
+def test_norm_dropout(layer):
+    rows, cols, eps = 130, 256, 1e-6
+    x, r, dy = _randn(rows, cols, seed=1), _randn(rows, cols, seed=2), _randn(rows, cols, seed=6)
+    w, beta = _randn(cols, seed=3, scale=0.3) + 1, _randn(cols, seed=4)
+    d = _spec(HI)
+    ks = torch.tensor(R.keep_scale(d.p))
+
+    def norm(xs):
+        st = _ln_stats(xs, eps, layer)
+        if layer:
+            y = torch.nn.functional.layer_norm(xs.double(), (cols,), w.double(), beta.double(), eps).to(BF16)
+        else:
+            y = (xs.float() * st[:, None]).to(BF16) * w
+        return y, st, xs
+    xs = (torch.where(_hmask(d, rows, cols, False) > 0, x.float() * ks, torch.zeros(())) + r.float()).to(BF16)
+    y, st, _ = norm(xs)
+    args = (layer, x, r, w, beta if layer else None, eps)
+    _ok(R.verify_norm_fwd, *args, y, st, xs, drop=d)
+    for name, f in FAULTS.items():
+        fd, scaled = f(d)
+        _rejects(R.verify_norm_fwd, *args, *norm((x.double() * _hmask(fd, rows, cols, scaled) + r.double()).to(BF16)),
+                 drop=d)
+    # backward: dx of the sum (with dres), dbranch = M dx, through autograd of the fp64 norm
+    xd = xs.double().requires_grad_(True)
+    if layer:
+        out = torch.nn.functional.layer_norm(xd, (cols,), w.double(), beta.double(), eps)
+    else:
+        out = xd * torch.rsqrt(xd.pow(2).mean(1, keepdim=True) + eps) * w.double()
+    out.backward(dy.double())
+    dx = xd.grad + r.double()               # r stands in for dres
+    xw = (xs.double() - st[:, 0:1].double()) * st[:, 1:2].double() if layer else (xs.float() * st[:, None]).to(BF16).double()
+    dw = (dy.double() * xw).sum(0).float()
+    db = dy.double().sum(0).float() if layer else None
+    bargs = (layer, dy, xs, w, st, r, dx.to(BF16), dw, None, db, None)
+    _ok(R.verify_norm_bwd, *bargs, drop=d, dbranch=(dx * _hmask(d, rows, cols)).to(BF16))
+    for name, f in FAULTS.items():
+        fd, scaled = f(d)
+        _rejects(R.verify_norm_bwd, *bargs, drop=d, dbranch=(dx * _hmask(fd, rows, cols, scaled)).to(BF16))
+
+
+@pytest.mark.parametrize("act", [R.ACT_GELU_TANH, R.ACT_GELU_ERF])
+def test_glu_dropout(act):
+    rows, cols = 128, 192
+    gate, up, dout = _randn(rows, cols, seed=1), _randn(rows, cols, seed=2), _randn(rows, cols, seed=3)
+    d = _spec(HI + 2)
+
+    def grads(m):
+        g, u = gate.double().requires_grad_(True), up.double().requires_grad_(True)
+        out = R.act64(act, g) * u * m
+        out.backward(dout.double())
+        return out.detach().to(BF16), g.grad.to(BF16), u.grad.to(BF16)
+    out, dg, du = grads(_hmask(d, rows, cols))
+    _ok(R.verify_glu_fwd, act, gate, up, out, d)
+    _ok(R.verify_glu_bwd, act, dout, gate, up, dg, du, d)
+    for name, f in FAULTS.items():
+        fd, scaled = f(d)
+        o_, dg_, du_ = grads(_hmask(fd, rows, cols, scaled))
+        _rejects(R.verify_glu_fwd, act, gate, up, o_, d)
+        _rejects(R.verify_glu_bwd, act, dout, gate, up, dg_, du_, d)
+
+
+def _attn_dropout_autograd(q, k, v, scale, rel, kvm, dout, m):
+    S = q.shape[1]
+    qd, kd, vd = (R._bhsd(t).double().requires_grad_(True) for t in (q, k, v))
+    relg = rel.double().requires_grad_(True)
+    i = torch.arange(S)
+    s = scale * qd @ kd.transpose(-1, -2) + relg[:, i[None, :] - i[:, None] + S - 1]
+    if kvm is not None:
+        s = s.masked_fill((kvm == 0)[:, None, None, :], float("-inf"))
+    lse = torch.logsumexp(s, -1)
+    o = (torch.softmax(s, -1) * m) @ vd
+    o.backward(R._bhsd(dout).double())
+    grads = [qd.grad, kd.grad, vd.grad, relg.grad]
+    return o.detach(), lse.detach(), grads
+
+
+@pytest.mark.parametrize("causal_bias", [False, True], ids=["rel_bias", "folded_causal_bias"])
+def test_sdpa_dropout(causal_bias):
+    """Attention dropout with a rel_bias; with the decoder's causal mask folded into it as -inf the reference gives p = 0
+    and a zero tolerance there (no NaN)."""
+    B, S, H, D = 2, 64, 2, 64
+    q, k, v = _randn(B, S, H, D, seed=1), _randn(B, S, H, D, seed=2), _randn(B, S, H, D, seed=3)
+    rel = (torch.randn(H, 2 * S - 1, generator=_g(4)) * 2).float()
+    if causal_bias:
+        rel[:, S:] = float("-inf")                 # offsets k - q > 0
+    kvm = None if causal_bias else torch.ones(B, S, dtype=torch.uint8)
+    if kvm is not None:
+        kvm[1, 50:] = 0
+    dout = _randn(B, S, H, D, seed=9)
+    d = _spec(HI + 1)
+
+    def mask(dd, scaled=True, transpose=False):
+        z = philox_ref.attn_keep_t(dd.seed, dd.stream, range(B), H, S, S, dd.p).double()
+        z = z.transpose(-1, -2) if transpose else z
+        return z * R.keep_scale(dd.p) if scaled else z
+    o, lse, (dq, dk, dv, drel) = _attn_dropout_autograd(q, k, v, 1.0, rel, kvm, dout, mask(d))
+    O, L2 = R._bhsd(o).to(BF16), (lse / math.log(2.0)).float()
+    assert not torch.isnan(O.float()).any()
+    fa = (q, k, v, 1.0, False, kvm, rel)
+    _ok(R.verify_sdpa_fwd, *fa, O, L2, d)
+    old = torch.zeros_like(rel)
+    ba = (q, k, v, O, dout, L2, 1.0, False)
+    DQ, DK, DV = (R._bhsd(t).to(BF16) for t in (dq, dk, dv))
+    _ok(R.verify_sdpa_bwd, *ba, DQ, DK, DV, kvm, rel, drel.float(), old, d)
+    faults = {"transposed (q, k)": mask(d, transpose=True)}
+    faults.update({name: mask(*f(d)) for name, f in FAULTS.items()})
+    for name, m in faults.items():
+        o_, lse_, (dq_, dk_, dv_, drel_) = _attn_dropout_autograd(q, k, v, 1.0, rel, kvm, dout, m)
+        _rejects(R.verify_sdpa_fwd, *fa, R._bhsd(o_).to(BF16), L2, d)
+        # the backward of a wrong mask, fed the right forward's O: dV alone already differs
+        _rejects(R.verify_sdpa_bwd, *ba, DQ, DK, R._bhsd(dv_).to(BF16), kvm, rel, drel.float(), old, d)
+
+
+def test_dropout_stream_invariants():
+    """launch_census.dropout_stream_problems on synthetic logs: a consistent two-forward log passes; a too-small n, a
+    counter that did not advance by n, an unused or doubly used site and a forward / backward mismatch are named."""
+    from launch_census import dropout_stream_problems as problems
+    n, b0 = 3, HI
+    shape = (2, 4, 8, 8)
+
+    def fb(base, site, kind=("sdpa_fwd", "sdpa_bwd"), p=0.1, sh=shape):
+        return [(kind[0], base, site, p, SEED, sh), (kind[1], base, site, p, SEED, sh)]
+    uses = []
+    for base in (b0, b0 + n):
+        uses += fb(base, 0) + fb(base, 1, ("dropout", "dropout"), sh=(16, 8)) + fb(base, 2, ("glu_fwd", "glu_bwd"))
+    adv = [(b0, n), (b0 + n, n)]
+    assert problems(adv, uses) == []
+    assert any("not range(2)" in m for m in problems([(b0, 2), (b0 + 2, 2)], uses))            # n too small
+    assert any("did not advance" in m for m in problems([(b0, n), (b0 + n - 1, n)], uses))       # off by one
+    assert any("unused [2]" in m for m in problems(adv, [u for u in uses if u[2] != 2 or u[1] != b0]))
+    assert any("drawn by" in m for m in problems(adv, uses + fb(b0, 0)[:1]))                    # a site drawn twice
+    bad = [u if u[0] != "glu_bwd" or u[1] != b0 else (u[0], u[1], u[2], 0.2, *u[4:]) for u in uses]
+    assert any("differ" in m for m in problems(adv, bad))                                        # p differs
+    bad = [u if u[0] != "sdpa_bwd" or u[1] != b0 else ("layernorm_bwd_dropout", *u[1:]) for u in uses]
+    assert any("drawn by" in m for m in problems(adv, bad))                                      # kinds differ
+
+
+# ------------------------------------------------------------------------------------------------------------- FP8
+@pytest.mark.parametrize("fmt", ["e4m3", "e5m2"])
+def test_fp8_quantize_and_gemm(fmt):
+    rows, cols = 64, 96
+    x = _randn(rows, cols, seed=1, scale=0.01 if fmt == "e5m2" else 1.0)
+    y, yt, sinv = fp8_ref.quantize(x.float().numpy(), fmt)
+    dt = ops_fp8_dtype = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}[fmt]
+    Y, YT = torch.from_numpy(y).view(dt), torch.from_numpy(yt).view(dt)
+    S = torch.tensor([sinv], dtype=F32)
+    _ok(R.verify_fp8_quantize, x, fmt, Y, YT, S)
+    _ok(R.verify_fp8_quantize, x, fmt, None, YT, S)
+    bad = Y.view(torch.uint8).clone(); bad[3, 5] ^= 1
+    _rejects(R.verify_fp8_quantize, x, fmt, bad.view(dt), None, S)
+    bad = YT.view(torch.uint8).clone(); bad[5, 3] ^= 1
+    _rejects(R.verify_fp8_quantize, x, fmt, None, bad.view(dt), S)
+    _rejects(R.verify_fp8_quantize, x, fmt, Y, YT, 1.0 / S)                 # the scale, not its inverse
+    # the GEMM: out (+)= bf16((A B^T) sa sb) on the decoded codes
+    w = _randn(80, cols, seed=2, scale=0.02)
+    wq, _, ws = fp8_ref.quantize(w.float().numpy(), "e4m3")
+    B8 = torch.from_numpy(wq).view(torch.float8_e4m3fn)
+    SB = torch.tensor([ws], dtype=F32)
+    a64, b64 = Y.float().double() * S.double(), B8.float().double() * SB.double()
+    old = _randn(rows, 80, seed=3)
+    for acc in (None, old):
+        ref = a64 @ b64.t() + (acc.double() if acc is not None else 0.0)
+        _ok(R.verify_gemm_fp8, Y, S, B8, SB, ref.to(BF16), acc)
+        uninv = (Y.float().double() / S.double()) @ b64.t() + (acc.double() if acc is not None else 0.0)
+        _rejects(R.verify_gemm_fp8, Y, S, B8, SB, uninv.to(BF16), acc)       # an FP8 scale used uninverted
+        bad = ref.to(BF16); bad[:, 40:80] = bad[:, 0:40].clone()
+        _rejects(R.verify_gemm_fp8, Y, S, B8, SB, bad, acc)
+    _rejects(R.verify_gemm_fp8, Y, S, B8, SB, (a64 @ b64.t()).to(BF16), old)  # the accumulate term lost
+    del ops_fp8_dtype
+
+
+# --------------------------------------------------------------------------------------------- weight-only int8 / int4
+def test_int8_quantize_and_gemm():
+    n, k, m = 96, 256, 40
+    w = _randn(n, k, seed=1, scale=0.05)
+    w[7] = 0                                               # a zero row: s = 0, q = 0
+    qn, sn = int8_ref.quantize(w.float().numpy())
+    q, s = torch.from_numpy(qn), torch.from_numpy(sn)
+    _ok(R.verify_quantize_w8, w, q, s)
+    bad = q.clone(); bad[3, 9] += 1
+    _rejects(R.verify_quantize_w8, w, bad, s)
+    _rejects(R.verify_quantize_w8, w, q, s * (1 + 2 ** -20))
+    a = _randn(m, k, seed=2)
+    ref = (a.double() @ q.double().t()) * s.double()
+    _ok(R.verify_gemm_w8a16, a, q, s, ref.to(BF16))
+    nb = (a.double() @ q.double().t()) * s.double().roll(1)   # the neighbouring channel's scale
+    _rejects(R.verify_gemm_w8a16, a, q, s, nb.to(BF16))
+
+
+def test_int4_quantize_and_gemm():
+    n, k, m = 64, 384, 24
+    w = _randn(n, k, seed=1, scale=0.05)
+    qn, sn = int4_ref.quantize(w.float().numpy())
+    q, s = torch.from_numpy(int4_ref.pack(qn)), torch.from_numpy(sn).to(BF16)
+    _ok(R.verify_quantize_w4, w, q, s)
+    bad = q.clone(); bad[3, 9] ^= 0x10
+    _rejects(R.verify_quantize_w4, w, bad, s)
+    _rejects(R.verify_quantize_w4, w, q, s.roll(1, 1))
+    W = torch.from_numpy(int4_ref.dequantize(qn, sn))
+    assert torch.equal(R.unpack_w4(q, s).float(), W)
+    a = _randn(m, k, seed=2)
+    _ok(R.verify_gemm_w4a16, a, q, s, (a.double() @ W.double().t()).to(BF16))
+    nb = torch.from_numpy(int4_ref.dequantize(qn, np.roll(sn, 1, axis=1)))   # the neighbouring group's scale
+    _rejects(R.verify_gemm_w4a16, a, q, s, (a.double() @ nb.double().t()).to(BF16))
+
+
+# --------------------------------------------------------------------------------------------------------- decoding
+def _decode_case(B=3, H=2, D=64, cap=320):
+    qd = _randn(B, H, D, seed=1)
+    kc, vc = _randn(B, cap, H, D, seed=2), _randn(B, cap, H, D, seed=3)
+    kvm = torch.ones(B, cap, dtype=torch.uint8)
+    kvm[2, :40] = 0                                        # a left-padded row
+    rel = torch.randn(H, 2 * cap - 1, generator=_g(4)).float()
+    return qd, kc, vc, kvm, rel
+
+
+def _decode_ref(q, kc, vc, L, scale, kvm, rel):
+    cap = kc.shape[1]
+    s = scale * torch.einsum("bhd,blhd->bhl", q.double(), kc[:, :L].double())
+    if rel is not None:
+        s = s + rel.double()[:, torch.arange(L) - (L - 1) + cap - 1][None]
+    if kvm is not None:
+        s = s.masked_fill((kvm[:, :L] == 0)[:, None, :], float("-inf"))
+    lse = torch.logsumexp(s, -1)
+    return torch.einsum("bhl,blhd->bhd", torch.softmax(s, -1), vc[:, :L].double()), lse / math.log(2.0)
+
+
+@pytest.mark.parametrize("variant", ["kv_mask", "rel_bias"])
+def test_attn_decode(variant):
+    q, kc, vc, kvm, rel = _decode_case()
+    kvm = kvm if variant == "kv_mask" else None
+    rel = rel if variant == "rel_bias" else None
+    scale = 0.125
+    L = 257
+    o, lse = _decode_ref(q, kc, vc, L, scale, kvm, rel)
+    _ok(R.verify_attn_decode, q, kc, vc, L, scale, kvm, rel, o.to(BF16), lse.float())
+    o1, lse1 = _decode_ref(q, kc, vc, L + 1, scale, kvm, rel) if rel is None else (None, None)
+    if rel is not None:   # one slot past kv_len, with the bias row of kv_len - 1
+        cap = kc.shape[1]
+        s = scale * q.double()[:, :, None, :].mul(kc[:, :L + 1].double().permute(0, 2, 1, 3)).sum(-1)
+        s = s + rel.double()[:, torch.arange(L + 1) - (L - 1) + cap - 1][None]
+        o1 = torch.einsum("bhl,blhd->bhd", torch.softmax(s, -1), vc[:, :L + 1].double())
+        lse1 = torch.logsumexp(s, -1) / math.log(2.0)
+    _rejects(R.verify_attn_decode, q, kc, vc, L, scale, kvm, rel, o1.to(BF16), lse.float())
+    _rejects(R.verify_attn_decode, q, kc, vc, L, scale, kvm, rel, o.to(BF16), lse1.float())
+
+
+def test_kv_append():
+    B, cap, H, D = 3, 40, 2, 64
+    kn, vn = _randn(B, H, D, seed=1), _randn(B, H, D, seed=2)
+    kb, vb = _randn(B, cap, H, D, seed=3), _randn(B, cap, H, D, seed=4)
+    mb = torch.zeros(B, cap, dtype=torch.uint8); mb[:, :20] = 1
+    L = 21
+
+    def appended(slot):
+        k, v, m = kb.clone(), vb.clone(), mb.clone()
+        k[:, slot], v[:, slot], m[:, slot] = kn, vn, 1
+        return k, v, m
+    _ok(R.verify_kv_append, kn, vn, L, kb, vb, mb, *appended(L - 1))
+    _rejects(R.verify_kv_append, kn, vn, L, kb, vb, mb, *appended(L))         # slot kv_len instead of kv_len - 1
+    k, v, m = appended(L - 1); m[0, 30] = 1
+    _rejects(R.verify_kv_append, kn, vn, L, kb, vb, mb, k, v, m)               # a stray mask bit
+    k, v, m = appended(L - 1); v[1, 3, 1, 7] += 1
+    _rejects(R.verify_kv_append, kn, vn, L, kb, vb, mb, k, v, m)               # another V element changed
+    _ok(R.verify_kv_append, kn, vn, cap + 1, kb, vb, mb, kb.clone(), vb.clone(), mb.clone())   # outside: no change
+
+
+def test_kv_reorder():
+    layers, rows, cap, slot = 3, 4, 24, 2 * 2 * 64
+    src = _randn(layers, rows, cap, slot, seed=1)
+    before = _randn(layers, rows, cap, slot, seed=2)
+    index = torch.tensor([2, 2, 0, 3])
+    L = 17
+    want = before.clone(); want[:, :, :L] = src[:, index, :L]
+    _ok(R.verify_kv_reorder, src, index, L, before, want)
+    past = want.clone(); past[:, :, L] = src[:, index, L]
+    _rejects(R.verify_kv_reorder, src, index, L, before, past)                # written past kv_len
+    other = want.clone(); other[1, :, :L] = src[2][index, :L]
+    _rejects(R.verify_kv_reorder, src, index, L, before, other)              # another layer's rows
