@@ -608,10 +608,9 @@ extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v,
                                     const int64_t* stream_base, int64_t site, fsb_stream_t st) {
   DropArgs d;
   if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  if (p > 0.f) {
-    FSB_REQUIRE(!causal, "sdpa_bwd_dropout: the causal flag is not supported with p > 0; fold the mask into rel_bias");
+  // causal composes with p > 0 as in fsb_sdpa_fwd_dropout: masked elements have P = 0, so their keep bits never matter
+  if (p > 0.f)
     FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536, "sdpa_bwd_dropout: sequences longer than 65536 are not supported with p > 0");
-  }
   return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
                   k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,

@@ -10,11 +10,10 @@ object with `.loss` and `.logits` / `.prediction_logits`, `state_dict()` in HF k
 step on libfsb200.so. `install()` rebinds the four names on the `transformers` module so that an UNMODIFIED script's
 `from transformers import MegatronBertForPreTraining` picks them up; `python -m fsb200.launch script.py ...` does that and then
 runs the script. GPT2LMHeadModel and MT5ForConditionalGeneration also carry `generate` (KV-cache decoding on the split-KV decode
-kernel, HF GenerationMixin semantics: fsb200/generation.py). BertForMaskedLM, MegatronBertForPreTraining and MT5ForConditionalGeneration apply the
-config's dropout in training mode (fsb200/models/bert.py, fsb200/models/t5.py). Anything outside the hot path (dropout > 0 in
-GPT-2, mT5 `generate` in training mode with dropout > 0, generation for the
-encoder-only BERT classes, output_attentions, generation keywords fsb200/generation.py does not implement) raises instead of
-silently differing."""
+kernel, HF GenerationMixin semantics: fsb200/generation.py). All four classes apply the config's dropout in training mode
+(fsb200/models/gpt2.py, fsb200/models/bert.py, fsb200/models/t5.py). Anything outside the hot path (GPT-2 / mT5 `generate` in
+training mode with dropout > 0, generation for the encoder-only BERT classes, output_attentions, generation keywords
+fsb200/generation.py does not implement) raises instead of silently differing."""
 import json
 import os
 

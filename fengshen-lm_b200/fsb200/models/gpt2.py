@@ -6,7 +6,14 @@ pre-LN blocks `x + attn(ln_1(x))`, `x + mlp(ln_2(x))`, final `ln_f`; fused `c_at
 (q | k | v contiguous thirds); `gelu_new`; learned positions `wte[ids] + wpe[pos]`; LM head tied to `wte`; shifted mean
 cross-entropy with ignore_index -100. State-dict keys follow HF (`transformer.h.N.attn.c_attn.weight`, ...).
 Conv1D's [in, out] layout maps onto the GEMM layouts without any transpose: forward = NN, dgrad = NT, wgrad = TN.
-Dropout probabilities must be 0 (parity / benchmark setting, SURVEY.md §8d); a non-zero value is rejected loudly.
+Dropout (`embd_pdrop`, `attn_pdrop`, `resid_pdrop`, each in [0, 1) and independent) applies in training mode
+(`model.training`, also under no_grad), at HF's sites: the embedding sum, the attention probabilities (inside the causal
+attention kernels: ops.sdpa_causal_dropout_fwd / _bwd) and the attention / MLP `c_proj` outputs, dropped by the LayerNorm
+that adds them to the residual stream (`ln_2`, the next block's `ln_1`, `ln_f`). Masks come from Philox (include/fsb200.h): a seed drawn once from
+torch.default_generator at construction (only when a probability is > 0) and a device stream counter that every training
+forward advances by its number of sites, so eager runs and replayed CUDA graphs draw the same fresh masks. In eval mode, or
+with all three probabilities 0, the forward and backward are the dropout-free kernels; `generate` in training mode with a
+non-zero probability is rejected (HF would drop).
 """
 import math
 from collections import namedtuple
@@ -34,9 +41,10 @@ class GPT2LMHeadModel(FlatModel):
         self.V, self.npos = g("vocab_size"), g("n_positions", g("max_position_embeddings", 1024))
         self.eps = g("layer_norm_epsilon", 1e-5)
         self.inner = g("n_inner") or 4 * self.h
-        for k in ("resid_pdrop", "embd_pdrop", "attn_pdrop"):
-            if g(k, 0.0) not in (0, 0.0):
-                raise RuntimeError(f"fsb200 GPT2: {k}={g(k)} — dropout is not implemented; set it to 0")
+        self.p_embd, self.p_attn, self.p_resid = (float(g(k, 0.0) or 0.0) for k in ("embd_pdrop", "attn_pdrop", "resid_pdrop"))
+        for k, v in (("embd_pdrop", self.p_embd), ("attn_pdrop", self.p_attn), ("resid_pdrop", self.p_resid)):
+            if not 0.0 <= v < 1.0:
+                raise RuntimeError(f"fsb200 GPT2: {k}={v} outside [0, 1)")
         if g("activation_function", "gelu_new") != "gelu_new":
             raise RuntimeError("fsb200 GPT2: only activation_function='gelu_new' is implemented")
         h, V = self.h, self.V
@@ -65,6 +73,17 @@ class GPT2LMHeadModel(FlatModel):
         self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
                       for b in self.transformer.h]
         self.reset_parameters(seed)
+        # dropout sites of one forward, in transformers' call order: 0 embeddings; for layer i, 1 + 3i attention probabilities,
+        # 2 + 3i attention c_proj output, 3 + 3i MLP c_proj output. A site whose probability is 0 keeps its number.
+        self.dropout_sites = 1 + 3 * self.nl
+        self.dropout_seed, self.dropout_counter = None, None
+        if max(self.p_embd, self.p_attn, self.p_resid) > 0:
+            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
+            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=self.flat.params.device)
+
+    def _drop(self, base, p, site):
+        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
+        return None if base is None or p == 0.0 else ops.Dropout(p, self.dropout_seed, base, site)
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -94,8 +113,16 @@ class GPT2LMHeadModel(FlatModel):
     def _forward_impl(self, ids, pos, mask, lab, B, S, save, want_logits):
         scale = 1.0 / math.sqrt(self.hn)
         acts = [] if save else None
-        hf, stf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale,
-                                                                             True, kv_mask=mask), acts)
+        base = None
+        if self.training and self.dropout_seed is not None:
+            base = ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+
+        def attend(i, q5):
+            drop = self._drop(base, self.p_attn, 1 + 3 * i)
+            if drop is None:
+                return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask)
+            return ops.sdpa_causal_dropout_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, drop, kv_mask=mask)
+        hf, stf, xf = self._stack(ids, pos, B, S, attend, acts, base)
         logits = self._head(hf)
         loss, ctx = None, None
         if lab is not None:
@@ -103,27 +130,34 @@ class GPT2LMHeadModel(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S)
+                ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
-    def _stack(self, ids, pos, B, S, attend, acts=None):
+    def _stack(self, ids, pos, B, S, attend, acts=None, base=None):
         """Embedding, the blocks and ln_f over ids [B * S] -> (hidden states, ln_f stats, residual stream). attend(i, q5) is
-        block i's attention over the packed q|k|v view [B, S, 3, heads, head_dim] -> (out, lse); `acts`, when given,
-        collects what the backward reads."""
+        block i's attention over the packed q|k|v view [B, S, 3, heads, head_dim] -> (out, lse), drawing its own probability
+        mask; `acts`, when given, collects what the backward reads. base: the forward's dropout stream base (None: no
+        dropout, as in generation's prefill and decode steps)."""
         h, nh, hn = self.h, self.nh, self.hn
         tr = self.transformer
+        pr = self.p_resid
+        D = lambda p, site: self._drop(base, p, site)
         self._need("no_decay"); self._need("wte")
         x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
+        if D(self.p_embd, 0) is not None:
+            x = ops.dropout(x, D(self.p_embd, 0))
         prev_m = None
         for i, (blk, pj) in enumerate(zip(tr.h, self._proj)):
             self._need(f"layer{i}")
             h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
-                                           self.eps, residual=None if prev_m is None else x)
+                                           self.eps, residual=None if prev_m is None else x,
+                                           drop=None if prev_m is None else D(pr, 3 * i))   # layer i-1's MLP output
             qkv = pj.c_attn(h1)
             o, lse = attend(i, qkv.view(B, S, 3, nh, hn))
             a = pj.attn_proj(o.view(B * S, h))
-            h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x)
+            h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x,
+                                            drop=D(pr, 2 + 3 * i))
             pre = None if acts is None else torch.empty((B * S, self.inner), dtype=torch.bfloat16, device=x.device)
             f = pj.c_fc(h2, epilogue=L.EPI_GELU_TANH, aux=pre)
             m = pj.mlp_proj(f)
@@ -132,7 +166,8 @@ class GPT2LMHeadModel(FlatModel):
             # free this block's temporaries before the next block allocates its own (the peak of a long prompt's prefill)
             del st1, h1, qkv, o, lse, a, st2, h2, pre, f
             x, prev_m = x1, m
-        return ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x)
+        return ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x,
+                                 drop=D(pr, 3 * self.nl))
 
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on GPT-2 (wenzhong_qa/README.md:58-67: sampling with top_p, num_return_sequences,
@@ -145,7 +180,11 @@ class GPT2LMHeadModel(FlatModel):
     # (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
-        """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded."""
+        """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded. Runs without
+        dropout; in training mode with a non-zero dropout probability it raises (HF would drop)."""
+        if self.training and self.dropout_seed is not None:
+            raise RuntimeError("fsb200 GPT2: generate in training mode with embd_pdrop / attn_pdrop / resid_pdrop > 0 would "
+                               "drop; call model.eval() first")
         dev = self.flat.params.device
         ids = input_ids.to(device=dev, dtype=torch.int64)
         B, S0 = ids.shape
@@ -201,10 +240,22 @@ class GPT2LMHeadModel(FlatModel):
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, hf, stf, xf, dlogits, ids, pos, mask, B, S = ctx
+        acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base = ctx
         h, nh, hn = self.h, self.nh, self.hn
         T = B * S
         acc = self.accumulate_grads
+        pr = self.p_resid
+        D = lambda p, site: self._drop(base, p, site)
+
+        def ln_bwd(dy, x, ln, st, drop, dres=None):
+            """(gradient of the LN input sum, gradient of its dropped branch) — the same tensor without dropout."""
+            if drop is None:
+                d = ops.layernorm_bwd(dy, x, ln.weight.data, st, ln.weight.main_grad, ln.bias.main_grad, accumulate=acc,
+                                      dres=dres)
+                return d, d
+            return ops.layernorm_bwd_dropout(dy, x, ln.weight.data, st, ln.weight.main_grad, ln.bias.main_grad, drop,
+                                             accumulate=acc, dres=dres)
+
         self._begin_backward()
         tr = self.transformer
         scale = 1.0 / math.sqrt(hn)
@@ -212,26 +263,31 @@ class GPT2LMHeadModel(FlatModel):
             ops.scale_inplace(dlogits, gloss)  # upstream scalar; the kernel exits immediately when it is 1.0
         dhf = self._head.backward(dlogits, hf, acc)   # tied head: written first, the embedding adds later
         del dlogits
-        dx = ops.layernorm_bwd(dhf, xf, tr.ln_f.weight.data, stf, tr.ln_f.weight.main_grad, tr.ln_f.bias.main_grad,
-                               accumulate=acc)
+        dx, dm = ln_bwd(dhf, xf, tr.ln_f, stf, D(pr, 3 * self.nl))     # d(residual), d(last MLP output)
         for i in reversed(range(self.nl)):
             blk, pj = tr.h[i], self._proj[i]
             x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f = acts[i]
             acts[i] = None
-            df = pj.mlp_proj.backward(dx, f, acc)
+            df = pj.mlp_proj.backward(dm, f, acc)
             dpre = ops.act_bwd_bias(L.ACT_GELU_TANH, df, pre, pj.c_fc.bias_grad, accumulate=acc)   # dGELU + c_fc bias grad
             dh2 = pj.c_fc.backward(dpre, h2, acc, colsum=False)
-            dx1 = ops.layernorm_bwd(dh2, x1, blk.ln_2.weight.data, st2, blk.ln_2.weight.main_grad,
-                                    blk.ln_2.bias.main_grad, accumulate=acc, dres=dx)
-            do = pj.attn_proj.backward(dx1, o.view(T, h), acc)
+            dx1, da = ln_bwd(dh2, x1, blk.ln_2, st2, D(pr, 2 + 3 * i), dres=dx)
+            do = pj.attn_proj.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask)
+            drop = D(self.p_attn, 1 + 3 * i)
+            if drop is None:
+                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
+                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask)
+            else:
+                ops.sdpa_causal_dropout_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale,
+                                            d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop, kv_mask=mask)
             dh1 = pj.c_attn.backward(dqkv, h1, acc)
-            dx = ops.layernorm_bwd(dh1, x, blk.ln_1.weight.data, st1, blk.ln_1.weight.main_grad,
-                                   blk.ln_1.bias.main_grad, accumulate=acc, dres=dx1)
+            # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped MLP output into x
+            dx, dm = ln_bwd(dh1, x, blk.ln_1, st1, D(pr, 3 * i) if i > 0 else None, dres=dx1)
             self._done(f"layer{i}")
+        if D(self.p_embd, 0) is not None:
+            dx = ops.dropout(dx, D(self.p_embd, 0))
         ops.embedding_bwd(ids, dx, tr.wte.weight.main_grad)  # accumulates onto the LM-head wgrad (tied weights)
         learned_pos_emb_bwd(pos, dx, tr.wpe.weight.main_grad, B, S, acc)
         self._done("wte")

@@ -341,7 +341,7 @@ class MT5ForConditionalGeneration(FlatModel):
         D = lambda site: self._drop(base, site)
         causal = True
         if D(E) is not None:
-            # the attention kernels take no causal flag under dropout: the mask becomes -inf at the offsets k - q > 0 of the
+            # under dropout the decoder keeps its causal mask folded into the bias: -inf at the offsets k - q > 0 of the
             # bias vector (index k - q + Sd - 1), as HF adds its causal mask to the position bias
             rel_d = rel_d.clone()
             rel_d[:, Sd:] = float("-inf")

@@ -315,7 +315,7 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
                  float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                  void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
-/* ---- dropout (BERT / MegatronBERT / mT5 training) -------------------------------------------------------------------
+/* ---- dropout (GPT-2 / BERT / MegatronBERT / mT5 training) -----------------------------------------------------------
  * torch.nn.functional.dropout semantics: an element is dropped with probability p and every kept element is scaled by
  * 1 / (1 - p). The keep bit is a pure function of (seed, stream, coordinates) through Philox4x32-10 (Random123; key =
  * (seed & 0xffffffff, seed >> 32)), so no mask is stored: the backward kernels regenerate it.
@@ -329,10 +329,10 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
  *               counter ((4 ka + ks) | (4 qa + qs) << 16, b * nheads + head, s & 0xffffffff, s >> 32); r = byte 2 qh + kh of
  *               output word 2 qp + kp. seq_q, seq_kv <= 65536.
  * fsb_sdpa_fwd_dropout / fsb_sdpa_bwd_dropout: fsb_sdpa_fwd / fsb_sdpa_bwd with dropout on the attention probabilities,
- *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. rel_bias composes with
- *   dropout; with p > 0 the causal flag is rejected: fold the causal mask into rel_bias instead (-inf at offsets k - q > 0,
- *   as T5's decoder adds its causal mask to the position bias). The backward must get the forward's seed, stream_base value
- *   and site.
+ *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. The causal flag,
+ *   kv_mask and rel_bias all compose with dropout (GPT-2: causal + padding; T5: relative bias). Z of an element is the same
+ *   whichever tiles a launch visits, so a causal launch still skips the key / query tiles wholly above the diagonal. The
+ *   backward must get the forward's seed, stream_base value and site.
  * fsb_layernorm_fwd_dropout: fsb_layernorm_fwd with sum_out = x * Z / (1 - p) + residual (residual required when p > 0): the
  *   dropped branch of a residual block. With p > 0 both LayerNorm entries take cols <= 12288. fsb_layernorm_bwd_dropout: fsb_layernorm_bwd that also writes dbranch = dx * Z / (1 - p)
  *   (dx already includes dres), the gradient of the branch x, beside dx, the gradient of the sum (and of the residual).

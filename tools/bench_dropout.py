@@ -11,8 +11,10 @@ Shapes: C3 attention = micro-batch 32 x 512, 32 heads, head dim 64; C1 attention
 Randeng-T5-784M width (d 1024, 16 heads x 64, d_ff 2816) at 32 x (enc 512 + dec 512): attention of the encoder (relative bias +
 padding mask), of the decoder (the causal flag at p = 0 against the causal mask folded into the bias at p = 0.1, which is what the
 model runs) and cross-attention; RMSNorm with a residual and the gated GeLU over the 16384 tokens; a 4 + 4-layer step with its
-peak memory. Prints one
-JSON line; card name and power limit come from nvidia-smi in the same process."""
+peak memory. C2 = Wenzhong-GPT2-110M (12 layers, hidden 768, 12 heads x 64) at 32 x 1024: causal attention at p = 0 and p = 0.1
+(the causal flag, which is what the model runs), the same attention at p = 0.1 with the causal mask folded into a bias vector
+instead (the mT5 route, for reference; no bias gradient), and the 12-layer step with all three probabilities 0 against 0.1.
+Prints one JSON line; card name and power limit come from nvidia-smi in the same process."""
 import argparse
 import json
 import math
@@ -115,6 +117,71 @@ def attention_t5(B, S, H, D, iters=50):
         out[name] = {f"p={p}": {"fwd_ms": statistics.median(x[0] for x in v), "bwd_ms": statistics.median(x[1] for x in v)}
                      for p, v in res.items()}
     return out
+
+
+def attention_gpt2(B, S, H, D, iters=50):
+    """C2 causal self-attention: the causal flag at p = 0 and p = 0.1, and the causal mask folded into a bias at p = 0.1."""
+    g = torch.Generator().manual_seed(0)
+    qkv = torch.randn(B, S, 3, H, D, generator=g).to(torch.bfloat16).cuda()
+    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+    dout = torch.randn(B, S, H, D, generator=g).to(torch.bfloat16).cuda()
+    folded = torch.zeros(H, 2 * S - 1, device="cuda")
+    folded[:, S:] = float("-inf")          # offsets k - q > 0
+    dq = torch.empty_like(qkv)
+    base = torch.zeros(1, dtype=torch.int64, device="cuda")
+    scale = 1.0 / math.sqrt(D)
+    forms = {"causal p=0.0": (0.0, True, None), "causal p=0.1": (0.1, True, None), "folded_bias p=0.1": (0.1, False, folded)}
+    res = {}
+    for _ in range(3):   # alternate the forms' windows
+        for name, (p, causal, rel) in forms.items():
+            drop = None if p == 0 else ops.Dropout(p, 1, base, 0)
+            if causal and drop is not None:   # what GPT-2 runs
+                fwd = lambda: ops.sdpa_causal_dropout_fwd(q, k, v, scale, drop)
+                bwd = lambda: ops.sdpa_causal_dropout_bwd(q, k, v, o, dout, lse, scale, dq[:, :, 0], dq[:, :, 1], dq[:, :, 2],
+                                                          drop)
+            else:
+                fwd = lambda: ops.sdpa_fwd(q, k, v, scale, causal, rel_bias=rel, drop=drop)
+                bwd = lambda: ops.sdpa_bwd(q, k, v, o, dout, lse, scale, causal, dq[:, :, 0], dq[:, :, 1], dq[:, :, 2],
+                                           rel_bias=rel, drop=drop)
+            o, lse = fwd()
+            f = kernel_ms(fwd, iters)
+            b = kernel_ms(bwd, iters)
+            res.setdefault(name, []).append((f, b))
+    return {name: {"fwd_ms": statistics.median(x[0] for x in v), "bwd_ms": statistics.median(x[1] for x in v)}
+            for name, v in res.items()}
+
+
+def step_gpt2(B, S, steps):
+    """The 12-layer C2 step (Wenzhong-GPT2-110M) on one micro-batch of B x S: tokens per second with embd_pdrop, attn_pdrop
+    and resid_pdrop all 0 against all 0.1."""
+    from fsb200.models.gpt2 import GPT2LMHeadModel
+    from fsb200.trainer import PretrainStep
+    cfg = dict(vocab_size=50264, n_positions=1024, n_embd=768, n_layer=12, n_head=12, layer_norm_epsilon=1e-5,
+               initializer_range=0.02, activation_function="gelu_new")
+    g = torch.Generator().manual_seed(1)
+    ids = torch.randint(1, cfg["vocab_size"] - 8, (B, S), generator=g).cuda()
+    batch = {"input_ids": ids, "labels": ids.clone()}
+    runs = {}
+    for p in (0.0, 0.1):
+        torch.manual_seed(0)
+        model = GPT2LMHeadModel(SimpleNamespace(embd_pdrop=p, attn_pdrop=p, resid_pdrop=p, **cfg), device="cuda")
+        runs[p] = PretrainStep(model, lambda s_: 1e-4, lr=1e-4, weight_decay=0.1, grad_clip=0.0)
+        for _ in range(3):
+            runs[p].step_device([batch])
+    torch.cuda.synchronize()
+    res = {}
+    for _ in range(3):
+        for p in (0.0, 0.1):
+            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            ev0.record()
+            for _ in range(steps):
+                runs[p].step_device([batch])
+            ev1.record()
+            torch.cuda.synchronize()
+            res.setdefault(p, []).append(B * S * steps / (ev0.elapsed_time(ev1) / 1e3))
+    del runs
+    torch.cuda.empty_cache()
+    return {f"p={p}": {"tokens_per_s": statistics.median(v)} for p, v in res.items()}
 
 
 def pointwise_t5(T, d, ff, iters=50):
@@ -239,7 +306,9 @@ def main():
            "step_C3_width_4_layers_32x512": step_throughput("C3", 32, 512, max(3, a.steps // 4)),
            "attention_C5_32x512_h16_d64": attention_t5(32, 512, 16, 64),
            "pointwise_C5_16384_tokens_d1024_ff2816": pointwise_t5(32 * 512, 1024, 2816),
-           "step_C5_width_4_4_layers_32x512": step_t5(32, 512, max(3, a.steps // 4))}
+           "step_C5_width_4_4_layers_32x512": step_t5(32, 512, max(3, a.steps // 4)),
+           "attention_C2_32x1024_h12_d64": attention_gpt2(32, 1024, 12, 64),
+           "step_C2_gpt2_110m_32x1024": step_gpt2(32, 1024, max(3, a.steps // 2))}
     line = json.dumps(out)
     print(line)
     if a.out:
