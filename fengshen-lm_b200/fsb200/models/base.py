@@ -138,6 +138,42 @@ class FlatModel(nn.Module):
         if hook is not None:
             hook()
 
+    # ---- dropout ----------------------------------------------------------------------------------------------------
+    # Masks come from Philox (include/fsb200.h): a seed drawn once from torch.default_generator at construction (only when a
+    # probability is > 0) and a device stream counter that every training forward advances by its number of sites, so eager
+    # runs and replayed CUDA graphs draw the same fresh masks. In eval mode, or with every probability 0, the forward and
+    # backward run the dropout-free kernels.
+    def _dropout_probs(self, model, *keys):
+        """The config's dropout probabilities `keys` (absent or None: 0), each checked to lie in [0, 1)."""
+        probs = tuple(float(getattr(self.config, k, 0.0) or 0.0) for k in keys)
+        for k, v in zip(keys, probs):
+            if not 0.0 <= v < 1.0:
+                raise RuntimeError(f"fsb200 {model}: {k}={v} outside [0, 1)")
+        return probs
+
+    def _init_dropout(self, sites, probs):
+        """`sites` dropout sites per forward; the seed and the stream counter when one of `probs` is > 0, else None."""
+        self.dropout_sites = sites
+        self.dropout_seed, self.dropout_counter = None, None
+        if max(probs) > 0:
+            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
+            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=self.flat.params.device)
+
+    def _dropout_base(self):
+        """The stream base of this forward's masks, advancing the counter; None (no dropout) unless training with a seed."""
+        if not self.training or self.dropout_seed is None:
+            return None
+        return ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+
+    def _drop(self, base, p, site):
+        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
+        return None if base is None or p == 0.0 else ops.Dropout(p, self.dropout_seed, base, site)
+
+    def _refuse_dropout_generate(self, model, keys):
+        """generate runs without dropout: in training mode with a probability > 0 it raises (HF would drop)."""
+        if self.training and self.dropout_seed is not None:
+            raise RuntimeError(f"fsb200 {model}: generate in training mode with {keys} > 0 would drop; call model.eval() first")
+
     # ---- forward ----------------------------------------------------------------------------------------------------
     def _step_or_forward(self, has_labels, want_logits, *inputs):
         """-> (loss, *outputs). With labels under grad mode, the step node: `loss.backward()` then runs `_backward_impl`.

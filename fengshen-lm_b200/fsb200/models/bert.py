@@ -12,10 +12,7 @@ State-dict keys follow HF.
 Dropout (hidden_dropout_prob, attention_probs_dropout_prob; the two may differ) applies in training mode (`model.training`,
 also under no_grad), at HF's sites: the embeddings (BERT: after the LN; MegatronBERT: the sum, no LN), the attention
 probabilities, and the attention-output and FFN-output branches before their residual add — fused into the attention kernels
-and the LayerNorms that add the branch to the residual. Masks come from Philox (include/fsb200.h): a seed drawn once from
-torch.default_generator at construction (only when a probability is > 0) and a stream counter on the device that every training
-forward advances by its number of sites, so eager runs and replayed CUDA graphs draw the same fresh masks. In eval mode, or
-with both probabilities 0, the forward and backward are the dropout-free kernels.
+and the LayerNorms that add the branch to the residual. Seed, stream counter and eval mode as in fsb200/models/base.py.
 """
 import math
 from collections import namedtuple
@@ -27,7 +24,7 @@ from .. import lib as L
 from .. import ops
 from ..flat import FlatSpec
 from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd
-from .layers import Linear
+from .layers import Linear, apply_dropout, residual_norm_bwd
 
 _Layer = namedtuple("_Layer", "qkv attn_out inter out")   # attention.self q|k|v, attention.output.dense, intermediate, output
 
@@ -41,11 +38,7 @@ class _BertFamily(FlatModel):
         self.h, self.nl, self.nh, self.V = g("hidden_size"), g("num_hidden_layers"), g("num_attention_heads"), g("vocab_size")
         self.ff, self.npos, self.ntype = g("intermediate_size"), g("max_position_embeddings", 512), g("type_vocab_size", 2)
         self.eps = g("layer_norm_eps", 1e-12)
-        self.p_hidden = float(g("hidden_dropout_prob", 0.0) or 0.0)
-        self.p_attn = float(g("attention_probs_dropout_prob", 0.0) or 0.0)
-        for k, v in (("hidden_dropout_prob", self.p_hidden), ("attention_probs_dropout_prob", self.p_attn)):
-            if not 0.0 <= v < 1.0:
-                raise RuntimeError(f"fsb200 BERT: {k}={v} outside [0, 1)")
+        self.p_hidden, self.p_attn = self._dropout_probs("BERT", "hidden_dropout_prob", "attention_probs_dropout_prob")
         act = g("hidden_act", "gelu")
         if act not in ("gelu", "gelu_new"):
             raise RuntimeError(f"fsb200 BERT: hidden_act={act!r} not implemented (gelu, gelu_new)")
@@ -108,15 +101,7 @@ class _BertFamily(FlatModel):
         self.reset_parameters(seed)
         # dropout sites of one forward: 0 embeddings; for layer i, 1 + 3i attention probabilities, 2 + 3i attention output,
         # 3 + 3i FFN output
-        self.dropout_sites = 1 + 3 * self.nl
-        self.dropout_seed, self.dropout_counter = None, None
-        if self.p_hidden > 0 or self.p_attn > 0:
-            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
-            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=dev)
-
-    def _drop(self, base, p, site):
-        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
-        return None if base is None or p == 0.0 else ops.Dropout(p, self.dropout_seed, base, site)
+        self._init_dropout(1 + 3 * self.nl, (self.p_hidden, self.p_attn))
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -153,9 +138,7 @@ class _BertFamily(FlatModel):
         E = "bert.embeddings."
         scale = 1.0 / math.sqrt(hn)
         self._need("no_decay"); self._need("emb")
-        base = None
-        if self.training and self.dropout_seed is not None:
-            base = ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+        base = self._dropout_base()
         ph, pa = self.p_hidden, self.p_attn
         D = lambda p, site: self._drop(base, p, site)
         emb = ops.embedding_fwd(ids, P(E + "word_embeddings.weight").data, pos=pos,
@@ -167,8 +150,7 @@ class _BertFamily(FlatModel):
         else:
             x, st_e, _ = ops.layernorm_fwd(emb, P(E + "LayerNorm.weight").data, P(E + "LayerNorm.bias").data, self.eps)
             emb_ctx = (emb, st_e)
-        if D(ph, 0) is not None:
-            x = ops.dropout(x, D(ph, 0))
+        x = apply_dropout(x, D(ph, 0))
         for i, pj in enumerate(self._proj):
             p = f"bert.encoder.layer.{i}."
             self._need(f"layer{i}")
@@ -248,14 +230,6 @@ class _BertFamily(FlatModel):
         acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base = ctx
         ph, pa = self.p_hidden, self.p_attn
         D = lambda p, site: self._drop(base, p, site)
-
-        def ln_bwd(dy, x, w, b, st, drop, dres=None):
-            """(gradient of the LN input sum, gradient of its dropped branch) — the same tensor without dropout."""
-            if drop is None:
-                d = ops.layernorm_bwd(dy, x, w.data, st, w.main_grad, b.main_grad, accumulate=acc, dres=dres)
-                return d, d
-            return ops.layernorm_bwd_dropout(dy, x, w.data, st, w.main_grad, b.main_grad, drop, accumulate=acc, dres=dres)
-
         h, nh, hn, pre = self.h, self.nh, self.hn, self.PRE_LN
         T = B * S
         P = self.P
@@ -293,7 +267,7 @@ class _BertFamily(FlatModel):
                     P(n).main_grad.zero_()
         if pre:
             ew, eb = P("bert.encoder.ln.weight"), P("bert.encoder.ln.bias")
-            dx, dmb = ln_bwd(dhf, xf, ew, eb, stf, D(ph, 3 * self.nl))
+            dx, dmb = residual_norm_bwd(dhf, xf, ew, eb, stf, D(ph, 3 * self.nl), acc)
         else:
             dx = dhf
         self._done("head")          # after the final encoder LN: its weight gradient is in the head bucket
@@ -305,7 +279,7 @@ class _BertFamily(FlatModel):
             else:
                 x, qkv, o, lse, x1, st2, h2, prea, f, s2, st3 = acts[i]
                 lw, lb = P(p + "output.LayerNorm.weight"), P(p + "output.LayerNorm.bias")
-                dsum, dm = ln_bwd(dx, s2, lw, lb, st3, D(ph, 3 + 3 * i))   # d(h2 + drop(m)), d(m)
+                dsum, dm = residual_norm_bwd(dx, s2, lw, lb, st3, D(ph, 3 + 3 * i), acc)   # d(h2 + drop(m)), d(m)
                 dres_in = None
             acts[i] = None
             df = pj.out.backward(dm, f, acc)
@@ -313,11 +287,11 @@ class _BertFamily(FlatModel):
             if pre:
                 dh2 = pj.inter.backward(dprea, h2, acc, colsum=False)
                 lw, lb = P(p + "ln.weight"), P(p + "ln.bias")
-                dx1, da = ln_bwd(dh2, x1, lw, lb, st2, D(ph, 2 + 3 * i), dres=dres_in)
+                dx1, da = residual_norm_bwd(dh2, x1, lw, lb, st2, D(ph, 2 + 3 * i), acc, dres=dres_in)
             else:
                 pj.inter.backward(dprea, h2, acc, dx=dsum, dx_accumulate=True, colsum=False)   # dh2 = d(h2+m) + dgrad(fc1)
                 lw, lb = P(p + "attention.output.LayerNorm.weight"), P(p + "attention.output.LayerNorm.bias")
-                dsum, da = ln_bwd(dsum, x1, lw, lb, st2, D(ph, 2 + 3 * i))       # d(x + drop(a)), d(a)
+                dsum, da = residual_norm_bwd(dsum, x1, lw, lb, st2, D(ph, 2 + 3 * i), acc)       # d(x + drop(a)), d(a)
             do = pj.attn_out.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
@@ -327,12 +301,11 @@ class _BertFamily(FlatModel):
                 dh1 = pj.qkv.backward(dqkv, h1, acc)
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")
                 # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped FFN output into x
-                dx, dmb = ln_bwd(dh1, x, lw, lb, st1, D(ph, 3 * i) if i > 0 else None, dres=dx1)
+                dx, dmb = residual_norm_bwd(dh1, x, lw, lb, st1, D(ph, 3 * i) if i > 0 else None, acc, dres=dx1)
             else:
                 dx = pj.qkv.backward(dqkv, x, acc, dx=dsum, dx_accumulate=True)   # dx_in = d(x+a) + dgrad(qkv)
             self._done(f"layer{i}")
-        if D(ph, 0) is not None:
-            dx = ops.dropout(dx, D(ph, 0))
+        dx = apply_dropout(dx, D(ph, 0))
         if not pre:
             emb, st_e = emb_ctx
             lw, lb = P(E + "LayerNorm.weight"), P(E + "LayerNorm.bias")

@@ -8,12 +8,9 @@ cross-entropy with ignore_index -100. State-dict keys follow HF (`transformer.h.
 Conv1D's [in, out] layout maps onto the GEMM layouts without any transpose: forward = NN, dgrad = NT, wgrad = TN.
 Dropout (`embd_pdrop`, `attn_pdrop`, `resid_pdrop`, each in [0, 1) and independent) applies in training mode
 (`model.training`, also under no_grad), at HF's sites: the embedding sum, the attention probabilities (inside the causal
-attention kernels: ops.sdpa_causal_dropout_fwd / _bwd) and the attention / MLP `c_proj` outputs, dropped by the LayerNorm
-that adds them to the residual stream (`ln_2`, the next block's `ln_1`, `ln_f`). Masks come from Philox (include/fsb200.h): a seed drawn once from
-torch.default_generator at construction (only when a probability is > 0) and a device stream counter that every training
-forward advances by its number of sites, so eager runs and replayed CUDA graphs draw the same fresh masks. In eval mode, or
-with all three probabilities 0, the forward and backward are the dropout-free kernels; `generate` in training mode with a
-non-zero probability is rejected (HF would drop).
+attention kernels) and the attention / MLP `c_proj` outputs, dropped by the LayerNorm that adds them to the residual stream
+(`ln_2`, the next block's `ln_1`, `ln_f`). Seed, stream counter and eval mode as in fsb200/models/base.py; `generate` in
+training mode with a non-zero probability is rejected (HF would drop).
 """
 import math
 from collections import namedtuple
@@ -27,7 +24,7 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd
-from .layers import Linear
+from .layers import Linear, apply_dropout, residual_norm_bwd
 
 _Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
 
@@ -41,10 +38,7 @@ class GPT2LMHeadModel(FlatModel):
         self.V, self.npos = g("vocab_size"), g("n_positions", g("max_position_embeddings", 1024))
         self.eps = g("layer_norm_epsilon", 1e-5)
         self.inner = g("n_inner") or 4 * self.h
-        self.p_embd, self.p_attn, self.p_resid = (float(g(k, 0.0) or 0.0) for k in ("embd_pdrop", "attn_pdrop", "resid_pdrop"))
-        for k, v in (("embd_pdrop", self.p_embd), ("attn_pdrop", self.p_attn), ("resid_pdrop", self.p_resid)):
-            if not 0.0 <= v < 1.0:
-                raise RuntimeError(f"fsb200 GPT2: {k}={v} outside [0, 1)")
+        self.p_embd, self.p_attn, self.p_resid = self._dropout_probs("GPT2", "embd_pdrop", "attn_pdrop", "resid_pdrop")
         if g("activation_function", "gelu_new") != "gelu_new":
             raise RuntimeError("fsb200 GPT2: only activation_function='gelu_new' is implemented")
         h, V = self.h, self.V
@@ -75,15 +69,7 @@ class GPT2LMHeadModel(FlatModel):
         self.reset_parameters(seed)
         # dropout sites of one forward, in transformers' call order: 0 embeddings; for layer i, 1 + 3i attention probabilities,
         # 2 + 3i attention c_proj output, 3 + 3i MLP c_proj output. A site whose probability is 0 keeps its number.
-        self.dropout_sites = 1 + 3 * self.nl
-        self.dropout_seed, self.dropout_counter = None, None
-        if max(self.p_embd, self.p_attn, self.p_resid) > 0:
-            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
-            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=self.flat.params.device)
-
-    def _drop(self, base, p, site):
-        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
-        return None if base is None or p == 0.0 else ops.Dropout(p, self.dropout_seed, base, site)
+        self._init_dropout(1 + 3 * self.nl, (self.p_embd, self.p_attn, self.p_resid))
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -113,15 +99,11 @@ class GPT2LMHeadModel(FlatModel):
     def _forward_impl(self, ids, pos, mask, lab, B, S, save, want_logits):
         scale = 1.0 / math.sqrt(self.hn)
         acts = [] if save else None
-        base = None
-        if self.training and self.dropout_seed is not None:
-            base = ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+        base = self._dropout_base()
 
         def attend(i, q5):
-            drop = self._drop(base, self.p_attn, 1 + 3 * i)
-            if drop is None:
-                return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask)
-            return ops.sdpa_causal_dropout_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, drop, kv_mask=mask)
+            return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask,
+                                drop=self._drop(base, self.p_attn, 1 + 3 * i))
         hf, stf, xf = self._stack(ids, pos, B, S, attend, acts, base)
         logits = self._head(hf)
         loss, ctx = None, None
@@ -144,9 +126,8 @@ class GPT2LMHeadModel(FlatModel):
         pr = self.p_resid
         D = lambda p, site: self._drop(base, p, site)
         self._need("no_decay"); self._need("wte")
-        x = ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S)
-        if D(self.p_embd, 0) is not None:
-            x = ops.dropout(x, D(self.p_embd, 0))
+        x = apply_dropout(ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S),
+                          D(self.p_embd, 0))
         prev_m = None
         for i, (blk, pj) in enumerate(zip(tr.h, self._proj)):
             self._need(f"layer{i}")
@@ -182,9 +163,7 @@ class GPT2LMHeadModel(FlatModel):
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded. Runs without
         dropout; in training mode with a non-zero dropout probability it raises (HF would drop)."""
-        if self.training and self.dropout_seed is not None:
-            raise RuntimeError("fsb200 GPT2: generate in training mode with embd_pdrop / attn_pdrop / resid_pdrop > 0 would "
-                               "drop; call model.eval() first")
+        self._refuse_dropout_generate("GPT2", "embd_pdrop / attn_pdrop / resid_pdrop")
         dev = self.flat.params.device
         ids = input_ids.to(device=dev, dtype=torch.int64)
         B, S0 = ids.shape
@@ -246,16 +225,6 @@ class GPT2LMHeadModel(FlatModel):
         acc = self.accumulate_grads
         pr = self.p_resid
         D = lambda p, site: self._drop(base, p, site)
-
-        def ln_bwd(dy, x, ln, st, drop, dres=None):
-            """(gradient of the LN input sum, gradient of its dropped branch) — the same tensor without dropout."""
-            if drop is None:
-                d = ops.layernorm_bwd(dy, x, ln.weight.data, st, ln.weight.main_grad, ln.bias.main_grad, accumulate=acc,
-                                      dres=dres)
-                return d, d
-            return ops.layernorm_bwd_dropout(dy, x, ln.weight.data, st, ln.weight.main_grad, ln.bias.main_grad, drop,
-                                             accumulate=acc, dres=dres)
-
         self._begin_backward()
         tr = self.transformer
         scale = 1.0 / math.sqrt(hn)
@@ -263,7 +232,8 @@ class GPT2LMHeadModel(FlatModel):
             ops.scale_inplace(dlogits, gloss)  # upstream scalar; the kernel exits immediately when it is 1.0
         dhf = self._head.backward(dlogits, hf, acc)   # tied head: written first, the embedding adds later
         del dlogits
-        dx, dm = ln_bwd(dhf, xf, tr.ln_f, stf, D(pr, 3 * self.nl))     # d(residual), d(last MLP output)
+        # d(residual), d(last MLP output)
+        dx, dm = residual_norm_bwd(dhf, xf, tr.ln_f.weight, tr.ln_f.bias, stf, D(pr, 3 * self.nl), acc)
         for i in reversed(range(self.nl)):
             blk, pj = tr.h[i], self._proj[i]
             x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f = acts[i]
@@ -271,23 +241,18 @@ class GPT2LMHeadModel(FlatModel):
             df = pj.mlp_proj.backward(dm, f, acc)
             dpre = ops.act_bwd_bias(L.ACT_GELU_TANH, df, pre, pj.c_fc.bias_grad, accumulate=acc)   # dGELU + c_fc bias grad
             dh2 = pj.c_fc.backward(dpre, h2, acc, colsum=False)
-            dx1, da = ln_bwd(dh2, x1, blk.ln_2, st2, D(pr, 2 + 3 * i), dres=dx)
+            dx1, da = residual_norm_bwd(dh2, x1, blk.ln_2.weight, blk.ln_2.bias, st2, D(pr, 2 + 3 * i), acc, dres=dx)
             do = pj.attn_proj.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
-            drop = D(self.p_attn, 1 + 3 * i)
-            if drop is None:
-                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
-                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask)
-            else:
-                ops.sdpa_causal_dropout_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale,
-                                            d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop, kv_mask=mask)
+            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
+                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))
             dh1 = pj.c_attn.backward(dqkv, h1, acc)
             # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped MLP output into x
-            dx, dm = ln_bwd(dh1, x, blk.ln_1, st1, D(pr, 3 * i) if i > 0 else None, dres=dx1)
+            dx, dm = residual_norm_bwd(dh1, x, blk.ln_1.weight, blk.ln_1.bias, st1, D(pr, 3 * i) if i > 0 else None, acc,
+                                       dres=dx1)
             self._done(f"layer{i}")
-        if D(self.p_embd, 0) is not None:
-            dx = ops.dropout(dx, D(self.p_embd, 0))
+        dx = apply_dropout(dx, D(self.p_embd, 0))
         ops.embedding_bwd(ids, dx, tr.wte.weight.main_grad)  # accumulates onto the LM-head wgrad (tied weights)
         learned_pos_emb_bwd(pos, dx, tr.wpe.weight.main_grad, B, S, acc)
         self._done("wte")

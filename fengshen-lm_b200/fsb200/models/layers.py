@@ -53,6 +53,27 @@ class Linear:
         return dx
 
 
+def residual_norm_bwd(dy, x, weight, bias, stats, drop, accumulate, dres=None):
+    """Backward of a norm over the sum of a residual and a branch dropped by `drop` (LayerNorm; RMSNorm when `bias` is
+    None): -> (gradient of the sum, gradient of the dropped branch), the same tensor when `drop` is None. Writes the
+    parameters' gradients into their .main_grad, adding to them when `accumulate`; dres is added to the sum's gradient."""
+    if bias is None:
+        if drop is None:
+            d = ops.rmsnorm_bwd(dy, x, weight.data, stats, weight.main_grad, accumulate=accumulate, dres=dres)
+            return d, d
+        return ops.rmsnorm_bwd_dropout(dy, x, weight.data, stats, weight.main_grad, drop, accumulate=accumulate, dres=dres)
+    if drop is None:
+        d = ops.layernorm_bwd(dy, x, weight.data, stats, weight.main_grad, bias.main_grad, accumulate=accumulate, dres=dres)
+        return d, d
+    return ops.layernorm_bwd_dropout(dy, x, weight.data, stats, weight.main_grad, bias.main_grad, drop, accumulate=accumulate,
+                                     dres=dres)
+
+
+def apply_dropout(x, drop):
+    """x through the standalone dropout site `drop` (forward and backward alike); x itself when drop is None."""
+    return x if drop is None else ops.dropout(x, drop)
+
+
 class GatedMLP:
     """m = wo(act(gate) * up) with [gate | up] = wi(h): wi is one projection over the adjacent gate and up weights, `act` the
     gate's activation (L.ACT_SILU for LLaMA, L.ACT_GELU_TANH for mT5). wi and wo are Linear or Fp8Linear."""

@@ -20,13 +20,11 @@ back the same way (deterministic diagonal sums inside the dQ kernel, csrc/attent
 every decoder layer's K|V-projection dgrad: accumulated in fp32 by the GEMM epilogue, rounded to bf16 once.
 Dropout (`dropout_rate`, in [0, 1)) applies in training mode (`model.training`, also under no_grad) at HF's sites, in HF's call
 order: the embeddings of each stack, the attention probabilities, the attention-output and FFN-output branches before their
-residual add, the gated activation before `wo`, and each stack's final-norm output. Philox masks as in bert.py: a seed drawn once
-from torch.default_generator at construction (only when the rate is > 0) and a device stream counter that every training forward
-advances by its number of sites. A branch is dropped by the RMSNorm that adds it to the residual stream, the gated activation by
-its kernel, the attention probabilities inside the attention kernels, the embeddings and final-norm outputs by the standalone
-dropout kernel. Under dropout the decoder self-attention passes its causal mask as -inf entries of the bias vector (T5 adds its
-causal mask to the position bias the same way) instead of the causal flag. In eval mode, or at rate 0, the forward and backward
-are the dropout-free kernels; `generate` in training mode with a non-zero rate is rejected (HF would drop).
+residual add, the gated activation before `wo`, and each stack's final-norm output. Seed, stream counter and eval mode as in
+fsb200/models/base.py. A branch is dropped by the RMSNorm that adds it to the residual stream, the gated activation by its
+kernel, the attention probabilities inside the attention kernels (the decoder's self-attention with the causal flag, at every
+rate), the embeddings and final-norm outputs by the standalone dropout kernel. `generate` in training mode with a non-zero rate
+is rejected (HF would drop).
 """
 import math
 from collections import namedtuple
@@ -41,7 +39,7 @@ from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from . import t5_bias as TB
 from .base import FlatModel, _Holder, flat_ids, key_mask
-from .layers import GatedMLP, Linear
+from .layers import GatedMLP, Linear, apply_dropout, residual_norm_bwd
 
 _Enc = namedtuple("_Enc", "qkv o mlp")             # a layer's projections: self-attention q|k|v and o, the gated FFN
 _Dec = namedtuple("_Dec", "qkv o cq ckv co mlp")   # ... and between them cross-attention q, k|v and o
@@ -62,9 +60,7 @@ class MT5ForConditionalGeneration(FlatModel):
         self.start_id = g("decoder_start_token_id", 0)
         if self.start_id is None:
             self.start_id = self.pad_id
-        self.p_drop = float(g("dropout_rate", 0.0) or 0.0)
-        if not 0.0 <= self.p_drop < 1.0:
-            raise RuntimeError(f"fsb200 MT5: dropout_rate={self.p_drop} outside [0, 1)")
+        self.p_drop, = self._dropout_probs("MT5", "dropout_rate")
         if g("feed_forward_proj", "gated-gelu") != "gated-gelu":
             raise RuntimeError("fsb200 MT5: only feed_forward_proj='gated-gelu' (T5 v1.1 / mT5) is implemented")
         # transformers 5.x FORCES tie_word_embeddings=True for MT5 configs (configuration_mt5.py __post_init__: "we have to tie
@@ -132,15 +128,7 @@ class MT5ForConditionalGeneration(FlatModel):
         # i: E + 1 + 6i self-attention probabilities, E + 2 + 6i its output, E + 3 + 6i cross-attention probabilities, E + 4 + 6i
         # its output, E + 5 + 6i gated activation, E + 6 + 6i FFN output; E + 1 + 6 Ld final-norm output.
         self.dec_site0 = 2 + 4 * self.ne
-        self.dropout_sites = 4 + 4 * self.ne + 6 * self.nd
-        self.dropout_seed, self.dropout_counter = None, None
-        if self.p_drop > 0:
-            self.dropout_seed = int(torch.randint(0, 2 ** 63 - 1, (1,), generator=torch.default_generator).item())
-            self.dropout_counter = torch.zeros(1, dtype=torch.int64, device=self.flat.params.device)
-
-    def _drop(self, base, site):
-        """The Dropout of one site of the forward whose stream base is `base` (None: no dropout in that forward)."""
-        return None if base is None or self.p_drop == 0.0 else ops.Dropout(self.p_drop, self.dropout_seed, base, site)
+        self._init_dropout(4 + 4 * self.ne + 6 * self.nd, (self.p_drop,))
 
     @torch.no_grad()
     def reset_parameters(self, seed=0):
@@ -200,10 +188,8 @@ class MT5ForConditionalGeneration(FlatModel):
         nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         Te = B * Se
-        D = lambda site: self._drop(base, site)
-        x, prev = ops.embedding_fwd(ids, P("shared.weight").data), None
-        if D(0) is not None:
-            x = ops.dropout(x, D(0))
+        D = lambda site: self._drop(base, self.p_drop, site)
+        x, prev = apply_dropout(ops.embedding_fwd(ids, P("shared.weight").data), D(0)), None
         eacts = []
         for i, pj in enumerate(self._enc):
             p = f"encoder.block.{i}.layer."
@@ -221,9 +207,7 @@ class MT5ForConditionalGeneration(FlatModel):
             x, prev = x1, m
         self._need("head")
         enc_h, rfe, xfe = self._norm(prev, x, "encoder.final_layer_norm.weight", D(4 * self.ne))
-        if D(1 + 4 * self.ne) is not None:
-            enc_h = ops.dropout(enc_h, D(1 + 4 * self.ne))
-        return eacts, enc_h, rfe, xfe
+        return eacts, apply_dropout(enc_h, D(1 + 4 * self.ne)), rfe, xfe
 
     def _decode(self, dec_ids, B, S, attend, cross_attend, acts=None, base=None):
         """Decoder stack over dec_ids [B * S] -> (final hidden states (after their dropout), their rstd, residual stream).
@@ -235,11 +219,9 @@ class MT5ForConditionalGeneration(FlatModel):
         P = self.P
         T = B * S
         E = self.dec_site0
-        D = lambda site: self._drop(base, site)
+        D = lambda site: self._drop(base, self.p_drop, site)
         self._need("no_decay"); self._need("shared")
-        y, prev = ops.embedding_fwd(dec_ids, P("shared.weight").data), None
-        if D(E) is not None:
-            y = ops.dropout(y, D(E))
+        y, prev = apply_dropout(ops.embedding_fwd(dec_ids, P("shared.weight").data), D(E)), None
         for i, pj in enumerate(self._dec):
             p = f"decoder.block.{i}.layer."
             self._need(f"dec{i}")
@@ -258,9 +240,7 @@ class MT5ForConditionalGeneration(FlatModel):
             y, prev = y2, m
         self._need("head")
         hf, rfd, xfd = self._norm(prev, y, "decoder.final_layer_norm.weight", D(E + 6 * self.nd))
-        if D(E + 1 + 6 * self.nd) is not None:
-            hf = ops.dropout(hf, D(E + 1 + 6 * self.nd))
-        return hf, rfd, xfd
+        return apply_dropout(hf, D(E + 1 + 6 * self.nd)), rfd, xfd
 
     # ---- KV-cache generation -----------------------------------------------------------------------------------------
     # transformers' GenerationMixin on MT5 (mt5_summary.py:41-49,131-139; finetune_t5.py:66-71). The encoder runs once; every
@@ -274,8 +254,7 @@ class MT5ForConditionalGeneration(FlatModel):
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); sequences start with
         decoder_start_token_id. Runs without dropout; in training mode with dropout_rate > 0 it raises (HF would drop)."""
-        if self.training and self.p_drop > 0:
-            raise RuntimeError("fsb200 MT5: generate in training mode with dropout_rate > 0 would drop; call model.eval() first")
+        self._refuse_dropout_generate("MT5", "dropout_rate")
         dev = self.flat.params.device
         nh, dk = self.nh, self.dk
         P = self.P
@@ -334,22 +313,13 @@ class MT5ForConditionalGeneration(FlatModel):
                                    self.nbuckets, self.maxdist)
         rel_d = TB.rel_bias_vector(P("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Sd, Sd, False,
                                    self.nbuckets, self.maxdist)
-        base = None
-        if self.training and self.dropout_seed is not None:
-            base = ops.dropout_advance(self.dropout_counter, self.dropout_sites)
+        base = self._dropout_base()
         E = self.dec_site0
-        D = lambda site: self._drop(base, site)
-        causal = True
-        if D(E) is not None:
-            # under dropout the decoder keeps its causal mask folded into the bias: -inf at the offsets k - q > 0 of the
-            # bias vector (index k - q + Sd - 1), as HF adds its causal mask to the position bias
-            rel_d = rel_d.clone()
-            rel_d[:, Sd:] = float("-inf")
-            causal = False
+        D = lambda site: self._drop(base, self.p_drop, site)
         eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save, base)
 
         def attend(i, q5):
-            return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, causal, rel_bias=rel_d, drop=D(E + 1 + 6 * i))
+            return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True, rel_bias=rel_d, drop=D(E + 1 + 6 * i))
 
         def cross_attend(i, qc):
             kvc = self._dec[i].ckv(enc_h)
@@ -366,33 +336,20 @@ class MT5ForConditionalGeneration(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, Sd, shift=0, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, causal, B, Se, Sd,
-                       base)
+                ctx = (eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, causal, B, Se, Sd, base = ctx
+        eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base = ctx
         d, nh, dk, inner = self.d, self.nh, self.dk, self.inner
         P = self.P
         Te, Td = B * Se, B * Sd
         acc = self.accumulate_grads
         dev = self.flat.params.device
         E = self.dec_site0
-        D = lambda site: self._drop(base, site)
-
-        def norm_bwd(dy, x, name, r, drop, dres=None):
-            """(gradient of the norm's input sum, gradient of its dropped branch) — the same tensor without dropout."""
-            s = P(name)
-            if drop is None:
-                g = ops.rmsnorm_bwd(dy, x, s.data, r, s.main_grad, accumulate=acc, dres=dres)
-                return g, g
-            return ops.rmsnorm_bwd_dropout(dy, x, s.data, r, s.main_grad, drop, accumulate=acc, dres=dres)
-
-        def undrop(g, site):
-            """gradient through a standalone dropout site"""
-            return g if D(site) is None else ops.dropout(g, D(site))
+        D = lambda site: self._drop(base, self.p_drop, site)
 
         self._begin_backward()
         if gloss is not None:
@@ -400,7 +357,8 @@ class MT5ForConditionalGeneration(FlatModel):
         dhf = self._head.backward(dlogits, hf, acc)   # tied head: written first, the embeddings add later
         del dlogits
         self._done("head")                      # lm_head is the bucket's only decayed parameter (the norms are no-decay)
-        dy, dm = norm_bwd(undrop(dhf, E + 1 + 6 * self.nd), xfd, "decoder.final_layer_norm.weight", rfd, D(E + 6 * self.nd))
+        dy, dm = residual_norm_bwd(apply_dropout(dhf, D(E + 1 + 6 * self.nd)), xfd, P("decoder.final_layer_norm.weight"), None,
+                                   rfd, D(E + 6 * self.nd), acc)
         drel_e = torch.zeros_like(rel_e)
         drel_d = torch.zeros_like(rel_d)
         denc32 = torch.empty((Te, d), dtype=torch.float32, device=dev)   # sum over decoder layers of the K|V dgrads
@@ -409,7 +367,7 @@ class MT5ForConditionalGeneration(FlatModel):
             y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms = dacts[i]
             dacts[i] = None
             dh3 = pj.mlp.backward(dm, ms, acc, drop=D(E + 5 + 6 * i))
-            dy2, dac = norm_bwd(dh3, y2, p + "2.layer_norm.weight", r3, D(E + 4 + 6 * i), dres=dy)
+            dy2, dac = residual_norm_bwd(dh3, y2, P(p + "2.layer_norm.weight"), None, r3, D(E + 4 + 6 * i), acc, dres=dy)
             # cross-attention
             doc = pj.co.backward(dac, oc.view(Td, inner), acc)
             dqc = torch.empty_like(qc)
@@ -419,33 +377,35 @@ class MT5ForConditionalGeneration(FlatModel):
                          dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1], kv_mask=mask, drop=D(E + 3 + 6 * i))
             dh2 = pj.cq.backward(dqc, h2, acc)
             pj.ckv.backward(dkvc, enc_h, acc, dx=denc32, dx_accumulate=(i != self.nd - 1))
-            dy1, da = norm_bwd(dh2, y1, p + "1.layer_norm.weight", r2, D(E + 2 + 6 * i), dres=dy2)
-            # causal self-attention with the decoder's relative-position bias (the causal mask folded into it under dropout)
+            dy1, da = residual_norm_bwd(dh2, y1, P(p + "1.layer_norm.weight"), None, r2, D(E + 2 + 6 * i), acc, dres=dy2)
+            # causal self-attention with the decoder's relative-position bias
             do = pj.o.backward(da, o.view(Td, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Sd, 3, nh, dk), dqkv.view(B, Sd, 3, nh, dk)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, causal,
+            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, True,
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], rel_bias=rel_d, drel_bias=drel_d, drop=D(E + 1 + 6 * i))
             dh1 = pj.qkv.backward(dqkv, h1, acc)
             # layer 0's norm had no residual (y = the embeddings); layer i's summed layer i-1's dropped FFN output into y
-            dy, dm = norm_bwd(dh1, y, p + "0.layer_norm.weight", r1, D(E + 6 * i) if i > 0 else None, dres=dy1)
+            dy, dm = residual_norm_bwd(dh1, y, P(p + "0.layer_norm.weight"), None, r1, D(E + 6 * i) if i > 0 else None, acc,
+                                       dres=dy1)
             if i == 0:
                 self._table_grad("decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", drel_d, Sd, False, acc)
             self._done(f"dec{i}")
-        ddec_emb = undrop(dy, E)                                          # gradient w.r.t. the decoder's input embeddings
+        ddec_emb = apply_dropout(dy, D(E))      # gradient w.r.t. the decoder's input embeddings
         # ---- encoder
         if self.nd > 0:
             denc = ops.cast_f32_to_bf16(denc32)
         else:
             denc = torch.zeros((Te, d), dtype=torch.bfloat16, device=dev)
         del denc32
-        dx, dm = norm_bwd(undrop(denc, 1 + 4 * self.ne), xfe, "encoder.final_layer_norm.weight", rfe, D(4 * self.ne))
+        dx, dm = residual_norm_bwd(apply_dropout(denc, D(1 + 4 * self.ne)), xfe, P("encoder.final_layer_norm.weight"), None,
+                                   rfe, D(4 * self.ne), acc)
         for i in reversed(range(self.ne)):
             p, pj = f"encoder.block.{i}.layer.", self._enc[i]
             x, r1, h1, qkv, o, lse, x1, r2, h2, ms = eacts[i]
             eacts[i] = None
             dh2 = pj.mlp.backward(dm, ms, acc, drop=D(3 + 4 * i))
-            dx1, da = norm_bwd(dh2, x1, p + "1.layer_norm.weight", r2, D(2 + 4 * i), dres=dx)
+            dx1, da = residual_norm_bwd(dh2, x1, P(p + "1.layer_norm.weight"), None, r2, D(2 + 4 * i), acc, dres=dx)
             do = pj.o.backward(da, o.view(Te, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Se, 3, nh, dk), dqkv.view(B, Se, 3, nh, dk)
@@ -453,11 +413,12 @@ class MT5ForConditionalGeneration(FlatModel):
                          d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, rel_bias=rel_e, drel_bias=drel_e,
                          drop=D(1 + 4 * i))
             dh1 = pj.qkv.backward(dqkv, h1, acc)
-            dx, dm = norm_bwd(dh1, x, p + "0.layer_norm.weight", r1, D(4 * i) if i > 0 else None, dres=dx1)
+            dx, dm = residual_norm_bwd(dh1, x, P(p + "0.layer_norm.weight"), None, r1, D(4 * i) if i > 0 else None, acc,
+                                       dres=dx1)
             if i == 0:
                 self._table_grad("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", drel_e, Se, True, acc)
             self._done(f"enc{i}")
-        dx = undrop(dx, 0)
+        dx = apply_dropout(dx, D(0))
         Wg = P("shared.weight").main_grad
         if not acc and not self.tied:
             Wg.zero_()

@@ -539,29 +539,12 @@ def _chk_rel(rel, H, Sq, Skv, name):
                            f"got {tuple(rel.shape)}")
 
 
-def _causal_dropout_refused(causal, drop, what):
-    if causal and drop is not None and drop.p > 0:
-        raise RuntimeError(f"fsb200 {what}: the causal flag with dropout p > 0 is not taken here (fold the mask into rel_bias, "
-                           f"as mT5 does, or call {what.replace('sdpa', 'sdpa_causal_dropout')})")
-
-
 def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop=None):
     """q,k,v: strided [B,S,H,D] bf16 views (e.g. slices of the packed QKV projection). Returns (out [B,Sq,H,D], lse).
-    rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias over the offset k - q (T5 relative-position bias).
-    drop: optional Dropout on the attention probabilities. With p > 0 causal must be False: a causal rel_bias (-inf at
-    offsets k - q > 0) expresses the same mask, and sdpa_causal_dropout_fwd runs the causal flag itself with dropout."""
-    _causal_dropout_refused(causal, drop, "sdpa_fwd")
-    return _sdpa_fwd(q, k, v, scale, causal, kv_mask, out, rel_bias, drop)
-
-
-def sdpa_causal_dropout_fwd(q, k, v, scale, drop, kv_mask=None, out=None):
-    """Causal attention (seq_q == seq_kv) with dropout on its probabilities, e.g. GPT-2's: sdpa_fwd's operands and result
-    with causal=True, and `drop` (a Dropout) taken together with the causal flag, so the key tiles wholly above the
-    diagonal stay skipped. The keep mask is the attention layout of include/fsb200.h."""
-    return _sdpa_fwd(q, k, v, scale, True, kv_mask, out, None, drop)
-
-
-def _sdpa_fwd(q, k, v, scale, causal, kv_mask, out, rel_bias, drop):
+    causal: mask the keys after each query (seq_q == seq_kv); the key tiles wholly above the diagonal are skipped.
+    kv_mask: optional uint8 [B, Skv] key-padding mask (0: masked). rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias
+    over the offset k - q (T5 relative-position bias). drop: optional Dropout on the attention probabilities, its keep mask
+    the attention layout of include/fsb200.h. The causal flag, kv_mask, rel_bias and drop compose."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -673,18 +656,8 @@ def kv_reorder(src, dst, index, kv_len):
 
 def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None, drop=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
-    rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=), deterministically.
-    drop: the forward's Dropout (same seed, base and site); with p > 0 causal must be False, as in sdpa_fwd."""
-    _causal_dropout_refused(causal, drop, "sdpa_bwd")
-    _sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, drop)
-
-
-def sdpa_causal_dropout_bwd(q, k, v, out, dout, lse, scale, dq, dk, dv, drop, kv_mask=None):
-    """Backward of sdpa_causal_dropout_fwd: sdpa_bwd's operands with causal=True and the forward's Dropout."""
-    _sdpa_bwd(q, k, v, out, dout, lse, scale, True, dq, dk, dv, kv_mask, None, None, drop)
-
-
-def _sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, drop):
+    causal, kv_mask and rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=),
+    deterministically. drop: the forward's Dropout (same seed, base and site)."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")

@@ -798,8 +798,7 @@ def _bhsd(t):
 def _scores(q, k, scale, causal, kv_mask, rel_bias, bs):
     """fp64 scores [nb, H, Sq, Skv] in natural-log units (masked: -inf) and the fp32 score error e_s of each: the D-deep
     fp32 dot product, D 2^-23 scale (|q||k|), plus 2^-22 (|scale q.k| + |bias|) for the scale, the bias fma and the
-    conversion to the log2 domain. A -inf bias (T5's causal mask folded into rel_bias under dropout) masks its position like
-    kv_mask does: score -inf, error 0."""
+    conversion to the log2 domain."""
     qd, kd = _bhsd(q[bs]).double(), _bhsd(k[bs]).double()
     D, Sq, Skv = q.shape[3], q.shape[1], k.shape[1]
     s = scale * (qd @ kd.transpose(-1, -2))
@@ -809,11 +808,8 @@ def _scores(q, k, scale, causal, kv_mask, rel_bias, bs):
         qi = torch.arange(Sq, device=q.device)[:, None]
         ki = torch.arange(Skv, device=q.device)[None, :]
         bias = rel_bias.double()[:, ki - qi + Sq - 1]           # [H, Sq, Skv]
-        fin = torch.isfinite(bias)                              # a folded causal mask: -inf, p = 0 and no error there
-        bias = torch.where(fin, bias, 0.0)
         s = s + bias
         e = e + 2.0 ** -22 * bias.abs()
-        keep = keep & fin[None]
     if causal:
         keep = keep & torch.ones((Sq, Skv), dtype=torch.bool, device=q.device).tril()
     if kv_mask is not None:

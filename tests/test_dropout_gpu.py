@@ -1,5 +1,6 @@
-"""GPU: dropout in the attention, LayerNorm and standalone kernels and in BERT / MegatronBERT training. Every mask is rebuilt
-by the numpy Philox of tests/philox_ref.py from the layout documented in include/fsb200.h, never read from the library."""
+"""GPU: dropout in the LayerNorm and standalone kernels and in BERT / MegatronBERT training (the attention dropout kernels
+against fp64: tests/test_attention_dropout_gpu.py). Every mask is rebuilt by the numpy Philox of tests/philox_ref.py from the
+layout documented in include/fsb200.h, never read from the library."""
 import math
 import os
 import sys
@@ -27,74 +28,20 @@ def _base(v):
     return torch.tensor([v], dtype=torch.int64, device=DEV)
 
 
-# ------------------------------------------------------------------------------------------------ attention
-def _ref_attention_dropout(q, k, v, scale, keep, p, kv_mask=None):
-    s = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale
-    if kv_mask is not None:
-        s = s.masked_fill(~kv_mask.bool()[:, None, None, :], float("-inf"))
-    pr = torch.softmax(s, -1)
-    pd = pr * keep / (1.0 - p)
-    return torch.einsum("bhqk,bkhd->bqhd", pd, v), torch.logsumexp(s, -1)
-
-
-@pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("S", [128, 200, 512])
-@pytest.mark.parametrize("masked", [False, True])
-@pytest.mark.parametrize("p", [0.1, 0.5])
-def test_sdpa_dropout_fwd_bwd_vs_fp64(D, S, masked, p):
-    B, Hh = 2, 2
-    g = torch.Generator().manual_seed(S + D)
-    qkv = torch.randn(B, S, 3, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-    mask = None
-    if masked:
-        mask = torch.ones(B, S, dtype=torch.uint8, device=DEV)
-        mask[0, S - 37:] = 0
-        mask[1, 5:21] = 0
-    scale = 1.0 / math.sqrt(D)
-    site, base = 3, _base(11)
-    drop = ops.Dropout(p, SEED, base, site)
-    out, lse = ops.sdpa_fwd(q, k, v, scale, False, kv_mask=mask, drop=drop)
-    dout = torch.randn(B, S, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    dqkv = torch.full_like(qkv, float("nan"))
-    ops.sdpa_bwd(q, k, v, out, dout, lse, scale, False, dqkv[:, :, 0], dqkv[:, :, 1], dqkv[:, :, 2], kv_mask=mask, drop=drop)
-    torch.cuda.synchronize()
-    keep = torch.from_numpy(R.attn_keep(SEED, 11 + site, B, Hh, S, S, p)).to(DEV, torch.float64)
-    qf, kf, vf = (t.double().detach().requires_grad_(True) for t in (q, k, v))
-    ref, ref_lse = _ref_attention_dropout(qf, kf, vf, scale, keep, p, mask)
-    assert (out.double() - ref).abs().max().item() < 2e-2 * max(1.0, ref.abs().max().item() / 4)
-    assert (lse.double() * math.log(2.0) - ref_lse).abs().max().item() < 2e-3
-    ref.backward(dout.double())
-    for name, got, want in (("dq", dqkv[:, :, 0], qf.grad), ("dk", dqkv[:, :, 1], kf.grad), ("dv", dqkv[:, :, 2], vf.grad)):
-        assert not torch.isnan(got.float()).any(), name
-        err = (got.double() - want).abs().max().item()
-        assert err < 3e-2 * max(1.0, want.abs().max().item()), f"{name}: {err}"
-
-
-def test_sdpa_dropout_rejects_causal_bias_and_bad_p():
-    q = torch.zeros(1, 128, 1, 64, dtype=torch.bfloat16, device=DEV)
-    with pytest.raises(RuntimeError, match="causal"):
-        ops.sdpa_fwd(q, q, q, 0.125, True, drop=ops.Dropout(0.1, 1, _base(0), 0))
+# ------------------------------------------------------------------------------------------------ op contract
+def test_sdpa_dropout_rejects_bad_p_and_long_sequences():
+    """p outside [0, 1) is refused when the Dropout is made; with p > 0 sequences are limited to 65536 (the attention mask
+    layout of include/fsb200.h), the causal flag included."""
     with pytest.raises(RuntimeError, match="outside"):
         ops.Dropout(1.0, 1, _base(0), 0)
+    k = torch.zeros(1, 65537, 1, 64, dtype=torch.bfloat16, device=DEV)
+    with pytest.raises(RuntimeError, match="65536"):
+        ops.sdpa_fwd(k, k, k, 0.125, True, drop=ops.Dropout(0.1, 1, _base(0), 0))
 
 
 def test_p_zero_entries_are_bit_identical_to_the_plain_ones():
-    B, S, Hh, D = 2, 200, 2, 64
     g = torch.Generator().manual_seed(0)
-    qkv = torch.randn(B, S, 3, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-    mask = torch.ones(B, S, dtype=torch.uint8, device=DEV)
-    mask[1, 150:] = 0
     d0 = ops.Dropout(0.0, 7, _base(0), 1)
-    o1, l1 = ops.sdpa_fwd(q, k, v, 0.125, False, kv_mask=mask)
-    o2, l2 = ops.sdpa_fwd(q, k, v, 0.125, False, kv_mask=mask, drop=d0)
-    assert torch.equal(o1, o2) and torch.equal(l1, l2)
-    dout = torch.randn(B, S, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    g1, g2 = torch.zeros_like(qkv), torch.zeros_like(qkv)
-    ops.sdpa_bwd(q, k, v, o1, dout, l1, 0.125, False, g1[:, :, 0], g1[:, :, 1], g1[:, :, 2], kv_mask=mask)
-    ops.sdpa_bwd(q, k, v, o1, dout, l1, 0.125, False, g2[:, :, 0], g2[:, :, 1], g2[:, :, 2], kv_mask=mask, drop=d0)
-    assert torch.equal(g1, g2)
     x = torch.randn(300, 768, generator=g).to(torch.bfloat16).to(DEV)
     r = torch.randn(300, 768, generator=g).to(torch.bfloat16).to(DEV)
     w = torch.randn(768, generator=g).to(torch.bfloat16).to(DEV)

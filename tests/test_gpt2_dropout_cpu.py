@@ -77,7 +77,7 @@ def _causal_dropout_autograd(q, k, v, scale, kvm, dout, m, causal=True):
     return o.detach(), lse.detach(), (qd.grad, kd.grad, vd.grad)
 
 
-def test_sdpa_causal_dropout_checkers():
+def test_causal_sdpa_dropout_checkers():
     """verify_sdpa_fwd / verify_sdpa_bwd with causal=True, a right-padding kv_mask and a DropSpec accept the exact answer and
     reject the mask of site + 1, a mask transposed in (q, k), a mask without its 1 / (1 - p), a stream that lost its high
     word, and an attention that ignores the causal mask."""

@@ -1,7 +1,7 @@
-"""GPU: GPT-2 dropout — causal + padding attention with dropout, and the model against transformers' GPT2LMHeadModel on
-replayed masks, in CUDA graphs, in generation, in the Wenzhong recipe and in a per-launch fp64 census at C2 width. Every mask
-is rebuilt by the numpy Philox of tests/philox_ref.py from the layout documented in include/fsb200.h, never read from the
-library."""
+"""GPU: GPT-2 dropout — the model against transformers' GPT2LMHeadModel on replayed masks, in CUDA graphs, in generation, in
+the Wenzhong recipe and in a per-launch fp64 census at C2 width (its causal attention against fp64:
+tests/test_attention_dropout_gpu.py). Every mask is rebuilt by the numpy Philox of tests/philox_ref.py from the layout
+documented in include/fsb200.h, never read from the library."""
 import copy
 import gc
 import math
@@ -25,99 +25,6 @@ from fsb200 import ops  # noqa: E402
 from fsb200.models.gpt2 import GPT2LMHeadModel  # noqa: E402
 
 DEV = "cuda"
-SEED = 0x2468_ACE0_1357_9BDF
-
-
-def _base(v):
-    return torch.tensor([v], dtype=torch.int64, device=DEV)
-
-
-# ------------------------------------------------------------------------------------------------ attention
-def _case(D, S, masked, seed):
-    B, Hh = 2, 2
-    g = torch.Generator().manual_seed(seed)
-    qkv = torch.randn(B, S, 3, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    mask = None
-    if masked:   # right padding, as a padded fine-tuning batch has it; row 1 ends inside a 128-row tile
-        mask = torch.ones(B, S, dtype=torch.uint8, device=DEV)
-        mask[1, S - 37:] = 0
-    dout = torch.randn(B, S, Hh, D, generator=g).to(torch.bfloat16).to(DEV)
-    return qkv, mask, dout
-
-
-def _run(qkv, mask, dout, scale, drop):
-    """Causal attention forward + backward: the plain entry points without `drop`, the causal-dropout ones with it."""
-    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-    dqkv = torch.full_like(qkv, float("nan"))
-    dq, dk, dv = dqkv[:, :, 0], dqkv[:, :, 1], dqkv[:, :, 2]
-    if drop is None:
-        out, lse = ops.sdpa_fwd(q, k, v, scale, True, kv_mask=mask)
-        ops.sdpa_bwd(q, k, v, out, dout, lse, scale, True, dq, dk, dv, kv_mask=mask)
-    else:
-        out, lse = ops.sdpa_causal_dropout_fwd(q, k, v, scale, drop, kv_mask=mask)
-        ops.sdpa_causal_dropout_bwd(q, k, v, out, dout, lse, scale, dq, dk, dv, drop, kv_mask=mask)
-    return out, lse, dqkv
-
-
-@pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("S", [128, 200, 1024])
-@pytest.mark.parametrize("masked", [False, True])
-@pytest.mark.parametrize("p", [0.1, 0.5])
-def test_sdpa_causal_dropout_vs_fp64(D, S, masked, p):
-    """S = 200 ends inside a query / key tile; the diagonal tiles are where the causal mask and the drop bits meet, in the
-    forward's two consumer warpgroups and the dK / dV kernel's transposed fragment."""
-    B, Hh = 2, 2
-    qkv, mask, dout = _case(D, S, masked, S + D)
-    scale = 1.0 / math.sqrt(D)
-    site, b0 = 4, (1 << 32) + 3          # a stream in the high word
-    drop = ops.Dropout(p, SEED, _base(b0), site)
-    out, lse, dqkv = _run(qkv, mask, dout, scale, drop)
-    torch.cuda.synchronize()
-    keep = torch.from_numpy(R.attn_keep(SEED, b0 + site, B, Hh, S, S, p)).to(DEV, torch.float64)
-    qf, kf, vf = (qkv[:, :, i].double().detach().requires_grad_(True) for i in range(3))
-    s = torch.einsum("bqhd,bkhd->bhqk", qf, kf) * scale
-    s = s.masked_fill(~torch.ones(S, S, dtype=torch.bool, device=DEV).tril(), float("-inf"))
-    if mask is not None:
-        s = s.masked_fill(~mask.bool()[:, None, None, :], float("-inf"))
-    ref = torch.einsum("bhqk,bkhd->bqhd", torch.softmax(s, -1) * keep / (1.0 - p), vf)
-    assert not torch.isnan(out.float()).any() and not torch.isnan(lse).any()
-    assert (out.double() - ref).abs().max().item() < 2e-2 * max(1.0, ref.abs().max().item() / 4)
-    assert (lse.double() * math.log(2.0) - torch.logsumexp(s, -1)).abs().max().item() < 2e-3
-    ref.backward(dout.double())
-    for name, got, want in (("dq", dqkv[:, :, 0], qf.grad), ("dk", dqkv[:, :, 1], kf.grad), ("dv", dqkv[:, :, 2], vf.grad)):
-        assert not torch.isnan(got.float()).any(), name
-        err = (got.double() - want).abs().max().item()
-        assert err < 3e-2 * max(1.0, want.abs().max().item()), f"{name}: {err}"
-    out2, lse2, dqkv2 = _run(qkv, mask, dout, scale, drop)
-    assert torch.equal(out, out2) and torch.equal(lse, lse2) and torch.equal(dqkv, dqkv2)   # deterministic
-
-
-def test_causal_p_zero_entries_are_bit_identical_to_the_plain_ones():
-    d0 = ops.Dropout(0.0, 7, _base(0), 1)
-    for masked in (False, True):
-        qkv, mask, dout = _case(64, 200, masked, 1)
-        a = _run(qkv, mask, dout, 0.125, None)
-        b = _run(qkv, mask, dout, 0.125, d0)
-        assert all(torch.equal(x, y) for x, y in zip(a, b)), masked
-
-
-def test_causal_dropout_entry_points_accept_what_sdpa_fwd_refuses():
-    """sdpa_fwd / sdpa_bwd keep refusing the causal flag with p > 0 (their callers fold the mask into rel_bias);
-    sdpa_causal_dropout_fwd / _bwd take exactly that call."""
-    q = torch.zeros(1, 128, 1, 64, dtype=torch.bfloat16, device=DEV)
-    drop = ops.Dropout(0.1, 1, _base(0), 0)
-    with pytest.raises(RuntimeError, match="causal"):
-        ops.sdpa_fwd(q, q, q, 0.125, True, drop=drop)
-    o, lse = ops.sdpa_causal_dropout_fwd(q, q, q, 0.125, drop)
-    dq = torch.full((1, 128, 3, 1, 64), float("nan"), dtype=torch.bfloat16, device=DEV)
-    with pytest.raises(RuntimeError, match="causal"):
-        ops.sdpa_bwd(q, q, q, o, q, lse, 0.125, True, dq[:, :, 0], dq[:, :, 1], dq[:, :, 2], drop=drop)
-    ops.sdpa_causal_dropout_bwd(q, q, q, o, q, lse, 0.125, dq[:, :, 0], dq[:, :, 1], dq[:, :, 2], drop)
-    torch.cuda.synchronize()
-    assert torch.isfinite(lse).all() and not torch.isnan(o.float()).any() and not torch.isnan(dq.float()).any()
-    with pytest.raises(RuntimeError, match="65536"):
-        k = torch.zeros(1, 65537, 1, 64, dtype=torch.bfloat16, device=DEV)
-        ops.sdpa_causal_dropout_fwd(k, k, k, 0.125, drop)
 
 
 # ------------------------------------------------------------------------------------------------ model
@@ -332,12 +239,13 @@ def test_wenzhong_recipe_with_dropout_trains(launched, tmp_path, monkeypatch):
         return rows
     monkeypatch.setattr(F, "qa_files", short_qa_files)
     seen = []
-    real_sdpa = ops.sdpa_causal_dropout_fwd
+    real_sdpa = ops.sdpa_fwd
 
-    def sdpa(q, k, v, scale, drop, kv_mask=None, **kw):
-        seen.append((kv_mask is not None, drop.p))
-        return real_sdpa(q, k, v, scale, drop, kv_mask=kv_mask, **kw)
-    monkeypatch.setattr(ops, "sdpa_causal_dropout_fwd", sdpa)
+    def sdpa(q, k, v, scale, causal, kv_mask=None, drop=None, **kw):
+        if causal and drop is not None:
+            seen.append((kv_mask is not None, drop.p))
+        return real_sdpa(q, k, v, scale, causal, kv_mask=kv_mask, drop=drop, **kw)
+    monkeypatch.setattr(ops, "sdpa_fwd", sdpa)
     # the recipe ends by comparing two no_grad forwards of one batch (its padding check); in training mode each would draw
     # its own masks, as transformers' would, so the model is evaluated in eval mode after fit
     real_fit = Trainer.fit
@@ -356,34 +264,7 @@ def test_wenzhong_recipe_with_dropout_trains(launched, tmp_path, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ per-launch census
-def check_sdpa_causal_dropout_fwd(real, bound, q, k, v, scale, drop, kv_mask=None, out=None):
-    """launch_refs.verify_sdpa_fwd of the causal call with its DropSpec."""
-    import launch_refs as LR
-    o, lse = ret = real(q, k, v, scale, drop, kv_mask=kv_mask, out=out)
-    LR.verify_sdpa_fwd(bound, q, k, v, scale, True, kv_mask, None, o, lse, LR.drop_spec(drop))
-    return ret
-
-
-def check_sdpa_causal_dropout_bwd(real, bound, q, k, v, out, dout, lse, scale, dq, dk, dv, drop, kv_mask=None):
-    """launch_refs.verify_sdpa_bwd of the causal call with its DropSpec."""
-    import launch_refs as LR
-    ret = real(q, k, v, out, dout, lse, scale, dq, dk, dv, drop, kv_mask=kv_mask)
-    LR.verify_sdpa_bwd(bound, q, k, v, out, dout, lse, scale, True, dq, dk, dv, kv_mask, None, None, None, LR.drop_spec(drop))
-    return ret
-
-
 def test_every_launch_of_a_gpt2_dropout_step_against_fp64(monkeypatch):
-    with pytest.MonkeyPatch.context() as mp:   # the census tables learn the two causal-dropout ops for this test only
-        import launch_census as C
-        real_shape = C._mask_shape
-        for op in ("sdpa_causal_dropout_fwd", "sdpa_causal_dropout_bwd"):
-            mp.setitem(C.DROP_KIND, op, "attention")
-        mp.setattr(C, "DROP_BACKWARD", C.DROP_BACKWARD | {"sdpa_causal_dropout_bwd"})
-        mp.setattr(C, "_mask_shape", lambda op, a: real_shape("sdpa_fwd" if op.startswith("sdpa_causal") else op, a))
-        _gpt2_dropout_census(monkeypatch)
-
-
-def _gpt2_dropout_census(monkeypatch):
     """One GPT-2 training step at C2 width (hidden 768, 12 heads, S 1024, 2 layers) with all three probabilities 0.1 and
     right-padded rows, every launch checked against fp64 (tests/launch_refs.py) as test_path_launches_gpu.py does for the
     BERT / T5 dropout steps; the stream counter is preset to 2^32 - 5 so that base + site carries into the high word."""
@@ -415,8 +296,7 @@ def _gpt2_dropout_census(monkeypatch):
     b["attention_mask"] = am
     b["labels"] = b["labels"].masked_fill(am == 0, -100)
     log = DropoutLog()
-    rec = Recorder(dict(LR.CHECKERS, sdpa_causal_dropout_fwd=check_sdpa_causal_dropout_fwd,
-                        sdpa_causal_dropout_bwd=check_sdpa_causal_dropout_bwd), extra_key=site_of, observe=log.observe)
+    rec = Recorder(LR.CHECKERS, extra_key=site_of, observe=log.observe)
     loss, growth = _run(monkeypatch, rec, lambda: stepper.step_device([b]))
     _finish(case, rec, growth, t0)
     assert math.isfinite(float(loss.item())), f"{case}: loss {loss.item()}"
@@ -427,7 +307,8 @@ def _gpt2_dropout_census(monkeypatch):
     assert not problems, f"{case}: " + "; ".join(problems[:5])
     checked_sites = {k[1][-1][1] for k in rec.checked if k[1] and k[1][-1][0] == "extra" and k[1][-1][1] is not None}
     assert checked_sites == set(range(n)), f"{case}: value-checked sites {sorted(checked_sites)}, want range({n})"
-    for op in ("sdpa_causal_dropout_fwd", "sdpa_causal_dropout_bwd"):
-        assert any(k[0] == op for k in rec.checked), f"{case}: no {op} call was checked"
+    for op in ("sdpa_fwd", "sdpa_bwd"):
+        assert any(k[0] == op and ("causal", True) in k[1] and ("drop", "Dropout") in k[1] for k in rec.checked), \
+            f"{case}: no causal {op} call carrying a drop was checked"
     del model, stepper, loss
     gc.collect(); torch.cuda.empty_cache()

@@ -537,12 +537,14 @@ def test_glu_dropout(act):
         _rejects(R.verify_glu_bwd, act, dout, gate, up, dg_, du_, d)
 
 
-def _attn_dropout_autograd(q, k, v, scale, rel, kvm, dout, m):
+def _attn_dropout_autograd(q, k, v, scale, causal, rel, kvm, dout, m):
     S = q.shape[1]
     qd, kd, vd = (R._bhsd(t).double().requires_grad_(True) for t in (q, k, v))
     relg = rel.double().requires_grad_(True)
     i = torch.arange(S)
     s = scale * qd @ kd.transpose(-1, -2) + relg[:, i[None, :] - i[:, None] + S - 1]
+    if causal:
+        s = s.masked_fill(~torch.ones(S, S, dtype=torch.bool).tril(), float("-inf"))
     if kvm is not None:
         s = s.masked_fill((kvm == 0)[:, None, None, :], float("-inf"))
     lse = torch.logsumexp(s, -1)
@@ -552,16 +554,14 @@ def _attn_dropout_autograd(q, k, v, scale, rel, kvm, dout, m):
     return o.detach(), lse.detach(), grads
 
 
-@pytest.mark.parametrize("causal_bias", [False, True], ids=["rel_bias", "folded_causal_bias"])
-def test_sdpa_dropout(causal_bias):
-    """Attention dropout with a rel_bias; with the decoder's causal mask folded into it as -inf the reference gives p = 0
-    and a zero tolerance there (no NaN)."""
+@pytest.mark.parametrize("causal", [False, True], ids=["rel_bias", "causal_rel_bias"])
+def test_sdpa_dropout(causal):
+    """Attention dropout with a rel_bias: with a padding mask (mT5's encoder) and with the causal flag (its decoder), where
+    the bias at the offsets k - q > 0 is finite and masked by the flag (no NaN)."""
     B, S, H, D = 2, 64, 2, 64
     q, k, v = _randn(B, S, H, D, seed=1), _randn(B, S, H, D, seed=2), _randn(B, S, H, D, seed=3)
     rel = (torch.randn(H, 2 * S - 1, generator=_g(4)) * 2).float()
-    if causal_bias:
-        rel[:, S:] = float("-inf")                 # offsets k - q > 0
-    kvm = None if causal_bias else torch.ones(B, S, dtype=torch.uint8)
+    kvm = None if causal else torch.ones(B, S, dtype=torch.uint8)
     if kvm is not None:
         kvm[1, 50:] = 0
     dout = _randn(B, S, H, D, seed=9)
@@ -571,19 +571,19 @@ def test_sdpa_dropout(causal_bias):
         z = philox_ref.attn_keep_t(dd.seed, dd.stream, range(B), H, S, S, dd.p).double()
         z = z.transpose(-1, -2) if transpose else z
         return z * R.keep_scale(dd.p) if scaled else z
-    o, lse, (dq, dk, dv, drel) = _attn_dropout_autograd(q, k, v, 1.0, rel, kvm, dout, mask(d))
+    o, lse, (dq, dk, dv, drel) = _attn_dropout_autograd(q, k, v, 1.0, causal, rel, kvm, dout, mask(d))
     O, L2 = R._bhsd(o).to(BF16), (lse / math.log(2.0)).float()
     assert not torch.isnan(O.float()).any()
-    fa = (q, k, v, 1.0, False, kvm, rel)
+    fa = (q, k, v, 1.0, causal, kvm, rel)
     _ok(R.verify_sdpa_fwd, *fa, O, L2, d)
     old = torch.zeros_like(rel)
-    ba = (q, k, v, O, dout, L2, 1.0, False)
+    ba = (q, k, v, O, dout, L2, 1.0, causal)
     DQ, DK, DV = (R._bhsd(t).to(BF16) for t in (dq, dk, dv))
     _ok(R.verify_sdpa_bwd, *ba, DQ, DK, DV, kvm, rel, drel.float(), old, d)
     faults = {"transposed (q, k)": mask(d, transpose=True)}
     faults.update({name: mask(*f(d)) for name, f in FAULTS.items()})
     for name, m in faults.items():
-        o_, lse_, (dq_, dk_, dv_, drel_) = _attn_dropout_autograd(q, k, v, 1.0, rel, kvm, dout, m)
+        o_, lse_, (dq_, dk_, dv_, drel_) = _attn_dropout_autograd(q, k, v, 1.0, causal, rel, kvm, dout, m)
         _rejects(R.verify_sdpa_fwd, *fa, R._bhsd(o_).to(BF16), L2, d)
         # the backward of a wrong mask, fed the right forward's O: dV alone already differs
         _rejects(R.verify_sdpa_bwd, *ba, DQ, DK, R._bhsd(dv_).to(BF16), kvm, rel, drel.float(), old, d)

@@ -1,5 +1,5 @@
-"""CPU: the mT5 dropout site table (fsb200/models/t5.py) against transformers' MT5 in training mode, and the decoder's causal
-mask folded into the relative-position bias vector, which is how the attention kernels see it under dropout."""
+"""CPU: the mT5 dropout site table (fsb200/models/t5.py) against transformers' MT5 in training mode, and the decoder's
+relative-position bias vector under the causal flag against HF's position bias plus causal mask."""
 import os
 import sys
 
@@ -62,7 +62,9 @@ def test_dropout_calls_follow_the_site_table(Le, Ld, monkeypatch):
 
 
 @pytest.mark.parametrize("S", [7, 40, 200])
-def test_folded_causal_bias_gives_hf_softmax(S):
+def test_hf_decoder_bias_is_rel_bias_under_the_causal_flag(S):
+    """HF's decoder self-attention adds position_bias + causal_mask to its scores: on and below the diagonal that is the
+    bias vector as the kernels index it (offset k - q), above it a mask, which the causal flag applies."""
     ref = _hf(H.MT5_SMALL, 0.0)
     nh = H.MT5_SMALL["num_heads"]
     att = ref.decoder.block[0].layer[0].SelfAttention
@@ -74,14 +76,15 @@ def test_folded_causal_bias_gives_hf_softmax(S):
     ids = torch.randint(2, H.MT5_SMALL["vocab_size"], (1, S))
     ref(input_ids=ids, labels=ids)
     hf_bias = seen["bias"][0]                                     # [heads, S, S]: position_bias + causal_mask
-    rel = TB.rel_bias_vector(att.relative_attention_bias.weight.detach(), S, S, False, 32, 128).clone()
-    rel[:, S:] = float("-inf")                                    # offsets k - q > 0 (index k - q + S - 1 >= S)
+    rel = TB.rel_bias_vector(att.relative_attention_bias.weight.detach(), S, S, False, 32, 128)
     q = torch.arange(S)[:, None]
     k = torch.arange(S)[None, :]
     mine = rel[:, k - q + S - 1]                                  # [heads, S, S] as the kernels index it
-    assert not torch.isinf(mine[:, :, 0]).any()                   # key 0 is never masked
+    causal = (k <= q).expand(S, S)
+    assert torch.equal(hf_bias[:, causal], mine[:, causal])
+    assert (hf_bias[:, ~causal] <= torch.finfo(hf_bias.dtype).min / 2).all()
     scores = torch.randn(nh, S, S, generator=torch.Generator().manual_seed(S))
     want = torch.softmax(scores + hf_bias, -1)
-    got = torch.softmax(scores + mine, -1)
+    got = torch.softmax((scores + mine).masked_fill(~causal, float("-inf")), -1)
     assert torch.allclose(got, want, atol=1e-6, rtol=0)
     assert torch.equal(got.triu(1), torch.zeros_like(got))        # exactly zero above the diagonal
