@@ -36,6 +36,7 @@ struct AttBwdParams {
   int seq_q, seq_kv, nheads, batch, causal;
   float scale, scale_log2;
   DropArgs drop;             // attention-probability dropout (kDropout only): the forward's seed, stream base and site
+  const int *seg_start, *seg_end;   // [batch, seq] segment bounds of each token (kSeg only; see fsb_sdpa_bwd_segments)
 };
 
 // ------------------------------------------------------------------------------------------------ delta preprocess
@@ -99,7 +100,8 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 
 // ================================================================================================ dQ kernel
 // kDropout: dS = P * (dP * Z / (1 - p) - delta), Z regenerated from philox.cuh (delta = rowsum(dO * O) is unchanged).
-template <int D, bool kBias, bool kDropout>
+// kSeg: as in attn_fwd_kernel, the key steps start at seg_start[q0] / AB_BN and each row also masks below its kmin.
+template <int D, bool kBias, bool kDropout, bool kSeg = false>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -116,6 +118,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int q0 = tile * AB_BM;
   const int n_all = (p.seq_kv + AB_BN - 1) / AB_BN;
   const int n_steps = p.causal ? min(n_all, (min(q0 + AB_BM, p.seq_q) + AB_BN - 1) / AB_BN) : n_all;
+  const int* seg_row = kSeg ? p.seg_start + int64_t(b) * p.seq_q : nullptr;
+  int j0 = 0;   // first key step, clamped into [0, q0]
+  if constexpr (kSeg) j0 = min(max(__ldg(seg_row + q0), 0), q0) / AB_BN;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
@@ -136,7 +141,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmQ, big_full, qc + h * 64, q0, b);
         tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmdO, big_full, dc + h * 64, q0, b);
       }
-      for (int j = 0; j < n_steps; ++j) {
+      for (int j = j0; j < n_steps; ++j) {
         const int st = ring.stage;
         ring.acquire();
         uint64_t* bar = ring.expect(2 * S::SML_BYTES);
@@ -162,7 +167,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const uint64_t dsc_kmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);  // MN-major view (dQ)
   const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
   const int n_rel = p.seq_q + p.seq_kv - 1;
-  int q_row[2], kmax[2];
+  int q_row[2], kmax[2], kmin[2] = {0, 0};
   float lse[2], delta[2];
   const float* brow[2];
 #pragma unroll
@@ -173,6 +178,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     lse[h] = ok ? p.lse[si] : INFINITY;
     delta[h] = ok ? p.delta[si] : 0.f;
     kmax[h] = p.causal ? min(q_row[h], p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
+    if constexpr (kSeg) kmin[h] = ok ? __ldg(seg_row + q_row[h]) : 0;   // first one
     // relative-position bias (mT5): this row reads entries (k - q_row + seq_q - 1) of its head's vector
     brow[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row[h], p.seq_q - 1)) : nullptr;
   }
@@ -185,8 +191,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   if constexpr (kDropout) dkey = drop_key(p.drop);
 
   mbar_wait(big_full, 0);
-  for (int j = 0; j < n_steps; ++j) {
-    const auto step = ring.at(j);
+  for (int j = j0; j < n_steps; ++j) {
+    const auto step = ring.at(j - j0);
     const uint64_t sto = uint64_t(step.stage) * (S::SML_BYTES >> 4);
     float s[32], dp[32];
     step.wait();
@@ -204,7 +210,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     wgmma_wait<0>();
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
-    const bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow;
+    const bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
+                           (kSeg && c0 < max(kmin[0], kmin[1]));
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
 #pragma unroll
@@ -215,6 +222,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         float pe = ex2_approx(x);
         if (need_mask) {
           bool keep = col <= kmax[h];
+          if constexpr (kSeg) keep = keep && col >= kmin[h];
           if (mrow != nullptr && keep) keep = mrow[col] != 0;
           pe = keep ? pe : 0.f;
         }
@@ -269,7 +277,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // ================================================================================================ dK / dV kernel
 // kDropout: dV += (P * Z / (1 - p))^T dO and dS^T = P^T * (dP^T * Z / (1 - p) - delta); a register row is a key row here, so
 // the mask comes from attn_drop_cols (same Philox calls as the row-major kernels, words picked along the other axis).
-template <int D, bool kBias, bool kDropout>
+// kSeg: key k is seen by the queries k <= q < seg_end[k]. The tile's last key has the largest end, so the query steps stop at
+// ceil(seg_end[last key] / AB_BN) (clamped into the sequence); each key row masks above its qmax = seg_end[k] - 1.
+template <int D, bool kBias, bool kDropout, bool kSeg = false>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -286,7 +296,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int kv0 = tile * AB_BM;
   const int n_q = (p.seq_q + AB_BN - 1) / AB_BN;
   const int i_start = p.causal ? min(n_q, kv0 / AB_BN) : 0;
-  const int n_steps = n_q - i_start;
+  const int* seg_row = kSeg ? p.seg_end + int64_t(b) * p.seq_kv : nullptr;
+  int i_end = n_q;
+  if constexpr (kSeg) i_end = min(n_q, (min(max(__ldg(seg_row + min(kv0 + AB_BM, p.seq_kv) - 1), 0), p.seq_q) + AB_BN - 1) / AB_BN);
+  const int n_steps = kSeg ? max(0, i_end - i_start) : n_q - i_start;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
@@ -344,6 +357,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     // relative-position bias: key row kv_row, query column qi -> entry (kv_row - qi + seq_q - 1) of the head's vector
     bkey[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (min(kv_row[h], p.seq_kv - 1) + p.seq_q - 1) : nullptr;
   }
+  // kSeg: the tile's first key has the smallest qmax (last query seeing it). Only the steps past it mask, and they re-read
+  // their rows' qmax from global memory: two more live registers would spill in the D = 128 kernel.
+  int qlim = 0;
+  if constexpr (kSeg) qlim = __ldg(seg_row + kv0) - 1;
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
@@ -373,6 +390,12 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
     const bool need_causal = p.causal && (qt0 < kv0 + AB_BM - 1);
+    const bool need_seg = kSeg && qt0 + AB_BN - 1 > qlim;
+    int qmax[2] = {0, 0};
+    if (need_seg) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) qmax[h] = row_ok[h] ? __ldg(p.seg_end + int64_t(b) * p.seq_kv + kv_row[h]) - 1 : -1;
+    }
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii) {
 #pragma unroll
@@ -387,7 +410,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
           float arg = s[4 * ii + e] * p.scale_log2 - lse_c;
           if constexpr (kBias) arg = fmaf(__ldg(bkey[h] - min(qi, p.seq_q - 1)), 1.4426950408889634f, arg);
           float x = ex2_approx(arg);
-          const bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]);
+          const bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]) && !(need_seg && qi > qmax[h]);
           x = keep ? x : 0.f;
           if constexpr (kDropout) {
             const bool z = (zbits >> (4 * ii + e)) & 1u;
@@ -471,14 +494,14 @@ static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq
   return size_t(batch) * nheads * n_qt * n_all * AB_DSTRIDE;
 }
 
-template <int D, bool kBias, bool kDropout>
+template <int D, bool kBias, bool kDropout, bool kSeg = false>
 static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                            int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
                            float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
   using SQ = AttBwdSmem<D, kBias>;
   using SK = AttBwdSmem<D, false>;
-  if (int rc = ensure_smem<attn_bwd_dq_kernel<D, kBias, kDropout>>(SQ::TOTAL, "sdpa_bwd")) return rc;
-  if (int rc = ensure_smem<attn_bwd_dkv_kernel<D, kBias, kDropout>>(SK::TOTAL, "sdpa_bwd")) return rc;
+  if (int rc = ensure_smem<attn_bwd_dq_kernel<D, kBias, kDropout, kSeg>>(SQ::TOTAL, "sdpa_bwd")) return rc;
+  if (int rc = ensure_smem<attn_bwd_dkv_kernel<D, kBias, kDropout, kSeg>>(SK::TOTAL, "sdpa_bwd")) return rc;
   // 1. delta
   {
     const int64_t groups = int64_t(p.batch) * p.seq_q * p.nheads;
@@ -503,7 +526,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   // 2. dQ
   {
     dim3 grid((p.seq_q + AB_BM - 1) / AB_BM, p.nheads, p.batch);
-    attn_bwd_dq_kernel<D, kBias, kDropout><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
+    attn_bwd_dq_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
     FSB_CUDA_LAUNCH_CHECK();
     if (kBias && drel_bias != nullptr) {
       const int n_rel = p.seq_q + p.seq_kv - 1, bs = dbias_bsplit(p.batch);
@@ -517,7 +540,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   // 3. dK, dV
   {
     dim3 grid((p.seq_kv + AB_BM - 1) / AB_BM, p.nheads, p.batch);
-    attn_bwd_dkv_kernel<D, kBias, kDropout><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
+    attn_bwd_dkv_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
     FSB_CUDA_LAUNCH_CHECK();
   }
   return FSB_OK;
@@ -534,7 +557,8 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
                     int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
                     int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
                     float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
-                    void* workspace, size_t workspace_bytes, const DropArgs* drop, fsb_stream_t st) {
+                    void* workspace, size_t workspace_bytes, const DropArgs* drop, const int* seg_start,
+                    const int* seg_end, fsb_stream_t st) {
   FSB_REQUIRE(q && k && v && o && dout && lse && delta && dq && dk && dv, "sdpa_bwd: null pointer");
   FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd: head_dim %d unsupported (64 or 128)", head_dim);
   FSB_REQUIRE(batch > 0 && seq_q > 0 && seq_kv > 0 && nheads > 0 && batch < 65536 && nheads < 65536, "sdpa_bwd: bad dims");
@@ -566,6 +590,15 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.do_head_stride = int(do_head_stride);
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
+  p.seg_start = seg_start; p.seg_end = seg_end;
+  if (seg_start != nullptr)   // fsb_sdpa_bwd_segments: causal, no bias, no dropout, no key mask
+    return head_dim == 128
+               ? launch_attn_bwd<128, false, false, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                          o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                          nullptr, (cudaStream_t)st)
+               : launch_attn_bwd<64, false, false, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                         nullptr, (cudaStream_t)st);
 #define FSB_BWD(DD, BB, DR)                                                                                              \
   launch_attn_bwd<DD, BB, DR>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride, do_row_stride,       \
                           o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
@@ -592,7 +625,7 @@ extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const v
                   k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
                   dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
-                  nullptr, st);
+                  nullptr, nullptr, nullptr, st);
 }
 
 extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
@@ -615,7 +648,27 @@ extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v,
                   k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
                   dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
-                  p > 0.f ? &d : nullptr, st);
+                  p > 0.f ? &d : nullptr, nullptr, nullptr, st);
+}
+
+extern "C" int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                     const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
+                                     int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
+                                     int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                     int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
+                                     int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                                     int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                                     int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
+                                     const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t st) {
+  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments: null segment bounds");
+  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
+              (long long)seq_kv);
+  FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd_segments: head_dim %d unsupported (64 or 128)", head_dim);
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, nullptr, seg_start,
+                  seg_end, st);
 }
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {

@@ -12,6 +12,8 @@ names (`llama.embed_in.word_embeddings.weight`, `llama.layers.N.attention.query_
     attention backward, norm backward with the residual-gradient add fused in).
 The causal mask is implicit (flash path semantics, transformer.py:441-448: `attention_mask` is not applied; identical to
 the `global` path when the mask is all ones — SURVEY.md Appendix B).
+Packed rows (several documents per row, fsb200/packing.py) pass `segment_ids`: attention then stays causal inside each
+segment and never crosses one (the varlen `cu_seqlens` semantics of the flash path, transformer.py:434-448).
 """
 import math
 from collections import namedtuple
@@ -298,7 +300,12 @@ class LlamaForCausalLM(FlatModel):
         return super().save_pretrained(path, **kw)
 
     # ---- forward ----------------------------------------------------------------------------------------------------
-    def forward(self, input_ids=None, attention_mask=None, position_ids=None, labels=None, return_logits=False, **_):
+    def forward(self, input_ids=None, attention_mask=None, position_ids=None, labels=None, return_logits=False,
+                segment_ids=None, **_):
+        """segment_ids: optional integer [B, S] (host or device) for packed rows; a segment is a maximal run of equal
+        consecutive values in a row. Every layer's attention is then causal inside each segment only, and the label of each
+        segment's first token is ignored (its prediction would cross a document boundary). Pass per-segment position_ids
+        (fsb200/packing.py emits them). None: one causal sequence per row, as before."""
         B, S = input_ids.shape
         dev = self.flat.params.device
         ids = flat_ids(input_ids, dev)
@@ -324,15 +331,28 @@ class LlamaForCausalLM(FlatModel):
         lab = flat_ids(labels, dev)
         if self.weight_format != "bf16" and lab is not None and torch.is_grad_enabled():
             raise _quantized_unsupported(self.weight_format, "a training forward (labels under grad mode)")
-        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S)
+        seg = ()
+        if segment_ids is not None:
+            if tuple(segment_ids.shape) != (B, S):
+                raise ValueError(f"segment_ids must be [batch, seq] = [{B}, {S}], got {tuple(segment_ids.shape)}")
+            seg_start, seg_end = ops.segment_bounds(segment_ids.to(device=dev, non_blocking=True))
+            if lab is not None:   # a segment's first token is not a target of the previous segment's last
+                first = (seg_start == torch.arange(S, dtype=torch.int32, device=dev)).view(-1)
+                lab = lab.masked_fill(first, -100)
+            seg = ((seg_start, seg_end),)
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S, *seg)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
 
-    def _forward_impl(self, ids, pos, lab, B, S, save, want_logits):
+    def _forward_impl(self, ids, pos, lab, B, S, seg=None, *, save, want_logits):
+        """seg: None or the (seg_start, seg_end) bounds of packed rows (ops.segment_bounds)."""
         scale = 1.0 / math.sqrt(self.hn)
         acts = [] if save else None
-        hf, rstdf, xf = self._stack(ids, pos, B, S, lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2],
-                                                                               scale, True), acts)
+        if seg is None:
+            attend = lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, True)
+        else:
+            attend = lambda i, q5: ops.sdpa_segments_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, *seg)
+        hf, rstdf, xf = self._stack(ids, pos, B, S, attend, acts)
         logits = self._head(hf)
         logits = self._tp_gather_columns(logits)   # ParallelLinear(parallel_output=False): full-vocabulary logits on every rank
         loss = None
@@ -342,7 +362,7 @@ class LlamaForCausalLM(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (acts, hf, rstdf, xf, dlogits, ids, pos, B, S)
+                ctx = (acts, hf, rstdf, xf, dlogits, ids, pos, B, S, seg)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
@@ -474,7 +494,7 @@ class LlamaForCausalLM(FlatModel):
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, hf, rstdf, xf, dlogits, ids, pos, B, S = ctx
+        acts, hf, rstdf, xf, dlogits, ids, pos, B, S, seg = ctx
         nh, hn, hl = self.nh_l, self.hn, self.h_l
         T = B * S
         acc = self.accumulate_grads
@@ -502,8 +522,12 @@ class LlamaForCausalLM(FlatModel):
             do = lp.dense.backward(dx1, os_, acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, nh, 3, hn), dqkv.view(B, S, nh, 3, hn)
-            ops.sdpa_bwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o, do.view(B, S, nh, hn), lse,
-                         1.0 / math.sqrt(hn), True, d5[:, :, :, 0], d5[:, :, :, 1], d5[:, :, :, 2])
+            if seg is None:
+                ops.sdpa_bwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o, do.view(B, S, nh, hn), lse,
+                             1.0 / math.sqrt(hn), True, d5[:, :, :, 0], d5[:, :, :, 1], d5[:, :, :, 2])
+            else:
+                ops.sdpa_segments_bwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o, do.view(B, S, nh, hn), lse,
+                                      1.0 / math.sqrt(hn), *seg, d5[:, :, :, 0], d5[:, :, :, 1], d5[:, :, :, 2])
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=0)
             ops.rope_inplace(dqkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, backward=True, offset=hn)
             dh1 = lp.qkv.backward(dqkv, h1s, acc)

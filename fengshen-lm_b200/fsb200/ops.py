@@ -683,3 +683,68 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
         L.call("fsb_sdpa_bwd", *args, _stream())
     else:
         L.call("fsb_sdpa_bwd_dropout", *args, *drop.args(), _stream())
+
+
+# ------------------------------------------------------------------------------------------------- packed sequences
+def segment_bounds(segment_ids):
+    """segment_ids: integer [B, S] (any device). A segment is a maximal run of equal consecutive values in a row, so every
+    integer tensor is valid. Returns (seg_start, seg_end), contiguous int32 [B, S] on segment_ids' device: the row position of
+    the first token of each token's segment and one past its last (include/fsb200.h, fsb_sdpa_fwd_segments). Torch ops
+    only, no host synchronisation: capturable in a CUDA graph."""
+    if segment_ids.dim() != 2 or segment_ids.dtype.is_floating_point or segment_ids.dtype.is_complex or \
+            segment_ids.dtype == torch.bool:
+        raise RuntimeError(f"fsb200: segment_ids must be an integer [batch, seq] tensor, got {segment_ids.dtype} "
+                           f"{tuple(segment_ids.shape)}")
+    B, S = segment_ids.shape
+    pos = torch.arange(S, dtype=torch.int32, device=segment_ids.device).expand(B, S)
+    first = torch.ones((B, S), dtype=torch.bool, device=segment_ids.device)   # token starts a segment
+    first[:, 1:] = segment_ids[:, 1:] != segment_ids[:, :-1]
+    last = torch.ones_like(first)                                              # token ends one
+    last[:, :-1] = first[:, 1:]
+    start = torch.cummax(torch.where(first, pos, 0), dim=1).values
+    end = torch.where(last, pos + 1, S).flip(1).cummin(dim=1).values.flip(1)
+    return start.to(torch.int32).contiguous(), end.to(torch.int32).contiguous()
+
+
+def _chk_bounds(seg_start, seg_end, B, S):
+    for t, n in ((seg_start, "seg_start"), (seg_end, "seg_end")):
+        _chk(t, torch.int32, n)
+        if tuple(t.shape) != (B, S) or not t.is_contiguous():
+            raise RuntimeError(f"fsb200: {n} must be contiguous int32 [batch, seq] = [{B}, {S}], got {tuple(t.shape)}")
+
+
+def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None):
+    """sdpa_fwd over rows that pack several sequences: causal inside each segment, nothing across segments. q, k, v as in
+    sdpa_fwd (seq_q == seq_kv); seg_start / seg_end from segment_bounds. Key / query tiles outside a tile's segments are
+    skipped. Returns (out [B, S, H, D], lse)."""
+    _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
+    B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
+    _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
+    _, _, _, _, v_rs, v_hs = _bshd(v, "v")
+    _chk_bounds(seg_start, seg_end, B, Sq)
+    if out is None:
+        out = torch.empty((B, Sq, H, D), dtype=_bf16, device=q.device)
+    _, _, _, _, o_rs, o_hs = _bshd(out, "out")
+    lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
+    L.call("fsb_sdpa_fwd_segments", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs,
+           k_hs, v_hs, o_hs, float(scale), _p(seg_start), _p(seg_end), _stream())
+    return out, lse
+
+
+def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv):
+    """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end); dq / dk / dv are written as in sdpa_bwd."""
+    B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
+    _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
+    _, _, _, _, v_rs, v_hs = _bshd(v, "v")
+    _, _, _, _, o_rs, o_hs = _bshd(out, "out")
+    _, _, _, _, do_rs, do_hs = _bshd(dout, "dout")
+    _, _, _, _, dq_rs, dq_hs = _bshd(dq, "dq")
+    _, _, _, _, dk_rs, dk_hs = _bshd(dk, "dk")
+    _, _, _, _, dv_rs, dv_hs = _bshd(dv, "dv")
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
+        _chk(t, _bf16, n)
+    _chk_bounds(seg_start, seg_end, B, Sq)
+    delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
+    L.call("fsb_sdpa_bwd_segments", _p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv),
+           B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs,
+           dk_hs, dv_hs, float(scale), _p(seg_start), _p(seg_end), _stream())

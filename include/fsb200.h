@@ -359,6 +359,32 @@ int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void
                          float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                          void* workspace, size_t workspace_bytes,
                          float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+/* ---- packed sequences (document-masked causal attention) -------------------------------------------------------------
+ * fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments: fsb_sdpa_fwd / fsb_sdpa_bwd with causal = 1 inside each segment of a row
+ * and nothing across segments, for rows that pack several documents. No kv_mask, rel_bias or dropout; seq_q == seq_kv;
+ * head_dim in {64, 128}. The bounds are two int32 [batch, seq] arrays, contiguous, indices relative to the row:
+ *   seg_start[b][t] : the position of the first token of t's segment;
+ *   seg_end[b][t]   : one past the position of its last token.
+ * Key k is visible to query q iff seg_start[q] <= k <= q (equivalently k <= q < seg_end[k]). The bounds are valid when every
+ * row is cut into contiguous segments [s, e) covering [0, seq) in order and both arrays hold each token's own segment.
+ * Then the key / query tiles wholly outside a tile's segments are never loaded: the forward and dQ pass start at the key
+ * tile of seg_start[first query of the tile], the dK / dV pass stops after the query tile of seg_end[last key of the tile].
+ * Invalid bounds give unspecified results but never an out-of-bounds access: the tile ranges are clamped into the
+ * sequence. The forward reads seg_start only; the backward needs the forward's seg_start and the matching seg_end. */
+int fsb_sdpa_fwd_segments(const void* q, const void* k, const void* v, void* o, float* lse,
+                          int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                          int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                          int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                          float scale, const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t stream);
+int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                          const float* lse, float* delta, void* dq, void* dk, void* dv,
+                          int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                          int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                          int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                          int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                          int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                          float scale, const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t stream);
+
 int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
                               void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
                               float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
