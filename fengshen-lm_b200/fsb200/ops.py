@@ -34,6 +34,13 @@ def _rows2d(t, name):
     return t.shape[0], t.shape[1], t.stride(0)
 
 
+def _span(t, n, name, what):
+    """Refuse t unless it is exactly the n contiguous elements the C entry addresses from its first element on."""
+    if not t.is_contiguous() or t.numel() != n:
+        raise RuntimeError(f"fsb200 {what}: {name} must be contiguous with {n} elements, got shape {tuple(t.shape)} "
+                           f"strides {t.stride()}")
+
+
 def workspace(nbytes, device, tag="default"):
     """Grow-only scratch buffer per (device, tag); caller-owned from the library's point of view."""
     key = (device, tag)
@@ -74,6 +81,7 @@ def gemm(layout, a, b, out=None, out_dtype=_bf16, bias=None, epilogue=L.EPI_NONE
     ldaux = 0
     if aux is not None:
         _chk(aux, _bf16, "aux")
+        if tuple(aux.shape) != (M, N): raise RuntimeError(f"fsb200 gemm: aux shape {tuple(aux.shape)} != ({M},{N})")
         _, _, ldaux = _rows2d(aux, "aux")
     ws, ws_bytes = None, 0
     if layout == L.GEMM_TN and bias is None and aux is None and epilogue == L.EPI_NONE:
@@ -268,6 +276,7 @@ def rmsnorm_fwd(x, scale, eps, residual=None, drop=None):
 
 def rmsnorm_bwd(dy, x, scale, rstd, dscale_out, accumulate=False, dres=None):
     rows, cols = x.shape
+    _span(dscale_out, cols, "dscale_out", "rmsnorm_bwd")
     dx = torch.empty_like(x)
     nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 0)
     ws = workspace(nbytes, x.device, "norm")
@@ -281,6 +290,7 @@ def rmsnorm_bwd_dropout(dy, x, scale, rstd, dscale_out, drop, accumulate=False, 
     """Backward of rmsnorm_fwd(..., residual, drop): returns (dx, dbranch) — the gradient of the sum (= of the residual)
     and the gradient of the dropped branch, dx * Z / (1 - p)."""
     rows, cols = x.shape
+    _span(dscale_out, cols, "dscale_out", "rmsnorm_bwd")
     dx = torch.empty_like(x)
     dbranch = torch.empty_like(x)
     nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 0)
@@ -309,6 +319,7 @@ def layernorm_fwd(x, gamma, beta, eps, residual=None, drop=None):
 
 def layernorm_bwd(dy, x, gamma, stats, dgamma_out, dbeta_out, accumulate=False, dres=None):
     rows, cols = x.shape
+    _span(dgamma_out, cols, "dgamma_out", "layernorm_bwd"); _span(dbeta_out, cols, "dbeta_out", "layernorm_bwd")
     dx = torch.empty_like(x)
     nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 1)
     ws = workspace(nbytes, x.device, "norm")
@@ -322,6 +333,7 @@ def layernorm_bwd_dropout(dy, x, gamma, stats, dgamma_out, dbeta_out, drop, accu
     """Backward of layernorm_fwd(..., residual, drop): returns (dx, dbranch) — the gradient of the sum (= of the residual)
     and the gradient of the dropped branch, dx * Z / (1 - p)."""
     rows, cols = x.shape
+    _span(dgamma_out, cols, "dgamma_out", "layernorm_bwd"); _span(dbeta_out, cols, "dbeta_out", "layernorm_bwd")
     dx = torch.empty_like(x)
     dbranch = torch.empty_like(x)
     nbytes = L.load().fsb_norm_bwd_workspace_bytes(rows, cols, 1)
@@ -353,6 +365,7 @@ def dropout_advance(counter, n):
     """Advance the device stream counter (int64 [1]) by n streams, on the device; returns the base this forward uses (a new
     int64 [1] device tensor, saved with the activations for the backward)."""
     _chk(counter, torch.int64, "dropout counter")
+    _span(counter, 1, "counter", "dropout_advance")
     saved = torch.empty(1, dtype=torch.int64, device=counter.device)
     L.call("fsb_dropout_advance", _p(counter), _p(saved), int(n), _stream())
     return saved
@@ -366,6 +379,8 @@ def dropout(x, drop, out=None):
         raise RuntimeError("fsb200 dropout: x must be contiguous")
     if out is None:
         out = torch.empty_like(x)
+    _chk(out, _bf16, "out")
+    _span(out, rows * cols, "out", "dropout")
     L.call("fsb_dropout", _p(x), _p(out), rows, cols, *drop.args(), _stream())
     return out
 
@@ -375,6 +390,10 @@ def rope_inplace(x, cos, sin, positions, nheads, head_dim, row_stride, head_stri
     """Rotate `nheads` heads per row in place. x is the flat packed buffer; `offset` (elements) selects q or k."""
     _chk(x, _bf16, "x")
     rows = positions.numel()
+    end = offset + (rows - 1) * row_stride + (nheads - 1) * head_stride + head_dim
+    if not x.is_contiguous() or offset < 0 or (rows > 0 and end > x.numel()):
+        raise RuntimeError(f"fsb200 rope_inplace: the heads addressed (up to element {end}) must lie inside the contiguous "
+                           f"x of {x.numel()} elements")
     L.call("fsb_rope_inplace", x.data_ptr() + 2 * offset, _p(cos), _p(sin), _p(positions), rows, nheads, head_dim,
            row_stride, head_stride, cos.shape[0], int(bool(backward)), _stream())
 
@@ -398,6 +417,9 @@ def glu_bwd(act, dout, gate, up, dgate, dup, drop=None):
     _, _, ldo = _rows2d(dout, "dout")
     _, _, ldg2 = _rows2d(dgate, "dgate")
     _, _, ldu2 = _rows2d(dup, "dup")
+    for t, n in ((up, "up"), (dout, "dout"), (dgate, "dgate"), (dup, "dup")):
+        if t.shape != gate.shape:
+            raise RuntimeError(f"fsb200 glu_bwd: {n} shape {tuple(t.shape)} != gate shape {tuple(gate.shape)}")
     args = (act, _p(dout), _p(gate), _p(up), _p(dgate), _p(dup), rows, cols, ldo, ldg, ldu, ldg2, ldu2)
     if drop is None:
         L.call("fsb_glu_bwd", *args, _stream())
@@ -424,6 +446,7 @@ def act_bwd_bias(act, dy, x, dbias, accumulate=False):
         raise RuntimeError("fsb200 act_bwd_bias: x and dy must be contiguous [rows, cols] of the same shape")
     rows, cols = x.shape
     dx = torch.empty_like(x)
+    _span(dbias, cols, "dbias", "act_bwd_bias")
     nbytes = L.load().fsb_act_bwd_bias_workspace_bytes(rows, cols)
     ws = workspace(nbytes, x.device, "act_bwd_bias")
     L.call("fsb_act_bwd_bias", act, _p(dy), _p(x), _p(dx), rows, cols, _p(dbias),
@@ -433,17 +456,21 @@ def act_bwd_bias(act, dy, x, dbias, accumulate=False):
 
 def add(a, b, out=None):
     if out is None: out = torch.empty_like(a)
+    for t, n in ((a, "a"), (b, "b"), (out, "out")):
+        _chk(t, _bf16, n); _span(t, a.numel(), n, "add")
     L.call("fsb_add", _p(a), _p(b), _p(out), a.numel(), _stream())
     return out
 
 
 def accumulate(acc32, x16, scale=1.0, overwrite=False):
     """acc32 (fp32) = (0 if overwrite else acc32) + scale * x16 (bf16)."""
+    _span(acc32, acc32.numel(), "acc32", "accumulate"); _span(x16, acc32.numel(), "x16", "accumulate")
     L.call("fsb_accumulate", _p(acc32), _p(x16), acc32.numel(), float(scale), int(bool(overwrite)), _stream())
 
 
 def scale_inplace(x16, scale_dev):
     """x16 (bf16, contiguous) *= scale_dev (0-d fp32 CUDA tensor); free when the scalar is 1."""
+    _span(x16, x16.numel(), "x16", "scale_inplace")
     if scale_dev.dtype != torch.float32 or not scale_dev.is_cuda:
         scale_dev = scale_dev.to(device=x16.device, dtype=torch.float32)
     L.call("fsb_scale_inplace", _p(x16), x16.numel(), _p(scale_dev), _stream())
@@ -452,6 +479,7 @@ def scale_inplace(x16, scale_dev):
 def colsum(x, out, accumulate=False):
     """out[c] (+)= sum_r x[r, c]; x bf16 [rows, cols] (unit inner stride); out bf16 or fp32 [cols]."""
     rows, cols, ld = _rows2d(x, "x")
+    _span(out, cols, "out", "colsum")
     nbytes = L.load().fsb_colsum_workspace_bytes(rows, cols)
     ws = workspace(nbytes, x.device, "colsum")
     L.call("fsb_colsum", _p(x), rows, cols, ld, _p(out), L.F32 if out.dtype == torch.float32 else L.BF16,
@@ -471,6 +499,9 @@ def embedding_bwd(ids, dout, dW, idx_mod=0):
     """dW[ids[t]] += dout[t]. With ids: deterministic — the ids are sorted (torch.sort: integer index plumbing) and every
     distinct row is summed in fp32 in a fixed order, one bf16 rounding. ids=None: row t % idx_mod (bf16 atomics)."""
     rows, cols = dout.shape
+    if dW.dim() != 2 or dW.shape[1] != cols or not dW.is_contiguous() or (ids is None and idx_mod > dW.shape[0]):
+        raise RuntimeError(f"fsb200 embedding_bwd: dW must be contiguous [rows, {cols}] (and hold idx_mod rows), got "
+                           f"{tuple(dW.shape)} strides {dW.stride()}")
     if ids is None:
         L.call("fsb_embedding_bwd", None, _p(dout), _p(dW), rows, cols, idx_mod, _stream())
         return
@@ -481,13 +512,16 @@ def embedding_bwd(ids, dout, dW, idx_mod=0):
 def cast_f32_to_bf16(x32, out=None):
     if out is None:
         out = torch.empty(x32.shape, dtype=_bf16, device=x32.device)
+    _chk(out, _bf16, "out")
+    _span(x32, x32.numel(), "x32", "cast_f32_to_bf16"); _span(out, x32.numel(), "out", "cast_f32_to_bf16")
     L.call("fsb_cast_f32_to_bf16", _p(x32), _p(out), x32.numel(), _stream())
     return out
 
 
 # ------------------------------------------------------------------------------------------------------ loss / optim
 def softmax_xent(logits, labels, seq_len, shift=1, ignore_index=-100, grad_scale=1.0, dlogits="inplace"):
-    """logits [rows, V] bf16 (rows = b*seq_len), labels int64 [rows]. Returns (loss scalar tensor, dlogits, n_valid)."""
+    """logits [rows, V] bf16 (rows = b*seq_len), labels int64 [rows]. Returns (loss scalar tensor, dlogits, n_valid).
+    dlogits: "inplace" (into logits), None / "none" (not computed) or a bf16 [rows, V] tensor with the logits' row stride."""
     _chk(logits, _bf16, "logits")
     rows, V, ld = _rows2d(logits, "logits")
     dev = logits.device
@@ -498,6 +532,11 @@ def softmax_xent(logits, labels, seq_len, shift=1, ignore_index=-100, grad_scale
         dl = logits if dlogits == "inplace" else None
     else:
         dl = dlogits
+    if dl is not None and dl is not logits:   # the entry writes dlogits with the logits' row stride (include/fsb200.h)
+        _chk(dl, _bf16, "dlogits")
+        if tuple(dl.shape) != (rows, V) or dl.stride(1) != 1 or (rows > 1 and dl.stride(0) != ld):
+            raise RuntimeError(f"fsb200 softmax_xent: dlogits must be bf16 [{rows}, {V}] with the logits' row stride {ld}, "
+                               f"got shape {tuple(dl.shape)} strides {dl.stride()}")
     L.call("fsb_softmax_xent_fwd_bwd", _p(logits), _p(labels), _p(dl), _p(row_loss), _p(loss), _p(n_valid), rows, V, ld,
            seq_len, shift, ignore_index, float(grad_scale), _stream())
     return loss, dl, n_valid
@@ -505,12 +544,17 @@ def softmax_xent(logits, labels, seq_len, shift=1, ignore_index=-100, grad_scale
 
 def adamw_flat(master, m, v, grad, param16, lr, beta1, beta2, eps, weight_decay, step, grad_scale=None, hyper=None):
     """hyper: optional fp32 CUDA tensor [lr, 1 - beta1^t, sqrt(1 - beta2^t)] read by the kernel instead of lr / step."""
+    n = master.numel()
+    for t, name in ((master, "master"), (m, "m"), (v, "v"), (grad, "grad"), (param16, "param16")):
+        if t is not None:
+            _span(t, n, name, "adamw_flat")
     L.call("fsb_adamw_flat", _p(master), _p(m), _p(v), _p(grad), L.F32 if grad.dtype == torch.float32 else L.BF16,
            _p(param16), master.numel(), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
            _p(grad_scale), _p(hyper), _stream())
 
 
 def sumsq(x, out, accumulate=False):
+    _span(x, x.numel(), "x", "sumsq"); _span(out, 1, "out", "sumsq")
     nbytes = L.load().fsb_sumsq_workspace_bytes()
     ws = workspace(nbytes, x.device, "sumsq")
     L.call("fsb_sumsq", _p(x), L.F32 if x.dtype == torch.float32 else L.BF16, x.numel(), _p(out), int(bool(accumulate)),
@@ -518,6 +562,9 @@ def sumsq(x, out, accumulate=False):
 
 
 def clip_coef(sumsq_t, max_norm, coef_out, norm_out=None):
+    _span(coef_out, 1, "coef_out", "clip_coef")
+    if norm_out is not None:
+        _span(norm_out, 1, "norm_out", "clip_coef")
     L.call("fsb_clip_coef", _p(sumsq_t), float(max_norm), _p(coef_out), _p(norm_out), _stream())
 
 
@@ -551,6 +598,7 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")
     if out is None:
         out = torch.empty((B, Sq, H, D), dtype=_bf16, device=q.device)
+    if tuple(out.shape) != (B, Sq, H, D): raise RuntimeError(f"fsb200: out shape {tuple(out.shape)} != {(B, Sq, H, D)}")
     _, _, _, _, o_rs, o_hs = _bshd(out, "out")
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     if kv_mask is not None:
@@ -654,6 +702,13 @@ def kv_reorder(src, dst, index, kv_len):
     L.call("fsb_kv_reorder", _p(src), _p(dst), _p(index), layers, rows, cap, slot, _p(kv_len), _stream())
 
 
+def _chk_grads(q, k, dq, dk, dv):
+    """dq has q's shape and dk / dv have k's: the backward writes every element of each."""
+    for t, ref, n in ((dq, q, "dq"), (dk, k, "dk"), (dv, k, "dv")):
+        if t.shape != ref.shape:
+            raise RuntimeError(f"fsb200: {n} shape {tuple(t.shape)} != {tuple(ref.shape)}")
+
+
 def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None, drop=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
     causal, kv_mask and rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=),
@@ -668,6 +723,7 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
     _, _, _, _, dv_rs, dv_hs = _bshd(dv, "dv")
     for t, n in ((dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
         _chk(t, _bf16, n)
+    _chk_grads(q, k, dq, dk, dv)
     delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     ws, ws_bytes = None, 0
     if rel_bias is not None:
@@ -724,6 +780,7 @@ def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None):
     _chk_bounds(seg_start, seg_end, B, Sq)
     if out is None:
         out = torch.empty((B, Sq, H, D), dtype=_bf16, device=q.device)
+    if tuple(out.shape) != (B, Sq, H, D): raise RuntimeError(f"fsb200: out shape {tuple(out.shape)} != {(B, Sq, H, D)}")
     _, _, _, _, o_rs, o_hs = _bshd(out, "out")
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     L.call("fsb_sdpa_fwd_segments", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs,
@@ -743,6 +800,7 @@ def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk
     _, _, _, _, dv_rs, dv_hs = _bshd(dv, "dv")
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
         _chk(t, _bf16, n)
+    _chk_grads(q, k, dq, dk, dv)
     _chk_bounds(seg_start, seg_end, B, Sq)
     delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     L.call("fsb_sdpa_bwd_segments", _p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv),

@@ -236,7 +236,8 @@ int fsb_cast_f32_to_bf16(const float* in, void* out, int64_t n, fsb_stream_t str
  * torch.nn.CrossEntropyLoss()(shift_logits, shift_labels), fengshen/models/llama/modeling_llama.py:334-339: mean NLL over
  * labels != ignore_index. Row t = (b, s) uses labels[t + shift] and is ignored when s + shift >= seq_len (the
  * shift-by-one without the `.contiguous()` copy of :336). logits bf16 [rows, vocab] (row stride ld); dlogits (may alias
- * logits, may be NULL) receives (softmax - onehot) * grad_scale / n_valid. row_loss fp32 [rows], loss fp32 [1],
+ * logits, may be NULL) receives (softmax - onehot) * grad_scale / n_valid as bf16 [rows, vocab] with the SAME row stride ld
+ * (an ignored row gets zeros): a separate dlogits must span (rows - 1) * ld + vocab elements. row_loss fp32 [rows], loss fp32 [1],
  * n_valid int32 [1] are device outputs (token-id side is bit-exact: n_valid and the one-hot index). */
 int fsb_softmax_xent_fwd_bwd(const void* logits, const int64_t* labels, void* dlogits, float* row_loss, float* loss,
                              int* n_valid, int64_t rows, int64_t vocab, int64_t ld, int64_t seq_len, int shift,
