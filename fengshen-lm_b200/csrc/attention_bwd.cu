@@ -100,7 +100,9 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 
 // ================================================================================================ dQ kernel
 // kDropout: dS = P * (dP * Z / (1 - p) - delta), Z regenerated from philox.cuh (delta = rowsum(dO * O) is unchanged).
-// kSeg: as in attn_fwd_kernel, the key steps start at seg_start[q0] / AB_BN and each row also masks below its kmin.
+// kSeg: as in attn_fwd_kernel, the key steps start at seg_start[q0] / AB_BN and each row also masks below its kmin. With
+// kDropout, a masked element has P = 0 and so dS = 0 whatever its keep bit, and a visible element's bit does not depend on
+// which steps the segment bounds skip (it is a function of its (q, k) only).
 template <int D, bool kBias, bool kDropout, bool kSeg = false>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -278,7 +280,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // kDropout: dV += (P * Z / (1 - p))^T dO and dS^T = P^T * (dP^T * Z / (1 - p) - delta); a register row is a key row here, so
 // the mask comes from attn_drop_cols (same Philox calls as the row-major kernels, words picked along the other axis).
 // kSeg: key k is seen by the queries k <= q < seg_end[k]. The tile's last key has the largest end, so the query steps stop at
-// ceil(seg_end[last key] / AB_BN) (clamped into the sequence); each key row masks above its qmax = seg_end[k] - 1.
+// ceil(seg_end[last key] / AB_BN) (clamped into the sequence); each key row masks above its qmax = seg_end[k] - 1. With
+// kDropout the segment mask zeroes P^T before the keep bits scale it, so both dV and dS^T are 0 past qmax whatever the bit.
 template <int D, bool kBias, bool kDropout, bool kSeg = false>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -591,6 +594,11 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.seg_start = seg_start; p.seg_end = seg_end;
+  if (seg_start != nullptr && drop != nullptr) {   // fsb_sdpa_bwd_segments_dropout with p > 0: head_dim 64 only
+    p.drop = *drop;
+    return launch_attn_bwd<64, false, true, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,
+                                                  do_row_stride, o_head_stride, delta, p, nullptr, nullptr, (cudaStream_t)st);
+  }
   if (seg_start != nullptr)   // fsb_sdpa_bwd_segments: causal, no bias, no dropout, no key mask
     return head_dim == 128
                ? launch_attn_bwd<128, false, false, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
@@ -669,6 +677,36 @@ extern "C" int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
                   dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, nullptr, seg_start,
                   seg_end, st);
+}
+
+extern "C" int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                             const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
+                                             int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                             int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
+                                             int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
+                                             int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride,
+                                             int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                             int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride,
+                                             int64_t dv_head_stride, float scale, const int32_t* seg_start,
+                                             const int32_t* seg_end, float p, uint64_t seed, const int64_t* stream_base,
+                                             int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_dropout: null segment bounds");
+  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_dropout: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
+              (long long)seq_kv);
+  FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd_segments_dropout: head_dim %d unsupported (64 or 128)",
+              head_dim);
+  if (p > 0.f) {
+    // GPT-2 (the one model with attention dropout that packs) runs head_dim 64; LLaMA has no attention dropout
+    FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_dropout: head_dim %d unsupported with p > 0 (64 only)", head_dim);
+    FSB_REQUIRE(seq_q <= 65536, "sdpa_bwd_segments_dropout: sequences longer than 65536 are not supported with p > 0");
+  }
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
+                  seg_start, seg_end, st);
 }
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {

@@ -49,6 +49,20 @@ def key_mask(attention_mask, dev):
     return attention_mask.to(device=dev, dtype=torch.uint8).contiguous()
 
 
+def packed_segments(segment_ids, lab, B, S, dev):
+    """The causal LMs' packed-row inputs: segment_ids, integer [B, S] (host or device; a segment is a maximal run of equal
+    consecutive values in a row), and the flat labels `lab` (int64 [B * S] or None). Returns ((seg_start, seg_end), labels):
+    the attention bounds of ops.segment_bounds, and the labels with each segment's first token ignored (its prediction would
+    cross a document boundary)."""
+    if tuple(segment_ids.shape) != (B, S):
+        raise ValueError(f"segment_ids must be [batch, seq] = [{B}, {S}], got {tuple(segment_ids.shape)}")
+    seg_start, seg_end = ops.segment_bounds(segment_ids.to(device=dev, non_blocking=True))
+    if lab is not None:   # a segment's first token is not a target of the previous segment's last
+        first = (seg_start == torch.arange(S, dtype=torch.int32, device=dev)).view(-1)
+        lab = lab.masked_fill(first, -100)
+    return (seg_start, seg_end), lab
+
+
 def learned_pos_emb_bwd(pos, dx, grad, B, S, accumulate):
     """Gradient of a learned absolute position table ([positions, h], `grad` = its main_grad) from the gradient dx [B * S, h]
     of the embedding sum. Without position ids row s is sum_b dx[b, s] (a column sum of dx viewed as [B, S * h]); with them,

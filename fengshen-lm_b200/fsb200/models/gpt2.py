@@ -11,6 +11,8 @@ Dropout (`embd_pdrop`, `attn_pdrop`, `resid_pdrop`, each in [0, 1) and independe
 attention kernels) and the attention / MLP `c_proj` outputs, dropped by the LayerNorm that adds them to the residual stream
 (`ln_2`, the next block's `ln_1`, `ln_f`). Seed, stream counter and eval mode as in fsb200/models/base.py; `generate` in
 training mode with a non-zero probability is rejected (HF would drop).
+Packed rows (several samples per row, fsb200/packing.py) pass `segment_ids`, as LlamaForCausalLM does: attention stays
+causal inside each segment, the attention-probability dropout included, and never crosses one.
 """
 import math
 from collections import namedtuple
@@ -23,10 +25,24 @@ from .. import lib as L
 from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
-from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd
+from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments
 from .layers import Linear, apply_dropout, residual_norm_bwd
 
 _Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
+
+
+def _refuse_key_padding(attention_mask):
+    """Packed rows carry no key mask: an attention_mask with zeros is refused, exactly on the host and with an asynchronous
+    device-side assert on the device (no synchronisation, so a CUDA-graph step stays capturable)."""
+    if attention_mask is None:
+        return
+    if attention_mask.is_cuda:
+        torch._assert_async((attention_mask != 0).all(),
+                            "fsb200 GPT2LMHeadModel: attention_mask has zeros together with segment_ids; packed rows "
+                            "need no key mask (the pad tail is a segment of its own)")
+    elif not bool((attention_mask != 0).all()):
+        raise ValueError("fsb200 GPT2LMHeadModel: attention_mask has zeros together with segment_ids; packed rows need no "
+                         "key mask (the pad tail is a segment of its own)")
 
 
 class GPT2LMHeadModel(FlatModel):
@@ -87,23 +103,38 @@ class GPT2LMHeadModel(FlatModel):
                 prm.normal_(0.0, s, generator=gen)
 
     # ---- forward ----------------------------------------------------------------------------------------------------
-    def forward(self, input_ids=None, attention_mask=None, labels=None, position_ids=None, return_logits=False, **_):
+    def forward(self, input_ids=None, attention_mask=None, labels=None, position_ids=None, return_logits=False,
+                segment_ids=None, **_):
+        """segment_ids: optional integer [B, S] (host or device) for packed rows; a segment is a maximal run of equal
+        consecutive values in a row. Every layer's attention is then causal inside each segment only, and the label of each
+        segment's first token is ignored. Pass per-segment position_ids (fsb200/packing.py emits them). No key mask is used:
+        the packer makes the pad tail a segment of its own, and an attention_mask with zeros is refused. None: one causal
+        sequence per row under attention_mask, as before."""
         B, S = input_ids.shape
         dev = self.flat.params.device
-        ids, lab, mask = flat_ids(input_ids, dev), flat_ids(labels, dev), key_mask(attention_mask, dev)
+        ids, lab = flat_ids(input_ids, dev), flat_ids(labels, dev)
         pos = None if position_ids is None else flat_ids(position_ids.expand(B, S), dev)
-        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, mask, lab, B, S)
+        if segment_ids is None:
+            seg, mask = (), key_mask(attention_mask, dev)
+        else:
+            _refuse_key_padding(attention_mask)
+            bounds, lab = packed_segments(segment_ids, lab, B, S, dev)
+            seg, mask = (bounds,), None
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, mask, lab, B, S, *seg)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
 
-    def _forward_impl(self, ids, pos, mask, lab, B, S, save, want_logits):
+    def _forward_impl(self, ids, pos, mask, lab, B, S, seg=None, *, save, want_logits):
+        """seg: None or the (seg_start, seg_end) bounds of packed rows (ops.segment_bounds); mask is then None."""
         scale = 1.0 / math.sqrt(self.hn)
         acts = [] if save else None
         base = self._dropout_base()
 
         def attend(i, q5):
-            return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask,
-                                drop=self._drop(base, self.p_attn, 1 + 3 * i))
+            drop = self._drop(base, self.p_attn, 1 + 3 * i)
+            if seg is not None:
+                return ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, *seg, drop=drop)
+            return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask, drop=drop)
         hf, stf, xf = self._stack(ids, pos, B, S, attend, acts, base)
         logits = self._head(hf)
         loss, ctx = None, None
@@ -112,7 +143,7 @@ class GPT2LMHeadModel(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base)
+                ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base, seg)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
@@ -219,7 +250,7 @@ class GPT2LMHeadModel(FlatModel):
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base = ctx
+        acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base, seg = ctx
         h, nh, hn = self.h, self.nh, self.hn
         T = B * S
         acc = self.accumulate_grads
@@ -245,8 +276,12 @@ class GPT2LMHeadModel(FlatModel):
             do = pj.attn_proj.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))
+            if seg is not None:
+                ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, *seg,
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(self.p_attn, 1 + 3 * i))
+            else:
+                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
+                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))
             dh1 = pj.c_attn.backward(dqkv, h1, acc)
             # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped MLP output into x
             dx, dm = residual_norm_bwd(dh1, x, blk.ln_1.weight, blk.ln_1.bias, st1, D(pr, 3 * i) if i > 0 else None, acc,

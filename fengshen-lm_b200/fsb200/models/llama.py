@@ -26,7 +26,7 @@ from .. import lib as L
 from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
-from .base import FlatModel, _Holder, flat_ids
+from .base import FlatModel, _Holder, flat_ids, packed_segments
 from .layers import Fp8Linear, GatedMLP, Linear
 
 
@@ -333,13 +333,8 @@ class LlamaForCausalLM(FlatModel):
             raise _quantized_unsupported(self.weight_format, "a training forward (labels under grad mode)")
         seg = ()
         if segment_ids is not None:
-            if tuple(segment_ids.shape) != (B, S):
-                raise ValueError(f"segment_ids must be [batch, seq] = [{B}, {S}], got {tuple(segment_ids.shape)}")
-            seg_start, seg_end = ops.segment_bounds(segment_ids.to(device=dev, non_blocking=True))
-            if lab is not None:   # a segment's first token is not a target of the previous segment's last
-                first = (seg_start == torch.arange(S, dtype=torch.int32, device=dev)).view(-1)
-                lab = lab.masked_fill(first, -100)
-            seg = ((seg_start, seg_end),)
+            bounds, lab = packed_segments(segment_ids, lab, B, S, dev)
+            seg = (bounds,)
         loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, lab, B, S, *seg)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)

@@ -6,8 +6,13 @@ collator's output and places the samples one after another into rows of exactly 
 order, with `segment_ids` that keep attention inside each sample (LlamaForCausalLM.forward(segment_ids=...)) and position ids
 that restart at 0 in each sample, so every sample sees the RoPE positions it had in the padded batch.
 
-`PackingCollator(inner, max_seq_length, pad_id)` wraps any collator that emits that format, so a script's own collator runs
-unchanged inside it. The number of rows varies from batch to batch; the samples handed to the collator do not change, so
+The Wenzhong-GPT2 QA recipe's batches have the same format: `GPT2QADataset.encode` pads every question + answer to
+`max_seq_length` with eos (its pad), labels -100 on every pad, and `default_collate` adds the `question` / `answer` strings,
+which the packer ignores. An eos inside the text is unlabelled there too, and stays an input. Packed, they feed
+GPT2LMHeadModel.forward(segment_ids=...), whose learned position embeddings then see each sample's own positions 0, 1, ...
+
+`PackingCollator(inner, max_seq_length, pad_id)` wraps any collator that emits that format (`default_collate` for the GPT-2
+dataset), so a script's own collator runs unchanged inside it. The number of rows varies from batch to batch; the samples handed to the collator do not change, so
 consumed-sample accounting is unaffected.
 """
 import torch

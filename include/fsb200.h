@@ -362,7 +362,8 @@ int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void
                          float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
 /* ---- packed sequences (document-masked causal attention) -------------------------------------------------------------
  * fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments: fsb_sdpa_fwd / fsb_sdpa_bwd with causal = 1 inside each segment of a row
- * and nothing across segments, for rows that pack several documents. No kv_mask, rel_bias or dropout; seq_q == seq_kv;
+ * and nothing across segments, for rows that pack several documents. No kv_mask or rel_bias (dropout: the
+ * fsb_sdpa_*_segments_dropout pair below); seq_q == seq_kv;
  * head_dim in {64, 128}. The bounds are two int32 [batch, seq] arrays, contiguous, indices relative to the row:
  *   seg_start[b][t] : the position of the first token of t's segment;
  *   seg_end[b][t]   : one past the position of its last token.
@@ -385,6 +386,28 @@ int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const voi
                           int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
                           int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
                           float scale, const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t stream);
+/* fsb_sdpa_fwd_segments_dropout / fsb_sdpa_bwd_segments_dropout: the segment entries with dropout on the attention
+ * probabilities (GPT-2 packed training), taking p, seed, stream_base and site as fsb_sdpa_*_dropout do. Visibility is the
+ * segment rule above; the keep mask Z is the attention layout of the dropout section, at the row-relative (q, k) of each
+ * element, so an element keeps the bit it has in an unsegmented causal launch and the skipped tiles draw nothing. O, the LSE
+ * (of the un-dropped P) and the gradients follow fsb_sdpa_*_dropout. p == 0 runs fsb_sdpa_*_segments and does not read the
+ * stream counter. Refused: null bounds, seq_q != seq_kv, head_dim other than 64 or 128, and with p > 0 head_dim != 64 or
+ * sequences longer than 65536. The backward must get the forward's bounds, seed, stream_base value and site. */
+int fsb_sdpa_fwd_segments_dropout(const void* q, const void* k, const void* v, void* o, float* lse,
+                                  int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                  int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                  float scale, const int32_t* seg_start, const int32_t* seg_end,
+                                  float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                  const float* lse, float* delta, void* dq, void* dk, void* dv,
+                                  int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                  int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                  int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                  int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                                  float scale, const int32_t* seg_start, const int32_t* seg_end,
+                                  float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
 
 int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
                               void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
