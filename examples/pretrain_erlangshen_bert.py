@@ -11,7 +11,11 @@ through its `datasets=` argument.
 
 `fsb200.launch` puts the compat packages on sys.path and binds `transformers.MegatronBertForPreTraining` to the fsb200-backed
 class. The recipe's DeepSpeed JSON (ZeRO stage, gradient_clipping) is read from $PL_DEEPSPEED_CONFIG_PATH as in the reference
-(pretrain_erlangshen_base.sh:24-39). Dropout must be 0 in config.json: fsb200 rejects dropout > 0 loudly."""
+(pretrain_erlangshen_base.sh:24-39). Dropout must be 0 in config.json: fsb200 rejects dropout > 0 loudly.
+
+--pack_sequences (off by default) wraps the collator, Python or --native_collator, in fsb200.packing.MLMPackingCollator: the
+documents of a batch are packed whole into rows of --max_seq_length instead of one padded document per row, and
+`forward(**batch)` hands the packed keys (segment_ids, position_ids, cls_positions) to the model."""
 import argparse
 import json
 import os
@@ -96,6 +100,8 @@ def parse_args(argv=None):
     parser = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     parser.add_argument('--native_collator', action='store_true', default=False,
                         help='assemble and mask the samples in libfsb200.so (fsb_bert_collate): same batches, ~1000x less host time')
+    parser.add_argument('--pack_sequences', action='store_true', default=False,
+                        help='pack the documents of each batch whole into rows of max_seq_length (fsb200.packing)')
     for add in (add_module_args, UniversalDataModule.add_data_specific_args, Trainer.add_argparse_args,
                 ErLangShenBert.add_module_specific_args, UniversalCheckpoint.add_argparse_args):
         parser = add(parser)
@@ -111,6 +117,9 @@ def build_data(args, tokenizer):
     collator = collator_cls(tokenizer=tokenizer, max_seq_length=args.max_seq_length, masked_lm_prob=args.masked_lm_prob,
                             content_key=args.sample_content_key)
     collator.setup()
+    if args.pack_sequences:
+        from fsb200.packing import MLMPackingCollator
+        collator = MLMPackingCollator(collator, args.max_seq_length, tokenizer.pad_token_id)
     return UniversalDataModule(tokenizer=tokenizer, args=args, collate_fn=collator,
                                datasets={args.train_datasets_field: JsonLines(args.train_file)})
 

@@ -103,7 +103,9 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 // kSeg: as in attn_fwd_kernel, the key steps start at seg_start[q0] / AB_BN and each row also masks below its kmin. With
 // kDropout, a masked element has P = 0 and so dS = 0 whatever its keep bit, and a visible element's bit does not depend on
 // which steps the segment bounds skip (it is a function of its (q, k) only).
-template <int D, bool kBias, bool kDropout, bool kSeg = false>
+// kSeg == kSegBidir: the key steps also stop at ceil(seg_end[last row] / AB_BN), clamped to hold the tile's diagonal step,
+// and each row masks above its kmax = seg_end[q] - 1 as well.
+template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -119,10 +121,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int head = blockIdx.y, b = blockIdx.z;
   const int q0 = tile * AB_BM;
   const int n_all = (p.seq_kv + AB_BN - 1) / AB_BN;
-  const int n_steps = p.causal ? min(n_all, (min(q0 + AB_BM, p.seq_q) + AB_BN - 1) / AB_BN) : n_all;
+  int n_steps = p.causal ? min(n_all, (min(q0 + AB_BM, p.seq_q) + AB_BN - 1) / AB_BN) : n_all;
   const int* seg_row = kSeg ? p.seg_start + int64_t(b) * p.seq_q : nullptr;
   int j0 = 0;   // first key step, clamped into [0, q0]
   if constexpr (kSeg) j0 = min(max(__ldg(seg_row + q0), 0), q0) / AB_BN;
+  const int* end_row = kSeg == kSegBidir ? p.seg_end + int64_t(b) * p.seq_q : nullptr;
+  if constexpr (kSeg == kSegBidir) {   // last key step: clamped into [the diagonal step, the last step]
+    const int e = min(max(__ldg(end_row + min(q0 + AB_BM, p.seq_q) - 1), 0), p.seq_kv);
+    n_steps = min(n_all, max(q0 / AB_BN + 1, (e + AB_BN - 1) / AB_BN));
+  }
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
@@ -181,6 +188,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     delta[h] = ok ? p.delta[si] : 0.f;
     kmax[h] = p.causal ? min(q_row[h], p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
     if constexpr (kSeg) kmin[h] = ok ? __ldg(seg_row + q_row[h]) : 0;   // first one
+    if constexpr (kSeg == kSegBidir) kmax[h] = ok ? min(__ldg(end_row + q_row[h]) - 1, kmax[h]) : kmax[h];
     // relative-position bias (mT5): this row reads entries (k - q_row + seq_q - 1) of its head's vector
     brow[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row[h], p.seq_q - 1)) : nullptr;
   }
@@ -212,8 +220,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     wgmma_wait<0>();
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
-    const bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
-                           (kSeg && c0 < max(kmin[0], kmin[1]));
+    bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
+                     (kSeg && c0 < max(kmin[0], kmin[1]));
+    if constexpr (kSeg == kSegBidir) need_mask = need_mask || c0 + AB_BN - 1 > min(kmax[0], kmax[1]);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
 #pragma unroll
@@ -282,7 +291,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // kSeg: key k is seen by the queries k <= q < seg_end[k]. The tile's last key has the largest end, so the query steps stop at
 // ceil(seg_end[last key] / AB_BN) (clamped into the sequence); each key row masks above its qmax = seg_end[k] - 1. With
 // kDropout the segment mask zeroes P^T before the keep bits scale it, so both dV and dS^T are 0 past qmax whatever the bit.
-template <int D, bool kBias, bool kDropout, bool kSeg = false>
+// kSeg == kSegBidir: key k is seen by the queries seg_start[k] <= q < seg_end[k]. The tile's first key has the smallest start,
+// so the query steps run from seg_start[first key] / AB_BN to ceil(seg_end[last key] / AB_BN), clamped into the sequence and
+// to hold the tile's diagonal steps; a step masks when it crosses a row's qmin = seg_start[k] or its qmax.
+template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -298,10 +310,15 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int head = blockIdx.y, b = blockIdx.z;
   const int kv0 = tile * AB_BM;
   const int n_q = (p.seq_q + AB_BN - 1) / AB_BN;
-  const int i_start = p.causal ? min(n_q, kv0 / AB_BN) : 0;
+  int i_start = p.causal ? min(n_q, kv0 / AB_BN) : 0;
   const int* seg_row = kSeg ? p.seg_end + int64_t(b) * p.seq_kv : nullptr;
   int i_end = n_q;
   if constexpr (kSeg) i_end = min(n_q, (min(max(__ldg(seg_row + min(kv0 + AB_BM, p.seq_kv) - 1), 0), p.seq_q) + AB_BN - 1) / AB_BN);
+  const int* start_row = kSeg == kSegBidir ? p.seg_start + int64_t(b) * p.seq_kv : nullptr;
+  if constexpr (kSeg == kSegBidir) {   // first query step clamped into [0, kv0]; the last at least the diagonal step
+    i_start = min(max(__ldg(start_row + kv0), 0), kv0) / AB_BN;
+    i_end = min(n_q, max(i_end, kv0 / AB_BN + 1));
+  }
   const int n_steps = kSeg ? max(0, i_end - i_start) : n_q - i_start;
 
   if (threadIdx.x == 0) {
@@ -364,6 +381,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   // their rows' qmax from global memory: two more live registers would spill in the D = 128 kernel.
   int qlim = 0;
   if constexpr (kSeg) qlim = __ldg(seg_row + kv0) - 1;
+  // kSegBidir: likewise the tile's last key has the largest qmin; only the steps before it mask below, re-reading their rows'
+  // qmin (both bounds live in registers would cost a spill)
+  int qlo = 0;
+  if constexpr (kSeg == kSegBidir) qlo = __ldg(start_row + min(kv0 + AB_BM, p.seq_kv) - 1);
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
@@ -399,6 +420,14 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
       for (int h = 0; h < 2; ++h) qmax[h] = row_ok[h] ? __ldg(p.seg_end + int64_t(b) * p.seq_kv + kv_row[h]) - 1 : -1;
     }
+    const bool need_lo = kSeg == kSegBidir && qt0 < qlo;
+    int qmin[2] = {0, 0};
+    if constexpr (kSeg == kSegBidir) {
+      if (need_lo) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) qmin[h] = row_ok[h] ? __ldg(start_row + kv_row[h]) : 0;
+      }
+    }
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii) {
 #pragma unroll
@@ -413,7 +442,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
           float arg = s[4 * ii + e] * p.scale_log2 - lse_c;
           if constexpr (kBias) arg = fmaf(__ldg(bkey[h] - min(qi, p.seq_q - 1)), 1.4426950408889634f, arg);
           float x = ex2_approx(arg);
-          const bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]) && !(need_seg && qi > qmax[h]);
+          bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]) && !(need_seg && qi > qmax[h]);
+          if constexpr (kSeg == kSegBidir) keep = keep && !(need_lo && qi < qmin[h]);
           x = keep ? x : 0.f;
           if constexpr (kDropout) {
             const bool z = (zbits >> (4 * ii + e)) & 1u;
@@ -497,7 +527,7 @@ static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq
   return size_t(batch) * nheads * n_qt * n_all * AB_DSTRIDE;
 }
 
-template <int D, bool kBias, bool kDropout, bool kSeg = false>
+template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                            int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
                            float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
@@ -594,17 +624,28 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.seg_start = seg_start; p.seg_end = seg_end;
+  if (seg_start != nullptr && !causal) {   // fsb_sdpa_bwd_segments_bidirectional: head_dim 64, no bias, no key mask
+    if (drop != nullptr) {
+      p.drop = *drop;
+      return launch_attn_bwd<64, false, true, kSegBidir>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                         nullptr, (cudaStream_t)st);
+    }
+    return launch_attn_bwd<64, false, false, kSegBidir>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                        o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                        nullptr, (cudaStream_t)st);
+  }
   if (seg_start != nullptr && drop != nullptr) {   // fsb_sdpa_bwd_segments_dropout with p > 0: head_dim 64 only
     p.drop = *drop;
-    return launch_attn_bwd<64, false, true, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,
+    return launch_attn_bwd<64, false, true, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,
                                                   do_row_stride, o_head_stride, delta, p, nullptr, nullptr, (cudaStream_t)st);
   }
   if (seg_start != nullptr)   // fsb_sdpa_bwd_segments: causal, no bias, no dropout, no key mask
     return head_dim == 128
-               ? launch_attn_bwd<128, false, false, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+               ? launch_attn_bwd<128, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
                                                           o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
                                                           nullptr, (cudaStream_t)st)
-               : launch_attn_bwd<64, false, false, true>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+               : launch_attn_bwd<64, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
                                                          o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
                                                          nullptr, (cudaStream_t)st);
 #define FSB_BWD(DD, BB, DR)                                                                                              \
@@ -706,6 +747,34 @@ extern "C" int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const
                   k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
                   dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
+                  seg_start, seg_end, st);
+}
+
+extern "C" int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k, const void* v, const void* o,
+                                                   const void* dout, const float* lse, float* delta, void* dq, void* dk,
+                                                   void* dv, int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads,
+                                                   int head_dim, int64_t q_row_stride, int64_t k_row_stride,
+                                                   int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride,
+                                                   int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                                                   int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride,
+                                                   int64_t o_head_stride, int64_t do_head_stride, int64_t dq_head_stride,
+                                                   int64_t dk_head_stride, int64_t dv_head_stride, float scale,
+                                                   const int32_t* seg_start, const int32_t* seg_end, float p,
+                                                   uint64_t seed, const int64_t* stream_base, int64_t site,
+                                                   fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_bidirectional: null segment bounds");
+  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_bidirectional: needs seq_q == seq_kv (got %lld and %lld)",
+              (long long)seq_q, (long long)seq_kv);
+  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_bidirectional: head_dim %d unsupported (64 only)", head_dim);
+  if (p > 0.f)
+    FSB_REQUIRE(seq_q <= 65536,
+                "sdpa_bwd_segments_bidirectional: sequences longer than 65536 are not supported with p > 0");
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, 0, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
                   seg_start, seg_end, st);
 }
 

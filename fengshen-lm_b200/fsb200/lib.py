@@ -121,6 +121,11 @@ SIGNATURES = {
                                               c_void_p, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
     "fsb_sdpa_bwd_segments_dropout": (c_int, [c_void_p] * 10 + [c_i64, c_i64, c_i64, c_int, c_int] + [c_i64] * 16 +
                                       [c_f32, c_void_p, c_void_p, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_sdpa_fwd_segments_bidirectional": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64,
+                                                    c_int, c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                                    c_f32, c_void_p, c_void_p, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
+    "fsb_sdpa_bwd_segments_bidirectional": (c_int, [c_void_p] * 10 + [c_i64, c_i64, c_i64, c_int, c_int] + [c_i64] * 16 +
+                                            [c_f32, c_void_p, c_void_p, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
     "fsb_layernorm_fwd_dropout": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64,
                                           c_f32, c_f32, c_u64, c_void_p, c_i64, c_void_p]),
     "fsb_layernorm_bwd_dropout": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -185,7 +190,8 @@ _NO_KERNEL = {"fsb_set_reserved_sms", "fsb_comm_unique_id", "fsb_comm_init", "fs
               "fsb_index_build_blocks_mapping", "fsb_index_build_blending_indices", "fsb_bert_collate"}   # host-only calls / NCCL's kernels, not ours
 _KERNELS_PER_CALL = {"fsb_rmsnorm_bwd": 2, "fsb_layernorm_bwd": 2, "fsb_softmax_xent_fwd_bwd": 3, "fsb_sdpa_bwd": 3,
                      "fsb_layernorm_bwd_dropout": 2, "fsb_rmsnorm_bwd_dropout": 2, "fsb_sdpa_bwd_dropout": 3,
-                     "fsb_sdpa_bwd_segments": 3, "fsb_sdpa_bwd_segments_dropout": 3, "fsb_sumsq": 2, "fsb_colsum": 2, "fsb_act_bwd_bias": 2, "fsb_attn_decode": 2, "fsb_fp8_quantize": 2}
+                     "fsb_sdpa_bwd_segments": 3, "fsb_sdpa_bwd_segments_dropout": 3, "fsb_sdpa_bwd_segments_bidirectional": 3,
+                     "fsb_sumsq": 2, "fsb_colsum": 2, "fsb_act_bwd_bias": 2, "fsb_attn_decode": 2, "fsb_fp8_quantize": 2}
 
 
 call_profiler = None  # optional: object with .add(name, ev0, ev1, work); set by bench.py --breakdown (CUDA events per call)

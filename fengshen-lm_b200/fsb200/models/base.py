@@ -50,10 +50,10 @@ def key_mask(attention_mask, dev):
 
 
 def packed_segments(segment_ids, lab, B, S, dev):
-    """The causal LMs' packed-row inputs: segment_ids, integer [B, S] (host or device; a segment is a maximal run of equal
-    consecutive values in a row), and the flat labels `lab` (int64 [B * S] or None). Returns ((seg_start, seg_end), labels):
-    the attention bounds of ops.segment_bounds, and the labels with each segment's first token ignored (its prediction would
-    cross a document boundary)."""
+    """Packed-row inputs: segment_ids, integer [B, S] (host or device; a segment is a maximal run of equal consecutive values
+    in a row), and the flat labels `lab` of a causal LM (int64 [B * S] or None). Returns ((seg_start, seg_end), labels): the
+    attention bounds of ops.segment_bounds, and the labels with each segment's first token ignored (its prediction would
+    cross a document boundary). Models whose targets are not shifted (the MLM encoders) pass lab=None."""
     if tuple(segment_ids.shape) != (B, S):
         raise ValueError(f"segment_ids must be [batch, seq] = [{B}, {S}], got {tuple(segment_ids.shape)}")
     seg_start, seg_end = ops.segment_bounds(segment_ids.to(device=dev, non_blocking=True))
@@ -61,6 +61,21 @@ def packed_segments(segment_ids, lab, B, S, dev):
         first = (seg_start == torch.arange(S, dtype=torch.int32, device=dev)).view(-1)
         lab = lab.masked_fill(first, -100)
     return (seg_start, seg_end), lab
+
+
+def refuse_key_padding(attention_mask, model):
+    """Packed rows carry no key mask: an attention_mask with zeros together with segment_ids is refused, exactly on the host
+    and with an asynchronous device-side assert on the device (no synchronisation, so a CUDA-graph step stays capturable).
+    `model` names the class in the message."""
+    if attention_mask is None:
+        return
+    if attention_mask.is_cuda:
+        torch._assert_async((attention_mask != 0).all(),
+                            f"fsb200 {model}: attention_mask has zeros together with segment_ids; packed rows "
+                            "need no key mask (the pad tail is a segment of its own)")
+    elif not bool((attention_mask != 0).all()):
+        raise ValueError(f"fsb200 {model}: attention_mask has zeros together with segment_ids; packed rows need no "
+                         "key mask (the pad tail is a segment of its own)")
 
 
 def learned_pos_emb_bwd(pos, dx, grad, B, S, accumulate):

@@ -13,6 +13,9 @@ Dropout (hidden_dropout_prob, attention_probs_dropout_prob; the two may differ) 
 also under no_grad), at HF's sites: the embeddings (BERT: after the LN; MegatronBERT: the sum, no LN), the attention
 probabilities, and the attention-output and FFN-output branches before their residual add — fused into the attention kernels
 and the LayerNorms that add the branch to the residual. Seed, stream counter and eval mode as in fsb200/models/base.py.
+Packed rows (several samples per row, fsb200/packing.py pack_mlm_batch) pass `segment_ids`: attention is then bidirectional
+inside each segment, the attention-probability dropout included, and never crosses one; MegatronBERT's sentence-order head
+reads each sample's [CLS] row from `cls_positions`.
 """
 import math
 from collections import namedtuple
@@ -23,7 +26,7 @@ import torch
 from .. import lib as L
 from .. import ops
 from ..flat import FlatSpec
-from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd
+from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments, refuse_key_padding
 from .layers import Linear, apply_dropout, residual_norm_bwd
 
 _Layer = namedtuple("_Layer", "qkv attn_out inter out")   # attention.self q|k|v, attention.output.dense, intermediate, output
@@ -117,21 +120,47 @@ class _BertFamily(FlatModel):
 
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, token_type_ids=None, position_ids=None, labels=None,
-                next_sentence_label=None, return_logits=False, **_):
+                next_sentence_label=None, return_logits=False, segment_ids=None, cls_positions=None, **_):
+        """segment_ids: optional integer [B, S] (host or device) for packed rows; a segment is a maximal run of equal
+        consecutive values in a row. Every layer's attention is then bidirectional inside each segment only (head_dim 64).
+        Pass per-sample position_ids (fsb200/packing.py emits them). No key mask is used: the packer makes the pad tail a
+        segment of its own, and an attention_mask with zeros is refused. cls_positions: int64 [n], the flat index
+        row * S + start of each sample's [CLS], in the order of next_sentence_label [n]; MegatronBERT's pooler reads those
+        rows (required with segment_ids and next_sentence_label; without either, no sentence-order logits are computed).
+        segment_ids=None: one sequence per row under attention_mask, as before."""
         B, S = input_ids.shape
         dev = self.flat.params.device
         c = lambda t: flat_ids(t, dev)
         ids, tt, pos, lab = c(input_ids), c(token_type_ids), c(position_ids), c(labels)
         nsl = c(next_sentence_label)
-        mask = key_mask(attention_mask, dev)
-        loss, logits, nsp = self._step_or_forward(lab is not None, return_logits, ids, tt, pos, mask, lab, nsl, B, S)
+        if segment_ids is None:
+            mask, packed = key_mask(attention_mask, dev), ()
+        else:
+            name = type(self).__name__
+            if self.hn != 64:
+                raise ValueError(f"fsb200 {name}: segment_ids need head_dim 64 (the bidirectional segment attention "
+                                 f"kernels), this config has head_dim {self.hn}")
+            if self.PRE_LN and nsl is not None and cls_positions is None:
+                raise ValueError(f"fsb200 {name}: segment_ids with next_sentence_label need cls_positions (the flat "
+                                 "index of each sample's [CLS]); token 0 of a packed row is one sample's only")
+            cls = c(cls_positions)
+            if cls is not None and nsl is not None and cls.numel() != nsl.numel():
+                raise ValueError(f"fsb200 {name}: cls_positions has {cls.numel()} entries, next_sentence_label "
+                                 f"{nsl.numel()}")
+            refuse_key_padding(attention_mask, name)
+            bounds, _ = packed_segments(segment_ids, None, B, S, dev)   # MLM targets are not shifted: no label is dropped
+            mask, packed = None, (bounds, cls)
+        loss, logits, nsp = self._step_or_forward(lab is not None, return_logits, ids, tt, pos, mask, lab, nsl, B, S,
+                                                  *packed)
         out = SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                               hidden_states=None, attentions=None)
         out.prediction_logits = out.logits
         out.seq_relationship_logits = None if nsp is None else nsp[:, :2]
         return out
 
-    def _forward_impl(self, ids, tt, pos, mask, lab, nsl, B, S, save, want_logits):
+    def _forward_impl(self, ids, tt, pos, mask, lab, nsl, B, S, seg=None, cls=None, *, save, want_logits):
+        """seg: None or the (seg_start, seg_end) bounds of packed rows (ops.segment_bounds); mask is then None and cls the
+        flat [CLS] rows of the samples (int64 [n]) or None (no sentence-order head)."""
         h, nh, hn, pre = self.h, self.nh, self.hn, self.PRE_LN
         T = B * S
         P = self.P
@@ -164,7 +193,12 @@ class _BertFamily(FlatModel):
                 attn_in = x
             qkv = pj.qkv(attn_in)
             q5 = qkv.view(B, S, 3, nh, hn)
-            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, False, kv_mask=mask, drop=D(pa, 1 + 3 * i))
+            if seg is not None:
+                o, lse = ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, *seg, drop=D(pa, 1 + 3 * i),
+                                               causal=False)
+            else:
+                o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, False, kv_mask=mask,
+                                      drop=D(pa, 1 + 3 * i))
             a = pj.attn_out(o.view(T, h))
             if pre:
                 h2, st2, x1 = ops.layernorm_fwd(a, P(p + "ln.weight").data, P(p + "ln.bias").data, self.eps, residual=x,
@@ -201,8 +235,9 @@ class _BertFamily(FlatModel):
         logits = self._decoder(tn)
         loss, ctx, nsp_logits = None, None, None
         nsp_ctx = None
-        if pre:
-            first = hf.view(B, S, h)[:, 0, :]                     # strided [B, h] view, row stride S*h
+        if pre and (seg is None or cls is not None):
+            # strided [B, h] view (row stride S*h), or the packed samples' [CLS] rows gathered into [n, h]
+            first = hf.view(B, S, h)[:, 0, :] if seg is None else hf.index_select(0, cls)
             ppre = self._pooler(first)
             pooled = ops.act_fwd(L.ACT_TANH, ppre)
             self._nsp_w[:2].copy_(P("cls.seq_relationship.weight").data)
@@ -214,20 +249,21 @@ class _BertFamily(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=0, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             dnsp = None
-            if pre and nsl is not None:
+            if nsp_logits is not None and nsl is not None:
                 keep_nsp = nsp_logits.clone()
                 nloss, dnsp, _ = ops.softmax_xent(nsp_logits, nsl, 1, shift=0, grad_scale=self.loss_scale,
                                                   dlogits="inplace" if save else None)
                 loss = loss + nloss                               # modeling_megatron_bert.py:776-779
                 nsp_logits = keep_nsp
             if save:
-                ctx = (acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base)
+                ctx = (acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base,
+                       seg, cls)
                 logits = keep
         return loss, (logits if want_logits else None), nsp_logits, ctx
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base = ctx
+        acts, emb_ctx, hf, stf, xf, tpre, tf, stt, tn, dlogits, nsp_ctx, dnsp, ids, tt, pos, mask, B, S, base, seg, cls = ctx
         ph, pa = self.p_hidden, self.p_attn
         D = lambda p, site: self._drop(base, p, site)
         h, nh, hn, pre = self.h, self.nh, self.hn, self.PRE_LN
@@ -259,7 +295,12 @@ class _BertFamily(FlatModel):
             else:
                 sw.main_grad.copy_(dw8[:2]); sb.main_grad.copy_(db8[:2])
             dppre = ops.act_bwd(L.ACT_TANH, dpooled, ppre)
-            self._pooler.backward(dppre, first, acc, dx=dhf.view(B, S, h)[:, 0, :], dx_accumulate=True)   # += into token 0 rows
+            if seg is None:
+                self._pooler.backward(dppre, first, acc, dx=dhf.view(B, S, h)[:, 0, :], dx_accumulate=True)   # += token 0 rows
+            else:   # the [CLS] rows are distinct: gather, accumulate as above (fp32 add, one rounding), scatter back
+                dcls = dhf.index_select(0, cls)
+                self._pooler.backward(dppre, first, acc, dx=dcls, dx_accumulate=True)
+                dhf.index_copy_(0, cls, dcls)
         elif pre:
             for n in ("cls.seq_relationship.weight", "cls.seq_relationship.bias", "bert.pooler.dense.weight",
                       "bert.pooler.dense.bias"):
@@ -295,8 +336,12 @@ class _BertFamily(FlatModel):
             do = pj.attn_out.backward(da, o.view(T, h), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, False,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
+            if seg is not None:
+                ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, *seg,
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(pa, 1 + 3 * i), causal=False)
+            else:
+                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, False,
+                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
             if pre:
                 dh1 = pj.qkv.backward(dqkv, h1, acc)
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")

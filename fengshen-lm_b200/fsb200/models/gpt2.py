@@ -25,24 +25,10 @@ from .. import lib as L
 from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
-from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments
+from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments, refuse_key_padding
 from .layers import Linear, apply_dropout, residual_norm_bwd
 
 _Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
-
-
-def _refuse_key_padding(attention_mask):
-    """Packed rows carry no key mask: an attention_mask with zeros is refused, exactly on the host and with an asynchronous
-    device-side assert on the device (no synchronisation, so a CUDA-graph step stays capturable)."""
-    if attention_mask is None:
-        return
-    if attention_mask.is_cuda:
-        torch._assert_async((attention_mask != 0).all(),
-                            "fsb200 GPT2LMHeadModel: attention_mask has zeros together with segment_ids; packed rows "
-                            "need no key mask (the pad tail is a segment of its own)")
-    elif not bool((attention_mask != 0).all()):
-        raise ValueError("fsb200 GPT2LMHeadModel: attention_mask has zeros together with segment_ids; packed rows need no "
-                         "key mask (the pad tail is a segment of its own)")
 
 
 class GPT2LMHeadModel(FlatModel):
@@ -117,7 +103,7 @@ class GPT2LMHeadModel(FlatModel):
         if segment_ids is None:
             seg, mask = (), key_mask(attention_mask, dev)
         else:
-            _refuse_key_padding(attention_mask)
+            refuse_key_padding(attention_mask, "GPT2LMHeadModel")
             bounds, lab = packed_segments(segment_ids, lab, B, S, dev)
             seg, mask = (bounds,), None
         loss, logits = self._step_or_forward(lab is not None, return_logits, ids, pos, mask, lab, B, S, *seg)

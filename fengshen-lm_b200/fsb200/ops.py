@@ -762,6 +762,9 @@ def segment_bounds(segment_ids):
     return start.to(torch.int32).contiguous(), end.to(torch.int32).contiguous()
 
 
+_NO_DROP = (0.0, 0, None, 0)   # p, seed, stream_base, site of an entry with a dropout signature, run without dropout
+
+
 def _chk_bounds(seg_start, seg_end, B, S):
     for t, n in ((seg_start, "seg_start"), (seg_end, "seg_end")):
         _chk(t, torch.int32, n)
@@ -769,11 +772,12 @@ def _chk_bounds(seg_start, seg_end, B, S):
             raise RuntimeError(f"fsb200: {n} must be contiguous int32 [batch, seq] = [{B}, {S}], got {tuple(t.shape)}")
 
 
-def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None):
+def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, causal=True):
     """sdpa_fwd over rows that pack several sequences: causal inside each segment, nothing across segments. q, k, v as in
     sdpa_fwd (seq_q == seq_kv); seg_start / seg_end from segment_bounds. Key / query tiles outside a tile's segments are
-    skipped. drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 when p > 0). Returns
-    (out [B, S, H, D], lse)."""
+    skipped. drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 when p > 0).
+    causal=False: bidirectional inside each segment (packed encoder rows: query q sees seg_start[q] <= k < seg_end[q]),
+    head_dim 64 only (fsb_sdpa_fwd_segments_bidirectional). Returns (out [B, S, H, D], lse)."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -786,15 +790,17 @@ def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None):
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     args = (_p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs, v_hs, o_hs,
             float(scale), _p(seg_start), _p(seg_end))
-    if drop is None:
+    if not causal:
+        L.call("fsb_sdpa_fwd_segments_bidirectional", *args, *(_NO_DROP if drop is None else drop.args()), _stream())
+    elif drop is None:
         L.call("fsb_sdpa_fwd_segments", *args, _stream())
     else:
         L.call("fsb_sdpa_fwd_segments_dropout", *args, *drop.args(), _stream())
     return out, lse
 
 
-def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv, drop=None):
-    """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end and drop); dq / dk / dv are written as in
+def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv, drop=None, causal=True):
+    """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end, drop and causal); dq / dk / dv are written as in
     sdpa_bwd."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -812,7 +818,9 @@ def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk
     args = (_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv, H, D, q_rs,
             k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs, float(scale),
             _p(seg_start), _p(seg_end))
-    if drop is None:
+    if not causal:
+        L.call("fsb_sdpa_bwd_segments_bidirectional", *args, *(_NO_DROP if drop is None else drop.args()), _stream())
+    elif drop is None:
         L.call("fsb_sdpa_bwd_segments", *args, _stream())
     else:
         L.call("fsb_sdpa_bwd_segments_dropout", *args, *drop.args(), _stream())

@@ -360,7 +360,7 @@ int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void
                          float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                          void* workspace, size_t workspace_bytes,
                          float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-/* ---- packed sequences (document-masked causal attention) -------------------------------------------------------------
+/* ---- packed sequences (document-masked causal and bidirectional attention) -------------------------------------------
  * fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments: fsb_sdpa_fwd / fsb_sdpa_bwd with causal = 1 inside each segment of a row
  * and nothing across segments, for rows that pack several documents. No kv_mask or rel_bias (dropout: the
  * fsb_sdpa_*_segments_dropout pair below); seq_q == seq_kv;
@@ -408,6 +408,36 @@ int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const void* v, c
                                   int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
                                   float scale, const int32_t* seg_start, const int32_t* seg_end,
                                   float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+/* fsb_sdpa_fwd_segments_bidirectional / fsb_sdpa_bwd_segments_bidirectional: bidirectional (encoder) attention inside each
+ * segment of a row and nothing across segments, for packed BERT / MegatronBERT rows, with optional dropout on the attention
+ * probabilities. Arguments as fsb_sdpa_*_segments_dropout; the same seg_start / seg_end bounds, and both are read by the
+ * forward as well as the backward. Key k is visible to query q iff seg_start[q] <= k < seg_end[q] (equivalently
+ * seg_start[k] <= q < seg_end[k]). With valid bounds (as above) the forward and dQ pass visit the key tiles from the one of
+ * seg_start[first query of the tile] to the one of seg_end[last query of the tile] - 1, and the dK / dV pass the query
+ * tiles from seg_start[first key of the tile] to seg_end[last key of the tile] - 1; a step masks only where it crosses a
+ * row's lower or upper bound. The ranges are clamped into the sequence and always hold the tile's diagonal tile, so invalid
+ * bounds give unspecified results but never an out-of-bounds access. Dropout as in fsb_sdpa_*_segments_dropout: the keep
+ * mask of an element is its bit at the row-relative (q, k) of an unsegmented non-causal launch, the LSE is that of the
+ * un-dropped P. p == 0 runs the dropout-free kernels and does not read the stream counter. No kv_mask or rel_bias.
+ * Refused: null bounds, seq_q != seq_kv, head_dim other than 64, and with p > 0 sequences longer than 65536. */
+int fsb_sdpa_fwd_segments_bidirectional(const void* q, const void* k, const void* v, void* o, float* lse,
+                                        int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                        int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
+                                        int64_t o_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                                        int64_t v_head_stride, int64_t o_head_stride, float scale,
+                                        const int32_t* seg_start, const int32_t* seg_end, float p, uint64_t seed,
+                                        const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                        const float* lse, float* delta, void* dq, void* dk, void* dv,
+                                        int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                        int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
+                                        int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
+                                        int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride,
+                                        int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                        int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride,
+                                        int64_t dv_head_stride, float scale, const int32_t* seg_start,
+                                        const int32_t* seg_end, float p, uint64_t seed, const int64_t* stream_base,
+                                        int64_t site, fsb_stream_t stream);
 
 int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
                               void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
