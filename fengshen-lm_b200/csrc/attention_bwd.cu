@@ -37,7 +37,25 @@ struct AttBwdParams {
   float scale, scale_log2;
   DropArgs drop;             // attention-probability dropout (kDropout only): the forward's seed, stream base and site
   const int *seg_start, *seg_end;   // [batch, seq] segment bounds of each token (kSeg only; see fsb_sdpa_bwd_segments)
+                                    // kSegCross: the dQ pass gets kv_start / kv_end, the dK / dV pass q_start / q_end
 };
+
+// The key steps [j0, j1) the dQ tile at q0 visits (attn_bwd_dq_kernel) and so the workspace slots of the bias gradient it
+// writes (attn_dbias_reduce_kernel reads the same ones). seg_row / end_row: the row's seg_start / seg_end (kSeg only).
+template <int kSeg>
+__device__ __forceinline__ int2 dq_step_range(const int* seg_row, const int* end_row, int q0, int seq_q, int seq_kv,
+                                              int causal) {
+  const int n_all = (seq_kv + AB_BN - 1) / AB_BN;
+  int n_steps = causal ? min(n_all, (min(q0 + AB_BM, seq_q) + AB_BN - 1) / AB_BN) : n_all;
+  int j0 = 0;   // first key step, clamped into [0, q0] (kSegCross: [0, seq_kv], there is no diagonal)
+  if constexpr (kSeg == kSegCross) j0 = min(max(__ldg(seg_row + q0), 0), seq_kv) / AB_BN;
+  else if constexpr (kSeg) j0 = min(max(__ldg(seg_row + q0), 0), q0) / AB_BN;
+  if constexpr (kSeg == kSegBidir || kSeg == kSegCross) {   // last key step: clamped into [the diagonal step, the last step]
+    const int e = min(max(__ldg(end_row + min(q0 + AB_BM, seq_q) - 1), 0), seq_kv);
+    n_steps = kSeg == kSegCross ? (e + AB_BN - 1) / AB_BN : min(n_all, max(q0 / AB_BN + 1, (e + AB_BN - 1) / AB_BN));
+  }
+  return make_int2(j0, n_steps);
+}
 
 // ------------------------------------------------------------------------------------------------ delta preprocess
 template <int D>
@@ -105,6 +123,9 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 // which steps the segment bounds skip (it is a function of its (q, k) only).
 // kSeg == kSegBidir: the key steps also stop at ceil(seg_end[last row] / AB_BN), clamped to hold the tile's diagonal step,
 // and each row masks above its kmax = seg_end[q] - 1 as well.
+// kSeg == kSegCross: as kSegBidir over kv_start / kv_end, with the steps clamped into the key sequence only; a tile whose
+// queries see no key visits no step and writes dQ = 0. kBias composes with kSegCausal and kSegBidir; the steps the bounds
+// skip write no bias-gradient slot, and the reduction reads only the slots of dq_step_range.
 template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -120,15 +141,15 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int tile = gridDim.x - 1 - blockIdx.x;
   const int head = blockIdx.y, b = blockIdx.z;
   const int q0 = tile * AB_BM;
+  constexpr bool kEnd = kSeg == kSegBidir || kSeg == kSegCross;   // rows bounded above by seg_end as well
   const int n_all = (p.seq_kv + AB_BN - 1) / AB_BN;
   int n_steps = p.causal ? min(n_all, (min(q0 + AB_BM, p.seq_q) + AB_BN - 1) / AB_BN) : n_all;
   const int* seg_row = kSeg ? p.seg_start + int64_t(b) * p.seq_q : nullptr;
   int j0 = 0;   // first key step, clamped into [0, q0]
-  if constexpr (kSeg) j0 = min(max(__ldg(seg_row + q0), 0), q0) / AB_BN;
-  const int* end_row = kSeg == kSegBidir ? p.seg_end + int64_t(b) * p.seq_q : nullptr;
-  if constexpr (kSeg == kSegBidir) {   // last key step: clamped into [the diagonal step, the last step]
-    const int e = min(max(__ldg(end_row + min(q0 + AB_BM, p.seq_q) - 1), 0), p.seq_kv);
-    n_steps = min(n_all, max(q0 / AB_BN + 1, (e + AB_BN - 1) / AB_BN));
+  const int* end_row = kEnd ? p.seg_end + int64_t(b) * p.seq_q : nullptr;
+  if constexpr (kSeg) {   // the same steps as dq_step_range (attn_dbias_reduce_kernel reads their slots)
+    const int2 range = dq_step_range<kSeg>(seg_row, end_row, q0, p.seq_q, p.seq_kv, p.causal);
+    j0 = range.x; n_steps = range.y;
   }
 
   if (threadIdx.x == 0) {
@@ -174,7 +195,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const uint64_t dsc_k = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), 0, 1024);              // K-major view (S)
   const uint64_t dsc_v = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML1), 0, 1024);
   const uint64_t dsc_kmn = make_smem_desc_sw128(smem_u32(smem + S::OFF_SML0), AB_BN * 128, 1024);  // MN-major view (dQ)
-  const uint8_t* mrow = p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
+  constexpr bool kNoKeyMask = kSeg == kSegCross || (kSeg != kSegNone && kBias);
+  const uint8_t* mrow = !kNoKeyMask && p.kv_mask ? p.kv_mask + int64_t(b) * p.seq_kv : nullptr;
   const int n_rel = p.seq_q + p.seq_kv - 1;
   int q_row[2], kmax[2], kmin[2] = {0, 0};
   float lse[2], delta[2];
@@ -188,7 +210,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     delta[h] = ok ? p.delta[si] : 0.f;
     kmax[h] = p.causal ? min(q_row[h], p.seq_kv - 1) : p.seq_kv - 1;   // last key column this row may attend to
     if constexpr (kSeg) kmin[h] = ok ? __ldg(seg_row + q_row[h]) : 0;   // first one
-    if constexpr (kSeg == kSegBidir) kmax[h] = ok ? min(__ldg(end_row + q_row[h]) - 1, kmax[h]) : kmax[h];
+    if constexpr (kEnd) kmax[h] = ok ? min(__ldg(end_row + q_row[h]) - 1, kmax[h]) : kmax[h];
     // relative-position bias (mT5): this row reads entries (k - q_row + seq_q - 1) of its head's vector
     brow[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (p.seq_q - 1 - min(q_row[h], p.seq_q - 1)) : nullptr;
   }
@@ -222,7 +244,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     wgmma_fence_acc(dp);
     bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
                      (kSeg && c0 < max(kmin[0], kmin[1]));
-    if constexpr (kSeg == kSegBidir) need_mask = need_mask || c0 + AB_BN - 1 > min(kmax[0], kmax[1]);
+    if constexpr (kEnd) need_mask = need_mask || c0 + AB_BN - 1 > min(kmax[0], kmax[1]);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
 #pragma unroll
@@ -294,6 +316,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 // kSeg == kSegBidir: key k is seen by the queries seg_start[k] <= q < seg_end[k]. The tile's first key has the smallest start,
 // so the query steps run from seg_start[first key] / AB_BN to ceil(seg_end[last key] / AB_BN), clamped into the sequence and
 // to hold the tile's diagonal steps; a step masks when it crosses a row's qmin = seg_start[k] or its qmax.
+// kSeg == kSegCross: as kSegBidir over q_start / q_end (the launch passes them as seg_start / seg_end), clamped into the
+// query sequence only; a tile whose keys no query sees visits no step and writes dK = dV = 0.
 template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -314,11 +338,13 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int* seg_row = kSeg ? p.seg_end + int64_t(b) * p.seq_kv : nullptr;
   int i_end = n_q;
   if constexpr (kSeg) i_end = min(n_q, (min(max(__ldg(seg_row + min(kv0 + AB_BM, p.seq_kv) - 1), 0), p.seq_q) + AB_BN - 1) / AB_BN);
-  const int* start_row = kSeg == kSegBidir ? p.seg_start + int64_t(b) * p.seq_kv : nullptr;
+  constexpr bool kLo = kSeg == kSegBidir || kSeg == kSegCross;   // key rows bounded below by seg_start as well
+  const int* start_row = kLo ? p.seg_start + int64_t(b) * p.seq_kv : nullptr;
   if constexpr (kSeg == kSegBidir) {   // first query step clamped into [0, kv0]; the last at least the diagonal step
     i_start = min(max(__ldg(start_row + kv0), 0), kv0) / AB_BN;
     i_end = min(n_q, max(i_end, kv0 / AB_BN + 1));
   }
+  if constexpr (kSeg == kSegCross) i_start = min(max(__ldg(start_row + kv0), 0), p.seq_q) / AB_BN;   // no diagonal
   const int n_steps = kSeg ? max(0, i_end - i_start) : n_q - i_start;
 
   if (threadIdx.x == 0) {
@@ -373,7 +399,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     kv_row[h] = kv0 + r_lo + 8 * h;
-    row_ok[h] = kv_row[h] < p.seq_kv && (p.kv_mask == nullptr || p.kv_mask[int64_t(b) * p.seq_kv + kv_row[h]] != 0);
+    row_ok[h] = kv_row[h] < p.seq_kv && (kSeg == kSegCross || (kSeg != kSegNone && kBias) || p.kv_mask == nullptr ||
+                                         p.kv_mask[int64_t(b) * p.seq_kv + kv_row[h]] != 0);
     // relative-position bias: key row kv_row, query column qi -> entry (kv_row - qi + seq_q - 1) of the head's vector
     bkey[h] = kBias ? p.rel_bias + int64_t(head) * n_rel + (min(kv_row[h], p.seq_kv - 1) + p.seq_q - 1) : nullptr;
   }
@@ -384,7 +411,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   // kSegBidir: likewise the tile's last key has the largest qmin; only the steps before it mask below, re-reading their rows'
   // qmin (both bounds live in registers would cost a spill)
   int qlo = 0;
-  if constexpr (kSeg == kSegBidir) qlo = __ldg(start_row + min(kv0 + AB_BM, p.seq_kv) - 1);
+  if constexpr (kLo) qlo = __ldg(start_row + min(kv0 + AB_BM, p.seq_kv) - 1);
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
@@ -420,9 +447,9 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
       for (int h = 0; h < 2; ++h) qmax[h] = row_ok[h] ? __ldg(p.seg_end + int64_t(b) * p.seq_kv + kv_row[h]) - 1 : -1;
     }
-    const bool need_lo = kSeg == kSegBidir && qt0 < qlo;
+    const bool need_lo = kLo && qt0 < qlo;
     int qmin[2] = {0, 0};
-    if constexpr (kSeg == kSegBidir) {
+    if constexpr (kLo) {
       if (need_lo) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) qmin[h] = row_ok[h] ? __ldg(start_row + kv_row[h]) : 0;
@@ -443,7 +470,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
           if constexpr (kBias) arg = fmaf(__ldg(bkey[h] - min(qi, p.seq_q - 1)), 1.4426950408889634f, arg);
           float x = ex2_approx(arg);
           bool keep = row_ok[h] && !(need_causal && qi < kv_row[h]) && !(need_seg && qi > qmax[h]);
-          if constexpr (kSeg == kSegBidir) keep = keep && !(need_lo && qi < qmin[h]);
+          if constexpr (kLo) keep = keep && !(need_lo && qi < qmin[h]);
           x = keep ? x : 0.f;
           if constexpr (kDropout) {
             const bool z = (zbits >> (4 * ii + e)) & 1u;
@@ -487,9 +514,13 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 // dBias[h, i] (+)= sum over (b, q tile, step) of the diagonal sums the dQ kernel left in the workspace, in a FIXED order
 // (deterministic). i = (k - q) + seq_q - 1. Stage 1: grid (i chunks, heads, batch splits) -> part2[split][h][i]; stage 2 adds
 // the splits onto the caller's fp32 vector.
+// kSeg (segment launches with a bias): a dQ tile writes only the slots of the steps it visits, so the sum for each
+// (b, q tile) runs over the steps of dq_step_range, read from the same bounds (seg_start / seg_end) with the same clamps.
+template <int kSeg = kSegNone>
 __global__ void __launch_bounds__(128) attn_dbias_reduce_kernel(const float* __restrict__ part, float* __restrict__ part2,
                                                                 int batch, int nheads, int seq_q, int seq_kv, int causal,
-                                                                int n_qtiles, int bsplit) {
+                                                                int n_qtiles, int bsplit, const int* seg_start = nullptr,
+                                                                const int* seg_end = nullptr) {
   const int n_rel = seq_q + seq_kv - 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int h = blockIdx.y, sp = blockIdx.z;
@@ -501,12 +532,19 @@ __global__ void __launch_bounds__(128) attn_dbias_reduce_kernel(const float* __r
   for (int b = b0; b < b1; ++b) {
     for (int tile = 0; tile < n_qtiles; ++tile) {
       const int q0 = tile * AB_BM;
-      const int n_steps = causal ? min(n_all, (min(q0 + AB_BM, seq_q) + AB_BN - 1) / AB_BN) : n_all;
+      int n_steps = causal ? min(n_all, (min(q0 + AB_BM, seq_q) + AB_BN - 1) / AB_BN) : n_all, j0 = 0;
+      if constexpr (kSeg != kSegNone) {
+        const int2 range = dq_step_range<kSeg>(seg_start + int64_t(b) * seq_q, seg_end + int64_t(b) * seq_q, q0, seq_q,
+                                               seq_kv, causal);
+        j0 = range.x; n_steps = range.y;
+      }
       const float* base = part + ((int64_t(b) * nheads + h) * n_qtiles + tile) * n_all * AB_DSTRIDE;
       // step j holds the diagonal k - q = d in slot t = d + q0 - 64 j + 127 when 0 <= t < 191
       const int hi = d + q0 + (AB_BM - 1), lo = d + q0 - (AB_BN - 1);
       if (hi < 0) continue;
-      const int j_lo = lo <= 0 ? 0 : (lo + AB_BN - 1) / AB_BN, j_hi = min(n_steps - 1, hi / AB_BN);
+      int j_lo = lo <= 0 ? 0 : (lo + AB_BN - 1) / AB_BN;
+      if constexpr (kSeg != kSegNone) j_lo = max(j_lo, j0);
+      const int j_hi = min(n_steps - 1, hi / AB_BN);
       for (int j = j_lo; j <= j_hi; ++j) acc += base[int64_t(j) * AB_DSTRIDE + (hi - j * AB_BN)];
     }
   }
@@ -530,7 +568,8 @@ static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq
 template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
                            int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
-                           float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st) {
+                           float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st,
+                           const int* q_start = nullptr, const int* q_end = nullptr) {
   using SQ = AttBwdSmem<D, kBias>;
   using SK = AttBwdSmem<D, false>;
   if (int rc = ensure_smem<attn_bwd_dq_kernel<D, kBias, kDropout, kSeg>>(SQ::TOTAL, "sdpa_bwd")) return rc;
@@ -561,16 +600,17 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
     dim3 grid((p.seq_q + AB_BM - 1) / AB_BM, p.nheads, p.batch);
     attn_bwd_dq_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
     FSB_CUDA_LAUNCH_CHECK();
-    if (kBias && drel_bias != nullptr) {
+    if (kBias && drel_bias != nullptr) {   // (only the bias kernels instantiate a reduction)
       const int n_rel = p.seq_q + p.seq_kv - 1, bs = dbias_bsplit(p.batch);
-      attn_dbias_reduce_kernel<<<dim3((n_rel + 127) / 128, p.nheads, bs), 128, 0, st>>>(
-          p.dbias_part, part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), bs);
+      attn_dbias_reduce_kernel<kBias ? kSeg : kSegNone><<<dim3((n_rel + 127) / 128, p.nheads, bs), 128, 0, st>>>(
+          p.dbias_part, part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), bs, p.seg_start, p.seg_end);
       FSB_CUDA_LAUNCH_CHECK();
       attn_dbias_final_kernel<<<dim3((n_rel + 127) / 128, p.nheads), 128, 0, st>>>(part2, drel_bias, p.nheads, n_rel, bs);
       FSB_CUDA_LAUNCH_CHECK();
     }
   }
   // 3. dK, dV
+  if constexpr (kSeg == kSegCross) { p.seg_start = q_start; p.seg_end = q_end; }   // the key-side ranges
   {
     dim3 grid((p.seq_kv + AB_BM - 1) / AB_BM, p.nheads, p.batch);
     attn_bwd_dkv_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
@@ -591,7 +631,7 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
                     int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
                     float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
                     void* workspace, size_t workspace_bytes, const DropArgs* drop, const int* seg_start,
-                    const int* seg_end, fsb_stream_t st) {
+                    const int* seg_end, fsb_stream_t st, const int* q_start = nullptr, const int* q_end = nullptr) {
   FSB_REQUIRE(q && k && v && o && dout && lse && delta && dq && dk && dv, "sdpa_bwd: null pointer");
   FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd: head_dim %d unsupported (64 or 128)", head_dim);
   FSB_REQUIRE(batch > 0 && seq_q > 0 && seq_kv > 0 && nheads > 0 && batch < 65536 && nheads < 65536, "sdpa_bwd: bad dims");
@@ -624,6 +664,28 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.seg_start = seg_start; p.seg_end = seg_end;
+  if (q_start != nullptr) {   // fsb_sdpa_bwd_segments_cross: head_dim 64, no bias, no key mask
+    if (drop != nullptr) {
+      p.drop = *drop;
+      return launch_attn_bwd<64, false, true, kSegCross>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                         nullptr, (cudaStream_t)st, q_start, q_end);
+    }
+    return launch_attn_bwd<64, false, false, kSegCross>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                        o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                        nullptr, (cudaStream_t)st, q_start, q_end);
+  }
+#define FSB_BWD_SEG(DR, SEG)                                                                                             \
+  launch_attn_bwd<64, true, DR, SEG>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,          \
+                                     do_row_stride, o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
+  if (seg_start != nullptr && rel_bias != nullptr) {   // fsb_sdpa_bwd_segments_bias: head_dim 64, no key mask
+    if (drop != nullptr) {
+      p.drop = *drop;
+      return causal ? FSB_BWD_SEG(true, kSegCausal) : FSB_BWD_SEG(true, kSegBidir);
+    }
+    return causal ? FSB_BWD_SEG(false, kSegCausal) : FSB_BWD_SEG(false, kSegBidir);
+  }
+#undef FSB_BWD_SEG
   if (seg_start != nullptr && !causal) {   // fsb_sdpa_bwd_segments_bidirectional: head_dim 64, no bias, no key mask
     if (drop != nullptr) {
       p.drop = *drop;
@@ -776,6 +838,60 @@ extern "C" int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k,
                   q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
                   dk_head_stride, dv_head_stride, scale, 0, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
                   seg_start, seg_end, st);
+}
+
+extern "C" int fsb_sdpa_bwd_segments_bias(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                          const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
+                                          int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
+                                          int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                          int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
+                                          int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                                          int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                                          int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                                          float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
+                                          const float* rel_bias, float* drel_bias, void* workspace,
+                                          size_t workspace_bytes, float p, uint64_t seed, const int64_t* stream_base,
+                                          int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_bias: null segment bounds");
+  FSB_REQUIRE(rel_bias, "sdpa_bwd_segments_bias: null rel_bias");
+  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_bias: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
+              (long long)seq_kv);
+  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_bias: head_dim %d unsupported (64 only)", head_dim);
+  if (p > 0.f)
+    FSB_REQUIRE(seq_q <= 65536, "sdpa_bwd_segments_bias: sequences longer than 65536 are not supported with p > 0");
+  // drel_bias without a large enough workspace is refused by sdpa_bwd
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, causal ? 1 : 0, nullptr, rel_bias, drel_bias, workspace,
+                  workspace_bytes, p > 0.f ? &d : nullptr, seg_start, seg_end, st);
+}
+
+extern "C" int fsb_sdpa_bwd_segments_cross(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                           const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
+                                           int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
+                                           int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                           int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
+                                           int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                                           int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                                           int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                                           float scale, const int32_t* kv_start, const int32_t* kv_end,
+                                           const int32_t* q_start, const int32_t* q_end, float p, uint64_t seed,
+                                           const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
+  FSB_REQUIRE(kv_start && kv_end && q_start && q_end, "sdpa_bwd_segments_cross: null segment bounds");
+  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_cross: head_dim %d unsupported (64 only)", head_dim);
+  if (p > 0.f)
+    FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536,
+                "sdpa_bwd_segments_cross: sequences longer than 65536 are not supported with p > 0");
+  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
+                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
+                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
+                  dk_head_stride, dv_head_stride, scale, 0, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
+                  kv_start, kv_end, st, q_start, q_end);
 }
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {

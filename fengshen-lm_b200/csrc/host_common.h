@@ -54,8 +54,9 @@ int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* d
 int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
                    int box_rows);
 // Segment mode (kSeg) of the attention forward / backward kernels for packed rows (fsb_sdpa_*_segments*): none, causal
-// inside each segment, or bidirectional inside each segment
-enum AttnSegMode : int { kSegNone = 0, kSegCausal = 1, kSegBidir = 2 };
+// inside each segment, bidirectional inside each segment, or cross-attention from each query's segment to its key range in
+// another sequence
+enum AttnSegMode : int { kSegNone = 0, kSegCausal = 1, kSegBidir = 2, kSegCross = 3 };
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

@@ -63,6 +63,33 @@ def packed_segments(segment_ids, lab, B, S, dev):
     return (seg_start, seg_end), lab
 
 
+def cross_segment_bounds(dec_ids, enc_ids):
+    """Cross-attention bounds of packed encoder-decoder rows (ops.sdpa_segments_fwd kv_bounds form): decoder segment x of
+    row b attends to the encoder segment of row b with the same id value. dec_ids: integer [B, Sd], enc_ids: integer
+    [B, Se], on one device, each non-decreasing along the row (so a segment is the run of one id). Returns
+    ((kv_start, kv_end), (q_start, q_end)), contiguous int32 [B, Sd] and [B, Se]: the encoder positions each decoder token
+    sees and the decoder positions that see each encoder token. An id with no match on the other side gets an empty range.
+    Torch ops only, no host synchronisation (capturable in a CUDA graph): decreasing ids are refused exactly for host
+    tensors and with an asynchronous device-side assert for device tensors."""
+    for t, n in ((dec_ids, "decoder segment ids"), (enc_ids, "encoder segment ids")):
+        if t.dim() != 2 or t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise ValueError(f"{n} must be an integer [batch, seq] tensor, got {t.dtype} {tuple(t.shape)}")
+    if dec_ids.shape[0] != enc_ids.shape[0] or dec_ids.device != enc_ids.device:
+        raise ValueError(f"decoder and encoder segment ids must share batch and device, got {tuple(dec_ids.shape)} on "
+                         f"{dec_ids.device} and {tuple(enc_ids.shape)} on {enc_ids.device}")
+    dec, enc = dec_ids.to(torch.int64).contiguous(), enc_ids.to(torch.int64).contiguous()
+    ordered = (dec[:, 1:] >= dec[:, :-1]).all() & (enc[:, 1:] >= enc[:, :-1]).all()
+    msg = "segment ids must be non-decreasing along each row (samples placed in order)"
+    if dec.is_cuda:
+        torch._assert_async(ordered, msg)
+    elif not bool(ordered):
+        raise ValueError(msg)
+    i32 = lambda t: t.to(torch.int32).contiguous()
+    kv = (i32(torch.searchsorted(enc, dec, right=False)), i32(torch.searchsorted(enc, dec, right=True)))
+    q = (i32(torch.searchsorted(dec, enc, right=False)), i32(torch.searchsorted(dec, enc, right=True)))
+    return kv, q
+
+
 def refuse_key_padding(attention_mask, model):
     """Packed rows carry no key mask: an attention_mask with zeros together with segment_ids is refused, exactly on the host
     and with an asynchronous device-side assert on the device (no synchronisation, so a CUDA-graph step stays capturable).

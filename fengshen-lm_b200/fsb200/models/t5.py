@@ -25,6 +25,10 @@ fsb200/models/base.py. A branch is dropped by the RMSNorm that adds it to the re
 kernel, the attention probabilities inside the attention kernels (the decoder's self-attention with the causal flag, at every
 rate), the embeddings and final-norm outputs by the standalone dropout kernel. `generate` in training mode with a non-zero rate
 is rejected (HF would drop).
+Packed rows (several samples per row, fsb200/packing.py pack_seq2seq_batch) pass `segment_ids` and `decoder_segment_ids`:
+the encoder's self-attention is then bidirectional inside each encoder segment, the decoder's causal inside each decoder
+segment, both with the relative-position bias (it depends on k - q only, so a segment sees the scores it would see alone),
+and each decoder segment's cross-attention reads only the encoder segment with the same id. The dropout sites are unchanged.
 """
 import math
 from collections import namedtuple
@@ -38,11 +42,25 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from . import t5_bias as TB
-from .base import FlatModel, _Holder, flat_ids, key_mask
+from .base import FlatModel, _Holder, cross_segment_bounds, flat_ids, key_mask, refuse_key_padding
 from .layers import GatedMLP, Linear, apply_dropout, residual_norm_bwd
 
 _Enc = namedtuple("_Enc", "qkv o mlp")             # a layer's projections: self-attention q|k|v and o, the gated FFN
 _Dec = namedtuple("_Dec", "qkv o cq ckv co mlp")   # ... and between them cross-attention q, k|v and o
+
+
+def shift_right(labels, start_id, pad_id, seg_start=None):
+    """MT5 _shift_right (:592): decoder_input_ids = [start] + labels[:-1], with -100 replaced by the pad id. seg_start
+    (int32 [B, S], packed rows, ops.segment_bounds of the decoder segment ids): every decoder segment starts from the start
+    id instead, so no sample sees the previous one's last label. Torch ops only (any device)."""
+    dec = labels.new_zeros(labels.shape)
+    dec[:, 1:] = labels[:, :-1]
+    dec[:, 0] = start_id
+    dec = dec.masked_fill(dec == -100, pad_id)
+    if seg_start is not None:
+        pos = torch.arange(labels.shape[1], dtype=seg_start.dtype, device=seg_start.device)
+        dec = dec.masked_fill(seg_start == pos, start_id)
+    return dec
 
 
 class MT5ForConditionalGeneration(FlatModel):
@@ -156,24 +174,53 @@ class MT5ForConditionalGeneration(FlatModel):
     # ---- forward ----------------------------------------------------------------------------------------------------
     def _shift_right(self, labels):
         """MT5 _shift_right (:592): decoder_input_ids = [start] + labels[:-1], with -100 replaced by the pad id."""
-        dec = labels.new_zeros(labels.shape)
-        dec[:, 1:] = labels[:, :-1]
-        dec[:, 0] = self.start_id
-        return dec.masked_fill(dec == -100, self.pad_id)
+        return shift_right(labels, self.start_id, self.pad_id)
 
-    def forward(self, input_ids=None, attention_mask=None, labels=None, decoder_input_ids=None, return_logits=False, **_):
+    def forward(self, input_ids=None, attention_mask=None, labels=None, decoder_input_ids=None, return_logits=False,
+                segment_ids=None, decoder_segment_ids=None, **_):
+        """segment_ids [B, Se] / decoder_segment_ids [B, Sd]: optional integer ids of packed rows (host or device; both or
+        neither), non-decreasing along each row; encoder and decoder segments with the same id value are one sample
+        (fsb200/packing.py numbers them 0..m-1 and gives each side's pad tail id m). head_dim (d_kv) 64 only. No key mask is
+        used: an attention_mask with zeros is refused. decoder_input_ids derived from labels restart at every decoder
+        segment with the start id, so no sample sees the previous one's last label; the loss covers every labelled decoder
+        position, as without packing. segment_ids=None: one sample per row under attention_mask, as before."""
         dev = self.flat.params.device
         B, Se = input_ids.shape
+        if (segment_ids is None) != (decoder_segment_ids is None):
+            raise ValueError("fsb200 MT5: pass segment_ids and decoder_segment_ids together (packed rows need both)")
+        packed = ()
+        if segment_ids is not None:
+            if self.dk != 64:
+                raise ValueError(f"fsb200 MT5: segment_ids need d_kv 64 (the packed attention kernels), this config has "
+                                 f"d_kv {self.dk}")
+            refuse_key_padding(attention_mask, "MT5")
+            packed = (self._packed_bounds(segment_ids, decoder_segment_ids, B, Se, dev),)
         if decoder_input_ids is None:
             if labels is None:
                 raise ValueError("fsb200 MT5: pass labels or decoder_input_ids")
-            decoder_input_ids = self._shift_right(labels.to(device=dev, dtype=torch.int64))
+            # packed: each decoder segment starts from the start id, as its sample would alone
+            decoder_input_ids = shift_right(labels.to(device=dev, dtype=torch.int64), self.start_id, self.pad_id,
+                                            packed[0][1][0] if packed else None)
         Sd = decoder_input_ids.shape[1]
         ids, dec_ids, lab = flat_ids(input_ids, dev), flat_ids(decoder_input_ids, dev), flat_ids(labels, dev)
-        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, dec_ids, key_mask(attention_mask, dev), lab,
-                                             B, Se, Sd)
+        mask = None if packed else key_mask(attention_mask, dev)
+        loss, logits = self._step_or_forward(lab is not None, return_logits, ids, dec_ids, mask, lab, B, Se, Sd, *packed)
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, Sd, self.V),
                                past_key_values=None, encoder_last_hidden_state=None)
+
+    @staticmethod
+    def _packed_bounds(segment_ids, decoder_segment_ids, B, Se, dev):
+        """-> (encoder (seg_start, seg_end), decoder (seg_start, seg_end), cross ((kv_start, kv_end), (q_start, q_end)))."""
+        enc, dec = segment_ids, decoder_segment_ids
+        if tuple(enc.shape) != (B, Se) or dec.dim() != 2 or dec.shape[0] != B:
+            raise ValueError(f"fsb200 MT5: segment_ids must be [batch, source length] = [{B}, {Se}] and decoder_segment_ids "
+                             f"[{B}, target length], got {tuple(enc.shape)} and {tuple(dec.shape)}")
+        if enc.device != dec.device:
+            enc, dec = enc.to(device=dev, non_blocking=True), dec.to(device=dev, non_blocking=True)
+        # on the ids' own device: host ids are checked exactly, device ids without a synchronisation
+        cross = tuple(tuple(t.to(device=dev, non_blocking=True) for t in side) for side in cross_segment_bounds(dec, enc))
+        to_dev = lambda t: t.to(device=dev, non_blocking=True)
+        return ops.segment_bounds(to_dev(enc)), ops.segment_bounds(to_dev(dec)), cross
 
     def _norm(self, prev, x, name, drop=None):
         """pre-norm with the pending residual add (of the branch `prev`, dropped by `drop`) fused in: returns (normed, rstd,
@@ -182,9 +229,10 @@ class MT5ForConditionalGeneration(FlatModel):
             return ops.rmsnorm_fwd(x, self.P(name).data, self.eps)
         return ops.rmsnorm_fwd(prev, self.P(name).data, self.eps, residual=x, drop=drop)
 
-    def _encode(self, ids, mask, B, Se, rel_e, save, base=None):
+    def _encode(self, ids, mask, B, Se, rel_e, save, base=None, seg=None):
         """Encoder stack over ids [B * Se]; returns (saved activations, final hidden states (after their dropout), their rstd,
-        residual stream). base: the forward's dropout stream base (None: no dropout)."""
+        residual stream). base: the forward's dropout stream base (None: no dropout). seg: the (seg_start, seg_end) bounds of
+        packed rows (mask is then None)."""
         nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         Te = B * Se
@@ -197,8 +245,12 @@ class MT5ForConditionalGeneration(FlatModel):
             h1, r1, x = self._norm(prev, x, p + "0.layer_norm.weight", D(4 * i))   # layer i-1's FFN output
             qkv = pj.qkv(h1)
             q5 = qkv.view(B, Se, 3, nh, dk)
-            o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, False, kv_mask=mask, rel_bias=rel_e,
-                                  drop=D(1 + 4 * i))
+            if seg is None:
+                o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, False, kv_mask=mask, rel_bias=rel_e,
+                                      drop=D(1 + 4 * i))
+            else:
+                o, lse = ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, *seg, drop=D(1 + 4 * i),
+                                               causal=False, rel_bias=rel_e)
             a = pj.o(o.view(Te, inner))
             h2, r2, x1 = self._norm(a, x, p + "1.layer_norm.weight", D(2 + 4 * i))
             m, ms = pj.mlp(h2, drop=D(3 + 4 * i))
@@ -304,7 +356,8 @@ class MT5ForConditionalGeneration(FlatModel):
         graphs.tok.copy_(start.view(-1))      # the first step decodes the start token
         return generation.run(graphs, start, c)
 
-    def _forward_impl(self, ids, dec_ids, mask, lab, B, Se, Sd, save, want_logits):
+    def _forward_impl(self, ids, dec_ids, mask, lab, B, Se, Sd, segs=None, *, save, want_logits):
+        """segs: None or the bounds of packed rows (_packed_bounds); mask is then None."""
         nh, dk = self.nh, self.dk
         P = self.P
         self._need("no_decay"); self._need("shared")
@@ -316,16 +369,24 @@ class MT5ForConditionalGeneration(FlatModel):
         base = self._dropout_base()
         E = self.dec_site0
         D = lambda site: self._drop(base, self.p_drop, site)
-        eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save, base)
+        enc_seg, dec_seg, cross = (None, None, None) if segs is None else segs
+        eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save, base, enc_seg)
 
         def attend(i, q5):
+            if dec_seg is not None:
+                return ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, *dec_seg, drop=D(E + 1 + 6 * i),
+                                             rel_bias=rel_d)
             return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True, rel_bias=rel_d, drop=D(E + 1 + 6 * i))
 
         def cross_attend(i, qc):
             kvc = self._dec[i].ckv(enc_h)
             kv5 = kvc.view(B, Se, 2, nh, dk)
-            oc, lsec = ops.sdpa_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, False, kv_mask=mask,
-                                    drop=D(E + 3 + 6 * i))
+            if cross is not None:
+                oc, lsec = ops.sdpa_segments_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, *cross[0],
+                                                 drop=D(E + 3 + 6 * i), causal=False, kv_bounds=cross[1])
+            else:
+                oc, lsec = ops.sdpa_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, False, kv_mask=mask,
+                                        drop=D(E + 3 + 6 * i))
             return oc, lsec, kvc
         dacts = [] if save else None
         hf, rfd, xfd = self._decode(dec_ids, B, Sd, attend, cross_attend, dacts, base)
@@ -336,13 +397,15 @@ class MT5ForConditionalGeneration(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, Sd, shift=0, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base)
+                ctx = (eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base,
+                       segs)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base = ctx
+        eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base, segs = ctx
+        enc_seg, dec_seg, cross = (None, None, None) if segs is None else segs
         d, nh, dk, inner = self.d, self.nh, self.dk, self.inner
         P = self.P
         Te, Td = B * Se, B * Sd
@@ -373,8 +436,14 @@ class MT5ForConditionalGeneration(FlatModel):
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             kv5, dkv5 = kvc.view(B, Se, 2, nh, dk), dkvc.view(B, Se, 2, nh, dk)
-            ops.sdpa_bwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], oc, doc.view(B, Sd, nh, dk), lsec, 1.0, False,
-                         dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1], kv_mask=mask, drop=D(E + 3 + 6 * i))
+            if cross is not None:
+                ops.sdpa_segments_bwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], oc, doc.view(B, Sd, nh, dk), lsec,
+                                      1.0, *cross[0], dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1],
+                                      drop=D(E + 3 + 6 * i), causal=False, kv_bounds=cross[1])
+            else:
+                ops.sdpa_bwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], oc, doc.view(B, Sd, nh, dk), lsec, 1.0,
+                             False, dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1], kv_mask=mask,
+                             drop=D(E + 3 + 6 * i))
             dh2 = pj.cq.backward(dqc, h2, acc)
             pj.ckv.backward(dkvc, enc_h, acc, dx=denc32, dx_accumulate=(i != self.nd - 1))
             dy1, da = residual_norm_bwd(dh2, y1, P(p + "1.layer_norm.weight"), None, r2, D(E + 2 + 6 * i), acc, dres=dy2)
@@ -382,8 +451,13 @@ class MT5ForConditionalGeneration(FlatModel):
             do = pj.o.backward(da, o.view(Td, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Sd, 3, nh, dk), dqkv.view(B, Sd, 3, nh, dk)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, True,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], rel_bias=rel_d, drel_bias=drel_d, drop=D(E + 1 + 6 * i))
+            if dec_seg is not None:
+                ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, *dec_seg,
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(E + 1 + 6 * i), rel_bias=rel_d,
+                                      drel_bias=drel_d)
+            else:
+                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, True,
+                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], rel_bias=rel_d, drel_bias=drel_d, drop=D(E + 1 + 6 * i))
             dh1 = pj.qkv.backward(dqkv, h1, acc)
             # layer 0's norm had no residual (y = the embeddings); layer i's summed layer i-1's dropped FFN output into y
             dy, dm = residual_norm_bwd(dh1, y, P(p + "0.layer_norm.weight"), None, r1, D(E + 6 * i) if i > 0 else None, acc,
@@ -409,9 +483,14 @@ class MT5ForConditionalGeneration(FlatModel):
             do = pj.o.backward(da, o.view(Te, inner), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Se, 3, nh, dk), dqkv.view(B, Se, 3, nh, dk)
-            ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Se, nh, dk), lse, 1.0, False,
-                         d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, rel_bias=rel_e, drel_bias=drel_e,
-                         drop=D(1 + 4 * i))
+            if enc_seg is not None:
+                ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Se, nh, dk), lse, 1.0, *enc_seg,
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(1 + 4 * i), causal=False,
+                                      rel_bias=rel_e, drel_bias=drel_e)
+            else:
+                ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Se, nh, dk), lse, 1.0, False,
+                             d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, rel_bias=rel_e, drel_bias=drel_e,
+                             drop=D(1 + 4 * i))
             dh1 = pj.qkv.backward(dqkv, h1, acc)
             dx, dm = residual_norm_bwd(dh1, x, P(p + "0.layer_norm.weight"), None, r1, D(4 * i) if i > 0 else None, acc,
                                        dres=dx1)

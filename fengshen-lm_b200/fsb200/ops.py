@@ -765,24 +765,44 @@ def segment_bounds(segment_ids):
 _NO_DROP = (0.0, 0, None, 0)   # p, seed, stream_base, site of an entry with a dropout signature, run without dropout
 
 
-def _chk_bounds(seg_start, seg_end, B, S):
-    for t, n in ((seg_start, "seg_start"), (seg_end, "seg_end")):
+def _chk_bounds(seg_start, seg_end, B, S, names=("seg_start", "seg_end")):
+    for t, n in zip((seg_start, seg_end), names):
         _chk(t, torch.int32, n)
         if tuple(t.shape) != (B, S) or not t.is_contiguous():
             raise RuntimeError(f"fsb200: {n} must be contiguous int32 [batch, seq] = [{B}, {S}], got {tuple(t.shape)}")
 
 
-def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, causal=True):
+def _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B):
+    """The optional operands of sdpa_segments_fwd / _bwd: rel_bias [H, Sq + Skv - 1] or kv_bounds (two int32 [B, Skv]),
+    not both; the cross form (kv_bounds) has no causal mask."""
+    if rel_bias is not None:
+        if kv_bounds is not None:
+            raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) takes no rel_bias")
+        _chk_rel(rel_bias, H, Sq, Skv, "rel_bias")
+    if kv_bounds is not None:
+        if causal:
+            raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) has no causal mask: pass causal=False")
+        _chk_bounds(kv_bounds[0], kv_bounds[1], B, Skv, ("q_start", "q_end"))
+
+
+def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, causal=True, rel_bias=None, kv_bounds=None):
     """sdpa_fwd over rows that pack several sequences: causal inside each segment, nothing across segments. q, k, v as in
     sdpa_fwd (seq_q == seq_kv); seg_start / seg_end from segment_bounds. Key / query tiles outside a tile's segments are
     skipped. drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 when p > 0).
     causal=False: bidirectional inside each segment (packed encoder rows: query q sees seg_start[q] <= k < seg_end[q]),
-    head_dim 64 only (fsb_sdpa_fwd_segments_bidirectional). Returns (out [B, S, H, D], lse)."""
+    head_dim 64 only (fsb_sdpa_fwd_segments_bidirectional).
+    rel_bias: the T5 relative-position bias of sdpa_fwd (fp32 [H, 2 S - 1]) added inside either segment form, head_dim 64
+    only (fsb_sdpa_fwd_segments_bias).
+    kv_bounds=(q_start, q_end): cross-attention from packed decoder rows to packed encoder rows (seq_q and seq_kv may
+    differ, causal=False): seg_start / seg_end are then the query side's key ranges kv_start / kv_end [B, Sq] and kv_bounds
+    the key side's query ranges [B, Skv] (models/base.py cross_segment_bounds), head_dim 64 only
+    (fsb_sdpa_fwd_segments_cross). Returns (out [B, Sq, H, D], lse)."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")
     _chk_bounds(seg_start, seg_end, B, Sq)
+    _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B)
     if out is None:
         out = torch.empty((B, Sq, H, D), dtype=_bf16, device=q.device)
     if tuple(out.shape) != (B, Sq, H, D): raise RuntimeError(f"fsb200: out shape {tuple(out.shape)} != {(B, Sq, H, D)}")
@@ -790,8 +810,13 @@ def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, c
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     args = (_p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs, v_hs, o_hs,
             float(scale), _p(seg_start), _p(seg_end))
-    if not causal:
-        L.call("fsb_sdpa_fwd_segments_bidirectional", *args, *(_NO_DROP if drop is None else drop.args()), _stream())
+    drop_args = _NO_DROP if drop is None else drop.args()
+    if kv_bounds is not None:
+        L.call("fsb_sdpa_fwd_segments_cross", *args, _p(kv_bounds[0]), _p(kv_bounds[1]), *drop_args, _stream())
+    elif rel_bias is not None:
+        L.call("fsb_sdpa_fwd_segments_bias", *args, int(bool(causal)), _p(rel_bias), *drop_args, _stream())
+    elif not causal:
+        L.call("fsb_sdpa_fwd_segments_bidirectional", *args, *drop_args, _stream())
     elif drop is None:
         L.call("fsb_sdpa_fwd_segments", *args, _stream())
     else:
@@ -799,8 +824,10 @@ def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, c
     return out, lse
 
 
-def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv, drop=None, causal=True):
-    """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end, drop and causal); dq / dk / dv are written as in
+def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv, drop=None, causal=True,
+                      rel_bias=None, drel_bias=None, kv_bounds=None):
+    """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end, drop, causal, rel_bias and kv_bounds); dq / dk / dv
+    are written as in sdpa_bwd. drel_bias (with rel_bias): fp32 [H, 2 S - 1], accumulated into (+=) deterministically, as in
     sdpa_bwd."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -814,12 +841,26 @@ def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk
         _chk(t, _bf16, n)
     _chk_grads(q, k, dq, dk, dv)
     _chk_bounds(seg_start, seg_end, B, Sq)
+    _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B)
+    ws, ws_bytes = None, 0
+    if drel_bias is not None:
+        if rel_bias is None:
+            raise RuntimeError("fsb200: drel_bias needs rel_bias")
+        _chk_rel(drel_bias, H, Sq, Skv, "drel_bias")
+        ws_bytes = int(L.load().fsb_sdpa_bwd_workspace_bytes(B, Sq, Skv, H))
+        ws = workspace(ws_bytes, q.device, "sdpa_dbias")
     delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     args = (_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv, H, D, q_rs,
             k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs, float(scale),
             _p(seg_start), _p(seg_end))
-    if not causal:
-        L.call("fsb_sdpa_bwd_segments_bidirectional", *args, *(_NO_DROP if drop is None else drop.args()), _stream())
+    drop_args = _NO_DROP if drop is None else drop.args()
+    if kv_bounds is not None:
+        L.call("fsb_sdpa_bwd_segments_cross", *args, _p(kv_bounds[0]), _p(kv_bounds[1]), *drop_args, _stream())
+    elif rel_bias is not None:
+        L.call("fsb_sdpa_bwd_segments_bias", *args, int(bool(causal)), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes,
+               *drop_args, _stream())
+    elif not causal:
+        L.call("fsb_sdpa_bwd_segments_bidirectional", *args, *drop_args, _stream())
     elif drop is None:
         L.call("fsb_sdpa_bwd_segments", *args, _stream())
     else:

@@ -438,6 +438,65 @@ int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k, const void
                                         int64_t dv_head_stride, float scale, const int32_t* seg_start,
                                         const int32_t* seg_end, float p, uint64_t seed, const int64_t* stream_base,
                                         int64_t site, fsb_stream_t stream);
+/* fsb_sdpa_fwd_segments_bias / fsb_sdpa_bwd_segments_bias: packed mT5 / T5 self-attention, the segment rule of
+ * fsb_sdpa_*_segments (causal = 1, the decoder) or of fsb_sdpa_*_segments_bidirectional (causal = 0, the encoder) plus the
+ * additive relative-position bias rel_bias of fsb_sdpa_fwd (fp32 [nheads, 2 seq - 1] over the offset k - q). The bias depends
+ * on (q, k) through k - q only, so inside a segment the scores are those of the segment run alone and no position ids are
+ * needed. The same seg_start / seg_end bounds for both directions; tile skipping and clamping as in those pairs. Dropout as
+ * in fsb_sdpa_*_segments_dropout (p == 0 runs the dropout-free kernels and does not read the stream counter). The backward
+ * accumulates the bias gradient into drel_bias (or skips it when null) as fsb_sdpa_bwd does, with the same workspace of
+ * fsb_sdpa_bwd_workspace_bytes bytes: the reduction reads exactly the per-step slots the dQ pass wrote (the steps the
+ * segment bounds skip are neither written nor read), so the workspace needs no clearing. No kv_mask. Refused: null bounds,
+ * a null rel_bias, seq_q != seq_kv, head_dim other than 64, drel_bias without a large enough workspace, and with p > 0
+ * sequences longer than 65536. */
+int fsb_sdpa_fwd_segments_bias(const void* q, const void* k, const void* v, void* o, float* lse,
+                               int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                               int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                               int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                               float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
+                               const float* rel_bias, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
+                               fsb_stream_t stream);
+int fsb_sdpa_bwd_segments_bias(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                               const float* lse, float* delta, void* dq, void* dk, void* dv,
+                               int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                               int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                               int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                               int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                               int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                               float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
+                               const float* rel_bias, float* drel_bias, void* workspace, size_t workspace_bytes,
+                               float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
+/* fsb_sdpa_fwd_segments_cross / fsb_sdpa_bwd_segments_cross: packed encoder-decoder cross-attention. Row b of the queries
+ * (seq_q decoder tokens) attends to row b of the keys (seq_kv encoder tokens); seq_q and seq_kv may differ. Four int32
+ * bounds arrays, contiguous, indices relative to the row:
+ *   kv_start[b][q], kv_end[b][q] ([batch, seq_q])  : query q sees the keys kv_start[q] <= k < kv_end[q];
+ *   q_start[b][k],  q_end[b][k]  ([batch, seq_kv]) : key k is seen by the queries q_start[k] <= q < q_end[k].
+ * They must describe the same visibility, and each array must be non-decreasing along the row (segments paired in order,
+ * e.g. by equal segment id). Then the forward and dQ pass visit the key tiles from the one of kv_start[first query of the
+ * tile] to the one of kv_end[last query of the tile] - 1, the dK / dV pass the query tiles from q_start[first key] to
+ * q_end[last key] - 1, clamped into the sequence. An empty range is legal: a query that sees no key writes O = 0 and
+ * LSE = +inf (which makes its dQ and its share of dK / dV exactly 0), and a key no query sees gets dK = dV = 0; every
+ * output element is written. Invalid bounds give unspecified results but never an out-of-bounds access. Dropout as in
+ * fsb_sdpa_*_segments_dropout: an element's keep bit is that of its row-relative (q, k) in an unsegmented non-causal launch.
+ * p == 0 runs the dropout-free kernels and does not read the stream counter. No kv_mask, no rel_bias. The forward reads
+ * kv_start / kv_end only. Refused: null bounds, head_dim other than 64, and with p > 0 sequences longer than 65536. */
+int fsb_sdpa_fwd_segments_cross(const void* q, const void* k, const void* v, void* o, float* lse,
+                                int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                float scale, const int32_t* kv_start, const int32_t* kv_end, const int32_t* q_start,
+                                const int32_t* q_end, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
+                                fsb_stream_t stream);
+int fsb_sdpa_bwd_segments_cross(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                const float* lse, float* delta, void* dq, void* dk, void* dv,
+                                int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
+                                int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
+                                int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
+                                int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
+                                int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
+                                float scale, const int32_t* kv_start, const int32_t* kv_end, const int32_t* q_start,
+                                const int32_t* q_end, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
+                                fsb_stream_t stream);
 
 int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
                               void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
