@@ -63,6 +63,8 @@ class Llama(pl.LightningModule):
         parser.add_argument('--num_heads', type=int, default=40)
         parser.add_argument('--vocab_size', type=int, default=39424)
         parser.add_argument('--num_samples', type=int, default=4096)
+        parser.add_argument('--gradient_checkpointing', action='store_true',
+                            help='recompute each layer in the backward instead of keeping its activations')
         return parent_parser
 
     def __init__(self, args):
@@ -74,6 +76,8 @@ class Llama(pl.LightningModule):
         config = LlamaConfig(vocab_size=self.hparams.vocab_size, hidden_size=self.hparams.hidden_size,
                              num_hidden_layers=self.hparams.num_layers, num_attention_heads=self.hparams.num_heads)
         self.model = LlamaForCausalLM(config).cuda()
+        if self.hparams.gradient_checkpointing:
+            self.model.gradient_checkpointing_enable()
         if stage == 'fit':
             self.total_steps = get_total_steps(self.trainer, self.hparams)
             print('Total steps: {}'.format(self.total_steps))

@@ -38,6 +38,8 @@ class LlamaForCausalLM(_FsbLlama):
         load_in_4bit=True (hf_quantizatin_inference.py:3,16): the same with int4 projections (one bf16 scale per row and
         group of 128 k), loaded the same way. Passing both flags raises ValueError.
         fp8=True (passed on to the model like the other keywords): train the layer projections in FP8 (fsb200/models/llama.py).
+        gradient_checkpointing=True (passed on the same way): recompute each layer in the backward instead of keeping its
+        activations, as `model.gradient_checkpointing_enable()` does after loading.
         device_map: None, "auto" or one device (the model lives on one GPU); a map over several devices raises."""
         if device_map is not None and device_map != "auto":
             if isinstance(device_map, dict):

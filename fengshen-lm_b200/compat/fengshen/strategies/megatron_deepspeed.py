@@ -24,7 +24,10 @@ class DeepSpeedStrategy(OriginDeepSpeedStrategy):
         """megatron_deepspeed.py:339-369 at PP = 1: load the kernels, build the tensor- / data-parallel groups, seed."""
         fused_kernels.load_fused_kernels()
         mpu.initialize_model_parallel(self.tensor_model_parallel_size, self.pipe_model_parallel_size)
-        if "activation_checkpointing" in self.config:  # accepted and ignored: the reference never recomputes (SURVEY §2.4)
+        # The `activation_checkpointing` block is accepted and ignored. In DeepSpeed it only configures
+        # deepspeed.checkpointing.checkpoint, which the reference model never calls (SURVEY §2.4), so honouring it would change
+        # the speed and memory of unmodified recipe runs. Recompute is the model's own switch: gradient_checkpointing_enable().
+        if "activation_checkpointing" in self.config:
             pass
         import torch
         torch.manual_seed(self.mpu_seed)

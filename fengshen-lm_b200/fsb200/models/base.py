@@ -147,6 +147,25 @@ class FlatModel(nn.Module):
     def P(self, name):
         return self._p[name]
 
+    # ---- activation recompute (HF PreTrainedModel's gradient-checkpointing names) --------------------------------------
+    supports_gradient_checkpointing = False   # a subclass that recomputes sets it and reads self.gradient_checkpointing
+    gradient_checkpointing = False
+
+    @property
+    def is_gradient_checkpointing(self):
+        return self.gradient_checkpointing
+
+    def gradient_checkpointing_enable(self, gradient_checkpointing_kwargs=None):
+        """Recompute activations in the backward instead of keeping them. gradient_checkpointing_kwargs (HF passes them on to
+        torch.utils.checkpoint, e.g. use_reentrant) are accepted and ignored: the recompute is the model's own."""
+        if not self.supports_gradient_checkpointing:
+            raise NotImplementedError(f"fsb200 {type(self).__name__}: activation recompute (gradient checkpointing) is not "
+                                      "implemented for this model; it keeps every layer's activations")
+        self.gradient_checkpointing = True
+
+    def gradient_checkpointing_disable(self):
+        self.gradient_checkpointing = False
+
     # The reference scripts call `.from_pretrained(..., torch_dtype=torch.half).cuda()`; parameters here are views into the
     # flat bf16 CUDA buffer and must never be re-allocated by nn.Module._apply.
     def cuda(self, device=None):

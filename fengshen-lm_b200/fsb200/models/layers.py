@@ -38,6 +38,10 @@ class Linear:
         """-> (the output, what backward reads of the input: x itself when `save`, else None)."""
         return self(x), (x if save else None)
 
+    def saved_input(self, x):
+        """What backward reads of the input x, without the GEMM: what forward(x, save=True) returns second."""
+        return x
+
     def backward(self, dy, x, accumulate, dx=None, dx_accumulate=False, colsum=True):
         """-> the gradient of the input x, given dy, the gradient of the output. Writes the weight's gradient (and the bias's)
         into the flat gradient buffer, adding to it when `accumulate`. dx: write the input gradient into this buffer instead,
@@ -81,12 +85,15 @@ class GatedMLP:
     def __init__(self, wi, wo, act):
         self.wi, self.wo, self.act = wi, wo, act
 
-    def __call__(self, h, save=True, drop=None):
+    def __call__(self, h, save=True, drop=None, out=True):
         """-> (m, what the backward reads; with save=False, only what a forward needs is computed). drop: optional
-        ops.Dropout on act(gate) * up, the input of wo (mT5's dropout inside the FFN)."""
+        ops.Dropout on act(gate) * up, the input of wo (mT5's dropout inside the FFN). out=False (with save): stop before
+        wo's GEMM, for a recompute whose m nothing reads; m is then None."""
         gu, hs = self.wi.forward(h, save)
         f = gu.shape[1] // 2
         act = ops.glu_fwd(self.act, gu[:, :f], gu[:, f:], drop=drop)
+        if not out:
+            return None, (hs, gu, self.wo.saved_input(act))
         m, acts = self.wo.forward(act, save)
         return m, (hs, gu, acts)
 
@@ -121,6 +128,12 @@ class Fp8Linear:
         xq, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=save)
         wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
         return ops.gemm_fp8(xq, sx, wq, sw), ((xt, sx) if save else None)
+
+    def saved_input(self, x):
+        """What backward reads of the input x, without the GEMM: x's transposed e4m3 codes and scale, the bits forward(x,
+        save=True) keeps (the scale depends on x's amax alone, and the cast writes both layouts independently)."""
+        _, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=False, colwise=True)
+        return xt, sx
 
     def backward(self, dy, saved, accumulate, dx=None, dx_accumulate=False):
         xt, sx = saved

@@ -73,8 +73,10 @@ class QuantizedLinear:
 
 
 class LlamaForCausalLM(FlatModel):
+    supports_gradient_checkpointing = True
+
     def __init__(self, config, device=None, world_size=None, seed=0, tp_group=None, load_in_8bit=False, load_in_4bit=False,
-                 fp8=False):
+                 fp8=False, gradient_checkpointing=False):
         """tp_group: the tensor-model-parallel process group (mpu.get_model_parallel_group()) or None. With t = its size > 1
         this rank holds the shard the reference's `part_{rank}` checkpoints hold (utils/llama_convert/convert_fs_llama_tp.py
         :143-181): heads / ff columns / vocabulary rows split t ways (ColumnParallelLinear mpu/layers.py:261-360 for QKV,
@@ -96,8 +98,16 @@ class LlamaForCausalLM(FlatModel):
         as do the master weights, the gradients and the optimizer state, so checkpoints and resume are unchanged. The training
         and no-grad (validation) forwards run FP8; `generate` runs the bf16 layer stack on the same weights. Results differ from
         bf16 by design. hidden_size, the MLP width and the tokens per micro-batch must be multiples of 16 (checked at the first
-        forward); tensor parallelism and load_in_8bit / load_in_4bit are refused."""
+        forward); tensor parallelism and load_in_8bit / load_in_4bit are refused.
+
+        gradient_checkpointing: activation recompute (also `gradient_checkpointing_enable()` / `_disable()`). The training
+        forward keeps only the residual stream entering each layer; the backward re-runs each layer's forward from it, up to
+        what the layer's backward reads (not the w2 GEMM), just before that layer's backward. The gradients are bit-identical
+        to those without it, at about one more forward of the layers; the activation memory of the layers drops from one
+        saved set per layer to one bf16 [tokens, hidden] tensor per layer plus one saved set. The no-grad forward and
+        `generate` keep nothing either way and are unaffected; so are int8 / int4 models, which do not train."""
         super().__init__(config)
+        self.gradient_checkpointing = bool(gradient_checkpointing)
         import torch.distributed as dist
         if load_in_8bit and load_in_4bit:
             raise ValueError("fsb200 LlamaForCausalLM: load_in_8bit and load_in_4bit are mutually exclusive; pass one")
@@ -339,15 +349,19 @@ class LlamaForCausalLM(FlatModel):
         return SimpleNamespace(loss=loss, logits=None if logits is None else logits.view(B, S, self.V),
                                past_key_values=None, hidden_states=None, attentions=None)
 
+    def _attend(self, seg):
+        """The training attention over a layer's q|k|v view (see _stack): causal, or inside the segments of packed rows
+        when seg holds their (seg_start, seg_end) bounds (ops.segment_bounds)."""
+        scale = 1.0 / math.sqrt(self.hn)
+        if seg is None:
+            return lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, True)
+        return lambda i, q5: ops.sdpa_segments_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, *seg)
+
     def _forward_impl(self, ids, pos, lab, B, S, seg=None, *, save, want_logits):
         """seg: None or the (seg_start, seg_end) bounds of packed rows (ops.segment_bounds)."""
-        scale = 1.0 / math.sqrt(self.hn)
         acts = [] if save else None
-        if seg is None:
-            attend = lambda i, q5: ops.sdpa_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, True)
-        else:
-            attend = lambda i, q5: ops.sdpa_segments_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], scale, *seg)
-        hf, rstdf, xf = self._stack(ids, pos, B, S, attend, acts)
+        recompute = save and self.gradient_checkpointing   # fixed for this step: the backward reads it from ctx
+        hf, rstdf, xf = self._stack(ids, pos, B, S, self._attend(seg), acts, checkpoints=recompute)
         logits = self._head(hf)
         logits = self._tp_gather_columns(logits)   # ParallelLinear(parallel_output=False): full-vocabulary logits on every rank
         loss = None
@@ -357,44 +371,56 @@ class LlamaForCausalLM(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, S, shift=1, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (acts, hf, rstdf, xf, dlogits, ids, pos, B, S, seg)
+                ctx = (acts, recompute, hf, rstdf, xf, dlogits, ids, pos, B, S, seg)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
-    def _stack(self, ids, pos, B, S, attend, acts=None, proj=None):
+    def _stack(self, ids, pos, B, S, attend, acts=None, proj=None, checkpoints=False):
         """Embedding, the layers and the final norm over ids [B * S] -> (hidden states, their rstd, residual stream).
         attend(i, q5) is layer i's attention over the per-head interleaved q|k|v view [B, S, heads, 3, head_dim] (rotary
-        embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads. proj: the layers'
-        projections (default self._proj)."""
-        nh, hn, hl = self.nh_l, self.hn, self.h_l      # LOCAL heads under tensor parallelism
-        save = acts is not None
+        embedding applied) -> (out, lse); `acts`, when given, collects what the backward reads: per layer the saved tuple of
+        `_layer`, or with `checkpoints` only the residual stream entering the layer, from which the backward recomputes the
+        rest. proj: the layers' projections (default self._proj)."""
+        save = acts is not None and not checkpoints
         self._need("no_decay"); self._need("embed_in")
         ids_l, emb_keep = self._local_ids(ids)
         x = ops.embedding_fwd(ids_l, self.llama.embed_in.word_embeddings.weight.data)
         if emb_keep is not None:      # VocabParallelEmbedding.forward (mpu/layers.py:104-130): foreign rows are zero, then all-reduce
             x.mul_(emb_keep)
             self._tp_all_reduce(x)
-        prev_m = None
-        for i, (lyr, lp) in enumerate(zip(self.llama.layers, self._proj if proj is None else proj)):
-            self._need(f"layer{i}")
-            h1, rstd1, x = ops.rmsnorm_fwd(x if prev_m is None else prev_m, lyr.input_layernorm.scale.data, self.eps,
-                                           residual=None if prev_m is None else x)
-            qkv, h1s = lp.qkv.forward(h1, save)   # h1s: what the QKV weight gradient reads of h1
-            ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
-            ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
-            o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
-            a, os_ = lp.dense.forward(o.view(B * S, hl), save)
-            self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
-            h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
-            m, ms = lp.mlp(h2, save)
-            self._tp_all_reduce(m)        # RowParallelLinear (w2)
+        m = None
+        for i, lp in enumerate(self._proj if proj is None else proj):
+            xs, x, m, saved = self._layer(i, lp, x, m, pos, B, S, attend, save)
             if acts is not None:
-                acts.append((x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms))
-            # free this layer's temporaries before the next layer allocates its own (the peak of a long prompt's prefill)
-            del rstd1, h1, h1s, qkv, o, os_, lse, a, rstd2, h2, ms
-            x, prev_m = x1, m
+                acts.append(xs if checkpoints else saved)
+            del xs, saved
         self._need("head")
-        return ops.rmsnorm_fwd(prev_m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
+        return ops.rmsnorm_fwd(m, self.llama.final_layer_norm.scale.data, self.eps, residual=x)
+
+    def _layer(self, i, lp, x, m, pos, B, S, attend, save, out=True):
+        """Layer i with projections lp over the residual stream x plus m, the previous layer's MLP output (None for the
+        first layer, or when x already is that sum) -> (xs, x1, m', saved): xs = x + m, the layer's input; x1 = xs + the
+        attention output; m' the MLP output; saved (with `save`) what the backward reads. Its temporaries are freed on
+        return, before the next layer allocates its own (the peak of a long prompt's prefill). out=False (with save): stop
+        before the w2 GEMM and its all-reduce, for a recompute whose m' nothing reads; m' is then None."""
+        nh, hn, hl = self.nh_l, self.hn, self.h_l      # LOCAL heads under tensor parallelism
+        lyr = self.llama.layers[i]
+        self._need(f"layer{i}")
+        # without a residual the kernel returns x itself; with one, the bf16-rounded sum, over which it takes the row
+        # statistics: a recompute from the stored sum reproduces h1 and rstd1 bit for bit (csrc/norm.cu, norm_fwd_kernel)
+        h1, rstd1, x = ops.rmsnorm_fwd(x if m is None else m, lyr.input_layernorm.scale.data, self.eps,
+                                       residual=None if m is None else x)
+        qkv, h1s = lp.qkv.forward(h1, save)   # h1s: what the QKV weight gradient reads of h1
+        ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=0)
+        ops.rope_inplace(qkv, self._cos, self._sin, pos, nh, hn, 3 * hl, 3 * hn, offset=hn)
+        o, lse = attend(i, qkv.view(B, S, nh, 3, hn))
+        a, os_ = lp.dense.forward(o.view(B * S, hl), save)
+        self._tp_all_reduce(a)        # RowParallelLinear: partial sums over the head shards (mpu/layers.py:451-470)
+        h2, rstd2, x1 = ops.rmsnorm_fwd(a, lyr.post_attention_layernorm.scale.data, self.eps, residual=x)
+        m, ms = lp.mlp(h2, save, out=out)
+        if out:
+            self._tp_all_reduce(m)    # RowParallelLinear (w2)
+        return x, x1, m, ((x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms) if save else None)
 
     # ---- KV-cache inference (SURVEY.md §8f rank 4) -----------------------------------------------------------------------
     # The reference decodes through HF's GenerationMixin: `prepare_inputs_for_generation` (modeling_llama.py:353-377) feeds the
@@ -489,7 +515,7 @@ class LlamaForCausalLM(FlatModel):
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        acts, hf, rstdf, xf, dlogits, ids, pos, B, S, seg = ctx
+        acts, recompute, hf, rstdf, xf, dlogits, ids, pos, B, S, seg = ctx
         nh, hn, hl = self.nh_l, self.hn, self.h_l
         T = B * S
         acc = self.accumulate_grads
@@ -504,9 +530,16 @@ class LlamaForCausalLM(FlatModel):
         self._done("head")
         fscale = self.llama.final_layer_norm.scale
         dx = ops.rmsnorm_bwd(dhf, xf, fscale.data, rstdf, fscale.main_grad, accumulate=acc)
+        attend = self._attend(seg) if recompute else None
         for i in reversed(range(self.nl)):
             lyr, lp = self.llama.layers[i], self._proj[i]
-            x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms = acts[i]
+            if recompute:   # layer i's forward again from its input, up to what its backward reads; the kernels are
+                # deterministic, so these are the bits the forward computed. The parameters are already gathered (_need is a
+                # no-op) and nothing here advances state (LLaMA has no dropout)
+                x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms = self._layer(i, lp, acts[i], None, pos, B, S, attend,
+                                                                             save=True, out=False)[3]
+            else:
+                x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms = acts[i]
             acts[i] = None
             # x_next = x1 + m  ->  dm = dx, residual gradient into x1 = dx
             dh2 = lp.mlp.backward(dx, ms, acc)
@@ -529,6 +562,8 @@ class LlamaForCausalLM(FlatModel):
             self._tp_all_reduce(dh1)      # column-parallel QKV: dgrad partial sums
             s1 = lyr.input_layernorm.scale
             dx = ops.rmsnorm_bwd(dh1, x, s1.data, rstd1, s1.main_grad, accumulate=acc, dres=dx1)
+            # free this layer's activations and transients before the next layer's recompute allocates its own
+            del x, rstd1, h1s, qkv, o, os_, lse, x1, rstd2, ms, dh2, dx1, do, dqkv, q5, d5, dh1
             self._done(f"layer{i}")
         W_in = self.llama.embed_in.word_embeddings.weight
         if not acc:

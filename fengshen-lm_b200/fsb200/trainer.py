@@ -26,7 +26,7 @@ class PretrainStep:
         # corrections) live in static device buffers that are refreshed before each replay. What a tracing compiler would do
         # for a launch-bound step (BERT-base at batch 8 is ~600 launches for ~1 ms of GPU work), done with the stream API.
         self.cuda_graph = bool(cuda_graph)
-        self._graph, self._static = None, None
+        self._graph, self._static, self._graph_recompute = None, None, None
         if self.cuda_graph:
             if self.engine.world > 1:
                 raise RuntimeError("PretrainStep(cuda_graph=True) is single-GPU: the engine's side-stream collectives of step t "
@@ -69,7 +69,15 @@ class PretrainStep:
         """One optimizer step from batches already resident on the device. Returns the loss as a 0-d device tensor."""
         eng = self.engine
         if self.cuda_graph:
+            # the graph holds the launches of the activation-recompute mode set at capture (model.gradient_checkpointing)
+            recompute = bool(getattr(self.model, "is_gradient_checkpointing", False))
+            if self._graph is not None and recompute != self._graph_recompute:
+                raise RuntimeError(f"PretrainStep(cuda_graph=True) captured its step with gradient checkpointing "
+                                   f"{'on' if self._graph_recompute else 'off'}; the model now has it "
+                                   f"{'on' if recompute else 'off'}, and a replay would run the captured mode. Set the mode "
+                                   "before the first step, or build a new PretrainStep")
             if self._graph is None:
+                self._graph_recompute = recompute
                 state = [eng.master, eng.exp_avg, eng.exp_avg_sq, self.model.flat.params]
                 counter = getattr(self.model, "dropout_counter", None)
                 if counter is not None:    # the dropout stream counter advances on the device in every training forward
