@@ -15,7 +15,10 @@ class. The recipe's DeepSpeed JSON (ZeRO stage, gradient_clipping) is read from 
 
 --pack_sequences (off by default) wraps the collator, Python or --native_collator, in fsb200.packing.MLMPackingCollator: the
 documents of a batch are packed whole into rows of --max_seq_length instead of one padded document per row, and
-`forward(**batch)` hands the packed keys (segment_ids, position_ids, cls_positions) to the model."""
+`forward(**batch)` hands the packed keys (segment_ids, position_ids, cls_positions) to the model.
+
+--fp8 (off by default) builds the model with `fp8=True`: each layer's four projections train in FP8 (e4m3 activations and
+weights, e5m2 gradients, per-tensor scales); the weights, gradients, optimizer state and checkpoints stay as without it."""
 import argparse
 import json
 import os
@@ -64,7 +67,9 @@ class ErLangShenBert(LightningModule):
         self.save_hyperparameters(args)
         self.tokenizer = tokenizer
         self.config = MegatronBertConfig.from_pretrained(args.model_path)
-        self.model = MegatronBertForPreTraining(self.config)
+        # fp8 is an fsb200 keyword: pass it only when asked, so that the default build is the reference's call
+        self.model = (MegatronBertForPreTraining(self.config, fp8=True) if getattr(args, 'fp8', False)
+                      else MegatronBertForPreTraining(self.config))
 
     def setup(self, stage):
         if stage == 'fit':
@@ -102,6 +107,8 @@ def parse_args(argv=None):
                         help='assemble and mask the samples in libfsb200.so (fsb_bert_collate): same batches, ~1000x less host time')
     parser.add_argument('--pack_sequences', action='store_true', default=False,
                         help='pack the documents of each batch whole into rows of max_seq_length (fsb200.packing)')
+    parser.add_argument('--fp8', action='store_true', default=False,
+                        help="train the layer projections in FP8 (fsb200's MegatronBertForPreTraining(config, fp8=True))")
     for add in (add_module_args, UniversalDataModule.add_data_specific_args, Trainer.add_argparse_args,
                 ErLangShenBert.add_module_specific_args, UniversalCheckpoint.add_argparse_args):
         parser = add(parser)

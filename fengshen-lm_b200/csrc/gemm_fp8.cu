@@ -15,9 +15,13 @@
 //   * Promotion: the four m64n128k32 wgmmas of a k-block write a fresh partial sum, which is added into a separate fp32
 //     accumulator once they retire (the tensor cores keep fewer than fp32's bits while they accumulate FP8 products). 64 + 64
 //     accumulator registers per thread.
-//   * Epilogue: acc * a_scale_inv * b_scale_inv (the scales read from device memory: a captured graph stays valid), plus the
-//     old D in fp32 when accumulating, rounded once to bf16, staged in 64-row x 64-column sub-tiles and stored by TMA, which
-//     clips ragged m / n edges. No split-K: results are deterministic.
+//   * Epilogue: acc * a_scale_inv * b_scale_inv (the scales read from device memory: a captured graph stays valid), then,
+//     in the kEpi instantiations only, + bias[n] -> aux = bf16(that value) -> GELU (gemm_epilogue.cuh, gemm.cu's device code),
+//     plus the old D in fp32 when accumulating, rounded once to bf16, staged in 64-row x 64-column sub-tiles and stored by
+//     TMA, which clips ragged m / n edges; aux leaves through the same staging buffers as a second store per sub-tile. The
+//     plain instantiations (no bias, aux or activation) are the ones LLaMA runs and carry none of that code. No split-K:
+//     results are deterministic.
+#include "gemm_epilogue.cuh"
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -47,12 +51,18 @@ struct F8Params {
   int M, N, K;
   int accumulate;
   int tiles_m, tiles_n, group_m;
+  // read by the kEpi instantiations only (appended, so the plain ones see the parameter block they always had)
+  const __nv_bfloat16* bias;   // [N] or null
+  int epilogue;                // fsb_gemm_epilogue
+  int has_aux;                 // tmAux is valid
 };
 
-template <bool kE5M2A>
+// kEpi: bias / GELU / aux in the epilogue. tmAux is the last parameter so that the plain kernels' parameter offsets are
+// unchanged.
+template <bool kE5M2A, bool kEpi>
 __global__ void __launch_bounds__(F8_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmD, const F8Params p) {
+                const __grid_constant__ CUtensorMap tmD, const F8Params p, const __grid_constant__ CUtensorMap tmAux) {
   using S = F8Smem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
@@ -69,7 +79,12 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     ring.init();
     fence_barrier_init();
   }
-  if (threadIdx.x == 128) tma_prefetch_desc(&tmD);
+  if (threadIdx.x == 128) {
+    tma_prefetch_desc(&tmD);
+    if constexpr (kEpi) {
+      if (p.has_aux) tma_prefetch_desc(&tmAux);
+    }
+  }
   __syncthreads();
 
   if (warp < 4) {
@@ -127,8 +142,51 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const int m0 = m_idx * F8_BM + wg * 64, n0 = n_idx * F8_BN;
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = acc[i] * sa * sb;
+      if constexpr (kEpi) {
+        // bias (0 without one, as gemm.cu: results do not depend on whether a bias was passed)
+#pragma unroll
+        for (int j = 0; j < F8_BN / 8; ++j) {
+          const int col = n0 + 8 * j + 2 * (lane & 3);
+          float bv0 = 0.f, bv1 = 0.f;
+          if (p.bias != nullptr && col < p.N) {   // N % 8 == 0: col < N implies col + 1 < N
+            bv0 = __bfloat162float(__ldg(p.bias + col));
+            bv1 = __bfloat162float(__ldg(p.bias + col + 1));
+          }
+          acc[4 * j] += bv0; acc[4 * j + 1] += bv1; acc[4 * j + 2] += bv0; acc[4 * j + 3] += bv1;
+        }
+      }
 #pragma unroll
       for (int g = 0; g < F8_BN / 64; ++g) {
+        if constexpr (kEpi) {
+          // pre-activation copy (bf16), through the staging buffers as D below. Written out rather than shared with D's
+          // store through a lambda: a lambda capturing these locals, even one the plain kernels never call, changed their
+          // instruction schedule.
+          if (p.has_aux) {
+            uint8_t* buf = epi_buf + (n_stored & 1) * S::EPI_BUF_BYTES;
+            if (leader) tma_store_wait_read<1>();
+            bar_sync(1 + wg, 128);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int j = 8 * g + jj;
+                *reinterpret_cast<uint32_t*>(buf + swz128(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                    pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+              }
+            fence_proxy_async();
+            bar_sync(1 + wg, 128);
+            if (leader) {
+              tma_store_2d(&tmAux, buf, n0 + 64 * g, m0);
+              tma_store_commit();
+            }
+            ++n_stored;
+          }
+#pragma unroll
+          for (int i = 32 * g; i < 32 * g + 32; ++i) {
+            if (p.epilogue == FSB_EPI_GELU_TANH) acc[i] = gelu_tanh_f(acc[i]);
+            else if (p.epilogue == FSB_EPI_GELU_ERF) acc[i] = gelu_erf_f(acc[i]);
+          }
+        }
         if (p.accumulate) {   // D += result: fp32 sum with the old value, rounded once
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
@@ -260,6 +318,14 @@ fp8_cast_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, int64_t rows, 
   }
 }
 
+template <bool kE5M2A, bool kEpi>
+static int launch_gemm_fp8(int grid, const F8Params& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
+                           const CUtensorMap& tmAux, cudaStream_t stream) {
+  if (int rc = ensure_smem<gemm_fp8_kernel<kE5M2A, kEpi>>(F8Smem::TOTAL, "gemm_fp8")) return rc;
+  gemm_fp8_kernel<kE5M2A, kEpi><<<grid, F8_THREADS, F8Smem::TOTAL, stream>>>(tmA, tmB, tmD, p, tmAux);
+  return FSB_OK;
+}
+
 }  // namespace fsb
 
 using namespace fsb;
@@ -299,8 +365,8 @@ extern "C" int fsb_fp8_quantize(const void* x, int64_t ldx, int64_t rows, int64_
 }
 
 extern "C" int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv,
-                            const void* b, int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, int accumulate,
-                            fsb_stream_t stream_) {
+                            const void* b, int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, const void* bias,
+                            int epilogue, int accumulate, void* aux, int64_t ldaux, fsb_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_fp8: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
   FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_fp8: dims too large");
@@ -313,8 +379,13 @@ extern "C" int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int 
   FSB_REQUIRE((reinterpret_cast<uintptr_t>(a_scale_inv) & 3) == 0 && (reinterpret_cast<uintptr_t>(b_scale_inv) & 3) == 0,
               "gemm_fp8: scale_inv pointers must be 4-byte aligned");
   FSB_REQUIRE(ldd >= n && ldd % 8 == 0, "gemm_fp8: ldd=%ld must be >= n and a multiple of 8", (long)ldd);
+  FSB_REQUIRE(epilogue >= FSB_EPI_NONE && epilogue <= FSB_EPI_GELU_ERF, "gemm_fp8: bad epilogue %d", epilogue);
+  FSB_REQUIRE(bias == nullptr || aligned16(bias), "gemm_fp8: bias must be 16-byte aligned");
+  FSB_REQUIRE(aux == nullptr || (aligned16(aux) && ldaux >= n && ldaux % 8 == 0),
+              "gemm_fp8: aux must be 16-byte aligned with ldaux=%ld >= n and a multiple of 8", (long)ldaux);
+  const bool epi = bias != nullptr || aux != nullptr || epilogue != FSB_EPI_NONE;
 
-  CUtensorMap tmA, tmB, tmD;
+  CUtensorMap tmA, tmB, tmD, tmAux;
   {
     uint64_t dims[2] = {uint64_t(k), uint64_t(m)};
     uint64_t strides[1] = {uint64_t(k)};
@@ -333,12 +404,22 @@ extern "C" int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int 
     uint32_t box[2] = {64, 64};
     if (int rc = make_tmap_bf16(&tmD, d, 2, dims, strides, box)) return rc;
   }
+  tmAux = tmD;   // never read without aux
+  if (aux != nullptr) {
+    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
+    uint64_t strides[1] = {uint64_t(ldaux) * 2};
+    uint32_t box[2] = {64, 64};
+    if (int rc = make_tmap_bf16(&tmAux, aux, 2, dims, strides, box)) return rc;
+  }
   F8Params p;
   p.D = static_cast<__nv_bfloat16*>(d);
   p.a_sinv = a_scale_inv; p.b_sinv = b_scale_inv;
   p.ldd = ldd;
   p.M = int(m); p.N = int(n); p.K = int(k);
   p.accumulate = accumulate;
+  p.bias = static_cast<const __nv_bfloat16*>(bias);
+  p.epilogue = epilogue;
+  p.has_aux = aux != nullptr;
   p.tiles_m = int((m + F8_BM - 1) / F8_BM);
   p.tiles_n = int((n + F8_BN - 1) / F8_BN);
   // rasterisation groups as gemm.cu's 128-wide tiles: 12 m-tiles, more while their A panels (128 x k bytes) fit ~32 MB of L2
@@ -348,13 +429,12 @@ extern "C" int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int 
   }
   const int num_tiles = p.tiles_m * p.tiles_n;
   const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
-  if (a_fmt == FSB_FP8_E5M2) {
-    if (int rc = ensure_smem<gemm_fp8_kernel<true>>(F8Smem::TOTAL, "gemm_fp8")) return rc;
-    gemm_fp8_kernel<true><<<grid, F8_THREADS, F8Smem::TOTAL, stream>>>(tmA, tmB, tmD, p);
-  } else {
-    if (int rc = ensure_smem<gemm_fp8_kernel<false>>(F8Smem::TOTAL, "gemm_fp8")) return rc;
-    gemm_fp8_kernel<false><<<grid, F8_THREADS, F8Smem::TOTAL, stream>>>(tmA, tmB, tmD, p);
-  }
+  int rc;
+  if (a_fmt == FSB_FP8_E5M2) rc = epi ? launch_gemm_fp8<true, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
+                                      : launch_gemm_fp8<true, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
+  else rc = epi ? launch_gemm_fp8<false, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
+                : launch_gemm_fp8<false, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
+  if (rc) return rc;
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }

@@ -52,7 +52,8 @@ class _HFSurface:
         if not os.path.isdir(path):
             raise FileNotFoundError(f"fsb200 {cls.__name__}.from_pretrained: {path!r} is not a local directory "
                                     "(there is no hub access on the product path)")
-        kw = {k: kwargs[k] for k in ("device", "world_size", "seed") if k in kwargs}
+        # model keywords: fp8 exists on BertForMaskedLM and MegatronBertForPreTraining (fsb200/models/bert.py)
+        kw = {k: kwargs[k] for k in ("device", "world_size", "seed", "fp8") if k in kwargs}
         cfg_cls = _hf_config(cls.config_name)
         if config is not None or state_dict is not None:
             # pretrain_t5.py:34-50: an edited config plus an edited state dict on top of the directory

@@ -16,6 +16,10 @@ and the LayerNorms that add the branch to the residual. Seed, stream counter and
 Packed rows (several samples per row, fsb200/packing.py pack_mlm_batch) pass `segment_ids`: attention is then bidirectional
 inside each segment, the attention-probability dropout included, and never crosses one; MegatronBERT's sentence-order head
 reads each sample's [CLS] row from `cls_positions`.
+fp8=True trains each layer's four projections in FP8 (layers.Fp8Linear, include/fsb200.h fsb_gemm_fp8): e4m3 activations
+and weights, e5m2 gradients, per-tensor power-of-two scales from each tensor's amax just before its cast, fp32 accumulation,
+the biases and the GELU (with its pre-activation copy) in the FP8 GEMM's epilogue. Embeddings, the MLM head, the pooler and
+sentence-order head, the LayerNorms and attention stay bf16, as do the master weights, the gradients and the optimizer state.
 """
 import math
 from collections import namedtuple
@@ -27,7 +31,7 @@ from .. import lib as L
 from .. import ops
 from ..flat import FlatSpec
 from .base import FlatModel, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments, refuse_key_padding
-from .layers import Linear, apply_dropout, residual_norm_bwd
+from .layers import Fp8Linear, Linear, apply_dropout, residual_norm_bwd
 
 _Layer = namedtuple("_Layer", "qkv attn_out inter out")   # attention.self q|k|v, attention.output.dense, intermediate, output
 
@@ -35,8 +39,13 @@ _Layer = namedtuple("_Layer", "qkv attn_out inter out")   # attention.self q|k|v
 class _BertFamily(FlatModel):
     PRE_LN = False
 
-    def __init__(self, config, device=None, world_size=None, seed=0):
+    def __init__(self, config, device=None, world_size=None, seed=0, fp8=False):
+        """fp8: train the layer projections (q|k|v, attention output, intermediate, output) in FP8; see the module
+        docstring. The training and no-grad (validation) forwards both run FP8; results differ from bf16 by design.
+        hidden_size, intermediate_size and the tokens per micro-batch must be multiples of 16 (checked at the first
+        forward)."""
         super().__init__(config)
+        self.fp8 = bool(fp8)
         g = lambda k, d=None: getattr(config, k, d)
         self.h, self.nl, self.nh, self.V = g("hidden_size"), g("num_hidden_layers"), g("num_attention_heads"), g("vocab_size")
         self.ff, self.npos, self.ntype = g("intermediate_size"), g("max_position_embeddings", 512), g("type_vocab_size", 2)
@@ -94,6 +103,8 @@ class _BertFamily(FlatModel):
         self._proj = [_Layer(Linear.span(self.flat, p + "attention.self.query.weight", 3 * h, h, p + "attention.self.query.bias"),
                              lin(p + "attention.output.dense"), lin(p + "intermediate.dense"), lin(p + "output.dense"))
                       for p in (f"bert.encoder.layer.{i}." for i in range(self.nl))]
+        if self.fp8:
+            self._proj = [_Layer(*(Fp8Linear(lp) for lp in pj)) for pj in self._proj]
         self._transform = lin("cls.predictions.transform.dense")
         self._decoder = Linear.of(P(E + "word_embeddings.weight"), P("cls.predictions.bias"))   # tied to the word embeddings
         if pre:
@@ -129,6 +140,10 @@ class _BertFamily(FlatModel):
         rows (required with segment_ids and next_sentence_label; without either, no sentence-order logits are computed).
         segment_ids=None: one sequence per row under attention_mask, as before."""
         B, S = input_ids.shape
+        if self.fp8 and (self.h % 16 or self.ff % 16 or (B * S) % 16):
+            raise ValueError(f"fsb200 {type(self).__name__}(fp8=True): hidden_size ({self.h}), intermediate_size "
+                             f"({self.ff}) and the tokens per micro-batch (batch {B} x sequence {S}) must be multiples of "
+                             "16 (the FP8 GEMM operands need 16-byte rows in both layouts)")
         dev = self.flat.params.device
         c = lambda t: flat_ids(t, dev)
         ids, tt, pos, lab = c(input_ids), c(token_type_ids), c(position_ids), c(labels)
@@ -191,7 +206,9 @@ class _BertFamily(FlatModel):
                 attn_in = h1
             else:
                 attn_in = x
-            qkv = pj.qkv(attn_in)
+            # qs / h2s / fs: what the projection's backward reads of its input (the input itself in bf16, its transposed
+            # e4m3 codes and scale in FP8), kept in place of inputs that nothing else in the backward reads
+            qkv, qs = pj.qkv.forward(attn_in, save)
             q5 = qkv.view(B, S, 3, nh, hn)
             if seg is not None:
                 o, lse = ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, *seg, drop=D(pa, 1 + 3 * i),
@@ -208,18 +225,18 @@ class _BertFamily(FlatModel):
                                                 P(p + "attention.output.LayerNorm.bias").data, self.eps, residual=x,
                                                 drop=D(ph, 2 + 3 * i))
             prea = torch.empty((T, self.ff), dtype=torch.bfloat16, device=x.device) if save else None
-            f = pj.inter(h2, epilogue=self.epi, aux=prea)
-            m = pj.out(f)
+            f, h2s = pj.inter.forward(h2, save, epilogue=self.epi, aux=prea)
+            m, fs = pj.out.forward(f, save)
             if pre:
                 if save:
-                    acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, prea, f))
+                    acts.append((x, st1, qs, qkv, o, lse, x1, st2, h2s, prea, fs))
                 x, prev_m = x1, m
             else:
                 xo, st3, s2 = ops.layernorm_fwd(m, P(p + "output.LayerNorm.weight").data,
                                                 P(p + "output.LayerNorm.bias").data, self.eps, residual=h2,
                                                 drop=D(ph, 3 + 3 * i))
                 if save:
-                    acts.append((x, qkv, o, lse, x1, st2, h2, prea, f, s2, st3))
+                    acts.append((qs, qkv, o, lse, x1, st2, h2s, prea, fs, s2, st3))
                 x = xo
         self._need("head")
         if pre:
@@ -315,25 +332,25 @@ class _BertFamily(FlatModel):
         for i in reversed(range(self.nl)):
             p, pj = f"bert.encoder.layer.{i}.", self._proj[i]
             if pre:
-                x, st1, h1, qkv, o, lse, x1, st2, h2, prea, f = acts[i]
+                x, st1, qs, qkv, o, lse, x1, st2, h2s, prea, fs = acts[i]
                 dm, dres_in = dmb, dx                      # x_next = x1 + drop(m)
             else:
-                x, qkv, o, lse, x1, st2, h2, prea, f, s2, st3 = acts[i]
+                qs, qkv, o, lse, x1, st2, h2s, prea, fs, s2, st3 = acts[i]
                 lw, lb = P(p + "output.LayerNorm.weight"), P(p + "output.LayerNorm.bias")
                 dsum, dm = residual_norm_bwd(dx, s2, lw, lb, st3, D(ph, 3 + 3 * i), acc)   # d(h2 + drop(m)), d(m)
                 dres_in = None
             acts[i] = None
-            df = pj.out.backward(dm, f, acc)
+            df = pj.out.backward(dm, fs, acc)
             dprea = ops.act_bwd_bias(self.act, df, prea, pj.inter.bias_grad, accumulate=acc)   # dGELU + its bias grad
             if pre:
-                dh2 = pj.inter.backward(dprea, h2, acc, colsum=False)
+                dh2 = pj.inter.backward(dprea, h2s, acc, colsum=False)
                 lw, lb = P(p + "ln.weight"), P(p + "ln.bias")
                 dx1, da = residual_norm_bwd(dh2, x1, lw, lb, st2, D(ph, 2 + 3 * i), acc, dres=dres_in)
             else:
-                pj.inter.backward(dprea, h2, acc, dx=dsum, dx_accumulate=True, colsum=False)   # dh2 = d(h2+m) + dgrad(fc1)
+                pj.inter.backward(dprea, h2s, acc, dx=dsum, dx_accumulate=True, colsum=False)   # dh2 = d(h2+m) + dgrad(fc1)
                 lw, lb = P(p + "attention.output.LayerNorm.weight"), P(p + "attention.output.LayerNorm.bias")
                 dsum, da = residual_norm_bwd(dsum, x1, lw, lb, st2, D(ph, 2 + 3 * i), acc)       # d(x + drop(a)), d(a)
-            do = pj.attn_out.backward(da, o.view(T, h), acc)
+            do = pj.attn_out.backward(da, pj.attn_out.saved_input(o.view(T, h)), acc)   # o is kept for attention anyway
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             if seg is not None:
@@ -343,12 +360,12 @@ class _BertFamily(FlatModel):
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, False,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(pa, 1 + 3 * i))
             if pre:
-                dh1 = pj.qkv.backward(dqkv, h1, acc)
+                dh1 = pj.qkv.backward(dqkv, qs, acc)
                 lw, lb = P(p + "attention.ln.weight"), P(p + "attention.ln.bias")
                 # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped FFN output into x
                 dx, dmb = residual_norm_bwd(dh1, x, lw, lb, st1, D(ph, 3 * i) if i > 0 else None, acc, dres=dx1)
             else:
-                dx = pj.qkv.backward(dqkv, x, acc, dx=dsum, dx_accumulate=True)   # dx_in = d(x+a) + dgrad(qkv)
+                dx = pj.qkv.backward(dqkv, qs, acc, dx=dsum, dx_accumulate=True)   # dx_in = d(x+a) + dgrad(qkv)
             self._done(f"layer{i}")
         dx = apply_dropout(dx, D(ph, 0))
         if not pre:

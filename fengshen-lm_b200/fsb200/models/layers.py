@@ -34,9 +34,9 @@ class Linear:
     def __call__(self, x, epilogue=L.EPI_NONE, aux=None):
         return ops.gemm(L.GEMM_NN if self.conv1d else L.GEMM_NT, x, self.weight, bias=self.bias, epilogue=epilogue, aux=aux)
 
-    def forward(self, x, save):
-        """-> (the output, what backward reads of the input: x itself when `save`, else None)."""
-        return self(x), (x if save else None)
+    def forward(self, x, save, epilogue=L.EPI_NONE, aux=None):
+        """-> (the output, what backward reads of the input: x itself when `save`, else None). epilogue / aux as __call__."""
+        return self(x, epilogue, aux), (x if save else None)
 
     def saved_input(self, x):
         """What backward reads of the input x, without the GEMM: what forward(x, save=True) returns second."""
@@ -108,26 +108,34 @@ class GatedMLP:
 
 
 class Fp8Linear:
-    """A Linear (HF layout, no bias) run in FP8 with just-in-time per-tensor scaling, with Linear's call surface. The weight
-    and its gradient stay the bf16 flat-buffer views of `lin`; the weight is cast on every call, so nothing goes stale after
-    an optimizer step.
-      forward: y = x W^T from x e4m3 and W e4m3, both row-major; when saving, x's transposed codes and scale are kept for the
-               weight gradient instead of x.
-      backward: dy e5m2 (both layouts) and W e4m3 (transposed): dx = dy (W^T)^T, dW (+)= dy^T (x^T)^T into the flat gradient.
+    """A Linear (HF layout, with or without a bias) run in FP8 with just-in-time per-tensor scaling, with Linear's call
+    surface. The weight, the bias and their gradients stay the bf16 flat-buffer views of `lin`; the weight is cast on every
+    call, so nothing goes stale after an optimizer step.
+      forward: y = x W^T (+ bias, epilogue, aux as Linear) from x e4m3 and W e4m3, both row-major; when saving, x's transposed
+               codes and scale are kept for the weight gradient instead of x.
+      backward: dy e5m2 (both layouts) and W e4m3 (transposed): dx = dy (W^T)^T, dW (+)= dy^T (x^T)^T into the flat gradient;
+                the bias gradient is the bf16 column sum of dy, as Linear's.
     The token count and both extents of W must be multiples of 16."""
 
     def __init__(self, lin):
-        if lin.conv1d or lin.bias is not None:
-            raise ValueError("fsb200 Fp8Linear: only bias-free [out, in] projections run in FP8")
+        if lin.conv1d:
+            raise ValueError("fsb200 Fp8Linear: only [out, in] projections run in FP8 (a Conv1D weight is [in, out])")
         self.lin = lin
 
-    def __call__(self, x):
-        return self.forward(x, False)[0]
+    @property
+    def bias_grad(self):
+        return self.lin.bias_grad
 
-    def forward(self, x, save):
+    def __call__(self, x, epilogue=L.EPI_NONE, aux=None):
+        return self.forward(x, False, epilogue, aux)[0]
+
+    def forward(self, x, save, epilogue=L.EPI_NONE, aux=None):
         xq, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=save)
         wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
-        return ops.gemm_fp8(xq, sx, wq, sw), ((xt, sx) if save else None)
+        # a bias-free projection without an epilogue (LLaMA's) makes the plain call it made before the epilogue existed
+        epi = {} if self.lin.bias is None and epilogue == L.EPI_NONE and aux is None else \
+            dict(bias=self.lin.bias, epilogue=epilogue, aux=aux)
+        return ops.gemm_fp8(xq, sx, wq, sw, **epi), ((xt, sx) if save else None)
 
     def saved_input(self, x):
         """What backward reads of the input x, without the GEMM: x's transposed e4m3 codes and scale, the bits forward(x,
@@ -135,10 +143,13 @@ class Fp8Linear:
         _, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=False, colwise=True)
         return xt, sx
 
-    def backward(self, dy, saved, accumulate, dx=None, dx_accumulate=False):
+    def backward(self, dy, saved, accumulate, dx=None, dx_accumulate=False, colsum=True):
+        """As Linear.backward, with `saved` what forward / saved_input returned."""
         xt, sx = saved
         dyq, dyt, sdy = ops.fp8_quantize(dy, "e5m2", rowwise=True, colwise=True)
         _, wt, sw = ops.fp8_quantize(self.lin.weight, "e4m3", rowwise=False, colwise=True)
         dx = ops.gemm_fp8(dyq, sdy, wt, sw, out=dx, accumulate=dx_accumulate)
         ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate)
+        if self.lin.bias is not None and colsum:
+            ops.colsum(dy, self.lin.bias_grad, accumulate=accumulate)
         return dx

@@ -146,17 +146,23 @@ int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, 
  *   an asynchronous clear of amax; deterministic (the maximum does not depend on order).
  * fsb_gemm_fp8: D[m, n] = bf16((sum_k A[m, k] B[n, k]) * a_scale_inv * b_scale_inv), the product accumulated in fp32 and
  *   promoted into a separate fp32 accumulator after every 128 k; with `accumulate`, D[m, n] = bf16(that fp32 value + D[m, n])
- *   with one rounding. A uint8 codes [m, k] and B uint8 codes [n, k], both contiguous (K-major), as fsb_fp8_quantize writes y
+ *   with one rounding. The epilogue is fsb_gemm_bf16's, in the same order:
+ *     acc * a_scale_inv * b_scale_inv (+ bias[n]) -> aux = bf16(that value) -> activation -> (+ D_old if accumulate) -> store,
+ *   with one rounding of D. bias: bf16 [n], may be NULL. epilogue: FSB_EPI_NONE / FSB_EPI_GELU_TANH / FSB_EPI_GELU_ERF,
+ *   evaluated with fsb_gemm_bf16's device code (the same fp32 pre-activation gives the same bits). aux: bf16 [m, n] with row
+ *   stride ldaux, may be NULL; receives the pre-activation. A uint8 codes [m, k] and B uint8 codes [n, k], both contiguous (K-major), as fsb_fp8_quantize writes y
  *   or yt; a_scale_inv / b_scale_inv: device fp32 scalars (read by the kernel, so a captured graph stays valid). Format pairs
  *   (a_fmt, b_fmt): (E4M3, E4M3) forward, (E5M2, E4M3) data and weight gradients; any other pair is an error.
- *   D bf16 [m, n], row stride ldd >= n a multiple of 8. Requirements: k % 16 == 0, n % 8 == 0, a / b / d 16-byte aligned;
+ *   D bf16 [m, n], row stride ldd >= n a multiple of 8. Requirements: k % 16 == 0, n % 8 == 0, a / b / d / bias / aux
+ *   16-byte aligned, ldaux >= n a multiple of 8;
  *   any m >= 1; rows of D at or beyond m and columns beyond n are not written. Persistent 128 x 128 tiles on the SMs that
  *   fsb_set_reserved_sms leaves to GEMMs, no K-split: deterministic (the result does not depend on the grid). */
 typedef enum { FSB_FP8_E4M3 = 0, FSB_FP8_E5M2 = 1 } fsb_fp8_format;
 int fsb_fp8_quantize(const void* x, int64_t ldx, int64_t rows, int64_t cols, int fmt, void* y, void* yt, float* scale_inv,
                      float* amax, fsb_stream_t stream);
 int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv, const void* b,
-                 int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, int accumulate, fsb_stream_t stream);
+                 int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, const void* bias, int epilogue, int accumulate,
+                 void* aux, int64_t ldaux, fsb_stream_t stream);
 
 /* ---- RMSNorm / LayerNorm ------------------------------------------------------------------------------------
  * RMSNorm.forward fengshen/models/megatron/layers/norms.py:44-52 (y = scale * cast(x * rsqrt(mean(x^2) + eps)), the cast to
