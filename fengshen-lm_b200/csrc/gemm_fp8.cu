@@ -1,4 +1,5 @@
-// fsb200 — FP8 training GEMM and its quantiser for sm_90a: the layer projections of a LLaMA model built with fp8=True.
+// fsb200 — FP8 training GEMM and its quantiser for sm_90a: the layer projections of a LLaMA, BERT, MegatronBERT or mT5
+// model built with fp8=True.
 // The recipe (include/fsb200.h): activations and weights e4m3, gradients e5m2, one power-of-two scale per tensor computed
 // just in time from the tensor's amax, fp32 accumulation, bf16 outputs.
 //

@@ -129,8 +129,15 @@ class Fp8Linear:
     def __call__(self, x, epilogue=L.EPI_NONE, aux=None):
         return self.forward(x, False, epilogue, aux)[0]
 
-    def forward(self, x, save, epilogue=L.EPI_NONE, aux=None):
-        xq, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=save)
+    @staticmethod
+    def quantize_input(x, save):
+        """x's e4m3 codes as forward makes them: (row-major codes, transposed codes when `save` else None, scale). Projections
+        that read the same x (mT5's cross-attention k|v over the encoder output) quantise it once and pass these as `codes`."""
+        return ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=save)
+
+    def forward(self, x, save, epilogue=L.EPI_NONE, aux=None, codes=None):
+        """codes: quantize_input(x, save), made once for several projections; x is then not read."""
+        xq, xt, sx = self.quantize_input(x, save) if codes is None else codes
         wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
         # a bias-free projection without an epilogue (LLaMA's) makes the plain call it made before the epilogue existed
         epi = {} if self.lin.bias is None and epilogue == L.EPI_NONE and aux is None else \

@@ -29,6 +29,14 @@ Packed rows (several samples per row, fsb200/packing.py pack_seq2seq_batch) pass
 the encoder's self-attention is then bidirectional inside each encoder segment, the decoder's causal inside each decoder
 segment, both with the relative-position bias (it depends on k - q only, so a segment sees the scores it would see alone),
 and each decoder segment's cross-attention reads only the encoder segment with the same id. The dropout sites are unchanged.
+fp8=True trains the layer projections in FP8 (layers.Fp8Linear, include/fsb200.h fsb_gemm_fp8): the encoder's q|k|v, o,
+wi_0|wi_1 and wo, and the decoder's q|k|v, o, cross q, cross k|v, cross o, wi_0|wi_1 and wo. e4m3 activations and weights, e5m2
+gradients, per-tensor power-of-two scales from each tensor's amax just before its cast, fp32 accumulation. The encoder output,
+which every decoder layer's cross k|v projection reads, is quantised once per forward and its codes shared; those projections'
+data gradients (bf16, the FP8 GEMM's output) are summed in fp32 (ops.accumulate), as the bf16 GEMM sums them in bf16
+training. The shared embedding, the LM head, the RMSNorms, the relative-bias attention and its bias gradient, the gated-GeLU
+kernel and the loss stay bf16, as do the master weights, the gradients and the optimizer state; `generate` runs the bf16
+projections.
 """
 import math
 from collections import namedtuple
@@ -43,7 +51,7 @@ from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from . import t5_bias as TB
 from .base import FlatModel, _Holder, cross_segment_bounds, flat_ids, key_mask, refuse_key_padding
-from .layers import GatedMLP, Linear, apply_dropout, residual_norm_bwd
+from .layers import Fp8Linear, GatedMLP, Linear, apply_dropout, residual_norm_bwd
 
 _Enc = namedtuple("_Enc", "qkv o mlp")             # a layer's projections: self-attention q|k|v and o, the gated FFN
 _Dec = namedtuple("_Dec", "qkv o cq ckv co mlp")   # ... and between them cross-attention q, k|v and o
@@ -64,8 +72,12 @@ def shift_right(labels, start_id, pad_id, seg_start=None):
 
 
 class MT5ForConditionalGeneration(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0):
+    def __init__(self, config, device=None, world_size=None, seed=0, fp8=False):
+        """fp8: train the layer projections in FP8; see the module docstring. The training and no-grad (validation) forwards
+        both run FP8; results differ from bf16 by design. d_model, d_ff and the tokens per micro-batch on both sides
+        (batch x source length, batch x target length) must be multiples of 16 (checked at the first forward)."""
         super().__init__(config)
+        self.fp8 = bool(fp8)
         g = lambda k, d=None: getattr(config, k, d)
         self.d, self.dk, self.nh, self.ff = g("d_model"), g("d_kv"), g("num_heads"), g("d_ff")
         self.ne = g("num_layers")
@@ -139,6 +151,11 @@ class MT5ForConditionalGeneration(FlatModel):
         self._dec = [_Dec(span(p + "0.SelfAttention.q", 3 * inner), lin(p + "0.SelfAttention.o"), lin(p + "1.EncDecAttention.q"),
                           span(p + "1.EncDecAttention.k", 2 * inner), lin(p + "1.EncDecAttention.o"), mlp(p + "2."))
                      for p in (f"decoder.block.{i}.layer." for i in range(self.nd))]
+        self._enc_bf16, self._dec_bf16 = self._enc, self._dec   # what generate runs
+        if self.fp8:
+            f8 = lambda pj: type(pj)(*(GatedMLP(Fp8Linear(q.wi), Fp8Linear(q.wo), q.act) if isinstance(q, GatedMLP)
+                                       else Fp8Linear(q) for q in pj))
+            self._enc, self._dec = [f8(pj) for pj in self._enc], [f8(pj) for pj in self._dec]
 
         self.reset_parameters(seed)
         # dropout sites of one forward. Encoder: 0 embeddings; layer i: 1 + 4i attention probabilities, 2 + 4i attention output,
@@ -202,6 +219,15 @@ class MT5ForConditionalGeneration(FlatModel):
             decoder_input_ids = shift_right(labels.to(device=dev, dtype=torch.int64), self.start_id, self.pad_id,
                                             packed[0][1][0] if packed else None)
         Sd = decoder_input_ids.shape[1]
+        if self.fp8:
+            bad = [f"{name} ({v})" for name, v in (("d_model", self.d), ("d_ff", self.ff),
+                                                    (f"batch {B} x source length {Se}", B * Se),
+                                                    (f"batch {B} x target length {Sd}", B * Sd)) if v % 16]
+            if bad:
+                raise ValueError(f"fsb200 MT5ForConditionalGeneration(fp8=True): {', '.join(bad)} not a multiple of 16 (the "
+                                 "FP8 GEMM operands need 16-byte rows in both layouts; d_model, d_ff and the tokens per "
+                                 "micro-batch on both sides must be). With the span-corruption collator's target length "
+                                 "of 114, the micro-batch must be a multiple of 8")
         ids, dec_ids, lab = flat_ids(input_ids, dev), flat_ids(decoder_input_ids, dev), flat_ids(labels, dev)
         mask = None if packed else key_mask(attention_mask, dev)
         loss, logits = self._step_or_forward(lab is not None, return_logits, ids, dec_ids, mask, lab, B, Se, Sd, *packed)
@@ -229,21 +255,22 @@ class MT5ForConditionalGeneration(FlatModel):
             return ops.rmsnorm_fwd(x, self.P(name).data, self.eps)
         return ops.rmsnorm_fwd(prev, self.P(name).data, self.eps, residual=x, drop=drop)
 
-    def _encode(self, ids, mask, B, Se, rel_e, save, base=None, seg=None):
+    def _encode(self, ids, mask, B, Se, rel_e, save, base=None, seg=None, proj=None):
         """Encoder stack over ids [B * Se]; returns (saved activations, final hidden states (after their dropout), their rstd,
         residual stream). base: the forward's dropout stream base (None: no dropout). seg: the (seg_start, seg_end) bounds of
-        packed rows (mask is then None)."""
+        packed rows (mask is then None). proj: the layers' projections (default self._enc)."""
         nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         Te = B * Se
         D = lambda site: self._drop(base, self.p_drop, site)
         x, prev = apply_dropout(ops.embedding_fwd(ids, P("shared.weight").data), D(0)), None
         eacts = []
-        for i, pj in enumerate(self._enc):
+        for i, pj in enumerate(self._enc if proj is None else proj):
             p = f"encoder.block.{i}.layer."
             self._need(f"enc{i}")
             h1, r1, x = self._norm(prev, x, p + "0.layer_norm.weight", D(4 * i))   # layer i-1's FFN output
-            qkv = pj.qkv(h1)
+            # qs: what q|k|v's backward reads of h1 (h1 itself in bf16, its transposed e4m3 codes and scale in FP8)
+            qkv, qs = pj.qkv.forward(h1, save)
             q5 = qkv.view(B, Se, 3, nh, dk)
             if seg is None:
                 o, lse = ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, False, kv_mask=mask, rel_bias=rel_e,
@@ -253,20 +280,21 @@ class MT5ForConditionalGeneration(FlatModel):
                                                causal=False, rel_bias=rel_e)
             a = pj.o(o.view(Te, inner))
             h2, r2, x1 = self._norm(a, x, p + "1.layer_norm.weight", D(2 + 4 * i))
-            m, ms = pj.mlp(h2, drop=D(3 + 4 * i))
+            m, ms = pj.mlp(h2, save, drop=D(3 + 4 * i))
             if save:
-                eacts.append((x, r1, h1, qkv, o, lse, x1, r2, h2, ms))
+                eacts.append((x, r1, qs, qkv, o, lse, x1, r2, ms))
             x, prev = x1, m
         self._need("head")
         enc_h, rfe, xfe = self._norm(prev, x, "encoder.final_layer_norm.weight", D(4 * self.ne))
         return eacts, apply_dropout(enc_h, D(1 + 4 * self.ne)), rfe, xfe
 
-    def _decode(self, dec_ids, B, S, attend, cross_attend, acts=None, base=None):
+    def _decode(self, dec_ids, B, S, attend, cross_attend, acts=None, base=None, proj=None):
         """Decoder stack over dec_ids [B * S] -> (final hidden states (after their dropout), their rstd, residual stream).
         attend(i, q5) is layer i's self-attention over the packed q|k|v view [B, S, 3, heads, d_kv] -> (out, lse);
         cross_attend(i, qc) its cross-attention from the query projection [B * S, inner] -> (out, lse, the encoder's K|V or
         None); `acts`, when given, collects what the backward reads. base: the forward's dropout stream base (None: no
-        dropout); the attention callbacks draw their own probability masks."""
+        dropout); the attention callbacks draw their own probability masks. proj: the layers' projections (default
+        self._dec)."""
         nh, dk, inner = self.nh, self.dk, self.inner
         P = self.P
         T = B * S
@@ -274,21 +302,22 @@ class MT5ForConditionalGeneration(FlatModel):
         D = lambda site: self._drop(base, self.p_drop, site)
         self._need("no_decay"); self._need("shared")
         y, prev = apply_dropout(ops.embedding_fwd(dec_ids, P("shared.weight").data), D(E)), None
-        for i, pj in enumerate(self._dec):
+        save = acts is not None
+        for i, pj in enumerate(self._dec if proj is None else proj):
             p = f"decoder.block.{i}.layer."
             self._need(f"dec{i}")
             h1, r1, y = self._norm(prev, y, p + "0.layer_norm.weight", D(E + 6 * i))   # layer i-1's FFN output
-            qkv = pj.qkv(h1)
+            qkv, qs = pj.qkv.forward(h1, save)
             o, lse = attend(i, qkv.view(B, S, 3, nh, dk))
             a = pj.o(o.view(T, inner))
             h2, r2, y1 = self._norm(a, y, p + "1.layer_norm.weight", D(E + 2 + 6 * i))
-            qc = pj.cq(h2)
+            qc, h2s = pj.cq.forward(h2, save)
             oc, lsec, kvc = cross_attend(i, qc)
             ac = pj.co(oc.view(T, inner))
             h3, r3, y2 = self._norm(ac, y1, p + "2.layer_norm.weight", D(E + 4 + 6 * i))
-            m, ms = pj.mlp(h3, drop=D(E + 5 + 6 * i))
-            if acts is not None:
-                acts.append((y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms))
+            m, ms = pj.mlp(h3, save, drop=D(E + 5 + 6 * i))
+            if save:
+                acts.append((y, r1, qs, qkv, o, lse, y1, r2, h2s, qc, kvc, oc, lsec, y2, r3, ms))
             y, prev = y2, m
         self._need("head")
         hf, rfd, xfd = self._norm(prev, y, "decoder.final_layer_norm.weight", D(E + 6 * self.nd))
@@ -319,12 +348,12 @@ class MT5ForConditionalGeneration(FlatModel):
         self._need("no_decay"); self._need("shared")
         rel_e = TB.rel_bias_vector(P("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight").data, Se, Se, True,
                                    self.nbuckets, self.maxdist)
-        _, enc_h, _, _ = self._encode(ids.view(-1), emask, B, Se, rel_e, False)
+        _, enc_h, _, _ = self._encode(ids.view(-1), emask, B, Se, rel_e, False, proj=self._enc_bf16)   # fp8=True: bf16
         R = B * c.expand
         cross = []
         for i in range(self.nd):
             self._need(f"dec{i}")
-            kvc = self._dec[i].ckv(enc_h).view(B, Se, 2, nh, dk)
+            kvc = self._dec_bf16[i].ckv(enc_h).view(B, Se, 2, nh, dk)
             cross.append(kvc.repeat_interleave(c.expand, 0) if c.expand > 1 else kvc)
         cmask = None if emask is None else emask.repeat_interleave(c.expand, 0).contiguous()
         cap = (max(c.max_length, 2) + 63) // 64 * 64
@@ -349,7 +378,7 @@ class MT5ForConditionalGeneration(FlatModel):
                 kv = b[i]
                 ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len)
                 return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, 1.0, rel_bias=rel_d)
-            hf, _, _ = self._decode(tok, R, 1, attend, cross_attend)
+            hf, _, _ = self._decode(tok, R, 1, attend, cross_attend, proj=self._dec_bf16)
             return self._head(hf).float()
 
         graphs = DecodeGraphs(self, R, caches, body)
@@ -371,6 +400,10 @@ class MT5ForConditionalGeneration(FlatModel):
         D = lambda site: self._drop(base, self.p_drop, site)
         enc_seg, dec_seg, cross = (None, None, None) if segs is None else segs
         eacts, enc_h, rfe, xfe = self._encode(ids, mask, B, Se, rel_e, save, base, enc_seg)
+        # every decoder layer's cross k|v projection reads enc_h: under fp8 its codes are made once and shared, and what the
+        # backward reads of it (enc_s) is kept once
+        enc_codes = self._dec[0].ckv.quantize_input(enc_h, save) if self.fp8 and self.nd else None
+        enc_s = enc_h if enc_codes is None else enc_codes[1:]
 
         def attend(i, q5):
             if dec_seg is not None:
@@ -379,7 +412,8 @@ class MT5ForConditionalGeneration(FlatModel):
             return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], 1.0, True, rel_bias=rel_d, drop=D(E + 1 + 6 * i))
 
         def cross_attend(i, qc):
-            kvc = self._dec[i].ckv(enc_h)
+            ckv = self._dec[i].ckv
+            kvc = ckv(enc_h) if enc_codes is None else ckv.forward(enc_h, False, codes=enc_codes)[0]
             kv5 = kvc.view(B, Se, 2, nh, dk)
             if cross is not None:
                 oc, lsec = ops.sdpa_segments_fwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], 1.0, *cross[0],
@@ -397,14 +431,14 @@ class MT5ForConditionalGeneration(FlatModel):
             loss, dlogits, _ = ops.softmax_xent(logits, lab, Sd, shift=0, grad_scale=self.loss_scale,
                                                 dlogits="inplace" if save else None)
             if save:
-                ctx = (eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base,
+                ctx = (eacts, dacts, enc_s, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base,
                        segs)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
 
     # ---- backward ---------------------------------------------------------------------------------------------------
     def _backward_impl(self, ctx, gloss):
-        eacts, dacts, enc_h, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base, segs = ctx
+        eacts, dacts, enc_s, rfe, xfe, hf, rfd, xfd, dlogits, ids, dec_ids, mask, rel_e, rel_d, B, Se, Sd, base, segs = ctx
         enc_seg, dec_seg, cross = (None, None, None) if segs is None else segs
         d, nh, dk, inner = self.d, self.nh, self.dk, self.inner
         P = self.P
@@ -427,12 +461,12 @@ class MT5ForConditionalGeneration(FlatModel):
         denc32 = torch.empty((Te, d), dtype=torch.float32, device=dev)   # sum over decoder layers of the K|V dgrads
         for i in reversed(range(self.nd)):
             p, pj = f"decoder.block.{i}.layer.", self._dec[i]
-            y, r1, h1, qkv, o, lse, y1, r2, h2, qc, kvc, oc, lsec, y2, r3, h3, ms = dacts[i]
+            y, r1, qs, qkv, o, lse, y1, r2, h2s, qc, kvc, oc, lsec, y2, r3, ms = dacts[i]
             dacts[i] = None
             dh3 = pj.mlp.backward(dm, ms, acc, drop=D(E + 5 + 6 * i))
             dy2, dac = residual_norm_bwd(dh3, y2, P(p + "2.layer_norm.weight"), None, r3, D(E + 4 + 6 * i), acc, dres=dy)
             # cross-attention
-            doc = pj.co.backward(dac, oc.view(Td, inner), acc)
+            doc = pj.co.backward(dac, pj.co.saved_input(oc.view(Td, inner)), acc)   # oc is kept for attention anyway
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             kv5, dkv5 = kvc.view(B, Se, 2, nh, dk), dkvc.view(B, Se, 2, nh, dk)
@@ -444,11 +478,14 @@ class MT5ForConditionalGeneration(FlatModel):
                 ops.sdpa_bwd(qc.view(B, Sd, nh, dk), kv5[:, :, 0], kv5[:, :, 1], oc, doc.view(B, Sd, nh, dk), lsec, 1.0,
                              False, dqc.view(B, Sd, nh, dk), dkv5[:, :, 0], dkv5[:, :, 1], kv_mask=mask,
                              drop=D(E + 3 + 6 * i))
-            dh2 = pj.cq.backward(dqc, h2, acc)
-            pj.ckv.backward(dkvc, enc_h, acc, dx=denc32, dx_accumulate=(i != self.nd - 1))
+            dh2 = pj.cq.backward(dqc, h2s, acc)
+            if self.fp8:   # the FP8 GEMM writes bf16: each layer's dgrad is rounded once, their sum is kept in fp32
+                ops.accumulate(denc32, pj.ckv.backward(dkvc, enc_s, acc), overwrite=(i == self.nd - 1))
+            else:
+                pj.ckv.backward(dkvc, enc_s, acc, dx=denc32, dx_accumulate=(i != self.nd - 1))
             dy1, da = residual_norm_bwd(dh2, y1, P(p + "1.layer_norm.weight"), None, r2, D(E + 2 + 6 * i), acc, dres=dy2)
             # causal self-attention with the decoder's relative-position bias
-            do = pj.o.backward(da, o.view(Td, inner), acc)
+            do = pj.o.backward(da, pj.o.saved_input(o.view(Td, inner)), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Sd, 3, nh, dk), dqkv.view(B, Sd, 3, nh, dk)
             if dec_seg is not None:
@@ -458,7 +495,7 @@ class MT5ForConditionalGeneration(FlatModel):
             else:
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Sd, nh, dk), lse, 1.0, True,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], rel_bias=rel_d, drel_bias=drel_d, drop=D(E + 1 + 6 * i))
-            dh1 = pj.qkv.backward(dqkv, h1, acc)
+            dh1 = pj.qkv.backward(dqkv, qs, acc)
             # layer 0's norm had no residual (y = the embeddings); layer i's summed layer i-1's dropped FFN output into y
             dy, dm = residual_norm_bwd(dh1, y, P(p + "0.layer_norm.weight"), None, r1, D(E + 6 * i) if i > 0 else None, acc,
                                        dres=dy1)
@@ -476,11 +513,11 @@ class MT5ForConditionalGeneration(FlatModel):
                                    rfe, D(4 * self.ne), acc)
         for i in reversed(range(self.ne)):
             p, pj = f"encoder.block.{i}.layer.", self._enc[i]
-            x, r1, h1, qkv, o, lse, x1, r2, h2, ms = eacts[i]
+            x, r1, qs, qkv, o, lse, x1, r2, ms = eacts[i]
             eacts[i] = None
             dh2 = pj.mlp.backward(dm, ms, acc, drop=D(3 + 4 * i))
             dx1, da = residual_norm_bwd(dh2, x1, P(p + "1.layer_norm.weight"), None, r2, D(2 + 4 * i), acc, dres=dx)
-            do = pj.o.backward(da, o.view(Te, inner), acc)
+            do = pj.o.backward(da, pj.o.saved_input(o.view(Te, inner)), acc)
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, Se, 3, nh, dk), dqkv.view(B, Se, 3, nh, dk)
             if enc_seg is not None:
@@ -491,7 +528,7 @@ class MT5ForConditionalGeneration(FlatModel):
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, Se, nh, dk), lse, 1.0, False,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, rel_bias=rel_e, drel_bias=drel_e,
                              drop=D(1 + 4 * i))
-            dh1 = pj.qkv.backward(dqkv, h1, acc)
+            dh1 = pj.qkv.backward(dqkv, qs, acc)
             dx, dm = residual_norm_bwd(dh1, x, P(p + "0.layer_norm.weight"), None, r1, D(4 * i) if i > 0 else None, acc,
                                        dres=dx1)
             if i == 0:

@@ -130,7 +130,7 @@ size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
                    void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
-/* ---- FP8 training GEMM (opt-in LLaMA precision, `fp8=True`) -------------------------------------------------------
+/* ---- FP8 training GEMM (opt-in `fp8=True`: LLaMA, BERT, MegatronBERT, mT5) ------------------------------------------
  * The "hybrid" recipe with just-in-time ("current") per-tensor scaling: activations and weights are e4m3 (largest finite
  * value 448), gradients e5m2 (57344); accumulation is fp32, outputs bf16.
  *

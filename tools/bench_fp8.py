@@ -22,7 +22,14 @@
 2. The C3-width step (24 layers, 32 heads, vocabulary 21248, seq 512, micro-batch 32, MLM + sentence order) at dropout 0
    and 0.1, fp8 and bf16 alternated as above.
 
-  python tools/bench_fp8.py [--model llama|megatronbert] [--reps 3] [--steps 6] [--warmup 2] [--skip-kernels]
+--model t5 measures Randeng-T5-784M (C5) width instead:
+1. Kernels at C5 width (d_model 1024, d_ff 2816, 16 heads of 64) with 32 x 512 = 16384 token rows on either side, for each
+   distinct projection shape (self q|k|v, the attention output projections, cross q, cross k|v, wi_0|wi_1, wo) in the same
+   three roles. mT5's projections have no bias and no epilogue. The quantiser rows as above.
+2. A C5-width step at reduced depth (12 encoder and 12 decoder layers, vocabulary 32600, encoder and decoder length 512,
+   micro-batch 32, span-corruption-shaped labels) at dropout 0 and 0.1, fp8 and bf16 alternated as above.
+
+  python tools/bench_fp8.py [--model llama|megatronbert|t5] [--reps 3] [--steps 6] [--warmup 2] [--skip-kernels]
                             [--skip-step] [--out DIR]
 
 Prints one JSON line per measurement, the card's name, power limit and max SM clock first; --out also writes them to
@@ -49,6 +56,7 @@ from fsb200 import ops  # noqa: E402
 from fsb200.engine import ZeroEngine  # noqa: E402
 from fsb200.models.bert import MegatronBertForPreTraining  # noqa: E402
 from fsb200.models.llama import LlamaForCausalLM  # noqa: E402
+from fsb200.models.t5 import MT5ForConditionalGeneration  # noqa: E402
 
 H, FF, T = 5120, 13824, 8192
 PROJ = (("qkv", 3 * H, H), ("dense", H, H), ("w1w3", 2 * FF, H), ("w2", H, FF))
@@ -56,6 +64,12 @@ C3_H, C3_FF, C3_T = 2048, 8192, 32 * 512
 # (name, out, in, forward epilogue, forward writes aux): every C3 projection has a bias
 C3_PROJ = (("qkv", 3 * C3_H, C3_H, L.EPI_NONE, False), ("attn_out", C3_H, C3_H, L.EPI_NONE, False),
            ("inter", C3_FF, C3_H, L.EPI_GELU_ERF, True), ("out", C3_H, C3_FF, L.EPI_NONE, False))
+C5_D, C5_FF, C5_INNER, C5_T = 1024, 2816, 16 * 64, 32 * 512
+# (name, out, in, forward epilogue, forward writes aux): the distinct C5 projection shapes; o stands for the encoder's and the
+# decoder's self- and cross-attention output projections, cq for the cross-attention query
+C5_PROJ = (("qkv", 3 * C5_INNER, C5_D, L.EPI_NONE, False), ("o", C5_D, C5_INNER, L.EPI_NONE, False),
+           ("cq", C5_INNER, C5_D, L.EPI_NONE, False), ("ckv", 2 * C5_INNER, C5_D, L.EPI_NONE, False),
+           ("wi", 2 * C5_FF, C5_D, L.EPI_NONE, False), ("wo", C5_D, C5_FF, L.EPI_NONE, False))
 HBM, PEAK_FP8, PEAK_BF16 = 3.35e12, 1979e12, 989e12
 
 
@@ -143,6 +157,22 @@ def _megatronbert(fp8, dropout):
     return MegatronBertForPreTraining(cfg, device="cuda", fp8=fp8), batch, dict(layers=nl, batch=B, seq=S)
 
 
+def _t5(fp8, dropout):
+    """C5 width: Randeng-T5-784M's config at 12 + 12 layers (of its 24 + 24), encoder and decoder length 512, micro-batch
+    32; the last 3 decoder positions of every row unlabelled, as hf_oracle.make_t5_batch does."""
+    nl, V, B, S = 12, 32600, 32, 512
+    cfg = SimpleNamespace(vocab_size=V, d_model=C5_D, d_kv=64, d_ff=C5_FF, num_layers=nl, num_decoder_layers=nl,
+                          num_heads=16, relative_attention_num_buckets=32, relative_attention_max_distance=128,
+                          dropout_rate=dropout, feed_forward_proj="gated-gelu", tie_word_embeddings=True,
+                          layer_norm_epsilon=1e-6, pad_token_id=0, decoder_start_token_id=0)
+    g = torch.Generator(device="cuda").manual_seed(1)
+    ids = torch.randint(2, V, (B, S), device="cuda", generator=g)
+    labels = torch.randint(2, V, (B, S), device="cuda", generator=g)
+    labels[:, -3:] = -100
+    return MT5ForConditionalGeneration(cfg, device="cuda", fp8=fp8), dict(input_ids=ids, labels=labels), \
+        dict(layers=nl, batch=B, seq=S)
+
+
 def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
     gc.collect()
     torch.cuda.empty_cache()
@@ -168,7 +198,7 @@ def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
         losses.append(one().detach())
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
-    extra = dict(model="megatronbert", dropout=dropout) if build is _megatronbert else {}
+    extra = {_megatronbert: dict(model="megatronbert", dropout=dropout), _t5: dict(model="t5", dropout=dropout)}.get(build, {})
     rec = dict(kind="step", **extra, fp8=fp8, **shape, steps=steps,
                tokens_per_s=round(B * S * steps / dt),
                step_ms=round(1e3 * dt / steps, 1), peak_alloc_gib=round(torch.cuda.max_memory_allocated() / 2 ** 30, 2),
@@ -189,7 +219,7 @@ def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=("llama", "megatronbert"), default="llama")
+    ap.add_argument("--model", choices=("llama", "megatronbert", "t5"), default="llama")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--steps", type=int, default=6)
     ap.add_argument("--warmup", type=int, default=2)
@@ -201,17 +231,20 @@ def main():
         raise SystemExit("bench_fp8: needs a CUDA device")
     sink = []
     emit(dict(kind="card", **card()), sink)
-    bert = a.model == "megatronbert"
+    bert, t5 = a.model == "megatronbert", a.model == "t5"
     if not a.skip_kernels:
         if bert:
             kernels(a.reps, sink, C3_PROJ, C3_T, bias=True)
+        elif t5:
+            kernels(a.reps, sink, C5_PROJ, C5_T)
         else:
             kernels(a.reps, sink)
     if not a.skip_step:
-        for dropout in ((0.0, 0.1) if bert else (0.0,)):
+        build = _megatronbert if bert else _t5 if t5 else _llama
+        for dropout in ((0.0, 0.1) if bert or t5 else (0.0,)):
             for r in range(a.reps):
                 for fp8 in ((True, False) if r % 2 == 0 else (False, True)):
-                    step(fp8, a.steps, a.warmup, sink, _megatronbert if bert else _llama, dropout)
+                    step(fp8, a.steps, a.warmup, sink, build, dropout)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "bench_fp8.jsonl"), "w") as f:
