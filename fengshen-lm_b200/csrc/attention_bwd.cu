@@ -239,12 +239,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const int c0 = j * AB_BN;
     uint32_t dw[kDropout ? AB_BN / 16 : 1][2];   // the forward's keep bits, regenerated while the tensor cores work
     if constexpr (kDropout) attn_drop_rows<AB_BN / 16>(dkey, uint32_t(b * p.nheads + head), q0 + r_lo, c0, lane, dw);
+    // key-mask bit 2 i + c: column c0 + 8 i + cq + c, fetched while the tensor cores compute S and dP
+    const uint32_t kbits = mrow != nullptr ? key_mask_bits<AB_BN / 8>(mrow, c0 + cq, p.seq_kv - 1) : ~0u;
     wgmma_wait<0>();
     wgmma_fence_acc(s);
     wgmma_fence_acc(dp);
-    bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
-                     (kSeg && c0 < max(kmin[0], kmin[1]));
-    if constexpr (kEnd) need_mask = need_mask || c0 + AB_BN - 1 > min(kmax[0], kmax[1]);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
 #pragma unroll
@@ -252,16 +251,33 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const int h = e >> 1, col = c0 + 8 * i + cq + (e & 1);
         float x = s[4 * i + e] * p.scale_log2 - lse[h];
         if constexpr (kBias) x = fmaf(__ldg(brow[h] + min(col, p.seq_kv - 1)), 1.4426950408889634f, x);
-        float pe = ex2_approx(x);
-        if (need_mask) {
-          bool keep = col <= kmax[h];
-          if constexpr (kSeg) keep = keep && col >= kmin[h];
-          if (mrow != nullptr && keep) keep = mrow[col] != 0;
-          pe = keep ? pe : 0.f;
+        s[4 * i + e] = ex2_approx(x);   // P
+      }
+    }
+    // one warp-uniform branch per step around straight-line selects, as in attn_fwd_kernel (masked P = 0)
+    bool need_mask = (p.causal && c0 + AB_BN - 1 > q0 + wg * 64) || (c0 + AB_BN > p.seq_kv) || mrow ||
+                     (kSeg && c0 < max(kmin[0], kmin[1]));
+    if constexpr (kEnd) need_mask = need_mask || c0 + AB_BN - 1 > min(kmax[0], kmax[1]);
+    if (__any_sync(0xffffffffu, need_mask)) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int h = e >> 1, col = c0 + 8 * i + cq + (e & 1);
+          bool keep = (col <= kmax[h]) & bool((kbits >> (2 * i + (e & 1))) & 1u);
+          if constexpr (kSeg) keep = keep & (col >= kmin[h]);
+          s[4 * i + e] = keep ? s[4 * i + e] : 0.f;
         }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int h = e >> 1;
         float dpe = dp[4 * i + e];
         if constexpr (kDropout) dpe = drop_keep(dw[i >> 1][e & 1], 2 * h + (i & 1), dkey.thr) ? dpe * p.drop.keep_scale : 0.f;
-        s[4 * i + e] = pe * (dpe - delta[h]);   // dS
+        s[4 * i + e] *= dpe - delta[h];   // dS = P (dP - delta)
       }
     }
     if constexpr (kBias) {

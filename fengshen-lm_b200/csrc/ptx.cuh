@@ -372,4 +372,18 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
   return v;
 }
 
+// Key-padding mask of one thread's columns of an attention score fragment: bit 2 i + c = (row[col0 + 8 i + c] != 0),
+// i < NG. Every byte is loaded unconditionally, its index clamped to `last`, so the loads issue back to back and can be
+// placed before the wait on the MMA that produces the scores; a clamped column lies past the row's last key and is masked
+// by its bound anyway.
+template <int NG>
+__device__ __forceinline__ uint32_t key_mask_bits(const uint8_t* row, int col0, int last) {
+  uint32_t bits = 0;
+#pragma unroll
+  for (int i = 0; i < NG; ++i)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) bits |= uint32_t(__ldg(row + min(col0 + 8 * i + c, last)) != 0) << (2 * i + c);
+  return bits;
+}
+
 }  // namespace fsb
