@@ -64,8 +64,11 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
                                                          int64_t o_row_stride, int64_t o_head_stride,
                                                          int64_t do_row_stride, int64_t do_head_stride, int batch, int seq,
                                                          int nheads) {
-  // one group of D/8 threads per (b, s, h)
-  constexpr int G = D / 8;
+  // one group of G threads per (b, s, h), each reading NV 8-element vectors (lane gl: vectors gl, gl + G, ...): G = D/8 and
+  // NV = 1 for D 64 / 128; D 96 takes G = 4 and NV = 3, so that a group never straddles a warp
+  constexpr int G = D == 96 ? 4 : D / 8;
+  constexpr int NV = D / (8 * G);
+  static_assert(32 % G == 0 && NV * 8 * G == D, "delta groups must tile a warp and the head");
   const int64_t gid = (blockIdx.x * int64_t(blockDim.x) + threadIdx.x) / G;
   const int gl = threadIdx.x % G;
   const int64_t total = int64_t(batch) * seq * nheads;
@@ -74,11 +77,14 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
   if (gid < total) {
     h = int(gid % nheads);
     bs = gid / nheads;
-    float a[8], b[8];
-    unpack8(*reinterpret_cast<const uint4*>(o + bs * o_row_stride + h * o_head_stride + gl * 8), a);
-    unpack8(*reinterpret_cast<const uint4*>(dout + bs * do_row_stride + h * do_head_stride + gl * 8), b);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s += a[j] * b[j];
+    for (int t = 0; t < NV; ++t) {
+      float a[8], b[8];
+      unpack8(*reinterpret_cast<const uint4*>(o + bs * o_row_stride + h * o_head_stride + (gl + t * G) * 8), a);
+      unpack8(*reinterpret_cast<const uint4*>(dout + bs * do_row_stride + h * do_head_stride + (gl + t * G) * 8), b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += a[j] * b[j];
+    }
   }
 #pragma unroll
   for (int off = G / 2; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
@@ -89,10 +95,12 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 }
 
 // ------------------------------------------------------------------------------------------------ shared layout
+// D = 96 stages whole 64-column panels as D = 128 does (DS = 128, the second panel half used); see attn_bwd_dq_kernel.
 template <int D, bool kDS>
 struct AttBwdSmem {
-  static constexpr int BIG_BYTES = AB_BM * D * 2;    // a resident 128-row tile
-  static constexpr int SML_BYTES = AB_BN * D * 2;    // a streamed 64-row tile
+  static constexpr int DS = (D + 63) / 64 * 64;      // staged columns
+  static constexpr int BIG_BYTES = AB_BM * DS * 2;   // a resident 128-row tile
+  static constexpr int SML_BYTES = AB_BN * DS * 2;   // a streamed 64-row tile
   static constexpr int STAGES = 3;                   // streamed-tile ring depth
   static constexpr int OFF_BIG0 = 0;                       // dQ: Q     | dKV: K
   static constexpr int OFF_BIG1 = OFF_BIG0 + BIG_BYTES;    // dQ: dO    | dKV: V
@@ -126,12 +134,15 @@ __device__ __forceinline__ void to_frag(const float (&x)[32], int kk, uint32_t (
 // kSeg == kSegCross: as kSegBidir over kv_start / kv_end, with the steps clamped into the key sequence only; a tile whose
 // queries see no key visits no step and writes dQ = 0. kBias composes with kSegCausal and kSegBidir; the steps the bounds
 // skip write no bias-gradient slot, and the reduction reads only the slots of dq_step_range.
+// D = 96: S and dP contract over exactly 6 k16 steps; dQ += dS K runs at N = 128 over the staged K panels (a dQ column
+// depends on the same K column only) and stores 96 columns. The dK / dV kernel does the same for S^T, dP^T, dV and dK.
 template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                    const AttBwdParams p) {
   using S = AttBwdSmem<D, kBias>;
+  constexpr int DS = S::DS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   uint64_t* big_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
@@ -167,7 +178,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       const int kc = head * p.k_head_stride, vc = head * p.v_head_stride;
       mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
 #pragma unroll
-      for (int h = 0; h < D / 64; ++h) {
+      for (int h = 0; h < DS / 64; ++h) {
         tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmQ, big_full, qc + h * 64, q0, b);
         tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmdO, big_full, dc + h * 64, q0, b);
       }
@@ -176,7 +187,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         ring.acquire();
         uint64_t* bar = ring.expect(2 * S::SML_BYTES);
 #pragma unroll
-        for (int h = 0; h < D / 64; ++h) {
+        for (int h = 0; h < DS / 64; ++h) {
           tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmK, bar, kc + h * 64, j * AB_BN, b);
           tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmV, bar, vc + h * 64, j * AB_BN, b);
         }
@@ -216,9 +227,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
   float* dpart = kBias && p.dbias_part ? p.dbias_part + ((int64_t(b) * p.nheads + head) * gridDim.x + tile) * n_all * AB_DSTRIDE
                                        : nullptr;
-  float dq[D / 2];
+  float dq[DS / 2];
 #pragma unroll
-  for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
+  for (int i = 0; i < DS / 2; ++i) dq[i] = 0.f;
   DropKey dkey;
   if constexpr (kDropout) dkey = drop_key(p.drop);
 
@@ -306,7 +317,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int kk = 0; kk < AB_BN / 16; ++kk) to_frag(s, kk, a[kk]);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dq, a[kk], dsc_kmn + sto + ((kk * 2048) >> 4), 1u);
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<DS, 1>(dq, a[kk], dsc_kmn + sto + ((kk * 2048) >> 4), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(dq);
@@ -340,6 +351,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                     const AttBwdParams p) {
   using S = AttBwdSmem<D, false>;
+  constexpr int DS = S::DS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   uint64_t* big_full = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
@@ -378,7 +390,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       const int kc = head * p.k_head_stride, vc = head * p.v_head_stride;
       mbar_expect_tx(big_full, 2 * S::BIG_BYTES);
 #pragma unroll
-      for (int h = 0; h < D / 64; ++h) {
+      for (int h = 0; h < DS / 64; ++h) {
         tma_load_3d(smem + S::OFF_BIG0 + h * (AB_BM * 128), &tmK, big_full, kc + h * 64, kv0, b);
         tma_load_3d(smem + S::OFF_BIG1 + h * (AB_BM * 128), &tmV, big_full, vc + h * 64, kv0, b);
       }
@@ -387,7 +399,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         ring.acquire();
         uint64_t* bar = ring.expect(2 * S::SML_BYTES);
 #pragma unroll
-        for (int h = 0; h < D / 64; ++h) {
+        for (int h = 0; h < DS / 64; ++h) {
           tma_load_3d(smem + S::OFF_SML0 + st * S::SML_BYTES + h * (AB_BN * 128), &tmQ, bar, qc + h * 64, (i_start + i) * AB_BN, b);
           tma_load_3d(smem + S::OFF_SML1 + st * S::SML_BYTES + h * (AB_BN * 128), &tmdO, bar, dc + h * 64, (i_start + i) * AB_BN, b);
         }
@@ -428,9 +440,9 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   // qmin (both bounds live in registers would cost a spill)
   int qlo = 0;
   if constexpr (kLo) qlo = __ldg(start_row + min(kv0 + AB_BM, p.seq_kv) - 1);
-  float dv[D / 2], dk[D / 2];
+  float dv[DS / 2], dk[DS / 2];
 #pragma unroll
-  for (int i = 0; i < D / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  for (int i = 0; i < DS / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
   DropKey dkey;
   if constexpr (kDropout) dkey = drop_key(p.drop);
 
@@ -504,9 +516,9 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     for (int kk = 0; kk < AB_BN / 16; ++kk) { to_frag(s, kk, pa[kk]); to_frag(dp, kk, da[kk]); }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dv, pa[kk], dsc_domn + sto + ((kk * 2048) >> 4), 1u);
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<DS, 1>(dv, pa[kk], dsc_domn + sto + ((kk * 2048) >> 4), 1u);
 #pragma unroll
-    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<D, 1>(dk, da[kk], dsc_qmn + sto + ((kk * 2048) >> 4), 1u);
+    for (int kk = 0; kk < AB_BN / 16; ++kk) wgmma_rs_dim<DS, 1>(dk, da[kk], dsc_qmn + sto + ((kk * 2048) >> 4), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(dv);
@@ -593,7 +605,7 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
   // 1. delta
   {
     const int64_t groups = int64_t(p.batch) * p.seq_q * p.nheads;
-    const int64_t threads = groups * (D / 8);
+    const int64_t threads = groups * (D == 96 ? 4 : D / 8);   // attn_delta_kernel's G
     attn_delta_kernel<D><<<unsigned((threads + 255) / 256), 256, 0, st>>>(
         (const __nv_bfloat16*)o, (const __nv_bfloat16*)dout, delta, o_rs, o_hs, do_rs, p.do_head_stride, p.batch, p.seq_q,
         p.nheads);
@@ -649,7 +661,9 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
                     void* workspace, size_t workspace_bytes, const DropArgs* drop, const int* seg_start,
                     const int* seg_end, fsb_stream_t st, const int* q_start = nullptr, const int* q_end = nullptr) {
   FSB_REQUIRE(q && k && v && o && dout && lse && delta && dq && dk && dv, "sdpa_bwd: null pointer");
-  FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd: head_dim %d unsupported (64 or 128)", head_dim);
+  // head_dim 96 only in the causal forms GPT-2 launches (see sdpa_fwd)
+  FSB_REQUIRE(head_dim == 64 || head_dim == 128 || (head_dim == 96 && causal && rel_bias == nullptr && q_start == nullptr),
+              "sdpa_bwd: head_dim %d unsupported (64 or 128; 96 causal without a bias only)", head_dim);
   FSB_REQUIRE(batch > 0 && seq_q > 0 && seq_kv > 0 && nheads > 0 && batch < 65536 && nheads < 65536, "sdpa_bwd: bad dims");
   FSB_REQUIRE(!causal || seq_q == seq_kv, "sdpa_bwd: causal needs seq_q == seq_kv");
   FSB_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) &&
@@ -713,11 +727,19 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
                                                         nullptr, (cudaStream_t)st);
   }
-  if (seg_start != nullptr && drop != nullptr) {   // fsb_sdpa_bwd_segments_dropout with p > 0: head_dim 64 only
+  if (seg_start != nullptr && drop != nullptr) {   // fsb_sdpa_bwd_segments_dropout with p > 0: head_dim 64 or 96
     p.drop = *drop;
+    if (head_dim == 96)
+      return launch_attn_bwd<96, false, true, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                          o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                          nullptr, (cudaStream_t)st);
     return launch_attn_bwd<64, false, true, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,
                                                   do_row_stride, o_head_stride, delta, p, nullptr, nullptr, (cudaStream_t)st);
   }
+  if (seg_start != nullptr && head_dim == 96)   // fsb_sdpa_bwd_segments_dropout at head_dim 96 with p == 0
+    return launch_attn_bwd<96, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
+                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
+                                                         nullptr, (cudaStream_t)st);
   if (seg_start != nullptr)   // fsb_sdpa_bwd_segments: causal, no bias, no dropout, no key mask
     return head_dim == 128
                ? launch_attn_bwd<128, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
@@ -732,9 +754,11 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   if (drop != nullptr) {
     p.drop = *drop;
     if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, true) : FSB_BWD(64, true, true);
+    if (head_dim == 96) return FSB_BWD(96, false, true);
     return head_dim == 128 ? FSB_BWD(128, false, true) : FSB_BWD(64, false, true);
   }
   if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, false) : FSB_BWD(64, true, false);
+  if (head_dim == 96) return FSB_BWD(96, false, false);
   return head_dim == 128 ? FSB_BWD(128, false, false) : FSB_BWD(64, false, false);
 #undef FSB_BWD
 }
@@ -790,6 +814,7 @@ extern "C" int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v
   FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments: null segment bounds");
   FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
               (long long)seq_kv);
+  // head_dim 96 reaches the same kernels through fsb_sdpa_bwd_segments_dropout (any p, 0 included)
   FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd_segments: head_dim %d unsupported (64 or 128)", head_dim);
   return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
                   k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
@@ -814,11 +839,13 @@ extern "C" int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const
   FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_dropout: null segment bounds");
   FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_dropout: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
               (long long)seq_kv);
-  FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd_segments_dropout: head_dim %d unsupported (64 or 128)",
-              head_dim);
+  FSB_REQUIRE(head_dim == 64 || head_dim == 96 || head_dim == 128,
+              "sdpa_bwd_segments_dropout: head_dim %d unsupported (64, 96 or 128)", head_dim);
   if (p > 0.f) {
-    // GPT-2 (the one model with attention dropout that packs) runs head_dim 64; LLaMA has no attention dropout
-    FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_dropout: head_dim %d unsupported with p > 0 (64 only)", head_dim);
+    // GPT-2 (the one model with attention dropout that packs) runs head_dim 64 (110M) or 96 (3.5B); LLaMA has no attention
+    // dropout
+    FSB_REQUIRE(head_dim == 64 || head_dim == 96, "sdpa_bwd_segments_dropout: head_dim %d unsupported with p > 0 (64 or 96)",
+                head_dim);
     FSB_REQUIRE(seq_q <= 65536, "sdpa_bwd_segments_dropout: sequences longer than 65536 are not supported with p > 0");
   }
   return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,

@@ -366,10 +366,16 @@ static int norm_fwd(const void* x, const void* residual, const void* gamma, cons
 template <bool kLayer, int T, int V, bool kDrop>
 static cudaError_t norm_bwd_smem_attr(size_t bytes) {
   static size_t configured = 0;
-  if (bytes > 48 * 1024 && bytes > configured) {
-    cudaError_t e = cudaFuncSetAttribute(norm_bwd_kernel<kLayer, T, V, kDrop>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         int(bytes));
+  if (bytes > configured) {
+    // the dynamic bytes and the kernel's static shared memory together may not pass 48 KiB without the opt-in (LayerNorm at
+    // 3072 columns asks for exactly 48 KiB of dynamic memory)
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, norm_bwd_kernel<kLayer, T, V, kDrop>);
     if (e != cudaSuccess) return e;
+    if (bytes + fa.sharedSizeBytes > 48 * 1024) {
+      e = cudaFuncSetAttribute(norm_bwd_kernel<kLayer, T, V, kDrop>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes));
+      if (e != cudaSuccess) return e;
+    }
     configured = bytes;
   }
   return cudaSuccess;

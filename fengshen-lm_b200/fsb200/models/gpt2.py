@@ -13,6 +13,8 @@ attention kernels) and the attention / MLP `c_proj` outputs, dropped by the Laye
 training mode with a non-zero probability is rejected (HF would drop).
 Packed rows (several samples per row, fsb200/packing.py) pass `segment_ids`, as LlamaForCausalLM does: attention stays
 causal inside each segment, the attention-probability dropout included, and never crosses one.
+Head widths 64 (Wenzhong-110M), 96 (the 3.5B Wenzhong / Yuyuan: 32 heads x 96) and 128 run; at 96 the KV-cache decode pads
+each head to 128 columns (see generate).
 """
 import math
 from collections import namedtuple
@@ -45,8 +47,8 @@ class GPT2LMHeadModel(FlatModel):
             raise RuntimeError("fsb200 GPT2: only activation_function='gelu_new' is implemented")
         h, V = self.h, self.V
         self.hn = h // self.nh
-        if self.hn not in (64, 128) or V % 8 or h % 8:
-            raise RuntimeError("fsb200 GPT2: head dim must be 64/128 and vocab/hidden multiples of 8 (pad the vocab)")
+        if self.hn not in (64, 96, 128) or V % 8 or h % 8:
+            raise RuntimeError("fsb200 GPT2: head dim must be 64/96/128 and vocab/hidden multiples of 8 (pad the vocab)")
 
         spec = FlatSpec()
         spec.add("transformer.wte.weight", (V, h), "wte")
@@ -69,6 +71,10 @@ class GPT2LMHeadModel(FlatModel):
         self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
                       for b in self.transformer.h]
         self.reset_parameters(seed)
+        # packed rows at head width 96 run the segment attention through its dropout entry, at p = 0 when the attention
+        # probabilities are not dropped (fsb_sdpa_*_segments itself takes head_dim 64 and 128): a Dropout that draws nothing
+        self._seg_nodrop = None if self.hn != 96 else \
+            ops.Dropout(0.0, 0, torch.zeros(1, dtype=torch.int64, device=self.flat.params.device), 0)
         # dropout sites of one forward, in transformers' call order: 0 embeddings; for layer i, 1 + 3i attention probabilities,
         # 2 + 3i attention c_proj output, 3 + 3i MLP c_proj output. A site whose probability is 0 keeps its number.
         self._init_dropout(1 + 3 * self.nl, (self.p_embd, self.p_attn, self.p_resid))
@@ -119,7 +125,8 @@ class GPT2LMHeadModel(FlatModel):
         def attend(i, q5):
             drop = self._drop(base, self.p_attn, 1 + 3 * i)
             if seg is not None:
-                return ops.sdpa_segments_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, *seg, drop=drop)
+                q, k, v = q5[:, :, 0], q5[:, :, 1], q5[:, :, 2]
+                return ops.sdpa_segments_fwd(q, k, v, scale, *seg, drop=self._seg_drop(drop))
             return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask, drop=drop)
         hf, stf, xf = self._stack(ids, pos, B, S, attend, acts, base)
         logits = self._head(hf)
@@ -132,6 +139,10 @@ class GPT2LMHeadModel(FlatModel):
                 ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base, seg)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
+
+    def _seg_drop(self, drop):
+        """The drop argument of the packed attention: `drop`, or at head width 96 without one the p = 0 Dropout."""
+        return drop if drop is not None else self._seg_nodrop
 
     def _stack(self, ids, pos, B, S, attend, acts=None, base=None):
         """Embedding, the blocks and ln_f over ids [B * S] -> (hidden states, ln_f stats, residual stream). attend(i, q5) is
@@ -176,6 +187,10 @@ class GPT2LMHeadModel(FlatModel):
     # kernel (ops.attn_decode). The decode step is one CUDA-graph replay (fsb200/decode_graph.py); beam search gathers the
     # cache, key mask and positions into the twin (ops.kv_reorder). Position ids follow transformers 5.5.0
     # (generation/utils.py:716-720): cumsum(mask) - 1, pads at 0.
+    # Head width 96 decodes on the head_dim 128 decode kernel over a zero-padded cache: the cache's last dimension is 128,
+    # the prefill and ops.kv_append write its first 96 columns, and each step copies q into the first 96 columns of a
+    # zero-padded [rows, heads, 128] buffer. The zero columns add nothing to q.k, the output's padded columns come out as
+    # P.0, and its first 96 feed attn_proj. Beam reorder moves whole slots and is unchanged.
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, **kwargs):
         """HF `generate` semantics (fsb200/generation.py lists what is implemented); prompts are LEFT-padded. Runs without
@@ -193,8 +208,11 @@ class GPT2LMHeadModel(FlatModel):
         R = ids.shape[0]
         cap = (max(c.max_length, S0 + 1) + 63) // 64 * 64
         scale = 1.0 / math.sqrt(self.hn)
+        hn, hc = self.hn, 128 if self.hn == 96 else self.hn   # head width, cached head width
+        pad = (lambda t: t[..., :hn]) if hc != hn else (lambda t: t)   # the head's columns of a cache view
+        q_pad = torch.zeros((R, self.nh, hc), dtype=torch.bfloat16, device=dev) if hc != hn else None
         # per cache: keys / values, key mask, next position id of every row
-        st = [SimpleNamespace(cache=torch.zeros((self.nl, R, cap, 2, self.nh, self.hn), dtype=torch.bfloat16, device=dev),
+        st = [SimpleNamespace(cache=torch.zeros((self.nl, R, cap, 2, self.nh, hc), dtype=torch.bfloat16, device=dev),
                               kv_mask=torch.zeros((R, cap), dtype=torch.uint8, device=dev),
                               count=torch.zeros(R, dtype=torch.int64, device=dev))
               for _ in range(2 if c.num_beams > 1 else 1)]
@@ -207,7 +225,7 @@ class GPT2LMHeadModel(FlatModel):
             pre = None if bool(mask.all()) else st[0].kv_mask[:, :S0].contiguous()
 
             def attend(i, q5):
-                st[0].cache[i][:, :S0].copy_(q5[:, :, 1:3])
+                pad(st[0].cache[i][:, :S0]).copy_(q5[:, :, 1:3])
                 return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=pre)
             return self._last_logits(ids.reshape(-1), pos.reshape(-1), R, S0, attend)
 
@@ -220,9 +238,13 @@ class GPT2LMHeadModel(FlatModel):
 
             def attend(i, q5):   # the key mask is shared by the layers: the first one sets the new slot's bit
                 kv = b.cache[i]
-                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], kv[:, :, 0], kv[:, :, 1], kv_len,
+                ops.kv_append(q5[:, 0, 1], q5[:, 0, 2], pad(kv[:, :, 0]), pad(kv[:, :, 1]), kv_len,
                               kv_mask=b.kv_mask if i == 0 else None)
-                return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=b.kv_mask)
+                if q_pad is None:
+                    return ops.attn_decode(q5[:, 0, 0], kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=b.kv_mask)
+                q_pad[..., :hn].copy_(q5[:, 0, 0])
+                o, lse = ops.attn_decode(q_pad, kv[:, :, 0], kv[:, :, 1], kv_len, scale, kv_mask=b.kv_mask)
+                return o[..., :hn].contiguous(), lse
             logits = self._last_logits(tok, b.count, R, 1, attend)
             b.count.add_(1)
             return logits
@@ -264,7 +286,7 @@ class GPT2LMHeadModel(FlatModel):
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             if seg is not None:
                 ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, *seg,
-                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(self.p_attn, 1 + 3 * i))
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=self._seg_drop(D(self.p_attn, 1 + 3 * i)))
             else:
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))

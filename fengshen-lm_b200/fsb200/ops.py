@@ -601,7 +601,8 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop
     causal: mask the keys after each query (seq_q == seq_kv); the key tiles wholly above the diagonal are skipped.
     kv_mask: optional uint8 [B, Skv] key-padding mask (0: masked). rel_bias: optional fp32 [H, Sq + Skv - 1] additive bias
     over the offset k - q (T5 relative-position bias). drop: optional Dropout on the attention probabilities, its keep mask
-    the attention layout of include/fsb200.h. The causal flag, kv_mask, rel_bias and drop compose."""
+    the attention layout of include/fsb200.h. The causal flag, kv_mask, rel_bias and drop compose. head_dim 64 or 128; 96
+    (GPT-2 3.5B) with causal=True and no rel_bias only."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -722,7 +723,7 @@ def _chk_grads(q, k, dq, dk, dv):
 def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, rel_bias=None, drel_bias=None, drop=None):
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
     causal, kv_mask and rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=),
-    deterministically. drop: the forward's Dropout (same seed, base and site)."""
+    deterministically. drop: the forward's Dropout (same seed, base and site). head_dim as in sdpa_fwd."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")
@@ -798,7 +799,9 @@ def _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B):
 def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, causal=True, rel_bias=None, kv_bounds=None):
     """sdpa_fwd over rows that pack several sequences: causal inside each segment, nothing across segments. q, k, v as in
     sdpa_fwd (seq_q == seq_kv); seg_start / seg_end from segment_bounds. Key / query tiles outside a tile's segments are
-    skipped. drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 when p > 0).
+    skipped. head_dim 64 or 128; 96 only with a drop (fsb_sdpa_fwd_segments_dropout; a Dropout with p = 0 runs the
+    dropout-free kernel). drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 or 96 when
+    p > 0).
     causal=False: bidirectional inside each segment (packed encoder rows: query q sees seg_start[q] <= k < seg_end[q]),
     head_dim 64 only (fsb_sdpa_fwd_segments_bidirectional).
     rel_bias: the T5 relative-position bias of sdpa_fwd (fp32 [H, 2 S - 1]) added inside either segment form, head_dim 64

@@ -292,7 +292,8 @@ int fsb_softmax_get_batch_per_block(int64_t sq, int64_t sk, int64_t batches, int
  *   element (b, s, head, d) of X lives at X + ((b*seq + s)*x_row_stride + head*x_head_stride + d)  (elements).
  * o: same addressing with o_*_stride. lse: fp32 [batch, nheads, seq_q], log2 domain (internal, consumed by bwd).
  * kv_mask: optional uint8 [batch, seq_kv], 1 = attend (HF additive padding mask), NULL = none.
- * causal=1 masks key > query (requires seq_q == seq_kv). head_dim in {64, 128}.
+ * causal=1 masks key > query (requires seq_q == seq_kv). head_dim in {64, 128}, and 96 with causal=1 and no rel_bias
+ *   (GPT-2 3.5B, 32 heads x 96; the kernels stage 128 columns and store 96; fsb_sdpa_*_dropout likewise).
  * rel_bias: optional fp32 [nheads, seq_q + seq_kv - 1], natural-log units, added to scale * q.k before the softmax:
  *   bias(h, q, k) = rel_bias[h][k - q + seq_q - 1]  — the T5 / mT5 relative-position bias (transformers
  *   mt5/modeling_mt5.py:181-235,:320: an embedding over bucket(k - q), shared by every layer of a stack), used by
@@ -370,7 +371,8 @@ int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void
  * fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments: fsb_sdpa_fwd / fsb_sdpa_bwd with causal = 1 inside each segment of a row
  * and nothing across segments, for rows that pack several documents. No kv_mask or rel_bias (dropout: the
  * fsb_sdpa_*_segments_dropout pair below); seq_q == seq_kv;
- * head_dim in {64, 128}. The bounds are two int32 [batch, seq] arrays, contiguous, indices relative to the row:
+ * head_dim in {64, 128} (head_dim 96 runs the same kernels through fsb_sdpa_*_segments_dropout, at p = 0 without
+ * dropout). The bounds are two int32 [batch, seq] arrays, contiguous, indices relative to the row:
  *   seg_start[b][t] : the position of the first token of t's segment;
  *   seg_end[b][t]   : one past the position of its last token.
  * Key k is visible to query q iff seg_start[q] <= k <= q (equivalently k <= q < seg_end[k]). The bounds are valid when every
@@ -396,8 +398,8 @@ int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const voi
  * probabilities (GPT-2 packed training), taking p, seed, stream_base and site as fsb_sdpa_*_dropout do. Visibility is the
  * segment rule above; the keep mask Z is the attention layout of the dropout section, at the row-relative (q, k) of each
  * element, so an element keeps the bit it has in an unsegmented causal launch and the skipped tiles draw nothing. O, the LSE
- * (of the un-dropped P) and the gradients follow fsb_sdpa_*_dropout. p == 0 runs fsb_sdpa_*_segments and does not read the
- * stream counter. Refused: null bounds, seq_q != seq_kv, head_dim other than 64 or 128, and with p > 0 head_dim != 64 or
+ * (of the un-dropped P) and the gradients follow fsb_sdpa_*_dropout. p == 0 runs the kernels of fsb_sdpa_*_segments and does
+ * not read the stream counter; at head_dim 96 this is the only entry to the packed kernels (fsb_sdpa_*_segments refuse 96). Refused: null bounds, seq_q != seq_kv, head_dim other than 64, 96 or 128, and with p > 0 head_dim 128 or
  * sequences longer than 65536. The backward must get the forward's bounds, seed, stream_base value and site. */
 int fsb_sdpa_fwd_segments_dropout(const void* q, const void* k, const void* v, void* o, float* lse,
                                   int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
