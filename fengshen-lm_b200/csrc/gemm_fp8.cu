@@ -1,5 +1,5 @@
-// fsb200 — FP8 training GEMM and its quantiser for sm_90a: the layer projections of a LLaMA, BERT, MegatronBERT or mT5
-// model built with fp8=True.
+// fsb200 — FP8 training GEMM and its quantiser for sm_90a: the layer projections of a LLaMA, BERT, MegatronBERT, mT5 or
+// GPT-2 model built with fp8=True.
 // The recipe (include/fsb200.h): activations and weights e4m3, gradients e5m2, one power-of-two scale per tensor computed
 // just in time from the tensor's amax, fp32 accumulation, bf16 outputs.
 //
@@ -22,6 +22,11 @@
 //     TMA, which clips ragged m / n edges; aux leaves through the same staging buffers as a second store per sub-tile. The
 //     plain instantiations (no bias, aux or activation) are the ones LLaMA runs and carry none of that code. No split-K:
 //     results are deterministic.
+// fsb_gemm_fp8_t: the same kernel with the kT flag, D[n, m] = the transpose of fsb_gemm_fp8's D. A GPT-2 Conv1D weight is
+//   stored [in, out], so its gradient x^T dy must land [in, out]; both FP8 wgmma operands are K-major, which makes the pair
+//   the kernel takes, (e5m2, e4m3), compute dy^T x = dW^T. The kT epilogue stages each 64 x 64 sub-tile transposed (stmatrix
+//   .trans into the same 128B-swizzled buffers) and TMA-stores it at swapped coordinates; main loop, producer and scales are
+//   shared, so the values are fsb_gemm_fp8's bit for bit.
 #include "gemm_epilogue.cuh"
 #include "host_common.h"
 #include "ptx.cuh"
@@ -59,8 +64,9 @@ struct F8Params {
 };
 
 // kEpi: bias / GELU / aux in the epilogue. tmAux is the last parameter so that the plain kernels' parameter offsets are
-// unchanged.
-template <bool kE5M2A, bool kEpi>
+// unchanged. kT: D is stored transposed, D[n, m] (fsb_gemm_fp8_t; plain epilogue only): each 64 x 64 sub-tile is staged
+// transposed by stmatrix .trans and TMA-stored at swapped coordinates, and the old D of `accumulate` is read at D[col][row].
+template <bool kE5M2A, bool kEpi, bool kT = false>
 __global__ void __launch_bounds__(F8_THREADS, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmD, const F8Params p, const __grid_constant__ CUtensorMap tmAux) {
@@ -196,28 +202,48 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int row = m0 + r + 8 * h;
-              if (row >= p.M || col >= p.N) continue;   // N % 8 == 0: col < N implies col + 1 < N
-              const uint32_t q = *reinterpret_cast<const uint32_t*>(p.D + int64_t(row) * p.ldd + col);
-              acc[4 * j + 2 * h] += bf16lo(q);
-              acc[4 * j + 2 * h + 1] += bf16hi(q);
+              if constexpr (kT) {   // element (row, col) is D[col][row]; any N, so col + 1 is bounded on its own
+                if (row >= p.M) continue;
+                if (col < p.N) acc[4 * j + 2 * h] += __bfloat162float(p.D[int64_t(col) * p.ldd + row]);
+                if (col + 1 < p.N) acc[4 * j + 2 * h + 1] += __bfloat162float(p.D[int64_t(col + 1) * p.ldd + row]);
+              } else {
+                if (row >= p.M || col >= p.N) continue;   // N % 8 == 0: col < N implies col + 1 < N
+                const uint32_t q = *reinterpret_cast<const uint32_t*>(p.D + int64_t(row) * p.ldd + col);
+                acc[4 * j + 2 * h] += bf16lo(q);
+                acc[4 * j + 2 * h + 1] += bf16hi(q);
+              }
             }
           }
         }
         uint8_t* buf = epi_buf + (n_stored & 1) * S::EPI_BUF_BYTES;
         if (leader) tma_store_wait_read<1>();   // the store that last used this buffer has read it out
         bar_sync(1 + wg, 128);
+        if constexpr (kT) {
+          // the sub-tile's column c (of 64) becomes buffer row c: 128 bytes = the warpgroup's 64 rows. One stmatrix per two
+          // 8-column groups: matrix i = (group jj + i / 2, rows r0 + 8 (i % 2)), r0 = 16 wl; lane 8 i + c addresses its row c.
+          const int mi = lane >> 3;
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
+          for (int jj = 0; jj < 8; jj += 2) {
             const int j = 8 * g + jj;
-            *reinterpret_cast<uint32_t*>(buf + swz128(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
-                pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            stmatrix_x4_trans(smem_u32(buf + swz128(8 * (jj + (mi >> 1)) + (lane & 7), 32 * wl + 16 * (mi & 1))),
+                              pack_bf16x2(acc[4 * j], acc[4 * j + 1]), pack_bf16x2(acc[4 * j + 2], acc[4 * j + 3]),
+                              pack_bf16x2(acc[4 * j + 4], acc[4 * j + 5]), pack_bf16x2(acc[4 * j + 6], acc[4 * j + 7]));
           }
+        } else {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int j = 8 * g + jj;
+              *reinterpret_cast<uint32_t*>(buf + swz128(r + 8 * h, 16 * jj + 4 * (lane & 3))) =
+                  pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+        }
         fence_proxy_async();
         bar_sync(1 + wg, 128);
         if (leader) {
-          tma_store_2d(&tmD, buf, n0 + 64 * g, m0);
+          if constexpr (kT) tma_store_2d(&tmD, buf, m0, n0 + 64 * g);
+          else tma_store_2d(&tmD, buf, n0 + 64 * g, m0);
           tma_store_commit();
         }
         ++n_stored;
@@ -319,11 +345,72 @@ fp8_cast_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, int64_t rows, 
   }
 }
 
-template <bool kE5M2A, bool kEpi>
+template <bool kE5M2A, bool kEpi, bool kT = false>
 static int launch_gemm_fp8(int grid, const F8Params& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                            const CUtensorMap& tmAux, cudaStream_t stream) {
-  if (int rc = ensure_smem<gemm_fp8_kernel<kE5M2A, kEpi>>(F8Smem::TOTAL, "gemm_fp8")) return rc;
-  gemm_fp8_kernel<kE5M2A, kEpi><<<grid, F8_THREADS, F8Smem::TOTAL, stream>>>(tmA, tmB, tmD, p, tmAux);
+  if (int rc = ensure_smem<gemm_fp8_kernel<kE5M2A, kEpi, kT>>(F8Smem::TOTAL, "gemm_fp8")) return rc;
+  gemm_fp8_kernel<kE5M2A, kEpi, kT><<<grid, F8_THREADS, F8Smem::TOTAL, stream>>>(tmA, tmB, tmD, p, tmAux);
+  return FSB_OK;
+}
+
+// The tensor maps, tile schedule and launch of fsb_gemm_fp8 (transposed = false: D [m, n]) and fsb_gemm_fp8_t (D [n, m]),
+// after each entry's own checks.
+static int run_gemm_fp8(bool transposed, int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv,
+                        const void* b, const float* b_scale_inv, void* d, int64_t ldd, const void* bias, int epilogue,
+                        int accumulate, void* aux, int64_t ldaux, cudaStream_t stream) {
+  const bool epi = bias != nullptr || aux != nullptr || epilogue != FSB_EPI_NONE;
+  CUtensorMap tmA, tmB, tmD, tmAux;
+  {
+    uint64_t dims[2] = {uint64_t(k), uint64_t(m)};
+    uint64_t strides[1] = {uint64_t(k)};
+    uint32_t box[2] = {uint32_t(F8_BK), uint32_t(F8_BM)};
+    if (int rc = make_tmap_u8(&tmA, a, 2, dims, strides, box)) return rc;
+  }
+  {
+    uint64_t dims[2] = {uint64_t(k), uint64_t(n)};
+    uint64_t strides[1] = {uint64_t(k)};
+    uint32_t box[2] = {uint32_t(F8_BK), uint32_t(F8_BN)};
+    if (int rc = make_tmap_u8(&tmB, b, 2, dims, strides, box)) return rc;
+  }
+  {
+    uint64_t dims[2] = {uint64_t(transposed ? m : n), uint64_t(transposed ? n : m)};
+    uint64_t strides[1] = {uint64_t(ldd) * 2};
+    uint32_t box[2] = {64, 64};
+    if (int rc = make_tmap_bf16(&tmD, d, 2, dims, strides, box)) return rc;
+  }
+  tmAux = tmD;   // never read without aux
+  if (aux != nullptr) {
+    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
+    uint64_t strides[1] = {uint64_t(ldaux) * 2};
+    uint32_t box[2] = {64, 64};
+    if (int rc = make_tmap_bf16(&tmAux, aux, 2, dims, strides, box)) return rc;
+  }
+  F8Params p;
+  p.D = static_cast<__nv_bfloat16*>(d);
+  p.a_sinv = a_scale_inv; p.b_sinv = b_scale_inv;
+  p.ldd = ldd;
+  p.M = int(m); p.N = int(n); p.K = int(k);
+  p.accumulate = accumulate;
+  p.bias = static_cast<const __nv_bfloat16*>(bias);
+  p.epilogue = epilogue;
+  p.has_aux = aux != nullptr;
+  p.tiles_m = int((m + F8_BM - 1) / F8_BM);
+  p.tiles_n = int((n + F8_BN - 1) / F8_BN);
+  // rasterisation groups as gemm.cu's 128-wide tiles: 12 m-tiles, more while their A panels (128 x k bytes) fit ~32 MB of L2
+  {
+    int64_t gm = (int64_t(32) << 20) / (int64_t(F8_BM) * k);
+    p.group_m = int(gm < 12 ? 12 : (gm > 64 ? 64 : gm));
+  }
+  const int num_tiles = p.tiles_m * p.tiles_n;
+  const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
+  int rc;
+  if (transposed) rc = launch_gemm_fp8<true, false, true>(grid, p, tmA, tmB, tmD, tmAux, stream);
+  else if (a_fmt == FSB_FP8_E5M2) rc = epi ? launch_gemm_fp8<true, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
+                                           : launch_gemm_fp8<true, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
+  else rc = epi ? launch_gemm_fp8<false, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
+                : launch_gemm_fp8<false, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
+  if (rc) return rc;
+  FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
 
@@ -384,58 +471,30 @@ extern "C" int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int 
   FSB_REQUIRE(bias == nullptr || aligned16(bias), "gemm_fp8: bias must be 16-byte aligned");
   FSB_REQUIRE(aux == nullptr || (aligned16(aux) && ldaux >= n && ldaux % 8 == 0),
               "gemm_fp8: aux must be 16-byte aligned with ldaux=%ld >= n and a multiple of 8", (long)ldaux);
-  const bool epi = bias != nullptr || aux != nullptr || epilogue != FSB_EPI_NONE;
+  return run_gemm_fp8(false, m, n, k, a, a_fmt, a_scale_inv, b, b_scale_inv, d, ldd, bias, epilogue, accumulate, aux, ldaux,
+                      stream);
+}
 
-  CUtensorMap tmA, tmB, tmD, tmAux;
-  {
-    uint64_t dims[2] = {uint64_t(k), uint64_t(m)};
-    uint64_t strides[1] = {uint64_t(k)};
-    uint32_t box[2] = {uint32_t(F8_BK), uint32_t(F8_BM)};
-    if (int rc = make_tmap_u8(&tmA, a, 2, dims, strides, box)) return rc;
-  }
-  {
-    uint64_t dims[2] = {uint64_t(k), uint64_t(n)};
-    uint64_t strides[1] = {uint64_t(k)};
-    uint32_t box[2] = {uint32_t(F8_BK), uint32_t(F8_BN)};
-    if (int rc = make_tmap_u8(&tmB, b, 2, dims, strides, box)) return rc;
-  }
-  {
-    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
-    uint64_t strides[1] = {uint64_t(ldd) * 2};
-    uint32_t box[2] = {64, 64};
-    if (int rc = make_tmap_bf16(&tmD, d, 2, dims, strides, box)) return rc;
-  }
-  tmAux = tmD;   // never read without aux
-  if (aux != nullptr) {
-    uint64_t dims[2] = {uint64_t(n), uint64_t(m)};
-    uint64_t strides[1] = {uint64_t(ldaux) * 2};
-    uint32_t box[2] = {64, 64};
-    if (int rc = make_tmap_bf16(&tmAux, aux, 2, dims, strides, box)) return rc;
-  }
-  F8Params p;
-  p.D = static_cast<__nv_bfloat16*>(d);
-  p.a_sinv = a_scale_inv; p.b_sinv = b_scale_inv;
-  p.ldd = ldd;
-  p.M = int(m); p.N = int(n); p.K = int(k);
-  p.accumulate = accumulate;
-  p.bias = static_cast<const __nv_bfloat16*>(bias);
-  p.epilogue = epilogue;
-  p.has_aux = aux != nullptr;
-  p.tiles_m = int((m + F8_BM - 1) / F8_BM);
-  p.tiles_n = int((n + F8_BN - 1) / F8_BN);
-  // rasterisation groups as gemm.cu's 128-wide tiles: 12 m-tiles, more while their A panels (128 x k bytes) fit ~32 MB of L2
-  {
-    int64_t gm = (int64_t(32) << 20) / (int64_t(F8_BM) * k);
-    p.group_m = int(gm < 12 ? 12 : (gm > 64 ? 64 : gm));
-  }
-  const int num_tiles = p.tiles_m * p.tiles_n;
-  const int grid = num_tiles < gemm_sms() ? num_tiles : gemm_sms();
-  int rc;
-  if (a_fmt == FSB_FP8_E5M2) rc = epi ? launch_gemm_fp8<true, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
-                                      : launch_gemm_fp8<true, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
-  else rc = epi ? launch_gemm_fp8<false, true>(grid, p, tmA, tmB, tmD, tmAux, stream)
-                : launch_gemm_fp8<false, false>(grid, p, tmA, tmB, tmD, tmAux, stream);
-  if (rc) return rc;
-  FSB_CUDA_LAUNCH_CHECK();
-  return FSB_OK;
+extern "C" int fsb_gemm_fp8_t(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv,
+                              const void* b, int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, const void* bias,
+                              int epilogue, int accumulate, void* aux, int64_t ldaux, fsb_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_fp8_t: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
+  FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_fp8_t: dims too large");
+  FSB_REQUIRE(k % 16 == 0, "gemm_fp8_t: k=%ld must be a multiple of 16", (long)k);
+  FSB_REQUIRE(m % 8 == 0, "gemm_fp8_t: m=%ld must be a multiple of 8 (D^T rows of m bf16 values need 16-byte strides)",
+              (long)m);
+  FSB_REQUIRE(a_fmt == FSB_FP8_E5M2 && b_fmt == FSB_FP8_E4M3,
+              "gemm_fp8_t: format pair (a %d, b %d) unsupported: only (e5m2, e4m3)", a_fmt, b_fmt);
+  FSB_REQUIRE(bias == nullptr && aux == nullptr && epilogue == FSB_EPI_NONE,
+              "gemm_fp8_t: no bias, aux or epilogue (got bias %s, aux %s, epilogue %d)", bias ? "set" : "NULL",
+              aux ? "set" : "NULL", epilogue);
+  FSB_REQUIRE(a && b && d && a_scale_inv && b_scale_inv, "gemm_fp8_t: null operand");
+  FSB_REQUIRE(aligned16(a) && aligned16(b) && aligned16(d), "gemm_fp8_t: a, b and d must be 16-byte aligned");
+  FSB_REQUIRE((reinterpret_cast<uintptr_t>(a_scale_inv) & 3) == 0 && (reinterpret_cast<uintptr_t>(b_scale_inv) & 3) == 0,
+              "gemm_fp8_t: scale_inv pointers must be 4-byte aligned");
+  FSB_REQUIRE(ldd >= m && ldd % 8 == 0, "gemm_fp8_t: ldd=%ld must be >= m and a multiple of 8", (long)ldd);
+  (void)ldaux;
+  return run_gemm_fp8(true, m, n, k, a, a_fmt, a_scale_inv, b, b_scale_inv, d, ldd, nullptr, FSB_EPI_NONE, accumulate,
+                      nullptr, 0, stream);
 }

@@ -226,6 +226,14 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_
 __device__ __forceinline__ uint32_t swz128(int row, int byte) {
   return uint32_t(row * 128 + ((((byte >> 4) ^ row) & 7) << 4) + (byte & 15));
 }
+// Four 8 x 8 b16 matrices stored transposed: register i holds matrix i's fragment (lane t: row t / 4, columns 2 (t % 4) and
+// + 1, the low half first, as the wgmma accumulator pairs), and row c of the stored matrix i (the fragment's column c) goes
+// to the 16 bytes at the shared address lane 8 i + c passes.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
 
 // m64nNk16, bf16 x bf16 -> fp32. kTA / kTB = 1: that operand is MN-major in shared memory. Register A operand (_rs): the
 // fragment of one 64 x 16 slice, four bf16 pairs per thread — (row, k..k+1), (row+8, k..k+1), (row, k+8..), (row+8, k+8..)

@@ -52,8 +52,8 @@ class _HFSurface:
         if not os.path.isdir(path):
             raise FileNotFoundError(f"fsb200 {cls.__name__}.from_pretrained: {path!r} is not a local directory "
                                     "(there is no hub access on the product path)")
-        # model keywords: fp8 exists on BertForMaskedLM, MegatronBertForPreTraining (fsb200/models/bert.py) and
-        # MT5ForConditionalGeneration (fsb200/models/t5.py)
+        # model keywords: fp8 exists on BertForMaskedLM, MegatronBertForPreTraining (fsb200/models/bert.py),
+        # MT5ForConditionalGeneration (fsb200/models/t5.py) and GPT2LMHeadModel (fsb200/models/gpt2.py)
         kw = {k: kwargs[k] for k in ("device", "world_size", "seed", "fp8") if k in kwargs}
         cfg_cls = _hf_config(cls.config_name)
         if config is not None or state_dict is not None:

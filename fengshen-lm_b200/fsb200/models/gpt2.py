@@ -15,6 +15,13 @@ Packed rows (several samples per row, fsb200/packing.py) pass `segment_ids`, as 
 causal inside each segment, the attention-probability dropout included, and never crosses one.
 Head widths 64 (Wenzhong-110M), 96 (the 3.5B Wenzhong / Yuyuan: 32 heads x 96) and 128 run; at 96 the KV-cache decode pads
 each head to 128 columns (see generate).
+fp8=True trains each block's c_attn, attn.c_proj, mlp.c_fc (bias, gelu_new and its pre-activation in the FP8 GEMM's
+epilogue) and mlp.c_proj in FP8 (layers.Fp8Conv1D, include/fsb200.h fsb_gemm_fp8 / fsb_gemm_fp8_t): e4m3 activations and
+weights, e5m2 gradients, per-tensor power-of-two scales from each tensor's amax just before its cast, fp32 accumulation. The
+forward keeps the transposed e4m3 codes of ln_1's and ln_2's outputs and of the GELU output instead of the bf16 tensors;
+attn.c_proj makes its input's codes from the attention output in the backward (attention keeps that output anyway). The
+embeddings, the tied LM head, the LayerNorms, attention, dGELU with the c_fc bias gradient, the loss and the optimizer stay
+bf16, as do the master weights and gradients; `generate` runs the bf16 projections.
 """
 import math
 from collections import namedtuple
@@ -28,14 +35,18 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments, refuse_key_padding
-from .layers import Linear, apply_dropout, residual_norm_bwd
+from .layers import Fp8Conv1D, Linear, apply_dropout, residual_norm_bwd
 
 _Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
 
 
 class GPT2LMHeadModel(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0):
+    def __init__(self, config, device=None, world_size=None, seed=0, fp8=False):
+        """fp8: train the block projections in FP8; see the module docstring. The training and no-grad (validation)
+        forwards both run FP8; results differ from bf16 by design. n_embd, the MLP's inner width and the tokens per
+        micro-batch (batch x sequence length) must be multiples of 16 (checked at the first forward)."""
         super().__init__(config)
+        self.fp8 = bool(fp8)
         g = lambda k, d=None: getattr(config, k, d)
         self.h, self.nl, self.nh = g("n_embd", g("hidden_size")), g("n_layer", g("num_hidden_layers")), \
             g("n_head", g("num_attention_heads"))
@@ -70,6 +81,9 @@ class GPT2LMHeadModel(FlatModel):
         conv1d = lambda m: Linear.of(m.weight, m.bias, conv1d=True)
         self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
                       for b in self.transformer.h]
+        self._proj_bf16 = self._proj   # what generate runs
+        if self.fp8:
+            self._proj = [_Block(*(Fp8Conv1D(q) for q in pj)) for pj in self._proj]
         self.reset_parameters(seed)
         # packed rows at head width 96 run the segment attention through its dropout entry, at p = 0 when the attention
         # probabilities are not dropped (fsb_sdpa_*_segments itself takes head_dim 64 and 128): a Dropout that draws nothing
@@ -103,6 +117,12 @@ class GPT2LMHeadModel(FlatModel):
         the packer makes the pad tail a segment of its own, and an attention_mask with zeros is refused. None: one causal
         sequence per row under attention_mask, as before."""
         B, S = input_ids.shape
+        if self.fp8:
+            bad = [f"{name} ({v})" for name, v in (("n_embd", self.h), ("the inner width", self.inner),
+                                                    (f"batch {B} x sequence length {S}", B * S)) if v % 16]
+            if bad:
+                raise ValueError(f"fsb200 GPT2LMHeadModel(fp8=True): {', '.join(bad)} not a multiple of 16 (the FP8 GEMM "
+                                 "operands need 16-byte rows in both layouts)")
         dev = self.flat.params.device
         ids, lab = flat_ids(input_ids, dev), flat_ids(labels, dev)
         pos = None if position_ids is None else flat_ids(position_ids.expand(B, S), dev)
@@ -144,11 +164,11 @@ class GPT2LMHeadModel(FlatModel):
         """The drop argument of the packed attention: `drop`, or at head width 96 without one the p = 0 Dropout."""
         return drop if drop is not None else self._seg_nodrop
 
-    def _stack(self, ids, pos, B, S, attend, acts=None, base=None):
+    def _stack(self, ids, pos, B, S, attend, acts=None, base=None, proj=None):
         """Embedding, the blocks and ln_f over ids [B * S] -> (hidden states, ln_f stats, residual stream). attend(i, q5) is
         block i's attention over the packed q|k|v view [B, S, 3, heads, head_dim] -> (out, lse), drawing its own probability
         mask; `acts`, when given, collects what the backward reads. base: the forward's dropout stream base (None: no
-        dropout, as in generation's prefill and decode steps)."""
+        dropout, as in generation's prefill and decode steps). proj: the blocks' projections (default self._proj)."""
         h, nh, hn = self.h, self.nh, self.hn
         tr = self.transformer
         pr = self.p_resid
@@ -157,23 +177,26 @@ class GPT2LMHeadModel(FlatModel):
         x = apply_dropout(ops.embedding_fwd(ids, tr.wte.weight.data, pos=pos, P=tr.wpe.weight.data, seq_len=S),
                           D(self.p_embd, 0))
         prev_m = None
-        for i, (blk, pj) in enumerate(zip(tr.h, self._proj)):
+        save = acts is not None
+        for i, (blk, pj) in enumerate(zip(tr.h, self._proj if proj is None else proj)):
             self._need(f"layer{i}")
             h1, st1, x = ops.layernorm_fwd(x if prev_m is None else prev_m, blk.ln_1.weight.data, blk.ln_1.bias.data,
                                            self.eps, residual=None if prev_m is None else x,
                                            drop=None if prev_m is None else D(pr, 3 * i))   # layer i-1's MLP output
-            qkv = pj.c_attn(h1)
+            # h1s, h2s, fs: what the projections' backward reads of their inputs (the tensors themselves in bf16, their
+            # transposed e4m3 codes and scales in FP8)
+            qkv, h1s = pj.c_attn.forward(h1, save)
             o, lse = attend(i, qkv.view(B, S, 3, nh, hn))
             a = pj.attn_proj(o.view(B * S, h))
             h2, st2, x1 = ops.layernorm_fwd(a, blk.ln_2.weight.data, blk.ln_2.bias.data, self.eps, residual=x,
                                             drop=D(pr, 2 + 3 * i))
             pre = None if acts is None else torch.empty((B * S, self.inner), dtype=torch.bfloat16, device=x.device)
-            f = pj.c_fc(h2, epilogue=L.EPI_GELU_TANH, aux=pre)
-            m = pj.mlp_proj(f)
+            f, h2s = pj.c_fc.forward(h2, save, epilogue=L.EPI_GELU_TANH, aux=pre)
+            m, fs = pj.mlp_proj.forward(f, save)
             if acts is not None:
-                acts.append((x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f))
+                acts.append((x, st1, h1s, qkv, o, lse, x1, st2, h2s, pre, fs))
             # free this block's temporaries before the next block allocates its own (the peak of a long prompt's prefill)
-            del st1, h1, qkv, o, lse, a, st2, h2, pre, f
+            del st1, h1, h1s, qkv, o, lse, a, st2, h2, h2s, pre, f, fs
             x, prev_m = x1, m
         return ops.layernorm_fwd(prev_m, tr.ln_f.weight.data, tr.ln_f.bias.data, self.eps, residual=x,
                                  drop=D(pr, 3 * self.nl))
@@ -253,7 +276,7 @@ class GPT2LMHeadModel(FlatModel):
 
     def _last_logits(self, ids, pos, B, S, attend):
         """fp32 logits [B, V] of the last position of every sequence."""
-        hf, _, _ = self._stack(ids, pos, B, S, attend)
+        hf, _, _ = self._stack(ids, pos, B, S, attend, proj=self._proj_bf16)   # fp8=True: bf16
         return self._head(hf.view(B, S, self.h)[:, -1].contiguous()).float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------
@@ -275,13 +298,13 @@ class GPT2LMHeadModel(FlatModel):
         dx, dm = residual_norm_bwd(dhf, xf, tr.ln_f.weight, tr.ln_f.bias, stf, D(pr, 3 * self.nl), acc)
         for i in reversed(range(self.nl)):
             blk, pj = tr.h[i], self._proj[i]
-            x, st1, h1, qkv, o, lse, x1, st2, h2, pre, f = acts[i]
+            x, st1, h1s, qkv, o, lse, x1, st2, h2s, pre, fs = acts[i]
             acts[i] = None
-            df = pj.mlp_proj.backward(dm, f, acc)
+            df = pj.mlp_proj.backward(dm, fs, acc)
             dpre = ops.act_bwd_bias(L.ACT_GELU_TANH, df, pre, pj.c_fc.bias_grad, accumulate=acc)   # dGELU + c_fc bias grad
-            dh2 = pj.c_fc.backward(dpre, h2, acc, colsum=False)
+            dh2 = pj.c_fc.backward(dpre, h2s, acc, colsum=False)
             dx1, da = residual_norm_bwd(dh2, x1, blk.ln_2.weight, blk.ln_2.bias, st2, D(pr, 2 + 3 * i), acc, dres=dx)
-            do = pj.attn_proj.backward(da, o.view(T, h), acc)
+            do = pj.attn_proj.backward(da, pj.attn_proj.saved_input(o.view(T, h)), acc)   # o is kept for attention anyway
             dqkv = torch.empty_like(qkv)
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             if seg is not None:
@@ -290,7 +313,7 @@ class GPT2LMHeadModel(FlatModel):
             else:
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))
-            dh1 = pj.c_attn.backward(dqkv, h1, acc)
+            dh1 = pj.c_attn.backward(dqkv, h1s, acc)
             # layer 0's LN had no residual (x = the embeddings); layer i's summed layer i-1's dropped MLP output into x
             dx, dm = residual_norm_bwd(dh1, x, blk.ln_1.weight, blk.ln_1.bias, st1, D(pr, 3 * i) if i > 0 else None, acc,
                                        dres=dx1)

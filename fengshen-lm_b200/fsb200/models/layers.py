@@ -138,7 +138,7 @@ class Fp8Linear:
     def forward(self, x, save, epilogue=L.EPI_NONE, aux=None, codes=None):
         """codes: quantize_input(x, save), made once for several projections; x is then not read."""
         xq, xt, sx = self.quantize_input(x, save) if codes is None else codes
-        wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
+        wq, sw = self._forward_weight()
         # a bias-free projection without an epilogue (LLaMA's) makes the plain call it made before the epilogue existed
         epi = {} if self.lin.bias is None and epilogue == L.EPI_NONE and aux is None else \
             dict(bias=self.lin.bias, epilogue=epilogue, aux=aux)
@@ -154,9 +154,46 @@ class Fp8Linear:
         """As Linear.backward, with `saved` what forward / saved_input returned."""
         xt, sx = saved
         dyq, dyt, sdy = ops.fp8_quantize(dy, "e5m2", rowwise=True, colwise=True)
-        _, wt, sw = ops.fp8_quantize(self.lin.weight, "e4m3", rowwise=False, colwise=True)
+        wt, sw = self._dgrad_weight()
         dx = ops.gemm_fp8(dyq, sdy, wt, sw, out=dx, accumulate=dx_accumulate)
-        ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate)
+        self._wgrad(dyt, sdy, xt, sx, accumulate)
         if self.lin.bias is not None and colsum:
             ops.colsum(dy, self.lin.bias_grad, accumulate=accumulate)
         return dx
+
+    # the weight's layout: the forward's B operand [out, in], the data gradient's [in, out], and the weight gradient's store
+    def _forward_weight(self):
+        wq, _, sw = ops.fp8_quantize(self.lin.weight, "e4m3")
+        return wq, sw
+
+    def _dgrad_weight(self):
+        _, wt, sw = ops.fp8_quantize(self.lin.weight, "e4m3", rowwise=False, colwise=True)
+        return wt, sw
+
+    def _wgrad(self, dyt, sdy, xt, sx, accumulate):
+        ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate)
+
+
+class Fp8Conv1D(Fp8Linear):
+    """A GPT-2 Conv1D (Linear(..., conv1d=True): weight [in, out], with or without a bias) in FP8: Fp8Linear's recipe, call
+    surface and saved codes, over the other weight layout.
+      forward: y = x W (+ bias, epilogue, aux) from x e4m3 row-major and W's transposed e4m3 codes (W^T [out, in]).
+      backward: dx = dy W^T from dy e5m2 row-major and W's row-major e4m3 codes; dW (+)= x^T dy written [in, out] into the flat
+                gradient by gemm_fp8(store_transposed=True) from dy^T e5m2 and x^T e4m3 codes (the FP8 GEMM takes (e5m2, e4m3) only, so it
+                computes dW^T = dy^T x and stores it transposed).
+    The same Conv1D as an Fp8Linear over W^T gives the same bits: y, dx and the bias gradient equal, dW its transpose.
+    The token count and both extents of W must be multiples of 16."""
+
+    def __init__(self, lin):
+        if not lin.conv1d:
+            raise ValueError("fsb200 Fp8Conv1D: only [in, out] Conv1D projections (an [out, in] Linear runs as Fp8Linear)")
+        self.lin = lin
+
+    def _forward_weight(self):
+        return Fp8Linear._dgrad_weight(self)
+
+    def _dgrad_weight(self):
+        return Fp8Linear._forward_weight(self)
+
+    def _wgrad(self, dyt, sdy, xt, sx, accumulate):
+        ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate, store_transposed=True)

@@ -203,34 +203,40 @@ def fp8_quantize(x, fmt, rowwise=True, colwise=False):
     return y, yt, sinv[:1]
 
 
-def gemm_fp8(a, a_scale_inv, b, b_scale_inv, out=None, accumulate=False, bias=None, epilogue=L.EPI_NONE, aux=None):
+def gemm_fp8(a, a_scale_inv, b, b_scale_inv, out=None, accumulate=False, bias=None, epilogue=L.EPI_NONE, aux=None,
+             store_transposed=False):
     """out[m, n] (+)= bf16((a[m, k] @ b[n, k]^T) * a_scale_inv * b_scale_inv), fp32 accumulation: a and b contiguous FP8
     codes as fp8_quantize returns them, (e4m3, e4m3) or (e5m2, e4m3); the scales fp32 [1] device tensors. `out` (bf16, unit
     inner stride) may be a strided view; `accumulate` adds into it with one rounding. bias (bf16 [n], contiguous), epilogue
-    and aux (bf16 [m, n], unit inner stride) as in `gemm`: scaled product (+ bias) -> aux -> activation -> (+ out)."""
+    and aux (bf16 [m, n], unit inner stride) as in `gemm`: scaled product (+ bias) -> aux -> activation -> (+ out).
+    store_transposed: out is [n, m] and receives the result transposed, bit for bit (fsb_gemm_fp8_t, a GPT-2 Conv1D's
+    [in, out] weight gradient from dy^T and x^T codes): (e5m2, e4m3) codes only, m a multiple of 8, any n; bias, epilogue
+    and aux are refused."""
+    op = "gemm_fp8_t" if store_transposed else "gemm_fp8"
     _chk(a_scale_inv, torch.float32, "a_scale_inv"); _chk(b_scale_inv, torch.float32, "b_scale_inv")
     for t, name in ((a, "a"), (b, "b")):
         _chk(t, None, name)
-        if t.dtype not in _FP8_CODE: raise RuntimeError(f"fsb200 gemm_fp8: {name} must hold FP8 codes, got {t.dtype}")
-        if t.dim() != 2 or not t.is_contiguous(): raise RuntimeError(f"fsb200 gemm_fp8: {name} must be contiguous 2-D")
+        if t.dtype not in _FP8_CODE: raise RuntimeError(f"fsb200 {op}: {name} must hold FP8 codes, got {t.dtype}")
+        if t.dim() != 2 or not t.is_contiguous(): raise RuntimeError(f"fsb200 {op}: {name} must be contiguous 2-D")
     m, k = a.shape
     n = b.shape[0]
-    if b.shape[1] != k: raise RuntimeError(f"fsb200 gemm_fp8: K mismatch {k} vs {b.shape[1]}")
+    if b.shape[1] != k: raise RuntimeError(f"fsb200 {op}: K mismatch {k} vs {b.shape[1]}")
+    shape = (n, m) if store_transposed else (m, n)
     if out is None:
-        if accumulate: raise RuntimeError("fsb200 gemm_fp8: accumulate needs an existing `out`")
-        out = torch.empty((m, n), dtype=_bf16, device=a.device)
+        if accumulate: raise RuntimeError(f"fsb200 {op}: accumulate needs an existing `out`")
+        out = torch.empty(shape, dtype=_bf16, device=a.device)
     _chk(out, _bf16, "out")
     orr, occ, ldd = _rows2d(out, "out")
-    if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_fp8: out shape {tuple(out.shape)} != ({m},{n})")
+    if (orr, occ) != shape: raise RuntimeError(f"fsb200 {op}: out shape {tuple(out.shape)} != ({shape[0]},{shape[1]})")
     if bias is not None:
         _chk(bias, _bf16, "bias")
-        if bias.numel() != n or not bias.is_contiguous(): raise RuntimeError(f"fsb200 gemm_fp8: bias must be contiguous [{n}]")
+        if bias.numel() != n or not bias.is_contiguous(): raise RuntimeError(f"fsb200 {op}: bias must be contiguous [{n}]")
     ldaux = 0
     if aux is not None:
         _chk(aux, _bf16, "aux")
-        if tuple(aux.shape) != (m, n): raise RuntimeError(f"fsb200 gemm_fp8: aux shape {tuple(aux.shape)} != ({m},{n})")
+        if tuple(aux.shape) != (m, n): raise RuntimeError(f"fsb200 {op}: aux shape {tuple(aux.shape)} != ({m},{n})")
         _, _, ldaux = _rows2d(aux, "aux")
-    L.call("fsb_gemm_fp8", m, n, k, _p(a), _FP8_CODE[a.dtype], _p(a_scale_inv), _p(b), _FP8_CODE[b.dtype], _p(b_scale_inv),
+    L.call("fsb_" + op, m, n, k, _p(a), _FP8_CODE[a.dtype], _p(a_scale_inv), _p(b), _FP8_CODE[b.dtype], _p(b_scale_inv),
            _p(out), ldd, _p(bias), epilogue, int(bool(accumulate)), _p(aux), ldaux, _stream(),
            tag=(f"{m}x{n}x{k} epi{epilogue} acc{int(bool(accumulate))}{' bias' if bias is not None else ''}"
                 f"{' aux' if aux is not None else ''}") if L.call_profiler is not None else None)

@@ -130,7 +130,7 @@ size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
                    void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
-/* ---- FP8 training GEMM (opt-in `fp8=True`: LLaMA, BERT, MegatronBERT, mT5) ------------------------------------------
+/* ---- FP8 training GEMM (opt-in `fp8=True`: LLaMA, BERT, MegatronBERT, mT5, GPT-2) -----------------------------------
  * The "hybrid" recipe with just-in-time ("current") per-tensor scaling: activations and weights are e4m3 (largest finite
  * value 448), gradients e5m2 (57344); accumulation is fp32, outputs bf16.
  *
@@ -156,13 +156,24 @@ int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, 
  *   D bf16 [m, n], row stride ldd >= n a multiple of 8. Requirements: k % 16 == 0, n % 8 == 0, a / b / d / bias / aux
  *   16-byte aligned, ldaux >= n a multiple of 8;
  *   any m >= 1; rows of D at or beyond m and columns beyond n are not written. Persistent 128 x 128 tiles on the SMs that
- *   fsb_set_reserved_sms leaves to GEMMs, no K-split: deterministic (the result does not depend on the grid). */
+ *   fsb_set_reserved_sms leaves to GEMMs, no K-split: deterministic (the result does not depend on the grid).
+ * fsb_gemm_fp8_t: D[n, m] (+)= bf16((sum_k A[m, k] B[n, k]) * a_scale_inv * b_scale_inv), the transpose of what fsb_gemm_fp8
+ *   writes for the same operands, bit for bit (same main loop, promotion, tile schedule and device-memory scales; with
+ *   `accumulate`, the fp32 sum with the old D[n, m] is rounded once). It is the weight gradient of a GPT-2 Conv1D, whose
+ *   weight is stored [in, out]: D = dW = x^T dy = (dy^T x)^T from A = dy^T, e5m2 codes [out, tokens], and B = x^T, e4m3
+ *   codes [in, tokens]. Only the pair (a_fmt, b_fmt) = (E5M2, E4M3); bias and aux must be NULL and epilogue FSB_EPI_NONE
+ *   (ldaux is ignored); anything else is an error. D bf16 [n, m], row stride ldd >= m a multiple of 8, so m % 8 == 0; any
+ *   n >= 1 (fsb_gemm_fp8's bounds swapped). k % 16 == 0, a / b / d 16-byte aligned. Ragged tile edges on both axes are
+ *   clipped: nothing outside D[:n, :m] of the strided view is read or written. */
 typedef enum { FSB_FP8_E4M3 = 0, FSB_FP8_E5M2 = 1 } fsb_fp8_format;
 int fsb_fp8_quantize(const void* x, int64_t ldx, int64_t rows, int64_t cols, int fmt, void* y, void* yt, float* scale_inv,
                      float* amax, fsb_stream_t stream);
 int fsb_gemm_fp8(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv, const void* b,
                  int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, const void* bias, int epilogue, int accumulate,
                  void* aux, int64_t ldaux, fsb_stream_t stream);
+int fsb_gemm_fp8_t(int64_t m, int64_t n, int64_t k, const void* a, int a_fmt, const float* a_scale_inv, const void* b,
+                   int b_fmt, const float* b_scale_inv, void* d, int64_t ldd, const void* bias, int epilogue, int accumulate,
+                   void* aux, int64_t ldaux, fsb_stream_t stream);
 
 /* ---- RMSNorm / LayerNorm ------------------------------------------------------------------------------------
  * RMSNorm.forward fengshen/models/megatron/layers/norms.py:44-52 (y = scale * cast(x * rsqrt(mean(x^2) + eps)), the cast to

@@ -29,7 +29,19 @@
 2. A C5-width step at reduced depth (12 encoder and 12 decoder layers, vocabulary 32600, encoder and decoder length 512,
    micro-batch 32, span-corruption-shaped labels) at dropout 0 and 0.1, fp8 and bf16 alternated as above.
 
-  python tools/bench_fp8.py [--model llama|megatronbert|t5] [--reps 3] [--steps 6] [--warmup 2] [--skip-kernels]
+--model gpt2 measures GPT-2 / Wenzhong, whose Conv1D weights are [in, out]:
+1. Kernels at C2 width (hidden 768, 32 x 1024 token rows) and at the 3.5B Wenzhong / Yuyuan width (hidden 3072, 4 x 1024
+   rows), for each projection (c_attn, attn.c_proj, c_fc with bias + gelu_new + pre-activation aux, mlp.c_proj) in the
+   three roles, each against the bf16 GEMM in the layout the bf16 model runs (forward NN, dgrad NT, wgrad TN). The forward
+   carries the bias on every projection. The weight gradient runs fsb_gemm_fp8_t (the transposed store into [in, out]); a
+   second row times plain fsb_gemm_fp8 on the same operands (its [out, in] result), so the transposed epilogue's cost
+   stands alone.
+2. Steps, ZeRO-2 on one GPU, fp8 and bf16 alternated as above: C2 width at 12 layers, 32 x 1024, dropout 0 and 0.1; the
+   3.5B width at 8 layers, seq 1024 x micro-batch 1, 2, 4; all 30 layers at micro-batch 1. Model TFLOP/s from
+   bench.flops_per_token. Then, per precision, the largest micro-batch at which 30 layers train, tried in increasing
+   order from 1 and stopped at the first out-of-memory error.
+
+  python tools/bench_fp8.py [--model llama|megatronbert|t5|gpt2] [--reps 3] [--steps 6] [--warmup 2] [--skip-kernels]
                             [--skip-step] [--out DIR]
 
 Prints one JSON line per measurement, the card's name, power limit and max SM clock first; --out also writes them to
@@ -50,11 +62,13 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch  # noqa: E402
 
 import __graft_entry__  # noqa: E402,F401  (puts the package on sys.path)
+import bench  # noqa: E402  (read only: workload, flops_per_token)
 from bench_int8 import card, graph_us  # noqa: E402
 from fsb200 import lib as L  # noqa: E402
 from fsb200 import ops  # noqa: E402
 from fsb200.engine import ZeroEngine  # noqa: E402
 from fsb200.models.bert import MegatronBertForPreTraining  # noqa: E402
+from fsb200.models.gpt2 import GPT2LMHeadModel  # noqa: E402
 from fsb200.models.llama import LlamaForCausalLM  # noqa: E402
 from fsb200.models.t5 import MT5ForConditionalGeneration  # noqa: E402
 
@@ -71,6 +85,10 @@ C5_PROJ = (("qkv", 3 * C5_INNER, C5_D, L.EPI_NONE, False), ("o", C5_D, C5_INNER,
            ("cq", C5_INNER, C5_D, L.EPI_NONE, False), ("ckv", 2 * C5_INNER, C5_D, L.EPI_NONE, False),
            ("wi", 2 * C5_FF, C5_D, L.EPI_NONE, False), ("wo", C5_D, C5_FF, L.EPI_NONE, False))
 HBM, PEAK_FP8, PEAK_BF16 = 3.35e12, 1979e12, 989e12
+# GPT-2 (name, out, in, forward epilogue, forward writes aux) at hidden h; every projection has a bias
+GPT2_PROJ = lambda h: (("c_attn", 3 * h, h, L.EPI_NONE, False), ("attn_proj", h, h, L.EPI_NONE, False),
+                       ("c_fc", 4 * h, h, L.EPI_GELU_TANH, True), ("mlp_proj", h, 4 * h, L.EPI_NONE, False))
+GPT2_WIDTHS = (("c2", 768, 32 * 1024), ("3.5b", 3072, 4 * 1024))
 
 
 def emit(rec, sink):
@@ -125,6 +143,59 @@ def kernels(reps, sink, proj=tuple(p + (L.EPI_NONE, False) for p in PROJ), T=T, 
             torch.cuda.empty_cache()
 
 
+def gpt2_kernels(reps, sink):
+    """GPT-2's Conv1D roles: the bf16 GEMM in the bf16 model's layouts (weight [in, out]) against the FP8 GEMMs on the codes
+    Fp8Conv1D passes. wgrad: fsb_gemm_fp8_t into [in, out]; wgrad_plain: fsb_gemm_fp8 on the same operands into [out, in]."""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    for width, h, T in GPT2_WIDTHS:
+        for name, n_out, k_in, epi, with_aux in GPT2_PROJ(h):
+            x = torch.randn((T, k_in), device="cuda", generator=g).to(torch.bfloat16)
+            w = (torch.randn((k_in, n_out), device="cuda", generator=g) * 0.02).to(torch.bfloat16)   # Conv1D [in, out]
+            dy = (torch.randn((T, n_out), device="cuda", generator=g) * 1e-3).to(torch.bfloat16)
+            bv = (torch.randn(n_out, device="cuda", generator=g) * 0.1).to(torch.bfloat16)
+            aux = torch.empty((T, n_out), dtype=torch.bfloat16, device="cuda") if with_aux else None
+            xq, xt, sx = ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=True)
+            wq, wt, sw = ops.fp8_quantize(w, "e4m3", rowwise=True, colwise=True)
+            dyq, dyt, sdy = ops.fp8_quantize(dy, "e5m2", rowwise=True, colwise=True)
+            y = torch.empty((T, n_out), dtype=torch.bfloat16, device="cuda")
+            dx = torch.empty((T, k_in), dtype=torch.bfloat16, device="cuda")
+            dw = torch.empty((k_in, n_out), dtype=torch.bfloat16, device="cuda")
+            dwt = torch.empty((n_out, k_in), dtype=torch.bfloat16, device="cuda")
+            roles = (
+                ("fwd", (T, n_out, k_in), lambda: ops.gemm(L.GEMM_NN, x, w, out=y, bias=bv, epilogue=epi, aux=aux),
+                 lambda: ops.gemm_fp8(xq, sx, wt, sw, out=y, bias=bv, epilogue=epi, aux=aux),
+                 lambda: ops.fp8_quantize(x, "e4m3", rowwise=True, colwise=True)),
+                ("dgrad", (T, k_in, n_out), lambda: ops.gemm(L.GEMM_NT, dy, w, out=dx),
+                 lambda: ops.gemm_fp8(dyq, sdy, wq, sw, out=dx),
+                 lambda: ops.fp8_quantize(dy, "e5m2", rowwise=True, colwise=True)),
+                ("wgrad", (n_out, k_in, T), lambda: ops.gemm(L.GEMM_TN, x, dy, out=dw),
+                 lambda: ops.gemm_fp8(dyt, sdy, xt, sx, out=dw, store_transposed=True), None),
+                ("wgrad_plain", (n_out, k_in, T), lambda: ops.gemm(L.GEMM_TN, x, dy, out=dw),
+                 lambda: ops.gemm_fp8(dyt, sdy, xt, sx, out=dwt), None))
+            for role, (m, n, k), bf, f8, q8 in roles:
+                t8, t16, tq = [], [], []
+                for _ in range(reps):
+                    t8.append(graph_us(f8)); t16.append(graph_us(bf))
+                    if q8 is not None:
+                        tq.append(graph_us(q8, calls=20))
+                flops = 2.0 * m * n * k
+                u8, u16 = statistics.median(t8), statistics.median(t16)
+                rec = dict(kind="gemm", model="gpt2", width=width, proj=name, role=role, m=m, n=n, k=k,
+                           epilogue=epi if role == "fwd" else L.EPI_NONE, aux=role == "fwd" and with_aux,
+                           fp8_us=round(u8, 1), fp8_us_all=[round(v, 1) for v in t8],
+                           bf16_us=round(u16, 1), bf16_us_all=[round(v, 1) for v in t16],
+                           fp8_tflops=round(flops / u8 / 1e6, 1), bf16_tflops=round(flops / u16 / 1e6, 1),
+                           speedup=round(u16 / u8, 3))
+                if tq:
+                    rows, cols = (T, k_in) if role == "fwd" else (T, n_out)
+                    qbytes = 2 * (2 * rows * cols) + 2 * rows * cols
+                    uq = statistics.median(tq)
+                    rec.update(quantize_us=round(uq, 1), quantize_gbs=round(qbytes / uq / 1e3, 1))
+                emit(rec, sink)
+            del x, w, dy, bv, aux, xq, xt, wq, wt, dyq, dyt, y, dx, dw, dwt
+            torch.cuda.empty_cache()
+
+
 def _scratch_bytes():
     return sum(b.numel() * b.element_size() for b in ops._ws_cache.values())
 
@@ -173,6 +244,55 @@ def _t5(fp8, dropout):
         dict(layers=nl, batch=B, seq=S)
 
 
+def _gpt2_shape(layers, h, heads, B, S=1024):
+    """A GPT-2 step builder: Wenzhong's vocabulary (50257 padded to 50304), `layers` blocks at hidden h, seq S, micro-batch
+    B, random ids."""
+    def build(fp8, dropout):
+        w = dict(bench.workload("gpt2-110m"), n_layer=layers, n_embd=h, n_head=heads, vocab_size=50304, n_positions=1024)
+        cfg = SimpleNamespace(vocab_size=w["vocab_size"], n_positions=w["n_positions"], n_embd=h, n_layer=layers,
+                              n_head=heads, layer_norm_epsilon=1e-5, initializer_range=0.02, resid_pdrop=dropout,
+                              embd_pdrop=dropout, attn_pdrop=dropout, activation_function="gelu_new")
+        g = torch.Generator(device="cuda").manual_seed(1)
+        ids = torch.randint(0, w["vocab_size"], (B, S), device="cuda", generator=g)
+        return GPT2LMHeadModel(cfg, device="cuda", fp8=fp8), dict(input_ids=ids, labels=ids), \
+            dict(layers=layers, batch=B, seq=S, model_tflops_per_token=bench.flops_per_token(dict(w, seq=S)))
+    build.gpt2 = dict(model="gpt2", width=h)
+    return build
+
+
+def gpt2_largest_micro_batch(fp8, sink, layers=30, limit=64):
+    """The largest micro-batch at which `layers` 3.5B-width blocks run a step (ZeRO-2, one GPU), trying 1, 2, ... and
+    stopping at the first out-of-memory error."""
+    best, reason = 0, None
+    gc.collect()
+    torch.cuda.empty_cache()
+    base, ws0 = torch.cuda.memory_allocated(), _scratch_bytes()
+    for B in range(1, limit + 1):
+        model = eng = batch = loss = None
+        try:
+            model, batch, _ = _gpt2_shape(layers, 3072, 32, B)(fp8, 0.0)
+            eng = ZeroEngine(model, lr=1e-4, stage=2)
+            loss = model(**batch).loss
+            loss.backward()
+            eng.backward_done()
+            eng.step()
+            torch.cuda.synchronize()
+            best = B
+        except torch.cuda.OutOfMemoryError as e:
+            reason = str(e).splitlines()[0]
+            break
+        finally:
+            # the loss's autograd graph holds the model: drop it too, or the next try starts beside this one
+            del model, eng, batch, loss
+            gc.collect()
+            torch.cuda.empty_cache()
+    left = torch.cuda.memory_allocated() - base - (_scratch_bytes() - ws0)
+    if left > 64 << 20:
+        raise SystemExit(f"bench_fp8: {left} bytes still allocated after the micro-batch search")
+    emit(dict(kind="largest_micro_batch", model="gpt2", width=3072, layers=layers, seq=1024, fp8=fp8, micro_batch=best,
+              stopped_by=reason), sink)
+
+
 def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
     gc.collect()
     torch.cuda.empty_cache()
@@ -180,6 +300,7 @@ def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
     model, batch, shape = build(fp8, dropout)
     B, S = shape["batch"], shape["seq"]
     eng = ZeroEngine(model, lr=1e-4)
+    per_token = shape.pop("model_tflops_per_token", None)
     losses = []
 
     def one():
@@ -199,6 +320,9 @@ def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     extra = {_megatronbert: dict(model="megatronbert", dropout=dropout), _t5: dict(model="t5", dropout=dropout)}.get(build, {})
+    if hasattr(build, "gpt2"):
+        extra = dict(build.gpt2, dropout=dropout, zero_stage=2,
+                     model_tflops=round(B * S * steps / dt * per_token / 1e12, 1))
     rec = dict(kind="step", **extra, fp8=fp8, **shape, steps=steps,
                tokens_per_s=round(B * S * steps / dt),
                step_ms=round(1e3 * dt / steps, 1), peak_alloc_gib=round(torch.cuda.max_memory_allocated() / 2 ** 30, 2),
@@ -219,7 +343,7 @@ def step(fp8, steps, warmup, sink, build=_llama, dropout=0.0):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=("llama", "megatronbert", "t5"), default="llama")
+    ap.add_argument("--model", choices=("llama", "megatronbert", "t5", "gpt2"), default="llama")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--steps", type=int, default=6)
     ap.add_argument("--warmup", type=int, default=2)
@@ -231,15 +355,26 @@ def main():
         raise SystemExit("bench_fp8: needs a CUDA device")
     sink = []
     emit(dict(kind="card", **card()), sink)
-    bert, t5 = a.model == "megatronbert", a.model == "t5"
+    bert, t5, gpt2 = a.model == "megatronbert", a.model == "t5", a.model == "gpt2"
     if not a.skip_kernels:
-        if bert:
+        if gpt2:
+            gpt2_kernels(a.reps, sink)
+        elif bert:
             kernels(a.reps, sink, C3_PROJ, C3_T, bias=True)
         elif t5:
             kernels(a.reps, sink, C5_PROJ, C5_T)
         else:
             kernels(a.reps, sink)
-    if not a.skip_step:
+    if not a.skip_step and gpt2:
+        runs = [(_gpt2_shape(12, 768, 12, 32), p) for p in (0.0, 0.1)] + \
+               [(_gpt2_shape(8, 3072, 32, B), 0.0) for B in (1, 2, 4)] + [(_gpt2_shape(30, 3072, 32, 1), 0.0)]
+        for build, dropout in runs:
+            for r in range(a.reps):
+                for fp8 in ((True, False) if r % 2 == 0 else (False, True)):
+                    step(fp8, a.steps, a.warmup, sink, build, dropout)
+        for fp8 in (False, True):
+            gpt2_largest_micro_batch(fp8, sink)
+    elif not a.skip_step:
         build = _megatronbert if bert else _t5 if t5 else _llama
         for dropout in ((0.0, 0.1) if bert or t5 else (0.0,)):
             for r in range(a.reps):
