@@ -36,8 +36,8 @@ struct AttBwdParams {
   int seq_q, seq_kv, nheads, batch, causal;
   float scale, scale_log2;
   DropArgs drop;             // attention-probability dropout (kDropout only): the forward's seed, stream base and site
-  const int *seg_start, *seg_end;   // [batch, seq] segment bounds of each token (kSeg only; see fsb_sdpa_bwd_segments)
-                                    // kSegCross: the dQ pass gets kv_start / kv_end, the dK / dV pass q_start / q_end
+  const int *seg_start, *seg_end;   // [batch, seq] segment bounds of each token (kSeg only; see the segment forms of fsb_sdpa_bwd)
+                                    // kSegCross: the dQ pass gets seg_start / seg_end, the dK / dV pass q_start / q_end
 };
 
 // The key steps [j0, j1) the dQ tile at q0 visits (attn_bwd_dq_kernel) and so the workspace slots of the bias gradient it
@@ -593,11 +593,17 @@ static inline size_t dbias_part_floats(int64_t batch, int64_t seq_q, int64_t seq
   return size_t(batch) * nheads * n_qt * n_all * AB_DSTRIDE;
 }
 
+// What the launcher reads besides AttBwdParams: the operands of the delta pass and of the tensor maps, the bias gradient and
+// its second workspace part, and the key-side ranges of a cross launch
+struct AttBwdOperands {
+  const void *q, *k, *v, *o, *dout;
+  int64_t q_rs, k_rs, v_rs, o_rs, do_rs, o_hs;
+  float *delta, *drel_bias, *part2;
+  const int *q_start, *q_end;   // kSegCross: the dK / dV pass's ranges
+};
+
 template <int D, bool kBias, bool kDropout, int kSeg = kSegNone>
-static int launch_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                           int64_t q_rs, int64_t k_rs, int64_t v_rs, int64_t o_rs, int64_t do_rs, int64_t o_hs,
-                           float* delta, AttBwdParams& p, float* drel_bias, float* part2, cudaStream_t st,
-                           const int* q_start = nullptr, const int* q_end = nullptr) {
+static int launch_attn_bwd(const AttBwdOperands& a, AttBwdParams& p, cudaStream_t st) {
   using SQ = AttBwdSmem<D, kBias>;
   using SK = AttBwdSmem<D, false>;
   if (int rc = ensure_smem<attn_bwd_dq_kernel<D, kBias, kDropout, kSeg>>(SQ::TOTAL, "sdpa_bwd")) return rc;
@@ -607,38 +613,38 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
     const int64_t groups = int64_t(p.batch) * p.seq_q * p.nheads;
     const int64_t threads = groups * (D == 96 ? 4 : D / 8);   // attn_delta_kernel's G
     attn_delta_kernel<D><<<unsigned((threads + 255) / 256), 256, 0, st>>>(
-        (const __nv_bfloat16*)o, (const __nv_bfloat16*)dout, delta, o_rs, o_hs, do_rs, p.do_head_stride, p.batch, p.seq_q,
-        p.nheads);
+        (const __nv_bfloat16*)a.o, (const __nv_bfloat16*)a.dout, a.delta, a.o_rs, a.o_hs, a.do_rs, p.do_head_stride, p.batch,
+        p.seq_q, p.nheads);
     FSB_CUDA_LAUNCH_CHECK();
   }
   CUtensorMap tq128, tdo128, tk64, tv64, tk128, tv128, tq64, tdo64;
   int rc;
   const int64_t wq = int64_t(p.nheads - 1) * p.q_head_stride + D, wk = int64_t(p.nheads - 1) * p.k_head_stride + D;
   const int64_t wv = int64_t(p.nheads - 1) * p.v_head_stride + D, wdo = int64_t(p.nheads - 1) * p.do_head_stride + D;
-  if ((rc = make_attn_tmap(&tq128, q, q_rs, wq, p.seq_q, p.batch, AB_BM))) return rc;
-  if ((rc = make_attn_tmap(&tdo128, dout, do_rs, wdo, p.seq_q, p.batch, AB_BM))) return rc;
-  if ((rc = make_attn_tmap(&tk64, k, k_rs, wk, p.seq_kv, p.batch, AB_BN))) return rc;
-  if ((rc = make_attn_tmap(&tv64, v, v_rs, wv, p.seq_kv, p.batch, AB_BN))) return rc;
-  if ((rc = make_attn_tmap(&tk128, k, k_rs, wk, p.seq_kv, p.batch, AB_BM))) return rc;
-  if ((rc = make_attn_tmap(&tv128, v, v_rs, wv, p.seq_kv, p.batch, AB_BM))) return rc;
-  if ((rc = make_attn_tmap(&tq64, q, q_rs, wq, p.seq_q, p.batch, AB_BN))) return rc;
-  if ((rc = make_attn_tmap(&tdo64, dout, do_rs, wdo, p.seq_q, p.batch, AB_BN))) return rc;
+  if ((rc = make_attn_tmap(&tq128, a.q, a.q_rs, wq, p.seq_q, p.batch, AB_BM))) return rc;
+  if ((rc = make_attn_tmap(&tdo128, a.dout, a.do_rs, wdo, p.seq_q, p.batch, AB_BM))) return rc;
+  if ((rc = make_attn_tmap(&tk64, a.k, a.k_rs, wk, p.seq_kv, p.batch, AB_BN))) return rc;
+  if ((rc = make_attn_tmap(&tv64, a.v, a.v_rs, wv, p.seq_kv, p.batch, AB_BN))) return rc;
+  if ((rc = make_attn_tmap(&tk128, a.k, a.k_rs, wk, p.seq_kv, p.batch, AB_BM))) return rc;
+  if ((rc = make_attn_tmap(&tv128, a.v, a.v_rs, wv, p.seq_kv, p.batch, AB_BM))) return rc;
+  if ((rc = make_attn_tmap(&tq64, a.q, a.q_rs, wq, p.seq_q, p.batch, AB_BN))) return rc;
+  if ((rc = make_attn_tmap(&tdo64, a.dout, a.do_rs, wdo, p.seq_q, p.batch, AB_BN))) return rc;
   // 2. dQ
   {
     dim3 grid((p.seq_q + AB_BM - 1) / AB_BM, p.nheads, p.batch);
     attn_bwd_dq_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SQ::TOTAL, st>>>(tq128, tdo128, tk64, tv64, p);
     FSB_CUDA_LAUNCH_CHECK();
-    if (kBias && drel_bias != nullptr) {   // (only the bias kernels instantiate a reduction)
+    if (kBias && a.drel_bias != nullptr) {   // (only the bias kernels instantiate a reduction)
       const int n_rel = p.seq_q + p.seq_kv - 1, bs = dbias_bsplit(p.batch);
       attn_dbias_reduce_kernel<kBias ? kSeg : kSegNone><<<dim3((n_rel + 127) / 128, p.nheads, bs), 128, 0, st>>>(
-          p.dbias_part, part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), bs, p.seg_start, p.seg_end);
+          p.dbias_part, a.part2, p.batch, p.nheads, p.seq_q, p.seq_kv, p.causal, int(grid.x), bs, p.seg_start, p.seg_end);
       FSB_CUDA_LAUNCH_CHECK();
-      attn_dbias_final_kernel<<<dim3((n_rel + 127) / 128, p.nheads), 128, 0, st>>>(part2, drel_bias, p.nheads, n_rel, bs);
+      attn_dbias_final_kernel<<<dim3((n_rel + 127) / 128, p.nheads), 128, 0, st>>>(a.part2, a.drel_bias, p.nheads, n_rel, bs);
       FSB_CUDA_LAUNCH_CHECK();
     }
   }
   // 3. dK, dV
-  if constexpr (kSeg == kSegCross) { p.seg_start = q_start; p.seg_end = q_end; }   // the key-side ranges
+  if constexpr (kSeg == kSegCross) { p.seg_start = a.q_start; p.seg_end = a.q_end; }   // the key-side ranges
   {
     dim3 grid((p.seq_kv + AB_BM - 1) / AB_BM, p.nheads, p.batch);
     attn_bwd_dkv_kernel<D, kBias, kDropout, kSeg><<<grid, AB_THREADS, SK::TOTAL, st>>>(tk128, tv128, tq64, tdo64, p);
@@ -651,21 +657,25 @@ static int launch_attn_bwd(const void* q, const void* k, const void* v, const vo
 
 using namespace fsb;
 
-static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
-                    float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads,
-                    int head_dim, int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                    int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                    int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                    int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                    float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
-                    void* workspace, size_t workspace_bytes, const DropArgs* drop, const int* seg_start,
-                    const int* seg_end, fsb_stream_t st, const int* q_start = nullptr, const int* q_end = nullptr) {
+extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                            const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q,
+                            int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride, int64_t k_row_stride,
+                            int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
+                            int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
+                            int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
+                            int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
+                            int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias, void* workspace,
+                            size_t workspace_bytes, const int32_t* seg_start, const int32_t* seg_end,
+                            const int32_t* q_start, const int32_t* q_end, float drop_p, uint64_t seed,
+                            const int64_t* stream_base, int64_t site, fsb_stream_t st) {
+  DropArgs d;
+  if (int rc = make_drop_args(drop_p, seed, stream_base, site, &d)) return rc;
+  AttnForm f;
+  if (int rc = resolve_attn_form("sdpa_bwd", head_dim, causal, kv_mask, rel_bias, seg_start, seg_end, q_start, q_end,
+                                 drop_p, seq_q, seq_kv, &f))
+    return rc;
   FSB_REQUIRE(q && k && v && o && dout && lse && delta && dq && dk && dv, "sdpa_bwd: null pointer");
-  // head_dim 96 only in the causal forms GPT-2 launches (see sdpa_fwd)
-  FSB_REQUIRE(head_dim == 64 || head_dim == 128 || (head_dim == 96 && causal && rel_bias == nullptr && q_start == nullptr),
-              "sdpa_bwd: head_dim %d unsupported (64 or 128; 96 causal without a bias only)", head_dim);
   FSB_REQUIRE(batch > 0 && seq_q > 0 && seq_kv > 0 && nheads > 0 && batch < 65536 && nheads < 65536, "sdpa_bwd: bad dims");
-  FSB_REQUIRE(!causal || seq_q == seq_kv, "sdpa_bwd: causal needs seq_q == seq_kv");
   FSB_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) &&
                   aligned16(dk) && aligned16(dv),
               "sdpa_bwd: 16-byte alignment required");
@@ -677,14 +687,15 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   AttBwdParams p;
   p.lse = lse; p.delta = delta; p.kv_mask = kv_mask;
   p.rel_bias = rel_bias; p.dbias_part = nullptr;
-  float* part2 = nullptr;
+  AttBwdOperands a = {q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride, do_row_stride,
+                      o_head_stride, delta, drel_bias, nullptr, q_start, q_end};
   if (drel_bias != nullptr) {
     const size_t need = fsb_sdpa_bwd_workspace_bytes(batch, seq_q, seq_kv, nheads);
     FSB_REQUIRE(workspace != nullptr && workspace_bytes >= need && aligned16(workspace),
                 "sdpa_bwd: the bias gradient needs a %zu-byte workspace (fsb_sdpa_bwd_workspace_bytes); got %zu", need,
                 workspace_bytes);
     p.dbias_part = static_cast<float*>(workspace);
-    part2 = p.dbias_part + dbias_part_floats(batch, seq_q, seq_kv, nheads);
+    a.part2 = p.dbias_part + dbias_part_floats(batch, seq_q, seq_kv, nheads);
   }
   p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
   p.dq_row_stride = dq_row_stride; p.dk_row_stride = dk_row_stride; p.dv_row_stride = dv_row_stride;
@@ -694,247 +705,36 @@ static int sdpa_bwd(const void* q, const void* k, const void* v, const void* o, 
   p.seq_q = int(seq_q); p.seq_kv = int(seq_kv); p.nheads = nheads; p.batch = int(batch); p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.seg_start = seg_start; p.seg_end = seg_end;
-  if (q_start != nullptr) {   // fsb_sdpa_bwd_segments_cross: head_dim 64, no bias, no key mask
-    if (drop != nullptr) {
-      p.drop = *drop;
-      return launch_attn_bwd<64, false, true, kSegCross>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                         nullptr, (cudaStream_t)st, q_start, q_end);
-    }
-    return launch_attn_bwd<64, false, false, kSegCross>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                        o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                        nullptr, (cudaStream_t)st, q_start, q_end);
+  if (f.dropout) p.drop = d;
+  const cudaStream_t s = (cudaStream_t)st;
+  switch (f.key()) {
+    case AttnForm{64, false, false, kSegNone}.key(): return launch_attn_bwd<64, false, false>(a, p, s);
+    case AttnForm{64, false, true, kSegNone}.key(): return launch_attn_bwd<64, false, true>(a, p, s);
+    case AttnForm{64, true, false, kSegNone}.key(): return launch_attn_bwd<64, true, false>(a, p, s);
+    case AttnForm{64, true, true, kSegNone}.key(): return launch_attn_bwd<64, true, true>(a, p, s);
+    case AttnForm{96, false, false, kSegNone}.key(): return launch_attn_bwd<96, false, false>(a, p, s);
+    case AttnForm{96, false, true, kSegNone}.key(): return launch_attn_bwd<96, false, true>(a, p, s);
+    case AttnForm{128, false, false, kSegNone}.key(): return launch_attn_bwd<128, false, false>(a, p, s);
+    case AttnForm{128, false, true, kSegNone}.key(): return launch_attn_bwd<128, false, true>(a, p, s);
+    case AttnForm{128, true, false, kSegNone}.key(): return launch_attn_bwd<128, true, false>(a, p, s);
+    case AttnForm{128, true, true, kSegNone}.key(): return launch_attn_bwd<128, true, true>(a, p, s);
+    case AttnForm{64, false, false, kSegCausal}.key(): return launch_attn_bwd<64, false, false, kSegCausal>(a, p, s);
+    case AttnForm{64, false, true, kSegCausal}.key(): return launch_attn_bwd<64, false, true, kSegCausal>(a, p, s);
+    case AttnForm{64, true, false, kSegCausal}.key(): return launch_attn_bwd<64, true, false, kSegCausal>(a, p, s);
+    case AttnForm{64, true, true, kSegCausal}.key(): return launch_attn_bwd<64, true, true, kSegCausal>(a, p, s);
+    case AttnForm{96, false, false, kSegCausal}.key(): return launch_attn_bwd<96, false, false, kSegCausal>(a, p, s);
+    case AttnForm{96, false, true, kSegCausal}.key(): return launch_attn_bwd<96, false, true, kSegCausal>(a, p, s);
+    case AttnForm{128, false, false, kSegCausal}.key(): return launch_attn_bwd<128, false, false, kSegCausal>(a, p, s);
+    case AttnForm{64, false, false, kSegBidir}.key(): return launch_attn_bwd<64, false, false, kSegBidir>(a, p, s);
+    case AttnForm{64, false, true, kSegBidir}.key(): return launch_attn_bwd<64, false, true, kSegBidir>(a, p, s);
+    case AttnForm{64, true, false, kSegBidir}.key(): return launch_attn_bwd<64, true, false, kSegBidir>(a, p, s);
+    case AttnForm{64, true, true, kSegBidir}.key(): return launch_attn_bwd<64, true, true, kSegBidir>(a, p, s);
+    case AttnForm{64, false, false, kSegCross}.key(): return launch_attn_bwd<64, false, false, kSegCross>(a, p, s);
+    case AttnForm{64, false, true, kSegCross}.key(): return launch_attn_bwd<64, false, true, kSegCross>(a, p, s);
   }
-#define FSB_BWD_SEG(DR, SEG)                                                                                             \
-  launch_attn_bwd<64, true, DR, SEG>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,          \
-                                     do_row_stride, o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
-  if (seg_start != nullptr && rel_bias != nullptr) {   // fsb_sdpa_bwd_segments_bias: head_dim 64, no key mask
-    if (drop != nullptr) {
-      p.drop = *drop;
-      return causal ? FSB_BWD_SEG(true, kSegCausal) : FSB_BWD_SEG(true, kSegBidir);
-    }
-    return causal ? FSB_BWD_SEG(false, kSegCausal) : FSB_BWD_SEG(false, kSegBidir);
-  }
-#undef FSB_BWD_SEG
-  if (seg_start != nullptr && !causal) {   // fsb_sdpa_bwd_segments_bidirectional: head_dim 64, no bias, no key mask
-    if (drop != nullptr) {
-      p.drop = *drop;
-      return launch_attn_bwd<64, false, true, kSegBidir>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                         nullptr, (cudaStream_t)st);
-    }
-    return launch_attn_bwd<64, false, false, kSegBidir>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                        o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                        nullptr, (cudaStream_t)st);
-  }
-  if (seg_start != nullptr && drop != nullptr) {   // fsb_sdpa_bwd_segments_dropout with p > 0: head_dim 64 or 96
-    p.drop = *drop;
-    if (head_dim == 96)
-      return launch_attn_bwd<96, false, true, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                          o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                          nullptr, (cudaStream_t)st);
-    return launch_attn_bwd<64, false, true, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride,
-                                                  do_row_stride, o_head_stride, delta, p, nullptr, nullptr, (cudaStream_t)st);
-  }
-  if (seg_start != nullptr && head_dim == 96)   // fsb_sdpa_bwd_segments_dropout at head_dim 96 with p == 0
-    return launch_attn_bwd<96, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                         nullptr, (cudaStream_t)st);
-  if (seg_start != nullptr)   // fsb_sdpa_bwd_segments: causal, no bias, no dropout, no key mask
-    return head_dim == 128
-               ? launch_attn_bwd<128, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                          o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                          nullptr, (cudaStream_t)st)
-               : launch_attn_bwd<64, false, false, kSegCausal>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride,
-                                                         o_row_stride, do_row_stride, o_head_stride, delta, p, nullptr,
-                                                         nullptr, (cudaStream_t)st);
-#define FSB_BWD(DD, BB, DR)                                                                                              \
-  launch_attn_bwd<DD, BB, DR>(q, k, v, o, dout, q_row_stride, k_row_stride, v_row_stride, o_row_stride, do_row_stride,       \
-                          o_head_stride, delta, p, drel_bias, part2, (cudaStream_t)st)
-  if (drop != nullptr) {
-    p.drop = *drop;
-    if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, true) : FSB_BWD(64, true, true);
-    if (head_dim == 96) return FSB_BWD(96, false, true);
-    return head_dim == 128 ? FSB_BWD(128, false, true) : FSB_BWD(64, false, true);
-  }
-  if (rel_bias != nullptr) return head_dim == 128 ? FSB_BWD(128, true, false) : FSB_BWD(64, true, false);
-  if (head_dim == 96) return FSB_BWD(96, false, false);
-  return head_dim == 128 ? FSB_BWD(128, false, false) : FSB_BWD(64, false, false);
-#undef FSB_BWD
-}
-
-extern "C" int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                            const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch, int64_t seq_q,
-                            int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride, int64_t k_row_stride,
-                            int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
-                            int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                            int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                            int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
-                            int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias, void* workspace,
-                            size_t workspace_bytes, fsb_stream_t st) {
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
-                  nullptr, nullptr, nullptr, st);
-}
-
-extern "C" int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                    const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
-                                    int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
-                                    int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                    int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
-                                    int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                                    int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                                    int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
-                                    int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
-                                    void* workspace, size_t workspace_bytes, float p, uint64_t seed,
-                                    const int64_t* stream_base, int64_t site, fsb_stream_t st) {
-  DropArgs d;
-  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  // causal composes with p > 0 as in fsb_sdpa_fwd_dropout: masked elements have P = 0, so their keep bits never matter
-  if (p > 0.f)
-    FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536, "sdpa_bwd_dropout: sequences longer than 65536 are not supported with p > 0");
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, causal, kv_mask, rel_bias, drel_bias, workspace, workspace_bytes,
-                  p > 0.f ? &d : nullptr, nullptr, nullptr, st);
-}
-
-extern "C" int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                     const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
-                                     int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
-                                     int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                     int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
-                                     int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                                     int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                                     int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride, float scale,
-                                     const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t st) {
-  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments: null segment bounds");
-  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
-              (long long)seq_kv);
-  // head_dim 96 reaches the same kernels through fsb_sdpa_bwd_segments_dropout (any p, 0 included)
-  FSB_REQUIRE(head_dim == 64 || head_dim == 128, "sdpa_bwd_segments: head_dim %d unsupported (64 or 128)", head_dim);
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, nullptr, seg_start,
-                  seg_end, st);
-}
-
-extern "C" int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                             const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
-                                             int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                             int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
-                                             int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
-                                             int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride,
-                                             int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                             int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride,
-                                             int64_t dv_head_stride, float scale, const int32_t* seg_start,
-                                             const int32_t* seg_end, float p, uint64_t seed, const int64_t* stream_base,
-                                             int64_t site, fsb_stream_t st) {
-  DropArgs d;
-  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_dropout: null segment bounds");
-  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_dropout: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
-              (long long)seq_kv);
-  FSB_REQUIRE(head_dim == 64 || head_dim == 96 || head_dim == 128,
-              "sdpa_bwd_segments_dropout: head_dim %d unsupported (64, 96 or 128)", head_dim);
-  if (p > 0.f) {
-    // GPT-2 (the one model with attention dropout that packs) runs head_dim 64 (110M) or 96 (3.5B); LLaMA has no attention
-    // dropout
-    FSB_REQUIRE(head_dim == 64 || head_dim == 96, "sdpa_bwd_segments_dropout: head_dim %d unsupported with p > 0 (64 or 96)",
-                head_dim);
-    FSB_REQUIRE(seq_q <= 65536, "sdpa_bwd_segments_dropout: sequences longer than 65536 are not supported with p > 0");
-  }
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, 1, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
-                  seg_start, seg_end, st);
-}
-
-extern "C" int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k, const void* v, const void* o,
-                                                   const void* dout, const float* lse, float* delta, void* dq, void* dk,
-                                                   void* dv, int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads,
-                                                   int head_dim, int64_t q_row_stride, int64_t k_row_stride,
-                                                   int64_t v_row_stride, int64_t o_row_stride, int64_t do_row_stride,
-                                                   int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                                                   int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride,
-                                                   int64_t o_head_stride, int64_t do_head_stride, int64_t dq_head_stride,
-                                                   int64_t dk_head_stride, int64_t dv_head_stride, float scale,
-                                                   const int32_t* seg_start, const int32_t* seg_end, float p,
-                                                   uint64_t seed, const int64_t* stream_base, int64_t site,
-                                                   fsb_stream_t st) {
-  DropArgs d;
-  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_bidirectional: null segment bounds");
-  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_bidirectional: needs seq_q == seq_kv (got %lld and %lld)",
-              (long long)seq_q, (long long)seq_kv);
-  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_bidirectional: head_dim %d unsupported (64 only)", head_dim);
-  if (p > 0.f)
-    FSB_REQUIRE(seq_q <= 65536,
-                "sdpa_bwd_segments_bidirectional: sequences longer than 65536 are not supported with p > 0");
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, 0, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
-                  seg_start, seg_end, st);
-}
-
-extern "C" int fsb_sdpa_bwd_segments_bias(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                          const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
-                                          int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
-                                          int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                          int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
-                                          int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                                          int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                                          int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                                          float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
-                                          const float* rel_bias, float* drel_bias, void* workspace,
-                                          size_t workspace_bytes, float p, uint64_t seed, const int64_t* stream_base,
-                                          int64_t site, fsb_stream_t st) {
-  DropArgs d;
-  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  FSB_REQUIRE(seg_start && seg_end, "sdpa_bwd_segments_bias: null segment bounds");
-  FSB_REQUIRE(rel_bias, "sdpa_bwd_segments_bias: null rel_bias");
-  FSB_REQUIRE(seq_q == seq_kv, "sdpa_bwd_segments_bias: needs seq_q == seq_kv (got %lld and %lld)", (long long)seq_q,
-              (long long)seq_kv);
-  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_bias: head_dim %d unsupported (64 only)", head_dim);
-  if (p > 0.f)
-    FSB_REQUIRE(seq_q <= 65536, "sdpa_bwd_segments_bias: sequences longer than 65536 are not supported with p > 0");
-  // drel_bias without a large enough workspace is refused by sdpa_bwd
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, causal ? 1 : 0, nullptr, rel_bias, drel_bias, workspace,
-                  workspace_bytes, p > 0.f ? &d : nullptr, seg_start, seg_end, st);
-}
-
-extern "C" int fsb_sdpa_bwd_segments_cross(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                           const float* lse, float* delta, void* dq, void* dk, void* dv, int64_t batch,
-                                           int64_t seq_q, int64_t seq_kv, int nheads, int head_dim, int64_t q_row_stride,
-                                           int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                           int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride,
-                                           int64_t dv_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                                           int64_t v_head_stride, int64_t o_head_stride, int64_t do_head_stride,
-                                           int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                                           float scale, const int32_t* kv_start, const int32_t* kv_end,
-                                           const int32_t* q_start, const int32_t* q_end, float p, uint64_t seed,
-                                           const int64_t* stream_base, int64_t site, fsb_stream_t st) {
-  DropArgs d;
-  if (int rc = make_drop_args(p, seed, stream_base, site, &d)) return rc;
-  FSB_REQUIRE(kv_start && kv_end && q_start && q_end, "sdpa_bwd_segments_cross: null segment bounds");
-  FSB_REQUIRE(head_dim == 64, "sdpa_bwd_segments_cross: head_dim %d unsupported (64 only)", head_dim);
-  if (p > 0.f)
-    FSB_REQUIRE(seq_q <= 65536 && seq_kv <= 65536,
-                "sdpa_bwd_segments_cross: sequences longer than 65536 are not supported with p > 0");
-  return sdpa_bwd(q, k, v, o, dout, lse, delta, dq, dk, dv, batch, seq_q, seq_kv, nheads, head_dim, q_row_stride,
-                  k_row_stride, v_row_stride, o_row_stride, do_row_stride, dq_row_stride, dk_row_stride, dv_row_stride,
-                  q_head_stride, k_head_stride, v_head_stride, o_head_stride, do_head_stride, dq_head_stride,
-                  dk_head_stride, dv_head_stride, scale, 0, nullptr, nullptr, nullptr, nullptr, 0, p > 0.f ? &d : nullptr,
-                  kv_start, kv_end, st, q_start, q_end);
+  set_error("sdpa_bwd: no kernel built for head_dim %d, bias %d, dropout %d, segment mode %d", f.d, f.bias, f.dropout,
+            int(f.seg));
+  return FSB_ERR_INVALID;
 }
 
 extern "C" size_t fsb_sdpa_bwd_workspace_bytes(int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads) {

@@ -165,8 +165,48 @@ int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_
   return make_tmap_bf16(tm, base, 3, dims, strides, box);
 }
 
+int resolve_attn_form(const char* what, int head_dim, int causal, const void* kv_mask, const void* rel_bias,
+                      const int32_t* seg_start, const int32_t* seg_end, const int32_t* q_start, const int32_t* q_end,
+                      float p, int64_t seq_q, int64_t seq_kv, AttnForm* form) {
+  FSB_REQUIRE(!seg_start == !seg_end && !q_start == !q_end && (seg_start || !q_start),
+              "%s: null segment bounds (seg_start / seg_end go together, and q_start / q_end need them)", what);
+  const bool bias = rel_bias != nullptr, dropout = p > 0.f;
+  FSB_REQUIRE(!dropout || (seq_q <= 65536 && seq_kv <= 65536),
+              "%s: sequences longer than 65536 are not supported with p > 0", what);
+  if (!seg_start) {
+    FSB_REQUIRE(!causal || seq_q == seq_kv, "%s: causal needs seq_q == seq_kv", what);
+    // head_dim 96 only in the causal forms GPT-2 3.5B (32 heads x 96) launches, never with a bias
+    FSB_REQUIRE(head_dim == 64 || head_dim == 128 || (head_dim == 96 && causal && !bias),
+                "%s: head_dim %d unsupported (64 or 128; 96 causal without a bias only)", what, head_dim);
+    *form = {head_dim, bias, dropout, kSegNone};
+    return FSB_OK;
+  }
+  FSB_REQUIRE(!kv_mask, "%s: segment bounds take no kv_mask", what);
+  if (q_start) {
+    FSB_REQUIRE(!causal && !bias, "%s: cross segments take no causal mask and no rel_bias", what);
+    FSB_REQUIRE(head_dim == 64, "%s: head_dim %d unsupported (64 only)", what, head_dim);
+    *form = {64, false, dropout, kSegCross};
+    return FSB_OK;
+  }
+  FSB_REQUIRE(seq_q == seq_kv, "%s: segment bounds need seq_q == seq_kv (got %lld and %lld)", what, (long long)seq_q,
+              (long long)seq_kv);
+  if (causal && !bias) {
+    // GPT-2 (the one model with attention dropout that packs) runs head_dim 64 (110M) or 96 (3.5B); LLaMA has no attention
+    // dropout
+    FSB_REQUIRE(head_dim == 64 || head_dim == 96 || head_dim == 128, "%s: head_dim %d unsupported (64, 96 or 128)", what,
+                head_dim);
+    FSB_REQUIRE(!dropout || head_dim != 128, "%s: head_dim %d unsupported with p > 0 (64 or 96)", what, head_dim);
+    *form = {head_dim, false, dropout, kSegCausal};
+    return FSB_OK;
+  }
+  // BERT-base and MegatronBERT-1.3B (bidirectional) and mT5-small through XL and Randeng-T5-784M (bias) all run head_dim 64
+  FSB_REQUIRE(head_dim == 64, "%s: head_dim %d unsupported (64 only)", what, head_dim);
+  *form = {64, bias, dropout, causal ? kSegCausal : kSegBidir};
+  return FSB_OK;
+}
+
 }  // namespace fsb
 
-extern "C" int fsb_version(void) { return 1000 * 0 + 1; }
+extern "C" int fsb_version(void) { return 1000 * 0 + 2; }
 extern "C" const char* fsb_last_error(void) { return fsb::g_err; }
 extern "C" int fsb_num_sms(void) { return fsb::num_sms(); }

@@ -53,10 +53,23 @@ int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* d
 // {64, box_rows, 1}
 int make_attn_tmap(CUtensorMap* tm, const void* base, int64_t row_stride, int64_t width, int64_t seq, int64_t batch,
                    int box_rows);
-// Segment mode (kSeg) of the attention forward / backward kernels for packed rows (fsb_sdpa_*_segments*): none, causal
-// inside each segment, bidirectional inside each segment, or cross-attention from each query's segment to its key range in
-// another sequence
+// Segment mode (kSeg) of the attention forward / backward kernels for packed rows (the segment forms of fsb_sdpa_fwd /
+// fsb_sdpa_bwd): none, causal inside each segment, bidirectional inside each segment, or cross-attention from each query's
+// segment to its key range in another sequence
 enum AttnSegMode : int { kSegNone = 0, kSegCausal = 1, kSegBidir = 2, kSegCross = 3 };
+
+// The kernel instantiation (D, kBias, kDropout, kSeg) one attention call runs; key() is what the launchers switch over.
+struct AttnForm {
+  int d;
+  bool bias, dropout;
+  AttnSegMode seg;
+  constexpr int key() const { return d << 8 | int(bias) << 4 | int(dropout) << 3 | int(seg); }
+};
+// The table of forms of include/fsb200.h, shared by fsb_sdpa_fwd and fsb_sdpa_bwd: picks the form from the arguments that
+// select it and refuses (FSB_ERR_INVALID, error string prefixed with `what`) every combination no kernel is built for.
+int resolve_attn_form(const char* what, int head_dim, int causal, const void* kv_mask, const void* rel_bias,
+                      const int32_t* seg_start, const int32_t* seg_end, const int32_t* q_start, const int32_t* q_end,
+                      float p, int64_t seq_q, int64_t seq_kv, AttnForm* form);
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 

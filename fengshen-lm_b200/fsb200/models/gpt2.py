@@ -85,10 +85,6 @@ class GPT2LMHeadModel(FlatModel):
         if self.fp8:
             self._proj = [_Block(*(Fp8Conv1D(q) for q in pj)) for pj in self._proj]
         self.reset_parameters(seed)
-        # packed rows at head width 96 run the segment attention through its dropout entry, at p = 0 when the attention
-        # probabilities are not dropped (fsb_sdpa_*_segments itself takes head_dim 64 and 128): a Dropout that draws nothing
-        self._seg_nodrop = None if self.hn != 96 else \
-            ops.Dropout(0.0, 0, torch.zeros(1, dtype=torch.int64, device=self.flat.params.device), 0)
         # dropout sites of one forward, in transformers' call order: 0 embeddings; for layer i, 1 + 3i attention probabilities,
         # 2 + 3i attention c_proj output, 3 + 3i MLP c_proj output. A site whose probability is 0 keeps its number.
         self._init_dropout(1 + 3 * self.nl, (self.p_embd, self.p_attn, self.p_resid))
@@ -146,7 +142,7 @@ class GPT2LMHeadModel(FlatModel):
             drop = self._drop(base, self.p_attn, 1 + 3 * i)
             if seg is not None:
                 q, k, v = q5[:, :, 0], q5[:, :, 1], q5[:, :, 2]
-                return ops.sdpa_segments_fwd(q, k, v, scale, *seg, drop=self._seg_drop(drop))
+                return ops.sdpa_segments_fwd(q, k, v, scale, *seg, drop=drop)
             return ops.sdpa_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale, True, kv_mask=mask, drop=drop)
         hf, stf, xf = self._stack(ids, pos, B, S, attend, acts, base)
         logits = self._head(hf)
@@ -159,10 +155,6 @@ class GPT2LMHeadModel(FlatModel):
                 ctx = (acts, hf, stf, xf, dlogits, ids, pos, mask, B, S, base, seg)
                 logits = keep
         return loss, (logits if want_logits else None), ctx
-
-    def _seg_drop(self, drop):
-        """The drop argument of the packed attention: `drop`, or at head width 96 without one the p = 0 Dropout."""
-        return drop if drop is not None else self._seg_nodrop
 
     def _stack(self, ids, pos, B, S, attend, acts=None, base=None, proj=None):
         """Embedding, the blocks and ln_f over ids [B * S] -> (hidden states, ln_f stats, residual stream). attend(i, q5) is
@@ -309,7 +301,7 @@ class GPT2LMHeadModel(FlatModel):
             q5, d5 = qkv.view(B, S, 3, nh, hn), dqkv.view(B, S, 3, nh, hn)
             if seg is not None:
                 ops.sdpa_segments_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, *seg,
-                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=self._seg_drop(D(self.p_attn, 1 + 3 * i)))
+                                      d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], drop=D(self.p_attn, 1 + 3 * i))
             else:
                 ops.sdpa_bwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], o, do.view(B, S, nh, hn), lse, scale, True,
                              d5[:, :, 0], d5[:, :, 1], d5[:, :, 2], kv_mask=mask, drop=D(self.p_attn, 1 + 3 * i))

@@ -609,6 +609,12 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop
     over the offset k - q (T5 relative-position bias). drop: optional Dropout on the attention probabilities, its keep mask
     the attention layout of include/fsb200.h. The causal flag, kv_mask, rel_bias and drop compose. head_dim 64 or 128; 96
     (GPT-2 3.5B) with causal=True and no rel_bias only."""
+    return _sdpa_fwd(q, k, v, scale, causal, kv_mask, rel_bias, drop, out)
+
+
+def _sdpa_fwd(q, k, v, scale, causal, kv_mask, rel_bias, drop, out, bounds=(None,) * 4):
+    """The one fsb_sdpa_fwd call of sdpa_fwd and sdpa_segments_fwd. bounds: (seg_start, seg_end, q_start, q_end), each
+    None or contiguous int32, the query-side pair [B, Sq] and the key-side pair [B, Skv]; the arguments select the form."""
     _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
@@ -624,12 +630,10 @@ def sdpa_fwd(q, k, v, scale, causal, kv_mask=None, out=None, rel_bias=None, drop
             raise RuntimeError("fsb200: kv_mask must be contiguous uint8 [batch, seq_kv]")
     if rel_bias is not None:
         _chk_rel(rel_bias, H, Sq, Skv, "rel_bias")
-    if drop is None:
-        L.call("fsb_sdpa_fwd", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs,
-               v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _stream())
-    else:
-        L.call("fsb_sdpa_fwd_dropout", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs,
-               k_hs, v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), *drop.args(), _stream())
+    _chk_bounds(bounds, B, Sq, Skv)
+    L.call("fsb_sdpa_fwd", _p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs,
+           v_hs, o_hs, float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), *map(_p, bounds),
+           *(_NO_DROP if drop is None else drop.args()), _stream())
     return out, lse
 
 
@@ -730,6 +734,11 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
     """All tensors strided [B,S,H,D] bf16 views; dq/dk/dv are written (e.g. slices of a packed dQKV buffer).
     causal, kv_mask and rel_bias as in sdpa_fwd; drel_bias (fp32 [H, Sq + Skv - 1]) is accumulated into (+=),
     deterministically. drop: the forward's Dropout (same seed, base and site). head_dim as in sdpa_fwd."""
+    _sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, drop)
+
+
+def _sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask, rel_bias, drel_bias, drop, bounds=(None,) * 4):
+    """The one fsb_sdpa_bwd call of sdpa_bwd and sdpa_segments_bwd (bounds as in _sdpa_fwd)."""
     B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
     _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
     _, _, _, _, v_rs, v_hs = _bshd(v, "v")
@@ -738,9 +747,10 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
     _, _, _, _, dq_rs, dq_hs = _bshd(dq, "dq")
     _, _, _, _, dk_rs, dk_hs = _bshd(dk, "dk")
     _, _, _, _, dv_rs, dv_hs = _bshd(dv, "dv")
-    for t, n in ((dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
         _chk(t, _bf16, n)
     _chk_grads(q, k, dq, dk, dv)
+    _chk_bounds(bounds, B, Sq, Skv)
     delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
     ws, ws_bytes = None, 0
     if rel_bias is not None:
@@ -749,20 +759,17 @@ def sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, kv_mask=None, r
         _chk_rel(drel_bias, H, Sq, Skv, "drel_bias")
         ws_bytes = int(L.load().fsb_sdpa_bwd_workspace_bytes(B, Sq, Skv, H))
         ws = workspace(ws_bytes, q.device, "sdpa_dbias")
-    args = (_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv,
-            H, D, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs,
-            float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes)
-    if drop is None:
-        L.call("fsb_sdpa_bwd", *args, _stream())
-    else:
-        L.call("fsb_sdpa_bwd_dropout", *args, *drop.args(), _stream())
+    L.call("fsb_sdpa_bwd", _p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv,
+           H, D, q_rs, k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs,
+           float(scale), int(bool(causal)), _p(kv_mask), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes, *map(_p, bounds),
+           *(_NO_DROP if drop is None else drop.args()), _stream())
 
 
 # ------------------------------------------------------------------------------------------------- packed sequences
 def segment_bounds(segment_ids):
     """segment_ids: integer [B, S] (any device). A segment is a maximal run of equal consecutive values in a row, so every
     integer tensor is valid. Returns (seg_start, seg_end), contiguous int32 [B, S] on segment_ids' device: the row position of
-    the first token of each token's segment and one past its last (include/fsb200.h, fsb_sdpa_fwd_segments). Torch ops
+    the first token of each token's segment and one past its last (include/fsb200.h, the segment forms of fsb_sdpa_fwd). Torch ops
     only, no host synchronisation: capturable in a CUDA graph."""
     if segment_ids.dim() != 2 or segment_ids.dtype.is_floating_point or segment_ids.dtype.is_complex or \
             segment_ids.dtype == torch.bool:
@@ -779,68 +786,45 @@ def segment_bounds(segment_ids):
     return start.to(torch.int32).contiguous(), end.to(torch.int32).contiguous()
 
 
-_NO_DROP = (0.0, 0, None, 0)   # p, seed, stream_base, site of an entry with a dropout signature, run without dropout
+_NO_DROP = (0.0, 0, None, 0)   # p, seed, stream_base, site of an attention call without dropout
 
 
-def _chk_bounds(seg_start, seg_end, B, S, names=("seg_start", "seg_end")):
-    for t, n in zip((seg_start, seg_end), names):
+def _chk_bounds(bounds, B, Sq, Skv):
+    """(seg_start, seg_end, q_start, q_end): each pair None or contiguous int32, [B, Sq] and [B, Skv]."""
+    for t, n, S in zip(bounds, ("seg_start", "seg_end", "q_start", "q_end"), (Sq, Sq, Skv, Skv)):
+        if t is None:
+            continue
         _chk(t, torch.int32, n)
         if tuple(t.shape) != (B, S) or not t.is_contiguous():
             raise RuntimeError(f"fsb200: {n} must be contiguous int32 [batch, seq] = [{B}, {S}], got {tuple(t.shape)}")
 
 
-def _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B):
-    """The optional operands of sdpa_segments_fwd / _bwd: rel_bias [H, Sq + Skv - 1] or kv_bounds (two int32 [B, Skv]),
-    not both; the cross form (kv_bounds) has no causal mask."""
+def _segment_bounds_arg(seg_start, seg_end, rel_bias, kv_bounds, causal):
+    """The bounds of sdpa_segments_fwd / _bwd; the cross form (kv_bounds) takes no rel_bias and has no causal mask."""
+    if kv_bounds is None:
+        return seg_start, seg_end, None, None
     if rel_bias is not None:
-        if kv_bounds is not None:
-            raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) takes no rel_bias")
-        _chk_rel(rel_bias, H, Sq, Skv, "rel_bias")
-    if kv_bounds is not None:
-        if causal:
-            raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) has no causal mask: pass causal=False")
-        _chk_bounds(kv_bounds[0], kv_bounds[1], B, Skv, ("q_start", "q_end"))
+        raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) takes no rel_bias")
+    if causal:
+        raise RuntimeError("fsb200: the cross-attention segment form (kv_bounds) has no causal mask: pass causal=False")
+    return seg_start, seg_end, kv_bounds[0], kv_bounds[1]
 
 
 def sdpa_segments_fwd(q, k, v, scale, seg_start, seg_end, out=None, drop=None, causal=True, rel_bias=None, kv_bounds=None):
     """sdpa_fwd over rows that pack several sequences: causal inside each segment, nothing across segments. q, k, v as in
     sdpa_fwd (seq_q == seq_kv); seg_start / seg_end from segment_bounds. Key / query tiles outside a tile's segments are
-    skipped. head_dim 64 or 128; 96 only with a drop (fsb_sdpa_fwd_segments_dropout; a Dropout with p = 0 runs the
-    dropout-free kernel). drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 or 96 when
-    p > 0).
+    skipped. head_dim 64, 96 or 128. drop: optional Dropout on the attention probabilities, as in sdpa_fwd (head_dim 64 or
+    96 when p > 0).
     causal=False: bidirectional inside each segment (packed encoder rows: query q sees seg_start[q] <= k < seg_end[q]),
-    head_dim 64 only (fsb_sdpa_fwd_segments_bidirectional).
+    head_dim 64 only.
     rel_bias: the T5 relative-position bias of sdpa_fwd (fp32 [H, 2 S - 1]) added inside either segment form, head_dim 64
-    only (fsb_sdpa_fwd_segments_bias).
+    only.
     kv_bounds=(q_start, q_end): cross-attention from packed decoder rows to packed encoder rows (seq_q and seq_kv may
-    differ, causal=False): seg_start / seg_end are then the query side's key ranges kv_start / kv_end [B, Sq] and kv_bounds
-    the key side's query ranges [B, Skv] (models/base.py cross_segment_bounds), head_dim 64 only
-    (fsb_sdpa_fwd_segments_cross). Returns (out [B, Sq, H, D], lse)."""
-    _chk(q, _bf16, "q"); _chk(k, _bf16, "k"); _chk(v, _bf16, "v")
-    B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
-    _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
-    _, _, _, _, v_rs, v_hs = _bshd(v, "v")
-    _chk_bounds(seg_start, seg_end, B, Sq)
-    _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B)
-    if out is None:
-        out = torch.empty((B, Sq, H, D), dtype=_bf16, device=q.device)
-    if tuple(out.shape) != (B, Sq, H, D): raise RuntimeError(f"fsb200: out shape {tuple(out.shape)} != {(B, Sq, H, D)}")
-    _, _, _, _, o_rs, o_hs = _bshd(out, "out")
-    lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
-    args = (_p(q), _p(k), _p(v), _p(out), _p(lse), B, Sq, Skv, H, D, q_rs, k_rs, v_rs, o_rs, q_hs, k_hs, v_hs, o_hs,
-            float(scale), _p(seg_start), _p(seg_end))
-    drop_args = _NO_DROP if drop is None else drop.args()
-    if kv_bounds is not None:
-        L.call("fsb_sdpa_fwd_segments_cross", *args, _p(kv_bounds[0]), _p(kv_bounds[1]), *drop_args, _stream())
-    elif rel_bias is not None:
-        L.call("fsb_sdpa_fwd_segments_bias", *args, int(bool(causal)), _p(rel_bias), *drop_args, _stream())
-    elif not causal:
-        L.call("fsb_sdpa_fwd_segments_bidirectional", *args, *drop_args, _stream())
-    elif drop is None:
-        L.call("fsb_sdpa_fwd_segments", *args, _stream())
-    else:
-        L.call("fsb_sdpa_fwd_segments_dropout", *args, *drop.args(), _stream())
-    return out, lse
+    differ, causal=False): seg_start / seg_end are then the query side's key ranges [B, Sq] and kv_bounds the key side's
+    query ranges [B, Skv] (models/base.py cross_segment_bounds), head_dim 64 only. The forms are those of fsb_sdpa_fwd
+    (include/fsb200.h). Returns (out [B, Sq, H, D], lse)."""
+    bounds = _segment_bounds_arg(seg_start, seg_end, rel_bias, kv_bounds, causal)
+    return _sdpa_fwd(q, k, v, scale, causal, None, rel_bias, drop, out, bounds)
 
 
 def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk, dv, drop=None, causal=True,
@@ -848,39 +832,7 @@ def sdpa_segments_bwd(q, k, v, out, dout, lse, scale, seg_start, seg_end, dq, dk
     """Backward of sdpa_segments_fwd (the forward's seg_start / seg_end, drop, causal, rel_bias and kv_bounds); dq / dk / dv
     are written as in sdpa_bwd. drel_bias (with rel_bias): fp32 [H, 2 S - 1], accumulated into (+=) deterministically, as in
     sdpa_bwd."""
-    B, Sq, H, D, q_rs, q_hs = _bshd(q, "q")
-    _, Skv, _, _, k_rs, k_hs = _bshd(k, "k")
-    _, _, _, _, v_rs, v_hs = _bshd(v, "v")
-    _, _, _, _, o_rs, o_hs = _bshd(out, "out")
-    _, _, _, _, do_rs, do_hs = _bshd(dout, "dout")
-    _, _, _, _, dq_rs, dq_hs = _bshd(dq, "dq")
-    _, _, _, _, dk_rs, dk_hs = _bshd(dk, "dk")
-    _, _, _, _, dv_rs, dv_hs = _bshd(dv, "dv")
-    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out"), (dout, "dout"), (dq, "dq"), (dk, "dk"), (dv, "dv")):
-        _chk(t, _bf16, n)
-    _chk_grads(q, k, dq, dk, dv)
-    _chk_bounds(seg_start, seg_end, B, Sq)
-    _chk_segment_forms(rel_bias, kv_bounds, causal, H, Sq, Skv, B)
-    ws, ws_bytes = None, 0
-    if drel_bias is not None:
-        if rel_bias is None:
-            raise RuntimeError("fsb200: drel_bias needs rel_bias")
-        _chk_rel(drel_bias, H, Sq, Skv, "drel_bias")
-        ws_bytes = int(L.load().fsb_sdpa_bwd_workspace_bytes(B, Sq, Skv, H))
-        ws = workspace(ws_bytes, q.device, "sdpa_dbias")
-    delta = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device)
-    args = (_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), B, Sq, Skv, H, D, q_rs,
-            k_rs, v_rs, o_rs, do_rs, dq_rs, dk_rs, dv_rs, q_hs, k_hs, v_hs, o_hs, do_hs, dq_hs, dk_hs, dv_hs, float(scale),
-            _p(seg_start), _p(seg_end))
-    drop_args = _NO_DROP if drop is None else drop.args()
-    if kv_bounds is not None:
-        L.call("fsb_sdpa_bwd_segments_cross", *args, _p(kv_bounds[0]), _p(kv_bounds[1]), *drop_args, _stream())
-    elif rel_bias is not None:
-        L.call("fsb_sdpa_bwd_segments_bias", *args, int(bool(causal)), _p(rel_bias), _p(drel_bias), _p(ws), ws_bytes,
-               *drop_args, _stream())
-    elif not causal:
-        L.call("fsb_sdpa_bwd_segments_bidirectional", *args, *drop_args, _stream())
-    elif drop is None:
-        L.call("fsb_sdpa_bwd_segments", *args, _stream())
-    else:
-        L.call("fsb_sdpa_bwd_segments_dropout", *args, *drop.args(), _stream())
+    bounds = _segment_bounds_arg(seg_start, seg_end, rel_bias, kv_bounds, causal)
+    if drel_bias is not None and rel_bias is None:
+        raise RuntimeError("fsb200: drel_bias needs rel_bias")
+    _sdpa_bwd(q, k, v, out, dout, lse, scale, causal, dq, dk, dv, None, rel_bias, drel_bias, drop, bounds)

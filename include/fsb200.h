@@ -303,22 +303,77 @@ int fsb_softmax_get_batch_per_block(int64_t sq, int64_t sk, int64_t batches, int
  *   element (b, s, head, d) of X lives at X + ((b*seq + s)*x_row_stride + head*x_head_stride + d)  (elements).
  * o: same addressing with o_*_stride. lse: fp32 [batch, nheads, seq_q], log2 domain (internal, consumed by bwd).
  * kv_mask: optional uint8 [batch, seq_kv], 1 = attend (HF additive padding mask), NULL = none.
- * causal=1 masks key > query (requires seq_q == seq_kv). head_dim in {64, 128}, and 96 with causal=1 and no rel_bias
- *   (GPT-2 3.5B, 32 heads x 96; the kernels stage 128 columns and store 96; fsb_sdpa_*_dropout likewise).
+ * causal=1 masks key > query (requires seq_q == seq_kv); the key / query tiles wholly above the diagonal are skipped.
  * rel_bias: optional fp32 [nheads, seq_q + seq_kv - 1], natural-log units, added to scale * q.k before the softmax:
  *   bias(h, q, k) = rel_bias[h][k - q + seq_q - 1]  — the T5 / mT5 relative-position bias (transformers
  *   mt5/modeling_mt5.py:181-235,:320: an embedding over bucket(k - q), shared by every layer of a stack), used by
  *   fengshen/examples/pretrain_t5/pretrain_t5.py:57-59 (scale = 1: T5 attention is unscaled, :300). NULL = none.
+ * seg_start / seg_end, q_start / q_end: segment bounds of packed rows (below); all NULL = unsegmented.
+ * p, seed, stream_base, site: dropout on the attention probabilities (the dropout section), O = (P * Z / (1 - p)) V; the
+ *   LSE is that of the un-dropped P, the backward's delta is unchanged. p == 0 runs the dropout-free kernels and does not
+ *   read stream_base. Z of an element is a function of its row-relative (q, k) only, so it is the same whichever tiles a
+ *   launch visits: the tiles that the causal rule or the segment bounds skip draw no bit another element needs, and a
+ *   masked element has P = 0 whatever its bit. The backward must get the forward's seed, stream_base value and site.
+ *
+ * The arguments select the form, and with it the kernels (p composes with every form):
+ *   form                    selected by                          head_dim                     causal kv_mask  rel_bias seq_q, seq_kv
+ *   dense                   no bounds                            64, 128; 96 causal, no bias  0 / 1  optional optional equal if causal
+ *   causal segments         seg_*, causal = 1, no rel_bias, q_*  64, 96, 128 (p > 0: 64, 96)  1      -        -        equal
+ *   bidirectional segments  seg_*, causal = 0, no rel_bias, q_*  64                           0      -        -        equal
+ *   biased segments         seg_* + rel_bias                     64                           0 / 1  -        required equal
+ *   cross segments          seg_* + q_start / q_end              64                           0      -        -        may differ
+ * head_dim 96 is GPT-2 3.5B's (32 heads x 96): the kernels stage 128 columns and store 96.
+ * With p > 0 every form refuses sequences longer than 65536. Refused as well: only one of seg_start / seg_end or of
+ * q_start / q_end, q_* without seg_*, and a kv_mask with segment bounds.
+ *
+ * Segment bounds: int32 arrays, contiguous, indices relative to the row. Self-attention (seq_q == seq_kv), two [batch, seq]:
+ *   seg_start[b][t] : the position of the first token of t's segment;
+ *   seg_end[b][t]   : one past the position of its last token.
+ * The bounds are valid when every row is cut into contiguous segments [s, e) covering [0, seq) in order and both arrays hold
+ * each token's own segment. Invalid bounds give unspecified results but never an out-of-bounds access: the tile ranges
+ * are clamped into the sequence.
+ *   causal segments: key k is visible to query q iff seg_start[q] <= k <= q (equivalently k <= q < seg_end[k]), nothing
+ *     across segments. The key / query tiles wholly outside a tile's segments are never loaded: the forward and dQ pass start
+ *     at the key tile of seg_start[first query of the tile], the dK / dV pass stops after the query tile of seg_end[last key
+ *     of the tile]. The forward reads seg_start only; the backward needs the forward's seg_start and the matching seg_end.
+ *     Dropout: an element keeps the bit it has in an unsegmented causal launch.
+ *   bidirectional segments (packed BERT / MegatronBERT encoder rows): key k is visible to query q iff
+ *     seg_start[q] <= k < seg_end[q] (equivalently seg_start[k] <= q < seg_end[k]); both bounds are read by the forward as
+ *     well as the backward. With valid bounds the forward and dQ pass visit the key tiles from the one of seg_start[first
+ *     query of the tile] to the one of seg_end[last query of the tile] - 1, and the dK / dV pass the query tiles from
+ *     seg_start[first key of the tile] to seg_end[last key of the tile] - 1; a step masks only where it crosses a row's
+ *     lower or upper bound. The ranges are clamped into the sequence and always hold the tile's diagonal tile. Dropout: the
+ *     keep mask of an element is its bit at the row-relative (q, k) of an unsegmented non-causal launch.
+ *   biased segments (packed mT5 / T5 self-attention): the causal (causal = 1, the decoder) or bidirectional (causal = 0, the
+ *     encoder) segment rule plus rel_bias (fp32 [nheads, 2 seq - 1] over the offset k - q). The bias depends on (q, k)
+ *     through k - q only, so inside a segment the scores are those of the segment run alone and no position ids are needed.
+ *     Tile skipping and clamping as in the unbiased rule. The backward accumulates the bias gradient into drel_bias (or
+ *     skips it when NULL) with the workspace of the dense form: the reduction reads exactly the per-step slots the dQ pass
+ *     wrote (the steps the segment bounds skip are neither written nor read), so the workspace needs no clearing.
+ *   cross segments (packed encoder-decoder cross-attention): row b of the queries (seq_q decoder tokens) attends to row b of
+ *     the keys (seq_kv encoder tokens), seq_q and seq_kv may differ. Four arrays:
+ *       seg_start[b][q], seg_end[b][q] ([batch, seq_q])  : query q sees the keys seg_start[q] <= k < seg_end[q];
+ *       q_start[b][k],   q_end[b][k]   ([batch, seq_kv]) : key k is seen by the queries q_start[k] <= q < q_end[k].
+ *     They must describe the same visibility, and each array must be non-decreasing along the row (segments paired in
+ *     order, e.g. by equal segment id). Then the forward and dQ pass visit the key tiles from the one of seg_start[first
+ *     query of the tile] to the one of seg_end[last query of the tile] - 1, the dK / dV pass the query tiles from
+ *     q_start[first key] to q_end[last key] - 1, clamped into the sequence. An empty range is legal: a query that sees no
+ *     key writes O = 0 and LSE = +inf (which makes its dQ and its share of dK / dV exactly 0), and a key no query sees gets
+ *     dK = dV = 0; every output element is written. Dropout: an element's keep bit is that of its row-relative (q, k) in an
+ *     unsegmented non-causal launch. The forward reads seg_start / seg_end only.
  */
 int fsb_sdpa_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
                  int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
                  int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                 float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, fsb_stream_t stream);
+                 float scale, int causal, const uint8_t* kv_mask, const float* rel_bias,
+                 const int32_t* seg_start, const int32_t* seg_end, const int32_t* q_start, const int32_t* q_end,
+                 float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
 
-/* Backward of fsb_sdpa_fwd. o/lse are the forward outputs; delta: fp32 scratch [batch, nheads, seq_q] (written here);
- * dq/dk/dv are written with their own strides (e.g. the three slices of a packed dQKV buffer). Deterministic.
- * rel_bias as in the forward; drel_bias (fp32 [nheads, seq_q + seq_kv - 1], may be NULL) is ACCUMULATED into:
+/* Backward of fsb_sdpa_fwd, with the forward's form arguments. o/lse are the forward outputs; delta: fp32 scratch
+ * [batch, nheads, seq_q] (written here); dq/dk/dv are written with their own strides (e.g. the three slices of a packed
+ * dQKV buffer). Deterministic.
+ * drel_bias (fp32 [nheads, seq_q + seq_kv - 1], may be NULL, needs rel_bias) is ACCUMULATED into:
  *   drel_bias[h][r] += sum over (batch, q) of dS[q, q + r - (seq_q - 1)]   (gradient w.r.t. the bias vector; the
  * [buckets, heads] table gradient is its scatter over bucket(r), autograd of T5Attention.compute_bias). It needs a workspace of
  * fsb_sdpa_bwd_workspace_bytes(batch, seq_q, seq_kv, nheads) bytes: per-step diagonal sums written by the dQ kernel and
@@ -332,7 +387,9 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
                  int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
                  float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
-                 void* workspace, size_t workspace_bytes, fsb_stream_t stream);
+                 void* workspace, size_t workspace_bytes,
+                 const int32_t* seg_start, const int32_t* seg_end, const int32_t* q_start, const int32_t* q_end,
+                 float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
 
 /* ---- dropout (GPT-2 / BERT / MegatronBERT / mT5 training) -----------------------------------------------------------
  * torch.nn.functional.dropout semantics: an element is dropped with probability p and every kept element is scaled by
@@ -347,11 +404,6 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
  *   attention : element (b, head, q, k) with q = 16 qa + 8 qh + 2 qs + qp and k = 16 ka + 8 kh + 2 ks + kp:
  *               counter ((4 ka + ks) | (4 qa + qs) << 16, b * nheads + head, s & 0xffffffff, s >> 32); r = byte 2 qh + kh of
  *               output word 2 qp + kp. seq_q, seq_kv <= 65536.
- * fsb_sdpa_fwd_dropout / fsb_sdpa_bwd_dropout: fsb_sdpa_fwd / fsb_sdpa_bwd with dropout on the attention probabilities,
- *   O = (P * Z / (1 - p)) V; the LSE is that of the un-dropped P, the backward's delta is unchanged. The causal flag,
- *   kv_mask and rel_bias all compose with dropout (GPT-2: causal + padding; T5: relative bias). Z of an element is the same
- *   whichever tiles a launch visits, so a causal launch still skips the key / query tiles wholly above the diagonal. The
- *   backward must get the forward's seed, stream_base value and site.
  * fsb_layernorm_fwd_dropout: fsb_layernorm_fwd with sum_out = x * Z / (1 - p) + residual (residual required when p > 0): the
  *   dropped branch of a residual block. With p > 0 both LayerNorm entries take cols <= 12288. fsb_layernorm_bwd_dropout: fsb_layernorm_bwd that also writes dbranch = dx * Z / (1 - p)
  *   (dx already includes dres), the gradient of the branch x, beside dx, the gradient of the sum (and of the residual).
@@ -362,161 +414,6 @@ int fsb_sdpa_bwd(const void* q, const void* k, const void* v, const void* o, con
  *   x == y is allowed.
  * fsb_dropout_advance: *saved = *stream_base; *stream_base += n (one thread on the device). A training forward calls it once
  *   and hands `saved` to every dropout call of that forward and of its backward, so a replayed CUDA graph draws new masks. */
-int fsb_sdpa_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse,
-                         int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                         int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                         int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                         float scale, int causal, const uint8_t* kv_mask, const float* rel_bias,
-                         float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-int fsb_sdpa_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                         const float* lse, float* delta, void* dq, void* dk, void* dv,
-                         int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                         int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                         int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                         int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                         int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                         float scale, int causal, const uint8_t* kv_mask, const float* rel_bias, float* drel_bias,
-                         void* workspace, size_t workspace_bytes,
-                         float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-/* ---- packed sequences (document-masked causal and bidirectional attention) -------------------------------------------
- * fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments: fsb_sdpa_fwd / fsb_sdpa_bwd with causal = 1 inside each segment of a row
- * and nothing across segments, for rows that pack several documents. No kv_mask or rel_bias (dropout: the
- * fsb_sdpa_*_segments_dropout pair below); seq_q == seq_kv;
- * head_dim in {64, 128} (head_dim 96 runs the same kernels through fsb_sdpa_*_segments_dropout, at p = 0 without
- * dropout). The bounds are two int32 [batch, seq] arrays, contiguous, indices relative to the row:
- *   seg_start[b][t] : the position of the first token of t's segment;
- *   seg_end[b][t]   : one past the position of its last token.
- * Key k is visible to query q iff seg_start[q] <= k <= q (equivalently k <= q < seg_end[k]). The bounds are valid when every
- * row is cut into contiguous segments [s, e) covering [0, seq) in order and both arrays hold each token's own segment.
- * Then the key / query tiles wholly outside a tile's segments are never loaded: the forward and dQ pass start at the key
- * tile of seg_start[first query of the tile], the dK / dV pass stops after the query tile of seg_end[last key of the tile].
- * Invalid bounds give unspecified results but never an out-of-bounds access: the tile ranges are clamped into the
- * sequence. The forward reads seg_start only; the backward needs the forward's seg_start and the matching seg_end. */
-int fsb_sdpa_fwd_segments(const void* q, const void* k, const void* v, void* o, float* lse,
-                          int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                          int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                          int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                          float scale, const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t stream);
-int fsb_sdpa_bwd_segments(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                          const float* lse, float* delta, void* dq, void* dk, void* dv,
-                          int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                          int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                          int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                          int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                          int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                          float scale, const int32_t* seg_start, const int32_t* seg_end, fsb_stream_t stream);
-/* fsb_sdpa_fwd_segments_dropout / fsb_sdpa_bwd_segments_dropout: the segment entries with dropout on the attention
- * probabilities (GPT-2 packed training), taking p, seed, stream_base and site as fsb_sdpa_*_dropout do. Visibility is the
- * segment rule above; the keep mask Z is the attention layout of the dropout section, at the row-relative (q, k) of each
- * element, so an element keeps the bit it has in an unsegmented causal launch and the skipped tiles draw nothing. O, the LSE
- * (of the un-dropped P) and the gradients follow fsb_sdpa_*_dropout. p == 0 runs the kernels of fsb_sdpa_*_segments and does
- * not read the stream counter; at head_dim 96 this is the only entry to the packed kernels (fsb_sdpa_*_segments refuse 96). Refused: null bounds, seq_q != seq_kv, head_dim other than 64, 96 or 128, and with p > 0 head_dim 128 or
- * sequences longer than 65536. The backward must get the forward's bounds, seed, stream_base value and site. */
-int fsb_sdpa_fwd_segments_dropout(const void* q, const void* k, const void* v, void* o, float* lse,
-                                  int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                  int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                  float scale, const int32_t* seg_start, const int32_t* seg_end,
-                                  float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-int fsb_sdpa_bwd_segments_dropout(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                  const float* lse, float* delta, void* dq, void* dk, void* dv,
-                                  int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                  int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                  int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                                  int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                  int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                                  float scale, const int32_t* seg_start, const int32_t* seg_end,
-                                  float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-/* fsb_sdpa_fwd_segments_bidirectional / fsb_sdpa_bwd_segments_bidirectional: bidirectional (encoder) attention inside each
- * segment of a row and nothing across segments, for packed BERT / MegatronBERT rows, with optional dropout on the attention
- * probabilities. Arguments as fsb_sdpa_*_segments_dropout; the same seg_start / seg_end bounds, and both are read by the
- * forward as well as the backward. Key k is visible to query q iff seg_start[q] <= k < seg_end[q] (equivalently
- * seg_start[k] <= q < seg_end[k]). With valid bounds (as above) the forward and dQ pass visit the key tiles from the one of
- * seg_start[first query of the tile] to the one of seg_end[last query of the tile] - 1, and the dK / dV pass the query
- * tiles from seg_start[first key of the tile] to seg_end[last key of the tile] - 1; a step masks only where it crosses a
- * row's lower or upper bound. The ranges are clamped into the sequence and always hold the tile's diagonal tile, so invalid
- * bounds give unspecified results but never an out-of-bounds access. Dropout as in fsb_sdpa_*_segments_dropout: the keep
- * mask of an element is its bit at the row-relative (q, k) of an unsegmented non-causal launch, the LSE is that of the
- * un-dropped P. p == 0 runs the dropout-free kernels and does not read the stream counter. No kv_mask or rel_bias.
- * Refused: null bounds, seq_q != seq_kv, head_dim other than 64, and with p > 0 sequences longer than 65536. */
-int fsb_sdpa_fwd_segments_bidirectional(const void* q, const void* k, const void* v, void* o, float* lse,
-                                        int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                        int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
-                                        int64_t o_row_stride, int64_t q_head_stride, int64_t k_head_stride,
-                                        int64_t v_head_stride, int64_t o_head_stride, float scale,
-                                        const int32_t* seg_start, const int32_t* seg_end, float p, uint64_t seed,
-                                        const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-int fsb_sdpa_bwd_segments_bidirectional(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                        const float* lse, float* delta, void* dq, void* dk, void* dv,
-                                        int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                        int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride,
-                                        int64_t o_row_stride, int64_t do_row_stride, int64_t dq_row_stride,
-                                        int64_t dk_row_stride, int64_t dv_row_stride, int64_t q_head_stride,
-                                        int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                        int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride,
-                                        int64_t dv_head_stride, float scale, const int32_t* seg_start,
-                                        const int32_t* seg_end, float p, uint64_t seed, const int64_t* stream_base,
-                                        int64_t site, fsb_stream_t stream);
-/* fsb_sdpa_fwd_segments_bias / fsb_sdpa_bwd_segments_bias: packed mT5 / T5 self-attention, the segment rule of
- * fsb_sdpa_*_segments (causal = 1, the decoder) or of fsb_sdpa_*_segments_bidirectional (causal = 0, the encoder) plus the
- * additive relative-position bias rel_bias of fsb_sdpa_fwd (fp32 [nheads, 2 seq - 1] over the offset k - q). The bias depends
- * on (q, k) through k - q only, so inside a segment the scores are those of the segment run alone and no position ids are
- * needed. The same seg_start / seg_end bounds for both directions; tile skipping and clamping as in those pairs. Dropout as
- * in fsb_sdpa_*_segments_dropout (p == 0 runs the dropout-free kernels and does not read the stream counter). The backward
- * accumulates the bias gradient into drel_bias (or skips it when null) as fsb_sdpa_bwd does, with the same workspace of
- * fsb_sdpa_bwd_workspace_bytes bytes: the reduction reads exactly the per-step slots the dQ pass wrote (the steps the
- * segment bounds skip are neither written nor read), so the workspace needs no clearing. No kv_mask. Refused: null bounds,
- * a null rel_bias, seq_q != seq_kv, head_dim other than 64, drel_bias without a large enough workspace, and with p > 0
- * sequences longer than 65536. */
-int fsb_sdpa_fwd_segments_bias(const void* q, const void* k, const void* v, void* o, float* lse,
-                               int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                               int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                               int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                               float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
-                               const float* rel_bias, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
-                               fsb_stream_t stream);
-int fsb_sdpa_bwd_segments_bias(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                               const float* lse, float* delta, void* dq, void* dk, void* dv,
-                               int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                               int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                               int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                               int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                               int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                               float scale, const int32_t* seg_start, const int32_t* seg_end, int causal,
-                               const float* rel_bias, float* drel_bias, void* workspace, size_t workspace_bytes,
-                               float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);
-/* fsb_sdpa_fwd_segments_cross / fsb_sdpa_bwd_segments_cross: packed encoder-decoder cross-attention. Row b of the queries
- * (seq_q decoder tokens) attends to row b of the keys (seq_kv encoder tokens); seq_q and seq_kv may differ. Four int32
- * bounds arrays, contiguous, indices relative to the row:
- *   kv_start[b][q], kv_end[b][q] ([batch, seq_q])  : query q sees the keys kv_start[q] <= k < kv_end[q];
- *   q_start[b][k],  q_end[b][k]  ([batch, seq_kv]) : key k is seen by the queries q_start[k] <= q < q_end[k].
- * They must describe the same visibility, and each array must be non-decreasing along the row (segments paired in order,
- * e.g. by equal segment id). Then the forward and dQ pass visit the key tiles from the one of kv_start[first query of the
- * tile] to the one of kv_end[last query of the tile] - 1, the dK / dV pass the query tiles from q_start[first key] to
- * q_end[last key] - 1, clamped into the sequence. An empty range is legal: a query that sees no key writes O = 0 and
- * LSE = +inf (which makes its dQ and its share of dK / dV exactly 0), and a key no query sees gets dK = dV = 0; every
- * output element is written. Invalid bounds give unspecified results but never an out-of-bounds access. Dropout as in
- * fsb_sdpa_*_segments_dropout: an element's keep bit is that of its row-relative (q, k) in an unsegmented non-causal launch.
- * p == 0 runs the dropout-free kernels and does not read the stream counter. No kv_mask, no rel_bias. The forward reads
- * kv_start / kv_end only. Refused: null bounds, head_dim other than 64, and with p > 0 sequences longer than 65536. */
-int fsb_sdpa_fwd_segments_cross(const void* q, const void* k, const void* v, void* o, float* lse,
-                                int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                float scale, const int32_t* kv_start, const int32_t* kv_end, const int32_t* q_start,
-                                const int32_t* q_end, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
-                                fsb_stream_t stream);
-int fsb_sdpa_bwd_segments_cross(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                const float* lse, float* delta, void* dq, void* dk, void* dv,
-                                int64_t batch, int64_t seq_q, int64_t seq_kv, int nheads, int head_dim,
-                                int64_t q_row_stride, int64_t k_row_stride, int64_t v_row_stride, int64_t o_row_stride,
-                                int64_t do_row_stride, int64_t dq_row_stride, int64_t dk_row_stride, int64_t dv_row_stride,
-                                int64_t q_head_stride, int64_t k_head_stride, int64_t v_head_stride, int64_t o_head_stride,
-                                int64_t do_head_stride, int64_t dq_head_stride, int64_t dk_head_stride, int64_t dv_head_stride,
-                                float scale, const int32_t* kv_start, const int32_t* kv_end, const int32_t* q_start,
-                                const int32_t* q_end, float p, uint64_t seed, const int64_t* stream_base, int64_t site,
-                                fsb_stream_t stream);
-
 int fsb_layernorm_fwd_dropout(const void* x, const void* residual, const void* gamma, const void* beta, void* y,
                               void* sum_out, float* mean_rstd, int64_t rows, int64_t cols, float eps,
                               float p, uint64_t seed, const int64_t* stream_base, int64_t site, fsb_stream_t stream);

@@ -1,7 +1,6 @@
 """GPU: causal attention at head_dim 96 (the 3.5B Wenzhong / Yuyuan GPT-2: 32 heads x 96), in every form GPT-2 launches:
 causal with an optional key mask, the same with dropout on the probabilities, and packed causal segments with and without
-dropout (fsb_sdpa_{fwd,bwd}[_dropout|_segments_dropout] at head_dim 96; the packed form without dropout is the segment
-dropout entry at p = 0, since fsb_sdpa_{fwd,bwd}_segments keep head_dim 64 and 128).
+dropout (the dense and causal segment forms of fsb_sdpa_{fwd,bwd} at head_dim 96).
 
 q / k / v are strided views of one packed [B, S, 3, H, 96] tensor, as GPT-2's c_attn output. References are fp64; the keep
 masks are rebuilt by the numpy Philox of tests/philox_ref.py. The D = 96 kernels stage whole 64-column panels, as the
@@ -30,12 +29,6 @@ def _base():
 
 def _drop(p):
     return None if p is None else ops.Dropout(p, SEED, _base(), SITE)
-
-
-def _seg_drop(p):
-    """The drop of a packed-segment launch at head_dim 96: the dropout entry, at p = 0 for the dropout-free form
-    (fsb_sdpa_*_segments itself takes head_dim 64 and 128)."""
-    return ops.Dropout(p or 0.0, SEED, _base(), SITE)
 
 
 def _case(B, S, H, seed, heads_total=None):
@@ -91,7 +84,6 @@ def _run(qkv, dout, H, mask=None, seg_ids=None, p=None, dqkv=None):
         ops.sdpa_bwd(q, k, v, out, dout, lse, scale, True, dq, dk, dv, kv_mask=mask, drop=drop)
     else:
         st, en = ops.segment_bounds(seg_ids)
-        drop = _seg_drop(p)
         out, lse = ops.sdpa_segments_fwd(q, k, v, scale, st, en, drop=drop)
         ops.sdpa_segments_bwd(q, k, v, out, dout, lse, scale, st, en, dq, dk, dv, drop=drop)
     torch.cuda.synchronize()
@@ -195,7 +187,7 @@ def test_forward_is_the_d128_forward_on_zero_padded_heads(form, S):
         q, k, v = t[:, :, 0], t[:, :, 1], t[:, :, 2]
         if segmented:
             st, en = ops.segment_bounds(_seg_ids(LAYOUTS[1024][:B] if S == 1024 else [[64, 65], [1, 128]], S))
-            outs.append(ops.sdpa_segments_fwd(q, k, v, scale, st, en, drop=_seg_drop(p)))   # D 128 runs p == 0
+            outs.append(ops.sdpa_segments_fwd(q, k, v, scale, st, en, drop=_drop(p)))
         else:
             outs.append(ops.sdpa_fwd(q, k, v, scale, True, kv_mask=mask, drop=_drop(p)))
     torch.cuda.synchronize()
@@ -249,9 +241,9 @@ def test_writes_stay_inside_each_head(form):
     if segmented:
         st, en = ops.segment_bounds(_seg_ids([[64, 65, 71], [1, 199]], S))
         out, lse = F.check_footprint("sdpa_segments_fwd", ops.sdpa_segments_fwd, (q, k, v, scale, st, en),
-                                     dict(out=o_all[:, :, 1:3], drop=_seg_drop(p)))
+                                     dict(out=o_all[:, :, 1:3], drop=_drop(p)))
         F.check_footprint("sdpa_segments_bwd", ops.sdpa_segments_bwd,
-                          (q, k, v, out, dout, lse, scale, st, en, dq, dk, dv), dict(drop=_seg_drop(p)))
+                          (q, k, v, out, dout, lse, scale, st, en, dq, dk, dv), dict(drop=_drop(p)))
     else:
         out, lse = F.check_footprint("sdpa_fwd", ops.sdpa_fwd, (q, k, v, scale, True),
                                      dict(kv_mask=mask, out=o_all[:, :, 1:3], drop=_drop(p)))
@@ -262,7 +254,7 @@ def test_writes_stay_inside_each_head(form):
 
 
 # ------------------------------------------------------------------------------------------------ refusals
-def test_forms_other_than_causal_refuse_head_dim_96():
+def test_head_dim_96_refuses_other_forms_and_runs_causal_segments_without_drop():
     B, S, H = 1, 128, 2
     qkv, _ = _case(B, S, H, seed=7)
     q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
@@ -274,9 +266,6 @@ def test_forms_other_than_causal_refuse_head_dim_96():
         ops.sdpa_fwd(q, k, v, 0.1, True, rel_bias=rel)
     with pytest.raises(RuntimeError, match="head_dim"):
         ops.sdpa_fwd(q, k, v, 0.1, False, drop=_drop(0.1))
-    # the plain segment entries keep head_dim 64 and 128; 96 runs through the dropout entry (p = 0 included)
-    with pytest.raises(RuntimeError, match="head_dim 96"):
-        ops.sdpa_segments_fwd(q, k, v, 0.1, st, en)
     with pytest.raises(RuntimeError, match="head_dim"):
         ops.sdpa_segments_fwd(q, k, v, 0.1, st, en, causal=False)
     with pytest.raises(RuntimeError, match="head_dim"):
@@ -289,7 +278,11 @@ def test_forms_other_than_causal_refuse_head_dim_96():
         ops.sdpa_bwd(q, k, v, q, q, lse, 0.1, False, d, d, d)
     with pytest.raises(RuntimeError, match="head_dim"):
         ops.sdpa_bwd(q, k, v, q, q, lse, 0.1, True, d, d, d, rel_bias=rel)
-    with pytest.raises(RuntimeError, match="head_dim 96"):
-        ops.sdpa_segments_bwd(q, k, v, q, q, lse, 0.1, st, en, d, d, d)
     with pytest.raises(RuntimeError, match="head_dim"):
         ops.sdpa_segments_bwd(q, k, v, q, q, lse, 0.1, st, en, d, d, d, causal=False)
+    # causal segments without a drop run at head_dim 96: the kernels a Dropout(0.0) selects, bit for bit
+    qkv, dout = _case(B, S, H, seed=8)
+    seg = _seg_ids([[60, 68]], S)
+    for x, y in zip(_run(qkv, dout, H, seg_ids=seg), _run(qkv, dout, H, seg_ids=seg, p=0.0)):
+        assert torch.equal(x.view(torch.int16) if x.dtype == torch.bfloat16 else x.view(torch.int32),
+                           y.view(torch.int16) if y.dtype == torch.bfloat16 else y.view(torch.int32))

@@ -1,7 +1,7 @@
 """GPU: the packed attention of mT5 / Randeng-T5 fine-tuning, with and without dropout on its probabilities:
-  * segment-masked self-attention with the relative-position bias (fsb_sdpa_{fwd,bwd}_segments_bias,
+  * segment-masked self-attention with the relative-position bias (the biased segment form of fsb_sdpa_{fwd,bwd},
     ops.sdpa_segments_*(rel_bias=...)): bidirectional inside each segment (the encoder) or causal inside it (the decoder);
-  * segment-paired cross-attention between rows of different lengths (fsb_sdpa_{fwd,bwd}_segments_cross,
+  * segment-paired cross-attention between rows of different lengths (the cross segment form of fsb_sdpa_{fwd,bwd},
     ops.sdpa_segments_*(kv_bounds=...)): decoder segment x of a row sees the encoder segment with id x of the same row.
 
 The fp64 reference builds the scores with the bias vector gathered at k - q, masks them with the segment pattern and applies
@@ -372,7 +372,7 @@ def _strides(*ts):
     return [t.stride(1) for t in ts], [t.stride(2) for t in ts]
 
 
-def test_refusals():
+def test_form_refusals():
     S = 128
     st, en = ops.segment_bounds(torch.zeros((1, S), dtype=torch.int64, device=DEV))
     rel = torch.zeros(H, 2 * S - 1, device=DEV)
@@ -392,41 +392,43 @@ def test_refusals():
     ws_need = int(L.load().fsb_sdpa_bwd_workspace_bytes(1, S, S, H))
     ws = torch.empty(ws_need, dtype=torch.uint8, device=DEV)
 
-    def fwd(name, p, S=S, Skv=S, bounds=True, bias=True, d=64):
-        ptr = lambda t: t.data_ptr() if bounds else None
-        tail = ((1, rel.data_ptr() if bias else None) if name == "fsb_sdpa_fwd_segments_bias" else (ptr(st), ptr(en)))
-        L.call(name, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), 1, S, Skv, H, d, rs, rs, rs,
-               ors, hs, hs, hs, ohs, 0.125, ptr(st), ptr(en), *tail, p, SEED, _base().data_ptr(), SITE, None)
+    def fwd(p, S=S, Skv=S, bounds=(st, en), qb=(None, None), causal=1, bias=True, d=64):
+        L.call("fsb_sdpa_fwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), 1, S, Skv, H, d,
+               rs, rs, rs, ors, hs, hs, hs, ohs, 0.125, causal, None, rel.data_ptr() if bias else None,
+               *map(ops._p, bounds + qb), p, SEED, _base().data_ptr(), SITE, None)
 
-    def bwd(name, p, S=S, Skv=S, bounds=True, bias=True, drel=False, ws_bytes=ws_need):
-        ptr = lambda t: t.data_ptr() if bounds else None
-        if name == "fsb_sdpa_bwd_segments_bias":
-            tail = (1, rel.data_ptr() if bias else None, rel.data_ptr() if drel else None, ws.data_ptr(), ws_bytes)
-        else:
-            tail = (ptr(st), ptr(en))
-        L.call(name, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), o.data_ptr(), lse.data_ptr(),
+    def bwd(p, S=S, Skv=S, bounds=(st, en), qb=(None, None), causal=1, bias=True, drel=False, ws_bytes=ws_need):
+        L.call("fsb_sdpa_bwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), o.data_ptr(), lse.data_ptr(),
                delta.data_ptr(), o.data_ptr(), o.data_ptr(), o.data_ptr(), 1, S, Skv, H, 64, rs, rs, rs, ors, ors, ors,
-               ors, ors, hs, hs, hs, ohs, ohs, ohs, ohs, ohs, 0.125, ptr(st), ptr(en), *tail, p, SEED,
+               ors, ors, hs, hs, hs, ohs, ohs, ohs, ohs, ohs, 0.125, causal, None, rel.data_ptr() if bias else None,
+               rel.data_ptr() if drel else None, ws.data_ptr(), ws_bytes, *map(ops._p, bounds + qb), p, SEED,
                _base().data_ptr(), SITE, None)
 
-    for call, name in ((fwd, "fsb_sdpa_fwd_segments_bias"), (fwd, "fsb_sdpa_fwd_segments_cross"),
-                       (bwd, "fsb_sdpa_bwd_segments_bias"), (bwd, "fsb_sdpa_bwd_segments_cross")):
-        for bad in (1.0, -0.1):
-            with pytest.raises(RuntimeError, match="outside"):
-                call(name, bad)
-        with pytest.raises(RuntimeError, match="65536"):
-            call(name, 0.1, S=65537, Skv=65537)
-        with pytest.raises(RuntimeError, match="null segment bounds"):
-            call(name, 0.1, bounds=False)
-    for name in ("fsb_sdpa_fwd_segments_bias", "fsb_sdpa_bwd_segments_bias"):
+    biased, cross = dict(causal=1, bias=True), dict(causal=0, bias=False, qb=(st, en))
+    for call in (fwd, bwd):
+        for form in (biased, cross):
+            for bad in (1.0, -0.1):
+                with pytest.raises(RuntimeError, match="outside"):
+                    call(bad, **form)
+            with pytest.raises(RuntimeError, match="65536"):
+                call(0.1, S=65537, Skv=65537, **form)
+            for half in ((st, None), (None, en)):
+                with pytest.raises(RuntimeError, match="null segment bounds"):
+                    call(0.1, **dict(form, bounds=half))
+        # the key-side bounds of the cross form: both or neither, and only beside the query-side ones
+        for qb, bounds in (((st, None), (st, en)), ((None, en), (st, en)), ((st, en), (None, None))):
+            with pytest.raises(RuntimeError, match="null segment bounds"):
+                call(0.1, **dict(cross, qb=qb, bounds=bounds))
         with pytest.raises(RuntimeError, match="seq_q == seq_kv"):
-            (fwd if "fwd" in name else bwd)(name, 0.0, Skv=64)
-        with pytest.raises(RuntimeError, match="null rel_bias"):
-            (fwd if "fwd" in name else bwd)(name, 0.0, bias=False)
+            call(0.0, Skv=64, **biased)
+        # the cross form has no causal mask and no bias
+        for extra in (dict(causal=1), dict(bias=True)):
+            with pytest.raises(RuntimeError, match="cross segments take no causal mask and no rel_bias"):
+                call(0.0, **dict(cross, **extra))
     with pytest.raises(RuntimeError, match="workspace"):
-        bwd("fsb_sdpa_bwd_segments_bias", 0.0, drel=True, ws_bytes=ws_need - 16)
+        bwd(0.0, drel=True, ws_bytes=ws_need - 16, **biased)
     with pytest.raises(RuntimeError, match="head_dim 128 unsupported"):
-        fwd("fsb_sdpa_fwd_segments_cross", 0.0, d=128)
+        fwd(0.0, d=128, **cross)
     # ops-level: no bias with the cross form, the cross form is not causal, drel_bias needs rel_bias
     with pytest.raises(RuntimeError, match="takes no rel_bias"):
         ops.sdpa_segments_fwd(q, k, v, 0.1, st, en, causal=False, rel_bias=rel, kv_bounds=(st, en))

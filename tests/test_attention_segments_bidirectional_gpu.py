@@ -1,5 +1,5 @@
 """GPU: segment-masked bidirectional attention, with and without dropout on its probabilities
-(fsb_sdpa_{fwd,bwd}_segments_bidirectional, ops.sdpa_segments_*(causal=False)), the attention of packed BERT / MegatronBERT
+(the bidirectional segment form of fsb_sdpa_{fwd,bwd}, ops.sdpa_segments_*(causal=False)), the attention of packed BERT / MegatronBERT
 pretraining.
 
 Key k is visible to query q iff both lie in the same segment. The keep mask of an element is that of the attention layout in
@@ -189,7 +189,7 @@ def test_p_zero_is_the_dropout_free_kernel_bit_for_bit():
 
 
 def test_default_causal_keeps_the_causal_segment_kernels():
-    """causal=True (the default) still launches fsb_sdpa_*_segments[_dropout]: the result is causal inside a segment."""
+    """causal=True (the default) still launches the causal segment kernels: the result is causal inside a segment."""
     S = 128
     seg_ids = _rows_from_lengths([[64, 64]], S)
     qkv, dout = _case(1, S, seed=17)
@@ -202,7 +202,7 @@ def test_default_causal_keeps_the_causal_segment_kernels():
     assert not torch.equal(o_bi[:, 0], v[:, 0])
 
 
-def test_refusals():
+def test_form_refusals():
     st, en = ops.segment_bounds(torch.zeros((1, 128), dtype=torch.int64, device=DEV))
     qkv = torch.zeros(1, 128, 3, 2, 128, dtype=torch.bfloat16, device=DEV)
     q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
@@ -217,36 +217,36 @@ def test_refusals():
     lse = torch.empty(1, 2, 128, dtype=torch.float32, device=DEV)
     rs, hs = qkv.stride(1), qkv.stride(3)
 
-    def fwd(p, S=128, Skv=None, bounds=True):
-        L.call("fsb_sdpa_fwd_segments_bidirectional", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+    def fwd(p, S=128, Skv=None, bounds=(st, en)):
+        L.call("fsb_sdpa_fwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                lse.data_ptr(), 1, S, S if Skv is None else Skv, 2, 64, rs, rs, rs, o.stride(1), hs, hs, hs, o.stride(2),
-               0.125, st.data_ptr() if bounds else None, en.data_ptr() if bounds else None, p, SEED, _base().data_ptr(),
-               SITE, None)
+               0.125, 0, None, None, *map(ops._p, bounds), None, None, p, SEED, _base().data_ptr(), SITE, None)
     for bad in (1.0, -0.1):
         with pytest.raises(RuntimeError, match="outside"):
             fwd(bad)
     with pytest.raises(RuntimeError, match="65536"):
         fwd(0.1, S=65537)
-    with pytest.raises(RuntimeError, match="null segment bounds"):
-        fwd(0.1, bounds=False)
+    for half in ((st, None), (None, en)):
+        with pytest.raises(RuntimeError, match="null segment bounds"):
+            fwd(0.1, bounds=half)
     with pytest.raises(RuntimeError, match="seq_q == seq_kv"):
         fwd(0.0, Skv=64)
     dq = torch.empty_like(o)
 
-    def bwd(p, S=128, Skv=None, bounds=True):
+    def bwd(p, S=128, Skv=None, bounds=(st, en)):
         delta = torch.empty(1, 2, 128, dtype=torch.float32, device=DEV)
-        L.call("fsb_sdpa_bwd_segments_bidirectional", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+        L.call("fsb_sdpa_bwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                o.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dq.data_ptr(), dq.data_ptr(), 1, S,
                S if Skv is None else Skv, 2, 64, rs, rs, rs, o.stride(1), o.stride(1), o.stride(1), o.stride(1),
                o.stride(1), hs, hs, hs, o.stride(2), o.stride(2), o.stride(2), o.stride(2), o.stride(2), 0.125,
-               st.data_ptr() if bounds else None, en.data_ptr() if bounds else None, p, SEED, _base().data_ptr(), SITE,
-               None)
+               0, None, None, None, None, 0, *map(ops._p, bounds), None, None, p, SEED, _base().data_ptr(), SITE, None)
     with pytest.raises(RuntimeError, match="outside"):
         bwd(1.5)
     with pytest.raises(RuntimeError, match="65536"):
         bwd(0.1, S=65537)
-    with pytest.raises(RuntimeError, match="null segment bounds"):
-        bwd(0.1, bounds=False)
+    for half in ((st, None), (None, en)):
+        with pytest.raises(RuntimeError, match="null segment bounds"):
+            bwd(0.1, bounds=half)
     with pytest.raises(RuntimeError, match="seq_q == seq_kv"):
         bwd(0.0, Skv=64)
 

@@ -1,5 +1,5 @@
-"""GPU: segment-masked causal attention with dropout on its probabilities (fsb_sdpa_{fwd,bwd}_segments_dropout,
-ops.sdpa_segments_*(drop=...)), the attention of packed GPT-2 training.
+"""GPU: segment-masked causal attention with dropout on its probabilities (the causal segment form of
+fsb_sdpa_{fwd,bwd} with p > 0, ops.sdpa_segments_*(drop=...)), the attention of packed GPT-2 training.
 
 The keep mask of an element is that of the attention layout in include/fsb200.h at its row-relative (q, k), rebuilt here by
 the numpy Philox of tests/philox_ref.py, never read from the library; the fp64 reference applies it under the block-diagonal
@@ -192,7 +192,7 @@ def test_p_zero_is_the_segment_kernel_bit_for_bit():
     assert all(torch.equal(x, y) for x, y in zip(a, b))
 
 
-def test_refusals():
+def test_form_refusals():
     drop = ops.Dropout(0.1, SEED, _base(), SITE)
     st, en = ops.segment_bounds(torch.zeros((1, 128), dtype=torch.int64, device=DEV))
     qkv = torch.zeros(1, 128, 3, 2, 128, dtype=torch.bfloat16, device=DEV)
@@ -210,30 +210,37 @@ def test_refusals():
     lse = torch.empty(1, 2, 128, dtype=torch.float32, device=DEV)
     rs, hs = qkv.stride(1), qkv.stride(3)
 
-    def fwd(p, S=128, bounds=True):
-        L.call("fsb_sdpa_fwd_segments_dropout", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
-               1, S, S, 2, 64, rs, rs, rs, o.stride(1), hs, hs, hs, o.stride(2), 0.125,
-               st.data_ptr() if bounds else None, en.data_ptr() if bounds else None, p, SEED, _base().data_ptr(), SITE,
-               None)
+    mask = torch.ones(1, 128, dtype=torch.uint8, device=DEV)
+
+    def fwd(p, S=128, bounds=(st, en), kv_mask=None):
+        L.call("fsb_sdpa_fwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+               1, S, S, 2, 64, rs, rs, rs, o.stride(1), hs, hs, hs, o.stride(2), 0.125, 1, ops._p(kv_mask), None,
+               *map(ops._p, bounds), None, None, p, SEED, _base().data_ptr(), SITE, None)
     for bad in (1.0, -0.1):
         with pytest.raises(RuntimeError, match="outside"):
             fwd(bad)
     with pytest.raises(RuntimeError, match="65536"):
         fwd(0.1, S=65537)
-    with pytest.raises(RuntimeError, match="null segment bounds"):
-        fwd(0.1, bounds=False)
+    for half in ((st, None), (None, en)):
+        with pytest.raises(RuntimeError, match="null segment bounds"):
+            fwd(0.1, bounds=half)
+    with pytest.raises(RuntimeError, match="kv_mask"):
+        fwd(0.1, kv_mask=mask)
     dq = torch.empty_like(o)
 
-    def bwd(p, S=128, bounds=True):
+    def bwd(p, S=128, bounds=(st, en), kv_mask=None):
         delta = torch.empty(1, 2, 128, dtype=torch.float32, device=DEV)
-        L.call("fsb_sdpa_bwd_segments_dropout", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), o.data_ptr(),
+        L.call("fsb_sdpa_bwd", q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), o.data_ptr(),
                lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dq.data_ptr(), dq.data_ptr(), 1, S, S, 2, 64,
                rs, rs, rs, o.stride(1), o.stride(1), o.stride(1), o.stride(1), o.stride(1), hs, hs, hs, o.stride(2),
-               o.stride(2), o.stride(2), o.stride(2), o.stride(2), 0.125, st.data_ptr() if bounds else None,
-               en.data_ptr() if bounds else None, p, SEED, _base().data_ptr(), SITE, None)
+               o.stride(2), o.stride(2), o.stride(2), o.stride(2), 0.125, 1, ops._p(kv_mask), None, None, None, 0,
+               *map(ops._p, bounds), None, None, p, SEED, _base().data_ptr(), SITE, None)
     with pytest.raises(RuntimeError, match="outside"):
         bwd(1.5)
     with pytest.raises(RuntimeError, match="65536"):
         bwd(0.1, S=65537)
-    with pytest.raises(RuntimeError, match="null segment bounds"):
-        bwd(0.1, bounds=False)
+    for half in ((st, None), (None, en)):
+        with pytest.raises(RuntimeError, match="null segment bounds"):
+            bwd(0.1, bounds=half)
+    with pytest.raises(RuntimeError, match="kv_mask"):
+        bwd(0.1, kv_mask=mask)

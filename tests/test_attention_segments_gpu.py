@@ -1,4 +1,5 @@
-"""GPU: segment-masked causal attention (fsb_sdpa_fwd_segments / fsb_sdpa_bwd_segments, ops.sdpa_segments_*) for packed rows.
+"""GPU: segment-masked causal attention (the causal segment form of fsb_sdpa_fwd / fsb_sdpa_bwd, ops.sdpa_segments_*) for
+packed rows.
 
 Each segment of a packed row is an independent causal attention, so every segment is checked against the fp64 bounds of the
 causal launch checkers (tests/launch_refs.py verify_sdpa_fwd / verify_sdpa_bwd) run on that segment's slices alone. Exact
@@ -190,11 +191,14 @@ def test_second_run_is_bit_identical():
                            y.view(torch.int16) if y.dtype == torch.bfloat16 else y.view(torch.int32))
 
 
-def test_refusals():
+def test_head_dim_96_runs_without_drop_and_seq_mismatch_refuses():
     st, en = ops.segment_bounds(torch.zeros((1, 128), dtype=torch.int64, device=DEV))
-    qkv = torch.zeros(1, 128, 2, 3, 96, dtype=torch.bfloat16, device=DEV)
-    with pytest.raises(RuntimeError, match="head_dim 96"):
-        ops.sdpa_segments_fwd(qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2], 0.1, st, en)
+    # head_dim 96 without a drop is no refusal: it runs the kernels a Dropout(0.0) selects, bit for bit
+    qkv = torch.randn(1, 128, 3, 2, 96, generator=torch.Generator().manual_seed(3)).to(DEV, torch.bfloat16)
+    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+    zero = ops.Dropout(0.0, 0, torch.zeros(1, dtype=torch.int64, device=DEV), 0)
+    for a, b in zip(ops.sdpa_segments_fwd(q, k, v, 0.1, st, en), ops.sdpa_segments_fwd(q, k, v, 0.1, st, en, drop=zero)):
+        assert torch.equal(a, b)
     q = torch.zeros(1, 128, 2, 64, dtype=torch.bfloat16, device=DEV)
     kv = torch.zeros(1, 256, 2, 64, dtype=torch.bfloat16, device=DEV)
     with pytest.raises(RuntimeError, match="seq_q == seq_kv"):

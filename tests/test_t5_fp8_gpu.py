@@ -266,12 +266,13 @@ def test_write_footprint_of_every_launch_of_a_c5_width_fp8_step(monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- bf16 unchanged
-def test_fp8_false_launch_sequence_is_the_bf16_models(monkeypatch):
+def test_fp8_false_launch_sequence_matches_the_bf16_record(monkeypatch):
     """fp8=False launches exactly what the model launched before it had an FP8 path: every kernel, in order, with its
     integer arguments (sizes, strides, flags, dropout sites, scratch sizes; device pointers and the stream left out), over two
     micro-batches of a dropout-0.1 step with GA 2 and the optimizer step, a packed step, a no-grad forward and a greedy
     generate. tests/golden/t5_bf16_launches.json holds that sequence, recorded on an H100 80GB HBM3 from the model as it
-    was before fp8 existed."""
+    was before fp8 existed, with the attention rows since translated to the current entry names fsb_sdpa_fwd /
+    fsb_sdpa_bwd (the integer arguments the old entries did not take inserted at the values the model passes)."""
     from transformers import MT5Config
     want = json.load(open(os.path.join(ROOT, "tests", "golden", "t5_bf16_launches.json")))
     got = []

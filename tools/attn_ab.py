@@ -1,5 +1,5 @@
-"""A/B tool for the attention kernels: save every output of every fsb_sdpa_* entry point over a fixed seeded case matrix,
-compare two such saves byte for byte, or time the forward and backward at the benchmark workloads' shapes.
+"""A/B tool for the attention kernels: save every output of every form of fsb_sdpa_fwd / fsb_sdpa_bwd over a fixed seeded
+case matrix, compare two such saves byte for byte, or time the forward and backward at the benchmark workloads' shapes.
 
     python tools/attn_ab.py --save DIR              # one .npy per output per case (needs a GPU)
     python tools/attn_ab.py --compare DIR_A DIR_B   # byte-equal check of two saves (CPU only); exit 1 on any difference

@@ -17,19 +17,19 @@ No corpus is read: the length mix is a seeded log-normal chosen here, and the ga
          the source pads only. Packed rows: 4 x 128 = 512 encoder tokens and 4 x 64 = 256 decoder tokens.
 
 1. Attention at the model's head shape (llama: 40 heads x 128, S 2048; gpt2: 12 heads x 64, S 1024, attention dropout
-   p = 0.1): the samples packed first fit into `--rows` rows. The segment kernels (fsb_sdpa_{fwd,bwd}_segments, with
-   dropout: fsb_sdpa_{fwd,bwd}_segments_dropout) against what the padded batch runs today: llama fsb_sdpa_fwd / _bwd with
-   causal = 1 on the same [rows, S] tensors; gpt2 the causal + key-mask + dropout kernels (fsb_sdpa_{fwd,bwd}_dropout) on
+   p = 0.1): the samples packed first fit into `--rows` rows. The segment kernels (the causal segment form of
+   fsb_sdpa_{fwd,bwd}, with or without dropout) against what the padded batch runs today: llama fsb_sdpa_fwd / _bwd with
+   causal = 1 on the same [rows, S] tensors; gpt2 the causal + key-mask + dropout kernels (fsb_sdpa_{fwd,bwd} with p > 0) on
    the padded [samples, S] tensors, one sample per row; megatronbert (32 heads x 64, S 512, p = 0.1) the bidirectional
-   segment kernels (fsb_sdpa_{fwd,bwd}_segments_bidirectional) against the non-causal key-mask + dropout kernels on the
+   segment kernels (the bidirectional segment form of fsb_sdpa_{fwd,bwd}) against the non-causal key-mask + dropout kernels on the
    padded [samples, S] tensors, and the FLOPs of a segment are 4 D H n^2 (every pair inside it). Device time per call (10 calls captured in one CUDA graph, replayed
    under CUDA events), alternated `--reps` times (medians and spread). TFLOP/s over the FLOPs the block-diagonal mask
    needs, counted from the lengths: forward 4 D H n (n + 1) / 2 per segment of n tokens (QK^T and PV over the causal
    pairs), backward 2.5 times that; the pad tail is not counted.
    mt5 (C5 head shape, 16 heads x 64, dropout 0.1): the three packed forms against what the padded batch runs today on
-   [samples, 128] / [samples, 64]: the encoder (fsb_sdpa_*_segments_bias, bidirectional) against the bias + key-mask
-   kernels, the decoder self-attention (fsb_sdpa_*_segments_bias, causal) against the causal bias kernels, and the
-   cross-attention (fsb_sdpa_*_segments_cross) against the key-mask kernels; FLOPs counted from the real pairs.
+   [samples, 128] / [samples, 64]: the encoder (the biased segment form, bidirectional) against the bias + key-mask
+   kernels, the decoder self-attention (the biased segment form, causal) against the causal bias kernels, and the
+   cross-attention (the cross segment form) against the key-mask kernels; FLOPs counted from the real pairs.
 2. The step, eager PretrainStep, `--samples` samples per micro-batch, padded against packed (fsb200/packing.py, rows of S).
    llama: Ziya width (hidden 5120, 40 heads, vocabulary 39424) at 4 layers, padded by the reference collator's dynamic
    padding to the longest sample. gpt2: GPT-2-110M (12 layers, hidden 768, vocabulary 50264) with the released dropout 0.1
