@@ -26,6 +26,11 @@
 //   * When the output tiles leave SMs idle (decode), K is split: split j writes its fp32 partial product to the caller's
 //     workspace and a second kernel sums the splits in order, scales (int8), rounds and stores D. The plan is a function of
 //     (m, n, k) and the SM count only, so graph replays equal eager calls bit for bit.
+//   * fsb_gemm_{w8a16,w4a16}_bias (GPT-2's Conv1D projections): the kEpi instantiations add bias[n] to the scaled sum and
+//     optionally apply gelu_tanh_f (gemm_epilogue.cuh, the bf16 and FP8 GEMMs' device code) before the one rounding, in the
+//     unsplit kernel's epilogue or, when K is split, in the reduce kernel after the splits are summed: once per element. The
+//     plain instantiations (fsb_gemm_w8a16 / fsb_gemm_w4a16) carry none of that code.
+#include "gemm_epilogue.cuh"
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -77,7 +82,22 @@ struct WqParams {
   float* ws;          // split-K partials [splits, M, N] fp32, or nullptr
   int M, N, K;
   int tiles_t, tiles_n, splits, num_kb;
+  const __nv_bfloat16* bias;   // [N]; read by the kEpi instantiations only (appended: the plain ones keep their offsets)
 };
+
+// The epilogue forms: what happens to the fp32 sum (scaled by s[n] for int8) before its one rounding to bf16
+constexpr int WQ_PLAIN = 0;       // nothing (fsb_gemm_w8a16 / fsb_gemm_w4a16)
+constexpr int WQ_BIAS = 1;        // + bias[n]
+constexpr int WQ_BIAS_GELU = 2;   // gelu_tanh(. + bias[n]) (GPT-2's c_fc: gelu_new)
+
+template <int kEpi>
+__device__ __forceinline__ float wq_epilogue(float v, float b) {
+  if constexpr (kEpi != WQ_PLAIN) {
+    v = __fadd_rn(v, b);   // never contracted with the int8 scale multiply: the unsplit and split paths round alike
+    if constexpr (kEpi == WQ_BIAS_GELU) v = gelu_tanh_f(v);
+  }
+  return v;
+}
 
 // Four int8 (bytes of x) -> two bf16x2 (bytes 0,1 -> lo; bytes 2,3 -> hi), exactly: x + 128 is placed in the mantissa of
 // 2^23 (fp32 0x4B000000 | (x ^ 0x80)), 2^23 + 128 is subtracted, and the integer result, at most 8 significant bits, keeps its
@@ -102,7 +122,7 @@ __device__ __forceinline__ uint32_t i4x2_to_bf16x2(uint32_t x, uint32_t s2) {
   return w;
 }
 
-template <class F, int BT>
+template <class F, int BT, int kEpi>
 __global__ void __launch_bounds__(W8_THREADS, 1)
 gemm_wq_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA,
                const __grid_constant__ CUtensorMap tmD, const WqParams p) {
@@ -254,6 +274,11 @@ gemm_wq_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         s0 = nrow0 < p.N ? __ldg(scale + nrow0) : 0.f;
         s1 = nrow1 < p.N ? __ldg(scale + nrow1) : 0.f;
       }
+      float b0 = 0.f, b1 = 0.f;
+      if constexpr (kEpi != WQ_PLAIN) {
+        b0 = nrow0 < p.N ? __bfloat162float(__ldg(p.bias + nrow0)) : 0.f;
+        b1 = nrow1 < p.N ? __bfloat162float(__ldg(p.bias + nrow1)) : 0.f;
+      }
       uint8_t* buf = smem + S::EPI_OFFSET + wg * (BT * 128);
       const int lr = wl * 16 + F::kRowsPerLine * g;   // weight row inside the warpgroup's 64 (the staging tile's column)
 #pragma unroll
@@ -261,9 +286,10 @@ gemm_wq_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int tok = 8 * j + 2 * tq + e;
-          *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * lr)) = __float2bfloat16_rn(acc[4 * j + e] * s0);
+          *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * lr)) =
+              __float2bfloat16_rn(wq_epilogue<kEpi>(acc[4 * j + e] * s0, b0));
           *reinterpret_cast<__nv_bfloat16*>(buf + swz128(tok, 2 * (lr + F::kPartner))) =
-              __float2bfloat16_rn(acc[4 * j + 2 + e] * s1);
+              __float2bfloat16_rn(wq_epilogue<kEpi>(acc[4 * j + 2 + e] * s1, b1));
         }
       fence_proxy_async();
       bar_sync(1 + wg, 128);
@@ -277,10 +303,12 @@ gemm_wq_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
 }
 
 // D[m, n:n+8] = bf16(s[n:n+8] * sum over splits of ws[split, m, n:n+8]), splits summed in order; int4 (kRowScale false)
-// stores the sum unscaled
-template <bool kRowScale>
+// stores the sum unscaled. kEpi: then the bias / GELU of wq_epilogue, as the unsplit kernel applies them (bias: the last
+// parameter, read by those instantiations only).
+template <bool kRowScale, int kEpi>
 __global__ void wq_splitk_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ scale, int splits, int64_t M,
-                                        int64_t N, __nv_bfloat16* __restrict__ D, int64_t ldd) {
+                                        int64_t N, __nv_bfloat16* __restrict__ D, int64_t ldd,
+                                        const __nv_bfloat16* __restrict__ bias) {
   const int64_t n8 = N / 8;
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < M * n8; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t m = i / n8, n = (i - m * n8) * 8;
@@ -296,6 +324,13 @@ __global__ void wq_splitk_reduce_kernel(const float* __restrict__ ws, const floa
     if constexpr (kRowScale) {
       const float4 s0 = *reinterpret_cast<const float4*>(scale + n), s1 = *reinterpret_cast<const float4*>(scale + n + 4);
       v[0] *= s0.x; v[1] *= s0.y; v[2] *= s0.z; v[3] *= s0.w; v[4] *= s1.x; v[5] *= s1.y; v[6] *= s1.z; v[7] *= s1.w;
+    }
+    if constexpr (kEpi != WQ_PLAIN) {
+      const uint4 bv = *reinterpret_cast<const uint4*>(bias + n);
+      v[0] = wq_epilogue<kEpi>(v[0], bf16lo(bv.x)); v[1] = wq_epilogue<kEpi>(v[1], bf16hi(bv.x));
+      v[2] = wq_epilogue<kEpi>(v[2], bf16lo(bv.y)); v[3] = wq_epilogue<kEpi>(v[3], bf16hi(bv.y));
+      v[4] = wq_epilogue<kEpi>(v[4], bf16lo(bv.z)); v[5] = wq_epilogue<kEpi>(v[5], bf16hi(bv.z));
+      v[6] = wq_epilogue<kEpi>(v[6], bf16lo(bv.w)); v[7] = wq_epilogue<kEpi>(v[7], bf16hi(bv.w));
     }
     *reinterpret_cast<uint4*>(D + m * ldd + n) = pack8(v);
   }
@@ -400,22 +435,46 @@ static size_t wq_workspace_bytes(int64_t m, int64_t n, int64_t k) {
   return plan.splits > 1 ? size_t(plan.splits) * size_t(m) * size_t(n) * sizeof(float) : 0;
 }
 
-template <class F, int BT>
+template <class F, int BT, int kEpi>
 static int launch_wq(const CUtensorMap& tmW, const CUtensorMap& tmA, const CUtensorMap& tmD, const WqParams& p,
                      cudaStream_t stream, const char* what) {
   using S = WqSmem<F, BT>;
-  if (int rc = ensure_smem<gemm_wq_kernel<F, BT>>(S::TOTAL, what)) return rc;
+  if (int rc = ensure_smem<gemm_wq_kernel<F, BT, kEpi>>(S::TOTAL, what)) return rc;
   const int64_t grid = int64_t(p.tiles_t) * p.tiles_n * p.splits;
-  gemm_wq_kernel<F, BT><<<unsigned(grid), W8_THREADS, S::TOTAL, stream>>>(tmW, tmA, tmD, p);
+  gemm_wq_kernel<F, BT, kEpi><<<unsigned(grid), W8_THREADS, S::TOTAL, stream>>>(tmW, tmA, tmD, p);
   FSB_CUDA_LAUNCH_CHECK();
   return FSB_OK;
 }
 
-// The checks and launch shared by fsb_gemm_w8a16 and fsb_gemm_w4a16 (`what` names the entry in messages). The format's own
-// k requirement is checked by the caller.
+// The GEMM kernel for the plan's token-tile width, then (K split) the reduce kernel
+template <class F, int kEpi>
+static int run_wq(const CUtensorMap& tmW, const CUtensorMap& tmA, const CUtensorMap& tmD, const WqParams& p, int bt,
+                  int64_t m, int64_t n, const void* s, void* d, int64_t ldd, cudaStream_t stream, const char* what) {
+  int rc = FSB_ERR_INVALID;
+  switch (bt) {
+    case 8: rc = launch_wq<F, 8, kEpi>(tmW, tmA, tmD, p, stream, what); break;
+    case 16: rc = launch_wq<F, 16, kEpi>(tmW, tmA, tmD, p, stream, what); break;
+    case 32: rc = launch_wq<F, 32, kEpi>(tmW, tmA, tmD, p, stream, what); break;
+    case 64: rc = launch_wq<F, 64, kEpi>(tmW, tmA, tmD, p, stream, what); break;
+    default: rc = launch_wq<F, 128, kEpi>(tmW, tmA, tmD, p, stream, what); break;
+  }
+  if (rc || p.splits == 1) return rc;
+  const int64_t work = m * (n / 8);
+  const int blocks = int(work / 256 + 1 < 4 * num_sms() ? work / 256 + 1 : 4 * num_sms());
+  wq_splitk_reduce_kernel<F::kRowScale, kEpi><<<blocks, 256, 0, stream>>>(
+      p.ws, static_cast<const float*>(F::kRowScale ? s : nullptr), p.splits, m, n, static_cast<__nv_bfloat16*>(d), ldd,
+      p.bias);
+  FSB_CUDA_LAUNCH_CHECK();
+  return FSB_OK;
+}
+
+// The checks and launch shared by fsb_gemm_{w8a16,w4a16}[_bias] (`what` names the entry in messages). The format's own
+// k requirement is checked by the caller. bias == nullptr: the plain GEMM (epilogue ignored); otherwise `epilogue`, already
+// checked to be FSB_EPI_NONE or FSB_EPI_GELU_TANH, selects the bias form.
 template <class F>
 static int gemm_wq(const char* what, int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const void* q,
-                   const void* s, void* d, int64_t ldd, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                   const void* s, const void* bias, int epilogue, void* d, int64_t ldd, void* workspace,
+                   size_t workspace_bytes, cudaStream_t stream) {
   FSB_REQUIRE(n % 8 == 0, "%s: n=%ld must be a multiple of 8", what, (long)n);
   FSB_REQUIRE(a && q && s && d, "%s: null operand", what);
   FSB_REQUIRE(aligned16(a) && aligned16(q) && aligned16(s) && aligned16(d), "%s: a, q, s and d must be 16-byte aligned",
@@ -460,20 +519,18 @@ static int gemm_wq(const char* what, int64_t m, int64_t n, int64_t k, const void
   p.tiles_n = int((n + W8_BM - 1) / W8_BM);
   p.splits = plan.splits;
   p.num_kb = int((k + W8_BK - 1) / W8_BK);
-  int rc = FSB_ERR_INVALID;
-  switch (plan.bt) {
-    case 8: rc = launch_wq<F, 8>(tmW, tmA, tmD, p, stream, what); break;
-    case 16: rc = launch_wq<F, 16>(tmW, tmA, tmD, p, stream, what); break;
-    case 32: rc = launch_wq<F, 32>(tmW, tmA, tmD, p, stream, what); break;
-    case 64: rc = launch_wq<F, 64>(tmW, tmA, tmD, p, stream, what); break;
-    default: rc = launch_wq<F, 128>(tmW, tmA, tmD, p, stream, what); break;
-  }
-  if (rc || plan.splits == 1) return rc;
-  const int64_t work = m * (n / 8);
-  const int blocks = int(work / 256 + 1 < 4 * num_sms() ? work / 256 + 1 : 4 * num_sms());
-  wq_splitk_reduce_kernel<F::kRowScale><<<blocks, 256, 0, stream>>>(p.ws, static_cast<const float*>(F::kRowScale ? s : nullptr),
-                                                                   plan.splits, m, n, static_cast<__nv_bfloat16*>(d), ldd);
-  FSB_CUDA_LAUNCH_CHECK();
+  p.bias = static_cast<const __nv_bfloat16*>(bias);
+  if (bias == nullptr) return run_wq<F, WQ_PLAIN>(tmW, tmA, tmD, p, plan.bt, m, n, s, d, ldd, stream, what);
+  if (epilogue == FSB_EPI_GELU_TANH) return run_wq<F, WQ_BIAS_GELU>(tmW, tmA, tmD, p, plan.bt, m, n, s, d, ldd, stream, what);
+  return run_wq<F, WQ_BIAS>(tmW, tmA, tmD, p, plan.bt, m, n, s, d, ldd, stream, what);
+}
+
+// The checks of the _bias entries' extra operands
+static int check_wq_bias(const char* what, const void* bias, int epilogue) {
+  FSB_REQUIRE(bias != nullptr, "%s: bias must not be NULL (the entry without _bias is the bias-free GEMM)", what);
+  FSB_REQUIRE(aligned16(bias), "%s: bias must be 16-byte aligned", what);
+  FSB_REQUIRE(epilogue == FSB_EPI_NONE || epilogue == FSB_EPI_GELU_TANH,
+              "%s: epilogue=%d unsupported (FSB_EPI_NONE or FSB_EPI_GELU_TANH)", what, epilogue);
   return FSB_OK;
 }
 
@@ -502,7 +559,19 @@ extern "C" int fsb_gemm_w8a16(int64_t m, int64_t n, int64_t k, const void* a, in
   FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w8a16: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
   FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w8a16: dims too large");
   FSB_REQUIRE(k % 16 == 0, "gemm_w8a16: k=%ld must be a multiple of 16", (long)k);
-  return gemm_wq<FmtW8>("gemm_w8a16", m, n, k, a, lda, q, s, d, ldd, workspace, workspace_bytes,
+  return gemm_wq<FmtW8>("gemm_w8a16", m, n, k, a, lda, q, s, nullptr, FSB_EPI_NONE, d, ldd, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int fsb_gemm_w8a16_bias(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const int8_t* q,
+                                   const float* s, const void* bias, int epilogue, void* d, int64_t ldd, void* workspace,
+                                   size_t workspace_bytes, fsb_stream_t stream_) {
+  FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w8a16_bias: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
+  FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w8a16_bias: dims too large");
+  FSB_REQUIRE(k % 16 == 0, "gemm_w8a16_bias: k=%ld must be a multiple of 16", (long)k);
+  if (int rc = check_wq_bias("gemm_w8a16_bias", bias, epilogue)) return rc;
+  // the plan and its workspace are fsb_gemm_w8a16's: named after it in the workspace message
+  return gemm_wq<FmtW8>("gemm_w8a16", m, n, k, a, lda, q, s, bias, epilogue, d, ldd, workspace, workspace_bytes,
                         static_cast<cudaStream_t>(stream_));
 }
 
@@ -534,6 +603,17 @@ extern "C" int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, in
   FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w4a16: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
   FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w4a16: dims too large");
   FSB_REQUIRE(k % W4_GROUP == 0, "gemm_w4a16: k=%ld must be a multiple of %d (the scale group)", (long)k, W4_GROUP);
-  return gemm_wq<FmtW4>("gemm_w4a16", m, n, k, a, lda, q, s, d, ldd, workspace, workspace_bytes,
+  return gemm_wq<FmtW4>("gemm_w4a16", m, n, k, a, lda, q, s, nullptr, FSB_EPI_NONE, d, ldd, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int fsb_gemm_w4a16_bias(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q,
+                                   const void* s, const void* bias, int epilogue, void* d, int64_t ldd, void* workspace,
+                                   size_t workspace_bytes, fsb_stream_t stream_) {
+  FSB_REQUIRE(m > 0 && n > 0 && k > 0, "gemm_w4a16_bias: non-positive dims m=%ld n=%ld k=%ld", (long)m, (long)n, (long)k);
+  FSB_REQUIRE(m < (1 << 30) && n < (1 << 30) && k < (1 << 30), "gemm_w4a16_bias: dims too large");
+  FSB_REQUIRE(k % W4_GROUP == 0, "gemm_w4a16_bias: k=%ld must be a multiple of %d (the scale group)", (long)k, W4_GROUP);
+  if (int rc = check_wq_bias("gemm_w4a16_bias", bias, epilogue)) return rc;
+  return gemm_wq<FmtW4>("gemm_w4a16", m, n, k, a, lda, q, s, bias, epilogue, d, ldd, workspace, workspace_bytes,
                         static_cast<cudaStream_t>(stream_));
 }

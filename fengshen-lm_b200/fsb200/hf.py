@@ -31,10 +31,26 @@ def _hf_config(name):
     return getattr(transformers, name)
 
 
+def _device_of_map(device_map, model):
+    """The one device a `device_map` (None, "auto", a device, or a dict of devices) places the model on; None for the default
+    device. A map over several devices raises: the model runs on one GPU."""
+    import torch
+    if device_map is None or device_map == "auto":
+        return None
+    if isinstance(device_map, dict):
+        devs = {torch.device(f"cuda:{v}" if isinstance(v, int) else v) for v in device_map.values()}
+        if len(devs) != 1:
+            raise NotImplementedError(f"fsb200 {model}: device_map over several devices {sorted(map(str, devs))} is not "
+                                      "implemented; the model runs on one GPU")
+        device_map = next(iter(devs))
+    return torch.device(f"cuda:{device_map}" if isinstance(device_map, int) else device_map)
+
+
 class _HFSurface:
     """from_pretrained / forward defaults shared by the four classes."""
     config_name = None
     RETURN_LOGITS = True     # HF outputs always carry logits; scripts that never read them may set this False to skip a copy
+    QUANTIZED = False        # from_pretrained(load_in_8bit / load_in_4bit=True) builds an int8 / int4 model (GPT-2 only)
 
     def __init__(self, config, *args, **kwargs):
         """The reference's HF-backed scripts build the model in LightningModule.__init__, BEFORE the Trainer has initialised
@@ -53,8 +69,18 @@ class _HFSurface:
             raise FileNotFoundError(f"fsb200 {cls.__name__}.from_pretrained: {path!r} is not a local directory "
                                     "(there is no hub access on the product path)")
         # model keywords: fp8 exists on BertForMaskedLM, MegatronBertForPreTraining (fsb200/models/bert.py),
-        # MT5ForConditionalGeneration (fsb200/models/t5.py) and GPT2LMHeadModel (fsb200/models/gpt2.py)
+        # MT5ForConditionalGeneration (fsb200/models/t5.py) and GPT2LMHeadModel (fsb200/models/gpt2.py); load_in_8bit /
+        # load_in_4bit on GPT2LMHeadModel only (the others refuse them rather than load a bf16 model)
         kw = {k: kwargs[k] for k in ("device", "world_size", "seed", "fp8") if k in kwargs}
+        for flag in ("load_in_8bit", "load_in_4bit"):
+            if kwargs.get(flag):
+                if not cls.QUANTIZED:
+                    raise NotImplementedError(f"fsb200 {cls.__name__}.from_pretrained: {flag}=True is not implemented for "
+                                              "this model (int8 / int4 inference covers GPT2LMHeadModel and LLaMA)")
+                kw[flag] = True
+        dev = _device_of_map(kwargs.get("device_map"), cls.__name__)
+        if dev is not None:
+            kw.setdefault("device", dev)
         cfg_cls = _hf_config(cls.config_name)
         if config is not None or state_dict is not None:
             # pretrain_t5.py:34-50: an edited config plus an edited state dict on top of the directory
@@ -89,6 +115,7 @@ class _HFSurface:
 
 class GPT2LMHeadModel(_HFSurface, _gpt2.GPT2LMHeadModel):
     config_name = "GPT2Config"
+    QUANTIZED = True
 
 
 class BertForMaskedLM(_HFSurface, _bert.BertForMaskedLM):

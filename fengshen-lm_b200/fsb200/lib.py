@@ -40,6 +40,10 @@ SIGNATURES = {
     "fsb_gemm_w4a16_workspace_bytes": (c_size, [c_i64, c_i64, c_i64]),
     "fsb_gemm_w4a16": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_size,
                                c_void_p]),
+    "fsb_gemm_w8a16_bias": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                    c_i64, c_void_p, c_size, c_void_p]),
+    "fsb_gemm_w4a16_bias": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                    c_i64, c_void_p, c_size, c_void_p]),
     "fsb_fp8_quantize": (c_int, [c_void_p, c_i64, c_i64, c_i64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "fsb_gemm_fp8": (c_int, [c_i64, c_i64, c_i64, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_i64,
                              c_void_p, c_int, c_int, c_void_p, c_i64, c_void_p]),

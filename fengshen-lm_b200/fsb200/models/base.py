@@ -11,6 +11,7 @@ from torch import nn
 from .. import ops
 from ..flat import FlatBuffers
 from . import export
+from .layers import WQ
 
 
 class _Holder(nn.Module):
@@ -183,7 +184,14 @@ class FlatModel(nn.Module):
     @torch.no_grad()
     def load_reference_state_dict(self, sd):
         """Copy a reference state dict (HF key names; fp32 / fp16 / bf16 tensors on any device) into the parameters. Every
-        parameter's key must be present with its shape; other keys (tied aliases, buffers) are ignored."""
+        parameter's key must be present with its shape; other keys (tied aliases, buffers) are ignored. An int8 / int4
+        model quantises each projection on the device as it arrives (_load_quantized_shard)."""
+        if self.weight_format != "bf16":
+            missing = (set(self._p) | set(self._wq_targets())) - set(sd)
+            if missing:
+                raise KeyError(f"missing key in state dict: {sorted(missing)[0]}")
+            self._load_quantized_shard(sd, set())
+            return
         for k, prm in self._p.items():
             if k not in sd:
                 raise KeyError(f"missing key in state dict: {k}")
@@ -195,6 +203,58 @@ class FlatModel(nn.Module):
     def save_pretrained(self, path, **_):
         """HF-style export (config.json + pytorch_model.bin with this class's HF key names): fsb200/models/export.py."""
         export.save_pretrained(self, path)
+
+    # ---- int8 / int4 inference-only models (load_in_8bit / load_in_4bit: LLaMA, GPT-2) -----------------------------------
+    # Such a model holds its layer projections as layers.QuantizedLinear (q + s) outside the flat buffers and lists them in
+    # `_wq` (per layer {projection: (q, s)}) and `_wq_targets()` ({state-dict key: (q, s) it quantises into}).
+    weight_format = "bf16"   # "int8" / "int4" for those models
+    wq_transposed = False    # the checkpoint stores the projections [in, out] (GPT-2's Conv1D), the transpose of [n, k]
+
+    @staticmethod
+    def _weight_shape(q, s):
+        """[n, k] of the bf16 weight that (q, s) holds: s has one row per weight row in both formats, q the k columns."""
+        return s.shape[0], q.shape[1]
+
+    @torch.no_grad()
+    def _load_quantized_shard(self, sd, loaded):
+        """Load the keys of `sd` (a whole state dict or one checkpoint shard) this int8 / int4 model holds: bf16 parameters
+        are copied, projections quantised on the device (one bf16 temporary at a time, transposed first when the checkpoint
+        stores them [in, out]). The shard's shapes are checked before anything is written. Adds the loaded keys to the set
+        `loaded` and returns the keys it does not yet hold."""
+        targets = self._wq_targets()
+        for k, v in sd.items():
+            want = None
+            if k in self._p:
+                want = tuple(self._p[k].shape)
+            elif k in targets:
+                want = tuple(self._weight_shape(*targets[k]))
+                want = want[::-1] if self.wq_transposed else want
+            if want is not None and tuple(v.shape) != want:
+                raise ValueError(f"shape mismatch for {k}: {tuple(v.shape)} vs {want}")
+        for k, v in sd.items():
+            v = v if v.dtype == torch.bfloat16 else v.to(torch.bfloat16)   # converted where it lies: one bf16 copy on the device
+            if k in self._p:
+                self._p[k].copy_(v)
+            elif k in targets:
+                q, s = targets[k]
+                tmp = v.to(q.device)
+                tmp = (tmp.t() if self.wq_transposed else tmp).contiguous()
+                WQ[self.weight_format][0](tmp, q, s)
+                del tmp
+            else:
+                continue
+            loaded.add(k)
+        return (set(self._p) | set(targets)) - loaded
+
+    def get_memory_footprint(self):
+        """Bytes held by the model's tensors: parameters (and their gradient buffer, if any), int8 / int4 weights and scales, and
+        buffers (transformers' `PreTrainedModel.get_memory_footprint`, which hf_quantizatin_inference.py prints)."""
+        n = self.flat.params.numel() * self.flat.params.element_size()
+        if self.flat.grads is not None:
+            n += self.flat.grads.numel() * self.flat.grads.element_size()
+        for wq in self._wq if self.weight_format != "bf16" else ():
+            n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in wq.values())
+        return n + sum(b.numel() * b.element_size() for b in self.buffers())
 
     # ---- engine hooks -----------------------------------------------------------------------------------------------
     def _need(self, bucket):

@@ -22,6 +22,11 @@ forward keeps the transposed e4m3 codes of ln_1's and ln_2's outputs and of the 
 attn.c_proj makes its input's codes from the attention output in the backward (attention keeps that output anyway). The
 embeddings, the tied LM head, the LayerNorms, attention, dGELU with the c_fc bias gradient, the loss and the optimizer stay
 bf16, as do the master weights and gradients; `generate` runs the bf16 projections.
+load_in_8bit / load_in_4bit (`from_pretrained(..., load_in_8bit=True)`): an inference-only model whose four block
+projections are held quantised (layers.QuantizedLinear: int8 per output channel, or int4 with a scale per row and group of
+128 k) from the transposed [out, in] weight, their biases bf16; c_fc's bias and gelu_new run in the W8A16 / W4A16 GEMM's
+epilogue (include/fsb200.h fsb_gemm_w8a16_bias). The no-grad forwards and `generate` run them; the embeddings, the tied LM
+head and the LayerNorms stay bf16, without a gradient buffer. Training, save_pretrained and fp8=True raise.
 """
 import math
 from collections import namedtuple
@@ -35,18 +40,38 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, key_mask, learned_pos_emb_bwd, packed_segments, refuse_key_padding
-from .layers import Fp8Conv1D, Linear, apply_dropout, residual_norm_bwd
+from .layers import WQ, Fp8Conv1D, Linear, QuantizedLinear, apply_dropout, quantized_unsupported, residual_norm_bwd
 
 _Block = namedtuple("_Block", "c_attn attn_proj c_fc mlp_proj")   # a block's projections
 
 
+_QKEYS = (("c_attn", "attn.c_attn"), ("attn_proj", "attn.c_proj"), ("c_fc", "mlp.c_fc"), ("mlp_proj", "mlp.c_proj"))
+
+
 class GPT2LMHeadModel(FlatModel):
-    def __init__(self, config, device=None, world_size=None, seed=0, fp8=False):
+    wq_transposed = True   # a checkpoint's Conv1D weights are [in, out]: quantised from their transpose
+
+    def __init__(self, config, device=None, world_size=None, seed=0, fp8=False, load_in_8bit=False, load_in_4bit=False):
         """fp8: train the block projections in FP8; see the module docstring. The training and no-grad (validation)
         forwards both run FP8; results differ from bf16 by design. n_embd, the MLP's inner width and the tokens per
-        micro-batch (batch x sequence length) must be multiples of 16 (checked at the first forward)."""
+        micro-batch (batch x sequence length) must be multiples of 16 (checked at the first forward).
+
+        load_in_8bit: an inference-only model. Each block's c_attn, attn.c_proj, mlp.c_fc and mlp.c_proj are held as int8
+        q [out, in] + fp32 per-output-channel scales s [out], quantised from the transposed Conv1D weight, and run through
+        the W8A16 GEMM with their bf16 bias (and gelu_new for c_fc) in its epilogue; wte, wpe (with the tied LM head), the
+        LayerNorms and the biases stay bf16 in flat buffers without a gradient buffer. Training, save_pretrained and fp8=True
+        raise. load_in_4bit: the same with int4 projections (a bf16 scale per row and group of 128 k); n_embd and the inner
+        width must then be multiples of 128."""
         super().__init__(config)
+        if load_in_8bit and load_in_4bit:
+            raise ValueError("fsb200 GPT2LMHeadModel: load_in_8bit and load_in_4bit are mutually exclusive; pass one")
+        if fp8 and (load_in_8bit or load_in_4bit):
+            raise ValueError("fsb200 GPT2LMHeadModel: fp8=True trains in FP8; it cannot be combined with load_in_8bit or "
+                             "load_in_4bit (inference-only weight formats)")
         self.fp8 = bool(fp8)
+        self.weight_format = "int8" if load_in_8bit else "int4" if load_in_4bit else "bf16"
+        self.load_in_8bit, self.load_in_4bit = self.weight_format == "int8", self.weight_format == "int4"
+        quantized = self.weight_format != "bf16"
         g = lambda k, d=None: getattr(config, k, d)
         self.h, self.nl, self.nh = g("n_embd", g("hidden_size")), g("n_layer", g("num_hidden_layers")), \
             g("n_head", g("num_attention_heads"))
@@ -60,6 +85,9 @@ class GPT2LMHeadModel(FlatModel):
         self.hn = h // self.nh
         if self.hn not in (64, 96, 128) or V % 8 or h % 8:
             raise RuntimeError("fsb200 GPT2: head dim must be 64/96/128 and vocab/hidden multiples of 8 (pad the vocab)")
+        if self.load_in_4bit and (h % 128 or self.inner % 128):
+            raise RuntimeError(f"fsb200 GPT2LMHeadModel(load_in_4bit=True): n_embd ({h}) and the inner width ({self.inner}) "
+                               "must be multiples of 128 (the int4 scale group)")
 
         spec = FlatSpec()
         spec.add("transformer.wte.weight", (V, h), "wte")
@@ -71,17 +99,25 @@ class GPT2LMHeadModel(FlatModel):
                          ("ln_2.weight", (h,)), ("ln_2.bias", (h,)), ("mlp.c_fc.weight", (h, self.inner)),
                          ("mlp.c_fc.bias", (self.inner,)), ("mlp.c_proj.weight", (self.inner, h)),
                          ("mlp.c_proj.bias", (h,))):
-                spec.add(p + n, s, bk)
+                if not (quantized and n.endswith(".weight") and not n.startswith("ln_")):   # int8 / int4: held as q + s
+                    spec.add(p + n, s, bk)
         spec.add("transformer.ln_f.weight", (h,), "wte")
         spec.add("transformer.ln_f.bias", (h,), "wte")
-        self._bind_flat(spec, device, world_size)
+        self._bind_flat(spec, device, world_size, grads=not quantized)
         self.lm_head = _Holder()
         self.lm_head.weight = self.transformer.wte.weight  # tied (modeling_gpt2.py:646)
         self._head = Linear.of(self.lm_head.weight)
-        conv1d = lambda m: Linear.of(m.weight, m.bias, conv1d=True)
-        self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
-                      for b in self.transformer.h]
-        self._proj_bf16 = self._proj   # what generate runs
+        if quantized:   # QuantizedLinear [n, k] = [out, in]: the Conv1D weight's transpose
+            qlin = lambda m, n, k: QuantizedLinear(self.weight_format, n, k, self.flat.params.device, bias=m.bias.data,
+                                                   model="GPT2LMHeadModel")
+            self._proj = [_Block(qlin(b.attn.c_attn, 3 * h, h), qlin(b.attn.c_proj, h, h),
+                                 qlin(b.mlp.c_fc, self.inner, h), qlin(b.mlp.c_proj, h, self.inner))
+                          for b in self.transformer.h]
+        else:
+            conv1d = lambda m: Linear.of(m.weight, m.bias, conv1d=True)
+            self._proj = [_Block(conv1d(b.attn.c_attn), conv1d(b.attn.c_proj), conv1d(b.mlp.c_fc), conv1d(b.mlp.c_proj))
+                          for b in self.transformer.h]
+        self._proj_generate = self._proj   # what generate runs: bf16 under fp8=True, the int8 / int4 projections if quantised
         if self.fp8:
             self._proj = [_Block(*(Fp8Conv1D(q) for q in pj)) for pj in self._proj]
         self.reset_parameters(seed)
@@ -103,6 +139,29 @@ class GPT2LMHeadModel(FlatModel):
             else:
                 s = std / math.sqrt(2 * self.nl) if name.endswith("c_proj.weight") else std
                 prm.normal_(0.0, s, generator=gen)
+        if self.weight_format != "bf16":   # each quantised projection: drawn in bf16 on the device and quantised, one at a time
+            for wq in self._wq:
+                for key, (q, s) in wq.items():
+                    tmp = torch.empty(self._weight_shape(q, s), dtype=torch.bfloat16, device=q.device)
+                    tmp.normal_(0.0, std / math.sqrt(2 * self.nl) if key in ("attn_proj", "mlp_proj") else std, generator=gen)
+                    WQ[self.weight_format][0](tmp, q, s)
+                    del tmp
+
+    # ---- int8 / int4 (load_in_8bit / load_in_4bit; loading and get_memory_footprint: FlatModel) -------------------------
+    @property
+    def _wq(self):
+        """Per block {projection: (q, s)} of an int8 / int4 model, projections named as _Block names them."""
+        return [{f: (getattr(pj, f).q, getattr(pj, f).s) for f, _ in _QKEYS} for pj in self._proj]
+
+    def _wq_targets(self):
+        """{state-dict key of a Conv1D weight: the (q, s) it quantises into}."""
+        return {f"transformer.h.{i}.{key}.weight": (getattr(pj, f).q, getattr(pj, f).s)
+                for i, pj in enumerate(self._proj) for f, key in _QKEYS}
+
+    def save_pretrained(self, path, **kw):
+        if self.weight_format != "bf16":
+            raise quantized_unsupported("GPT2LMHeadModel", self.weight_format, f"save_pretrained ({self.weight_format} export)")
+        return super().save_pretrained(path, **kw)
 
     # ---- forward ----------------------------------------------------------------------------------------------------
     def forward(self, input_ids=None, attention_mask=None, labels=None, position_ids=None, return_logits=False,
@@ -121,6 +180,8 @@ class GPT2LMHeadModel(FlatModel):
                                  "operands need 16-byte rows in both layouts)")
         dev = self.flat.params.device
         ids, lab = flat_ids(input_ids, dev), flat_ids(labels, dev)
+        if self.weight_format != "bf16" and lab is not None and torch.is_grad_enabled():
+            raise quantized_unsupported("GPT2LMHeadModel", self.weight_format, "a training forward (labels under grad mode)")
         pos = None if position_ids is None else flat_ids(position_ids.expand(B, S), dev)
         if segment_ids is None:
             seg, mask = (), key_mask(attention_mask, dev)
@@ -268,7 +329,7 @@ class GPT2LMHeadModel(FlatModel):
 
     def _last_logits(self, ids, pos, B, S, attend):
         """fp32 logits [B, V] of the last position of every sequence."""
-        hf, _, _ = self._stack(ids, pos, B, S, attend, proj=self._proj_bf16)   # fp8=True: bf16
+        hf, _, _ = self._stack(ids, pos, B, S, attend, proj=self._proj_generate)
         return self._head(hf.view(B, S, self.h)[:, -1].contiguous()).float()
 
     # ---- backward ---------------------------------------------------------------------------------------------------

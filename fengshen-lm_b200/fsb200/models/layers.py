@@ -1,5 +1,5 @@
 """The linear maps and the gated MLP the fsb200 models share: forward and hand-written backward over views into the flat
-buffers (fsb200/flat.py)."""
+buffers (fsb200/flat.py); and the int8 / int4 projection of the inference-only models (load_in_8bit / load_in_4bit)."""
 import torch
 
 from .. import lib as L
@@ -197,3 +197,43 @@ class Fp8Conv1D(Fp8Linear):
 
     def _wgrad(self, dyt, sdy, xt, sx, accumulate):
         ops.gemm_fp8(dyt, sdy, xt, sx, out=self.lin.weight_grad, accumulate=accumulate, store_transposed=True)
+
+
+# weight format -> (quantiser, (q dtype, q shape, s dtype, s shape) of an [n, k] weight)
+WQ = {
+    "int8": (ops.quantize_w8, lambda n, k: (torch.int8, (n, k), torch.float32, (n,))),
+    "int4": (ops.quantize_w4, lambda n, k: (torch.uint8, (n // 2, k), torch.bfloat16, (n, k // 128))),
+}
+
+
+def quantized_unsupported(model, fmt, what):
+    """The error an int8 / int4 model (`model` names its class) raises for `what`."""
+    return NotImplementedError(f"fsb200 {model}: {what} is not implemented for an {fmt} (load_in_{fmt[3:]}bit=True) "
+                               "model; it only runs inference")
+
+
+class QuantizedLinear:
+    """A layer projection of an int8 / int4 model, with Linear's call surface: the [n, k] weight held as q + scales s in the
+    format's layout (WQ) and run through the W8A16 / W4A16 GEMM, with an optional bf16 bias [n] (GPT-2's Conv1D; bias and
+    epilogue then run in the GEMM's epilogue). Inference only: saving inputs for a backward, aux and backward raise.
+    `model` names the owning class in those errors."""
+
+    def __init__(self, fmt, n, k, device, bias=None, model="model"):
+        qd, qs, sd, ss = WQ[fmt][1](n, k)
+        self.fmt, self.model = fmt, model
+        self.q, self.s = torch.zeros(qs, dtype=qd, device=device), torch.zeros(ss, dtype=sd, device=device)
+        self.bias = bias
+
+    def __call__(self, x, epilogue=L.EPI_NONE):
+        gemm = ops.gemm_w8a16 if self.fmt == "int8" else ops.gemm_w4a16
+        if self.bias is None and epilogue == L.EPI_NONE:   # LLaMA's projections: the bias-free call
+            return gemm(x, self.q, self.s)
+        return gemm(x, self.q, self.s, bias=self.bias, epilogue=epilogue)
+
+    def forward(self, x, save, epilogue=L.EPI_NONE, aux=None):
+        if save or aux is not None:
+            raise quantized_unsupported(self.model, self.fmt, "a forward that keeps activations for a backward")
+        return self(x, epilogue), None
+
+    def backward(self, *_, **__):
+        raise quantized_unsupported(self.model, self.fmt, "backward")

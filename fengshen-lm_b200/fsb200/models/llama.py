@@ -27,7 +27,7 @@ from .. import ops
 from ..decode_graph import DecodeGraphs
 from ..flat import FlatSpec
 from .base import FlatModel, _Holder, flat_ids, packed_segments
-from .layers import Fp8Linear, GatedMLP, Linear
+from .layers import WQ, Fp8Linear, GatedMLP, Linear, QuantizedLinear, quantized_unsupported
 
 
 def llama_ff_dim(hidden_size, multiple_of=256):
@@ -39,37 +39,14 @@ def _init_normal_(t, std, gen):
     t.copy_(torch.empty(t.shape, dtype=torch.float32).normal_(0.0, std, generator=gen).to(t.dtype))
 
 
-# weight format -> (quantiser, (q dtype, q shape, s dtype, s shape) of an [n, k] weight)
-_WQ = {
-    "int8": (ops.quantize_w8, lambda n, k: (torch.int8, (n, k), torch.float32, (n,))),
-    "int4": (ops.quantize_w4, lambda n, k: (torch.uint8, (n // 2, k), torch.bfloat16, (n, k // 128))),
-}
+# weight format -> (quantiser, q / s layout): the table layers.QuantizedLinear reads, shared with GPT-2
+_WQ = WQ
 
 _Layer = namedtuple("_Layer", "qkv dense mlp")   # a layer's projections: query_key_value, dense, the gated MLP (w1 | w3, w2)
 
 
 def _quantized_unsupported(fmt, what):
-    return NotImplementedError(f"fsb200 LlamaForCausalLM: {what} is not implemented for an {fmt} (load_in_{fmt[3:]}bit=True) "
-                               "model; it only runs inference")
-
-
-class QuantizedLinear:
-    """A layer projection of an int8 / int4 model, with Linear's call surface: the [n, k] weight held as q + scales s in the
-    format's layout (_WQ) and run through the W8A16 / W4A16 GEMM. Inference only: its backward raises."""
-
-    def __init__(self, fmt, n, k, device):
-        qd, qs, sd, ss = _WQ[fmt][1](n, k)
-        self.fmt = fmt
-        self.q, self.s = torch.zeros(qs, dtype=qd, device=device), torch.zeros(ss, dtype=sd, device=device)
-
-    def __call__(self, x):
-        return (ops.gemm_w8a16 if self.fmt == "int8" else ops.gemm_w4a16)(x, self.q, self.s)
-
-    def forward(self, x, save):
-        return self(x), None
-
-    def backward(self, *_, **__):
-        raise _quantized_unsupported(self.fmt, "backward")
+    return quantized_unsupported("LlamaForCausalLM", fmt, what)
 
 
 class LlamaForCausalLM(FlatModel):
@@ -165,7 +142,7 @@ class LlamaForCausalLM(FlatModel):
         spec.add("embed_out.final_linear.weight", (self.V_l, h), "head")
         self._bind_flat(spec, device, world_size, tp=self.tp, grads=not quantized)
         if quantized:   # w1 | w3 is one [2ff, h] operand as in the bf16 layout
-            qlin = lambda n, k: QuantizedLinear(self.weight_format, n, k, self.flat.params.device)
+            qlin = lambda n, k: QuantizedLinear(self.weight_format, n, k, self.flat.params.device, model="LlamaForCausalLM")
             self._proj = [_Layer(qlin(3 * h, h), qlin(h, h), GatedMLP(qlin(2 * self.ff, h), qlin(h, self.ff), L.ACT_SILU))
                           for _ in range(nl)]
         else:
@@ -230,23 +207,7 @@ class LlamaForCausalLM(FlatModel):
                     _WQ[self.weight_format][0](tmp, q, s)
                     del tmp
 
-    # ---- int8 / int4 (load_in_8bit / load_in_4bit) ---------------------------------------------------------------------
-    @staticmethod
-    def _weight_shape(q, s):
-        """[n, k] of the bf16 weight that (q, s) holds: s has one row per weight row in both formats, q the k columns."""
-        return s.shape[0], q.shape[1]
-
-    @torch.no_grad()
-    def load_reference_state_dict(self, sd):
-        """As FlatModel.load_reference_state_dict; a quantised model quantises each projection on the device as it arrives."""
-        if self.weight_format == "bf16":
-            return super().load_reference_state_dict(sd)
-        targets = set(self._p) | set(self._wq_targets())
-        missing = targets - set(sd)
-        if missing:
-            raise KeyError(f"missing key in state dict: {sorted(missing)[0]}")
-        self._load_quantized_shard(sd, set())
-
+    # ---- int8 / int4 (load_in_8bit / load_in_4bit; loading and get_memory_footprint: FlatModel) -------------------------
     @property
     def _wq(self):
         """Per layer {projection: (q, s)} of an int8 / int4 model (w13: the w1 | w3 operand), as `_w8` / `_w4` name them."""
@@ -269,40 +230,6 @@ class LlamaForCausalLM(FlatModel):
             out.update({p + "attention.query_key_value.weight": (qkv.q, qkv.s), p + "attention.dense.weight": (dense.q, dense.s),
                         p + "mlp.w1.weight": (q1, s1), p + "mlp.w3.weight": (q3, s3), p + "mlp.w2.weight": (mlp.wo.q, mlp.wo.s)})
         return out
-
-    @torch.no_grad()
-    def _load_quantized_shard(self, sd, loaded):
-        """Load the keys of `sd` (a whole state dict or one checkpoint shard) this int8 / int4 model holds: bf16 parameters
-        are copied, projections quantised on the device (one bf16 temporary at a time). The shard's shapes are checked before
-        anything is written. Adds the loaded keys to the set `loaded` and returns the keys it does not yet hold."""
-        targets = self._wq_targets()
-        for k, v in sd.items():
-            want = tuple(self._p[k].shape) if k in self._p else tuple(self._weight_shape(*targets[k])) if k in targets else None
-            if want is not None and tuple(v.shape) != want:
-                raise ValueError(f"shape mismatch for {k}: {tuple(v.shape)} vs {want}")
-        for k, v in sd.items():
-            v = v if v.dtype == torch.bfloat16 else v.to(torch.bfloat16)   # converted where it lies: one bf16 copy on the device
-            if k in self._p:
-                self._p[k].copy_(v)
-            elif k in targets:
-                q, s = targets[k]
-                tmp = v.to(q.device).contiguous()
-                _WQ[self.weight_format][0](tmp, q, s)
-                del tmp
-            else:
-                continue
-            loaded.add(k)
-        return (set(self._p) | set(targets)) - loaded
-
-    def get_memory_footprint(self):
-        """Bytes held by the model's tensors: parameters (and their gradient buffer, if any), int8 / int4 weights and scales, and
-        buffers (transformers' `PreTrainedModel.get_memory_footprint`, which hf_quantizatin_inference.py prints)."""
-        n = self.flat.params.numel() * self.flat.params.element_size()
-        if self.flat.grads is not None:
-            n += self.flat.grads.numel() * self.flat.grads.element_size()
-        for wq in self._wq if self.weight_format != "bf16" else ():
-            n += sum(q.numel() * q.element_size() + s.numel() * s.element_size() for q, s in wq.values())
-        return n + sum(b.numel() * b.element_size() for b in self.buffers())
 
     def save_pretrained(self, path, **kw):
         if self.weight_format != "bf16":

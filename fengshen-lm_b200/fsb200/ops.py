@@ -119,9 +119,35 @@ def quantize_w8(w, q=None, s=None):
     return q, s
 
 
-def gemm_w8a16(a, q, s, out=None):
+def _wq_bias(what, bias, epilogue, n):
+    """The bias / epilogue arguments of gemm_w8a16 / gemm_w4a16 checked: bias None (the plain GEMM: epilogue must be
+    EPI_NONE) or a contiguous bf16 [n] tensor with epilogue EPI_NONE or EPI_GELU_TANH."""
+    if bias is None:
+        if epilogue != L.EPI_NONE:
+            raise RuntimeError(f"fsb200 {what}: an epilogue needs a bias (the bias-free GEMM has none)")
+        return
+    _chk(bias, _bf16, "bias")
+    if bias.numel() != n or not bias.is_contiguous():
+        raise RuntimeError(f"fsb200 {what}: bias must be contiguous [{n}], got shape {tuple(bias.shape)}")
+    if epilogue not in (L.EPI_NONE, L.EPI_GELU_TANH):
+        raise RuntimeError(f"fsb200 {what}: epilogue {epilogue} unsupported (EPI_NONE or EPI_GELU_TANH)")
+
+
+def _wq_call(what, m, n, k, a, lda, q, s, out, ldd, ws, ws_bytes, bias, epilogue):
+    """fsb_<what> without a bias, fsb_<what>_bias with one."""
+    tag = f"{m}x{n}x{k}{'' if bias is None else f' bias epi{epilogue}'}" if L.call_profiler is not None else None
+    if bias is None:
+        L.call(f"fsb_{what}", m, n, k, _p(a), lda, _p(q), _p(s), _p(out), ldd, _p(ws), ws_bytes, _stream(), tag=tag)
+    else:
+        L.call(f"fsb_{what}_bias", m, n, k, _p(a), lda, _p(q), _p(s), _p(bias), epilogue, _p(out), ldd, _p(ws), ws_bytes,
+               _stream(), tag=tag)
+
+
+def gemm_w8a16(a, q, s, out=None, bias=None, epilogue=L.EPI_NONE):
     """out[m, n] = bf16(s[n] * (a[m, k] @ q[n, k]^T)), fp32 accumulation: a bf16 (unit inner stride), q int8 [n, k]
-    contiguous and s fp32 [n] as quantize_w8 returns them. `out` (bf16, unit inner stride) may be a strided view."""
+    contiguous and s fp32 [n] as quantize_w8 returns them. `out` (bf16, unit inner stride) may be a strided view.
+    bias (bf16 [n]): out = bf16(act(s[n] * (a @ q^T) + bias[n])), act by epilogue (EPI_NONE or EPI_GELU_TANH), through
+    fsb_gemm_w8a16_bias; None makes the bias-free call."""
     _chk(a, _bf16, "a"); _chk(q, torch.int8, "q"); _chk(s, torch.float32, "s")
     m, k, lda = _rows2d(a, "a")
     if q.dim() != 2 or not q.is_contiguous(): raise RuntimeError("fsb200 gemm_w8a16: q must be contiguous [n, k]")
@@ -133,10 +159,10 @@ def gemm_w8a16(a, q, s, out=None):
     _chk(out, _bf16, "out")
     orr, occ, ldd = _rows2d(out, "out")
     if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_w8a16: out shape {tuple(out.shape)} != ({m},{n})")
+    _wq_bias("gemm_w8a16", bias, epilogue, n)
     ws_bytes = int(L.load().fsb_gemm_w8a16_workspace_bytes(m, n, k))
     ws = workspace(ws_bytes, a.device, "gemm_w8a16") if ws_bytes else None
-    L.call("fsb_gemm_w8a16", m, n, k, _p(a), lda, _p(q), _p(s), _p(out), ldd, _p(ws), ws_bytes, _stream(),
-           tag=f"{m}x{n}x{k}" if L.call_profiler is not None else None)
+    _wq_call("gemm_w8a16", m, n, k, a, lda, q, s, out, ldd, ws, ws_bytes, bias, epilogue)
     return out
 
 
@@ -158,10 +184,10 @@ def quantize_w4(w, q=None, s=None):
     return q, s
 
 
-def gemm_w4a16(a, q, s, out=None):
+def gemm_w4a16(a, q, s, out=None, bias=None, epilogue=L.EPI_NONE):
     """out[m, n] = bf16(a[m, k] @ W^[n, k]^T), fp32 accumulation, W^ = bf16(q * s) the dequantised int4 weight: a bf16
     (unit inner stride), q uint8 [n / 2, k] and s bf16 [n, k / 128] contiguous as quantize_w4 returns them. `out` (bf16,
-    unit inner stride) may be a strided view."""
+    unit inner stride) may be a strided view. bias / epilogue as gemm_w8a16 (fsb_gemm_w4a16_bias)."""
     _chk(a, _bf16, "a"); _chk(q, torch.uint8, "q"); _chk(s, _bf16, "s")
     m, k, lda = _rows2d(a, "a")
     if q.dim() != 2 or not q.is_contiguous(): raise RuntimeError("fsb200 gemm_w4a16: q must be contiguous [n / 2, k]")
@@ -174,10 +200,10 @@ def gemm_w4a16(a, q, s, out=None):
     _chk(out, _bf16, "out")
     orr, occ, ldd = _rows2d(out, "out")
     if (orr, occ) != (m, n): raise RuntimeError(f"fsb200 gemm_w4a16: out shape {tuple(out.shape)} != ({m},{n})")
+    _wq_bias("gemm_w4a16", bias, epilogue, n)
     ws_bytes = int(L.load().fsb_gemm_w4a16_workspace_bytes(m, n, k))
     ws = workspace(ws_bytes, a.device, "gemm_w4a16") if ws_bytes else None
-    L.call("fsb_gemm_w4a16", m, n, k, _p(a), lda, _p(q), _p(s), _p(out), ldd, _p(ws), ws_bytes, _stream(),
-           tag=f"{m}x{n}x{k}" if L.call_profiler is not None else None)
+    _wq_call("gemm_w4a16", m, n, k, a, lda, q, s, out, ldd, ws, ws_bytes, bias, epilogue)
     return out
 
 

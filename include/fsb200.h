@@ -130,6 +130,22 @@ size_t fsb_gemm_w4a16_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int fsb_gemm_w4a16(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
                    void* d, int64_t ldd, void* workspace, size_t workspace_bytes, fsb_stream_t stream);
 
+/* ---- weight-only GEMMs with a bias / GELU epilogue (int8 / int4 GPT-2: Conv1D projections carry a bias) ----------
+ * fsb_gemm_w8a16_bias: D[m, n] = bf16(act(s[n] * sum_k A[m, k] q[n, k] + bias[n])).
+ * fsb_gemm_w4a16_bias: D[m, n] = bf16(act(sum_k A[m, k] W^[n, k] + bias[n])).
+ *   fp32 throughout: the sum (times s[n] for int8), + bias[n], then act, rounded once to bf16 — the order of
+ *   fsb_gemm_bf16's epilogue. bias: bf16 [n], non-NULL, 16-byte aligned. epilogue: FSB_EPI_NONE (act = identity) or
+ *   FSB_EPI_GELU_TANH (act = gelu_new, fsb_gemm_bf16's device code: the same fp32 pre-activation gives the same bits);
+ *   anything else is an error. Operands, requirements, plan and workspace (fsb_gemm_w8a16_workspace_bytes /
+ *   fsb_gemm_w4a16_workspace_bytes) as fsb_gemm_w8a16 / fsb_gemm_w4a16. A call that splits K sums the fp32 partials in
+ *   order first and applies scale, bias and act once per element after. */
+int fsb_gemm_w8a16_bias(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const int8_t* q, const float* s,
+                        const void* bias, int epilogue, void* d, int64_t ldd, void* workspace, size_t workspace_bytes,
+                        fsb_stream_t stream);
+int fsb_gemm_w4a16_bias(int64_t m, int64_t n, int64_t k, const void* a, int64_t lda, const uint8_t* q, const void* s,
+                        const void* bias, int epilogue, void* d, int64_t ldd, void* workspace, size_t workspace_bytes,
+                        fsb_stream_t stream);
+
 /* ---- FP8 training GEMM (opt-in `fp8=True`: LLaMA, BERT, MegatronBERT, mT5, GPT-2) -----------------------------------
  * The "hybrid" recipe with just-in-time ("current") per-tensor scaling: activations and weights are e4m3 (largest finite
  * value 448), gradients e5m2 (57344); accumulation is fp32, outputs bf16.
